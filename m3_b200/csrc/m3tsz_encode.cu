@@ -7,8 +7,8 @@
 // (ts, value) inputs are staged through a transposed shared-memory tile from
 // coalesced 128-byte loads, each datapoint's code (<= 32-bit header + <= 64-bit
 // payload) is merged into a per-lane bit accumulator with funnel shifts, full
-// 32-bit words go to a transposed output tile, and the tile is written back
-// with coalesced 128-byte stores per series.
+// 32-bit words go to a transposed output tile, and every lane writes its own
+// series' words back in whole 32-byte sectors.
 //
 // Format: SURVEY.md Appendix A; reference encode path
 //   m3tsz/encoder.go:90-250, m3tsz/timestamp_encoder.go:72-259,
@@ -26,14 +26,20 @@ namespace m3tsz {
 
 constexpr int ENC_WARPS = 4;
 constexpr int ENC_STRIDE = 33;
-constexpr int ENC_IN_T = 8;     // datapoints per input tile (double buffered, cp.async)
+constexpr int ENC_IN_T = 8;     // datapoints per input tile of the series-major stage (double buffered, cp.async)
 #ifndef M3_ENC_OUT_W
-#define M3_ENC_OUT_W 24  // output tile words per lane (smaller tile = more L1)
+// output tile words per lane (smaller tile = more L1): the 24 words that 16-byte flushes used, plus 4 for the
+// larger leftover of whole-sector flushes, so a flush cycle still adds about as many words as before
+#define M3_ENC_OUT_W 28
 #endif
-// Residency the launch bounds promise.  The input-tile stages (IN = 0, 1) use ~46 KB of shared memory per block,
-// so the 132 KB carveout below holds 2 of them; the Gauge stage (IN = 2) has no input tiles and fits more.
+// Residency the launch bounds promise.  The series-major stage (IN = 0) uses ~48 KB of shared memory per block,
+// so the 132 KB carveout below holds 2 of them; the point-major stage (IN = 1) uses ~31 KB and fits 4; the Gauge
+// stage (IN = 2) has no input tiles and fits more.
 #ifndef M3_ENC_MIN_BLOCKS
 #define M3_ENC_MIN_BLOCKS 2
+#endif
+#ifndef M3_ENC_MIN_BLOCKS_PM
+#define M3_ENC_MIN_BLOCKS_PM 4
 #endif
 #ifndef M3_ENC_MIN_BLOCKS_AGG
 #define M3_ENC_MIN_BLOCKS_AGG 4
@@ -44,11 +50,19 @@ constexpr int ENC_IN_T = 8;     // datapoints per input tile (double buffered, c
 constexpr int ENC_OUT_W = M3_ENC_OUT_W;   // output tile words per lane
 constexpr int ENC_GUARD = 10;   // words a single datapoint (no annotation) may add
 constexpr int ENC_OUT_TILE_WORDS = ENC_OUT_W * ENC_STRIDE;
+// A flush writes whole 32-byte sectors and leaves up to 7 words in the tile.  The tile is flushed once it holds
+// more than ENC_OUT_W - ENC_GUARD words; that must be at least one sector, so every flush makes room.
+static_assert(ENC_OUT_W - ENC_GUARD >= 8, "output tile too small for sector flushes");
 #ifndef M3_ENC_IN_T_PM
-// rows per input tile of the point-major input stage (IN = 1).  With the cp.async fills a smaller tile leaves more
-// L1 to the fills; with tensor copies (M3_ENC_BULK_PM = 2, which do not allocate L1 lines) one copy per array costs
-// the same whatever the box, so the larger tile wins.
-#define M3_ENC_IN_T_PM 8
+// rows per input tile of the point-major input stage (IN = 1).  With tensor copies (M3_ENC_BULK_PM = 2, which do
+// not allocate L1 lines) one copy per array costs the same whatever the box; the tile size sets the shared memory
+// per warp and with it the residency.  Measured with M3_ENC_NSTAGE_PM (enc_carveout_kb() has the numbers):
+// 4 x 2 (4 blocks at 132 KB) was the fastest; 2 x 2 (5 blocks), 2 x 4 and 4 x 3 (3 blocks) were slower.
+#define M3_ENC_IN_T_PM 4
+#endif
+#ifndef M3_ENC_NSTAGE_PM
+// input tiles in flight per warp in the point-major stage (a ring of stages, one mbarrier each)
+#define M3_ENC_NSTAGE_PM 2
 #endif
 // input stage IN: 0 series-major tiles (8 rows: one 64-byte segment per series and array), 1 point-major
 // tiles, 2 Gauge aggregates read directly (no input tiles)
@@ -70,6 +84,10 @@ __host__ __device__ constexpr int enc_in_t() {
   return IN == 1 ? M3_ENC_IN_T_PM : ENC_IN_T;
 }
 template <int IN>
+__host__ __device__ constexpr int enc_nstage() {
+  return IN == 1 ? M3_ENC_NSTAGE_PM : 2;
+}
+template <int IN>
 __host__ __device__ constexpr int enc_bulk() {
   return IN == 1 ? M3_ENC_BULK_PM : 0;
 }
@@ -86,8 +104,9 @@ __host__ __device__ constexpr int enc_in_stride() {
 }
 template <int IN>
 __host__ __device__ constexpr size_t enc_warp_smem() {
-  const size_t raw = ((IN == 0 || IN == 1) ? 4 * (size_t)(enc_in_t<IN>() * enc_in_stride<IN>()) * 8 : 0) +
-                     (size_t)ENC_OUT_TILE_WORDS * 4 + (enc_bulk<IN>() ? 16 : 0);  // (+ two mbarriers per warp)
+  const size_t raw =
+      ((IN == 0 || IN == 1) ? 2 * (size_t)enc_nstage<IN>() * (enc_in_t<IN>() * enc_in_stride<IN>()) * 8 : 0) +
+      (size_t)ENC_OUT_TILE_WORDS * 4 + (enc_bulk<IN>() ? 8 * enc_nstage<IN>() : 0);  // (+ one mbarrier per stage)
   return enc_bulk<IN>() == 2 ? ((raw + 127) & ~(size_t)127) : raw;  // tensor copies land on 128-byte boundaries
 }
 
@@ -699,7 +718,8 @@ __device__ __forceinline__ void enc_mbar_wait(uint32_t bar, uint32_t parity) {
 //         series = (tile_start + (i+1)*tile_step, Gauge.ValueOf(agg)) unless window i is empty
 //         (count == 0: skipped) -- the tile aggregation's re-encode without a gather pass.
 template <bool INT_OPT, bool PACKED, int IN>
-__global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_AGG : M3_ENC_MIN_BLOCKS)
+__global__ void __launch_bounds__(ENC_WARPS * 32,
+                                  (IN == 2) ? M3_ENC_MIN_BLOCKS_AGG : (IN == 1 ? M3_ENC_MIN_BLOCKS_PM : M3_ENC_MIN_BLOCKS))
     encode_kernel(const EncodeParams p
 #if M3_ENC_BULK_PM == 2
                   ,
@@ -712,6 +732,8 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
   // the direct input stages (IN != 0) need no input tiles: only the output tile lives in shared memory
   constexpr bool STAGED = (IN == 0 || IN == 1);  // inputs go through the shared-memory tiles
   constexpr int IN_T = enc_in_t<IN>();  // datapoints per input tile
+  static_assert((IN_T & (IN_T - 1)) == 0, "tile rows must be a power of two");
+  constexpr uint32_t NSTAGE = (uint32_t)enc_nstage<IN>();  // input tiles in flight (ring of buffers)
   constexpr int IN_STRIDE = enc_in_stride<IN>();  // cells per tile row
   constexpr int IN_TILE_DW = IN_T * IN_STRIDE;  // one array (ts or val), one buffer
   constexpr int BULK = enc_bulk<IN>();  // 0 cp.async fills, 1 1-D bulk copies per row, 2 one 2-D tensor copy per array
@@ -719,11 +741,11 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
   uint8_t *wbase = reinterpret_cast<uint8_t *>(smem) + warp * WARP_SMEM;
   // in_tiles: [buffer][array (0 ts, 1 val)][row][lane]
   uint64_t *in_tiles = reinterpret_cast<uint64_t *>(wbase);
-  uint32_t *out_tile = STAGED ? reinterpret_cast<uint32_t *>(in_tiles + 4 * IN_TILE_DW)
+  uint32_t *out_tile = STAGED ? reinterpret_cast<uint32_t *>(in_tiles + 2 * NSTAGE * IN_TILE_DW)
                               : reinterpret_cast<uint32_t *>(wbase);
 
-  // BULK: two mbarriers per warp (one per tile buffer) behind the output tile; `bulk_seq` counts the tiles this
-  // warp has requested through them (buffer = seq & 1, phase parity = (seq >> 1) & 1), across batches
+  // BULK: one mbarrier per tile buffer behind the output tile; `bulk_seq` counts the tiles this warp has requested
+  // through them (buffer = seq % NSTAGE, phase parity = (seq / NSTAGE) & 1), across batches
   const uint32_t mbar0 = BULK ? enc_smem_addr(out_tile + ENC_OUT_TILE_WORDS) : 0u;
   uint32_t bulk_seq = 0;
 #if M3_ENC_BULK_PM == 2
@@ -733,8 +755,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
 #endif
   if (BULK) {
     if (lane == 0) {
-      enc_mbar_init(mbar0, 1);
-      enc_mbar_init(mbar0 + 8, 1);
+      for (uint32_t b = 0; b < NSTAGE; b++) enc_mbar_init(mbar0 + 8u * b, 1);
       enc_mbar_init_fence();
     }
     __syncwarp();
@@ -821,44 +842,40 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
   }
   const uint32_t max_pts = __reduce_max_sync(FULL_MASK, n_pts);
 
-  // Lane-local flush: every lane streams the complete 16-byte groups of ITS OWN
-  // column to its slot (big-endian byte order) and keeps the <= 3 leftover words.
+  // Lane-local flush: every lane streams the complete 32-byte sectors of ITS OWN column to its slot (big-endian
+  // byte order, two 16-byte stores per sector) and keeps the <= 7 leftover words, so no store leaves an L2 sector
+  // half written.  The last flush also writes the final 16-byte group (the tail pads the stream to one).  The
+  // sectors are whole in memory when out_stride is a multiple of 32 bytes, as the bench's is.
   uint8_t *my_out = PACKED ? p.out + (warp_slot * 32ull + (uint64_t)lane) * p.out_stride
                            : p.out + sidx * p.out_stride;
-  auto flush_out = [&]() {
+  auto flush_out = [&](bool last) {
     __syncwarp();
     const uint32_t kmax = __reduce_max_sync(FULL_MASK, s.k);
-    const uint32_t full = s.k >> 2;
-    uint4 *dst = reinterpret_cast<uint4 *>(my_out + (uint64_t)s.words_out * 4ull);
-    for (uint32_t q = 0; q < (kmax >> 2); q++) {
-      if (q < full) {
-        const uint32_t *tp = out_tile + (4 * q) * ENC_STRIDE + lane;
+    const uint32_t grp = last ? s.k >> 2 : (s.k >> 3) << 1;  // 16-byte groups this lane writes
+    const uint32_t grp_max = last ? kmax >> 2 : (kmax >> 3) << 1;
+    uint8_t *dst = my_out + (uint64_t)s.words_out * 4ull;
+    for (uint32_t q = 0; q < grp_max; q++) {
+      const uint32_t *tp = out_tile + (4 * q) * ENC_STRIDE + lane;
+      if (q < grp) {  // (a predicated store instead of the branch costs ~20 registers: all four loads stay live)
         uint4 v;
         v.x = __byte_perm(tp[0], 0, 0x0123);
         v.y = __byte_perm(tp[ENC_STRIDE], 0, 0x0123);
         v.z = __byte_perm(tp[2 * ENC_STRIDE], 0, 0x0123);
         v.w = __byte_perm(tp[3 * ENC_STRIDE], 0, 0x0123);
-        dst[q] = v;
+        *reinterpret_cast<uint4 *>(dst + 16ull * q) = v;
       }
     }
-    const uint32_t rem = s.k & 3u;
-    uint32_t r0 = 0, r1 = 0, r2 = 0;
-    {
-      const uint32_t *tp = out_tile + (4 * full) * ENC_STRIDE + lane;
-      if (rem > 0) r0 = tp[0];
-      if (rem > 1) r1 = tp[ENC_STRIDE];
-      if (rem > 2) r2 = tp[2 * ENC_STRIDE];
-    }
-    __syncwarp();
-    if (rem > 0) out_tile[lane] = r0;
-    if (rem > 1) out_tile[ENC_STRIDE + lane] = r1;
-    if (rem > 2) out_tile[2 * ENC_STRIDE + lane] = r2;
-    s.words_out += 4 * full;
+    // move the leftover words to the top of the lane's column: the rows do not overlap, because a flush that
+    // writes anything writes at least a sector (done >= 8 > rem), and the last flush leaves nothing
+    const uint32_t done = 4 * grp, rem = s.k - done;
+    if (done)
+      for (uint32_t i = 0; i < rem; i++) out_tile[i * ENC_STRIDE + lane] = out_tile[(done + i) * ENC_STRIDE + lane];
+    s.words_out += done;
     s.k = rem;
     __syncwarp();
   };
 
-  // asynchronous staging of input tile `tile` (rows tile*IN_T ..) into buffer tile&1:
+  // asynchronous staging of input tile `tile` (rows tile*IN_T ..) into buffer (tile_base + tile) % NSTAGE:
   // lanes 0-7 / 8-15: ts / value rows of series 2i, lanes 16-23 / 24-31: of series 2i+1
   const int st_r = lane & (IN_T - 1);
   const int st_arr = (lane >> 3) & 1;
@@ -867,17 +884,17 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
   // this batch's tiles come by bulk copy: a full warp of series of one length (rows of 32 x 8 bytes, all in range)
   // (tensor copies zero-fill what is out of range, so they serve every batch)
   const bool bulk = BULK && bulk_args && (BULK == 2 || uniform_n);
-  const uint32_t tile_base = bulk ? bulk_seq : 0u;  // buffer of tile t: (tile_base + t) & 1
+  const uint32_t tile_base = bulk ? bulk_seq : 0u;  // buffer of tile t: (tile_base + t) % NSTAGE
   auto stage = [&](uint32_t tile) {
     const uint32_t row0 = tile * IN_T;
     if (row0 >= max_pts) return;
+    const uint32_t buf = (tile_base + tile) % NSTAGE;
 #if M3_ENC_BULK_PM == 2
     if (BULK == 2 && bulk) {
       if (lane == 0) {
-        const uint32_t g = tile_base + tile;
-        const uint32_t bar = mbar0 + (g & 1u) * 8u;
+        const uint32_t bar = mbar0 + buf * 8u;
         enc_mbar_expect_tx(bar, 2u * (uint32_t)IN_TILE_DW * 8u);  // the whole box counts, in range or not
-        const uint32_t d0 = enc_smem_addr(in_tiles + ((g & 1u) * 2u) * IN_TILE_DW);
+        const uint32_t d0 = enc_smem_addr(in_tiles + (buf * 2u) * IN_TILE_DW);
         enc_tma_2d(d0, &tmaps.ts, (int)warp_s0, (int)row0, bar);
         enc_tma_2d(d0 + (uint32_t)IN_TILE_DW * 8u, &tmaps.val, (int)warp_s0, (int)row0, bar);
       }
@@ -886,13 +903,12 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
 #endif
     if (BULK == 1 && bulk) {
       if (lane == 0) {
-        const uint32_t g = tile_base + tile;
-        const uint32_t bar = mbar0 + (g & 1u) * 8u;
+        const uint32_t bar = mbar0 + buf * 8u;
         const uint32_t nrow = (max_pts - row0 < (uint32_t)IN_T) ? max_pts - row0 : (uint32_t)IN_T;
         enc_mbar_expect_tx(bar, nrow * 512u);
         const uint64_t *st = reinterpret_cast<const uint64_t *>(p.ts) + (uint64_t)row0 * p.n_series + warp_s0;
         const uint64_t *sv = reinterpret_cast<const uint64_t *>(p.val) + (uint64_t)row0 * p.n_series + warp_s0;
-        const uint32_t d0 = enc_smem_addr(in_tiles + ((g & 1u) * 2u) * IN_TILE_DW);
+        const uint32_t d0 = enc_smem_addr(in_tiles + (buf * 2u) * IN_TILE_DW);
 #pragma unroll
         for (int r = 0; r < IN_T; r++) {
           if ((uint32_t)r < nrow) {
@@ -907,10 +923,10 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
     }
     if (IN == 1) {
       // point-major inputs: a row of the tile is 32 consecutive elements of the array -- every lane
-      // copies its own column (8 rows x 2 arrays), sources coalesced across the warp, no shuffles
+      // copies its own column (IN_T rows x 2 arrays), sources coalesced across the warp, no shuffles
       const uint64_t *st = reinterpret_cast<const uint64_t *>(p.ts) + (uint64_t)row0 * p.n_series + sidx;
       const uint64_t *sv = reinterpret_cast<const uint64_t *>(p.val) + (uint64_t)row0 * p.n_series + sidx;
-      const uint32_t d0 = enc_smem_addr(in_tiles + ((tile & 1u) * 2u) * IN_TILE_DW + lane);
+      const uint32_t d0 = enc_smem_addr(in_tiles + (buf * 2u) * IN_TILE_DW + lane);
       const uint32_t lim = s.err == 0 ? n_pts : 0u;  // (0 for a lane without a series)
 #pragma unroll
       for (int r = 0; r < IN_T; r++) {
@@ -926,7 +942,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
     const uint64_t *src = (st_arr ? reinterpret_cast<const uint64_t *>(p.val)
                                   : reinterpret_cast<const uint64_t *>(p.ts)) +
                           (warp_s0 + st_jo) * p.points_stride + row0 + st_r;
-    const uint32_t dst0 = enc_smem_addr(in_tiles + ((tile & 1u) * 2u + (uint32_t)st_arr) * IN_TILE_DW +
+    const uint32_t dst0 = enc_smem_addr(in_tiles + (buf * 2u + (uint32_t)st_arr) * IN_TILE_DW +
                                         st_r * IN_STRIDE + st_jo);
     const uint64_t step = 2ull * p.points_stride;
     if (uniform_n && row0 + IN_T <= max_pts) {
@@ -944,9 +960,11 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
     }
   };
 
-  if (STAGED) {
-    stage(0);
-    if (!(BULK && bulk)) asm volatile("cp.async.commit_group;\n" ::: "memory");
+  if (STAGED) {  // the first NSTAGE - 1 tiles; the loop requests each next one as it starts a tile
+    for (uint32_t t = 0; t + 1 < NSTAGE; t++) {
+      stage(t);
+      if (!(BULK && bulk)) asm volatile("cp.async.commit_group;\n" ::: "memory");
+    }
   }
   // direct input stages: element `row` of this lane's series
   auto load_row = [&](uint32_t row, int64_t &t_o, uint64_t &v_o, bool &skip_o) {
@@ -1002,20 +1020,21 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
     const bool tile_last = UNR > 1 ? (ph == IN_T - 1) : ((iter & (IN_T - 1)) == IN_T - 1);
     const bool active = s.err == 0 && iter < n_pts && !(IN == 2 && sk_pf);  // (n_pts is 0 without a series)
 
-    // ---- input pipeline: request tile t+1, wait for tile t ----
+    // ---- input pipeline: request tile t+NSTAGE-1, wait for tile t ----
     if (STAGED && tile_first) {
-      __syncwarp();  // everyone is done reading the buffer about to be overwritten
-      stage(iter / IN_T + 1);
+      __syncwarp();  // everyone is done reading the buffer about to be overwritten (tile t-1's)
+      stage(iter / IN_T + NSTAGE - 1);
       const uint32_t g = tile_base + iter / IN_T;  // (tile_base is 0 unless this batch is bulk-filled)
+      const uint32_t buf = g % NSTAGE;
       if (BULK && bulk) {
-        enc_mbar_wait(mbar0 + (g & 1u) * 8u, (g >> 1) & 1u);  // every lane: the tile's bytes have landed
+        enc_mbar_wait(mbar0 + buf * 8u, (g / NSTAGE) & 1u);  // every lane: the tile's bytes have landed
       } else {
         asm volatile("cp.async.commit_group;\n" ::: "memory");
-        asm volatile("cp.async.wait_group 1;\n" ::: "memory");
+        asm volatile("cp.async.wait_group %0;\n" ::"n"(NSTAGE - 1) : "memory");
       }
       __syncwarp();
-      // row 0 of the tile that just landed; rows 1..7 are fetched one datapoint ahead below
-      const uint64_t *tile = in_tiles + ((g & 1u) * 2u) * IN_TILE_DW + lane;
+      // row 0 of the tile that just landed; rows 1..IN_T-1 are fetched one datapoint ahead below
+      const uint64_t *tile = in_tiles + (buf * 2u) * IN_TILE_DW + lane;
       t_pf = (int64_t)tile[0];
       fb_pf = tile[IN_TILE_DW];
       in_next = tile + IN_STRIDE;
@@ -1023,7 +1042,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
 
     // ---- make room in the output tile ----
     const bool tight = active && (s.k > (uint32_t)(ENC_OUT_W - ENC_GUARD));
-    if (__any_sync(FULL_MASK, tight)) flush_out();
+    if (__any_sync(FULL_MASK, tight)) flush_out(false);
 
     // ---- annotations (warp-cooperative; timestamp_encoder.go:166-195) ----
     bool want_ann = false;
@@ -1075,7 +1094,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
             rem--;
           }
           if (!__any_sync(FULL_MASK, rem > 0)) break;
-          flush_out();
+          flush_out(false);
         }
       }
     }
@@ -1197,7 +1216,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, (IN == 2) ? M3_ENC_MIN_BLOCKS_
   } else {
     s.k = 0;
   }
-  flush_out();
+  flush_out(true);
   const uint64_t my_len = (total_bits + 7) >> 3;
   if (valid && IN == 2 && p.n_tiles_out) p.n_tiles_out[sidx] = s.n_enc;
   if (valid && p.out_bits) p.out_bits[sidx] = total_bits;  // incl. the end-of-stream marker, before padding
@@ -1285,11 +1304,16 @@ constexpr size_t enc_block_smem() {
 }
 
 // Shared-memory carveout of the encode kernels (the rest of the SM's 256 KB of L1 + shared memory is L1).
-// Point-major encode of 500 k x 1440 on an H100 SXM (700 W, 1980 MHz), int-optimised: 14.72 / 10.46 / 10.45 /
-// 11.89 / 13.02 ms at 64 / 100 / 132 / 164 / 196 KB, 13.95 at 228 KB and with the driver's own choice (4 blocks,
-// 28 KB of L1).  At 132 KB (2 blocks, 124 KB of L1) the other stages, same shape, against the driver's choice:
-// series-major encode 12.26 vs 15.15 ms, packed output 15.52 vs 18.64 (point-major inputs 13.62 vs 17.49), tile
-// re-encode (IN = 2, residency not limited by shared memory) 9.20 vs 9.20.  M3TSZ_ENC_CARVEOUT_KB=K overrides.
+// At 132 KB (124 KB of L1) the point-major stage holds 4 blocks (31 KB each: 16 warps per SM), the series-major
+// stage 2 (48 KB each) and the Gauge stage 5 (register-limited).  Point-major encode of 500 k x 1440,
+// int-optimised, on an H100 SXM (400 W power limit, 1980 MHz max SM clock), median of 3:
+// * with 16-byte flushes and 8-row tiles (8 warps): 10.39 / 10.38 / 11.94 / 14.10 ms at 100 / 132 / 164 / 228 KB;
+//   4-row tiles, 4 blocks at 132 KB (16 warps, the same L1): 12.93 ms.  More warps at equal L1 were slower, so
+//   L1 size was not the cause.  Without the flush's global stores (wrong bytes, a diagnostic build) 8 and 16
+//   warps took 7.43 and 6.06 ms: half-written sectors were what made more warps slower.
+// * with whole-sector flushes: 10.29 ms at 8 warps; 8.46 ms with 4-row tiles at 16 warps (132 KB), 9.31 at
+//   100 KB (3 blocks); 2-row tiles at 20 warps 8.52; 4-row x 3 stages at 164 KB (16 warps, 92 KB of L1) 8.57.
+// M3TSZ_ENC_CARVEOUT_KB=K overrides.
 static int enc_carveout_kb() {
   static const int kb = [] {
     const char *c = getenv("M3TSZ_ENC_CARVEOUT_KB");
