@@ -7,7 +7,9 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("M3TSZ_B200_LIB") or os.path.join(_HERE, "libm3tsz_b200.so")  # env: tuning builds
+# M3TSZ_B200_LIB names another build of the library to load instead, so that two builds can be compared
+# run for run on the same machine
+LIB_PATH = os.environ.get("M3TSZ_B200_LIB") or os.path.join(_HERE, "libm3tsz_b200.so")
 
 OK = 0
 ERR_EOF = 1

@@ -366,16 +366,6 @@ int m3tsz_encode_batch_packed_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
       p.in_mode = 1;
     }
   }
-  {
-    // optional start-up phase spread of the persistent warps (tuning knob, off by default: the
-    // copy phase costs warp residency, not DRAM contention, so spreading the warps out did not help)
-    static const long ns_per_dp = [] {
-      const char *e = getenv("M3TSZ_ENC_STAGGER_NS_PER_DP");
-      return e ? atol(e) : 0L;
-    }();
-    const uint64_t n_batches = (n_series + 31) / 32;
-    if (ns_per_dp > 0 && n_batches >= 3 * (slots / 32)) p.stagger_ns = points_stride * (uint64_t)ns_per_dp;
-  }
   CK(launch_encode(p, opts->int_optimized != 0, st));
   ctx->launches++;
   return M3TSZ_OK;

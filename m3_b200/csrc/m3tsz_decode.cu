@@ -14,60 +14,28 @@
 // Format: SURVEY.md Appendix A; reference decode path
 //   m3tsz/iterator.go:81-219, m3tsz/timestamp_iterator.go:80-326,
 //   m3tsz/float_encoder_iterator.go:105-165, istream.go:73-115.
-#include <cstdlib>
 #include "m3tsz_common.cuh"
 #include "m3tsz_kernels.h"
 
 namespace m3tsz {
 
-// Tuning knobs (overridable with -D for sweeps)
-#ifndef M3_DEC_TRIGGER
-#define M3_DEC_TRIGGER 24  // <= this many requested words ahead: the lane triggers a refill event
-#endif
-#ifndef M3_DEC_CHK
-#define M3_DEC_CHK 4  // ring bookkeeping every CHK datapoints
-#endif
-#ifndef M3_DEC_SAFE_MIN
-#define M3_DEC_SAFE_MIN 12  // fewer landed words ahead than this: confirm the copy in flight
-#endif
-#ifndef M3_DEC_MIN_BLOCKS
-#define M3_DEC_MIN_BLOCKS 4  // 4 x 4 warps with ~110 registers beat 5 blocks squeezed into 96
-#endif
-#ifndef M3_DEC_RING64_PLAIN
-#define M3_DEC_RING64_PLAIN 0  // ... not series-major decode (more shared-memory wavefronts, see the parse)
-#endif
-#ifndef M3_DEC_RING64
-#define M3_DEC_RING64 1  // fused-downsample and point-major kernels read the ring as 8-byte pairs (see the parse)
-#endif
-#ifndef M3_DEC_MIN_BLOCKS_DS
-#define M3_DEC_MIN_BLOCKS_DS 5  // fused-downsample kernels: 5 x 4 warps at 96 registers beat 4 blocks
-#endif
-#ifndef M3_DEC_WARPS
-#define M3_DEC_WARPS 4
-#endif
-constexpr int DEC_WARPS = M3_DEC_WARPS;  // warps per block
-#ifndef M3_DEC_RING
-#define M3_DEC_RING 64
-#endif
-constexpr int DEC_RING = M3_DEC_RING;  // staged words per lane (ring buffer, power of two)
+// <= this many requested words ahead: the lane triggers a refill event.  It has to leave DEC_CHK * 80 bits + the
+// fast path's window landed after a group.
+constexpr int DEC_TRIGGER = 24;
+constexpr int DEC_CHK = 4;        // datapoints per ring bookkeeping / group pre-check
+constexpr int DEC_SAFE_MIN = 12;  // fewer landed words ahead than this: confirm the copy in flight
+constexpr int DEC_MIN_BLOCKS = 4;     // 4 x 4 warps with ~110 registers beat 5 blocks squeezed into 96
+constexpr int DEC_MIN_BLOCKS_DS = 5;  // fused-downsample kernels: 5 x 4 warps at 96 registers beat 4 blocks
+constexpr int DEC_WARPS = 4;      // warps per block
+constexpr int DEC_RING = 64;      // staged words per lane (ring buffer, power of two)
 constexpr int DEC_FILL = 16;      // words per lane per asynchronous refill chunk
-constexpr int DEC_TRIGGER = M3_DEC_TRIGGER;
 constexpr int DEC_ACCEPT = DEC_RING - DEC_FILL;  // lanes with <= this many words ahead take a chunk
 constexpr int DEC_GROUP = 4;      // datapoints per output group (one 32-byte sector per array)
 constexpr int DEC_FAST_WORDS = 4; // the fast path reads 4 consecutive words
 
 constexpr int DEC_QUADS = DEC_RING / 4;  // + 1 mirror quad (copy of quad 0) so quad q+1 is always at +1
 constexpr int DEC_IN_TILE_WORDS = (DEC_QUADS + 1) * 32 * 4;
-static_assert(M3_DEC_CHK == DEC_GROUP, "ring bookkeeping runs once per output group");
-// The kernels without register-resident output groups (point-major decode, fused downsample) may
-// run the ring bookkeeping / group pre-check every CHK_WIDE datapoints; the refill trigger then has
-// to leave CHK_WIDE * 80 bits + the window landed after a group: TRIGGER_WIDE.
-#ifndef M3_DEC_CHK_WIDE
-#define M3_DEC_CHK_WIDE 4
-#endif
-#ifndef M3_DEC_TRIGGER_WIDE
-#define M3_DEC_TRIGGER_WIDE 24
-#endif
+static_assert(DEC_CHK == DEC_GROUP, "ring bookkeeping runs once per output group");
 constexpr size_t DEC_WARP_SMEM_PLAIN = (size_t)DEC_IN_TILE_WORDS * 4;
 static_assert(DEC_WARP_SMEM_PLAIN % 16 == 0, "every warp's ring must stay 16-byte aligned");
 
@@ -433,18 +401,8 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, uint32
   asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes)
                : "memory");
 }
-#ifndef M3_DEC_CPASYNC_CG
-#define M3_DEC_CPASYNC_CG 0  // 1: cp.async.cg (L2 only) for whole-chunk refills
-#endif
-#ifndef M3_DEC_L2_PREFETCH
-#define M3_DEC_L2_PREFETCH 0  // 1: pull the chunk after the one being copied into L2
-#endif
 __device__ __forceinline__ void cp_async16_full(uint32_t dst, const void *src) {
-#if M3_DEC_CPASYNC_CG
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(dst), "l"(src) : "memory");
-#else
   asm volatile("cp.async.ca.shared.global [%0], [%1], 16;\n" ::"r"(dst), "l"(src) : "memory");
-#endif
 }
 // Lane-local refill: the lane copies the 64-byte chunk at global word index gw
 // (a multiple of 16) of ITS OWN stream into quads slot_q0..slot_q0+3 of its own
@@ -461,13 +419,6 @@ __device__ __forceinline__ void ring_fill(uint32_t ring_lane_addr, const uint8_t
     cp_async16_full(dst + 1024u, src + 32);
     cp_async16_full(dst + 1536u, src + 48);
     if (slot_q0 == 0) cp_async16_full(ring_lane_addr + DEC_QUADS * 512u, src);
-#if M3_DEC_L2_PREFETCH
-    // the refill after this one then finds its chunk in L2 instead of waiting on a DRAM row
-    if ((uint64_t)gw * 4ull + 128ull <= nbytes) {
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(src + 64));
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(src + 96));
-    }
-#endif
   } else if (take) {
 #pragma unroll
     for (uint32_t k = 0; k < 4; k++) {
@@ -504,16 +455,16 @@ struct DsAcc {
 // MODE 0: plain decode (ts, value) ; 1: fused 5-tuple-less downsample (sum, count, min, max);
 // 2: downsample + last (+ lastAt scratch).
 template <bool INT_OPT, int MODE>
-__global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? M3_DEC_MIN_BLOCKS_DS : M3_DEC_MIN_BLOCKS)
+__global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? DEC_MIN_BLOCKS_DS : DEC_MIN_BLOCKS)
     decode_kernel(const DecodeParams p) {
   // MODE 0: plain decode, series-major output [series][point]; 3: plain decode, point-major output
   // [point][series] (every step's 32 lanes store 32 consecutive elements: coalesced 256-byte rows);
   // 1: fused downsample (sum, count, min, max); 2: + last / lastAt
-  constexpr bool RING64 = ((MODE == 1 || MODE == 2 || MODE == 3) && M3_DEC_RING64) || M3_DEC_RING64_PLAIN;
+  // The fused-downsample and point-major kernels read the ring as 8-byte pairs; series-major decode keeps the
+  // 16-byte reads (the pairs cost more shared-memory wavefronts, see the parse).
+  constexpr bool RING64 = (MODE != 0);
   constexpr bool DS = (MODE == 1 || MODE == 2), LAST = (MODE == 2), PLAIN = (MODE == 0 || MODE == 3),
                  PM = (MODE == 3);
-  constexpr int CHK = (MODE == 0) ? M3_DEC_CHK : M3_DEC_CHK_WIDE;
-  constexpr int TRIGGER = (MODE == 0) ? DEC_TRIGGER : M3_DEC_TRIGGER_WIDE;
   extern __shared__ __align__(16) uint32_t smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -665,7 +616,7 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? M3_
   for (;;) {  // one group of DEC_GROUP datapoints per iteration
     if (!__any_sync(FULL_MASK, live)) break;
 
-    // ---- ring maintenance (every M3_DEC_CHK datapoints) ----
+    // ---- ring maintenance (every DEC_CHK datapoints) ----
     // A refill EVENT is warp-wide: it first waits for the previous event's copies
     // (issued many datapoints ago, so normally landed), then every lane with room
     // takes another 16-word chunk.  Lanes that nevertheless run dry fall back to
@@ -674,8 +625,8 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? M3_
       const bool active = live;
       const uint32_t cw = s.pos >> 5;
       int avail = (int)(filled - cw);
-      if (__any_sync(FULL_MASK, active && (avail <= TRIGGER ||
-                                           ((int)(safe - cw) < M3_DEC_SAFE_MIN && filled > safe)))) {
+      if (__any_sync(FULL_MASK, active && (avail <= DEC_TRIGGER ||
+                                           ((int)(safe - cw) < DEC_SAFE_MIN && filled > safe)))) {
         cp_async_wait_all();
         __syncwarp();
         if (avail < 0) {  // the slow path skipped past the ring (annotation): restart at cw
@@ -687,10 +638,10 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? M3_
         for (int rep = 0; rep < 3; rep++) {
           // first pass: everyone with room tops up when someone is at the trigger level;
           // later passes only serve lanes that are still short (start-up / restart)
-          const bool trig = __any_sync(FULL_MASK, active && avail <= TRIGGER);
+          const bool trig = __any_sync(FULL_MASK, active && avail <= DEC_TRIGGER);
           if (!trig) break;
           const uint32_t fmask =
-              __ballot_sync(FULL_MASK, active && avail <= (rep == 0 ? DEC_ACCEPT : TRIGGER));
+              __ballot_sync(FULL_MASK, active && avail <= (rep == 0 ? DEC_ACCEPT : DEC_TRIGGER));
           if (!fmask) break;
           ring_fill(ring_lane_addr, p.streams, p.streams_bytes, (fmask >> lane) & 1u, gbase + filled,
                     (filled >> 2) & (DEC_QUADS - 1));
@@ -708,12 +659,12 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? M3_
     }
 
     // Hot-path conditions that cannot change while the group stays on the hot path,
-    // checked once with margins for M3_DEC_CHK datapoints of <= 80 bits each: words
+    // checked once with margins for DEC_CHK datapoints of <= 80 bits each: words
     // landed, distance to the end of the stream, not the first datapoint and no
     // wrap of prev_time to 0 (first <=> PrevTime == 0, timestamp_iterator.go:89),
     // float mode.
-    bool pre_ok = fast_en && (((s.pos + 80u * (CHK - 1)) >> 5) + DEC_FAST_WORDS <= safe) &&
-                  (s.pos + 80u * CHK <= s.end) && (s.prev_time > 0) &&
+    bool pre_ok = fast_en && (((s.pos + 80u * (DEC_CHK - 1)) >> 5) + DEC_FAST_WORDS <= safe) &&
+                  (s.pos + 80u * DEC_CHK <= s.end) && (s.prev_time > 0) &&
                   ((uint64_t)s.prev_delta < (1ull << 60)) && (!INT_OPT || s.is_float);
     if (DS) {
       // fused downsample, additionally: timestamps strictly increasing in steps of at most one
@@ -725,14 +676,14 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? M3_
       // (a finished lane keeps d < 0 and delta == 0: the hot path's advance test needs no `active`)
       acc.d = live ? (int64_t)((uint64_t)s.prev_time - (uint64_t)acc.w_end) : -1ll;
       pre_ok = pre_ok && acc.in_open && acc.cur_w == acc.hi_w && s.prev_delta > 0 && s.prev_delta <= p.window &&
-               (uint32_t)acc.cur_w + (uint32_t)CHK < p.n_windows;
+               (uint32_t)acc.cur_w + (uint32_t)DEC_CHK < p.n_windows;
     }
     // one vote per group: the per-datapoint vote below then only looks at the header bits.  The flag is
     // warp-uniform: a general-path datapoint (taken by the whole warp) clears it for the rest of the group.
     bool group_ok = __all_sync(FULL_MASK, pre_ok || !live);
 
 #pragma unroll
-    for (int rr = 0; rr < CHK; rr++) {
+    for (int rr = 0; rr < DEC_CHK; rr++) {
       const bool active = live;
       const uint32_t cw = s.pos >> 5;
       int64_t t = 0;
@@ -1137,7 +1088,7 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? M3_
       dt += DEC_GROUP;
       dv += DEC_GROUP;
     }
-    group_row0 += CHK;
+    group_row0 += DEC_CHK;
   }
   cp_async_wait_all();
 
@@ -1169,19 +1120,7 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? M3_
 
 template <bool INT_OPT, int MODE>
 static cudaError_t launch_one(const DecodeParams &p, cudaStream_t stream) {
-  constexpr size_t warp_smem = DEC_WARP_SMEM_PLAIN;
-  size_t smem = warp_smem * DEC_WARPS;
-  // tuning knob: M3TSZ_DEC_CAP_BLOCKS=N pads the block's shared memory so that at most N blocks are
-  // resident per SM (228 KB per SM, 1 KB reserved per block)
-  static const int cap_blocks = [] {
-    const char *e = getenv("M3TSZ_DEC_CAP_BLOCKS");
-    return e ? atoi(e) : 0;
-  }();
-  if (cap_blocks > 0) {
-    const size_t per = (228u * 1024u) / (size_t)cap_blocks - 1024u;
-    if (per > smem) smem = per & ~(size_t)1023;
-    if (smem > 227u * 1024u) smem = 227u * 1024u;
-  }
+  constexpr size_t smem = DEC_WARP_SMEM_PLAIN * DEC_WARPS;
   cudaError_t e = cudaFuncSetAttribute(decode_kernel<INT_OPT, MODE>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
@@ -1189,12 +1128,8 @@ static cudaError_t launch_one(const DecodeParams &p, cudaStream_t stream) {
   // L1, which holds the fills in flight (cp.async.ca allocates a line per request).  Measured on an H100 SXM (700 W, 1980 MHz) at
   // 500 k x 1440, int-optimised (ms, carveout 100 / 132 / 164 / 196 / 228 KB): point-major decode 8.22 / 7.59 /
   // 7.60 / 7.58 / 8.57, fused downsample 6.36 / 5.37 / 5.00 / 4.98 / 5.78.  So: plain decode 4 blocks + 92 KB
-  // of L1, fused downsample 5 blocks + 60 KB.  M3TSZ_DEC_CARVEOUT_KB overrides (tuning).
-  static const int carveout_env = [] {
-    const char *c = getenv("M3TSZ_DEC_CARVEOUT_KB");
-    return c ? atoi(c) : 0;
-  }();
-  const int carveout_kb = carveout_env > 0 ? carveout_env : ((MODE == 1 || MODE == 2) ? 196 : 164);
+  // of L1, fused downsample 5 blocks + 60 KB.
+  constexpr int carveout_kb = (MODE == 1 || MODE == 2) ? 196 : 164;
   e = cudaFuncSetAttribute(decode_kernel<INT_OPT, MODE>, cudaFuncAttributePreferredSharedMemoryCarveout,
                            carveout_kb * 100 / 228);
   if (e != cudaSuccess) return e;

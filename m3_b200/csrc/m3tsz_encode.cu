@@ -14,7 +14,6 @@
 //   m3tsz/encoder.go:90-250, m3tsz/timestamp_encoder.go:72-259,
 //   m3tsz/float_encoder_iterator.go:69-103, m3tsz/int_sig_bits_tracker.go:35-91,
 //   m3tsz/m3tsz.go:78-119, ostream.go:133-221, scheme.go:198-220.
-#include <cstdlib>
 #include <cstring>
 #include <cub/device/device_scan.cuh>
 #include <cuda.h>  // CUtensorMap (types only: the encoder is resolved through cudaGetDriverEntryPoint)
@@ -27,71 +26,49 @@ namespace m3tsz {
 constexpr int ENC_WARPS = 4;
 constexpr int ENC_STRIDE = 33;
 constexpr int ENC_IN_T = 8;     // datapoints per input tile of the series-major stage (double buffered, cp.async)
-#ifndef M3_ENC_OUT_W
 // output tile words per lane (smaller tile = more L1): the 24 words that 16-byte flushes used, plus 4 for the
 // larger leftover of whole-sector flushes, so a flush cycle still adds about as many words as before
-#define M3_ENC_OUT_W 28
-#endif
+constexpr int ENC_OUT_W = 28;
 // Residency the launch bounds promise.  The series-major stage (IN = 0) uses ~48 KB of shared memory per block,
 // so the 132 KB carveout below holds 2 of them; the point-major stage (IN = 1) uses ~31 KB and fits 4; the Gauge
 // stage (IN = 2) has no input tiles and fits more.
-#ifndef M3_ENC_MIN_BLOCKS
-#define M3_ENC_MIN_BLOCKS 2
-#endif
-#ifndef M3_ENC_MIN_BLOCKS_PM
-#define M3_ENC_MIN_BLOCKS_PM 4
-#endif
-#ifndef M3_ENC_MIN_BLOCKS_AGG
-#define M3_ENC_MIN_BLOCKS_AGG 4
-#endif
-#ifndef M3_ENC_UNROLL_PM
-#define M3_ENC_UNROLL_PM 0  // 1: unroll the datapoint loop over one input tile (larger code, was slower)
-#endif
-constexpr int ENC_OUT_W = M3_ENC_OUT_W;   // output tile words per lane
+constexpr int ENC_MIN_BLOCKS = 2;
+constexpr int ENC_MIN_BLOCKS_PM = 4;
+constexpr int ENC_MIN_BLOCKS_AGG = 4;
 constexpr int ENC_GUARD = 10;   // words a single datapoint (no annotation) may add
 constexpr int ENC_OUT_TILE_WORDS = ENC_OUT_W * ENC_STRIDE;
 // A flush writes whole 32-byte sectors and leaves up to 7 words in the tile.  The tile is flushed once it holds
 // more than ENC_OUT_W - ENC_GUARD words; that must be at least one sector, so every flush makes room.
 static_assert(ENC_OUT_W - ENC_GUARD >= 8, "output tile too small for sector flushes");
-#ifndef M3_ENC_IN_T_PM
-// rows per input tile of the point-major input stage (IN = 1).  With tensor copies (M3_ENC_BULK_PM = 2, which do
-// not allocate L1 lines) one copy per array costs the same whatever the box; the tile size sets the shared memory
-// per warp and with it the residency.  Measured with M3_ENC_NSTAGE_PM (enc_carveout_kb() has the numbers):
-// 4 x 2 (4 blocks at 132 KB) was the fastest; 2 x 2 (5 blocks), 2 x 4 and 4 x 3 (3 blocks) were slower.
-#define M3_ENC_IN_T_PM 4
-#endif
-#ifndef M3_ENC_NSTAGE_PM
+// rows per input tile of the point-major input stage (IN = 1).  Tensor copies do not allocate L1 lines, so one
+// copy per array costs the same whatever the box; the tile size sets the shared memory per warp and with it the
+// residency.  Measured with ENC_NSTAGE_PM (ENC_CARVEOUT_KB has the numbers): 4 x 2 (4 blocks at 132 KB) was the
+// fastest; 2 x 2 (5 blocks), 2 x 4 and 4 x 3 (3 blocks) were slower.
+constexpr int ENC_IN_T_PM = 4;
 // input tiles in flight per warp in the point-major stage (a ring of stages, one mbarrier each)
-#define M3_ENC_NSTAGE_PM 2
-#endif
+constexpr int ENC_NSTAGE_PM = 2;
 // input stage IN: 0 series-major tiles (8 rows: one 64-byte segment per series and array), 1 point-major
 // tiles, 2 Gauge aggregates read directly (no input tiles)
-#ifndef M3_ENC_BULK_PM
-// 1: the point-major input stage (IN = 1) fills its tiles with TMA 1-D bulk copies (cp.async.bulk, one 256-byte
-// row of 32 series per copy, issued by one lane, completion on a per-warp mbarrier) whenever a batch is a full
-// warp of equally long series and the arrays / row pitch are 16-byte aligned; other batches keep the lane-local
-// 8-byte cp.async fills.  A tile row is then 32 datapoints exactly (no padding column: bulk destinations must be
-// 16-byte aligned and the lane-local reads are conflict-free either way).
-// 2: the same tiles by TMA TENSOR copies: the arrays are described as 2-D tensors [points][series] of 8-byte
-// elements (cuTensorMapEncodeTiled, box = IN_T rows x 32 series), so one cp.async.bulk.tensor.2d per array moves a
-// whole tile; rows past the end and series past n_series are zero-filled by the hardware, which makes ragged
-// batches and the last partial tile the same code.  Needs 16-byte aligned arrays and an even n_series < 2^31,
-// else the cp.async fills.
-#define M3_ENC_BULK_PM 2
-#endif
 template <int IN>
 __host__ __device__ constexpr int enc_in_t() {
-  return IN == 1 ? M3_ENC_IN_T_PM : ENC_IN_T;
+  return IN == 1 ? ENC_IN_T_PM : ENC_IN_T;
 }
 template <int IN>
 __host__ __device__ constexpr int enc_nstage() {
-  return IN == 1 ? M3_ENC_NSTAGE_PM : 2;
+  return IN == 1 ? ENC_NSTAGE_PM : 2;
 }
+// The point-major stage (IN = 1) fills its tiles by TMA tensor copies: the arrays are described as 2-D tensors
+// [points][series] of 8-byte elements (cuTensorMapEncodeTiled, box = IN_T rows x 32 series), so one
+// cp.async.bulk.tensor.2d per array moves a whole tile; rows past the end and series past n_series are
+// zero-filled by the hardware, which makes ragged batches and the last partial tile the same code.  A tile row is
+// then 32 datapoints exactly (no padding column: the copies' destinations must be 16-byte aligned, and the
+// lane-local reads are conflict-free either way).  Needs 16-byte aligned arrays and an even n_series < 2^31, else
+// the stage keeps the lane-local 8-byte cp.async fills.
 template <int IN>
-__host__ __device__ constexpr int enc_bulk() {
-  return IN == 1 ? M3_ENC_BULK_PM : 0;
+__host__ __device__ constexpr bool enc_bulk() {
+  return IN == 1;
 }
-// the two tensor maps of the point-major input arrays (M3_ENC_BULK_PM == 2), a __grid_constant__ kernel parameter
+// the two tensor maps of the point-major input arrays, a __grid_constant__ kernel parameter
 struct EncTensorMaps {
   alignas(64) CUtensorMap ts;
   alignas(64) CUtensorMap val;
@@ -107,7 +84,7 @@ __host__ __device__ constexpr size_t enc_warp_smem() {
   const size_t raw =
       ((IN == 0 || IN == 1) ? 2 * (size_t)enc_nstage<IN>() * (enc_in_t<IN>() * enc_in_stride<IN>()) * 8 : 0) +
       (size_t)ENC_OUT_TILE_WORDS * 4 + (enc_bulk<IN>() ? 8 * enc_nstage<IN>() : 0);  // (+ one mbarrier per stage)
-  return enc_bulk<IN>() == 2 ? ((raw + 127) & ~(size_t)127) : raw;  // tensor copies land on 128-byte boundaries
+  return enc_bulk<IN>() ? ((raw + 127) & ~(size_t)127) : raw;  // tensor copies land on 128-byte boundaries
 }
 
 struct EncLane {
@@ -662,24 +639,17 @@ __device__ __forceinline__ uint32_t enc_smem_addr(const void *p) {
 __device__ __forceinline__ void enc_cp_async8(uint32_t dst, const void *src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(dst), "l"(src) : "memory");
 }
-// ---- TMA 1-D bulk copies + mbarrier (M3_ENC_BULK_PM) ----
+// ---- TMA tensor copies + mbarrier (point-major input stage) ----
 __device__ __forceinline__ void enc_mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count) : "memory");
 }
 __device__ __forceinline__ void enc_mbar_init_fence() {
-  // make the initialised barriers visible to the async proxy (the bulk copies' complete_tx)
+  // make the initialised barriers visible to the async proxy (the tensor copies' complete_tx)
   asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
 }
 __device__ __forceinline__ void enc_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory");
-}
-// global -> shared bulk copy of `bytes` (multiple of 16; both addresses 16-byte aligned), completion counted
-// in bytes on the mbarrier
-__device__ __forceinline__ void enc_bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
 }
 // one box of a 2-D tensor (tensor map in param space) -> shared memory; c0 = innermost coordinate
 __device__ __forceinline__ void enc_tma_2d(uint32_t dst, const CUtensorMap *tm, int c0, int c1, uint32_t bar) {
@@ -719,13 +689,8 @@ __device__ __forceinline__ void enc_mbar_wait(uint32_t bar, uint32_t parity) {
 //         (count == 0: skipped) -- the tile aggregation's re-encode without a gather pass.
 template <bool INT_OPT, bool PACKED, int IN>
 __global__ void __launch_bounds__(ENC_WARPS * 32,
-                                  (IN == 2) ? M3_ENC_MIN_BLOCKS_AGG : (IN == 1 ? M3_ENC_MIN_BLOCKS_PM : M3_ENC_MIN_BLOCKS))
-    encode_kernel(const EncodeParams p
-#if M3_ENC_BULK_PM == 2
-                  ,
-                  const __grid_constant__ EncTensorMaps tmaps
-#endif
-    ) {
+                                  (IN == 2) ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
+    encode_kernel(const EncodeParams p, const __grid_constant__ EncTensorMaps tmaps) {
   extern __shared__ __align__(128) uint32_t smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -736,7 +701,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   constexpr uint32_t NSTAGE = (uint32_t)enc_nstage<IN>();  // input tiles in flight (ring of buffers)
   constexpr int IN_STRIDE = enc_in_stride<IN>();  // cells per tile row
   constexpr int IN_TILE_DW = IN_T * IN_STRIDE;  // one array (ts or val), one buffer
-  constexpr int BULK = enc_bulk<IN>();  // 0 cp.async fills, 1 1-D bulk copies per row, 2 one 2-D tensor copy per array
+  constexpr bool BULK = enc_bulk<IN>();  // one 2-D tensor copy per array and tile where the arrays allow it
   constexpr size_t WARP_SMEM = enc_warp_smem<IN>();
   uint8_t *wbase = reinterpret_cast<uint8_t *>(smem) + warp * WARP_SMEM;
   // in_tiles: [buffer][array (0 ts, 1 val)][row][lane]
@@ -748,11 +713,9 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   // through them (buffer = seq % NSTAGE, phase parity = (seq / NSTAGE) & 1), across batches
   const uint32_t mbar0 = BULK ? enc_smem_addr(out_tile + ENC_OUT_TILE_WORDS) : 0u;
   uint32_t bulk_seq = 0;
-#if M3_ENC_BULK_PM == 2
-  const bool bulk_args = BULK && tmaps.ok != 0;
-#else
-  const bool bulk_args = BULK && ((((uintptr_t)p.ts | (uintptr_t)p.val) & 15u) == 0) && ((p.n_series & 1ull) == 0);
-#endif
+  // the tiles come by tensor copy (they zero-fill what is out of range, so they serve every batch) unless the
+  // host could not describe the arrays
+  const bool bulk = BULK && tmaps.ok != 0;
   if (BULK) {
     if (lane == 0) {
       for (uint32_t b = 0; b < NSTAGE; b++) enc_mbar_init(mbar0 + 8u * b, 1);
@@ -763,21 +726,6 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
 
   const uint64_t n_batches = (p.n_series + 31) >> 5;
   const uint64_t warp_slot = (uint64_t)blockIdx.x * ENC_WARPS + warp;  // PACKED: scratch slot set
-  if (PACKED && p.stagger_ns) {
-    // Batches of equal length keep the persistent warps in lockstep: everyone packs bits (ALU
-    // bound, DRAM half idle), then everyone copies (DRAM bound, ALU idle).  Spreading the warps'
-    // phases over one batch period lets the copies of some overlap the bit packing of the others.
-    const uint32_t h = (uint32_t)warp_slot * 2654435761u;  // golden-ratio hash: phases mix within an SM
-    const uint64_t delay = ((uint64_t)(h >> 8) * p.stagger_ns) >> 24;
-    uint64_t t0, t1;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-    for (;;) {
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-      if (t1 - t0 >= delay) break;
-      const uint64_t rem = delay - (t1 - t0);
-      __nanosleep((unsigned)(rem > 20000 ? 20000 : rem));
-    }
-  }
   for (uint64_t batch_iter = 0;; batch_iter++) {
   uint64_t batch;
   if (PACKED) {
@@ -881,43 +829,18 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   const int st_arr = (lane >> 3) & 1;
   const int st_jo = lane >> 4;
   const bool uniform_n = __all_sync(FULL_MASK, !valid || n_pts == max_pts) && __all_sync(FULL_MASK, valid);
-  // this batch's tiles come by bulk copy: a full warp of series of one length (rows of 32 x 8 bytes, all in range)
-  // (tensor copies zero-fill what is out of range, so they serve every batch)
-  const bool bulk = BULK && bulk_args && (BULK == 2 || uniform_n);
   const uint32_t tile_base = bulk ? bulk_seq : 0u;  // buffer of tile t: (tile_base + t) % NSTAGE
   auto stage = [&](uint32_t tile) {
     const uint32_t row0 = tile * IN_T;
     if (row0 >= max_pts) return;
     const uint32_t buf = (tile_base + tile) % NSTAGE;
-#if M3_ENC_BULK_PM == 2
-    if (BULK == 2 && bulk) {
+    if (bulk) {
       if (lane == 0) {
         const uint32_t bar = mbar0 + buf * 8u;
         enc_mbar_expect_tx(bar, 2u * (uint32_t)IN_TILE_DW * 8u);  // the whole box counts, in range or not
         const uint32_t d0 = enc_smem_addr(in_tiles + (buf * 2u) * IN_TILE_DW);
         enc_tma_2d(d0, &tmaps.ts, (int)warp_s0, (int)row0, bar);
         enc_tma_2d(d0 + (uint32_t)IN_TILE_DW * 8u, &tmaps.val, (int)warp_s0, (int)row0, bar);
-      }
-      return;
-    }
-#endif
-    if (BULK == 1 && bulk) {
-      if (lane == 0) {
-        const uint32_t bar = mbar0 + buf * 8u;
-        const uint32_t nrow = (max_pts - row0 < (uint32_t)IN_T) ? max_pts - row0 : (uint32_t)IN_T;
-        enc_mbar_expect_tx(bar, nrow * 512u);
-        const uint64_t *st = reinterpret_cast<const uint64_t *>(p.ts) + (uint64_t)row0 * p.n_series + warp_s0;
-        const uint64_t *sv = reinterpret_cast<const uint64_t *>(p.val) + (uint64_t)row0 * p.n_series + warp_s0;
-        const uint32_t d0 = enc_smem_addr(in_tiles + (buf * 2u) * IN_TILE_DW);
-#pragma unroll
-        for (int r = 0; r < IN_T; r++) {
-          if ((uint32_t)r < nrow) {
-            enc_bulk_g2s(d0 + (uint32_t)(r * IN_STRIDE) * 8u, st, 256u, bar);
-            enc_bulk_g2s(d0 + (uint32_t)(IN_TILE_DW + r * IN_STRIDE) * 8u, sv, 256u, bar);
-          }
-          st += p.n_series;
-          sv += p.n_series;
-        }
       }
       return;
     }
@@ -963,7 +886,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   if (STAGED) {  // the first NSTAGE - 1 tiles; the loop requests each next one as it starts a tile
     for (uint32_t t = 0; t + 1 < NSTAGE; t++) {
       stage(t);
-      if (!(BULK && bulk)) asm volatile("cp.async.commit_group;\n" ::: "memory");
+      if (!bulk) asm volatile("cp.async.commit_group;\n" ::: "memory");
     }
   }
   // direct input stages: element `row` of this lane's series
@@ -994,7 +917,6 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   uint64_t fb_pf1 = 0;
   bool sk_pf = false, sk_pf1 = false;
 
-  uint32_t iter = 0;
   int64_t t_pf = 0;
   uint64_t fb_pf = 0;
   if (!STAGED) {  // two rows in flight
@@ -1004,20 +926,9 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   bool steady = false;  // same s/ms/us/ns unit as the batch's and not the first datapoint
   bool hot_ok = false;  // steady, and float mode when int-optimised: both only change on the slow path
   const uint64_t *in_next = in_tiles + lane;  // this lane's ts cell of the row to fetch next (value: + one tile)
-  // Optional (-DM3_ENC_UNROLL_PM=1): the point-major stage walks a tile with a statically unrolled inner loop
-  // (the phase of `iter` inside the tile is the unroll index, so the tile tests below are compile-time).
-  // Measured slower (four copies of the three tiers do not pay for seven instructions).
-  constexpr int UNR = (IN == 1 && M3_ENC_UNROLL_PM) ? IN_T : 1;
-  bool more = true;
-  while (more) {
-#pragma unroll
-  for (int ph = 0; ph < UNR; ph++) {
-    if (iter >= max_pts) {  // warp-uniform (n_pts is 0 for lanes without a series)
-      more = false;
-      break;
-    }
-    const bool tile_first = UNR > 1 ? (ph == 0) : ((iter & (IN_T - 1)) == 0);
-    const bool tile_last = UNR > 1 ? (ph == IN_T - 1) : ((iter & (IN_T - 1)) == IN_T - 1);
+  for (uint32_t iter = 0; iter < max_pts; iter++) {  // warp-uniform (n_pts is 0 for lanes without a series)
+    const bool tile_first = (iter & (IN_T - 1)) == 0;
+    const bool tile_last = (iter & (IN_T - 1)) == IN_T - 1;
     const bool active = s.err == 0 && iter < n_pts && !(IN == 2 && sk_pf);  // (n_pts is 0 without a series)
 
     // ---- input pipeline: request tile t+NSTAGE-1, wait for tile t ----
@@ -1026,7 +937,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       stage(iter / IN_T + NSTAGE - 1);
       const uint32_t g = tile_base + iter / IN_T;  // (tile_base is 0 unless this batch is bulk-filled)
       const uint32_t buf = g % NSTAGE;
-      if (BULK && bulk) {
+      if (bulk) {
         enc_mbar_wait(mbar0 + buf * 8u, (g / NSTAGE) & 1u);  // every lane: the tile's bytes have landed
       } else {
         asm volatile("cp.async.commit_group;\n" ::: "memory");
@@ -1188,11 +1099,9 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
         }
       }
     }
-    iter++;
-  }  // ph
-  }  // while (more)
+  }
   if (STAGED) asm volatile("cp.async.wait_all;\n" ::: "memory");
-  if (BULK && bulk) bulk_seq += (max_pts + (uint32_t)IN_T - 1u) / (uint32_t)IN_T;  // every requested tile was waited for
+  if (bulk) bulk_seq += (max_pts + (uint32_t)IN_T - 1u) / (uint32_t)IN_T;  // every requested tile was waited for
 
   // ---- tail: end-of-stream marker + zero padding (scheme.go:198-211) ----
   uint64_t total_bits = 0;
@@ -1313,16 +1222,8 @@ constexpr size_t enc_block_smem() {
 //   warps took 7.43 and 6.06 ms: half-written sectors were what made more warps slower.
 // * with whole-sector flushes: 10.29 ms at 8 warps; 8.46 ms with 4-row tiles at 16 warps (132 KB), 9.31 at
 //   100 KB (3 blocks); 2-row tiles at 20 warps 8.52; 4-row x 3 stages at 164 KB (16 warps, 92 KB of L1) 8.57.
-// M3TSZ_ENC_CARVEOUT_KB=K overrides.
-static int enc_carveout_kb() {
-  static const int kb = [] {
-    const char *c = getenv("M3TSZ_ENC_CARVEOUT_KB");
-    return c && atoi(c) > 0 ? atoi(c) : 132;
-  }();
-  return kb;
-}
+constexpr int ENC_CARVEOUT_KB = 132;
 
-#if M3_ENC_BULK_PM == 2
 // Tensor maps of the point-major input arrays: ts / val as [points_stride][n_series] tensors of 8-byte elements,
 // box = enc_in_t<1>() rows x 32 series, no swizzle, zero fill outside.  ok = 0 when the arrays cannot be described
 // (then the kernel keeps its cp.async fills).
@@ -1340,7 +1241,7 @@ static void enc_build_tensor_maps(const EncodeParams &p, EncTensorMaps &tm) {
       f = nullptr;
     return reinterpret_cast<encode_tiled_fn>(f);
   }();
-  if (!fn || getenv("M3TSZ_ENC_NO_TMA")) return;
+  if (!fn) return;
   if (p.in_mode != 1 || !p.ts || !p.val) return;
   if ((((uintptr_t)p.ts | (uintptr_t)p.val) & 15u) != 0) return;
   if ((p.n_series & 1ull) != 0 || p.n_series >= (1ull << 31) || p.points_stride == 0 ||
@@ -1358,7 +1259,6 @@ static void enc_build_tensor_maps(const EncodeParams &p, EncTensorMaps &tm) {
                         CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   tm.ok = (a == CUDA_SUCCESS && b == CUDA_SUCCESS) ? 1 : 0;
 }
-#endif
 
 template <bool INT_OPT, bool PACKED, int IN>
 static cudaError_t launch_encode_one(const EncodeParams &p, cudaStream_t stream) {
@@ -1371,20 +1271,16 @@ static cudaError_t launch_encode_one(const EncodeParams &p, cudaStream_t stream)
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   e = cudaFuncSetAttribute(encode_kernel<INT_OPT, PACKED, IN>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                           enc_carveout_kb() * 100 / 228);
+                           ENC_CARVEOUT_KB * 100 / 228);
   if (e != cudaSuccess) return e;
   if (PACKED) {
     const uint64_t resident = encode_packed_resident_blocks();
     if (resident == 0) return cudaErrorInvalidValue;
     if (blocks > resident) blocks = resident;
   }
-#if M3_ENC_BULK_PM == 2
   EncTensorMaps tm;
   enc_build_tensor_maps(p, tm);  // (ok = 0 for the other input stages)
   encode_kernel<INT_OPT, PACKED, IN><<<(unsigned)blocks, ENC_WARPS * 32, smem, stream>>>(p, tm);
-#else
-  encode_kernel<INT_OPT, PACKED, IN><<<(unsigned)blocks, ENC_WARPS * 32, smem, stream>>>(p);
-#endif
   return cudaGetLastError();
 }
 
@@ -1397,7 +1293,7 @@ uint64_t encode_packed_resident_blocks() {
   int best = 0;
   auto probe = [&](auto kernel, size_t sm) {
     int n = 0;
-    cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, enc_carveout_kb() * 100 / 228);
+    cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, ENC_CARVEOUT_KB * 100 / 228);
     if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm) == cudaSuccess &&
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, ENC_WARPS * 32, sm) == cudaSuccess && n > best)
       best = n;

@@ -70,7 +70,6 @@ struct EncodeParams {
   unsigned long long *packed_cursor;   // bytes allocated so far (zero on entry)
   unsigned long long *batch_counter;   // work counter (zero on entry)
   uint32_t align;
-  uint64_t stagger_ns;  // start-up phase spread of the persistent warps (0 = none)
   // input stage (see encode_kernel): 0 series-major ts/val, 1 point-major ts/val, 2 Gauge aggregates
   int in_mode;
   const double *tile_sum, *tile_min, *tile_max, *tile_last;  // window-major [points_stride][n_series]
