@@ -397,12 +397,15 @@ __device__ __forceinline__ uint32_t smem_addr(const void *p) {
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 
+// The fills ask L2 for the whole 128-byte line (.L2::128B) of every 16-byte request: a 64-byte chunk is half a
+// line, and the lane fetches the other half about 9 datapoints later, long after its DRAM row has closed -- with
+// the hint, that half is already in L2 (DESIGN.md §3.2(c)).
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, uint32_t src_bytes) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes)
+  asm volatile("cp.async.ca.shared.global.L2::128B [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes)
                : "memory");
 }
 __device__ __forceinline__ void cp_async16_full(uint32_t dst, const void *src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16;\n" ::"r"(dst), "l"(src) : "memory");
+  asm volatile("cp.async.ca.shared.global.L2::128B [%0], [%1], 16;\n" ::"r"(dst), "l"(src) : "memory");
 }
 // Lane-local refill: the lane copies the 64-byte chunk at global word index gw
 // (a multiple of 16) of ITS OWN stream into quads slot_q0..slot_q0+3 of its own
