@@ -87,52 +87,36 @@ class BatchCodec:
         assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
         S = offsets.numel() - 1 if lengths is None else lengths.numel()
         dev = self.device
-        if lengths is not None or want_events or point_major:
-            if out is None:
-                shape = (max_points, S) if point_major else (S, max_points)
-                out = DecodeResult(
-                    ts=torch.empty(shape, dtype=torch.int64, device=dev),
-                    values=torch.empty(shape, dtype=torch.float64, device=dev),
-                    n_points=torch.empty(S, dtype=torch.int32, device=dev),
-                    status=torch.empty(S, dtype=torch.int32, device=dev),
-                    unit=torch.empty(S, dtype=torch.uint8, device=dev),
-                    annotations=(torch.empty((S, 16), dtype=torch.uint8, device=dev)
-                                 if want_annotations else None))
-            ex = capi.DecodeExtras()
-            ex.d_lengths = lengths.data_ptr() if lengths is not None else None
-            ex.point_major = 1 if point_major else 0
-            if want_events:
-                if out.unit_first is None:
-                    out.unit_first = torch.empty(S, dtype=torch.uint8, device=dev)
-                if out.events is None or out.events.shape[0] < want_events:
-                    out.events = torch.zeros((int(want_events), 32), dtype=torch.uint8, device=dev)
-                if out.event_count is None:
-                    out.event_count = torch.zeros(1, dtype=torch.int64, device=dev)
-                out.event_count.zero_()
-                ex.d_unit_first = out.unit_first.data_ptr()
-                ex.d_events = out.events.data_ptr()
-                ex.events_capacity = int(out.events.shape[0])
-                ex.d_event_count = out.event_count.data_ptr()
-            rc = capi.lib().m3tsz_decode_batch_ex(
-                self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), S,
-                _ptr(out.ts), _ptr(out.values), max_points, _ptr(out.n_points), _ptr(out.status),
-                _ptr(out.unit), _ptr(out.annotations), C.byref(ex), _cuda_stream_ptr(dev))
-            self.ctx.check(rc, "m3tsz_decode_batch_ex")
-            return out
         if out is None:
+            shape = (max_points, S) if point_major else (S, max_points)
             out = DecodeResult(
-                ts=torch.empty((S, max_points), dtype=torch.int64, device=dev),
-                values=torch.empty((S, max_points), dtype=torch.float64, device=dev),
+                ts=torch.empty(shape, dtype=torch.int64, device=dev),
+                values=torch.empty(shape, dtype=torch.float64, device=dev),
                 n_points=torch.empty(S, dtype=torch.int32, device=dev),
                 status=torch.empty(S, dtype=torch.int32, device=dev),
                 unit=torch.empty(S, dtype=torch.uint8, device=dev),
                 annotations=(torch.empty((S, 16), dtype=torch.uint8, device=dev)
                              if want_annotations else None))
-        rc = capi.lib().m3tsz_decode_batch(
+        ex = capi.DecodeExtras()
+        ex.d_lengths = lengths.data_ptr() if lengths is not None else None
+        ex.point_major = 1 if point_major else 0
+        if want_events:
+            if out.unit_first is None:
+                out.unit_first = torch.empty(S, dtype=torch.uint8, device=dev)
+            if out.events is None or out.events.shape[0] < want_events:
+                out.events = torch.zeros((int(want_events), 32), dtype=torch.uint8, device=dev)
+            if out.event_count is None:
+                out.event_count = torch.zeros(1, dtype=torch.int64, device=dev)
+            out.event_count.zero_()
+            ex.d_unit_first = out.unit_first.data_ptr()
+            ex.d_events = out.events.data_ptr()
+            ex.events_capacity = int(out.events.shape[0])
+            ex.d_event_count = out.event_count.data_ptr()
+        rc = capi.lib().m3tsz_decode_batch_ex(
             self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), S,
             _ptr(out.ts), _ptr(out.values), max_points, _ptr(out.n_points), _ptr(out.status),
-            _ptr(out.unit), _ptr(out.annotations), _cuda_stream_ptr(dev))
-        self.ctx.check(rc, "m3tsz_decode_batch")
+            _ptr(out.unit), _ptr(out.annotations), C.byref(ex), _cuda_stream_ptr(dev))
+        self.ctx.check(rc, "m3tsz_decode_batch_ex")
         return out
 
     def decode_downsample(self, streams, offsets, range_start_ns, window_ns, n_windows,
@@ -141,14 +125,14 @@ class BatchCodec:
         assert offsets.dtype == torch.int64 and offsets.is_cuda
         S = offsets.numel() - 1
         dev = self.device
-        if want_last:
-            if out is None:
-                mk = lambda dt: torch.empty((n_windows, S), dtype=dt, device=dev)
-                out = DownsampleResult(
-                    sum=mk(torch.float64), count=mk(torch.int64), min=mk(torch.float64),
-                    max=mk(torch.float64), n_points=torch.empty(S, dtype=torch.int32, device=dev),
-                    status=torch.empty(S, dtype=torch.int32, device=dev), last=mk(torch.float64),
-                    last_at=mk(torch.int64))
+        if out is None:
+            mk = lambda dt: torch.empty((n_windows, S), dtype=dt, device=dev)
+            out = DownsampleResult(
+                sum=mk(torch.float64), count=mk(torch.int64), min=mk(torch.float64), max=mk(torch.float64),
+                n_points=torch.empty(S, dtype=torch.int32, device=dev),
+                status=torch.empty(S, dtype=torch.int32, device=dev),
+                last=mk(torch.float64) if want_last else None, last_at=mk(torch.int64) if want_last else None)
+        if want_last:  # a different kernel: it also keeps Gauge.Last() / LastAt()
             rc = capi.lib().m3tsz_decode_downsample_last_batch(
                 self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), S,
                 int(range_start_ns), int(window_ns), int(n_windows), _ptr(out.sum), _ptr(out.count),
@@ -156,19 +140,10 @@ class BatchCodec:
                 _ptr(out.status), _cuda_stream_ptr(dev))
             self.ctx.check(rc, "m3tsz_decode_downsample_last_batch")
             return out
-        if out is None:
-            out = DownsampleResult(
-                sum=torch.empty((n_windows, S), dtype=torch.float64, device=dev),
-                count=torch.empty((n_windows, S), dtype=torch.int64, device=dev),
-                min=torch.empty((n_windows, S), dtype=torch.float64, device=dev),
-                max=torch.empty((n_windows, S), dtype=torch.float64, device=dev),
-                n_points=torch.empty(S, dtype=torch.int32, device=dev),
-                status=torch.empty(S, dtype=torch.int32, device=dev))
         rc = capi.lib().m3tsz_decode_downsample_batch(
             self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), S,
             int(range_start_ns), int(window_ns), int(n_windows), _ptr(out.sum), _ptr(out.count),
-            _ptr(out.min), _ptr(out.max), _ptr(out.n_points), _ptr(out.status),
-            _cuda_stream_ptr(dev))
+            _ptr(out.min), _ptr(out.max), _ptr(out.n_points), _ptr(out.status), _cuda_stream_ptr(dev))
         self.ctx.check(rc, "m3tsz_decode_downsample_batch")
         return out
 
@@ -199,21 +174,14 @@ class BatchCodec:
         a_off = a_ent = a_bytes = None
         if annotations is not None:
             a_off, a_ent, a_bytes = annotations
-        if point_major:
-            ex = capi.EncodeExtras(None, None, 1, 0)
-            rc = capi.lib().m3tsz_encode_batch_ex(
-                self.ctx.handle, C.byref(self.opts), _ptr(ts), _ptr(values), S, P, _ptr(n_points),
-                _ptr(start), int(unit), _ptr(units), _ptr(a_off), _ptr(a_ent), _ptr(a_bytes),
-                _ptr(out.out), out.out.shape[1], _ptr(out.out_len), _ptr(out.status), C.byref(ex),
-                _cuda_stream_ptr(dev))
-            self.ctx.check(rc, "m3tsz_encode_batch_ex")
-            return out
-        rc = capi.lib().m3tsz_encode_batch(
+        ex = capi.EncodeExtras()
+        ex.point_major_input = 1 if point_major else 0
+        rc = capi.lib().m3tsz_encode_batch_ex(
             self.ctx.handle, C.byref(self.opts), _ptr(ts), _ptr(values), S, P, _ptr(n_points),
             _ptr(start), int(unit), _ptr(units), _ptr(a_off), _ptr(a_ent), _ptr(a_bytes),
-            _ptr(out.out), out.out.shape[1], _ptr(out.out_len), _ptr(out.status),
+            _ptr(out.out), out.out.shape[1], _ptr(out.out_len), _ptr(out.status), C.byref(ex),
             _cuda_stream_ptr(dev))
-        self.ctx.check(rc, "m3tsz_encode_batch")
+        self.ctx.check(rc, "m3tsz_encode_batch_ex")
         return out
 
     def encode_packed(self, ts, values, start, unit=capi.UNIT_S, n_points=None, units=None,

@@ -20,6 +20,89 @@ using namespace m3tsz;
 
 using namespace m3tsz::host;
 
+static bool valid_align(uint32_t align) {
+  return align == 1 || align == 4 || align == 8 || align == 16 || align == 32 || align == 64;
+}
+
+// The stream addressing both decode entry points check, and the DecodeParams fields they share.
+static bool decode_params(const m3tsz_options *opts, const uint8_t *d_streams, uint64_t streams_bytes,
+                          const uint64_t *d_offsets, const uint64_t *d_lengths, uint64_t n_series,
+                          uint32_t *d_n_points, int32_t *d_status, DecodeParams &p) {
+  if (!d_streams || !d_offsets || ((uintptr_t)d_streams & 15u) ||
+      streams_bytes >= (1ull << 34))  // 32-bit word / byte offsets inside the kernel; split larger batches
+    return false;
+  memset(&p, 0, sizeof(p));
+  p.streams = d_streams;
+  p.streams_bytes = streams_bytes;
+  p.offsets = d_offsets;
+  p.lengths = d_lengths;
+  p.n_series = n_series;
+  p.default_unit = opts->default_time_unit;
+  p.n_points = d_n_points;
+  p.status = d_status;
+  return true;
+}
+
+// The inputs both encode entry points check (pointers, alignments, the annotation triple, and
+// point-major input, which takes no units or annotations), and the EncodeParams fields they share.
+static bool encode_params(const m3tsz_options *opts, const int64_t *d_ts, const double *d_val, uint64_t n_series,
+                          uint64_t points_stride, const uint32_t *d_n_points, const int64_t *d_start, int32_t unit,
+                          const uint8_t *d_units, const uint64_t *d_ann_series_off,
+                          const m3tsz_annotation_entry *d_ann_entries, const uint8_t *d_ann_bytes,
+                          uint64_t *d_out_len, int32_t *d_status, const m3tsz_encode_extras *extras,
+                          EncodeParams &p) {
+  if (!d_ts || !d_val || !d_start || !d_out_len || points_stride > 0xffffffffull || ((uintptr_t)d_ts & 7u) ||
+      ((uintptr_t)d_val & 7u))
+    return false;
+  if (d_ann_series_off && (!d_ann_entries || !d_ann_bytes)) return false;
+  const bool point_major = extras && extras->point_major_input;
+  if (point_major && (d_units || d_ann_series_off)) return false;
+  memset(&p, 0, sizeof(p));
+  p.ts = d_ts;
+  p.val = d_val;
+  p.n_series = n_series;
+  p.points_stride = points_stride;
+  p.n_points = d_n_points;
+  p.start = d_start;
+  p.unit = unit;
+  p.units = d_units;
+  p.ann_series_off = d_ann_series_off;
+  p.ann_entries = d_ann_entries;
+  p.ann_bytes = d_ann_bytes;
+  p.default_unit = opts->default_time_unit;
+  p.out_len = d_out_len;
+  p.status = d_status;
+  if (extras) {
+    p.last_value = extras->d_last_value;
+    p.out_bits = extras->d_out_bits;
+  }
+  p.in_mode = point_major ? 1 : 0;
+  return true;
+}
+
+// Packed mode: the kernel encodes into a set of context slots of slot_bytes each and appends
+// every finished stream at an `align`ed cursor (*d_total_bytes, zeroed by the caller) in d_packed.
+static int packed_params(m3tsz_ctx *ctx, uint64_t n_series, uint64_t slot_bytes, uint32_t align,
+                         uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_offsets,
+                         uint64_t *d_total_bytes, cudaStream_t st, EncodeParams &p) {
+  const uint64_t slots = encode_packed_scratch_slots(n_series);
+  if (slots == 0) return set_cuda_error(ctx, cudaGetLastError(), "encode_packed_scratch_slots");
+  void *scratch = nullptr, *ctr = nullptr;
+  int rc;
+  if ((rc = ensure(ctx, kSlotPackedSlots, slots * slot_bytes, &scratch))) return rc;
+  if ((rc = ensure(ctx, kSlotBatchCounter, 64, &ctr))) return rc;
+  CK(cudaMemsetAsync(ctr, 0, 64, st));
+  p.out = (uint8_t *)scratch;
+  p.out_stride = slot_bytes;
+  p.packed = d_packed;
+  p.packed_capacity = packed_capacity;
+  p.packed_off = d_offsets;
+  p.packed_cursor = reinterpret_cast<unsigned long long *>(d_total_bytes);
+  p.batch_counter = reinterpret_cast<unsigned long long *>(ctr);
+  p.align = align;
+  return M3TSZ_OK;
+}
+
 extern "C" {
 
 int m3tsz_version(void) { return M3TSZ_B200_VERSION; }
@@ -114,29 +197,20 @@ int m3tsz_decode_batch_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8
                           const m3tsz_decode_extras *ex, void *stream) {
   if (!ctx || !valid_opts(opts)) return M3TSZ_ERR_INVALID_ARG;
   if (n_series == 0) return M3TSZ_OK;
-  if (!d_streams || !d_offsets || !d_ts || !d_val || max_points == 0 ||
-      max_points >= (1ull << 27) || ((uintptr_t)d_streams & 15u) ||
-      streams_bytes >= (1ull << 34))  // 32-bit word / byte offsets inside the kernel; split larger batches
+  DecodeParams p;
+  if (!decode_params(opts, d_streams, streams_bytes, d_offsets, ex ? ex->d_lengths : nullptr, n_series,
+                     d_n_points, d_status, p) ||
+      !d_ts || !d_val || max_points == 0 || max_points >= (1ull << 27))
     return M3TSZ_ERR_INVALID_ARG;
   if (ex && ex->d_events && (!ex->d_event_count || ex->events_capacity == 0)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
-  DecodeParams p;
-  memset(&p, 0, sizeof(p));
-  p.streams = d_streams;
-  p.streams_bytes = streams_bytes;
-  p.offsets = d_offsets;
-  p.n_series = n_series;
-  p.default_unit = opts->default_time_unit;
   p.ts = d_ts;
   p.val = d_val;
   p.cap = max_points;
-  p.n_points = d_n_points;
-  p.status = d_status;
   p.unit_out = d_unit;
   p.ann_out = d_ann;
   if (ex) {
-    p.lengths = ex->d_lengths;
     p.unit_first_out = ex->d_unit_first;
     if (ex->d_events) {
       p.events = ex->d_events;
@@ -167,9 +241,10 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
                            void *stream) {
   if (!ctx || !valid_opts(opts)) return M3TSZ_ERR_INVALID_ARG;
   if (n_series == 0) return M3TSZ_OK;
-  if (!d_streams || !d_offsets || !d_sum || !d_count || !d_min || !d_max || window_ns <= 0 ||
-      n_windows == 0 || n_windows > 0x7fffffffu || ((uintptr_t)d_streams & 15u) ||
-      streams_bytes >= (1ull << 34) || (want_last && !d_last))
+  DecodeParams p;
+  if (!decode_params(opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, d_n_points, d_status, p) ||
+      !d_sum || !d_count || !d_min || !d_max || window_ns <= 0 || n_windows == 0 || n_windows > 0x7fffffffu ||
+      (want_last && !d_last))
     return M3TSZ_ERR_INVALID_ARG;
   // range_start + n_windows*window must not overflow int64
   if ((__int128)range_start_ns + (__int128)n_windows * (__int128)window_ns > (__int128)INT64_MAX)
@@ -178,18 +253,10 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   if (want_last && !d_last_at) {  // lastAt lives in context scratch
     void *sc = nullptr;
-    int rc = ensure(ctx, 12, (size_t)n_series * n_windows * 8, &sc);
+    int rc = ensure(ctx, kSlotWinLastAt, (size_t)n_series * n_windows * 8, &sc);
     if (rc) return rc;
     d_last_at = (int64_t *)sc;
   }
-  DecodeParams p;
-  memset(&p, 0, sizeof(p));
-  p.streams = d_streams;
-  p.streams_bytes = streams_bytes;
-  p.offsets = d_offsets;
-  p.lengths = d_lengths;
-  p.n_series = n_series;
-  p.default_unit = opts->default_time_unit;
   p.range_start = range_start_ns;
   p.window = window_ns;
   p.n_windows = n_windows;
@@ -199,8 +266,6 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
   p.ds_max = d_max;
   p.ds_last = d_last;
   p.ds_last_at = d_last_at;
-  p.n_points = d_n_points;
-  p.status = d_status;
   CK(launch_decode(p, opts->int_optimized != 0, want_last ? 2 : 1, (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
@@ -238,39 +303,15 @@ int m3tsz_encode_batch_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const int64
                           const m3tsz_encode_extras *extras, void *stream) {
   if (!ctx || !valid_opts(opts)) return M3TSZ_ERR_INVALID_ARG;
   if (n_series == 0) return M3TSZ_OK;
-  if (!d_ts || !d_val || !d_start || !d_out || !d_out_len || points_stride > 0xffffffffull ||
-      (out_stride & 15u) || out_stride == 0 || out_stride > (1ull << 33) ||
-      ((uintptr_t)d_out & 15u) || ((uintptr_t)d_ts & 7u) || ((uintptr_t)d_val & 7u))
+  EncodeParams p;
+  if (!encode_params(opts, d_ts, d_val, n_series, points_stride, d_n_points, d_start, unit, d_units,
+                     d_ann_series_off, d_ann_entries, d_ann_bytes, d_out_len, d_status, extras, p) ||
+      !d_out || (out_stride & 15u) || out_stride == 0 || out_stride > (1ull << 33) || ((uintptr_t)d_out & 15u))
     return M3TSZ_ERR_INVALID_ARG;
-  if (d_ann_series_off && (!d_ann_entries || !d_ann_bytes)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
-  EncodeParams p;
-  memset(&p, 0, sizeof(p));
-  p.ts = d_ts;
-  p.val = d_val;
-  p.n_series = n_series;
-  p.points_stride = points_stride;
-  p.n_points = d_n_points;
-  p.start = d_start;
-  p.unit = unit;
-  p.units = d_units;
-  p.ann_series_off = d_ann_series_off;
-  p.ann_entries = d_ann_entries;
-  p.ann_bytes = d_ann_bytes;
-  p.default_unit = opts->default_time_unit;
   p.out = d_out;
   p.out_stride = out_stride;
-  p.out_len = d_out_len;
-  p.status = d_status;
-  if (extras) {
-    p.last_value = extras->d_last_value;
-    p.out_bits = extras->d_out_bits;
-    if (extras->point_major_input) {
-      if (d_units || d_ann_series_off) return M3TSZ_ERR_INVALID_ARG;
-      p.in_mode = 1;
-    }
-  }
   CK(launch_encode(p, opts->int_optimized != 0, (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
@@ -311,61 +352,23 @@ int m3tsz_encode_batch_packed_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
                                  uint64_t packed_capacity, uint64_t *d_offsets, uint64_t *d_out_len,
                                  int32_t *d_status, uint64_t *d_total_bytes, const m3tsz_encode_extras *extras,
                                  void *stream) {
-  if (!ctx || !valid_opts(opts) || !d_total_bytes) return M3TSZ_ERR_INVALID_ARG;
-  if (!(align == 1 || align == 4 || align == 8 || align == 16 || align == 32 || align == 64))
-    return M3TSZ_ERR_INVALID_ARG;
+  if (!ctx || !valid_opts(opts) || !d_total_bytes || !valid_align(align)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   cudaStream_t st = (cudaStream_t)stream;
   CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
   if (n_series == 0) return M3TSZ_OK;
-  if (!d_ts || !d_val || !d_start || !d_packed || !d_offsets || !d_out_len ||
-      points_stride > 0xffffffffull || ((uintptr_t)d_packed & 63u) || ((uintptr_t)d_ts & 7u) ||
-      ((uintptr_t)d_val & 7u))
+  EncodeParams p;
+  if (!encode_params(opts, d_ts, d_val, n_series, points_stride, d_n_points, d_start, unit, d_units,
+                     d_ann_series_off, d_ann_entries, d_ann_bytes, d_out_len, d_status, extras, p) ||
+      !d_packed || !d_offsets || ((uintptr_t)d_packed & 63u))
     return M3TSZ_ERR_INVALID_ARG;
-  if (d_ann_series_off && (!d_ann_entries || !d_ann_bytes)) return M3TSZ_ERR_INVALID_ARG;
   if (slot_bytes == 0) slot_bytes = m3tsz_encode_bound_units(points_stride, d_units != nullptr);
   slot_bytes = (slot_bytes + 15) & ~15ull;
   if (slot_bytes > (1ull << 33)) return M3TSZ_ERR_INVALID_ARG;
-  const uint64_t slots = encode_packed_scratch_slots(n_series);
-  if (slots == 0) return set_cuda_error(ctx, cudaGetLastError(), "encode_packed_scratch_slots");
-  void *scratch = nullptr, *ctr = nullptr;
-  int rc;
-  if ((rc = ensure(ctx, 36, slots * slot_bytes, &scratch))) return rc;
-  if ((rc = ensure(ctx, 37, 64, &ctr))) return rc;
-  CK(cudaMemsetAsync(ctr, 0, 64, st));
-  EncodeParams p;
-  memset(&p, 0, sizeof(p));
-  p.ts = d_ts;
-  p.val = d_val;
-  p.n_series = n_series;
-  p.points_stride = points_stride;
-  p.n_points = d_n_points;
-  p.start = d_start;
-  p.unit = unit;
-  p.units = d_units;
-  p.ann_series_off = d_ann_series_off;
-  p.ann_entries = d_ann_entries;
-  p.ann_bytes = d_ann_bytes;
-  p.default_unit = opts->default_time_unit;
-  p.out = (uint8_t *)scratch;
-  p.out_stride = slot_bytes;
-  p.out_len = d_out_len;
-  p.status = d_status;
-  p.packed = d_packed;
-  p.packed_capacity = packed_capacity;
-  p.packed_off = d_offsets;
-  p.packed_cursor = reinterpret_cast<unsigned long long *>(d_total_bytes);
-  p.batch_counter = reinterpret_cast<unsigned long long *>(ctr);
-  p.align = align;
-  if (extras) {
-    p.last_value = extras->d_last_value;
-    p.out_bits = extras->d_out_bits;
-    if (extras->point_major_input) {
-      if (d_units || d_ann_series_off) return M3TSZ_ERR_INVALID_ARG;
-      p.in_mode = 1;
-    }
-  }
+  int rc = packed_params(ctx, n_series, slot_bytes, align, d_packed, packed_capacity, d_offsets, d_total_bytes,
+                         st, p);
+  if (rc) return rc;
   CK(launch_encode(p, opts->int_optimized != 0, st));
   ctx->launches++;
   return M3TSZ_OK;
@@ -376,13 +379,13 @@ int m3tsz_compact_streams(m3tsz_ctx *ctx, const uint8_t *d_slots, uint64_t slot_
                           uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_offsets,
                           void *stream) {
   if (!ctx || !d_offsets || (n_series && (!d_slots || !d_len || !d_packed))) return M3TSZ_ERR_INVALID_ARG;
-  if (!(align == 1 || align == 4 || align == 8 || align == 16 || align == 32 || align == 64)) return M3TSZ_ERR_INVALID_ARG;
+  if (!valid_align(align)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   cudaStream_t st = (cudaStream_t)stream;
   size_t tmp_bytes = compact_scan_tmp_bytes(n_series);
   void *tmp = nullptr;
-  int rc = ensure(ctx, 15, tmp_bytes, &tmp);
+  int rc = ensure(ctx, kSlotCompactTmp, tmp_bytes, &tmp);
   if (rc) return rc;
   CK(cudaMemsetAsync(ctx->d_flag, 0, sizeof(int32_t), st));
   CK(launch_compact(d_slots, slot_stride, d_len, n_series, align, d_packed, packed_capacity,
@@ -445,20 +448,22 @@ int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const
     CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
     return M3TSZ_OK;
   }
+  if (!valid_align(align) || !d_packed || !d_out_offsets || !d_out_len || ((uintptr_t)d_packed & 63u))
+    return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   // context scratch: window-major aggregates, then series-major tiles
   const size_t wb = (size_t)n_series * n_windows * 8;
   void *d_sum, *d_cnt, *d_min, *d_max, *d_last, *d_lat, *d_sst, *d_np, *d_es = nullptr;
   int rc;
-  if ((rc = ensure(ctx, 8, wb, &d_sum))) return rc;
-  if ((rc = ensure(ctx, 9, wb, &d_cnt))) return rc;
-  if ((rc = ensure(ctx, 10, wb, &d_min))) return rc;
-  if ((rc = ensure(ctx, 11, wb, &d_max))) return rc;
-  if ((rc = ensure(ctx, 12, wb, &d_lat))) return rc;
-  if ((rc = ensure(ctx, 38, wb, &d_last))) return rc;
-  if ((rc = ensure(ctx, 4, n_series * 4, &d_np))) return rc;
-  if ((rc = ensure(ctx, 5, n_series * 4, &d_sst))) return rc;
+  if ((rc = ensure(ctx, kSlotWinSum, wb, &d_sum))) return rc;
+  if ((rc = ensure(ctx, kSlotWinCount, wb, &d_cnt))) return rc;
+  if ((rc = ensure(ctx, kSlotWinMin, wb, &d_min))) return rc;
+  if ((rc = ensure(ctx, kSlotWinMax, wb, &d_max))) return rc;
+  if ((rc = ensure(ctx, kSlotWinLastAt, wb, &d_lat))) return rc;
+  if ((rc = ensure(ctx, kSlotWinLast, wb, &d_last))) return rc;
+  if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_np))) return rc;
+  if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_sst))) return rc;
   // 1. fused decode + Gauge windows (with `last`)
   rc = downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                        n_windows, (double *)d_sum, (int64_t *)d_cnt, (double *)d_min, (double *)d_max,
@@ -466,52 +471,35 @@ int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   if (rc) return rc;
   // 2. re-encode straight from the window-major aggregates (the encoder's input stage skips empty
   //    windows, stamps the window end and takes Gauge.ValueOf(agg_type)) into the packed buffer
-  {
-    if (!(align == 1 || align == 4 || align == 8 || align == 16 || align == 32 || align == 64))
-      return M3TSZ_ERR_INVALID_ARG;
-    if (!d_packed || !d_out_offsets || !d_out_len || ((uintptr_t)d_packed & 63u)) return M3TSZ_ERR_INVALID_ARG;
-    CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
-    const uint64_t slot_bytes = m3tsz_encode_bound(n_windows);
-    const uint64_t slots = encode_packed_scratch_slots(n_series);
-    if (slots == 0) return set_cuda_error(ctx, cudaGetLastError(), "encode_packed_scratch_slots");
-    void *scratch = nullptr, *ctr = nullptr;
-    if ((rc = ensure(ctx, 36, slots * slot_bytes, &scratch))) return rc;
-    if ((rc = ensure(ctx, 37, 64, &ctr))) return rc;
-    CK(cudaMemsetAsync(ctr, 0, 64, st));
-    // every series' encoder starts at the tile range's start (the target block's start)
-    if ((rc = ensure(ctx, 39, n_series * 8, &d_es))) return rc;
-    CK(launch_fill_i64((int64_t *)d_es, start_ns, n_series, st));
-    EncodeParams p;
-    memset(&p, 0, sizeof(p));
-    p.n_series = n_series;
-    p.points_stride = n_windows;
-    p.start = (const int64_t *)d_es;
-    p.unit = out_unit;
-    p.default_unit = opts->default_time_unit;
-    p.out = (uint8_t *)scratch;
-    p.out_stride = slot_bytes;
-    p.out_len = d_out_len;
-    p.status = d_status;
-    p.packed = d_packed;
-    p.packed_capacity = packed_capacity;
-    p.packed_off = d_out_offsets;
-    p.packed_cursor = reinterpret_cast<unsigned long long *>(d_total_bytes);
-    p.batch_counter = reinterpret_cast<unsigned long long *>(ctr);
-    p.align = align;
-    p.in_mode = 2;
-    p.tile_sum = (const double *)d_sum;
-    p.tile_count = (const int64_t *)d_cnt;
-    p.tile_min = (const double *)d_min;
-    p.tile_max = (const double *)d_max;
-    p.tile_last = (const double *)d_last;
-    p.tile_src_status = (const int32_t *)d_sst;
-    p.tile_start = start_ns;
-    p.tile_step = step_ns;
-    p.agg_type = agg_type;
-    p.n_tiles_out = d_n_tiles;
-    CK(launch_encode(p, opts->int_optimized != 0, st));
-    ctx->launches += 2;
-  }
+  CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
+  EncodeParams p;
+  memset(&p, 0, sizeof(p));
+  if ((rc = packed_params(ctx, n_series, m3tsz_encode_bound(n_windows), align, d_packed, packed_capacity,
+                          d_out_offsets, d_total_bytes, st, p)))
+    return rc;
+  // every series' encoder starts at the tile range's start (the target block's start)
+  if ((rc = ensure(ctx, kSlotTileStarts, n_series * 8, &d_es))) return rc;
+  CK(launch_fill_i64((int64_t *)d_es, start_ns, n_series, st));
+  p.n_series = n_series;
+  p.points_stride = n_windows;
+  p.start = (const int64_t *)d_es;
+  p.unit = out_unit;
+  p.default_unit = opts->default_time_unit;
+  p.out_len = d_out_len;
+  p.status = d_status;
+  p.in_mode = 2;
+  p.tile_sum = (const double *)d_sum;
+  p.tile_count = (const int64_t *)d_cnt;
+  p.tile_min = (const double *)d_min;
+  p.tile_max = (const double *)d_max;
+  p.tile_last = (const double *)d_last;
+  p.tile_src_status = (const int32_t *)d_sst;
+  p.tile_start = start_ns;
+  p.tile_step = step_ns;
+  p.agg_type = agg_type;
+  p.n_tiles_out = d_n_tiles;
+  CK(launch_encode(p, opts->int_optimized != 0, st));
+  ctx->launches += 2;
   CK(launch_tiles_status((const int32_t *)d_sst, d_status, n_series, st));
   ctx->launches++;
   return M3TSZ_OK;
@@ -600,7 +588,7 @@ int m3tsz_checksum_batch(m3tsz_ctx *ctx, const uint8_t *d_streams, uint64_t stre
 // --------------------------------------------------------------------------
 // host-buffer variants
 // --------------------------------------------------------------------------
-static int m3tsz_decode_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *h_streams,
+int m3tsz_decode_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *h_streams,
                             uint64_t streams_bytes, const uint64_t *h_offsets, uint64_t n_series,
                             int64_t *h_ts, double *h_val, uint64_t max_points,
                             uint32_t *h_n_points, int32_t *h_status, uint8_t *h_unit,
@@ -610,16 +598,17 @@ static int m3tsz_decode_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opt
   if (!h_streams || !h_offsets || !h_ts || !h_val || max_points == 0) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  DrainStreams drain{ctx};
   void *d_streams, *d_off, *d_ts, *d_val, *d_n, *d_st, *d_unit = nullptr, *d_ann = nullptr;
   int rc;
-  if ((rc = ensure(ctx, 0, streams_bytes + 16, &d_streams))) return rc;
-  if ((rc = ensure(ctx, 1, (n_series + 1) * 8, &d_off))) return rc;
-  if ((rc = ensure(ctx, 2, n_series * max_points * 8, &d_ts))) return rc;
-  if ((rc = ensure(ctx, 3, n_series * max_points * 8, &d_val))) return rc;
-  if ((rc = ensure(ctx, 4, n_series * 4, &d_n))) return rc;
-  if ((rc = ensure(ctx, 5, n_series * 4, &d_st))) return rc;
-  if (h_unit && (rc = ensure(ctx, 6, n_series, &d_unit))) return rc;
-  if (h_ann && (rc = ensure(ctx, 7, n_series * sizeof(m3tsz_annotation_ref), &d_ann))) return rc;
+  if ((rc = ensure(ctx, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
+  if ((rc = ensure(ctx, kSlotSeriesIndex, (n_series + 1) * 8, &d_off))) return rc;
+  if ((rc = ensure(ctx, kSlotTs, n_series * max_points * 8, &d_ts))) return rc;
+  if ((rc = ensure(ctx, kSlotVal, n_series * max_points * 8, &d_val))) return rc;
+  if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_n))) return rc;
+  if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_st))) return rc;
+  if (h_unit && (rc = ensure(ctx, kSlotUnit, n_series, &d_unit))) return rc;
+  if (h_ann && (rc = ensure(ctx, kSlotAnnRefs, n_series * sizeof(m3tsz_annotation_ref), &d_ann))) return rc;
   // Chunked pipeline over two streams: the H2D copy of chunk c+1 overlaps the
   // kernel and the D2H copy of chunk c (PCIe is full duplex).
   cudaStream_t sts[2] = {ctx->stream, ctx->stream2};
@@ -658,21 +647,7 @@ static int m3tsz_decode_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opt
   return M3TSZ_OK;
 }
 
-int m3tsz_decode_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *h_streams,
-                            uint64_t streams_bytes, const uint64_t *h_offsets, uint64_t n_series,
-                            int64_t *h_ts, double *h_val, uint64_t max_points,
-                            uint32_t *h_n_points, int32_t *h_status, uint8_t *h_unit,
-                            m3tsz_annotation_ref *h_ann) {
-  const int rc = m3tsz_decode_batch_host_impl(ctx, opts, h_streams, streams_bytes, h_offsets, n_series, h_ts, h_val, max_points, h_n_points, h_status, h_unit, h_ann);
-  if (ctx && ctx->stream) {  // never return with copies from / into the caller's buffers in flight
-    DeviceGuard guard(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-    cudaStreamSynchronize(ctx->stream2);
-  }
-  return rc;
-}
-
-static int m3tsz_decode_downsample_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opts,
+int m3tsz_decode_downsample_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts,
                                        const uint8_t *h_streams, uint64_t streams_bytes,
                                        const uint64_t *h_offsets, uint64_t n_series,
                                        int64_t range_start_ns, int64_t window_ns,
@@ -684,18 +659,19 @@ static int m3tsz_decode_downsample_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_o
   if (!h_streams || !h_offsets || !h_sum || !h_count || !h_min || !h_max) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  DrainStreams drain{ctx};
   cudaStream_t st = ctx->stream;
   const size_t wb = (size_t)n_series * n_windows * 8;
   void *d_streams, *d_off, *d_sum, *d_cnt, *d_min, *d_max, *d_n, *d_st;
   int rc;
-  if ((rc = ensure(ctx, 0, streams_bytes + 16, &d_streams))) return rc;
-  if ((rc = ensure(ctx, 1, (n_series + 1) * 8, &d_off))) return rc;
-  if ((rc = ensure(ctx, 8, wb, &d_sum))) return rc;
-  if ((rc = ensure(ctx, 9, wb, &d_cnt))) return rc;
-  if ((rc = ensure(ctx, 10, wb, &d_min))) return rc;
-  if ((rc = ensure(ctx, 11, wb, &d_max))) return rc;
-  if ((rc = ensure(ctx, 4, n_series * 4, &d_n))) return rc;
-  if ((rc = ensure(ctx, 5, n_series * 4, &d_st))) return rc;
+  if ((rc = ensure(ctx, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
+  if ((rc = ensure(ctx, kSlotSeriesIndex, (n_series + 1) * 8, &d_off))) return rc;
+  if ((rc = ensure(ctx, kSlotWinSum, wb, &d_sum))) return rc;
+  if ((rc = ensure(ctx, kSlotWinCount, wb, &d_cnt))) return rc;
+  if ((rc = ensure(ctx, kSlotWinMin, wb, &d_min))) return rc;
+  if ((rc = ensure(ctx, kSlotWinMax, wb, &d_max))) return rc;
+  if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_n))) return rc;
+  if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_st))) return rc;
   CK(cudaMemcpyAsync(d_streams, h_streams, streams_bytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_off, h_offsets, (n_series + 1) * 8, cudaMemcpyHostToDevice, st));
   rc = m3tsz_decode_downsample_batch(ctx, opts, (const uint8_t *)d_streams, streams_bytes,
@@ -713,23 +689,7 @@ static int m3tsz_decode_downsample_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_o
   return M3TSZ_OK;
 }
 
-int m3tsz_decode_downsample_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts,
-                                       const uint8_t *h_streams, uint64_t streams_bytes,
-                                       const uint64_t *h_offsets, uint64_t n_series,
-                                       int64_t range_start_ns, int64_t window_ns,
-                                       uint32_t n_windows, double *h_sum, int64_t *h_count,
-                                       double *h_min, double *h_max, uint32_t *h_n_points,
-                                       int32_t *h_status) {
-  const int rc = m3tsz_decode_downsample_batch_host_impl(ctx, opts, h_streams, streams_bytes, h_offsets, n_series, range_start_ns, window_ns, n_windows, h_sum, h_count, h_min, h_max, h_n_points, h_status);
-  if (ctx && ctx->stream) {  // never return with copies from / into the caller's buffers in flight
-    DeviceGuard guard(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-    cudaStreamSynchronize(ctx->stream2);
-  }
-  return rc;
-}
-
-static int m3tsz_encode_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const int64_t *h_ts,
+int m3tsz_encode_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const int64_t *h_ts,
                             const double *h_val, uint64_t n_series, uint64_t points_stride,
                             const uint32_t *h_n_points, const int64_t *h_start, int32_t unit,
                             const uint8_t *h_units, const uint64_t *h_ann_series_off,
@@ -742,9 +702,10 @@ static int m3tsz_encode_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opt
   h_offsets[0] = 0;
   if (n_series == 0) return M3TSZ_OK;
   if (!h_ts || !h_val || !h_start || !h_packed) return M3TSZ_ERR_INVALID_ARG;
-  if (!(align == 1 || align == 4 || align == 8 || align == 16 || align == 32 || align == 64)) return M3TSZ_ERR_INVALID_ARG;
+  if (!valid_align(align)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  DrainStreams drain{ctx};
   cudaStream_t sts[2] = {ctx->stream, ctx->stream2};
   const uint64_t ann_total = h_ann_series_off ? ann_bytes_len + 16 * h_ann_series_off[n_series] : 0;
   const uint64_t out_stride = m3tsz_encode_bound_units(points_stride, h_units != nullptr) + ((ann_total + 15) & ~15ull);
@@ -753,18 +714,18 @@ static int m3tsz_encode_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opt
   int rc;
   // whole-batch device inputs that are small: start, n_points, annotations
   void *d_start, *d_np = nullptr, *d_aoff = nullptr, *d_aent = nullptr, *d_abytes = nullptr;
-  if ((rc = ensure(ctx, 1, (n_series + 1) * 8, &d_start))) return rc;
+  if ((rc = ensure(ctx, kSlotSeriesIndex, (n_series + 1) * 8, &d_start))) return rc;
   CK(cudaMemcpyAsync(d_start, h_start, n_series * 8, cudaMemcpyHostToDevice, sts[0]));
   if (h_n_points) {
-    if ((rc = ensure(ctx, 4, n_series * 4, &d_np))) return rc;
+    if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_np))) return rc;
     CK(cudaMemcpyAsync(d_np, h_n_points, n_series * 4, cudaMemcpyHostToDevice, sts[0]));
   }
   if (h_ann_series_off) {
     if (!h_ann_entries || (!h_ann_bytes && ann_bytes_len)) return M3TSZ_ERR_INVALID_ARG;
     const uint64_t n_ent = h_ann_series_off[n_series];
-    if ((rc = ensure(ctx, 7, (n_series + 1) * 8, &d_aoff))) return rc;
-    if ((rc = ensure(ctx, 13, n_ent * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
-    if ((rc = ensure(ctx, 14, ann_bytes_len, &d_abytes))) return rc;
+    if ((rc = ensure(ctx, kSlotAnnSeriesOff, (n_series + 1) * 8, &d_aoff))) return rc;
+    if ((rc = ensure(ctx, kSlotAnnEntries, n_ent * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
+    if ((rc = ensure(ctx, kSlotAnnBytes, ann_bytes_len, &d_abytes))) return rc;
     CK(cudaMemcpyAsync(d_aoff, h_ann_series_off, (n_series + 1) * 8, cudaMemcpyHostToDevice, sts[0]));
     if (n_ent)
       CK(cudaMemcpyAsync(d_aent, h_ann_entries, n_ent * sizeof(m3tsz_annotation_entry),
@@ -784,18 +745,17 @@ static int m3tsz_encode_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opt
   // every start is rounded up to `align`: budget the aligned worst case per stream
   const uint64_t packed_stride = (out_stride + align - 1) & ~(uint64_t)(align - 1);
   for (int i = 0; i < 2; i++) {
-    const int b = 16 + i * 10;
     ln[i].units = nullptr;
     ln[i].busy = false;
-    if ((rc = ensure(ctx, b + 0, ch * row_bytes, &ln[i].ts))) return rc;
-    if ((rc = ensure(ctx, b + 1, ch * row_bytes, &ln[i].val))) return rc;
-    if (h_units && (rc = ensure(ctx, b + 2, ch * points_stride, &ln[i].units))) return rc;
-    if ((rc = ensure(ctx, b + 3, ch * out_stride, &ln[i].out))) return rc;
-    if ((rc = ensure(ctx, b + 4, ch * 8, &ln[i].len))) return rc;
-    if ((rc = ensure(ctx, b + 5, ch * 4, &ln[i].st))) return rc;
-    if ((rc = ensure(ctx, b + 6, ch * packed_stride + 64, &ln[i].packed))) return rc;
-    if ((rc = ensure(ctx, b + 7, (ch + 1) * 8, &ln[i].off))) return rc;
-    if ((rc = ensure(ctx, b + 8, tmp_bytes, &ln[i].tmp))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 0), ch * row_bytes, &ln[i].ts))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 1), ch * row_bytes, &ln[i].val))) return rc;
+    if (h_units && (rc = ensure(ctx, lane_slot(i, 2), ch * points_stride, &ln[i].units))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 3), ch * out_stride, &ln[i].out))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 4), ch * 8, &ln[i].len))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 5), ch * 4, &ln[i].st))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 6), ch * packed_stride + 64, &ln[i].packed))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 7), (ch + 1) * 8, &ln[i].off))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 8), tmp_bytes, &ln[i].tmp))) return rc;
     if ((rc = ensure_stage(ctx, i, (ch + 1) * 8 + 8))) return rc;
   }
   CK(cudaMemsetAsync(ctx->d_flag, 0, 2 * sizeof(int32_t), sts[0]));
@@ -864,23 +824,6 @@ static int m3tsz_encode_batch_host_impl(m3tsz_ctx *ctx, const m3tsz_options *opt
   return M3TSZ_OK;
 }
 
-int m3tsz_encode_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const int64_t *h_ts,
-                            const double *h_val, uint64_t n_series, uint64_t points_stride,
-                            const uint32_t *h_n_points, const int64_t *h_start, int32_t unit,
-                            const uint8_t *h_units, const uint64_t *h_ann_series_off,
-                            const m3tsz_annotation_entry *h_ann_entries,
-                            const uint8_t *h_ann_bytes, uint64_t ann_bytes_len, uint32_t align,
-                            uint8_t *h_packed, uint64_t packed_capacity, uint64_t *h_offsets,
-                            uint64_t *h_out_len, int32_t *h_status) {
-  const int rc = m3tsz_encode_batch_host_impl(ctx, opts, h_ts, h_val, n_series, points_stride, h_n_points, h_start, unit, h_units, h_ann_series_off, h_ann_entries, h_ann_bytes, ann_bytes_len, align, h_packed, packed_capacity, h_offsets, h_out_len, h_status);
-  if (ctx && ctx->stream) {  // never return with copies from / into the caller's buffers in flight
-    DeviceGuard guard(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-    cudaStreamSynchronize(ctx->stream2);
-  }
-  return rc;
-}
-
 
 // --------------------------------------------------------------------------
 // Fetch path with host buffers: only compressed bytes go up, only the merged result
@@ -901,6 +844,7 @@ int m3tsz_fetch_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
     return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  DrainStreams drain{ctx};
   cudaStream_t sts[2] = {ctx->stream, ctx->stream2};
   // series per chunk: ~8 chunks, whole sequences of whole series
   uint64_t ch = (n_series + 7) / 8;
@@ -927,30 +871,24 @@ int m3tsz_fetch_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
   }
   void *d_streams, *d_off;
   int rc;
-  if ((rc = ensure(ctx, 0, streams_bytes + 16, &d_streams))) return rc;
-  if ((rc = ensure(ctx, 1, (n_seq + 1) * 8, &d_off))) return rc;
+  if ((rc = ensure(ctx, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
+  if ((rc = ensure(ctx, kSlotSeriesIndex, (n_seq + 1) * 8, &d_off))) return rc;
   struct Lane {
     void *ts, *val, *n, *st, *meta, *ots, *oval, *on, *ost;
   } ln[2];
   const size_t meta_words = (max_k + 1) + (max_r + 1) + (ch + 1);
   for (int i = 0; i < 2; i++) {
-    const int b = 16 + i * 10;
-    if ((rc = ensure(ctx, b + 0, max_q * max_points * 8, &ln[i].ts))) return rc;
-    if ((rc = ensure(ctx, b + 1, max_q * max_points * 8, &ln[i].val))) return rc;
-    if ((rc = ensure(ctx, b + 2, max_q * 4, &ln[i].n))) return rc;
-    if ((rc = ensure(ctx, b + 3, max_q * 4, &ln[i].st))) return rc;
-    if ((rc = ensure(ctx, b + 4, meta_words * 8, &ln[i].meta))) return rc;
-    if ((rc = ensure(ctx, b + 5, ch * out_cap * 8, &ln[i].ots))) return rc;
-    if ((rc = ensure(ctx, b + 6, ch * out_cap * 8, &ln[i].oval))) return rc;
-    if ((rc = ensure(ctx, b + 7, ch * 4, &ln[i].on))) return rc;
-    if ((rc = ensure(ctx, b + 8, ch * 4, &ln[i].ost))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 0), max_q * max_points * 8, &ln[i].ts))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 1), max_q * max_points * 8, &ln[i].val))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 2), max_q * 4, &ln[i].n))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 3), max_q * 4, &ln[i].st))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 4), meta_words * 8, &ln[i].meta))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 5), ch * out_cap * 8, &ln[i].ots))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 6), ch * out_cap * 8, &ln[i].oval))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 7), ch * 4, &ln[i].on))) return rc;
+    if ((rc = ensure(ctx, lane_slot(i, 8), ch * 4, &ln[i].ost))) return rc;
     if ((rc = ensure_stage(ctx, i, meta_words * 8))) return rc;
   }
-  auto fail = [&](int code) {  // never return with copies into the caller's buffers in flight
-    cudaStreamSynchronize(sts[0]);
-    cudaStreamSynchronize(sts[1]);
-    return code;
-  };
   CK(cudaMemcpyAsync(d_off, h_offsets, (n_seq + 1) * 8, cudaMemcpyHostToDevice, sts[0]));
   CK(cudaEventRecord(ctx->ev, sts[0]));
   CK(cudaStreamWaitEvent(sts[1], ctx->ev, 0));
@@ -964,40 +902,36 @@ int m3tsz_fetch_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
     const uint64_t k0 = h_replica_off[r0], k1 = h_replica_off[r1];
     const uint64_t q0 = h_slice_off[k0], q1 = h_slice_off[k1], nq = q1 - q0;
     const uint64_t b0 = h_offsets[q0], b1 = h_offsets[q1];
-    if (b1 < b0 || b1 > streams_bytes) return fail(M3TSZ_ERR_INVALID_ARG);
-    if (cudaStreamSynchronize(st) != cudaSuccess) return fail(M3TSZ_ERR_CUDA);  // lane buffers + staging are free again
+    if (b1 < b0 || b1 > streams_bytes) return M3TSZ_ERR_INVALID_ARG;
+    CK(cudaStreamSynchronize(st));  // lane buffers + staging are free again
     // iterator structure of the chunk, rebased to the chunk's first sequence / slice / replica
     uint64_t *m = (uint64_t *)ctx->h_stage[i];
     uint64_t *m_slice = m, *m_rep = m + (max_k + 1), *m_ser = m_rep + (max_r + 1);
     for (uint64_t j = k0; j <= k1; j++) m_slice[j - k0] = h_slice_off[j] - q0;
     for (uint64_t j = r0; j <= r1; j++) m_rep[j - r0] = h_replica_off[j] - k0;
     for (uint64_t j = s0; j <= s1; j++) m_ser[j - s0] = h_series_off[j] - r0;
-    if (cudaMemcpyAsync(L.meta, m, meta_words * 8, cudaMemcpyHostToDevice, st) != cudaSuccess)
-      return fail(M3TSZ_ERR_CUDA);
-    if (b1 > b0 && cudaMemcpyAsync((uint8_t *)d_streams + b0, h_streams + b0, b1 - b0, cudaMemcpyHostToDevice, st) !=
-                       cudaSuccess)
-      return fail(M3TSZ_ERR_CUDA);
+    CK(cudaMemcpyAsync(L.meta, m, meta_words * 8, cudaMemcpyHostToDevice, st));
+    if (b1 > b0)
+      CK(cudaMemcpyAsync((uint8_t *)d_streams + b0, h_streams + b0, b1 - b0, cudaMemcpyHostToDevice, st));
     if (nq) {
       rc = m3tsz_decode_batch(ctx, opts, (const uint8_t *)d_streams, streams_bytes, (const uint64_t *)d_off + q0, nq,
                               (int64_t *)L.ts, (double *)L.val, max_points, (uint32_t *)L.n, (int32_t *)L.st,
                               nullptr, nullptr, st);
-      if (rc) return fail(rc);
+      if (rc) return rc;
     }
     const uint64_t *dm = (const uint64_t *)L.meta;
     rc = m3tsz_merge_series_batch(ctx, (const int64_t *)L.ts, (const double *)L.val, max_points,
                                   (const uint32_t *)L.n, (const int32_t *)L.st, dm, dm + (max_k + 1),
                                   dm + (max_k + 1) + (max_r + 1), ns, start_ns, end_ns, strategy, (int64_t *)L.ots,
                                   (double *)L.oval, out_cap, (uint32_t *)L.on, (int32_t *)L.ost, st);
-    if (rc) return fail(rc);
-    if (cudaMemcpyAsync(h_ts_out + s0 * out_cap, L.ots, ns * out_cap * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaMemcpyAsync(h_val_out + s0 * out_cap, L.oval, ns * out_cap * 8, cudaMemcpyDeviceToHost, st) !=
-            cudaSuccess ||
-        cudaMemcpyAsync(h_n_out + s0, L.on, ns * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaMemcpyAsync(h_status + s0, L.ost, ns * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess)
-      return fail(M3TSZ_ERR_CUDA);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(h_ts_out + s0 * out_cap, L.ots, ns * out_cap * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_val_out + s0 * out_cap, L.oval, ns * out_cap * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_n_out + s0, L.on, ns * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_status + s0, L.ost, ns * 4, cudaMemcpyDeviceToHost, st));
   }
-  if (cudaStreamSynchronize(sts[0]) != cudaSuccess || cudaStreamSynchronize(sts[1]) != cudaSuccess)
-    return set_cuda_error(ctx, cudaGetLastError(), "m3tsz_fetch_batch_host");
+  CK(cudaStreamSynchronize(sts[0]));
+  CK(cudaStreamSynchronize(sts[1]));
   return M3TSZ_OK;
 }
 

@@ -17,6 +17,69 @@ struct Scratch {
   size_t bytes = 0;
 };
 
+// Context scratch slots: grow-only device buffers that live as long as the context (see
+// ensure()).  Calls that name the same slot share its memory:
+//
+//   slot          holds                                          used by
+//   0             streams                                        decode_host, downsample_host, fetch
+//   1             offsets, or the encoder starts                 decode_host, downsample_host, fetch; encode_host
+//   2, 3          decoded ts, val                                decode_host
+//   4, 5          n_points, status                               decode_host, downsample_host, tiles,
+//                                                                encode_host (4)
+//   6             unit                                           decode_host
+//   7             annotation refs, or annotation series offsets  decode_host; encode_host
+//   8-11          window sum / count / min / max                 downsample_host, tiles
+//   12            lastAt                                         downsample_last with a NULL d_last_at, tiles
+//   13, 14        annotation entries, annotation bytes           encode_host
+//   15            compaction scan temp                           compact_streams
+//   16-24, 26-34  pipeline lane 0 / 1, buffers 0-8 (lane_slot)   encode_host, fetch
+//   36, 37        packed slot sets, batch counter                packed encode, tiles
+//   38, 39        window last, tile encoder starts               tiles
+//   40-47         streaming handles, under handle_mu             m3tsz_stream.cu
+//
+// Slots 25 and 35 are unused.
+enum Slot : int {
+  kSlotStreams = 0,
+  kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
+  kSlotTs = 2,
+  kSlotVal = 3,
+  kSlotNPoints = 4,
+  kSlotStatus = 5,
+  kSlotUnit = 6,
+  kSlotAnnRefs = 7,       // decode output
+  kSlotAnnSeriesOff = 7,  // encode input
+  kSlotWinSum = 8,
+  kSlotWinCount = 9,
+  kSlotWinMin = 10,
+  kSlotWinMax = 11,
+  kSlotWinLastAt = 12,
+  kSlotAnnEntries = 13,
+  kSlotAnnBytes = 14,
+  kSlotCompactTmp = 15,
+  kSlotLaneBase = 16,
+  kSlotPackedSlots = 36,
+  kSlotBatchCounter = 37,
+  kSlotWinLast = 38,
+  kSlotTileStarts = 39,
+  // streaming handles: an encoder's buffers, or an iterator's
+  kSlotEncTs = 40,
+  kSlotEncVal = 41,
+  kSlotEncUnit = 42,
+  kSlotHandleMeta = 43,  // both: small per-call results
+  kSlotEncOut = 44,
+  kSlotEncAnnOff = 45,
+  kSlotEncAnnEntries = 46,
+  kSlotEncAnnBytes = 47,
+  kSlotIterStream = 40,
+  kSlotIterTs = 41,
+  kSlotIterVal = 42,
+  kSlotIterEvents = 44,
+  kNumSlots = 48
+};
+
+// Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.
+inline Slot lane_slot(int lane, int k) { return Slot(kSlotLaneBase + 10 * lane + k); }
+
 struct m3tsz_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;   // used by the *_host entry points
@@ -24,7 +87,7 @@ struct m3tsz_ctx {
   cudaEvent_t ev = nullptr;
   uint64_t launches = 0;
   char last_error[256] = {0};
-  Scratch s[48];
+  Scratch s[kNumSlots];
   int32_t *d_flag = nullptr;  // [2]
   void *h_stage[2] = {nullptr, nullptr};  // pinned staging for per-chunk offsets
   size_t h_stage_bytes[2] = {0, 0};
@@ -45,7 +108,7 @@ inline int set_cuda_error(m3tsz_ctx *ctx, cudaError_t e, const char *where) {
     if (_e != cudaSuccess) return set_cuda_error(ctx, _e, #call); \
   } while (0)
 
-inline int ensure(m3tsz_ctx *ctx, int slot, size_t bytes, void **out) {
+inline int ensure(m3tsz_ctx *ctx, Slot slot, size_t bytes, void **out) {
   Scratch &sc = ctx->s[slot];
   if (bytes == 0) bytes = 16;
   if (sc.bytes < bytes) {
@@ -103,6 +166,16 @@ struct DeviceGuard {
   }
   ~DeviceGuard() {
     if (prev >= 0) cudaSetDevice(prev);
+  }
+};
+
+// Declared right after a *_host call's DeviceGuard: however the call returns, it does not
+// leave copies from or into the caller's buffers in flight on the context's streams.
+struct DrainStreams {
+  m3tsz_ctx *ctx;
+  ~DrainStreams() {
+    cudaStreamSynchronize(ctx->stream);
+    cudaStreamSynchronize(ctx->stream2);
   }
 };
 
