@@ -264,6 +264,64 @@ uint64_t m3tsz_encode_bound(uint64_t n_points);
 uint64_t m3tsz_encode_bound_units(uint64_t n_points, int per_datapoint_units);
 
 /* ------------------------------------------------------------------------
+ * Encoder sets: n_series OPEN encoders that live on the device and take datapoints over many calls -- the write
+ * path BufferBucket.write -> encoder.Encode(dp, unit, annotation) (src/dbnode/storage/series/buffer.go:1261-1364)
+ * for thousands of series per call, plus Stream() snapshots for readers of the open block (buffer.go:1366-1391,
+ * m3tsz/encoder.go:282-297).
+ *
+ * One open encoder = one 128-byte m3tsz_encoder_state in caller-owned device memory (16-byte aligned) plus one
+ * slot of buf_stride bytes in a caller-owned [n_series][buf_stride] buffer (buf_stride % 16 == 0; a multiple of
+ * 32 makes every write a whole 32-byte sector).  The state holds positions, never pointers, so a caller whose
+ * slots are full copies [n][stride] into a larger [n][stride2] buffer (each slot's first stride bytes) and goes on
+ * appending with stride2.
+ *
+ * The slot only ever receives whole 32-byte sectors of the stream (at most 7 words plus the partial word wait in
+ * the state); a snapshot writes the rest at the committed position.
+ * ---------------------------------------------------------------------- */
+typedef struct m3tsz_encoder_state {
+  int64_t start_ns;      /* Reset(start), encoder.go:262-279 */
+  uint64_t num_encoded;  /* NumEncoded(), encoder.go:299-302 */
+  int64_t last_ts;       /* LastEncoded().TimestampNanos (valid when num_encoded > 0) */
+  double last_value;     /* LastEncoded().Value incl. the scaled-int / 0 quirk (as m3tsz_encode_extras.d_last_value) */
+  uint64_t ann_checksum; /* LastAnnotationChecksum(): XXH64 of the last annotation written, encoder.go:321-327 */
+  uint64_t bits;         /* stream bits so far, before the tail: Len() = num_encoded ? ceil((bits + 11) / 8) : 0 */
+  uint64_t internal[10]; /* codec state, opaque */
+} m3tsz_encoder_state;
+
+/* Reset(start) of every encoder of the set (encoder.go:262-279): empty streams, d_start [n_series] ns.  The state
+ * records opts->int_optimized; the other calls refuse a state reset in the other mode. */
+int m3tsz_encoder_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, m3tsz_encoder_state *d_state,
+                            uint64_t n_series, const int64_t *d_start, void *stream);
+
+/* Appends d_n_points[s] (NULL: points_stride each; 0 leaves the encoder and its slot untouched) datapoints to
+ * encoder s, one launch for the whole set.  Inputs as m3tsz_encode_batch_ex: series-major [n][points_stride], or
+ * point-major [points_stride][n] when point_major_input != 0 (then d_units and annotations must be NULL), unit /
+ * d_units, the sparse annotation list (dp_index counts within this call).  An annotation is written when its
+ * XXH64 differs from the state's ann_checksum, as the reference decides.
+ *
+ * A series stops at its first datapoint that fails: d_status[s] = M3TSZ_ERR_DOD_OVERFLOW,
+ * M3TSZ_ERR_UNRECOGNIZED_UNIT, M3TSZ_ERR_CAPACITY (the slot cannot hold 56 bytes past the stream so far -- the
+ * datapoint's worst case plus a snapshot tail -- and its annotation rounded up to 4 bytes + 16) or
+ * M3TSZ_ERR_INVALID_ARG (a state reset with the
+ * other int_optimized, or n_points > points_stride).  d_n_appended[s] counts the datapoints taken; state and
+ * slot are then exactly as after the last one taken (nothing of the failing datapoint is written), so dropping
+ * it and appending the rest gives the stream of the sequence without it. */
+int m3tsz_encoder_set_append(m3tsz_ctx *ctx, const m3tsz_options *opts, m3tsz_encoder_state *d_state,
+                             uint64_t n_series, const int64_t *d_ts, const double *d_val, uint64_t points_stride,
+                             const uint32_t *d_n_points, int32_t unit, const uint8_t *d_units,
+                             const uint64_t *d_ann_series_off, const m3tsz_annotation_entry *d_ann_entries,
+                             const uint8_t *d_ann_bytes, int32_t point_major_input, uint8_t *d_buf,
+                             uint64_t buf_stride, uint32_t *d_n_appended, int32_t *d_status, void *stream);
+
+/* Stream() of every encoder without closing it: writes the tail (the state's leftover words, end-of-stream marker,
+ * zero pad) at the committed position, so that d_buf[s * buf_stride, + d_len[s]) is the reference's head || tail,
+ * d_len[s] = 0 for an empty encoder.  The state is unchanged; the next append overwrites the tail.  The snapshot
+ * decodes with m3tsz_decode_batch_ex (d_offsets[s] = s * buf_stride, extras.d_lengths = d_len) and packs with
+ * m3tsz_compact_streams (slot_stride = buf_stride). */
+int m3tsz_encoder_set_stream(m3tsz_ctx *ctx, const m3tsz_encoder_state *d_state, uint64_t n_series,
+                             uint8_t *d_buf, uint64_t buf_stride, uint64_t *d_len, void *stream);
+
+/* ------------------------------------------------------------------------
  * Batch encode straight into ONE packed buffer (the fileset data-file layout,
  * src/dbnode/persist/fs/write.go: concatenated segments + index entries that
  * carry (Offset, Size), persist/schema/types.go:70-78) -- no per-series slots,

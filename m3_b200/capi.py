@@ -93,7 +93,10 @@ EXPORTED_SYMBOLS = [
     "m3tsz_iter_err", "m3tsz_iter_close",
     "m3tsz_encoder_pool_create", "m3tsz_encoder_pool_get", "m3tsz_encoder_pool_destroy",
     "m3tsz_iter_pool_create", "m3tsz_iter_pool_get", "m3tsz_iter_pool_destroy",
+    "m3tsz_encoder_set_reset", "m3tsz_encoder_set_append", "m3tsz_encoder_set_stream",
 ]
+
+ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
 
 
 def lib():
@@ -234,6 +237,13 @@ def lib():
                                               u64, vp, vp, u64, i32, i32, vp]
     L.m3tsz_checksum_batch.restype = C.c_int
     L.m3tsz_checksum_batch.argtypes = [vp, vp, u64, vp, vp, u64, vp, vp, vp, vp]
+    L.m3tsz_encoder_set_reset.restype = C.c_int
+    L.m3tsz_encoder_set_reset.argtypes = [vp, po, vp, u64, vp, vp]
+    L.m3tsz_encoder_set_append.restype = C.c_int
+    L.m3tsz_encoder_set_append.argtypes = [vp, po, vp, u64, vp, vp, u64, vp, i32, vp, vp, vp, vp, i32, vp, u64,
+                                           vp, vp, vp]
+    L.m3tsz_encoder_set_stream.restype = C.c_int
+    L.m3tsz_encoder_set_stream.argtypes = [vp, vp, u64, vp, u64, vp, vp]
     _lib = L
     return L
 

@@ -230,6 +230,11 @@ class BatchCodec:
         self.ctx.check(rc, "m3tsz_compact_streams")
         return packed, offsets
 
+    def encoder_set(self, start: torch.Tensor, stride: int) -> "EncoderSet":
+        """S open encoders on the device (S = start.numel(), start int64 [S] ns), each with a slot of `stride`
+        bytes (a multiple of 16): the write path's encoders, appended to over many calls."""
+        return EncoderSet(self, start, stride)
+
     # ------------------------------------------------------------------ merge (row N1)
     def merge_series(self, ts, values, n_points, seq_status, slice_off, replica_off, series_off,
                      out_cap, start_ns=0, end_ns=0, strategy=0, point_major=False):
@@ -356,3 +361,105 @@ class BatchCodec:
 
     def launch_count(self):
         return self.ctx.launch_count()
+
+
+class EncoderSet:
+    """Open encoders that live on the device (m3tsz_encoder_set_*): a state tensor uint8 [S, 128]
+    (m3tsz_encoder_state) and a slot buffer uint8 [S, stride].  append() continues every stream, stream()
+    snapshots them without closing; the public prefix of the state answers NumEncoded / LastEncoded /
+    LastAnnotationChecksum / Len without a launch."""
+
+    def __init__(self, codec: BatchCodec, start: torch.Tensor, stride: int):
+        assert stride > 0 and stride % 16 == 0
+        self.codec = codec
+        self.n_series = start.numel()
+        dev = codec.device
+        self.state = torch.empty((self.n_series, capi.ENCODER_STATE_BYTES), dtype=torch.uint8, device=dev)
+        self.buf = torch.zeros((self.n_series, stride), dtype=torch.uint8, device=dev)
+        self.reset(start)
+
+    @property
+    def stride(self) -> int:
+        return self.buf.shape[1]
+
+    def reset(self, start: torch.Tensor):
+        """Reset(start) of every encoder: empty streams (the slots' bytes are then free)."""
+        assert start.dtype == torch.int64 and start.is_cuda and start.numel() == self.n_series
+        start = start.contiguous()
+        rc = capi.lib().m3tsz_encoder_set_reset(self.codec.ctx.handle, C.byref(self.codec.opts), _ptr(self.state),
+                                                self.n_series, _ptr(start), _cuda_stream_ptr(self.codec.device))
+        self.codec.ctx.check(rc, "m3tsz_encoder_set_reset")
+
+    def append(self, ts: torch.Tensor, values: torch.Tensor, n_points: Optional[torch.Tensor] = None,
+               units: Optional[torch.Tensor] = None, annotations=None, point_major=False, unit=capi.UNIT_S):
+        """Appends ts / values int64 / float64 [S, P] ([P, S] when point_major) to the encoders; n_points
+        (int32 [S]) takes the first n_points[s] of series s, 0 leaves it untouched.  units / annotations as
+        BatchCodec.encode (series-major only; annotation dp_index counts within this call).  Returns
+        (n_appended int32 [S], status int32 [S]): a series stops at its first failing datapoint, and its state
+        is as after the last datapoint taken."""
+        assert ts.dtype == torch.int64 and values.dtype == torch.float64
+        assert ts.is_cuda and values.is_cuda and ts.is_contiguous() and values.is_contiguous()
+        S, P = (ts.shape[1], ts.shape[0]) if point_major else ts.shape
+        assert S == self.n_series
+        dev = self.codec.device
+        if P == 0:  # nothing to append (an empty tensor may have no storage to point at)
+            return (torch.zeros(S, dtype=torch.int32, device=dev), torch.zeros(S, dtype=torch.int32, device=dev))
+        n_appended = torch.empty(S, dtype=torch.int32, device=dev)
+        status = torch.empty(S, dtype=torch.int32, device=dev)
+        a_off = a_ent = a_bytes = None
+        if annotations is not None:
+            a_off, a_ent, a_bytes = annotations
+        rc = capi.lib().m3tsz_encoder_set_append(
+            self.codec.ctx.handle, C.byref(self.codec.opts), _ptr(self.state), S, _ptr(ts), _ptr(values), P,
+            _ptr(n_points), int(unit), _ptr(units), _ptr(a_off), _ptr(a_ent), _ptr(a_bytes),
+            1 if point_major else 0, _ptr(self.buf), self.stride, _ptr(n_appended), _ptr(status),
+            _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_encoder_set_append")
+        return n_appended, status
+
+    def stream(self) -> EncodeResult:
+        """Stream() of every encoder: out = the slot buffer [S, stride], out_len = the snapshot lengths (0 for an
+        empty encoder), as BatchCodec.encode returns them.  compact() takes it as it is; decode takes
+        out.view(-1) with offsets = self.offsets() and lengths = out_len."""
+        dev = self.codec.device
+        out_len = torch.empty(self.n_series, dtype=torch.int64, device=dev)
+        rc = capi.lib().m3tsz_encoder_set_stream(self.codec.ctx.handle, _ptr(self.state), self.n_series,
+                                                 _ptr(self.buf), self.stride, _ptr(out_len), _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_encoder_set_stream")
+        return EncodeResult(out=self.buf, out_len=out_len,
+                            status=torch.zeros(self.n_series, dtype=torch.int32, device=dev))
+
+    def offsets(self) -> torch.Tensor:
+        """Start of every slot in buf.view(-1), for decode(..., lengths=...)."""
+        return torch.arange(self.n_series, dtype=torch.int64, device=self.codec.device) * self.stride
+
+    def grow(self, stride: int):
+        """Moves the slots into a buffer of `stride` bytes each (the state holds positions, not pointers)."""
+        assert stride % 16 == 0 and stride >= self.stride
+        buf = torch.zeros((self.n_series, stride), dtype=torch.uint8, device=self.codec.device)
+        buf[:, : self.stride] = self.buf
+        self.buf = buf
+
+    # public prefix of m3tsz_encoder_state: start_ns, num_encoded, last_ts, last_value, ann_checksum, bits
+    def _field(self, i):
+        return self.state.view(torch.int64)[:, i]
+
+    @property
+    def num_encoded(self) -> torch.Tensor:
+        return self._field(1)
+
+    @property
+    def last_encoded(self):
+        """(ts int64 [S], value float64 [S]): LastEncoded(), meaningful where num_encoded > 0."""
+        return self._field(2), self.state.view(torch.float64)[:, 3]
+
+    @property
+    def ann_checksum(self) -> torch.Tensor:
+        """LastAnnotationChecksum() as int64 [S] (the uint64's bits)."""
+        return self._field(4)
+
+    @property
+    def len(self) -> torch.Tensor:
+        """Len(): stream bytes with the tail, 0 for an empty encoder."""
+        n, bits = self._field(1), self._field(5)
+        return torch.where(n > 0, (bits + 11 + 7) // 8, torch.zeros_like(bits))

@@ -43,16 +43,17 @@ static bool decode_params(const m3tsz_options *opts, const uint8_t *d_streams, u
   return true;
 }
 
-// The inputs both encode entry points check (pointers, alignments, the annotation triple, and
+// The inputs the encode entry points check (pointers, alignments, the annotation triple, and
 // point-major input, which takes no units or annotations), and the EncodeParams fields they share.
+// The batch encoders need d_start and d_out_len; an encoder-set append takes both from its states.
 static bool encode_params(const m3tsz_options *opts, const int64_t *d_ts, const double *d_val, uint64_t n_series,
                           uint64_t points_stride, const uint32_t *d_n_points, const int64_t *d_start, int32_t unit,
                           const uint8_t *d_units, const uint64_t *d_ann_series_off,
                           const m3tsz_annotation_entry *d_ann_entries, const uint8_t *d_ann_bytes,
                           uint64_t *d_out_len, int32_t *d_status, const m3tsz_encode_extras *extras,
-                          EncodeParams &p) {
-  if (!d_ts || !d_val || !d_start || !d_out_len || points_stride > 0xffffffffull || ((uintptr_t)d_ts & 7u) ||
-      ((uintptr_t)d_val & 7u))
+                          EncodeParams &p, bool append = false) {
+  if (!d_ts || !d_val || (!append && (!d_start || !d_out_len)) || points_stride > 0xffffffffull ||
+      ((uintptr_t)d_ts & 7u) || ((uintptr_t)d_val & 7u))
     return false;
   if (d_ann_series_off && (!d_ann_entries || !d_ann_bytes)) return false;
   const bool point_major = extras && extras->point_major_input;
@@ -327,6 +328,61 @@ int m3tsz_encode_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const int64_t 
   return m3tsz_encode_batch_ex(ctx, opts, d_ts, d_val, n_series, points_stride, d_n_points, d_start, unit,
                                d_units, d_ann_series_off, d_ann_entries, d_ann_bytes, d_out, out_stride,
                                d_out_len, d_status, nullptr, stream);
+}
+
+int m3tsz_encoder_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, m3tsz_encoder_state *d_state,
+                            uint64_t n_series, const int64_t *d_start, void *stream) {
+  if (!ctx || !valid_opts(opts)) return M3TSZ_ERR_INVALID_ARG;
+  if (n_series == 0) return M3TSZ_OK;
+  if (!d_state || !d_start || ((uintptr_t)d_state & 15u)) return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  CK(launch_encoder_set_reset(d_state, n_series, d_start, opts->default_time_unit, opts->int_optimized != 0,
+                              (cudaStream_t)stream));
+  ctx->launches++;
+  return M3TSZ_OK;
+}
+
+int m3tsz_encoder_set_append(m3tsz_ctx *ctx, const m3tsz_options *opts, m3tsz_encoder_state *d_state,
+                             uint64_t n_series, const int64_t *d_ts, const double *d_val, uint64_t points_stride,
+                             const uint32_t *d_n_points, int32_t unit, const uint8_t *d_units,
+                             const uint64_t *d_ann_series_off, const m3tsz_annotation_entry *d_ann_entries,
+                             const uint8_t *d_ann_bytes, int32_t point_major_input, uint8_t *d_buf,
+                             uint64_t buf_stride, uint32_t *d_n_appended, int32_t *d_status, void *stream) {
+  if (!ctx || !valid_opts(opts)) return M3TSZ_ERR_INVALID_ARG;
+  if (n_series == 0) return M3TSZ_OK;
+  m3tsz_encode_extras ex;
+  memset(&ex, 0, sizeof(ex));
+  ex.point_major_input = point_major_input;
+  EncodeParams p;
+  if (!encode_params(opts, d_ts, d_val, n_series, points_stride, d_n_points, nullptr, unit, d_units,
+                     d_ann_series_off, d_ann_entries, d_ann_bytes, nullptr, d_status, &ex, p, true) ||
+      !d_state || ((uintptr_t)d_state & 15u) || !d_n_appended || !d_status || !d_buf || (buf_stride & 15u) ||
+      buf_stride == 0 || buf_stride > (1ull << 33) || ((uintptr_t)d_buf & 15u))
+    return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  p.out = d_buf;
+  p.out_stride = buf_stride;
+  p.state = d_state;
+  p.n_appended = d_n_appended;
+  CK(launch_encode_append(p, opts->int_optimized != 0, (cudaStream_t)stream));
+  ctx->launches++;
+  return M3TSZ_OK;
+}
+
+int m3tsz_encoder_set_stream(m3tsz_ctx *ctx, const m3tsz_encoder_state *d_state, uint64_t n_series,
+                             uint8_t *d_buf, uint64_t buf_stride, uint64_t *d_len, void *stream) {
+  if (!ctx) return M3TSZ_ERR_INVALID_ARG;
+  if (n_series == 0) return M3TSZ_OK;
+  if (!d_state || ((uintptr_t)d_state & 15u) || !d_buf || !d_len || (buf_stride & 15u) || buf_stride == 0 ||
+      ((uintptr_t)d_buf & 15u))
+    return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  CK(launch_encoder_set_stream(d_state, n_series, d_buf, buf_stride, d_len, (cudaStream_t)stream));
+  ctx->launches++;
+  return M3TSZ_OK;
 }
 
 int m3tsz_encode_batch_packed(m3tsz_ctx *ctx, const m3tsz_options *opts, const int64_t *d_ts,

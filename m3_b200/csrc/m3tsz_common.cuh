@@ -7,6 +7,7 @@
 
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/m3tsz_b200.h"
 
@@ -102,6 +103,65 @@ __device__ __forceinline__ double mult_pow10(int m) {
     case 5: return 100000.0;
     default: return 1000000.0;
   }
+}
+
+// XXH64, seed 0 (cespare/xxhash/v2 Sum64, go.mod:10): TimestampEncoder keeps the checksum of the last annotation
+// written (timestamp_encoder.go:56,166-195) and rewrites an annotation only when its checksum differs; Encoder.
+// LastAnnotationChecksum() exposes it (encoder.go:321-327).  One definition for the streaming handles (host) and the
+// encoder sets' append kernel (device).  Little-endian byte order: x86-64 / aarch64 hosts and the GPU.
+__host__ __device__ inline uint64_t xxh64(const uint8_t *d, size_t n) {
+  const uint64_t P1 = 11400714785074694791ull, P2 = 14029467366897019727ull, P3 = 1609587929392839161ull,
+                 P4 = 9650029242287828579ull, P5 = 2870177450012600261ull;
+  auto rotl = [](uint64_t x, int r) { return (x << r) | (x >> (64 - r)); };
+  auto xround = [&](uint64_t acc, uint64_t in) { return rotl(acc + in * P2, 31) * P1; };
+  auto rd64 = [](const uint8_t *p) {
+    uint64_t v;
+    memcpy(&v, p, 8);
+    return v;
+  };
+  auto rd32 = [](const uint8_t *p) {
+    uint32_t v;
+    memcpy(&v, p, 4);
+    return v;
+  };
+  const uint8_t *p = d, *end = d + n;
+  uint64_t h;
+  if (n >= 32) {
+    uint64_t v1 = P1 + P2, v2 = P2, v3 = 0, v4 = 0 - P1;
+    while (p + 32 <= end) {
+      v1 = xround(v1, rd64(p));
+      v2 = xround(v2, rd64(p + 8));
+      v3 = xround(v3, rd64(p + 16));
+      v4 = xround(v4, rd64(p + 24));
+      p += 32;
+    }
+    h = rotl(v1, 1) + rotl(v2, 7) + rotl(v3, 12) + rotl(v4, 18);
+    h = (h ^ xround(0, v1)) * P1 + P4;
+    h = (h ^ xround(0, v2)) * P1 + P4;
+    h = (h ^ xround(0, v3)) * P1 + P4;
+    h = (h ^ xround(0, v4)) * P1 + P4;
+  } else {
+    h = P5;
+  }
+  h += (uint64_t)n;
+  while (p + 8 <= end) {
+    h = rotl(h ^ xround(0, rd64(p)), 27) * P1 + P4;
+    p += 8;
+  }
+  if (p + 4 <= end) {
+    h = rotl(h ^ ((uint64_t)rd32(p) * P1), 23) * P2 + P3;
+    p += 4;
+  }
+  while (p < end) {
+    h = rotl(h ^ ((uint64_t)*p * P5), 11) * P1;
+    p++;
+  }
+  h ^= h >> 33;
+  h *= P2;
+  h ^= h >> 29;
+  h *= P3;
+  h ^= h >> 32;
+  return h;
 }
 
 // Big-endian 32-bit word `widx` of a byte buffer whose base is 4-byte aligned.

@@ -15,6 +15,7 @@
 //   m3tsz/float_encoder_iterator.go:69-103, m3tsz/int_sig_bits_tracker.go:35-91,
 //   m3tsz/m3tsz.go:78-119, ostream.go:133-221, scheme.go:198-220.
 #include <cstring>
+#include <type_traits>
 #include <cub/device/device_scan.cuh>
 #include <cuda.h>  // CUtensorMap (types only: the encoder is resolved through cudaGetDriverEntryPoint)
 
@@ -633,6 +634,123 @@ __device__ __forceinline__ void tier2_commit(EncLane &s, uint32_t *tile, int lan
   }
 }
 
+// the append mode's own per-lane variables (encode_kernel)
+struct EncAppendVars {
+  uint32_t n_enc0 = 0;  // datapoints the encoder held before this call
+  uint64_t ann_cs = 0;  // XXH64 of the last annotation written
+};
+struct EncNoVars {};
+
+// ---- encoder sets: the state record between appends (DESIGN.md §4.6) ------------------------------------------
+// m3tsz_encoder_state.internal: what EncLane holds besides the public prefix.  The output tile's leftover words
+// (fewer than a sector) and the partial word wait here, so the slot only receives whole sectors and words_out
+// stays a multiple of 8; words_out = bits / 32 - k.  prev_time is last_ts (start_ns before the first datapoint).
+struct EncStateInternal {
+  uint32_t left[7];  // leftover words, stream order
+  uint32_t carry;    // partial word: its top `sh` bits
+  int64_t prev_delta;
+  uint64_t prev_bits;
+  double int_val;
+  uint64_t meta;  // sh:5 k:3 plz:7 ptz:7 unit:4 num_sig:7 hi_lower_sig:7 n_lower_sig:3 max_mult:3 is_float:1, tag:16
+  uint64_t reserved[2];
+};
+static_assert(sizeof(EncStateInternal) == sizeof(((m3tsz_encoder_state *)0)->internal), "state layout");
+static_assert(sizeof(m3tsz_encoder_state) == 128, "state layout");
+// the tag records the mode the state was reset in (an append in the other mode is refused)
+__host__ __device__ __forceinline__ uint64_t enc_state_tag(bool int_opt) { return int_opt ? 0xe3a1u : 0xe3a0u; }
+
+// Reset(start), encoder.go:262-279 (+ NewTimestampEncoder's empty-annotation checksum, timestamp_encoder.go:56)
+__host__ __device__ __forceinline__ void enc_state_reset(m3tsz_encoder_state &st, int64_t start, int default_unit,
+                                                         bool int_opt) {
+  memset(&st, 0, sizeof(st));
+  st.start_ns = start;
+  st.ann_checksum = xxh64(nullptr, 0);
+  EncStateInternal &in = *reinterpret_cast<EncStateInternal *>(st.internal);
+  in.meta = (64ull << 8) | ((uint64_t)initial_time_unit(start, default_unit) << 22) | (enc_state_tag(int_opt) << 48);
+}
+
+// state -> lane (+ leftover words into the lane's tile column).  M3TSZ_ERR_INVALID_ARG when the state was reset in
+// the other mode (nothing is loaded then).
+template <bool INT_OPT>
+__device__ __forceinline__ int enc_state_load(const m3tsz_encoder_state &st, EncLane &s, uint32_t *tile, int lane,
+                                              uint64_t &ann_cs) {
+  const EncStateInternal &in = *reinterpret_cast<const EncStateInternal *>(st.internal);
+  const uint64_t m = in.meta;
+  if ((m >> 48) != enc_state_tag(INT_OPT)) return M3TSZ_ERR_INVALID_ARG;
+  s.sh = (uint32_t)(m & 31u);
+  s.k = (uint32_t)((m >> 5) & 7u);
+  s.plz = (int)((m >> 8) & 127u);
+  s.ptz = (int)((m >> 15) & 127u);
+  s.unit = (int)((m >> 22) & 15u);
+  s.num_sig = (int)((m >> 26) & 127u);
+  s.hi_lower_sig = (int)((m >> 33) & 127u);
+  s.n_lower_sig = (int)((m >> 40) & 7u);
+  s.max_mult = (int)((m >> 43) & 7u);
+  s.is_float = ((m >> 46) & 1u) != 0;
+  for (uint32_t i = 0; i < s.k; i++) tile[i * ENC_STRIDE + lane] = in.left[i];
+  s.carry = in.carry;
+  s.words_out = (uint32_t)(st.bits >> 5) - s.k;
+  s.n_enc = (uint32_t)st.num_encoded;
+  s.prev_time = st.num_encoded ? st.last_ts : st.start_ns;
+  s.prev_delta = in.prev_delta;
+  s.prev_bits = in.prev_bits;
+  s.int_val = in.int_val;
+  s.err = 0;
+  ann_cs = st.ann_checksum;
+  return 0;
+}
+
+// lane -> state, after a flush that left s.k <= 7 words in the tile
+template <bool INT_OPT>
+__device__ __forceinline__ void enc_state_save(m3tsz_encoder_state &st, const EncLane &s, const uint32_t *tile,
+                                               int lane, uint64_t ann_cs) {
+  EncStateInternal &in = *reinterpret_cast<EncStateInternal *>(st.internal);
+  for (uint32_t i = 0; i < 7; i++) in.left[i] = i < s.k ? tile[i * ENC_STRIDE + lane] : 0u;
+  in.carry = s.carry;
+  in.prev_delta = s.prev_delta;
+  in.prev_bits = s.prev_bits;
+  in.int_val = s.int_val;
+  in.meta = (uint64_t)s.sh | ((uint64_t)s.k << 5) | ((uint64_t)s.plz << 8) | ((uint64_t)s.ptz << 15) |
+            ((uint64_t)s.unit << 22) | ((uint64_t)s.num_sig << 26) | ((uint64_t)s.hi_lower_sig << 33) |
+            ((uint64_t)s.n_lower_sig << 40) | ((uint64_t)s.max_mult << 43) | ((uint64_t)s.is_float << 46) |
+            (enc_state_tag(INT_OPT) << 48);
+  st.num_encoded = s.n_enc;
+  st.last_ts = s.prev_time;
+  // LastEncoded().Value (encoder.go:305-319), as the batch encoder's d_last_value
+  st.last_value = (INT_OPT && s.is_float) ? __longlong_as_double((long long)s.prev_bits) : (INT_OPT ? s.int_val : 0.0);
+  st.ann_checksum = ann_cs;
+  st.bits = ((uint64_t)s.words_out + s.k) * 32ull + s.sh;
+}
+
+// The checks encode_time makes on a datapoint (timestamp_encoder.go:104-164), made before anything of it is
+// written: append mode drops a failing datapoint as a whole, annotation included.
+__device__ __forceinline__ int enc_check_time(const EncLane &s, int64_t t, int u) {
+  if (!unit_is_valid(u)) return M3TSZ_ERR_UNRECOGNIZED_UNIT;
+  if (u != s.unit || u > 2) return 0;  // a unit change writes a 64-bit delta-of-delta; us / ns have 64-bit buckets
+  const int64_t delta = (int64_t)((uint64_t)t - (uint64_t)s.prev_time);
+  const int64_t dod = div_unit((int64_t)((uint64_t)delta - (uint64_t)s.prev_delta), u);
+  return dod != (int64_t)(int32_t)dod ? M3TSZ_ERR_DOD_OVERFLOW : 0;
+}
+
+// Stream()'s tail at the committed position (scheme.go:198-211): the leftover words, the partial word with the
+// end-of-stream marker, zero words up to a whole 16-byte group.  Fills w (big-endian word values) and returns the
+// number of words (0, 4, 8 or 12) that go to the slot from word `at` on (the committed words_out).
+__host__ __device__ __forceinline__ uint32_t enc_snapshot_words(const m3tsz_encoder_state &st, uint32_t w[12],
+                                                                uint64_t &at) {
+  if (st.num_encoded == 0) return 0;
+  const EncStateInternal &in = *reinterpret_cast<const EncStateInternal *>(st.internal);
+  const uint32_t sh = (uint32_t)(in.meta & 31u), k = (uint32_t)((in.meta >> 5) & 7u);
+  at = (st.bits >> 5) - k;
+  uint32_t n = 0;
+  for (; n < k; n++) w[n] = in.left[n];
+  const uint64_t eos = (uint64_t)((kMarkerOpcode << 2) | (uint32_t)kMarkerEOS) << (64 - kMarkerBits);
+  const uint64_t acc = ((uint64_t)in.carry << 32) | (eos >> sh);
+  w[n++] = (uint32_t)(acc >> 32);
+  if (sh + kMarkerBits > 32) w[n++] = (uint32_t)acc;
+  while (n & 3u) w[n++] = 0u;
+  return n;
+}
+
 __device__ __forceinline__ uint32_t enc_smem_addr(const void *p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -687,10 +805,15 @@ __device__ __forceinline__ void enc_mbar_wait(uint32_t bar, uint32_t parity) {
 // IN = 2: the Gauge aggregates of the fused decode+downsample kernel (window-major): datapoint i of a
 //         series = (tile_start + (i+1)*tile_step, Gauge.ValueOf(agg)) unless window i is empty
 //         (count == 0: skipped) -- the tile aggregation's re-encode without a gather pass.
-template <bool INT_OPT, bool PACKED, int IN>
+// APPEND: encoder-set append (DESIGN.md §4.6).  Every lane continues the open encoder p.state[s] in slot p.out +
+//   s * out_stride: the prologue loads the state (leftover words into the output tile), each datapoint is checked
+//   before anything of it is written, and the epilogue flushes whole sectors and saves the state instead of
+//   writing the tail.
+template <bool INT_OPT, bool PACKED, int IN, bool APPEND = false>
 __global__ void __launch_bounds__(ENC_WARPS * 32,
                                   (IN == 2) ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
     encode_kernel(const EncodeParams p, const __grid_constant__ EncTensorMaps tmaps) {
+  static_assert(!APPEND || (!PACKED && IN != 2), "append mode writes its own slots from staged inputs");
   extern __shared__ __align__(128) uint32_t smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -766,7 +889,23 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   uint64_t last_ann_off = 0;
   uint32_t last_ann_len = 0;  // 0 = no annotation written yet
   const uint32_t slot_words = (uint32_t)(p.out_stride >> 2);
-  if (valid) {
+  // APPEND only (nothing of it exists in the batch instantiations, whose code stays as it was)
+  std::conditional_t<APPEND, EncAppendVars, EncNoVars> av;
+  if constexpr (APPEND) {
+    if (valid) {
+      n_pts = p.n_points ? p.n_points[sidx] : (uint32_t)p.points_stride;
+      if (n_pts > p.points_stride) s.err = M3TSZ_ERR_INVALID_ARG;
+      if (p.ann_series_off) {
+        ann_i = p.ann_series_off[sidx];
+        ann_end = p.ann_series_off[sidx + 1];
+      }
+      // a series without datapoints (or with bad arguments) loads nothing and keeps its state and slot
+      if (n_pts > 0 && s.err == 0) s.err = enc_state_load<INT_OPT>(p.state[sidx], s, out_tile, lane, av.ann_cs);
+      if (s.err) n_pts = 0;
+      av.n_enc0 = s.n_enc;
+      if (n_pts > 0 && s.n_enc == 0) put64(s, out_tile, lane, (uint64_t)s.prev_time, 64);  // WriteFirstTime :89-102
+    }
+  } else if (valid) {
     n_pts = (IN != 2 && p.n_points) ? p.n_points[sidx] : (uint32_t)p.points_stride;
     if (IN == 2 && p.tile_src_status && p.tile_src_status[sidx] != 0) n_pts = 0;  // failed source stream: no tiles
     if (n_pts > p.points_stride) {
@@ -943,11 +1082,15 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   }
   bool steady = false;  // same s/ms/us/ns unit as the batch's and not the first datapoint
   bool hot_ok = false;  // steady, and float mode when int-optimised: both only change on the slow path
+  if constexpr (APPEND) {  // the loaded encoder's
+    steady = !p.units && p.unit == s.unit && (s.unit >= 1 && s.unit <= 4) && s.n_enc > 0;
+    hot_ok = steady && (!INT_OPT || s.is_float);
+  }
   const uint64_t *in_next = in_tiles + lane;  // this lane's ts cell of the row to fetch next (value: + one tile)
   for (uint32_t iter = 0; iter < max_pts; iter++) {  // warp-uniform (n_pts is 0 for lanes without a series)
     const bool tile_first = (iter & (IN_T - 1)) == 0;
     const bool tile_last = (iter & (IN_T - 1)) == IN_T - 1;
-    const bool active = s.err == 0 && iter < n_pts && !(IN == 2 && sk_pf);  // (n_pts is 0 without a series)
+    bool active = s.err == 0 && iter < n_pts && !(IN == 2 && sk_pf);  // (n_pts is 0 without a series)
 
     // ---- input pipeline: request tile t+NSTAGE-1, wait for tile t ----
     if (STAGED && tile_first) {
@@ -969,6 +1112,22 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       in_next = tile + IN_STRIDE;
     }
 
+    // ---- append mode: check the datapoint before any of it (annotation included) is written ----
+    if constexpr (APPEND) {
+      if (active) {
+        const int u = p.units ? (int)p.units[sidx * p.points_stride + iter] : p.unit;
+        // room for the datapoint's worst case, its annotation (marker + varint + bytes) and a snapshot's tail
+        uint64_t need = (uint64_t)s.words_out + s.k + ENC_GUARD + 4;
+        if (p.ann_series_off && ann_i < ann_end) {
+          const m3tsz_annotation_entry e = p.ann_entries[ann_i];
+          if (e.dp_index == iter && e.length > 0) need += (e.length + 3) / 4 + 4;
+        }
+        s.err = enc_check_time(s, t_pf, u);
+        if (s.err == 0 && need > slot_words) s.err = M3TSZ_ERR_CAPACITY;
+        active = s.err == 0;
+      }
+    }
+
     // ---- make room in the output tile ----
     const bool tight = active && (s.k > (uint32_t)(ENC_OUT_W - ENC_GUARD));
     if (__any_sync(FULL_MASK, tight)) flush_out(false);
@@ -985,12 +1144,19 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
           a_off = e.byte_offset;
           a_len = e.length;
           if (a_len > 0) {
-            // rewritten only when it differs from the last annotation written
-            // (xxhash64 inequality in the reference == byte inequality here)
-            bool same = (a_len == last_ann_len);
-            for (uint32_t i = 0; same && i < a_len; i++)
-              same = p.ann_bytes[a_off + i] == p.ann_bytes[last_ann_off + i];
-            want_ann = !same;
+            if constexpr (APPEND) {
+              // the last annotation written may belong to an earlier call: compare checksums, as the reference does
+              const uint64_t h = xxh64(p.ann_bytes + a_off, a_len);
+              want_ann = h != av.ann_cs;
+              av.ann_cs = h;
+            } else {
+              // rewritten only when it differs from the last annotation written
+              // (xxhash64 inequality in the reference == byte inequality here)
+              bool same = (a_len == last_ann_len);
+              for (uint32_t i = 0; same && i < a_len; i++)
+                same = p.ann_bytes[a_off + i] == p.ann_bytes[last_ann_off + i];
+              want_ann = !same;
+            }
           }
         }
       }
@@ -1059,8 +1225,9 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       if (__all_sync(FULL_MASK, hot || !active)) {
         // every live lane: '0' (zero DoD) [+ '1' no-update] + XOR code, one merge.  The state update is
         // unconditional where an inactive lane is a FINISHED lane (IN 0 / 1); with IN = 2 a lane may sit
-        // out one row (an empty window) and must keep its state.
-        const bool upd = (IN != 2) || active;
+        // out one row (an empty window) and must keep its state, and so must every lane in append mode, whose state
+        // outlives the call.
+        const bool upd = (IN != 2 && !APPEND) || active;
         if (upd) s.prev_time = t;
         const uint32_t pre = INT_OPT ? 1u : 0u;  // '0' zero DoD [+ '1' no-update]
         const int pb = INT_OPT ? 2 : 1;
@@ -1120,6 +1287,17 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   }
   if (STAGED) asm volatile("cp.async.wait_all;\n" ::: "memory");
   if (bulk) bulk_seq += (max_pts + (uint32_t)IN_T - 1u) / (uint32_t)IN_T;  // every requested tile was waited for
+
+  if constexpr (APPEND) {
+    // ---- whole sectors to the slot, the rest (<= 7 words + the partial word) into the state ----
+    flush_out(false);
+    if (valid) {
+      if (s.n_enc != av.n_enc0) enc_state_save<INT_OPT>(p.state[sidx], s, out_tile, lane, av.ann_cs);
+      p.n_appended[sidx] = s.n_enc - av.n_enc0;
+      p.status[sidx] = s.err;
+    }
+    continue;  // (one batch per warp)
+  }
 
   // ---- tail: end-of-stream marker + zero padding (scheme.go:198-211) ----
   uint64_t total_bits = 0;
@@ -1280,17 +1458,17 @@ static void enc_build_tensor_maps(const EncodeParams &p, EncTensorMaps &tm) {
   tm.ok = (a == CUDA_SUCCESS && b == CUDA_SUCCESS) ? 1 : 0;
 }
 
-template <bool INT_OPT, bool PACKED, int IN>
+template <bool INT_OPT, bool PACKED, int IN, bool APPEND = false>
 static cudaError_t launch_encode_one(const EncodeParams &p, cudaStream_t stream) {
   constexpr size_t smem = enc_block_smem<IN>();
   const uint64_t per_block = (uint64_t)ENC_WARPS * 32ull;
   uint64_t blocks = (p.n_series + per_block - 1) / per_block;
   if (blocks == 0) return cudaSuccess;
   if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
-  cudaError_t e = cudaFuncSetAttribute(encode_kernel<INT_OPT, PACKED, IN>,
+  cudaError_t e = cudaFuncSetAttribute(encode_kernel<INT_OPT, PACKED, IN, APPEND>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(encode_kernel<INT_OPT, PACKED, IN>, cudaFuncAttributePreferredSharedMemoryCarveout,
+  e = cudaFuncSetAttribute(encode_kernel<INT_OPT, PACKED, IN, APPEND>, cudaFuncAttributePreferredSharedMemoryCarveout,
                            ENC_CARVEOUT_KB * 100 / 228);
   if (e != cudaSuccess) return e;
   if (PACKED) {
@@ -1300,7 +1478,7 @@ static cudaError_t launch_encode_one(const EncodeParams &p, cudaStream_t stream)
   }
   EncTensorMaps tm;
   enc_build_tensor_maps(p, tm);  // (ok = 0 for the other input stages)
-  encode_kernel<INT_OPT, PACKED, IN><<<(unsigned)blocks, ENC_WARPS * 32, smem, stream>>>(p, tm);
+  encode_kernel<INT_OPT, PACKED, IN, APPEND><<<(unsigned)blocks, ENC_WARPS * 32, smem, stream>>>(p, tm);
   return cudaGetLastError();
 }
 
@@ -1351,6 +1529,61 @@ cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_
     return int_optimized ? launch_encode_one<true, true, 0>(p, stream) : launch_encode_one<false, true, 0>(p, stream);
   }
   return int_optimized ? launch_encode_one<true, false, 0>(p, stream) : launch_encode_one<false, false, 0>(p, stream);
+}
+
+// ---------------------------------------------------------------------------
+// encoder sets (DESIGN.md §4.6)
+// ---------------------------------------------------------------------------
+cudaError_t launch_encode_append(const EncodeParams &p, bool int_optimized, cudaStream_t stream) {
+  if (p.in_mode == 1)
+    return int_optimized ? launch_encode_one<true, false, 1, true>(p, stream)
+                         : launch_encode_one<false, false, 1, true>(p, stream);
+  return int_optimized ? launch_encode_one<true, false, 0, true>(p, stream)
+                       : launch_encode_one<false, false, 0, true>(p, stream);
+}
+
+__global__ void encoder_set_reset_kernel(m3tsz_encoder_state *state, uint64_t n, const int64_t *start,
+                                         int default_unit, bool int_opt) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  m3tsz_encoder_state st;
+  enc_state_reset(st, start[i], default_unit, int_opt);
+  state[i] = st;
+}
+
+// one thread per encoder: its tail (<= 3 16-byte groups) at the committed position of its slot
+__global__ void encoder_set_stream_kernel(const m3tsz_encoder_state *state, uint64_t n, uint8_t *buf,
+                                          uint64_t stride, uint64_t *len) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const m3tsz_encoder_state st = state[i];
+  uint32_t w[12];
+  uint64_t at = 0;
+  const uint32_t nw = enc_snapshot_words(st, w, at);
+  if (nw) {
+    uint4 *dst = reinterpret_cast<uint4 *>(buf + i * stride + at * 4ull);
+    for (uint32_t g = 0; g < nw / 4; g++)
+      dst[g] = make_uint4(__byte_perm(w[4 * g], 0, 0x0123), __byte_perm(w[4 * g + 1], 0, 0x0123),
+                          __byte_perm(w[4 * g + 2], 0, 0x0123), __byte_perm(w[4 * g + 3], 0, 0x0123));
+  }
+  len[i] = st.num_encoded ? (st.bits + kMarkerBits + 7) >> 3 : 0ull;
+}
+
+cudaError_t launch_encoder_set_reset(m3tsz_encoder_state *state, uint64_t n, const int64_t *start, int default_unit,
+                                     bool int_optimized, cudaStream_t stream) {
+  const unsigned tb = 256;
+  if ((n + tb - 1) / tb > 0x7fffffffull) return cudaErrorInvalidValue;
+  encoder_set_reset_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, stream>>>(state, n, start, default_unit,
+                                                                             int_optimized);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_encoder_set_stream(const m3tsz_encoder_state *state, uint64_t n, uint8_t *buf, uint64_t stride,
+                                      uint64_t *len, cudaStream_t stream) {
+  const unsigned tb = 256;
+  if ((n + tb - 1) / tb > 0x7fffffffull) return cudaErrorInvalidValue;
+  encoder_set_stream_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, stream>>>(state, n, buf, stride, len);
+  return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------

@@ -78,9 +78,18 @@ struct EncodeParams {
   int64_t tile_start, tile_step;
   int agg_type;
   uint32_t *n_tiles_out;  // optional [n_series]
+  // encoder-set append (launch_encode_append): per-series state in, updated in place; datapoints taken
+  m3tsz_encoder_state *state;
+  uint32_t *n_appended;
 };
 
 uint64_t encode_packed_resident_blocks();
+// encoder sets (m3tsz_encode.cu): append runs encode_kernel's append mode over p.state / p.out (the slots)
+cudaError_t launch_encode_append(const EncodeParams &p, bool int_optimized, cudaStream_t stream);
+cudaError_t launch_encoder_set_reset(m3tsz_encoder_state *state, uint64_t n, const int64_t *start, int default_unit,
+                                     bool int_optimized, cudaStream_t stream);
+cudaError_t launch_encoder_set_stream(const m3tsz_encoder_state *state, uint64_t n, uint8_t *buf, uint64_t stride,
+                                      uint64_t *len, cudaStream_t stream);
 uint64_t encode_packed_scratch_slots(uint64_t n_series);  // slots of out_stride bytes the packed mode needs
 cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_t stream);
 
