@@ -419,6 +419,64 @@ int m3tsz_decode_downsample_last_batch(m3tsz_ctx *ctx, const m3tsz_options *opts
                                        double *d_last, int64_t *d_last_at, uint32_t *d_n_points,
                                        int32_t *d_status, void *stream);
 
+/* ------------------------------------------------------------------------
+ * Fused decode + downsample for either metric type the aggregator keeps per
+ * window (src/aggregator/aggregation): the same decode, windows and
+ * out-of-order handling as m3tsz_decode_downsample_last_batch, one outputs
+ * struct.  metric_type is the reference's metric.Type id
+ * (src/metrics/metric/types.go:35-38):
+ *
+ *   M3TSZ_METRIC_GAUGE: aggregation.Gauge (gauge.go:73-106).  d_sum, d_count,
+ *     d_min, d_max are required.  d_sum_sq asks for the Gauge with expensive
+ *     aggregations: sumSq += v*v after the NaN check, multiply and add rounded
+ *     separately, 0 for an empty window.  d_last / d_last_at as in
+ *     m3tsz_decode_downsample_last_batch (with d_sum_sq, a NULL d_last or
+ *     d_last_at is kept in context scratch).  The counter_* fields must be NULL.
+ *   M3TSZ_METRIC_COUNTER: aggregation.Counter (counter.go:44-78) fed
+ *     int64(value) with Go/amd64 semantics (truncation toward zero; NaN, +-Inf
+ *     and values outside [-2^63, 2^63) give MinInt64), as the coordinator's
+ *     ingest does (src/cmd/services/m3coordinator/ingest/write.go:560-567).
+ *     int64 sum / min / max / sumSq, wrapping like Go; an empty window has sum 0,
+ *     sumSq 0, count 0, min MaxInt64, max MinInt64.  d_count, d_counter_sum,
+ *     d_counter_min, d_counter_max are required, d_counter_sum_sq is optional
+ *     (context scratch when NULL); the Gauge fields must be NULL.
+ *
+ * Every output is window-major [n_windows][n_series].  d_n_points / d_status
+ * are optional, as in the other downsample calls.  d_lengths may be NULL (CSR
+ * offsets) or give stream s = [d_offsets[s], d_offsets[s] + d_lengths[s]).
+ * Missing, mixed or unknown fields / metric types: M3TSZ_ERR_INVALID_ARG
+ * before any launch.
+ * ---------------------------------------------------------------------- */
+enum { /* metric.Type ids, src/metrics/metric/types.go:35-38 */
+  M3TSZ_METRIC_COUNTER = 1,
+  M3TSZ_METRIC_GAUGE = 3
+};
+typedef struct m3tsz_downsample_outputs {
+  int32_t metric_type;
+  int32_t reserved;     /* 0 */
+  /* Gauge */
+  double *d_sum;
+  double *d_min;
+  double *d_max;
+  double *d_sum_sq;
+  double *d_last;
+  int64_t *d_last_at;
+  /* both */
+  int64_t *d_count;
+  /* Counter */
+  int64_t *d_counter_sum;
+  int64_t *d_counter_min;
+  int64_t *d_counter_max;
+  int64_t *d_counter_sum_sq;
+  /* per series */
+  uint32_t *d_n_points;
+  int32_t *d_status;
+} m3tsz_downsample_outputs;
+int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                               uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                               uint64_t n_series, int64_t range_start_ns, int64_t window_ns, uint32_t n_windows,
+                               const m3tsz_downsample_outputs *out, void *stream);
+
 int m3tsz_decode_downsample_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts,
                                        const uint8_t *h_streams, uint64_t streams_bytes,
                                        const uint64_t *h_offsets, uint64_t n_series,
@@ -534,8 +592,11 @@ enum { /* aggregation.Type ids, src/metrics/aggregation/type.go:31-38 */
   M3TSZ_AGG_MAX = 3,
   M3TSZ_AGG_MEAN = 4,
   M3TSZ_AGG_COUNT = 6,
-  M3TSZ_AGG_SUM = 7
+  M3TSZ_AGG_SUM = 7,
+  M3TSZ_AGG_SUMSQ = 8, /* m3tsz_aggregate_tiles_ex only */
+  M3TSZ_AGG_STDEV = 9  /* m3tsz_aggregate_tiles_ex only */
 };
+/* Gauge with the six types above; SumSq / Stdev are rejected here (m3tsz_aggregate_tiles_ex has them). */
 int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                                 uint64_t streams_bytes, const uint64_t *d_offsets,
                                 const uint64_t *d_lengths, uint64_t n_series, int64_t start_ns,
@@ -543,6 +604,23 @@ int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const
                                 uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
                                 uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
                                 uint32_t *d_n_tiles, uint64_t *d_total_bytes, void *stream);
+
+/* The same for either metric type (M3TSZ_METRIC_*; one call per type: the caller groups series the way
+ * AggregateTilesOptions.MetricTypeByName does).  Valid pairs (metrics/aggregation/type.go:178-196):
+ *   Gauge: Last, Min, Max, Mean, Count, Sum, SumSq, Stdev -- Gauge.ValueOf, gauge.go:144-165;
+ *   Counter: Min, Max, Mean, Count, Sum, SumSq, Stdev -- Counter.ValueOf, counter.go:112-134, over the
+ *   windows of m3tsz_decode_downsample_ex's Counter (float64() of the int64 aggregates).
+ * Stdev = aggregation.stdev (common.go:29-37): 0 when count*(count-1) == 0, else
+ * sqrt((count*sumSq - sum*sum) / (count*(count-1))) with every operation rounded on its own.
+ * Gauge with one of the six types above gives exactly m3tsz_aggregate_tiles_batch's bytes.
+ * Any other pair: M3TSZ_ERR_INVALID_ARG before any launch. */
+int m3tsz_aggregate_tiles_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                             uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                             uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                             int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
+                             uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                             uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
+                             uint64_t *d_total_bytes, void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

@@ -25,6 +25,8 @@ ERR_CUDA = 102
 ERR_NO_DEVICE = 103
 
 AGG_LAST, AGG_MIN, AGG_MAX, AGG_MEAN, AGG_COUNT, AGG_SUM = 1, 2, 3, 4, 6, 7  # aggregation.Type ids
+AGG_SUMSQ, AGG_STDEV = 8, 9  # the expensive aggregations (m3tsz_aggregate_tiles_ex only)
+METRIC_COUNTER, METRIC_GAUGE = 1, 3  # metric.Type ids
 
 UNIT_NONE, UNIT_S, UNIT_MS, UNIT_US, UNIT_NS, UNIT_MIN, UNIT_HOUR, UNIT_DAY, UNIT_YEAR = range(9)
 
@@ -61,6 +63,15 @@ class EncodeExtras(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class DownsampleOutputs(C.Structure):
+    """m3tsz_downsample_outputs (device pointers; 0 = not wanted)."""
+    _fields_ = [("metric_type", C.c_int32), ("reserved", C.c_int32),
+                ("d_sum", C.c_void_p), ("d_min", C.c_void_p), ("d_max", C.c_void_p), ("d_sum_sq", C.c_void_p),
+                ("d_last", C.c_void_p), ("d_last_at", C.c_void_p), ("d_count", C.c_void_p),
+                ("d_counter_sum", C.c_void_p), ("d_counter_min", C.c_void_p), ("d_counter_max", C.c_void_p),
+                ("d_counter_sum_sq", C.c_void_p), ("d_n_points", C.c_void_p), ("d_status", C.c_void_p)]
+
+
 class AnnotationEntry(C.Structure):
     _fields_ = [("dp_index", C.c_uint32), ("length", C.c_uint32), ("byte_offset", C.c_uint64)]
 
@@ -94,6 +105,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_encoder_pool_create", "m3tsz_encoder_pool_get", "m3tsz_encoder_pool_destroy",
     "m3tsz_iter_pool_create", "m3tsz_iter_pool_get", "m3tsz_iter_pool_destroy",
     "m3tsz_encoder_set_reset", "m3tsz_encoder_set_append", "m3tsz_encoder_set_stream",
+    "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -244,6 +256,12 @@ def lib():
                                            vp, vp, vp]
     L.m3tsz_encoder_set_stream.restype = C.c_int
     L.m3tsz_encoder_set_stream.argtypes = [vp, vp, u64, vp, u64, vp, vp]
+    L.m3tsz_decode_downsample_ex.restype = C.c_int
+    L.m3tsz_decode_downsample_ex.argtypes = [vp, po, vp, u64, vp, vp, u64, i64, i64, u32,
+                                             C.POINTER(DownsampleOutputs), vp]
+    L.m3tsz_aggregate_tiles_ex.restype = C.c_int
+    L.m3tsz_aggregate_tiles_ex.argtypes = [vp, po, vp, u64, vp, vp, u64, i64, i64, u32, i32, i32, i32, u32, vp,
+                                           u64, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 

@@ -60,6 +60,10 @@ class DownsampleResult:
     status: torch.Tensor
     last: Optional[torch.Tensor] = None     # float64 [W, S] Gauge.Last() (want_last)
     last_at: Optional[torch.Tensor] = None  # int64 [W, S] Gauge.LastAt() in ns
+    # Gauge sumSq (want_sum_sq), float64 [W, S]; a Counter's (metric=METRIC_COUNTER) is int64 [W, S], like its
+    # sum / min / max
+    sum_sq: Optional[torch.Tensor] = None
+    metric: int = capi.METRIC_GAUGE
 
 
 class BatchCodec:
@@ -120,9 +124,16 @@ class BatchCodec:
         return out
 
     def decode_downsample(self, streams, offsets, range_start_ns, window_ns, n_windows,
-                          out: Optional[DownsampleResult] = None, want_last=False) -> DownsampleResult:
+                          out: Optional[DownsampleResult] = None, want_last=False, metric=capi.METRIC_GAUGE,
+                          want_sum_sq=False, lengths: Optional[torch.Tensor] = None) -> DownsampleResult:
+        """Window-major [W, S] aggregates of aggregation.Gauge (metric=METRIC_GAUGE; want_sum_sq adds sumSq, and
+        with it last / last_at) or aggregation.Counter (metric=METRIC_COUNTER: int64 sum / min / max / sum_sq of
+        int64(value)).  `lengths` (int64 [S]) gives stream s = offsets[s] .. + lengths[s]."""
         assert streams.dtype == torch.uint8 and streams.is_cuda
         assert offsets.dtype == torch.int64 and offsets.is_cuda
+        if metric != capi.METRIC_GAUGE or want_sum_sq or lengths is not None:
+            return self._decode_downsample_ex(streams, offsets, range_start_ns, window_ns, n_windows, out,
+                                              want_last, metric, want_sum_sq, lengths)
         S = offsets.numel() - 1
         dev = self.device
         if out is None:
@@ -145,6 +156,40 @@ class BatchCodec:
             int(range_start_ns), int(window_ns), int(n_windows), _ptr(out.sum), _ptr(out.count),
             _ptr(out.min), _ptr(out.max), _ptr(out.n_points), _ptr(out.status), _cuda_stream_ptr(dev))
         self.ctx.check(rc, "m3tsz_decode_downsample_batch")
+        return out
+
+    def _decode_downsample_ex(self, streams, offsets, range_start_ns, window_ns, n_windows, out, want_last, metric,
+                              want_sum_sq, lengths) -> DownsampleResult:
+        counter = metric == capi.METRIC_COUNTER
+        if metric not in (capi.METRIC_GAUGE, capi.METRIC_COUNTER) or (counter and want_last):
+            raise capi.M3tszError(capi.ERR_INVALID_ARG, "metric %r with want_last=%r" % (metric, want_last))
+        S = offsets.numel() - 1 if lengths is None else lengths.numel()
+        dev = self.device
+        if out is None:
+            mk = lambda dt: torch.empty((n_windows, S), dtype=dt, device=dev)
+            agg = torch.int64 if counter else torch.float64
+            last = want_last or (want_sum_sq and not counter)  # the Gauge's sumSq kernel keeps last / lastAt
+            out = DownsampleResult(
+                sum=mk(agg), count=mk(torch.int64), min=mk(agg), max=mk(agg),
+                n_points=torch.empty(S, dtype=torch.int32, device=dev),
+                status=torch.empty(S, dtype=torch.int32, device=dev),
+                last=mk(torch.float64) if last and not counter else None,
+                last_at=mk(torch.int64) if last and not counter else None,
+                sum_sq=mk(agg) if (want_sum_sq or counter) else None, metric=metric)
+        o = capi.DownsampleOutputs()
+        o.metric_type = metric
+        addr = lambda t: t.data_ptr() if t is not None else None
+        if counter:
+            o.d_counter_sum, o.d_counter_min, o.d_counter_max = addr(out.sum), addr(out.min), addr(out.max)
+            o.d_counter_sum_sq = addr(out.sum_sq)
+        else:
+            o.d_sum, o.d_min, o.d_max = addr(out.sum), addr(out.min), addr(out.max)
+            o.d_sum_sq, o.d_last, o.d_last_at = addr(out.sum_sq), addr(out.last), addr(out.last_at)
+        o.d_count, o.d_n_points, o.d_status = addr(out.count), addr(out.n_points), addr(out.status)
+        rc = capi.lib().m3tsz_decode_downsample_ex(
+            self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), _ptr(lengths), S,
+            int(range_start_ns), int(window_ns), int(n_windows), C.byref(o), _cuda_stream_ptr(dev))
+        self.ctx.check(rc, "m3tsz_decode_downsample_ex")
         return out
 
     # ------------------------------------------------------------------ encode
@@ -279,9 +324,9 @@ class BatchCodec:
 
     def aggregate_tiles(self, streams, offsets, start_ns, step_ns, n_windows, agg_type=capi.AGG_LAST,
                         out_unit=capi.UNIT_S, lengths=None, align=64, capacity=None,
-                        out: Optional["PackedResult"] = None):
-        """storage.TileAggregator compute: decode -> Gauge per Step window -> re-encode (packed).
-        Returns (PackedResult, n_tiles int32 [S])."""
+                        out: Optional["PackedResult"] = None, metric_type=capi.METRIC_GAUGE):
+        """storage.TileAggregator compute: decode -> Gauge (or Counter: metric_type=METRIC_COUNTER) per Step
+        window -> re-encode (packed).  Returns (PackedResult, n_tiles int32 [S])."""
         S = offsets.numel() - 1 if lengths is None else lengths.numel()
         dev = self.device
         if out is None:
@@ -294,6 +339,14 @@ class BatchCodec:
                 status=torch.empty(S, dtype=torch.int32, device=dev),
                 total=torch.zeros(1, dtype=torch.int64, device=dev))
         n_tiles = torch.empty(S, dtype=torch.int32, device=dev)
+        if metric_type != capi.METRIC_GAUGE or agg_type in (capi.AGG_SUMSQ, capi.AGG_STDEV):
+            rc = capi.lib().m3tsz_aggregate_tiles_ex(
+                self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets),
+                _ptr(lengths), S, int(start_ns), int(step_ns), int(n_windows), int(metric_type), int(agg_type),
+                int(out_unit), int(align), _ptr(out.packed), out.packed.numel(), _ptr(out.offsets),
+                _ptr(out.out_len), _ptr(out.status), _ptr(n_tiles), _ptr(out.total), _cuda_stream_ptr(dev))
+            self.ctx.check(rc, "m3tsz_aggregate_tiles_ex")
+            return out, n_tiles
         rc = capi.lib().m3tsz_aggregate_tiles_batch(
             self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets),
             _ptr(lengths), S, int(start_ns), int(step_ns), int(n_windows), int(agg_type), int(out_unit),

@@ -272,6 +272,77 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
   return M3TSZ_OK;
 }
 
+// m3tsz_decode_downsample_ex: a Gauge without sumSq is downsample_impl (modes 1 / 2, today's kernels); a Gauge
+// with sumSq is mode 4, a Counter mode 5.
+int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                               uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                               uint64_t n_series, int64_t range_start_ns, int64_t window_ns, uint32_t n_windows,
+                               const m3tsz_downsample_outputs *o, void *stream) {
+  if (!ctx || !valid_opts(opts) || !o || o->reserved != 0) return M3TSZ_ERR_INVALID_ARG;
+  const bool gauge = o->metric_type == M3TSZ_METRIC_GAUGE, counter = o->metric_type == M3TSZ_METRIC_COUNTER;
+  if (gauge) {
+    if (o->d_counter_sum || o->d_counter_min || o->d_counter_max || o->d_counter_sum_sq ||
+        (o->d_last_at && !o->d_last && !o->d_sum_sq))
+      return M3TSZ_ERR_INVALID_ARG;
+    if (!o->d_sum_sq)
+      return downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, range_start_ns,
+                             window_ns, n_windows, o->d_sum, o->d_count, o->d_min, o->d_max, o->d_last,
+                             o->d_last_at, o->d_last != nullptr, o->d_n_points, o->d_status, stream);
+  } else if (counter) {
+    if (o->d_sum || o->d_min || o->d_max || o->d_sum_sq || o->d_last || o->d_last_at) return M3TSZ_ERR_INVALID_ARG;
+  } else {
+    return M3TSZ_ERR_INVALID_ARG;
+  }
+  if (n_series == 0) return M3TSZ_OK;
+  DecodeParams p;
+  if (!decode_params(opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, o->d_n_points, o->d_status,
+                     p) ||
+      !o->d_count || window_ns <= 0 || n_windows == 0 || n_windows > 0x7fffffffu ||
+      (gauge && (!o->d_sum || !o->d_min || !o->d_max)) ||
+      (counter && (!o->d_counter_sum || !o->d_counter_min || !o->d_counter_max)))
+    return M3TSZ_ERR_INVALID_ARG;
+  if ((__int128)range_start_ns + (__int128)n_windows * (__int128)window_ns > (__int128)INT64_MAX)
+    return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  // what the caller leaves out but the kernel keeps (to re-open a committed window exactly) lives in scratch
+  const size_t wb = (size_t)n_series * n_windows * 8;
+  void *sc = nullptr;
+  int rc;
+  p.range_start = range_start_ns;
+  p.window = window_ns;
+  p.n_windows = n_windows;
+  p.ds_count = o->d_count;
+  if (gauge) {
+    p.ds_sum = o->d_sum;
+    p.ds_min = o->d_min;
+    p.ds_max = o->d_max;
+    p.ds_sum_sq = o->d_sum_sq;
+    p.ds_last = o->d_last;
+    p.ds_last_at = o->d_last_at;
+    if (!p.ds_last) {
+      if ((rc = ensure(ctx, kSlotWinLast, wb, &sc))) return rc;
+      p.ds_last = (double *)sc;
+    }
+    if (!p.ds_last_at) {
+      if ((rc = ensure(ctx, kSlotWinLastAt, wb, &sc))) return rc;
+      p.ds_last_at = (int64_t *)sc;
+    }
+  } else {
+    p.ds_isum = o->d_counter_sum;
+    p.ds_imin = o->d_counter_min;
+    p.ds_imax = o->d_counter_max;
+    p.ds_isum_sq = o->d_counter_sum_sq;
+    if (!p.ds_isum_sq) {
+      if ((rc = ensure(ctx, kSlotWinSumSq, wb, &sc))) return rc;
+      p.ds_isum_sq = (int64_t *)sc;
+    }
+  }
+  CK(launch_decode(p, opts->int_optimized != 0, gauge ? 4 : 5, (cudaStream_t)stream));
+  ctx->launches++;
+  return M3TSZ_OK;
+}
+
 int m3tsz_decode_downsample_batch(m3tsz_ctx *ctx, const m3tsz_options *opts,
                                   const uint8_t *d_streams, uint64_t streams_bytes,
                                   const uint64_t *d_offsets, uint64_t n_series,
@@ -487,17 +558,14 @@ int m3tsz_prom_convert_batch(m3tsz_ctx *ctx, const int64_t *d_ts, const double *
   return M3TSZ_OK;
 }
 
-int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                                uint64_t streams_bytes, const uint64_t *d_offsets,
-                                const uint64_t *d_lengths, uint64_t n_series, int64_t start_ns,
-                                int64_t step_ns, uint32_t n_windows, int32_t agg_type, int32_t out_unit,
-                                uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
-                                uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
-                                uint32_t *d_n_tiles, uint64_t *d_total_bytes, void *stream) {
-  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status) return M3TSZ_ERR_INVALID_ARG;
-  if (!(agg_type == M3TSZ_AGG_LAST || agg_type == M3TSZ_AGG_MIN || agg_type == M3TSZ_AGG_MAX ||
-        agg_type == M3TSZ_AGG_MEAN || agg_type == M3TSZ_AGG_COUNT || agg_type == M3TSZ_AGG_SUM))
-    return M3TSZ_ERR_INVALID_ARG;
+// Both tile calls, after the caller checked ctx, opts, d_total_bytes, d_status and the (metric, type) pair.
+static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
+                                uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                                uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
+                                uint64_t *d_total_bytes, void *stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (n_series == 0) {
     DeviceGuard guard(ctx->device);
@@ -520,10 +588,39 @@ int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   if ((rc = ensure(ctx, kSlotWinLast, wb, &d_last))) return rc;
   if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_np))) return rc;
   if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_sst))) return rc;
-  // 1. fused decode + Gauge windows (with `last`)
-  rc = downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                       n_windows, (double *)d_sum, (int64_t *)d_cnt, (double *)d_min, (double *)d_max,
-                       (double *)d_last, (int64_t *)d_lat, true, (uint32_t *)d_np, (int32_t *)d_sst, st);
+  // 1. fused decode + windows: the Gauge with `last` (mode 2), + sumSq for SumSq / Stdev (mode 4), or the Counter
+  //    (mode 5, its int64 sum / min / max in the Gauge's slots)
+  const bool counter = metric_type == M3TSZ_METRIC_COUNTER;
+  const bool sq = counter || agg_type == M3TSZ_AGG_SUMSQ || agg_type == M3TSZ_AGG_STDEV;
+  void *d_sq = nullptr;
+  if (!sq) {
+    rc = downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                         n_windows, (double *)d_sum, (int64_t *)d_cnt, (double *)d_min, (double *)d_max,
+                         (double *)d_last, (int64_t *)d_lat, true, (uint32_t *)d_np, (int32_t *)d_sst, st);
+  } else {
+    if ((rc = ensure(ctx, kSlotWinSumSq, wb, &d_sq))) return rc;
+    m3tsz_downsample_outputs o;
+    memset(&o, 0, sizeof(o));
+    o.metric_type = counter ? M3TSZ_METRIC_COUNTER : M3TSZ_METRIC_GAUGE;
+    o.d_count = (int64_t *)d_cnt;
+    if (counter) {
+      o.d_counter_sum = (int64_t *)d_sum;
+      o.d_counter_min = (int64_t *)d_min;
+      o.d_counter_max = (int64_t *)d_max;
+      o.d_counter_sum_sq = (int64_t *)d_sq;
+    } else {
+      o.d_sum = (double *)d_sum;
+      o.d_min = (double *)d_min;
+      o.d_max = (double *)d_max;
+      o.d_sum_sq = (double *)d_sq;
+      o.d_last = (double *)d_last;
+      o.d_last_at = (int64_t *)d_lat;
+    }
+    o.d_n_points = (uint32_t *)d_np;
+    o.d_status = (int32_t *)d_sst;
+    rc = m3tsz_decode_downsample_ex(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
+                                    step_ns, n_windows, &o, st);
+  }
   if (rc) return rc;
   // 2. re-encode straight from the window-major aggregates (the encoder's input stage skips empty
   //    windows, stamps the window end and takes Gauge.ValueOf(agg_type)) into the packed buffer
@@ -544,21 +641,70 @@ int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   p.out_len = d_out_len;
   p.status = d_status;
   p.in_mode = 2;
-  p.tile_sum = (const double *)d_sum;
   p.tile_count = (const int64_t *)d_cnt;
-  p.tile_min = (const double *)d_min;
-  p.tile_max = (const double *)d_max;
-  p.tile_last = (const double *)d_last;
+  if (counter) {
+    p.tile_isum = (const int64_t *)d_sum;
+    p.tile_imin = (const int64_t *)d_min;
+    p.tile_imax = (const int64_t *)d_max;
+  } else {
+    p.tile_sum = (const double *)d_sum;
+    p.tile_min = (const double *)d_min;
+    p.tile_max = (const double *)d_max;
+    p.tile_last = (const double *)d_last;
+  }
+  p.tile_sum_sq = d_sq;  // (NULL unless SumSq / Stdev / Counter)
   p.tile_src_status = (const int32_t *)d_sst;
   p.tile_start = start_ns;
   p.tile_step = step_ns;
   p.agg_type = agg_type;
+  p.metric_type = metric_type;
   p.n_tiles_out = d_n_tiles;
   CK(launch_encode(p, opts->int_optimized != 0, st));
   ctx->launches += 2;
   CK(launch_tiles_status((const int32_t *)d_sst, d_status, n_series, st));
   ctx->launches++;
   return M3TSZ_OK;
+}
+
+int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                uint64_t streams_bytes, const uint64_t *d_offsets,
+                                const uint64_t *d_lengths, uint64_t n_series, int64_t start_ns,
+                                int64_t step_ns, uint32_t n_windows, int32_t agg_type, int32_t out_unit,
+                                uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+                                uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
+                                uint32_t *d_n_tiles, uint64_t *d_total_bytes, void *stream) {
+  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status) return M3TSZ_ERR_INVALID_ARG;
+  if (!(agg_type == M3TSZ_AGG_LAST || agg_type == M3TSZ_AGG_MIN || agg_type == M3TSZ_AGG_MAX ||
+        agg_type == M3TSZ_AGG_MEAN || agg_type == M3TSZ_AGG_COUNT || agg_type == M3TSZ_AGG_SUM))
+    return M3TSZ_ERR_INVALID_ARG;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, M3TSZ_METRIC_GAUGE, agg_type, out_unit, align, d_packed, packed_capacity,
+                              d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream);
+}
+
+// aggregation.Type.IsValidForGauge / IsValidForCounter, src/metrics/aggregation/type.go:178-196
+static bool valid_tile_pair(int32_t metric_type, int32_t agg_type) {
+  switch (agg_type) {
+    case M3TSZ_AGG_LAST: return metric_type == M3TSZ_METRIC_GAUGE;
+    case M3TSZ_AGG_MIN: case M3TSZ_AGG_MAX: case M3TSZ_AGG_MEAN: case M3TSZ_AGG_COUNT: case M3TSZ_AGG_SUM:
+    case M3TSZ_AGG_SUMSQ: case M3TSZ_AGG_STDEV:
+      return metric_type == M3TSZ_METRIC_GAUGE || metric_type == M3TSZ_METRIC_COUNTER;
+    default: return false;
+  }
+}
+
+int m3tsz_aggregate_tiles_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                             uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                             uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                             int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
+                             uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                             uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
+                             uint64_t *d_total_bytes, void *stream) {
+  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !valid_tile_pair(metric_type, agg_type))
+    return M3TSZ_ERR_INVALID_ARG;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, metric_type, agg_type, out_unit, align, d_packed, packed_capacity,
+                              d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream);
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

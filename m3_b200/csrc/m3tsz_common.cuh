@@ -105,6 +105,27 @@ __device__ __forceinline__ double mult_pow10(int m) {
   }
 }
 
+// Go int64(float64) on amd64 (CVTTSD2SQ): truncation toward zero; out of range / NaN -> MinInt64.  The
+// Counter aggregation takes its values this way (int64(dp.Value), m3coordinator ingest/write.go:560-567).  The
+// encoder's classifier has the same conversion as go_f64_to_u64_via_i64 (m3tsz_encode.cu), where the host tests
+// of the encoder compile it from; tests/test_independent_aggregations.py checks that the two agree.
+__device__ __forceinline__ int64_t go_f64_to_i64(double a) {
+  if (!(a >= -9223372036854775808.0 && a < 9223372036854775808.0)) return (int64_t)0x8000000000000000ull;
+  return (int64_t)__double2ll_rz(a);
+}
+
+// aggregation.stdev (src/aggregator/aggregation/common.go:29-37): div = count*(count-1) in int64 (0: result 0),
+// num = float64(count)*sumSq - sum*sum as two roundings each (no fusion), sqrt(num / float64(div)).  Every NaN this
+// arithmetic can make on amd64 is the invalid-operation default 0xFFF8000000000000 (Inf - Inf, sqrt of a negative,
+// or one carried in `sum` from +Inf + -Inf), so a NaN result is written as that.
+__device__ __forceinline__ double agg_stdev(int64_t count, double sum_sq, double sum) {
+  const int64_t div = (int64_t)((uint64_t)count * (uint64_t)(count - 1));
+  if (div == 0) return 0.0;
+  const double num = __dsub_rn(__dmul_rn(__ll2double_rn(count), sum_sq), __dmul_rn(sum, sum));
+  const double r = __dsqrt_rn(__ddiv_rn(num, __ll2double_rn(div)));
+  return r == r ? r : __longlong_as_double((long long)0xFFF8000000000000ull);
+}
+
 // XXH64, seed 0 (cespare/xxhash/v2 Sum64, go.mod:10): TimestampEncoder keeps the checksum of the last annotation
 // written (timestamp_encoder.go:56,166-195) and rewrites an annotation only when its checksum differs; Encoder.
 // LastAnnotationChecksum() exposes it (encoder.go:321-327).  One definition for the streaming handles (host) and the

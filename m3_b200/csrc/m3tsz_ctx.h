@@ -29,15 +29,19 @@ struct Scratch {
 //   6             unit                                           decode_host
 //   7             annotation refs, or annotation series offsets  decode_host; encode_host
 //   8-11          window sum / count / min / max                 downsample_host, tiles
-//   12            lastAt                                         downsample_last with a NULL d_last_at, tiles
+//                 (a Counter's int64 sum / count / min / max:    tiles
+//                 the same 8 bytes per window)
+//   12            lastAt                                         downsample_last / downsample_ex with a NULL
+//                                                                d_last_at, tiles
 //   13, 14        annotation entries, annotation bytes           encode_host
 //   15            compaction scan temp                           compact_streams
 //   16-24, 26-34  pipeline lane 0 / 1, buffers 0-8 (lane_slot)   encode_host, fetch
+//   25            window sumSq (Gauge float64 / Counter int64)   downsample_ex with a NULL sum_sq, tiles
 //   36, 37        packed slot sets, batch counter                packed encode, tiles
-//   38, 39        window last, tile encoder starts               tiles
+//   38, 39        window last, tile encoder starts               tiles, downsample_ex (38, NULL d_last); tiles
 //   40-47         streaming handles, under handle_mu             m3tsz_stream.cu
 //
-// Slots 25 and 35 are unused.
+// Slot 35 is unused.
 enum Slot : int {
   kSlotStreams = 0,
   kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
@@ -57,6 +61,7 @@ enum Slot : int {
   kSlotAnnBytes = 14,
   kSlotCompactTmp = 15,
   kSlotLaneBase = 16,
+  kSlotWinSumSq = 25,  // between the two pipeline lanes' slot ranges
   kSlotPackedSlots = 36,
   kSlotBatchCounter = 37,
   kSlotWinLast = 38,

@@ -435,8 +435,20 @@ __device__ __forceinline__ void ring_fill(uint32_t ring_lane_addr, const uint8_t
   }
 }
 
+// The fused-downsample modes: 1 Gauge (sum, count, min, max), 2 + last / lastAt, 4 + sumSq (the Gauge with
+// expensive aggregations), 5 Counter (int64 sum, count, min, max, sumSq).
+__host__ __device__ constexpr bool dec_ds_mode(int mode) { return mode == 1 || mode == 2 || mode == 4 || mode == 5; }
+// 4 and 5 carry two more 64-bit accumulators than mode 2 and start from the same budget (-Xptxas -v reports no
+// spills at 96 registers)
+__host__ __device__ constexpr int dec_min_blocks(int mode) { return dec_ds_mode(mode) ? DEC_MIN_BLOCKS_DS : DEC_MIN_BLOCKS; }
+
+// window accumulator type: the Gauge's float64, the Counter's int64 (counter.go:31-41)
+template <bool COUNTER> struct DsVal { using T = double; };
+template <> struct DsVal<true> { using T = int64_t; };
+
 // Fused-downsample per-lane accumulator: aggregation.Gauge of the open window
-// (/root/reference/src/aggregator/aggregation/gauge.go:31-106).
+// (/root/reference/src/aggregator/aggregation/gauge.go:31-106), or aggregation.Counter (counter.go:31-78) in mode 5.
+template <typename V>
 struct DsAcc {
   int64_t d;      // hot path: (time of the last datapoint) - w_end while the group's pre-check holds
   int64_t w_end;  // exclusive end of the open window
@@ -446,8 +458,10 @@ struct DsAcc {
   // sum as gauge.go:92; min / max start at +inf / -inf instead of NaN: with `v < mn` / `v > mx`
   // that takes the same decisions as gauge.go:93-99 on every sequence of values (a NaN value never
   // compares true, signed zeros keep the first one seen), and "no value seen" is the one state
-  // mn == +inf && mx == -inf, written out as NaN / NaN
-  double sum, mn, mx;
+  // mn == +inf && mx == -inf, written out as NaN / NaN.  Counter: min / max start at MaxInt64 / MinInt64 and are
+  // written as they are (counter.go:44-78)
+  V sum, mn, mx;
+  V sq;              // modes 4, 5: sumSq (gauge.go:101-103, counter.go:72-74)
   uint32_t cnt;      // datapoints in the open window (NaNs counted, gauge.go:85)
   uint32_t n_sync;   // s.n when cnt was last brought up to date: s.n - n_sync = hot datapoints since (all of
                      // them in the open window), folded into cnt at the next commit / general-path visit
@@ -456,18 +470,21 @@ struct DsAcc {
 };
 
 // MODE 0: plain decode (ts, value) ; 1: fused 5-tuple-less downsample (sum, count, min, max);
-// 2: downsample + last (+ lastAt scratch).
+// 2: downsample + last (+ lastAt scratch); 4: + sumSq; 5: Counter downsample.
 template <bool INT_OPT, int MODE>
-__global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? DEC_MIN_BLOCKS_DS : DEC_MIN_BLOCKS)
+__global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
     decode_kernel(const DecodeParams p) {
   // MODE 0: plain decode, series-major output [series][point]; 3: plain decode, point-major output
   // [point][series] (every step's 32 lanes store 32 consecutive elements: coalesced 256-byte rows);
-  // 1: fused downsample (sum, count, min, max); 2: + last / lastAt
+  // 1: fused downsample (sum, count, min, max); 2: + last / lastAt; 4: + sumSq (Gauge with expensive
+  // aggregations); 5: Counter (int64(value): sum, count, min, max, sumSq; no last, no NaN vote)
   // The fused-downsample and point-major kernels read the ring as 8-byte pairs; series-major decode keeps the
   // 16-byte reads (the pairs cost more shared-memory wavefronts, see the parse).
   constexpr bool RING64 = (MODE != 0);
-  constexpr bool DS = (MODE == 1 || MODE == 2), LAST = (MODE == 2), PLAIN = (MODE == 0 || MODE == 3),
+  constexpr bool DS = dec_ds_mode(MODE), LAST = (MODE == 2 || MODE == 4), PLAIN = (MODE == 0 || MODE == 3),
                  PM = (MODE == 3);
+  constexpr bool SQ = (MODE == 4), CTR = (MODE == 5);  // Gauge sumSq / Counter
+  using V = typename DsVal<CTR>::T;
   extern __shared__ __align__(16) uint32_t smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -530,16 +547,25 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? DEC
   int plz = 64, ptz = 0;
 
   const double kNaN = __longlong_as_double((long long)kGoNaNBits);
-  DsAcc acc;
+  constexpr int64_t kMaxI64 = 0x7fffffffffffffffll, kMinI64 = (int64_t)0x8000000000000000ull;
+  DsAcc<V> acc;
   acc.d = 0;
   acc.w_end = 0;
   acc.cur_w = -1;
   acc.hi_w = -1;
   acc.o = 0;
   acc.in_open = false;
-  acc.sum = 0.0;
-  acc.mn = __longlong_as_double(0x7ff0000000000000ll);
-  acc.mx = __longlong_as_double((long long)0xfff0000000000000ull);
+  if constexpr (CTR) {
+    acc.sum = 0;
+    acc.mn = kMaxI64;
+    acc.mx = kMinI64;
+    acc.sq = 0;
+  } else {
+    acc.sum = 0.0;
+    acc.mn = __longlong_as_double(0x7ff0000000000000ll);
+    acc.mx = __longlong_as_double((long long)0xfff0000000000000ull);
+    if constexpr (SQ) acc.sq = 0.0;
+  }
   acc.cnt = 0;
   acc.n_sync = 0;
   acc.last_t = 0;
@@ -552,44 +578,91 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? DEC
   const double kNegInf = __longlong_as_double((long long)0xfff0000000000000ull);
   auto ds_store = [&]() {  // commit the open window's aggregate
     const uint64_t o = acc.o;
-    const bool none = acc.mn == kPosInf && acc.mx == kNegInf;  // no non-NaN value in the window
-    p.ds_sum[o] = acc.sum;
-    p.ds_count[o] = (int64_t)acc.cnt;
-    p.ds_min[o] = none ? kNaN : acc.mn;
-    p.ds_max[o] = none ? kNaN : acc.mx;
-    if (LAST) {
-      p.ds_last[o] = __longlong_as_double((long long)acc.last_v);
-      p.ds_last_at[o] = acc.last_t;
+    if constexpr (CTR) {
+      p.ds_isum[o] = acc.sum;
+      p.ds_count[o] = (int64_t)acc.cnt;
+      p.ds_imin[o] = acc.mn;
+      p.ds_imax[o] = acc.mx;
+      p.ds_isum_sq[o] = acc.sq;
+    } else {
+      const bool none = acc.mn == kPosInf && acc.mx == kNegInf;  // no non-NaN value in the window
+      p.ds_sum[o] = acc.sum;
+      p.ds_count[o] = (int64_t)acc.cnt;
+      p.ds_min[o] = none ? kNaN : acc.mn;
+      p.ds_max[o] = none ? kNaN : acc.mx;
+      if (LAST) {
+        p.ds_last[o] = __longlong_as_double((long long)acc.last_v);
+        p.ds_last_at[o] = acc.last_t;
+      }
+      if constexpr (SQ) p.ds_sum_sq[o] = acc.sq;
     }
   };
   auto ds_store_empty = [&](int32_t w) {  // NewGauge: sum 0, count 0, min/max NaN, last 0 (gauge.go:45-51)
     const uint64_t o = (uint64_t)(uint32_t)w * p.n_series + sidx;
-    p.ds_sum[o] = 0.0;
-    p.ds_count[o] = 0;
-    p.ds_min[o] = kNaN;
-    p.ds_max[o] = kNaN;
-    if (LAST) {
-      p.ds_last[o] = 0.0;
-      p.ds_last_at[o] = 0;
+    if constexpr (CTR) {  // NewCounter: sum 0, count 0, min MaxInt64, max MinInt64, sumSq 0 (counter.go:44-50)
+      p.ds_isum[o] = 0;
+      p.ds_count[o] = 0;
+      p.ds_imin[o] = kMaxI64;
+      p.ds_imax[o] = kMinI64;
+      p.ds_isum_sq[o] = 0;
+    } else {
+      p.ds_sum[o] = 0.0;
+      p.ds_count[o] = 0;
+      p.ds_min[o] = kNaN;
+      p.ds_max[o] = kNaN;
+      if (LAST) {
+        p.ds_last[o] = 0.0;
+        p.ds_last_at[o] = 0;
+      }
+      if constexpr (SQ) p.ds_sum_sq[o] = 0.0;
     }
   };
   auto ds_reset = [&]() {
-    acc.sum = 0.0;
-    acc.cnt = 0;
-    acc.mn = kPosInf;
-    acc.mx = kNegInf;
+    if constexpr (CTR) {
+      acc.sum = 0;
+      acc.cnt = 0;
+      acc.mn = kMaxI64;
+      acc.mx = kMinI64;
+      acc.sq = 0;
+    } else {
+      acc.sum = 0.0;
+      acc.cnt = 0;
+      acc.mn = kPosInf;
+      acc.mx = kNegInf;
+      if constexpr (SQ) acc.sq = 0.0;
+    }
+  };
+  // Counter.Update without lastAt and count (counter.go:52-78): x = int64(value), int64 arithmetic that wraps
+  auto ctr_add = [&](uint64_t vbits) {
+    const int64_t x = go_f64_to_i64(__longlong_as_double((long long)vbits));
+    acc.sum = (int64_t)((uint64_t)acc.sum + (uint64_t)x);
+    if (acc.mx < x) acc.mx = x;
+    if (acc.mn > x) acc.mn = x;
+    acc.sq = (int64_t)((uint64_t)acc.sq + (uint64_t)x * (uint64_t)x);
   };
   auto ds_add = [&](uint64_t vbits) {  // Gauge.updateTotals without `last` and `count` (gauge.go:85-101)
-    const double dv = __longlong_as_double((long long)vbits);
-    if (dv == dv) acc.sum = __dadd_rn(acc.sum, dv);
-    if (dv > acc.mx) acc.mx = dv;
-    if (dv < acc.mn) acc.mn = dv;
+    if constexpr (CTR) {
+      ctr_add(vbits);
+    } else {
+      const double dv = __longlong_as_double((long long)vbits);
+      if (dv == dv) acc.sum = __dadd_rn(acc.sum, dv);
+      if (dv > acc.mx) acc.mx = dv;
+      if (dv < acc.mn) acc.mn = dv;
+      if constexpr (SQ) {  // after the NaN check, a separate multiply and add (gauge.go:101-103)
+        if (dv == dv) acc.sq = __dadd_rn(acc.sq, __dmul_rn(dv, dv));
+      }
+    }
   };
   auto ds_add_no_nan = [&](uint64_t vbits) {  // ... when no lane of the warp holds a NaN
-    const double dv = __longlong_as_double((long long)vbits);
-    acc.sum = __dadd_rn(acc.sum, dv);
-    if (dv > acc.mx) acc.mx = dv;
-    if (dv < acc.mn) acc.mn = dv;
+    if constexpr (CTR) {
+      ctr_add(vbits);
+    } else {
+      const double dv = __longlong_as_double((long long)vbits);
+      acc.sum = __dadd_rn(acc.sum, dv);
+      if (dv > acc.mx) acc.mx = dv;
+      if (dv < acc.mn) acc.mn = dv;
+      if constexpr (SQ) acc.sq = __dadd_rn(acc.sq, __dmul_rn(dv, dv));
+    }
   };
 
   // refills are DEC_FILL-word aligned: start at the stream's first word rounded down
@@ -795,7 +868,7 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? DEC
             const bool adv = d_hi >= 0;
             const uint64_t nb = s.prev_bits ^ xr;
             const double nbd = __longlong_as_double((long long)nb);
-            if (__any_sync(FULL_MASK, adv || nbd != nbd)) {
+            if (__any_sync(FULL_MASK, adv || (!CTR && nbd != nbd))) {  // (a Counter needs no NaN vote)
               if (adv) {  // it opens the next window: commit the one it leaves
                 const uint32_t hot_n = s.n - acc.n_sync;  // hot datapoints since cnt was last updated
                 if (LAST && hot_n) {  // `last` of in-order datapoints = the previous one
@@ -1021,17 +1094,26 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, (MODE == 1 || MODE == 2) ? DEC
               ds_reset();
             } else {  // out-of-order timestamp: reopen a committed window
               const uint64_t o = acc.o;
-              acc.sum = p.ds_sum[o];
-              acc.cnt = (uint32_t)p.ds_count[o];
-              acc.mn = p.ds_min[o];
-              acc.mx = p.ds_max[o];
-              if (acc.mn != acc.mn) {  // stored as NaN / NaN: no value yet
-                acc.mn = kPosInf;
-                acc.mx = kNegInf;
-              }
-              if (LAST) {
-                acc.last_v = (uint64_t)__double_as_longlong(p.ds_last[o]);
-                acc.last_t = p.ds_last_at[o];
+              if constexpr (CTR) {
+                acc.sum = p.ds_isum[o];
+                acc.cnt = (uint32_t)p.ds_count[o];
+                acc.mn = p.ds_imin[o];
+                acc.mx = p.ds_imax[o];
+                acc.sq = p.ds_isum_sq[o];
+              } else {
+                acc.sum = p.ds_sum[o];
+                acc.cnt = (uint32_t)p.ds_count[o];
+                acc.mn = p.ds_min[o];
+                acc.mx = p.ds_max[o];
+                if (acc.mn != acc.mn) {  // stored as NaN / NaN: no value yet
+                  acc.mn = kPosInf;
+                  acc.mx = kNegInf;
+                }
+                if (LAST) {
+                  acc.last_v = (uint64_t)__double_as_longlong(p.ds_last[o]);
+                  acc.last_t = p.ds_last_at[o];
+                }
+                if constexpr (SQ) acc.sq = p.ds_sum_sq[o];
               }
             }
             acc.cur_w = (int32_t)nw;
@@ -1132,7 +1214,7 @@ static cudaError_t launch_one(const DecodeParams &p, cudaStream_t stream) {
   // 500 k x 1440, int-optimised (ms, carveout 100 / 132 / 164 / 196 / 228 KB): point-major decode 8.22 / 7.59 /
   // 7.60 / 7.58 / 8.57, fused downsample 6.36 / 5.37 / 5.00 / 4.98 / 5.78.  So: plain decode 4 blocks + 92 KB
   // of L1, fused downsample 5 blocks + 60 KB.
-  constexpr int carveout_kb = (MODE == 1 || MODE == 2) ? 196 : 164;
+  constexpr int carveout_kb = dec_ds_mode(MODE) ? 196 : 164;
   e = cudaFuncSetAttribute(decode_kernel<INT_OPT, MODE>, cudaFuncAttributePreferredSharedMemoryCarveout,
                            carveout_kb * 100 / 228);
   if (e != cudaSuccess) return e;
@@ -1144,13 +1226,16 @@ static cudaError_t launch_one(const DecodeParams &p, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
-// mode: 0 plain decode (series-major), 1 fused downsample (sum/count/min/max), 2 + last, 3 plain decode (point-major)
+// mode: 0 plain decode (series-major), 1 fused downsample (sum/count/min/max), 2 + last, 3 plain decode (point-major),
+// 4 fused downsample + last + sumSq, 5 fused Counter downsample
 cudaError_t launch_decode(const DecodeParams &p, bool int_optimized, int mode, cudaStream_t stream) {
   switch (mode) {
     case 0: return int_optimized ? launch_one<true, 0>(p, stream) : launch_one<false, 0>(p, stream);
     case 1: return int_optimized ? launch_one<true, 1>(p, stream) : launch_one<false, 1>(p, stream);
     case 2: return int_optimized ? launch_one<true, 2>(p, stream) : launch_one<false, 2>(p, stream);
     case 3: return int_optimized ? launch_one<true, 3>(p, stream) : launch_one<false, 3>(p, stream);
+    case 4: return int_optimized ? launch_one<true, 4>(p, stream) : launch_one<false, 4>(p, stream);
+    case 5: return int_optimized ? launch_one<true, 5>(p, stream) : launch_one<false, 5>(p, stream);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -1058,14 +1058,37 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       skip_o = (c == 0);
       t_o = p.tile_start + (int64_t)(row + 1) * p.tile_step;  // the window's end boundary
       double v = 0.0;
-      switch (p.agg_type) {  // Gauge.ValueOf, gauge.go:144-165 (uniform switch)
-        case M3TSZ_AGG_LAST: v = __ldg(p.tile_last + o); break;
-        case M3TSZ_AGG_MIN: v = __ldg(p.tile_min + o); break;
-        case M3TSZ_AGG_MAX: v = __ldg(p.tile_max + o); break;
-        case M3TSZ_AGG_MEAN: v = c == 0 ? 0.0 : __ddiv_rn(__ldg(p.tile_sum + o), __ll2double_rn(c)); break;
-        case M3TSZ_AGG_COUNT: v = __ll2double_rn(c); break;
-        case M3TSZ_AGG_SUM: v = __ldg(p.tile_sum + o); break;
-        default: break;
+      if (p.metric_type == M3TSZ_METRIC_COUNTER) {
+        // Counter.ValueOf, counter.go:112-134: float64() of the int64 aggregates (uniform switch)
+        switch (p.agg_type) {
+          case M3TSZ_AGG_MIN: v = __ll2double_rn(__ldg(p.tile_imin + o)); break;
+          case M3TSZ_AGG_MAX: v = __ll2double_rn(__ldg(p.tile_imax + o)); break;
+          case M3TSZ_AGG_MEAN:
+            v = c == 0 ? 0.0 : __ddiv_rn(__ll2double_rn(__ldg(p.tile_isum + o)), __ll2double_rn(c));
+            break;
+          case M3TSZ_AGG_COUNT: v = __ll2double_rn(c); break;
+          case M3TSZ_AGG_SUM: v = __ll2double_rn(__ldg(p.tile_isum + o)); break;
+          case M3TSZ_AGG_SUMSQ: v = __ll2double_rn(__ldg(static_cast<const int64_t *>(p.tile_sum_sq) + o)); break;
+          case M3TSZ_AGG_STDEV:
+            v = agg_stdev(c, __ll2double_rn(__ldg(static_cast<const int64_t *>(p.tile_sum_sq) + o)),
+                          __ll2double_rn(__ldg(p.tile_isum + o)));
+            break;
+          default: break;
+        }
+      } else {
+        switch (p.agg_type) {  // Gauge.ValueOf, gauge.go:144-165 (uniform switch)
+          case M3TSZ_AGG_LAST: v = __ldg(p.tile_last + o); break;
+          case M3TSZ_AGG_MIN: v = __ldg(p.tile_min + o); break;
+          case M3TSZ_AGG_MAX: v = __ldg(p.tile_max + o); break;
+          case M3TSZ_AGG_MEAN: v = c == 0 ? 0.0 : __ddiv_rn(__ldg(p.tile_sum + o), __ll2double_rn(c)); break;
+          case M3TSZ_AGG_COUNT: v = __ll2double_rn(c); break;
+          case M3TSZ_AGG_SUM: v = __ldg(p.tile_sum + o); break;
+          case M3TSZ_AGG_SUMSQ: v = __ldg(static_cast<const double *>(p.tile_sum_sq) + o); break;
+          case M3TSZ_AGG_STDEV:
+            v = agg_stdev(c, __ldg(static_cast<const double *>(p.tile_sum_sq) + o), __ldg(p.tile_sum + o));
+            break;
+          default: break;
+        }
       }
       v_o = (uint64_t)__double_as_longlong(v);
     }

@@ -39,13 +39,24 @@ struct DecodeParams {
   m3tsz_dp_event *events;
   uint64_t events_capacity;
   unsigned long long *event_count;
+  // modes 4 and 5 (after every older field, which keep their parameter offsets; window-major like the above)
+  double *ds_sum_sq;    // mode 4: Gauge sumSq (+ the mode 2 outputs)
+  int64_t *ds_isum, *ds_imin, *ds_imax, *ds_isum_sq;  // mode 5: Counter (+ ds_count)
 };
 
-// mode: 0 plain decode, 1 fused downsample (sum/count/min/max), 2 fused downsample + last
+// mode: 0 plain decode, 1 fused downsample (sum/count/min/max), 2 fused downsample + last, 3 point-major decode,
+// 4 fused downsample + last + sumSq, 5 fused Counter downsample
 cudaError_t launch_decode(const DecodeParams &p, bool int_optimized, int mode, cudaStream_t stream);
 
+// The layout stays what it was before the tile stage's Counter and sumSq inputs: the kernel's second parameter (the
+// tensor maps) follows this one, and every other encode_kernel keeps its parameter offsets and SASS.  The tile
+// stage (IN = 2) reads no ts / val, so its window sumSq shares that first pointer, and a Counter's int64 sum / min /
+// max share the Gauge's pointers.
 struct EncodeParams {
-  const int64_t *ts;
+  union {
+    const int64_t *ts;
+    const void *tile_sum_sq;  // IN = 2, SumSq / Stdev: window-major sumSq, double (Gauge) or int64 (Counter)
+  };
   const double *val;
   uint64_t n_series;
   uint64_t points_stride;
@@ -72,11 +83,16 @@ struct EncodeParams {
   uint32_t align;
   // input stage (see encode_kernel): 0 series-major ts/val, 1 point-major ts/val, 2 Gauge aggregates
   int in_mode;
-  const double *tile_sum, *tile_min, *tile_max, *tile_last;  // window-major [points_stride][n_series]
+  // window-major [points_stride][n_series]; a Counter's (metric_type M3TSZ_METRIC_COUNTER) are int64
+  union { const double *tile_sum; const int64_t *tile_isum; };
+  union { const double *tile_min; const int64_t *tile_imin; };
+  union { const double *tile_max; const int64_t *tile_imax; };
+  const double *tile_last;
   const int64_t *tile_count;
   const int32_t *tile_src_status;  // optional [n_series]
   int64_t tile_start, tile_step;
   int agg_type;
+  int metric_type;        // M3TSZ_METRIC_COUNTER, or the Gauge (M3TSZ_METRIC_GAUGE, or 0)
   uint32_t *n_tiles_out;  // optional [n_series]
   // encoder-set append (launch_encode_append): per-series state in, updated in place; datapoints taken
   m3tsz_encoder_state *state;

@@ -1,6 +1,7 @@
 #!/usr/bin/env python3
 """Transcribes the reference's own golden vectors for the M3TSZ path into
-tests/golden/m3tsz_goldens.json.
+tests/golden/m3tsz_goldens.json, and those of the aggregator's Gauge / Counter arithmetic into
+tests/golden/m3tsz_agg_goldens.json.
 
 Run in the build container only (it reads /root/reference, which does not exist
 on the GPU box):   python scripts/make_goldens.py
@@ -17,6 +18,8 @@ import re
 REF = "/root/reference/src/dbnode/encoding"
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden",
                    "m3tsz_goldens.json")
+# the aggregator's Gauge with expensive aggregations and its Counter (tests/agg_oracle_lib.py)
+OUT_AGG = os.path.join(os.path.dirname(OUT), "m3tsz_agg_goldens.json")
 
 SEC = 1_000_000_000
 MS = 1_000_000
@@ -402,10 +405,43 @@ def main():
         ],
     }
 
+    # ---- the expensive aggregations and the Counter: src/aggregator/aggregation/{gauge,counter,common}_test.go ----
+    # (a file of their own, tests/golden/m3tsz_agg_goldens.json, bound by tests/agg_oracle_lib.py).  value_of maps
+    # aggregation.Type ids to the expected ValueOf; "stdev" entries hold [expected, delta] (require.InDelta)
+    hundred = [float(i) for i in range(1, 101)]
+    agg = {
+        "src": "aggregator/aggregation/gauge_test.go:59-75,108-170, counter_test.go:33-43,54-87, "
+               "common_test.go:31-33",
+        "gauge": [
+            {"name": "1..100 expensive", "src_line": "gauge_test.go:108-147", "times": list(range(100)),
+             "values": hundred,
+             "value_of": {"1": 100.0, "2": 1.0, "3": 100.0, "4": 50.5, "6": 100.0, "7": 5050.0, "8": 338350.0},
+             "stdev": [29.01149, 0.001]},
+            {"name": "empty expensive", "src_line": "gauge_test.go:149-170", "times": [], "values": [],
+             "value_of": {"1": 0.0, "2": "NaN", "3": "NaN", "4": 0.0, "6": 0.0, "7": 0.0, "8": 0.0},
+             "stdev": [0.0, 0.0]},
+            {"name": "1,2,3 expensive", "src_line": "gauge_test.go:59-75", "times": [0, 1, 2],
+             "values": [1.0, 2.0, 3.0],
+             "value_of": {"1": 3.0, "2": 1.0, "3": 3.0, "4": 2.0, "6": 3.0, "8": 14.0}},
+        ],
+        "counter": [
+            {"name": "1..100 default", "src_line": "counter_test.go:33-43", "values": hundred,
+             "sum": 5050, "value_of": {"7": 5050.0, "6": 100.0, "4": 50.5}},
+            {"name": "1..100 expensive", "src_line": "counter_test.go:54-87", "values": hundred, "sum": 5050,
+             "value_of": {"2": 1.0, "3": 100.0, "4": 50.5, "6": 100.0, "7": 5050.0, "8": 338350.0},
+             "stdev": [29.01149, 0.001], "invalid_value_of": {"1": 0.0}},
+        ],
+        "stdev": [{"src_line": "common_test.go:31-33", "count": 100, "sum_sq": 338350.0, "sum": 5050.0,
+                   "want": 29.01149, "delta": 0.001}],
+    }
+
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f, indent=1)
     print("wrote", OUT, "fixtures:", len(g["fixtures_b64"]["streams"]))
+    with open(OUT_AGG, "w") as f:
+        json.dump(agg, f, indent=1)
+    print("wrote", OUT_AGG)
 
 
 if __name__ == "__main__":
