@@ -825,6 +825,8 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   constexpr int IN_STRIDE = enc_in_stride<IN>();  // cells per tile row
   constexpr int IN_TILE_DW = IN_T * IN_STRIDE;  // one array (ts or val), one buffer
   constexpr bool BULK = enc_bulk<IN>();  // one 2-D tensor copy per array and tile where the arrays allow it
+  // the point-major batch stage checks the hot tier's slow-changing preconditions once per input tile (below)
+  constexpr bool GROUPS = IN == 1 && !APPEND;
   constexpr size_t WARP_SMEM = enc_warp_smem<IN>();
   uint8_t *wbase = reinterpret_cast<uint8_t *>(smem) + warp * WARP_SMEM;
   // in_tiles: [buffer][array (0 ts, 1 val)][row][lane]
@@ -1110,30 +1112,64 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
     hot_ok = steady && (!INT_OPT || s.is_float);
   }
   const uint64_t *in_next = in_tiles + lane;  // this lane's ts cell of the row to fetch next (value: + one tile)
-  for (uint32_t iter = 0; iter < max_pts; iter++) {  // warp-uniform (n_pts is 0 for lanes without a series)
-    const bool tile_first = (iter & (IN_T - 1)) == 0;
-    const bool tile_last = (iter & (IN_T - 1)) == IN_T - 1;
-    bool active = s.err == 0 && iter < n_pts && !(IN == 2 && sk_pf);  // (n_pts is 0 without a series)
 
-    // ---- input pipeline: request tile t+NSTAGE-1, wait for tile t ----
-    if (STAGED && tile_first) {
-      __syncwarp();  // everyone is done reading the buffer about to be overwritten (tile t-1's)
-      stage(iter / IN_T + NSTAGE - 1);
-      const uint32_t g = tile_base + iter / IN_T;  // (tile_base is 0 unless this batch is bulk-filled)
-      const uint32_t buf = g % NSTAGE;
-      if (bulk) {
-        enc_mbar_wait(mbar0 + buf * 8u, (g / NSTAGE) & 1u);  // every lane: the tile's bytes have landed
-      } else {
-        asm volatile("cp.async.commit_group;\n" ::: "memory");
-        asm volatile("cp.async.wait_group %0;\n" ::"n"(NSTAGE - 1) : "memory");
-      }
-      __syncwarp();
-      // row 0 of the tile that just landed; rows 1..IN_T-1 are fetched one datapoint ahead below
-      const uint64_t *tile = in_tiles + (buf * 2u) * IN_TILE_DW + lane;
-      t_pf = (int64_t)tile[0];
-      fb_pf = tile[IN_TILE_DW];
-      in_next = tile + IN_STRIDE;
+  // ---- input pipeline: request tile t+NSTAGE-1, wait for tile t (the one starting at row `iter`) ----
+  auto begin_tile = [&](uint32_t iter) {
+    __syncwarp();  // everyone is done reading the buffer about to be overwritten (tile t-1's)
+    stage(iter / IN_T + NSTAGE - 1);
+    const uint32_t g = tile_base + iter / IN_T;  // (tile_base is 0 unless this batch is bulk-filled)
+    const uint32_t buf = g % NSTAGE;
+    if (bulk) {
+      enc_mbar_wait(mbar0 + buf * 8u, (g / NSTAGE) & 1u);  // every lane: the tile's bytes have landed
+    } else {
+      asm volatile("cp.async.commit_group;\n" ::: "memory");
+      asm volatile("cp.async.wait_group %0;\n" ::"n"(NSTAGE - 1) : "memory");
     }
+    __syncwarp();
+    // row 0 of the tile that just landed; rows 1..IN_T-1 are fetched one datapoint ahead below
+    const uint64_t *tile = in_tiles + (buf * 2u) * IN_TILE_DW + lane;
+    t_pf = (int64_t)tile[0];
+    fb_pf = tile[IN_TILE_DW];
+    in_next = tile + IN_STRIDE;
+  };
+
+  // ---- the hot tier's code: '0' (zero DoD) [+ '1' no-update] + XOR code, one merge ----
+  // The state update is unconditional (upd) where an inactive lane is a FINISHED lane (IN 0 / 1); with IN = 2 a
+  // lane may sit out one row (an empty window) and must keep its state, and so must every lane in append mode,
+  // whose state outlives the call.
+  auto hot_commit = [&](int64_t t, uint64_t fb, bool upd, bool emit) {
+    if (upd) s.prev_time = t;
+    const uint32_t pre = INT_OPT ? 1u : 0u;  // '0' zero DoD [+ '1' no-update]
+    const int pb = INT_OPT ? 2 : 1;
+    const uint64_t x = s.prev_bits ^ fb;
+    int cl, ct;
+    lz_tz(x, cl, ct);  // (64, 0) for x == 0
+    const bool zero = !INT_OPT && (x == 0);  // int-optimised: a repeat is not a hot datapoint (fb != prev_bits)
+    const bool cont = !zero && cl >= s.plz && ct >= s.ptz;
+    const int nm = 64 - cl - ct;
+    // payload left-aligned: (x >> ptz) << (64 - plen) == x << plz, (x >> ct) << (64 - nm) == x << cl
+    const uint64_t P = shl64_clamp(x, (uint32_t)(cont ? s.plz : cl));  // (x == 0: cl = 64 shifts everything out)
+    const int plen = zero ? 0 : (cont ? 64 - s.plz - s.ptz : nm);
+    const uint32_t hdr = zero ? (pre << 1)
+                              : (cont ? ((pre << 2) | 2u)
+                                      : ((pre << 14) | (3u << 12) | ((uint32_t)cl << 6) | (uint32_t)(nm - 1)));
+    const int hb = pb + (zero ? 1 : (cont ? 2 : 14));
+    if (upd) {
+      s.plz = cl;  // PrevXOR := x
+      s.ptz = ct;
+      s.prev_bits = fb;
+    }
+    if (emit) {
+      emit_code_p(s, out_tile, lane, hdr, hb, P, plen);
+      s.n_enc++;
+    }
+  };
+
+  // one datapoint, every tier, with every per-datapoint check (the tile of row `iter` has landed)
+  auto row_active = [&](uint32_t iter) {
+    return s.err == 0 && iter < n_pts && !(IN == 2 && sk_pf);  // (n_pts is 0 without a series)
+  };
+  auto encode_row = [&](uint32_t iter, bool tile_last, bool active) {
 
     // ---- append mode: check the datapoint before any of it (annotation included) is written ----
     if constexpr (APPEND) {
@@ -1246,36 +1282,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       if (INT_OPT) hot = hot && fb != s.prev_bits;
       Tier2 c2;
       if (__all_sync(FULL_MASK, hot || !active)) {
-        // every live lane: '0' (zero DoD) [+ '1' no-update] + XOR code, one merge.  The state update is
-        // unconditional where an inactive lane is a FINISHED lane (IN 0 / 1); with IN = 2 a lane may sit
-        // out one row (an empty window) and must keep its state, and so must every lane in append mode, whose state
-        // outlives the call.
-        const bool upd = (IN != 2 && !APPEND) || active;
-        if (upd) s.prev_time = t;
-        const uint32_t pre = INT_OPT ? 1u : 0u;  // '0' zero DoD [+ '1' no-update]
-        const int pb = INT_OPT ? 2 : 1;
-        const uint64_t x = s.prev_bits ^ fb;
-        int cl, ct;
-        lz_tz(x, cl, ct);  // (64, 0) for x == 0
-        const bool zero = !INT_OPT && (x == 0);  // int-optimised: a repeat is not a hot datapoint (fb != prev_bits)
-        const bool cont = !zero && cl >= s.plz && ct >= s.ptz;
-        const int nm = 64 - cl - ct;
-        // payload left-aligned: (x >> ptz) << (64 - plen) == x << plz, (x >> ct) << (64 - nm) == x << cl
-        const uint64_t P = shl64_clamp(x, (uint32_t)(cont ? s.plz : cl));  // (x == 0: cl = 64 shifts everything out)
-        const int plen = zero ? 0 : (cont ? 64 - s.plz - s.ptz : nm);
-        const uint32_t hdr = zero ? (pre << 1)
-                                  : (cont ? ((pre << 2) | 2u)
-                                          : ((pre << 14) | (3u << 12) | ((uint32_t)cl << 6) | (uint32_t)(nm - 1)));
-        const int hb = pb + (zero ? 1 : (cont ? 2 : 14));
-        if (upd) {
-          s.plz = cl;  // PrevXOR := x
-          s.ptz = ct;
-          s.prev_bits = fb;
-        }
-        if (active) {
-          emit_code_p(s, out_tile, lane, hdr, hb, P, plen);
-          s.n_enc++;
-        }
+        hot_commit(t, fb, (IN != 2 && !APPEND) || active, active);  // every live lane
       } else if (__all_sync(FULL_MASK, tier2_candidate<INT_OPT>(s, active && room && steady, delta, fb, v, c2) ||
                                            !active)) {
         // second tier: small delta-of-delta + (float XOR | float repeat | int diff | int
@@ -1306,6 +1313,57 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
           hot_ok = steady && (!INT_OPT || s.is_float);
         }
       }
+    }
+  };
+
+  if constexpr (GROUPS) {
+    // Tile -> row.  What only changes every few rows or on the slow path is checked once per input tile, with
+    // margins for IN_T hot datapoints of at most 2 + 14 + 64 bits (3 words) each: every live lane has all IN_T rows
+    // (no lane ends inside the tile), room in its slot for them, and the hot tier's preconditions; there are no
+    // annotations.  Inside such a tile the per-datapoint vote only looks at the data.  The first datapoint that
+    // fails it, and every later row of the tile, takes encode_row with all of its checks.  A lane that is not
+    // live is finished or failed for the whole tile and votes yes, as it does in encode_row.
+    for (uint32_t row0 = 0; row0 < max_pts; row0 += IN_T) {  // warp-uniform
+      begin_tile(row0);
+      uint32_t iter = row0;
+      const bool live = s.err == 0 && row0 < n_pts;
+      const bool pre = hot_ok && row0 + IN_T <= n_pts &&
+                       s.words_out + s.k + (uint32_t)(3 * (IN_T - 1) + ENC_GUARD + 4) <= slot_words;
+      if (!p.ann_series_off && row0 + IN_T <= max_pts && __all_sync(FULL_MASK, pre || !live)) {
+        // room in the output tile for IN_T hot codes: at most 10 words past a column of <= ENC_OUT_W - ENC_GUARD
+        if (__any_sync(FULL_MASK, live && s.k > (uint32_t)(ENC_OUT_W - ENC_GUARD))) flush_out(false);
+#pragma unroll 1
+        for (; iter < row0 + IN_T; iter++) {
+          const int64_t t = t_pf;
+          const uint64_t fb = fb_pf;
+          const bool more = iter + 1 < row0 + IN_T;
+          if (more) {  // fetch the next row
+            t_pf = (int64_t)in_next[0];
+            fb_pf = in_next[IN_TILE_DW];
+            in_next += IN_STRIDE;
+          }
+          const int64_t delta = (int64_t)((uint64_t)t - (uint64_t)s.prev_time);
+          bool hot = delta == s.prev_delta;
+          if (INT_OPT) hot = hot && fb != s.prev_bits && !maybe_int(__longlong_as_double((long long)fb));
+          if (!__all_sync(FULL_MASK, hot || !live)) {  // this row and the rest of the tile: encode_row
+            t_pf = t;
+            fb_pf = fb;
+            if (more) in_next -= IN_STRIDE;
+            break;
+          }
+          hot_commit(t, fb, true, live);
+        }
+      }
+      const uint32_t row_end = min(row0 + (uint32_t)IN_T, max_pts);
+#pragma unroll 1
+      for (; iter < row_end; iter++) encode_row(iter, iter == row0 + IN_T - 1, row_active(iter));
+    }
+  } else {
+    for (uint32_t iter = 0; iter < max_pts; iter++) {  // warp-uniform (n_pts is 0 for lanes without a series)
+      const bool tile_last = (iter & (IN_T - 1)) == IN_T - 1;
+      const bool active = row_active(iter);
+      if (STAGED && (iter & (IN_T - 1)) == 0) begin_tile(iter);
+      encode_row(iter, tile_last, active);
     }
   }
   if (STAGED) asm volatile("cp.async.wait_all;\n" ::: "memory");
