@@ -68,6 +68,7 @@ enum {
   M3TSZ_ERR_OUT_OF_ORDER = 13,     /* errOutOfOrderIterator, encoding/iterators.go:229-236 */
   M3TSZ_ERR_TOO_MANY_ITERATORS = 14, /* > 12 replicas per series or readers per block slice */
   M3TSZ_ERR_CHECKSUM_MISMATCH = 15, /* errSeekChecksumMismatch, persist/fs/seek.go:50-51, read.go:395-397 */
+  M3TSZ_ERR_TOO_MANY_ENCODERS = 16, /* errTooManyEncoders, storage/series/buffer.go:57 */
   /* library-level conditions */
   M3TSZ_ERR_CAPACITY = 100,        /* more datapoints / bytes than the caller's buffer holds */
   M3TSZ_ERR_INVALID_ARG = 101,
@@ -320,6 +321,42 @@ int m3tsz_encoder_set_append(m3tsz_ctx *ctx, const m3tsz_options *opts, m3tsz_en
  * m3tsz_compact_streams (slot_stride = buf_stride). */
 int m3tsz_encoder_set_stream(m3tsz_ctx *ctx, const m3tsz_encoder_state *d_state, uint64_t n_series,
                              uint8_t *d_buf, uint64_t buf_stride, uint64_t *d_len, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Buffer buckets: BufferBucket.write (src/dbnode/storage/series/buffer.go:1261-1364) for n_series buckets per call.
+ * A bucket holds up to n_encoders (K, 1..M3TSZ_MAX_BUCKET_ENCODERS) in-order encoders; K plays the role of
+ * EncodersPerBlockLimit.  Encoder 0 of series s is record s of an encoder set (d_state / d_buf, reset with
+ * m3tsz_encoder_set_reset; append / stream keep working on it).  Encoders 1..K-1 are opened on demand from an
+ * overflow pool: d_pool_state [pool_capacity] + d_pool_buf [pool_capacity][pool_stride], *d_pool_count records in
+ * use, and d_table [n_series][K-1] (int32) naming the pool record of encoder i + 1 (-1: not open).  Resetting the
+ * pool is *d_pool_count = 0 and d_table = -1; all of it holds positions, not pointers, so growing is a copy.  With
+ * K = 1 the pool arguments may be NULL / 0.
+ *
+ * The datapoints of one call are processed in call order, one write each: the first encoder whose last write is
+ * before the datapoint takes it; a datapoint equal to an encoder's last write (timestamp, LastEncoded().Value --
+ * the scaled int in int-optimised mode, 0 without it -- and the checksum of the last annotation written) is a
+ * no-op; otherwise a new encoder is opened (start = encoder 0's start_ns), or the write fails with
+ * M3TSZ_ERR_TOO_MANY_ENCODERS when K are open.  A t == 0 datapoint on an empty encoder 0 fails with
+ * M3TSZ_ERR_NO_DATAPOINTS (LastEncoded errors); DOD_OVERFLOW / UNRECOGNIZED_UNIT are decided against the target
+ * encoder.  A failed write changes nothing and later datapoints of the call go on.
+ *
+ * Inputs as m3tsz_encoder_set_append.  d_result (int8, the inputs' layout): 0 written, -1 unchanged, else the
+ * failed write's status (3, 4, 6, 16, or 100 = M3TSZ_ERR_CAPACITY).  d_status[s]: M3TSZ_OK; M3TSZ_ERR_CAPACITY when
+ * the target's slot lacks room for the datapoint (the bound of m3tsz_encoder_set_append, with every earlier
+ * datapoint of the call counted at its worst case: a slot of m3tsz_encode_bound_units(P, 1) bytes takes P) or no
+ * pool record is free -- that datapoint and every later one of the series get CAPACITY and nothing of them is
+ * written, so growing and re-sending exactly those gives the unstopped result; or M3TSZ_ERR_INVALID_ARG (encoder 0
+ * reset in the other mode, or n_points > points_stride): the series is untouched and its d_result not written.
+ * ---------------------------------------------------------------------- */
+#define M3TSZ_MAX_BUCKET_ENCODERS 12
+int m3tsz_encoder_set_write(m3tsz_ctx *ctx, const m3tsz_options *opts, m3tsz_encoder_state *d_state, uint8_t *d_buf,
+                            uint64_t buf_stride, uint64_t n_series, m3tsz_encoder_state *d_pool_state,
+                            uint8_t *d_pool_buf, uint64_t pool_stride, uint64_t pool_capacity, uint32_t *d_pool_count,
+                            int32_t *d_table, int32_t n_encoders, const int64_t *d_ts, const double *d_val,
+                            uint64_t points_stride, const uint32_t *d_n_points, int32_t unit, const uint8_t *d_units,
+                            const uint64_t *d_ann_series_off, const m3tsz_annotation_entry *d_ann_entries,
+                            const uint8_t *d_ann_bytes, int32_t point_major_input, int8_t *d_result,
+                            int32_t *d_status, void *stream);
 
 /* ------------------------------------------------------------------------
  * Batch encode straight into ONE packed buffer (the fileset data-file layout,

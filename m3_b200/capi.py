@@ -19,6 +19,7 @@ ERR_UNRECOGNIZED_UNIT = 6
 ERR_INVALID_MULT = 7
 ERR_OUT_OF_ORDER = 13
 ERR_TOO_MANY_ITERATORS = 14
+ERR_TOO_MANY_ENCODERS = 16
 ERR_CAPACITY = 100
 ERR_INVALID_ARG = 101
 ERR_CUDA = 102
@@ -105,10 +106,11 @@ EXPORTED_SYMBOLS = [
     "m3tsz_encoder_pool_create", "m3tsz_encoder_pool_get", "m3tsz_encoder_pool_destroy",
     "m3tsz_iter_pool_create", "m3tsz_iter_pool_get", "m3tsz_iter_pool_destroy",
     "m3tsz_encoder_set_reset", "m3tsz_encoder_set_append", "m3tsz_encoder_set_stream",
-    "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex",
+    "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex", "m3tsz_encoder_set_write",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
+MAX_BUCKET_ENCODERS = 12  # M3TSZ_MAX_BUCKET_ENCODERS
 
 
 def lib():
@@ -254,6 +256,9 @@ def lib():
     L.m3tsz_encoder_set_append.restype = C.c_int
     L.m3tsz_encoder_set_append.argtypes = [vp, po, vp, u64, vp, vp, u64, vp, i32, vp, vp, vp, vp, i32, vp, u64,
                                            vp, vp, vp]
+    L.m3tsz_encoder_set_write.restype = C.c_int
+    L.m3tsz_encoder_set_write.argtypes = [vp, po, vp, vp, u64, u64, vp, vp, u64, u64, vp, vp, i32, vp, vp, u64, vp,
+                                          i32, vp, vp, vp, vp, i32, vp, vp, vp]
     L.m3tsz_encoder_set_stream.restype = C.c_int
     L.m3tsz_encoder_set_stream.argtypes = [vp, vp, u64, vp, u64, vp, vp]
     L.m3tsz_decode_downsample_ex.restype = C.c_int

@@ -280,6 +280,14 @@ class BatchCodec:
         bytes (a multiple of 16): the write path's encoders, appended to over many calls."""
         return EncoderSet(self, start, stride)
 
+    def bucket_set(self, start: torch.Tensor, stride: int, encoders=4, pool_records: Optional[int] = None,
+                   pool_stride: Optional[int] = None) -> "BucketSet":
+        """S buffer buckets (BufferBucket.write, m3tsz_encoder_set_write): encoder 0 of bucket s is an encoder set
+        of slots of `stride` bytes; up to encoders - 1 more per bucket open on demand from a pool of `pool_records`
+        (default S) records of `pool_stride` (default `stride`) bytes."""
+        return BucketSet(self, start, stride, encoders, start.numel() if pool_records is None else pool_records,
+                         stride if pool_stride is None else pool_stride)
+
     # ------------------------------------------------------------------ merge (row N1)
     def merge_series(self, ts, values, n_points, seq_status, slice_off, replica_off, series_off,
                      out_cap, start_ns=0, end_ns=0, strategy=0, point_major=False):
@@ -516,3 +524,159 @@ class EncoderSet:
         """Len(): stream bytes with the tail, 0 for an empty encoder."""
         n, bits = self._field(1), self._field(5)
         return torch.where(n > 0, (bits + 11 + 7) // 8, torch.zeros_like(bits))
+
+
+class BucketSet:
+    """Buffer buckets on the device: per series up to `encoders` (K) in-order encoders, as BufferBucket keeps them
+    (src/dbnode/storage/series/buffer.go:1261-1391).  Encoder 0 of every series is `primary` (an EncoderSet); the
+    others come from an overflow pool: `pool` uint8 [M, 128] states, `pool_buf` uint8 [M, pool_stride] slots,
+    `pool_count` int32 [1] records in use and `table` int32 [S, K-1] (the pool record of encoder i + 1, -1: not
+    open).  write() routes every datapoint as BufferBucket.write does; read() merges a bucket's encoders as a
+    reader of the open block sees them."""
+
+    def __init__(self, codec: BatchCodec, start: torch.Tensor, stride: int, encoders: int, pool_records: int,
+                 pool_stride: int):
+        assert 1 <= encoders <= capi.MAX_BUCKET_ENCODERS
+        assert pool_stride > 0 and pool_stride % 16 == 0 and pool_records > 0
+        self.codec = codec
+        self.encoders = int(encoders)
+        self.primary = EncoderSet(codec, start, stride)
+        self.n_series = self.primary.n_series
+        dev = codec.device
+        M = int(pool_records) if self.encoders > 1 else 0
+        self.pool = torch.zeros((M, capi.ENCODER_STATE_BYTES), dtype=torch.uint8, device=dev)
+        self.pool_buf = torch.zeros((M, pool_stride), dtype=torch.uint8, device=dev)
+        self.pool_count = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.table = torch.full((self.n_series, self.encoders - 1), -1, dtype=torch.int32, device=dev)
+
+    def reset(self, start: torch.Tensor):
+        """Reset(start) of every bucket: encoder 0 empty, every overflow record free."""
+        self.primary.reset(start)
+        self.pool_count.zero_()
+        self.table.fill_(-1)
+
+    def write(self, ts: torch.Tensor, values: torch.Tensor, n_points: Optional[torch.Tensor] = None,
+              units: Optional[torch.Tensor] = None, annotations=None, point_major=False, unit=capi.UNIT_S):
+        """BufferBucket.write of every datapoint, in call order per series; inputs as EncoderSet.append.  Returns
+        (result int8 in the inputs' shape: 0 written, -1 unchanged, else the failed write's status; status int32
+        [S]: OK, ERR_CAPACITY -- that datapoint and the rest of the series were not written: grow() and send them
+        again -- or ERR_INVALID_ARG)."""
+        assert ts.dtype == torch.int64 and values.dtype == torch.float64
+        assert ts.is_cuda and values.is_cuda and ts.is_contiguous() and values.is_contiguous()
+        S, P = (ts.shape[1], ts.shape[0]) if point_major else ts.shape
+        assert S == self.n_series
+        dev = self.codec.device
+        result = torch.zeros(ts.shape, dtype=torch.int8, device=dev)
+        status = torch.zeros(S, dtype=torch.int32, device=dev)
+        if P == 0:
+            return result, status
+        a_off = a_ent = a_bytes = None
+        if annotations is not None:
+            a_off, a_ent, a_bytes = annotations
+        M = self.pool.shape[0]
+        pr = self.primary
+        rc = capi.lib().m3tsz_encoder_set_write(
+            self.codec.ctx.handle, C.byref(self.codec.opts), _ptr(pr.state), _ptr(pr.buf), pr.stride, S,
+            _ptr(self.pool) if M else None, _ptr(self.pool_buf) if M else None, self.pool_stride, M,
+            _ptr(self.pool_count), _ptr(self.table) if self.encoders > 1 else None, self.encoders, _ptr(ts),
+            _ptr(values), P, _ptr(n_points), int(unit), _ptr(units), _ptr(a_off), _ptr(a_ent), _ptr(a_bytes),
+            1 if point_major else 0, _ptr(result), _ptr(status), _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_encoder_set_write")
+        return result, status
+
+    @property
+    def stride(self) -> int:
+        return self.primary.stride
+
+    @property
+    def pool_stride(self) -> int:
+        return self.pool_buf.shape[1]
+
+    def grow(self, stride: Optional[int] = None, pool_stride: Optional[int] = None,
+             pool_records: Optional[int] = None):
+        """Larger primary slots, pool slots or pool (every record keeps its position)."""
+        if stride is not None:
+            self.primary.grow(stride)
+        M, ps = self.pool.shape[0], self.pool_stride
+        M2 = M if pool_records is None or self.encoders == 1 else int(pool_records)
+        ps2 = ps if pool_stride is None else int(pool_stride)
+        assert M2 >= M and ps2 >= ps and ps2 % 16 == 0
+        if (M2, ps2) != (M, ps):
+            pool = torch.zeros((M2, capi.ENCODER_STATE_BYTES), dtype=torch.uint8, device=self.codec.device)
+            pool[:M] = self.pool
+            buf = torch.zeros((M2, ps2), dtype=torch.uint8, device=self.codec.device)
+            buf[:M, :ps] = self.pool_buf
+            self.pool, self.pool_buf = pool, buf
+
+    def open_encoders(self) -> torch.Tensor:
+        """Encoders open per bucket, int64 [S] (encoder 0 always counts)."""
+        return 1 + (self.table >= 0).sum(1)
+
+    def encoder_state(self, i: int):
+        """(state uint8 [S, 128] of encoder i of every bucket, open bool [S]); rows of buckets where encoder i is
+        not open are zero.  The public prefix (m3tsz_encoder_state) answers NumEncoded / LastEncoded /
+        LastAnnotationChecksum / Len, as EncoderSet's accessors read it."""
+        if i == 0:
+            return self.primary.state, torch.ones(self.n_series, dtype=torch.bool, device=self.codec.device)
+        rec = self.table[:, i - 1].long()
+        is_open = rec >= 0
+        st = self.pool[rec.clamp(min=0)] * is_open[:, None].to(torch.uint8)
+        return st, is_open
+
+    def num_encoded(self, i: int) -> torch.Tensor:
+        return self.encoder_state(i)[0].view(torch.int64)[:, 1]
+
+    def last_encoded(self, i: int):
+        st = self.encoder_state(i)[0]
+        return st.view(torch.int64)[:, 2], st.view(torch.float64)[:, 3]
+
+    def ann_checksum(self, i: int) -> torch.Tensor:
+        return self.encoder_state(i)[0].view(torch.int64)[:, 4]
+
+    def stream(self):
+        """Stream() of every encoder: (primary EncodeResult [S], pool EncodeResult [records in use]); pool record r
+        of bucket s is table[s, i - 1] for encoder i."""
+        used = int(self.pool_count.item())
+        dev = self.codec.device
+        pool_len = torch.zeros(used, dtype=torch.int64, device=dev)
+        if used:
+            rc = capi.lib().m3tsz_encoder_set_stream(self.codec.ctx.handle, _ptr(self.pool), used,
+                                                     _ptr(self.pool_buf), self.pool_stride, _ptr(pool_len),
+                                                     _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_encoder_set_stream")
+        pool = EncodeResult(out=self.pool_buf[:used], out_len=pool_len,
+                            status=torch.zeros(used, dtype=torch.int32, device=dev))
+        return self.primary.stream(), pool
+
+    def read(self, out_cap: int, start_ns=0, end_ns=0):
+        """What a reader of the open block sees (BufferBucket.streams, buffer.go:1366-1391, merged by a
+        MultiReaderIterator): every encoder's snapshot decoded, then merged per series -- encoder 0, then the open
+        overflow encoders by index, as readers of one block slice, equal timestamps going to the last pushed.
+        Returns merge_series' (ts [S, out_cap], values, n int32 [S], status int32 [S])."""
+        prim, pool = self.stream()
+        S, dev = self.n_series, self.codec.device
+        decs = []
+        for enc, n in ((prim, S), (pool, pool.out.shape[0])):
+            if n == 0:
+                continue
+            stride = enc.out.shape[1]
+            offs = torch.arange(n, dtype=torch.int64, device=dev) * stride
+            d = self.codec.decode(enc.out.reshape(-1), offs, out_cap, lengths=enc.out_len)
+            # an empty encoder is no stream at all (streams() skips it)
+            empty = enc.out_len == 0
+            d.n_points.masked_fill_(empty, 0)
+            d.status.masked_fill_(empty, 0)
+            decs.append(d)
+        cat = lambda f: torch.cat([getattr(d, f) for d in decs])
+        ts, vals, npts, st = cat("ts"), cat("values"), cat("n_points"), cat("status")
+        # sequences in series order: encoder 0 of s, then its open overflow records in encoder order
+        idx = torch.cat([torch.arange(S, dtype=torch.int64, device=dev)[:, None], S + self.table.long()], 1)
+        is_open = torch.cat([torch.ones((S, 1), dtype=torch.bool, device=dev), self.table >= 0], 1)
+        seq = idx[is_open]
+        counts = is_open.sum(1)
+        slice_off = torch.zeros(S + 1, dtype=torch.int64, device=dev)
+        slice_off[1:] = torch.cumsum(counts, 0)
+        ident = torch.arange(S + 1, dtype=torch.int64, device=dev)
+        return self.codec.merge_series(ts[seq].contiguous(), vals[seq].contiguous(), npts[seq].contiguous(),
+                                       st[seq].contiguous(), slice_off, ident, ident, out_cap, start_ns, end_ns,
+                                       strategy=0)

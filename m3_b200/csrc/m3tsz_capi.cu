@@ -125,6 +125,7 @@ const char *m3tsz_status_string(int st) {
     case M3TSZ_ERR_UNEXPECTED_EOF: return "unexpected EOF";
     case M3TSZ_ERR_OUT_OF_ORDER: return "values are out of order from inner iterator";
     case M3TSZ_ERR_TOO_MANY_ITERATORS: return "too many replicas / readers for one series";
+    case M3TSZ_ERR_TOO_MANY_ENCODERS: return "too many encoders per block";
     case M3TSZ_ERR_CHECKSUM_MISMATCH: return "checksum does not match expected checksum";
     case M3TSZ_ERR_CAPACITY: return "output capacity exceeded";
     case M3TSZ_ERR_INVALID_ARG: return "invalid argument";
@@ -453,6 +454,96 @@ int m3tsz_encoder_set_stream(m3tsz_ctx *ctx, const m3tsz_encoder_state *d_state,
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   CK(launch_encoder_set_stream(d_state, n_series, d_buf, buf_stride, d_len, (cudaStream_t)stream));
   ctx->launches++;
+  return M3TSZ_OK;
+}
+
+int m3tsz_encoder_set_write(m3tsz_ctx *ctx, const m3tsz_options *opts, m3tsz_encoder_state *d_state, uint8_t *d_buf,
+                            uint64_t buf_stride, uint64_t n_series, m3tsz_encoder_state *d_pool_state,
+                            uint8_t *d_pool_buf, uint64_t pool_stride, uint64_t pool_capacity, uint32_t *d_pool_count,
+                            int32_t *d_table, int32_t n_encoders, const int64_t *d_ts, const double *d_val,
+                            uint64_t points_stride, const uint32_t *d_n_points, int32_t unit, const uint8_t *d_units,
+                            const uint64_t *d_ann_series_off, const m3tsz_annotation_entry *d_ann_entries,
+                            const uint8_t *d_ann_bytes, int32_t point_major_input, int8_t *d_result,
+                            int32_t *d_status, void *stream) {
+  if (!ctx || !valid_opts(opts) || n_encoders < 1 || n_encoders > M3TSZ_MAX_BUCKET_ENCODERS)
+    return M3TSZ_ERR_INVALID_ARG;
+  if (n_series == 0) return M3TSZ_OK;
+  m3tsz_encode_extras ex;
+  memset(&ex, 0, sizeof(ex));
+  ex.point_major_input = point_major_input;
+  EncodeParams p;
+  auto bad_slots = [](const void *st, const uint8_t *buf, uint64_t stride) {
+    return !st || ((uintptr_t)st & 15u) || !buf || ((uintptr_t)buf & 15u) || (stride & 15u) || stride == 0 ||
+           stride > (1ull << 33);
+  };
+  if (!encode_params(opts, d_ts, d_val, n_series, points_stride, d_n_points, nullptr, unit, d_units,
+                     d_ann_series_off, d_ann_entries, d_ann_bytes, nullptr, d_status, &ex, p, true) ||
+      !d_result || !d_status || bad_slots(d_state, d_buf, buf_stride) || n_series >= (1ull << 31) ||
+      points_stride == 0)
+    return M3TSZ_ERR_INVALID_ARG;
+  if (n_encoders > 1 && (bad_slots(d_pool_state, d_pool_buf, pool_stride) || !d_pool_count || !d_table ||
+                         pool_capacity == 0 || pool_capacity >= (1ull << 31)))
+    return M3TSZ_ERR_INVALID_ARG;
+  if (n_encoders == 1) pool_capacity = 0;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  const cudaStream_t st = (cudaStream_t)stream;
+  void *target = nullptr, *touched = nullptr, *count = nullptr;
+  int rc;
+  if ((rc = ensure(ctx, kSlotRouteTarget, n_series * points_stride, &target))) return rc;
+  if ((rc = ensure(ctx, kSlotRouteTouched, pool_capacity * sizeof(RouteTouched), &touched))) return rc;
+  if ((rc = ensure(ctx, kSlotRouteCount, sizeof(uint32_t), &count))) return rc;
+  CK(cudaMemsetAsync(count, 0, sizeof(uint32_t), st));
+  RouteParams r;
+  memset(&r, 0, sizeof(r));
+  r.state = d_state;
+  r.n_series = n_series;
+  r.slot_words = buf_stride >> 2;
+  r.pool_state = d_pool_state;
+  r.pool_capacity = pool_capacity;
+  r.pool_slot_words = pool_stride >> 2;
+  r.pool_count = d_pool_count;
+  r.table = d_table;
+  r.n_encoders = n_encoders;
+  r.default_unit = opts->default_time_unit;
+  r.ts = d_ts;
+  r.val = d_val;
+  r.points_stride = points_stride;
+  r.n_points = d_n_points;
+  r.unit = unit;
+  r.point_major = point_major_input ? 1 : 0;
+  r.units = d_units;
+  r.ann_series_off = d_ann_series_off;
+  r.ann_entries = d_ann_entries;
+  r.ann_bytes = d_ann_bytes;
+  r.target = (uint8_t *)target;
+  r.result = d_result;
+  r.status = d_status;
+  r.touched = (RouteTouched *)touched;
+  r.n_touched = (uint32_t *)count;
+  const bool int_opt = opts->int_optimized != 0;
+  CK(launch_route(r, int_opt, st));
+  ctx->launches++;
+  // encoder 0 of every bucket over the original inputs, then the overflow records the route gave datapoints
+  p.route_target = (const uint8_t *)target;
+  p.route_n_in = n_series;
+  p.out = d_buf;
+  p.out_stride = buf_stride;
+  p.state = d_state;
+  p.status = nullptr;
+  CK(launch_encode_routed(p, int_opt, st));
+  ctx->launches++;
+  if (n_encoders > 1) {
+    const uint64_t most = n_series * (uint64_t)(n_encoders - 1);
+    p.n_series = most < pool_capacity ? most : pool_capacity;
+    p.out = d_pool_buf;
+    p.out_stride = pool_stride;
+    p.state = d_pool_state;
+    p.route_touched = (const RouteTouched *)touched;
+    p.route_n_touched = (const uint32_t *)count;
+    CK(launch_encode_routed(p, int_opt, st));
+    ctx->launches++;
+  }
   return M3TSZ_OK;
 }
 

@@ -40,6 +40,7 @@ struct Scratch {
 //   36, 37        packed slot sets, batch counter                packed encode, tiles
 //   38, 39        window last, tile encoder starts               tiles, downsample_ex (38, NULL d_last); tiles
 //   40-47         streaming handles, under handle_mu             m3tsz_stream.cu
+//   48-50         route targets, touched records, their count    encoder_set_write
 //
 // Slot 35 is unused.
 enum Slot : int {
@@ -79,7 +80,11 @@ enum Slot : int {
   kSlotIterTs = 41,
   kSlotIterVal = 42,
   kSlotIterEvents = 44,
-  kNumSlots = 48
+  // bucket writes
+  kSlotRouteTarget = 48,
+  kSlotRouteTouched = 49,
+  kSlotRouteCount = 50,
+  kNumSlots = 51
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

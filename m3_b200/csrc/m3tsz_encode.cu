@@ -50,6 +50,9 @@ constexpr int ENC_IN_T_PM = 4;
 constexpr int ENC_NSTAGE_PM = 2;
 // input stage IN: 0 series-major tiles (8 rows: one 64-byte segment per series and array), 1 point-major
 // tiles, 2 Gauge aggregates read directly (no input tiles)
+// IN = 3 (append mode only): a bucket write's share of one encoder (DESIGN.md §4.11).  Each lane reads its own
+// series' datapoints directly (the lanes of the overflow pass belong to scattered series) and takes the ones the
+// route kernel sent to its encoder.
 template <int IN>
 __host__ __device__ constexpr int enc_in_t() {
   return IN == 1 ? ENC_IN_T_PM : ENC_IN_T;
@@ -751,6 +754,212 @@ __host__ __device__ __forceinline__ uint32_t enc_snapshot_words(const m3tsz_enco
   return n;
 }
 
+// ---- bucket writes: routing (DESIGN.md §4.11) ------------------------------------------------------------------
+// What the router keeps of one encoder of a bucket during a call: lastWriteAt, what enc_check_time reads, the
+// LastEncoded value and annotation checksum as of the call's start, and an upper bound of the stream's bits.
+struct RouteEnc {
+  int64_t lw;  // lastWriteAt (buffer.go:1228-1231): 0 before the first write
+  int64_t prev_time, prev_delta;
+  double last_value;
+  uint64_t ann_cs;
+  uint64_t bits;  // >= the bits the append will have written, the first datapoint's 64-bit start included
+  uint64_t n_enc;
+  int unit;
+  int32_t rec;      // pool record, -1 for encoder 0
+  uint32_t n_call;  // datapoints of this call routed to it
+};
+
+__device__ __forceinline__ void route_enc_load(const m3tsz_encoder_state &st, RouteEnc &r, int32_t rec) {
+  const EncStateInternal &in = *reinterpret_cast<const EncStateInternal *>(st.internal);
+  r.n_enc = st.num_encoded;
+  r.lw = r.n_enc ? st.last_ts : 0;
+  r.prev_time = r.n_enc ? st.last_ts : st.start_ns;
+  r.prev_delta = in.prev_delta;
+  r.unit = (int)((in.meta >> 22) & 15u);
+  r.last_value = st.last_value;
+  r.ann_cs = st.ann_checksum;
+  r.bits = st.bits + (r.n_enc ? 0u : 64u);
+  r.rec = rec;
+  r.n_call = 0;
+}
+
+// datapoint j of series s in the inputs' layout
+__device__ __forceinline__ uint64_t route_at(const RouteParams &p, uint64_t s, uint32_t j) {
+  return p.point_major ? (uint64_t)j * p.n_series + s : s * p.points_stride + j;
+}
+
+// LastEncoded().Value of encoder `enc` after the datapoints of this call routed to it before datapoint j_end: its
+// state as of the call's start, then the encoder's own value step for each of them (the time step does not touch
+// the value state).  Only int-optimised mode needs it: without, the value is always 0.
+template <bool INT_OPT>
+__device__ __noinline__ double route_last_value(const RouteParams &p, const m3tsz_encoder_state &st, uint64_t s,
+                                                uint32_t j_end, int enc, uint32_t *tile, int lane) {
+  EncLane e;
+  uint64_t cs;
+  enc_state_load<INT_OPT>(st, e, tile, lane, cs);
+  for (uint32_t j = 0; j < j_end; j++) {
+    const uint64_t at = route_at(p, s, j);
+    if (p.target[at] != (uint8_t)enc) continue;
+    uint32_t hdr = 0;
+    int hb = 0, plen;
+    uint64_t payload;
+    encode_value<INT_OPT>(e, p.val[at], hdr, hb, payload, plen);
+    e.n_enc++;
+  }
+  return e.is_float ? __longlong_as_double((long long)e.prev_bits) : e.int_val;
+}
+
+// BufferBucket.write for every datapoint of series s in call order (buffer.go:1261-1364): the target of each
+// datapoint (p.target), its result (p.result) and the series' status; opens pool records and lists the ones that
+// take datapoints in p.touched.  `tile` is a 7-row column of shared memory for enc_state_load's leftover words.
+template <bool INT_OPT>
+__device__ __forceinline__ void route_series(const RouteParams &p, uint64_t s, uint32_t *tile, int lane) {
+  const uint32_t n = p.n_points ? p.n_points[s] : (uint32_t)p.points_stride;
+  if (n == 0) {
+    p.status[s] = M3TSZ_OK;
+    return;
+  }
+  const m3tsz_encoder_state &st0 = p.state[s];
+  if (n > p.points_stride ||
+      (reinterpret_cast<const EncStateInternal *>(st0.internal)->meta >> 48) != enc_state_tag(INT_OPT)) {
+    p.status[s] = M3TSZ_ERR_INVALID_ARG;
+    return;
+  }
+  RouteEnc r0;
+  route_enc_load(st0, r0, -1);
+  const int64_t start = st0.start_ns;
+  RouteEnc ro[M3TSZ_MAX_BUCKET_ENCODERS - 1];
+  int n_open = 0;  // encoders open, 0 until the overflow encoders are loaded (in-order traffic never needs them)
+  int32_t *row = p.table + s * (uint64_t)(p.n_encoders - 1);
+  uint64_t ann_i = 0, ann_end = 0;
+  if (p.ann_series_off) {
+    ann_i = p.ann_series_off[s];
+    ann_end = p.ann_series_off[s + 1];
+  }
+  int32_t status = M3TSZ_OK;
+  for (uint32_t j = 0; j < n; j++) {
+    const uint64_t at = route_at(p, s, j);
+    const uint8_t *a_ptr = nullptr;
+    uint32_t a_len = 0;
+    if (ann_i < ann_end && p.ann_entries[ann_i].dp_index == j) {
+      a_ptr = p.ann_bytes + p.ann_entries[ann_i].byte_offset;
+      a_len = p.ann_entries[ann_i].length;
+      ann_i++;
+    }
+    int res = M3TSZ_ERR_CAPACITY;
+    int tgt = 0xff;
+    if (status == M3TSZ_OK) {
+      const int64_t t = p.ts[at];
+      const double v = p.val[at];
+      const int u = p.units ? (int)p.units[at] : p.unit;
+      // the append's room check for this datapoint: its worst case, its annotation and a snapshot's tail
+      const uint64_t ann_words = a_len ? (a_len + 3) / 4 + 4 : 0;
+      bool have_cs = false;
+      uint64_t cs = 0;
+      auto ann_cs = [&]() {
+        if (!have_cs) cs = xxh64(a_ptr, a_len);
+        have_cs = true;
+        return cs;
+      };
+      // 0: go on with the next encoder, 1: write here, 2: unchanged, 3: LastEncoded failed
+      auto scan = [&](const RouteEnc &r, int i) {
+        if (t == r.lw) {
+          if (r.n_enc == 0) return 3;
+          double lv = r.last_value;
+          if (INT_OPT && r.n_call)
+            lv = route_last_value<INT_OPT>(p, i ? p.pool_state[r.rec] : st0, s, j, i, tile, lane);
+          return (lv == v && r.ann_cs == ann_cs()) ? 2 : 0;
+        }
+        return t > r.lw ? 1 : 0;
+      };
+      // the write's checks, made before it is committed: the encoder's time checks, then room in its slot
+      auto check = [&](const RouteEnc &r, uint64_t slot_words) {
+        EncLane e;
+        e.unit = r.unit;
+        e.prev_time = r.prev_time;
+        e.prev_delta = r.prev_delta;
+        const int err = enc_check_time(e, t, u);
+        if (err) return err;
+        return (r.bits >> 5) + ENC_GUARD + 4 + ann_words > slot_words ? (int)M3TSZ_ERR_CAPACITY : 0;
+      };
+      // encode_time's state update, and the datapoint's worst case: a unit change writes a marker and a 64-bit
+      // delta-of-delta (83 bits), else at most '1111' + 64 bits; the value at most 80 bits
+      auto commit = [&](RouteEnc &r) {
+        const int64_t delta = (int64_t)((uint64_t)t - (uint64_t)r.prev_time);
+        r.bits += (u != r.unit ? 83u : 68u) + 80u + 32u * ann_words;
+        if (u != r.unit) {
+          r.unit = u;
+          r.prev_delta = 0;
+        } else {
+          r.prev_delta = delta;
+        }
+        r.prev_time = t;
+        r.lw = t;
+        r.n_enc++;
+        r.n_call++;
+        if (a_len) r.ann_cs = ann_cs();
+      };
+      int k = scan(r0, 0), hit = k == 1 ? 0 : -1;
+      if (k == 0) {
+        if (n_open == 0) {
+          n_open = 1;
+          for (; n_open < p.n_encoders && row[n_open - 1] >= 0; n_open++)
+            route_enc_load(p.pool_state[row[n_open - 1]], ro[n_open - 1], row[n_open - 1]);
+        }
+        for (int i = 1; i < n_open && k == 0; i++) {
+          k = scan(ro[i - 1], i);
+          if (k == 1) hit = i;
+        }
+      }
+      if (k == 2) {
+        res = -1;
+      } else if (k == 3) {
+        res = M3TSZ_ERR_NO_DATAPOINTS;
+      } else if (hit == 0) {
+        res = check(r0, p.slot_words);
+        if (res == 0) commit(r0);
+      } else if (hit > 0) {
+        res = check(ro[hit - 1], p.pool_slot_words);
+        if (res == 0) commit(ro[hit - 1]);
+      } else if (n_open >= p.n_encoders) {
+        res = M3TSZ_ERR_TOO_MANY_ENCODERS;
+      } else {
+        // a new encoder: Reset(block start), opened only once its first write is known to succeed
+        RouteEnc &r = ro[n_open - 1];
+        m3tsz_encoder_state fresh;
+        enc_state_reset(fresh, start, p.default_unit, INT_OPT);
+        route_enc_load(fresh, r, -1);
+        res = check(r, p.pool_slot_words);
+        if (res == 0) {
+          const uint32_t rec = atomicAdd(p.pool_count, 1u);
+          if (rec >= p.pool_capacity) {
+            atomicSub(p.pool_count, 1u);
+            res = M3TSZ_ERR_CAPACITY;
+          } else {
+            p.pool_state[rec] = fresh;
+            row[n_open - 1] = (int32_t)rec;
+            r.rec = (int32_t)rec;
+            commit(r);
+            hit = n_open++;
+          }
+        }
+      }
+      if (res == 0) tgt = hit;
+      if (res == M3TSZ_ERR_CAPACITY) status = M3TSZ_ERR_CAPACITY;
+    }
+    p.target[at] = (uint8_t)tgt;
+    p.result[at] = (int8_t)res;
+  }
+  p.status[s] = status;
+  uint32_t n_touched = 0;
+  for (int i = 1; i < n_open; i++) n_touched += ro[i - 1].n_call ? 1u : 0u;
+  if (n_touched) {
+    uint32_t k = atomicAdd(p.n_touched, n_touched);
+    for (int i = 1; i < n_open; i++)
+      if (ro[i - 1].n_call) p.touched[k++] = RouteTouched{(uint32_t)ro[i - 1].rec, (uint32_t)s, (uint32_t)i, 0u};
+  }
+}
+
 __device__ __forceinline__ uint32_t enc_smem_addr(const void *p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -811,9 +1020,10 @@ __device__ __forceinline__ void enc_mbar_wait(uint32_t bar, uint32_t parity) {
 //   writing the tail.
 template <bool INT_OPT, bool PACKED, int IN, bool APPEND = false>
 __global__ void __launch_bounds__(ENC_WARPS * 32,
-                                  (IN == 2) ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
+                                  (IN == 2 || IN == 3) ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
     encode_kernel(const EncodeParams p, const __grid_constant__ EncTensorMaps tmaps) {
   static_assert(!APPEND || (!PACKED && IN != 2), "append mode writes its own slots from staged inputs");
+  static_assert(IN != 3 || APPEND, "the routed input stage continues open encoders");
   extern __shared__ __align__(128) uint32_t smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
@@ -857,6 +1067,10 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
     unsigned long long b = 0;
     if (lane == 0) b = atomicAdd(p.batch_counter, 1ull);
     batch = __shfl_sync(FULL_MASK, b, 0);
+  } else if (IN == 3) {
+    // grid-stride: the overflow pass launches a bounded grid over as many lanes as records could have been touched,
+    // and a warp stops at its first batch past the touched ones (below)
+    batch = warp_slot + batch_iter * ((uint64_t)gridDim.x * ENC_WARPS);
   } else {
     if (batch_iter) break;
     batch = warp_slot;
@@ -864,7 +1078,19 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   if (batch >= n_batches) break;
   const uint64_t warp_s0 = batch * 32ull;
   const uint64_t sidx = warp_s0 + lane;
-  const bool valid = sidx < p.n_series;
+  const bool valid = sidx < p.n_series && (IN != 3 || !p.route_touched || sidx < *p.route_n_touched);
+  // the lane's input series and encoder record, and (IN = 3) the encoder index whose datapoints it takes
+  uint64_t in_s = sidx, rec = sidx;
+  uint32_t lane_enc = 0;
+  if constexpr (IN == 3) {
+    if (p.route_touched && !__any_sync(FULL_MASK, valid)) break;  // (overflow pass: past the touched records)
+    if (p.route_touched && valid) {
+      const RouteTouched e = p.route_touched[sidx];
+      rec = e.rec;
+      in_s = e.series;
+      lane_enc = e.enc;
+    }
+  }
 
   EncLane s;
   s.carry = 0;
@@ -895,14 +1121,14 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   std::conditional_t<APPEND, EncAppendVars, EncNoVars> av;
   if constexpr (APPEND) {
     if (valid) {
-      n_pts = p.n_points ? p.n_points[sidx] : (uint32_t)p.points_stride;
+      n_pts = p.n_points ? p.n_points[in_s] : (uint32_t)p.points_stride;
       if (n_pts > p.points_stride) s.err = M3TSZ_ERR_INVALID_ARG;
       if (p.ann_series_off) {
-        ann_i = p.ann_series_off[sidx];
-        ann_end = p.ann_series_off[sidx + 1];
+        ann_i = p.ann_series_off[in_s];
+        ann_end = p.ann_series_off[in_s + 1];
       }
       // a series without datapoints (or with bad arguments) loads nothing and keeps its state and slot
-      if (n_pts > 0 && s.err == 0) s.err = enc_state_load<INT_OPT>(p.state[sidx], s, out_tile, lane, av.ann_cs);
+      if (n_pts > 0 && s.err == 0) s.err = enc_state_load<INT_OPT>(p.state[rec], s, out_tile, lane, av.ann_cs);
       if (s.err) n_pts = 0;
       av.n_enc0 = s.n_enc;
       if (n_pts > 0 && s.n_enc == 0) put64(s, out_tile, lane, (uint64_t)s.prev_time, 64);  // WriteFirstTime :89-102
@@ -942,10 +1168,12 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   // banks (4q + i + column) % 32 are distinct.  The sectors are whole in memory when out_stride is a multiple of 32
   // bytes, as the bench's is.
   uint8_t *my_out = PACKED ? p.out + (warp_slot * 32ull + (uint64_t)lane) * p.out_stride
-                           : p.out + sidx * p.out_stride;
+                           : p.out + rec * p.out_stride;
   const uint32_t par = (lane >> 2) & 1u;  // 0: this lane's column is its pair's column A, 1: column B
-  // the partner's slot (lane l ^ 4 is 4 slots away in both output modes)
+  // the partner's slot (lane l ^ 4 is 4 slots away in both output modes; the overflow records of IN = 3 lie anywhere)
   uint8_t *o_out = par ? my_out - 4ull * p.out_stride : my_out + 4ull * p.out_stride;
+  if constexpr (IN == 3)
+    o_out = reinterpret_cast<uint8_t *>(__shfl_xor_sync(FULL_MASK, reinterpret_cast<unsigned long long>(my_out), 4));
   auto flush_out = [&](bool last) {
     __syncwarp();
     const uint32_t grp = last ? s.k >> 2 : (s.k >> 3) << 1;  // 16-byte groups of this lane's column (<= 7)
@@ -1054,6 +1282,12 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
     t_o = 0;
     v_o = 0;
     if (!valid || row >= n_pts) return;
+    if constexpr (IN == 3) {  // the inputs' own layout (in_mode 1: point-major)
+      const uint64_t o = p.in_mode ? (uint64_t)row * p.route_n_in + in_s : in_s * p.points_stride + row;
+      t_o = __ldg(p.ts + o);
+      v_o = (uint64_t)__double_as_longlong(__ldg(p.val + o));
+      return;
+    }
     const uint64_t o = (uint64_t)row * p.n_series + sidx;
     if (IN == 2) {
       const int64_t c = __ldg(p.tile_count + o);
@@ -1173,8 +1407,15 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
 
     // ---- append mode: check the datapoint before any of it (annotation included) is written ----
     if constexpr (APPEND) {
+      if constexpr (IN == 3) {
+        // only the datapoints routed to this lane's encoder; the annotations of the others are passed over
+        if (active) active = p.route_target[p.in_mode ? (uint64_t)iter * p.route_n_in + in_s
+                                                      : in_s * p.points_stride + iter] == lane_enc;
+        if (p.ann_series_off)
+          while (ann_i < ann_end && p.ann_entries[ann_i].dp_index < iter) ann_i++;
+      }
       if (active) {
-        const int u = p.units ? (int)p.units[sidx * p.points_stride + iter] : p.unit;
+        const int u = p.units ? (int)p.units[in_s * p.points_stride + iter] : p.unit;
         // room for the datapoint's worst case, its annotation (marker + varint + bytes) and a snapshot's tail
         uint64_t need = (uint64_t)s.words_out + s.k + ENC_GUARD + 4;
         if (p.ann_series_off && ann_i < ann_end) {
@@ -1297,7 +1538,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
         if (!room) {
           s.err = M3TSZ_ERR_CAPACITY;
         } else {
-          const int u = p.units ? (int)p.units[sidx * p.points_stride + iter] : p.unit;
+          const int u = p.units ? (int)p.units[in_s * p.points_stride + iter] : p.unit;
           uint32_t hdr;
           int hb;
           encode_time(s, out_tile, lane, t, u, hdr, hb);
@@ -1373,9 +1614,15 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
     // ---- whole sectors to the slot, the rest (<= 7 words + the partial word) into the state ----
     flush_out(false);
     if (valid) {
-      if (s.n_enc != av.n_enc0) enc_state_save<INT_OPT>(p.state[sidx], s, out_tile, lane, av.ann_cs);
-      p.n_appended[sidx] = s.n_enc - av.n_enc0;
-      p.status[sidx] = s.err;
+      if (s.n_enc != av.n_enc0) enc_state_save<INT_OPT>(p.state[rec], s, out_tile, lane, av.ann_cs);
+      // A routed lane reports nothing: route_series already gave every datapoint its result, and its room bound
+      // (each earlier datapoint of the call at its worst case) implies the check above, as its time checks are
+      // encode_time's, so s.err stays 0 here.  A change to either check must keep that implication;
+      // tests/test_device_route_on_host.py asserts it for every routed datapoint.
+      if (IN != 3) {
+        p.n_appended[sidx] = s.n_enc - av.n_enc0;
+        p.status[sidx] = s.err;
+      }
     }
     continue;  // (one batch per warp)
   }
@@ -1546,6 +1793,12 @@ static cudaError_t launch_encode_one(const EncodeParams &p, cudaStream_t stream)
   uint64_t blocks = (p.n_series + per_block - 1) / per_block;
   if (blocks == 0) return cudaSuccess;
   if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
+  if (IN == 3 && p.route_touched) {  // the overflow pass: a grid-stride loop over a grid of a few blocks per SM
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev))
+      return cudaErrorInvalidValue;
+    if (blocks > 8ull * (uint64_t)sms) blocks = 8ull * (uint64_t)sms;
+  }
   cudaError_t e = cudaFuncSetAttribute(encode_kernel<INT_OPT, PACKED, IN, APPEND>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
@@ -1558,7 +1811,10 @@ static cudaError_t launch_encode_one(const EncodeParams &p, cudaStream_t stream)
     if (blocks > resident) blocks = resident;
   }
   EncTensorMaps tm;
-  enc_build_tensor_maps(p, tm);  // (ok = 0 for the other input stages)
+  if (IN == 3)
+    memset(&tm, 0, sizeof(tm));  // (in_mode names the routed stage's input layout; it reads no tiles)
+  else
+    enc_build_tensor_maps(p, tm);  // (ok = 0 for the other input stages)
   encode_kernel<INT_OPT, PACKED, IN, APPEND><<<(unsigned)blocks, ENC_WARPS * 32, smem, stream>>>(p, tm);
   return cudaGetLastError();
 }
@@ -1621,6 +1877,32 @@ cudaError_t launch_encode_append(const EncodeParams &p, bool int_optimized, cuda
                          : launch_encode_one<false, false, 1, true>(p, stream);
   return int_optimized ? launch_encode_one<true, false, 0, true>(p, stream)
                        : launch_encode_one<false, false, 0, true>(p, stream);
+}
+
+cudaError_t launch_encode_routed(const EncodeParams &p, bool int_optimized, cudaStream_t stream) {
+  return int_optimized ? launch_encode_one<true, false, 3, true>(p, stream)
+                       : launch_encode_one<false, false, 3, true>(p, stream);
+}
+
+// one thread per bucket (route_series); a 7-row tile column per lane for enc_state_load's leftover words
+constexpr int ROUTE_THREADS = 128;
+template <bool INT_OPT>
+__global__ void __launch_bounds__(ROUTE_THREADS) route_kernel(const RouteParams p) {
+  __shared__ uint32_t tile[ROUTE_THREADS / 32][7 * ENC_STRIDE];
+  const uint64_t s = (uint64_t)blockIdx.x * ROUTE_THREADS + threadIdx.x;
+  if (s >= p.n_series) return;
+  route_series<INT_OPT>(p, s, tile[threadIdx.x >> 5], threadIdx.x & 31);
+}
+
+cudaError_t launch_route(const RouteParams &p, bool int_optimized, cudaStream_t stream) {
+  const uint64_t blocks = (p.n_series + ROUTE_THREADS - 1) / ROUTE_THREADS;
+  if (blocks == 0) return cudaSuccess;
+  if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
+  if (int_optimized)
+    route_kernel<true><<<(unsigned)blocks, ROUTE_THREADS, 0, stream>>>(p);
+  else
+    route_kernel<false><<<(unsigned)blocks, ROUTE_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
 }
 
 __global__ void encoder_set_reset_kernel(m3tsz_encoder_state *state, uint64_t n, const int64_t *start,

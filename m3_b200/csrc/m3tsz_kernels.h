@@ -87,10 +87,14 @@ struct EncodeParams {
   union { const double *tile_sum; const int64_t *tile_isum; };
   union { const double *tile_min; const int64_t *tile_imin; };
   union { const double *tile_max; const int64_t *tile_imax; };
-  const double *tile_last;
-  const int64_t *tile_count;
-  const int32_t *tile_src_status;  // optional [n_series]
-  int64_t tile_start, tile_step;
+  // bucket writes (launch_encode_routed, IN = 3) share the tile stage's fields: the target encoder of every
+  // datapoint, in the inputs' layout; lane j of the overflow pass continues record route_touched[j].rec (NULL: the
+  // primary pass, lane s continues encoder 0 of series s); route_n_in is the number of input series
+  union { const double *tile_last; const uint8_t *route_target; };
+  union { const int64_t *tile_count; const struct RouteTouched *route_touched; };
+  union { const int32_t *tile_src_status; const uint32_t *route_n_touched; };  // tile_src_status: optional [n_series]
+  union { int64_t tile_start; uint64_t route_n_in; };
+  int64_t tile_step;
   int agg_type;
   int metric_type;        // M3TSZ_METRIC_COUNTER, or the Gauge (M3TSZ_METRIC_GAUGE, or 0)
   uint32_t *n_tiles_out;  // optional [n_series]
@@ -99,6 +103,41 @@ struct EncodeParams {
   uint32_t *n_appended;
 };
 
+// an overflow record that a bucket write gave datapoints: pool record, its series, its encoder index (1..K-1)
+struct RouteTouched {
+  uint32_t rec, series, enc, reserved;
+};
+
+// what the route kernel reads and writes (launch_route, m3tsz_encode.cu)
+struct RouteParams {
+  m3tsz_encoder_state *state;  // [n_series]: encoder 0 of every bucket
+  uint64_t n_series;
+  uint64_t slot_words;  // words per primary slot
+  m3tsz_encoder_state *pool_state;  // [pool_capacity]: encoders 1..K-1
+  uint64_t pool_capacity;
+  uint64_t pool_slot_words;
+  uint32_t *pool_count;  // records in use
+  int32_t *table;        // [n_series][K - 1] pool record of encoder i + 1, -1 = not open
+  int n_encoders;        // K
+  int default_unit;
+  const int64_t *ts;
+  const double *val;
+  uint64_t points_stride;
+  const uint32_t *n_points;
+  int unit;
+  int point_major;
+  const uint8_t *units;
+  const uint64_t *ann_series_off;
+  const m3tsz_annotation_entry *ann_entries;
+  const uint8_t *ann_bytes;
+  uint8_t *target;  // per datapoint: encoder index, 0xff = not written
+  int8_t *result;
+  int32_t *status;
+  RouteTouched *touched;  // [pool_capacity]
+  uint32_t *n_touched;
+};
+static_assert(sizeof(EncodeParams) == 288, "the tensor maps follow EncodeParams: its size fixes their offset");
+
 uint64_t encode_packed_resident_blocks();
 // encoder sets (m3tsz_encode.cu): append runs encode_kernel's append mode over p.state / p.out (the slots)
 cudaError_t launch_encode_append(const EncodeParams &p, bool int_optimized, cudaStream_t stream);
@@ -106,6 +145,10 @@ cudaError_t launch_encoder_set_reset(m3tsz_encoder_state *state, uint64_t n, con
                                      bool int_optimized, cudaStream_t stream);
 cudaError_t launch_encoder_set_stream(const m3tsz_encoder_state *state, uint64_t n, uint8_t *buf, uint64_t stride,
                                       uint64_t *len, cudaStream_t stream);
+// bucket writes: route every datapoint to an encoder of its bucket, then append each encoder's share (encode_kernel's
+// routed mode, once over the primary set and once over the overflow records the route touched)
+cudaError_t launch_route(const RouteParams &p, bool int_optimized, cudaStream_t stream);
+cudaError_t launch_encode_routed(const EncodeParams &p, bool int_optimized, cudaStream_t stream);
 uint64_t encode_packed_scratch_slots(uint64_t n_series);  // slots of out_stride bytes the packed mode needs
 cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_t stream);
 

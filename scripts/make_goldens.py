@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """Transcribes the reference's own golden vectors for the M3TSZ path into
-tests/golden/m3tsz_goldens.json, and those of the aggregator's Gauge / Counter arithmetic into
-tests/golden/m3tsz_agg_goldens.json.
+tests/golden/m3tsz_goldens.json, those of the aggregator's Gauge / Counter arithmetic into
+tests/golden/m3tsz_agg_goldens.json, and the buffer bucket's write tables into
+tests/golden/m3tsz_buffer_goldens.json.
 
 Run in the build container only (it reads /root/reference, which does not exist
 on the GPU box):   python scripts/make_goldens.py
@@ -20,6 +21,8 @@ OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "g
                    "m3tsz_goldens.json")
 # the aggregator's Gauge with expensive aggregations and its Counter (tests/agg_oracle_lib.py)
 OUT_AGG = os.path.join(os.path.dirname(OUT), "m3tsz_agg_goldens.json")
+# BufferBucket.write (storage/series/buffer.go:1261-1364): the write tables of storage/series/buffer_test.go
+OUT_BUFFER = os.path.join(os.path.dirname(OUT), "m3tsz_buffer_goldens.json")
 
 SEC = 1_000_000_000
 MS = 1_000_000
@@ -435,6 +438,55 @@ def main():
                    "want": 29.01149, "delta": 0.001}],
     }
 
+    # ---- buffer buckets: storage/series/buffer_test.go (the bucket writes, m3tsz_encoder_set_write) ----
+    # Every case is one bucket at a block start; each write is (offset from the block start in ns, value, unit) with
+    # the reference's wasWritten and error.  "read" is what the reference asserts a reader of the bucket sees,
+    # (offset, value) in time order; "encoders" the number of in-order encoders it asserts, where it does.
+    # TestEncoderLimit asserts no read: its "read" is its successful writes in time order (the offsets are
+    # distinct).  Its limit 0 means no limit.
+    def limit_case(desc, limit, writes):
+        ws = [{"offset_ns": off * MS, "value": float(i), "unit": MSU, "written": not tm,
+               "error": "too many encoders per block" if tm else None} for i, (off, tm) in enumerate(writes)]
+        read = sorted((w["offset_ns"], w["value"]) for w in ws if w["written"])
+        return {"name": "TestEncoderLimit/" + desc, "src_line": "buffer_test.go:2022-2255", "limit": limit,
+                "writes": ws, "read": [list(r) for r in read]}
+
+    def sec_writes(rows):
+        return [{"offset_ns": off * SEC, "value": float(v), "unit": S, "written": w, "error": None}
+                for off, v, w in rows]
+
+    buffer = {
+        "src": "dbnode/storage/series/buffer_test.go",
+        "cases": [
+            {"name": "TestBufferWriteOutOfOrder", "src_line": "buffer_test.go:337-381", "limit": 0,
+             "writes": sec_writes([(0, 1, True), (10, 2, True), (5, 3, True)]), "encoders": 2,
+             "last_encoded_offsets_ns": [10 * SEC, 5 * SEC],
+             "read": [[0, 1.0], [5 * SEC, 3.0], [10 * SEC, 2.0]]},
+            {"name": "TestBufferBucketWriteDuplicateUpserts", "src_line": "buffer_test.go:574-638", "limit": 0,
+             "writes": sec_writes([(0, 1, True), (10, 2, True), (50, 3, True), (50, 4, True),
+                                   (10, 5, True), (40, 6, True), (60, 7, True),
+                                   (40, 8, True), (70, 9, True),
+                                   (10, 10, True), (80, 11, True)]),
+             "read": [[0, 1.0], [10 * SEC, 10.0], [40 * SEC, 8.0], [50 * SEC, 4.0], [60 * SEC, 7.0],
+                      [70 * SEC, 9.0], [80 * SEC, 11.0]]},
+            {"name": "TestBufferBucketDuplicatePointsNotWrittenButUpserted", "src_line": "buffer_test.go:640-709",
+             "limit": 0,
+             "writes": sec_writes([(0, 1, True), (0, 1, False), (0, 1, False), (0, 1, False), (10, 2, True),
+                                   (0, 1, True), (10, 2, False), (10, 5, True),
+                                   (0, 1, True), (20, 8, True),
+                                   (0, 10, True), (20, 10, True)]),
+             "read": [[0, 10.0], [10 * SEC, 5.0], [20 * SEC, 10.0]]},
+            limit_case("one encoder, no limit", 0, [(1, False), (2, False), (3, False), (4, False)]),
+            limit_case("many encoders, no limit", 0, [(o, False) for o in range(9, 1, -1)]),
+            limit_case("within limit", 3, [(3, False), (2, False), (1, False)]),
+            limit_case("within limit, many writes", 2,
+                       [(10, False), (11, False), (12, False), (1, False), (2, False), (13, False), (3, False)]),
+            limit_case("too many encoders", 3, [(5, False), (4, False), (3, False), (2, True)]),
+            limit_case("too many encoders, more writes", 2,
+                       [(10, False), (2, False), (3, False), (11, False), (1, True), (4, False)]),
+        ],
+    }
+
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f, indent=1)
@@ -442,6 +494,9 @@ def main():
     with open(OUT_AGG, "w") as f:
         json.dump(agg, f, indent=1)
     print("wrote", OUT_AGG)
+    with open(OUT_BUFFER, "w") as f:
+        json.dump(buffer, f, indent=1)
+    print("wrote", OUT_BUFFER)
 
 
 if __name__ == "__main__":
