@@ -599,6 +599,9 @@ int m3tsz_fetch_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
  *     sum, stamped with the window's last datapoint, :84-98,113-118.
  * Inputs [n_series][cap] + d_n_points; outputs [n_series][out_cap] + d_n_out (the
  * number of samples; > out_cap => d_status M3TSZ_ERR_CAPACITY, first out_cap stored).
+ * A series with d_n_points[s] > cap (a decode or merge row that hit its capacity) is
+ * refused: d_status M3TSZ_ERR_INVALID_ARG, d_n_out 0, nothing of its input row read and
+ * nothing of its output row written; the other series are converted as usual.
  * d_handle_resets and d_status may be NULL.  In-place (outputs == inputs, out_cap ==
  * cap) is allowed.
  * ---------------------------------------------------------------------- */

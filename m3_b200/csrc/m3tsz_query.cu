@@ -17,6 +17,15 @@ namespace m3tsz {
 // ---------------------------------------------------------------------------
 // Prometheus epilogue
 // ---------------------------------------------------------------------------
+// A count larger than the row (decode or merge output that hit its capacity) is refused like the
+// encoder refuses it: nothing of the row is read, nothing of the output row is written, n_out = 0 and
+// INVALID_ARG.  Converting only the stored prefix would hand back e.g. a counter's cumulative sum over
+// part of its datapoints with status OK.
+__device__ __forceinline__ void prom_refuse_row(const PromParams &p, uint64_t s) {
+  p.n_out[s] = 0;
+  if (p.status) p.status[s] = M3TSZ_ERR_INVALID_ARG;
+}
+
 // Plain conversion (no tolerance, no counter normalisation): every datapoint is
 // independent -- one warp per series, lanes stride over the datapoints (coalesced).
 __global__ void prom_simple_kernel(const PromParams p) {
@@ -24,6 +33,10 @@ __global__ void prom_simple_kernel(const PromParams p) {
   const int lane = threadIdx.x & 31;
   if (w >= p.n_series) return;
   const uint32_t n = p.n_points[w];
+  if (n > p.cap) {
+    if (lane == 0) prom_refuse_row(p, w);
+    return;
+  }
   const uint32_t m = n < p.out_cap ? n : (uint32_t)p.out_cap;
   const int64_t *ts = p.ts + w * p.cap;
   const double *val = p.val + w * p.cap;
@@ -45,6 +58,10 @@ __global__ void prom_general_kernel(const PromParams p) {
   const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= p.n_series) return;
   const uint32_t n = p.n_points[s];
+  if (n > p.cap) {
+    prom_refuse_row(p, s);
+    return;
+  }
   const int64_t *ts = p.ts + s * p.cap;
   const double *val = p.val + s * p.cap;
   int64_t *to = p.ts_out + s * p.out_cap;

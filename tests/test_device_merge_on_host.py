@@ -142,6 +142,34 @@ def test_merge_kernels_on_host_match_oracle(dev, seed, strategy):
         assert fast_total > 0  # the register-resident fast kernel handled part of the batch itself
 
 
+@pytest.mark.parametrize("seed", range(3))
+@pytest.mark.parametrize("strategy", [0, 1, 2, 3])
+def test_merge_kernels_on_host_special_values(dev, seed, strategy):
+    """the special-value batches of test_independent_merge (NaN payloads, +-Inf, +-0 at equal timestamps, 1-12
+    replicas, 1-4 readers per slice; and 1-4 replicas of single-reader slices, the fast kernel's shape), filter on
+    and off, both layouts: every value bit for bit against the oracle"""
+    from test_merge_oracle import build
+    rng = np.random.default_rng(1300 + seed * 5 + strategy)
+    series = M.special_value_series(rng, 60) + M.special_value_series(rng, 60, replicas=(1, 4), readers=(1, 1))
+    ts, vals, npts, st, slice_off, replica_off, series_off = build(series)
+    fast_total = 0
+    for start, end in ((0, 0), M.SPECIAL_RANGE):
+        o_ts, o_val, o_n, o_st = O.series_merge_batch(ts, vals, npts, st, slice_off, replica_off, series_off,
+                                                      start=start, end=end, strategy=strategy,
+                                                      out_cap=max(1, int(npts.sum())))
+        for point_major in (False, True):
+            d_ts, d_val, d_n, d_st, n_fast = _run(dev, ts, vals, npts, st, slice_off, replica_off, series_off,
+                                                  start, end, strategy, point_major)
+            assert (d_st == o_st).all() and (d_n == o_n).all()
+            for s in range(len(series)):
+                k = int(o_n[s])
+                assert (d_ts[s, :k] == o_ts[s, :k]).all(), s
+                assert (d_val[s, :k].view(np.uint64) == o_val[s, :k].view(np.uint64)).all(), s
+            fast_total += n_fast
+    if strategy == 0:
+        assert fast_total > 0
+
+
 def test_merge_kernels_on_host_rf3_fetch_shape(dev):
     """the shape a fetch normally has (and the bench measures): 3 replicas x 1 block x 1 reader, identical
     timestamps, replica values that differ now and then -- all of it on the fast kernel"""

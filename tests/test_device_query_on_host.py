@@ -2,7 +2,7 @@
 `prom_general_kernel`, one thread per series) compiled for the host from the CUDA source and run thread by thread
 the way `launch_prom` picks and shapes them; compared with the oracle's iteratorToPromResult restatement and the
 independent Python one (tests/test_independent_query_rows.py) on random batches: counters with resets, tolerance
-clamps, NaN, empty series, output capacity overflow."""
+clamps, NaN, empty series, output capacity overflow, and rows whose count exceeds their capacity (refused unread)."""
 import ctypes as C
 import os
 import subprocess
@@ -114,22 +114,65 @@ def test_prom_kernels_on_host_match_oracle_and_model(dev, mode):
     if mode in ("resets", "both", "small_cap"):
         handle = (rng.random(S) < 0.6).astype(np.uint8)
     out_cap = cap + 1 if mode != "small_cap" else 20
-    t_out = np.zeros((S, out_cap), dtype=np.int64)
-    v_out = np.zeros((S, out_cap), dtype=np.float64)
-    n_out = np.zeros(S, dtype=np.uint32)
-    st = np.zeros(S, dtype=np.int32)
+    t_out, v_out, n_out, st, was_simple = _convert(dev, ts, vals, n, S, cap, resolution, handle, tol, until, out_cap)
+    assert was_simple == (1 if mode == "simple" else 0)
+    for s in range(S):
+        _assert_series(ts, vals, n, s, resolution, handle, tol, until, out_cap, t_out, v_out, n_out, st)
+
+
+T_FILL, V_FILL = -777, np.uint64(0x7FF4DEADBEEF0001)  # output prefill: an int and a NaN bit pattern nobody computes
+
+
+def _convert(dev, ts, vals, n, S, cap, resolution, handle, tol, until, out_cap):
+    """runs the epilogue over the first S rows of ts / vals (which may have more rows) into prefilled outputs"""
+    t_out = np.full((S, out_cap), T_FILL, dtype=np.int64)
+    v_out = np.full((S, out_cap), V_FILL, dtype=np.uint64).view(np.float64)
+    n_out = np.full(S, 12345, dtype=np.uint32)
+    st = np.full(S, -1, dtype=np.int32)
     p = lambda a: C.c_void_p(a.ctypes.data)
     was_simple = dev.dev_prom(p(ts), p(vals), C.c_uint64(cap), p(n), C.c_uint64(S), C.c_int64(resolution),
                               None if handle is None else p(handle), C.c_double(tol), C.c_int64(until), p(t_out),
                               p(v_out), C.c_uint64(out_cap), p(n_out), p(st))
+    return t_out, v_out, n_out, st, was_simple
+
+
+def _assert_series(ts, vals, n, s, resolution, handle, tol, until, out_cap, t_out, v_out, n_out, st):
+    """series s equals the oracle's and the independent model's conversion of its n[s] datapoints"""
+    k = int(n[s])
+    h = bool(handle[s]) if handle is not None else False
+    o_ts, o_v = O.prom_convert_series(ts[s, :k], vals[s, :k], resolution, h, tol, until)
+    ref = prom_convert(ts[s, :k].tolist(), vals[s, :k].tolist(), resolution, h, tol, until)
+    assert len(ref) == len(o_ts) == int(n_out[s]), (s, len(ref), len(o_ts), int(n_out[s]))
+    assert int(st[s]) == (100 if len(ref) > out_cap else 0), s  # M3TSZ_ERR_CAPACITY
+    m = min(len(ref), out_cap)
+    assert t_out[s, :m].tolist() == o_ts[:m].tolist() == [r[0] for r in ref[:m]], s
+    assert (v_out[s, :m].view(np.uint64) == o_v[:m].view(np.uint64)).all(), s
+
+
+@pytest.mark.parametrize("mode", ["simple", "tolerance", "resets"])
+def test_prom_kernels_on_host_refuse_rows_shorter_than_their_count(dev, mode):
+    """n_points[s] > cap is what decode and merge report for a row that hit its capacity.  Such a series gets
+    INVALID_ARG and n_out 0, and its output row keeps what was there; its input row is not read (the rows after the
+    last series hold sentinels that would be converted otherwise).  A series with n_points == cap right before it and
+    every other series convert as usual."""
+    rng = np.random.default_rng({"simple": 11, "tolerance": 12, "resets": 13}[mode])
+    S, cap, extra = 40, 24, 2
+    ts, vals, n = _batch(rng, S + extra, cap)  # rows S.. are memory after the last series
+    ts[S:] = 1599955200 * SEC
+    vals[S:] = 4321.0
+    n = n[:S].copy()
+    mid, last = S // 2, S - 1
+    n[mid - 1], n[mid], n[last] = cap, cap + 3, cap + cap // 2
+    resolution = 300 * SEC
+    tol = 1e-3 if mode == "tolerance" else 0.0
+    until = int(ts[:S].max()) if tol else 0
+    handle = (np.arange(S) % 3 != 1).astype(np.uint8) if mode == "resets" else None
+    out_cap = cap + 1
+    t_out, v_out, n_out, st, was_simple = _convert(dev, ts, vals, n, S, cap, resolution, handle, tol, until, out_cap)
     assert was_simple == (1 if mode == "simple" else 0)
     for s in range(S):
-        k = int(n[s])
-        h = bool(handle[s]) if handle is not None else False
-        o_ts, o_v = O.prom_convert_series(ts[s, :k], vals[s, :k], resolution, h, tol, until)
-        ref = prom_convert(ts[s, :k].tolist(), vals[s, :k].tolist(), resolution, h, tol, until)
-        assert len(ref) == len(o_ts) == int(n_out[s]), (s, len(ref), len(o_ts), int(n_out[s]))
-        assert int(st[s]) == (100 if len(ref) > out_cap else 0), s  # M3TSZ_ERR_CAPACITY
-        m = min(len(ref), out_cap)
-        assert t_out[s, :m].tolist() == o_ts[:m].tolist() == [r[0] for r in ref[:m]], s
-        assert (v_out[s, :m].view(np.uint64) == o_v[:m].view(np.uint64)).all(), s
+        if s in (mid, last):
+            assert int(st[s]) == 101 and int(n_out[s]) == 0, (s, int(st[s]), int(n_out[s]))  # M3TSZ_ERR_INVALID_ARG
+            assert (t_out[s] == T_FILL).all() and (v_out[s].view(np.uint64) == V_FILL).all(), s
+        else:
+            _assert_series(ts, vals, n, s, resolution, handle, tol, until, out_cap, t_out, v_out, n_out, st)

@@ -5,7 +5,8 @@ over block slices, SeriesIterator over replicas with the [start, end) filter), c
 oracle (oracle/m3tsz_merge_oracle.c, itself pinned by the reference's table tests) on random fetch shapes:
 replicas x block slices x readers per slice, duplicate timestamps with different values (the tie-break order
 that swap-removal perturbs), empty readers, reader errors, out-of-order blocks, range filters, equal-timestamp
-strategies."""
+strategies -- also over NaN payloads, +-Inf and +-0, where the strategies' sort and frequency count follow Go's
+comparison rules rather than Python's."""
 import numpy as np
 import pytest
 
@@ -34,6 +35,17 @@ class SeqIter:
         return self.ts[self.i], self.vals[self.i]
 
 
+def insertion_sort(items, less):
+    """sort.Slice on <= 12 elements (the merge's limit) is Go's insertionSortLessFunc, in place: the order it leaves
+    in `earliest` is where the next current() starts from.  With NaN values `less` is not a strict weak order, and
+    this is the order Go produces, not Python's list.sort."""
+    for i in range(1, len(items)):
+        j = i
+        while j > 0 and less(items[j], items[j - 1]):
+            items[j], items[j - 1] = items[j - 1], items[j]
+            j -= 1
+
+
 class Iterators:  # iterators.go
     def __init__(self):
         self.values, self.earliest, self.earliest_at = [], [], TIME_MAX
@@ -42,15 +54,16 @@ class Iterators:  # iterators.go
 
     def current(self):
         e = self.earliest
-        if self.strategy == 1:    # highest value: ascending sort, take the last
-            e.sort(key=lambda it: it.current()[1])
-        elif self.strategy == 2:  # lowest value
-            e.sort(key=lambda it: -it.current()[1])
-        elif self.strategy == 3:  # highest frequency
-            freq = {}
-            for it in e:
-                freq[it.current()[1]] = freq.get(it.current()[1], 0) + 1
-            e.sort(key=lambda it: freq[it.current()[1]])
+        val = lambda it: it.current()[1]
+        if self.strategy == 1:    # IterateHighestValue: sort by <, take the last
+            insertion_sort(e, lambda a, b: val(a) < val(b))
+        elif self.strategy == 2:  # IterateLowestValue
+            insertion_sort(e, lambda a, b: val(a) > val(b))
+        elif self.strategy == 3:  # IterateHighestFrequencyValue
+            # valueFrequencies is a map[float64]int: a key is found again only by ==, so +0 and -0 are one key and
+            # a NaN key is never found again (every NaN increment adds a new entry; the lookup in `less` reads 0)
+            freq = lambda it: sum(1 for o in e if val(o) == val(it))
+            insertion_sort(e, lambda a, b: freq(a) < freq(b))
         return e[-1].current()
 
     def push(self, it):
@@ -233,6 +246,86 @@ def _random_case(rng, n_series):
         ts[q, : len(t)], vals[q, : len(t)] = t, v
     return (seqs, ts, vals, np.array(n_points + ([] if seqs else [0]), dtype=np.uint32),
             np.array(status + ([] if seqs else [0]), dtype=np.int32), slice_off, replica_off, series_off, base)
+
+
+# Values where the strategies' comparisons are subtle: NaN (three payloads, one of them negative) is neither < nor >
+# anything and never equal to itself, the two zeros are ==, the infinities compare like numbers.
+SPECIAL_BITS = np.array([0x7FF8000000000000, 0x7FF8000000000001, 0xFFF8000000000000, 0x7FF0000000000000,
+                         0xFFF0000000000000, 0x0000000000000000, 0x8000000000000000], dtype=np.uint64)
+SPECIAL_VALUES = SPECIAL_BITS.view(np.float64).tolist() + [1.0, -2.5, 3.0]
+SPECIAL_START = 1_600_000_000 * 10 ** 9
+
+
+def special_value_series(rng, n_series, replicas=(1, 12), readers=(1, 4), n_blocks=(1, 2)):
+    """Series in the nested form of test_merge_oracle.build: replicas x block slices x readers x [(value, ts)].
+    Timestamps come from a grid of 8 per block, so most of them are equal across replicas and across the readers of
+    a slice; every value comes from SPECIAL_VALUES (bits kept: Python floats carry NaN payloads)."""
+    series = []
+    for _ in range(n_series):
+        reps = []
+        for _r in range(int(rng.integers(replicas[0], replicas[1] + 1))):
+            slices = []
+            for b in range(int(rng.integers(n_blocks[0], n_blocks[1] + 1))):
+                rds = []
+                for _q in range(int(rng.integers(readers[0], readers[1] + 1))):
+                    slots = np.unique(rng.integers(0, 8, size=int(rng.integers(0, 9))))
+                    rds.append([(SPECIAL_VALUES[int(rng.integers(0, len(SPECIAL_VALUES)))],
+                                 SPECIAL_START + int(b * 8 + k) * 10 ** 9) for k in slots])
+                slices.append(rds)
+            reps.append(slices)
+        series.append(reps)
+    return series
+
+
+SPECIAL_RANGE = (SPECIAL_START + 3 * 10 ** 9, SPECIAL_START + 12 * 10 ** 9)  # cuts into both blocks
+
+
+def model_merge(series, start, end, strategy):
+    """the object model over series in test_merge_oracle.build's nested form -> [(datapoints, err)] per series"""
+    out = []
+    for replicas in series:
+        reps = []
+        for slices in replicas:
+            its = []
+            for readers in slices:
+                sl = []
+                for rd in readers:
+                    err = 0
+                    if isinstance(rd, tuple):
+                        rd, err = rd
+                    sl.append(SeqIter([t for _, t in rd], [v for v, _ in rd], err))
+                its.append(sl)
+            reps.append(MultiReaderIter(its))
+        out.append(series_iterate(reps, start, end, strategy))
+    return out
+
+
+def bits(values):
+    return np.array(values, dtype=np.float64).view(np.uint64)
+
+
+@pytest.mark.parametrize("seed", range(4))
+@pytest.mark.parametrize("strategy", [0, 1, 2, 3])
+def test_iterator_layer_model_matches_merge_oracle_on_special_values(seed, strategy):
+    """NaN with payloads, +-Inf and +-0 at equal timestamps: the strategies' sort with < / > (false on NaN), the
+    frequency count (0 for NaN, one key for +-0) and the insertion order they leave in `earliest`, 1 to 12 replicas,
+    1 to 4 readers per slice, the range filter on and off; every value compared bit for bit."""
+    from test_merge_oracle import build
+    rng = np.random.default_rng(700 + seed * 11 + strategy)
+    series = special_value_series(rng, 80)
+    ts, vals, npts, st, slice_off, replica_off, series_off = build(series)
+    ties = 0
+    for start, end in ((0, 0), SPECIAL_RANGE):
+        o_ts, o_val, o_n, o_st = O.series_merge_batch(ts, vals, npts, st, slice_off, replica_off, series_off,
+                                                      start=start, end=end, strategy=strategy)
+        for s, (out, err) in enumerate(model_merge(series, start, end, strategy)):
+            assert int(o_st[s]) == err == 0, (s, int(o_st[s]), err)
+            assert int(o_n[s]) == len(out), (s, int(o_n[s]), len(out))
+            assert o_ts[s, : len(out)].tolist() == [p[0] for p in out], s
+            assert (o_val[s, : len(out)].view(np.uint64) == bits([p[1] for p in out])).all(), s
+            if not start:
+                ties += len(out) < sum(len(rd) for r in series[s] for sl in r for rd in sl)
+    assert ties > 40  # most series merge equal timestamps
 
 
 @pytest.mark.parametrize("seed", range(8))
