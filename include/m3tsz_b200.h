@@ -662,6 +662,63 @@ int m3tsz_aggregate_tiles_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const ui
                              uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
                              uint64_t *d_total_bytes, void *stream);
 
+/* Tile aggregation with the aggregator's transformations (GenericElem.processValue,
+ * src/aggregator/aggregator/generic_elem.go:804-950): each non-empty window's value
+ * ValueOf(agg_type) at t = the window's end runs through `ops` in order before it is
+ * written.  `ops` is the parsed transformation list of a pipeline without a rollup
+ * (newParsedPipeline, aggregator/elem_base.go:682-752), transformation.Type ids:
+ *   ABSOLUTE  math.Abs (the sign bit cleared, a NaN keeps its payload);
+ *   PERSECOND (v - prev_v) * 1e9 / (t - prev_t), two roundings; prev = the previous
+ *             non-empty window's binary-op input and end, (0, NaN) when there is none;
+ *             math.NaN() if prev_t >= t, either value is NaN or the difference is < 0;
+ *   INCREASE  v - prev_v, a NaN prev_v counting as 0; math.NaN() if prev_t >= t, v is
+ *             NaN or the difference is < 0 (so -0 passes);
+ *   ADD       a running sum over the element's life that skips NaN (one per Add op);
+ *   RESET     v passes; also writes (t + max(step_ns / 2, 1), 0) after it (only the
+ *             last Reset's; not written at timestamp 0).
+ * NaN results: math.NaN() is 0x7FF8000000000001; a NaN made by arithmetic (Inf - Inf) is
+ * amd64's 0xFFF8000000000000; a NaN carried from one input keeps its payload.
+ * discard_nan != 0 (DiscardNaNAggregatedValues, the reference default): a window whose
+ * result is NaN writes nothing, its Reset datapoint included; its binary-op input and
+ * Add sums still count.  At most M3TSZ_MAX_TRANSFORMS ops (the reference has no limit),
+ * at most one PerSecond / Increase (maxSupportedTransformationDerivativeOrder = 1), no
+ * unknown id: else M3TSZ_ERR_INVALID_ARG before any launch.
+ * d_state (optional, [n_series], caller-owned, all zeros = a new element) carries the
+ * previous window and the Add sums from one call to the next: splitting the windows into
+ * consecutive calls writes the same datapoints as one call.  A series' record is written
+ * only when its d_status is M3TSZ_OK: after a source decode error or M3TSZ_ERR_CAPACITY it
+ * is left as it was, so re-running those series with a larger buffer gives the unstopped
+ * result.  NULL: every series starts new and nothing is saved.
+ * d_n_tiles counts every datapoint written, Reset datapoints included; with a Reset op the
+ * series' slot bound is m3tsz_encode_bound(2 * n_windows).  n_ops == 0 gives exactly
+ * m3tsz_aggregate_tiles_ex's bytes.  One aggregation type per call: the reference's Add
+ * op is one closure shared by all of an element's aggregation types; here each call's
+ * type keeps its own sums. */
+enum { /* transformation.Type ids, src/metrics/transformation/type.go:36-43 */
+  M3TSZ_TRANSFORM_ABSOLUTE = 1,
+  M3TSZ_TRANSFORM_PERSECOND = 2,
+  M3TSZ_TRANSFORM_INCREASE = 3,
+  M3TSZ_TRANSFORM_ADD = 4,
+  M3TSZ_TRANSFORM_RESET = 5
+};
+#define M3TSZ_MAX_TRANSFORMS 8
+typedef struct m3tsz_transform_state {
+  int32_t has_prev;                   /* a non-empty window has been through the binary op */
+  int32_t reserved0;
+  int64_t prev_t;                     /* its end */
+  double prev_v;                      /* the binary op's input there (consumedValues) */
+  double sum[M3TSZ_MAX_TRANSFORMS];   /* sum[k]: the running sum of the Add op at position k */
+  uint64_t reserved1;
+} m3tsz_transform_state;              /* 96 bytes */
+int m3tsz_aggregate_tiles_transform(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                    uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                    uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                    int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
+                                    uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                                    uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
+                                    uint64_t *d_total_bytes, const int32_t *ops, uint32_t n_ops,
+                                    int32_t discard_nan, m3tsz_transform_state *d_state, void *stream);
+
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the
  * reference's interfaces (INTEGRATION.md §2 is that shim):

@@ -28,6 +28,10 @@ ERR_NO_DEVICE = 103
 AGG_LAST, AGG_MIN, AGG_MAX, AGG_MEAN, AGG_COUNT, AGG_SUM = 1, 2, 3, 4, 6, 7  # aggregation.Type ids
 AGG_SUMSQ, AGG_STDEV = 8, 9  # the expensive aggregations (m3tsz_aggregate_tiles_ex only)
 METRIC_COUNTER, METRIC_GAUGE = 1, 3  # metric.Type ids
+# transformation.Type ids (m3tsz_aggregate_tiles_transform)
+TRANSFORM_ABSOLUTE, TRANSFORM_PERSECOND, TRANSFORM_INCREASE, TRANSFORM_ADD, TRANSFORM_RESET = 1, 2, 3, 4, 5
+MAX_TRANSFORMS = 8  # M3TSZ_MAX_TRANSFORMS
+TRANSFORM_STATE_BYTES = 96  # sizeof(m3tsz_transform_state)
 
 UNIT_NONE, UNIT_S, UNIT_MS, UNIT_US, UNIT_NS, UNIT_MIN, UNIT_HOUR, UNIT_DAY, UNIT_YEAR = range(9)
 
@@ -107,6 +111,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_iter_pool_create", "m3tsz_iter_pool_get", "m3tsz_iter_pool_destroy",
     "m3tsz_encoder_set_reset", "m3tsz_encoder_set_append", "m3tsz_encoder_set_stream",
     "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex", "m3tsz_encoder_set_write",
+    "m3tsz_aggregate_tiles_transform",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -267,6 +272,10 @@ def lib():
     L.m3tsz_aggregate_tiles_ex.restype = C.c_int
     L.m3tsz_aggregate_tiles_ex.argtypes = [vp, po, vp, u64, vp, vp, u64, i64, i64, u32, i32, i32, i32, u32, vp,
                                            u64, vp, vp, vp, vp, vp, vp]
+    L.m3tsz_aggregate_tiles_transform.restype = C.c_int
+    L.m3tsz_aggregate_tiles_transform.argtypes = [vp, po, vp, u64, vp, vp, u64, i64, i64, u32, i32, i32, i32, u32,
+                                                  vp, u64, vp, vp, vp, vp, vp, C.POINTER(C.c_int32), u32, i32, vp,
+                                                  vp]
     _lib = L
     return L
 

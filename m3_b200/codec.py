@@ -332,14 +332,20 @@ class BatchCodec:
 
     def aggregate_tiles(self, streams, offsets, start_ns, step_ns, n_windows, agg_type=capi.AGG_LAST,
                         out_unit=capi.UNIT_S, lengths=None, align=64, capacity=None,
-                        out: Optional["PackedResult"] = None, metric_type=capi.METRIC_GAUGE):
+                        out: Optional["PackedResult"] = None, metric_type=capi.METRIC_GAUGE, transforms=(),
+                        discard_nan=True, state: Optional[torch.Tensor] = None):
         """storage.TileAggregator compute: decode -> Gauge (or Counter: metric_type=METRIC_COUNTER) per Step
-        window -> re-encode (packed).  Returns (PackedResult, n_tiles int32 [S])."""
+        window -> re-encode (packed).  Returns (PackedResult, n_tiles int32 [S]).
+        transforms: the pipeline's transformation ids (capi.TRANSFORM_*), applied in order to every non-empty
+        window's value (m3tsz_aggregate_tiles_transform); discard_nan drops a window whose result is NaN; state
+        (transform_state(S)) carries each series' previous window and Add sums from one call to the next."""
         S = offsets.numel() - 1 if lengths is None else lengths.numel()
         dev = self.device
+        transforms = [int(t) for t in transforms]
         if out is None:
             if capacity is None:
-                capacity = S * self.encode_bound(n_windows)
+                rows = 2 * n_windows if capi.TRANSFORM_RESET in transforms else n_windows
+                capacity = S * self.encode_bound(rows)
             out = PackedResult(
                 packed=torch.empty(capacity, dtype=torch.uint8, device=dev),
                 offsets=torch.empty(S, dtype=torch.int64, device=dev),
@@ -347,6 +353,19 @@ class BatchCodec:
                 status=torch.empty(S, dtype=torch.int32, device=dev),
                 total=torch.zeros(1, dtype=torch.int64, device=dev))
         n_tiles = torch.empty(S, dtype=torch.int32, device=dev)
+        if transforms:
+            if state is not None:
+                assert state.is_cuda and state.is_contiguous() and state.dtype == torch.uint8
+                assert state.shape == (S, capi.TRANSFORM_STATE_BYTES)
+            ops = (C.c_int32 * len(transforms))(*transforms)
+            rc = capi.lib().m3tsz_aggregate_tiles_transform(
+                self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets),
+                _ptr(lengths), S, int(start_ns), int(step_ns), int(n_windows), int(metric_type), int(agg_type),
+                int(out_unit), int(align), _ptr(out.packed), out.packed.numel(), _ptr(out.offsets),
+                _ptr(out.out_len), _ptr(out.status), _ptr(n_tiles), _ptr(out.total), ops, len(transforms),
+                1 if discard_nan else 0, _ptr(state), _cuda_stream_ptr(dev))
+            self.ctx.check(rc, "m3tsz_aggregate_tiles_transform")
+            return out, n_tiles
         if metric_type != capi.METRIC_GAUGE or agg_type in (capi.AGG_SUMSQ, capi.AGG_STDEV):
             rc = capi.lib().m3tsz_aggregate_tiles_ex(
                 self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets),
@@ -362,6 +381,11 @@ class BatchCodec:
             _ptr(out.status), _ptr(n_tiles), _ptr(out.total), _cuda_stream_ptr(dev))
         self.ctx.check(rc, "m3tsz_aggregate_tiles_batch")
         return out, n_tiles
+
+    def transform_state(self, n_series: int) -> torch.Tensor:
+        """A zeroed m3tsz_transform_state per series (uint8 [S, 96]): every series a new element, for
+        aggregate_tiles(..., transforms=..., state=...)."""
+        return torch.zeros((n_series, capi.TRANSFORM_STATE_BYTES), dtype=torch.uint8, device=self.device)
 
     def segment_checksums(self, streams, offsets, lengths=None, expected=None):
         """Adler-32 of every stream (ts.Segment.CalculateChecksum, src/dbnode/ts/segment.go:60-76)

@@ -649,14 +649,24 @@ int m3tsz_prom_convert_batch(m3tsz_ctx *ctx, const int64_t *d_ts, const double *
   return M3TSZ_OK;
 }
 
-// Both tile calls, after the caller checked ctx, opts, d_total_bytes, d_status and the (metric, type) pair.
+// The transformation list of m3tsz_aggregate_tiles_transform, as the tile stage reads it: op k in bits 4k .. 4k + 3
+// of one word, 0 ending the list (a non-empty list is never 0).
+struct TileTransforms {
+  uint32_t ops = 0;
+  bool reset = false;  // a Reset op: two rows per window
+  int32_t discard_nan = 0;
+  m3tsz_transform_state *state = nullptr;
+};
+
+// Every tile call, after the caller checked ctx, opts, d_total_bytes, d_status, the (metric, type) pair and the
+// transformation list (xf.ops == 0: none, the stage of m3tsz_aggregate_tiles_ex).
 static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                                 uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
                                 uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
                                 int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
                                 uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
                                 uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
-                                uint64_t *d_total_bytes, void *stream) {
+                                uint64_t *d_total_bytes, void *stream, const TileTransforms &xf = TileTransforms()) {
   cudaStream_t st = (cudaStream_t)stream;
   if (n_series == 0) {
     DeviceGuard guard(ctx->device);
@@ -718,7 +728,9 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
   EncodeParams p;
   memset(&p, 0, sizeof(p));
-  if ((rc = packed_params(ctx, n_series, m3tsz_encode_bound(n_windows), align, d_packed, packed_capacity,
+  // (a Reset op writes up to two datapoints per window)
+  const uint64_t rows = xf.reset ? 2ull * n_windows : (uint64_t)n_windows;
+  if ((rc = packed_params(ctx, n_series, m3tsz_encode_bound(rows), align, d_packed, packed_capacity,
                           d_out_offsets, d_total_bytes, st, p)))
     return rc;
   // every series' encoder starts at the tile range's start (the target block's start)
@@ -750,6 +762,12 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   p.agg_type = agg_type;
   p.metric_type = metric_type;
   p.n_tiles_out = d_n_tiles;
+  if (xf.ops) {
+    p.in_mode = 4;
+    p.xf_ops = xf.ops;
+    p.xf_discard_nan = xf.discard_nan ? 1 : 0;
+    p.xf_state = xf.state;
+  }
   CK(launch_encode(p, opts->int_optimized != 0, st));
   ctx->launches += 2;
   CK(launch_tiles_status((const int32_t *)d_sst, d_status, n_series, st));
@@ -796,6 +814,34 @@ int m3tsz_aggregate_tiles_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const ui
   return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                               n_windows, metric_type, agg_type, out_unit, align, d_packed, packed_capacity,
                               d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream);
+}
+
+int m3tsz_aggregate_tiles_transform(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                    uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                    uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                    int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
+                                    uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                                    uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
+                                    uint64_t *d_total_bytes, const int32_t *ops, uint32_t n_ops,
+                                    int32_t discard_nan, m3tsz_transform_state *d_state, void *stream) {
+  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !valid_tile_pair(metric_type, agg_type))
+    return M3TSZ_ERR_INVALID_ARG;
+  // newParsedPipeline (aggregator/elem_base.go:682-752): known types, derivative order <= 1
+  if (n_ops > M3TSZ_MAX_TRANSFORMS || (n_ops && !ops)) return M3TSZ_ERR_INVALID_ARG;
+  TileTransforms xf;
+  int binary = 0;
+  for (uint32_t k = 0; k < n_ops; k++) {
+    if (ops[k] < M3TSZ_TRANSFORM_ABSOLUTE || ops[k] > M3TSZ_TRANSFORM_RESET) return M3TSZ_ERR_INVALID_ARG;
+    binary += ops[k] == M3TSZ_TRANSFORM_PERSECOND || ops[k] == M3TSZ_TRANSFORM_INCREASE;
+    xf.reset |= ops[k] == M3TSZ_TRANSFORM_RESET;
+    xf.ops |= (uint32_t)ops[k] << (4 * k);
+  }
+  if (binary > 1) return M3TSZ_ERR_INVALID_ARG;
+  xf.discard_nan = discard_nan;
+  xf.state = d_state;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, metric_type, agg_type, out_unit, align, d_packed, packed_capacity,
+                              d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream, xf);
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

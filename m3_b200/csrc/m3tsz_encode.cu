@@ -49,7 +49,7 @@ constexpr int ENC_IN_T_PM = 4;
 // input tiles in flight per warp in the point-major stage (a ring of stages, one mbarrier each)
 constexpr int ENC_NSTAGE_PM = 2;
 // input stage IN: 0 series-major tiles (8 rows: one 64-byte segment per series and array), 1 point-major
-// tiles, 2 Gauge aggregates read directly (no input tiles)
+// tiles, 2 Gauge aggregates read directly (no input tiles), 4 the same through the transformations
 // IN = 3 (append mode only): a bucket write's share of one encoder (DESIGN.md §4.11).  Each lane reads its own
 // series' datapoints directly (the lanes of the overflow pass belong to scattered series) and takes the ones the
 // route kernel sent to its encoder.
@@ -83,11 +83,20 @@ template <int IN>
 __host__ __device__ constexpr int enc_in_stride() {
   return enc_bulk<IN>() ? 32 : ENC_STRIDE;
 }
+// The tile stage with transformations (IN = 4) keeps every lane's m3tsz_transform_state in shared memory behind the
+// output tile (in registers the sums pushed the int-optimised kernel past its 128 registers into spills).  A lane's
+// record is padded to 104 bytes (26 words): the 16 lanes of a half-warp's 8-byte access then hit distinct bank pairs.
+struct XfSlot {
+  m3tsz_transform_state st;
+  uint64_t pad;
+};
+static_assert(sizeof(XfSlot) == 104 && (ENC_OUT_TILE_WORDS * 4) % 8 == 0, "transformation state slots");
 template <int IN>
 __host__ __device__ constexpr size_t enc_warp_smem() {
   const size_t raw =
       ((IN == 0 || IN == 1) ? 2 * (size_t)enc_nstage<IN>() * (enc_in_t<IN>() * enc_in_stride<IN>()) * 8 : 0) +
-      (size_t)ENC_OUT_TILE_WORDS * 4 + (enc_bulk<IN>() ? 8 * enc_nstage<IN>() : 0);  // (+ one mbarrier per stage)
+      (size_t)ENC_OUT_TILE_WORDS * 4 + (enc_bulk<IN>() ? 8 * enc_nstage<IN>() : 0) +  // (+ one mbarrier per stage)
+      (IN == 4 ? 32 * sizeof(XfSlot) : 0);
   return enc_bulk<IN>() ? ((raw + 127) & ~(size_t)127) : raw;  // tensor copies land on 128-byte boundaries
 }
 
@@ -997,6 +1006,74 @@ __device__ __forceinline__ void enc_mbar_wait(uint32_t bar, uint32_t parity) {
       : "memory");
 }
 
+// ---------------------------------------------------------------------------
+// the aggregator's transformations on a window's value (DESIGN.md §4.8, GenericElem.processValue,
+// src/aggregator/aggregator/generic_elem.go:830-889), run by the lane that owns the series
+// ---------------------------------------------------------------------------
+constexpr uint64_t kXfEmptyNaN = 0x7FF8000000000001ull;  // emptyDatapoint's value: Go's math.NaN()
+constexpr uint64_t kXfOpNaN = 0xFFF8000000000000ull;     // amd64's default NaN of an invalid operation (Inf - Inf)
+
+__device__ __forceinline__ bool xf_isnan(double x) { return x != x; }
+__device__ __forceinline__ double xf_bits(uint64_t b) { return __longlong_as_double((long long)b); }
+
+// perSecond, metrics/transformation/binary.go:49-60.  Neither input is NaN past the first test, so the only NaN the
+// arithmetic makes is Inf - Inf; `diff < 0` is false for it and the rest carries it.
+__device__ __forceinline__ double xf_per_second(int64_t pt, double pv, int64_t t, double v) {
+  if (pt >= t || xf_isnan(pv) || xf_isnan(v)) return xf_bits(kXfEmptyNaN);
+  const double diff = __dsub_rn(v, pv);
+  if (xf_isnan(diff)) return xf_bits(kXfOpNaN);
+  if (diff < 0) return xf_bits(kXfEmptyNaN);
+  const int64_t dt = (int64_t)((uint64_t)t - (uint64_t)pt);
+  return __ddiv_rn(__dmul_rn(diff, 1e9), __ll2double_rn(dt));
+}
+
+// increase, binary.go:66-88
+__device__ __forceinline__ double xf_increase(int64_t pt, double pv, int64_t t, double v) {
+  if (pt >= t || xf_isnan(v)) return xf_bits(kXfEmptyNaN);
+  const double diff = __dsub_rn(v, xf_isnan(pv) ? 0.0 : pv);
+  if (xf_isnan(diff)) return xf_bits(kXfOpNaN);
+  return diff < 0 ? xf_bits(kXfEmptyNaN) : diff;
+}
+
+// One non-empty window (end t, value v) through the op list `ops` (op k in bits 4k .. 4k + 3, 0 ends the list).
+// Updates st (the binary op's previous window, the Add sums) and v; extra_t = the Reset datapoint's timestamp, 0 for
+// none (a Reset datapoint at 0 is not written either, generic_elem.go:920).  The loop is unrolled, so st.sum[k] has
+// a fixed offset.
+__device__ __forceinline__ void xf_window(uint32_t ops, int64_t step, m3tsz_transform_state &st, int64_t t,
+                                          double &v, int64_t &extra_t) {
+  extra_t = 0;
+#pragma unroll
+  for (int k = 0; k < M3TSZ_MAX_TRANSFORMS; k++) {
+    const uint32_t op = (ops >> (4 * k)) & 0xfu;
+    if (op == 0) break;
+    if (op == M3TSZ_TRANSFORM_ABSOLUTE) {  // math.Abs, unary.go:35-40
+      v = xf_bits((uint64_t)__double_as_longlong(v) & 0x7FFFFFFFFFFFFFFFull);
+    } else if (op == M3TSZ_TRANSFORM_ADD) {  // unary.go:46-54: curr += v unless v is NaN
+      if (!xf_isnan(v)) {
+        const double a = st.sum[k];
+        double r = __dadd_rn(a, v);
+        // amd64 ADDSD keeps a NaN operand's payload (quieted); only `a` can be one here.  Inf + -Inf: default NaN
+        if (xf_isnan(r))
+          r = xf_isnan(a) ? xf_bits((uint64_t)__double_as_longlong(a) | 0x0008000000000000ull) : xf_bits(kXfOpNaN);
+        st.sum[k] = r;
+      }
+      v = st.sum[k];
+    } else if (op == M3TSZ_TRANSFORM_PERSECOND || op == M3TSZ_TRANSFORM_INCREASE) {
+      // prev = the previous non-empty window's input to this op (consumedValues), (0, NaN) without one
+      const int64_t pt = st.has_prev ? st.prev_t : 0;
+      const double pv = st.has_prev ? st.prev_v : xf_bits(kXfEmptyNaN);
+      const double in = v;
+      v = op == M3TSZ_TRANSFORM_PERSECOND ? xf_per_second(pt, pv, t, in) : xf_increase(pt, pv, t, in);
+      st.has_prev = 1;
+      st.prev_t = t;
+      st.prev_v = in;
+    } else if (op == M3TSZ_TRANSFORM_RESET) {  // unary_multi.go:46-54: int64(math.Max(float64(step / 2), 1))
+      const int64_t rw = (int64_t)__double2ll_rz(fmax(__ll2double_rn(step / 2), 1.0));
+      extra_t = (int64_t)((uint64_t)t + (uint64_t)rw);
+    }
+  }
+}
+
 // PACKED = false: one warp per 32-series batch, every series writes its own slot
 //   p.out + s * p.out_stride (fixed stride).
 // PACKED = true : persistent warps fetch batches from a counter, encode into a per-warp
@@ -1014,15 +1091,21 @@ __device__ __forceinline__ void enc_mbar_wait(uint32_t bar, uint32_t parity) {
 // IN = 2: the Gauge aggregates of the fused decode+downsample kernel (window-major): datapoint i of a
 //         series = (tile_start + (i+1)*tile_step, Gauge.ValueOf(agg)) unless window i is empty
 //         (count == 0: skipped) -- the tile aggregation's re-encode without a gather pass.
+// IN = 4: IN = 2 with the aggregator's transformations (xf_window, p.xf_ops): the lane runs each non-empty window's
+//         value through the op list as it loads the row, and skips a NaN result when p.xf_discard_nan is set.
+//         With a Reset op a window takes two rows: 2i its datapoint, 2i + 1 the Reset datapoint (or skipped).  The
+//         prologue loads the series' p.xf_state record (zeros without one), the epilogue saves it when the
+//         series' status is OK.
 // APPEND: encoder-set append (DESIGN.md §4.6).  Every lane continues the open encoder p.state[s] in slot p.out +
 //   s * out_stride: the prologue loads the state (leftover words into the output tile), each datapoint is checked
 //   before anything of it is written, and the epilogue flushes whole sectors and saves the state instead of
 //   writing the tail.
 template <bool INT_OPT, bool PACKED, int IN, bool APPEND = false>
 __global__ void __launch_bounds__(ENC_WARPS * 32,
-                                  (IN == 2 || IN == 3) ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
+                                  IN >= 2 ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
     encode_kernel(const EncodeParams p, const __grid_constant__ EncTensorMaps tmaps) {
-  static_assert(!APPEND || (!PACKED && IN != 2), "append mode writes its own slots from staged inputs");
+  static_assert(!APPEND || (!PACKED && IN != 2 && IN != 4), "append mode writes its own slots from staged inputs");
+  constexpr bool TILES = IN == 2 || IN == 4;  // the tile aggregation's re-encode (IN = 4: with transformations)
   static_assert(IN != 3 || APPEND, "the routed input stage continues open encoders");
   extern __shared__ __align__(128) uint32_t smem[];
   const int lane = threadIdx.x & 31;
@@ -1119,6 +1202,19 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   const uint32_t slot_words = (uint32_t)(p.out_stride >> 2);
   // APPEND only (nothing of it exists in the batch instantiations, whose code stays as it was)
   std::conditional_t<APPEND, EncAppendVars, EncNoVars> av;
+  // IN = 4 only: the series' transformation state (this lane's slot behind the output tile), and the Reset datapoint
+  // of the window loaded last
+  bool xf_reset = false;
+  m3tsz_transform_state *xs = nullptr;
+  int64_t xf_extra_t = 0;
+  if constexpr (IN == 4) {
+    for (int k = 0; k < M3TSZ_MAX_TRANSFORMS; k++) xf_reset |= ((p.xf_ops >> (4 * k)) & 0xfu) == M3TSZ_TRANSFORM_RESET;
+    xs = &(reinterpret_cast<XfSlot *>(wbase + ENC_OUT_TILE_WORDS * 4) + lane)->st;
+    if (valid && p.xf_state)
+      *xs = p.xf_state[sidx];
+    else
+      memset(xs, 0, sizeof(*xs));
+  }
   if constexpr (APPEND) {
     if (valid) {
       n_pts = p.n_points ? p.n_points[in_s] : (uint32_t)p.points_stride;
@@ -1134,12 +1230,13 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       if (n_pts > 0 && s.n_enc == 0) put64(s, out_tile, lane, (uint64_t)s.prev_time, 64);  // WriteFirstTime :89-102
     }
   } else if (valid) {
-    n_pts = (IN != 2 && p.n_points) ? p.n_points[sidx] : (uint32_t)p.points_stride;
-    if (IN == 2 && p.tile_src_status && p.tile_src_status[sidx] != 0) n_pts = 0;  // failed source stream: no tiles
+    n_pts = (!TILES && p.n_points) ? p.n_points[sidx] : (uint32_t)p.points_stride;
+    if (TILES && p.tile_src_status && p.tile_src_status[sidx] != 0) n_pts = 0;  // failed source stream: no tiles
     if (n_pts > p.points_stride) {
       s.err = M3TSZ_ERR_INVALID_ARG;
       n_pts = 0;
     }
+    if (IN == 4 && xf_reset) n_pts *= 2;  // two rows per window
     const int64_t start = p.start[sidx];
     s.prev_time = start;
     s.unit = initial_time_unit(start, p.default_unit);  // encoder.reset :268-272
@@ -1288,8 +1385,16 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       v_o = (uint64_t)__double_as_longlong(__ldg(p.val + o));
       return;
     }
+    if constexpr (IN == 4) {
+      if (xf_reset && (row & 1u)) {  // the Reset datapoint of window row / 2 (0: none, or its window was skipped)
+        skip_o = xf_extra_t == 0;
+        t_o = xf_extra_t;  // (value +0)
+        return;
+      }
+      if (xf_reset) row >>= 1;
+    }
     const uint64_t o = (uint64_t)row * p.n_series + sidx;
-    if (IN == 2) {
+    if (TILES) {
       const int64_t c = __ldg(p.tile_count + o);
       skip_o = (c == 0);
       t_o = p.tile_start + (int64_t)(row + 1) * p.tile_step;  // the window's end boundary
@@ -1324,6 +1429,16 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
             v = agg_stdev(c, __ldg(static_cast<const double *>(p.tile_sum_sq) + o), __ldg(p.tile_sum + o));
             break;
           default: break;
+        }
+      }
+      if constexpr (IN == 4) {
+        xf_extra_t = 0;
+        if (!skip_o) {
+          xf_window(p.xf_ops, p.tile_step, *xs, t_o, v, xf_extra_t);
+          if (p.xf_discard_nan && xf_isnan(v)) {  // DiscardNaNAggregatedValues: nothing of the window
+            skip_o = true;
+            xf_extra_t = 0;
+          }
         }
       }
       v_o = (uint64_t)__double_as_longlong(v);
@@ -1368,7 +1483,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   };
 
   // ---- the hot tier's code: '0' (zero DoD) [+ '1' no-update] + XOR code, one merge ----
-  // The state update is unconditional (upd) where an inactive lane is a FINISHED lane (IN 0 / 1); with IN = 2 a
+  // The state update is unconditional (upd) where an inactive lane is a FINISHED lane (IN 0 / 1); with IN = 2 / 4 a
   // lane may sit out one row (an empty window) and must keep its state, and so must every lane in append mode,
   // whose state outlives the call.
   auto hot_commit = [&](int64_t t, uint64_t fb, bool upd, bool emit) {
@@ -1401,7 +1516,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
 
   // one datapoint, every tier, with every per-datapoint check (the tile of row `iter` has landed)
   auto row_active = [&](uint32_t iter) {
-    return s.err == 0 && iter < n_pts && !(IN == 2 && sk_pf);  // (n_pts is 0 without a series)
+    return s.err == 0 && iter < n_pts && !(TILES && sk_pf);  // (n_pts is 0 without a series)
   };
   auto encode_row = [&](uint32_t iter, bool tile_last, bool active) {
 
@@ -1523,7 +1638,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       if (INT_OPT) hot = hot && fb != s.prev_bits;
       Tier2 c2;
       if (__all_sync(FULL_MASK, hot || !active)) {
-        hot_commit(t, fb, (IN != 2 && !APPEND) || active, active);  // every live lane
+        hot_commit(t, fb, (!TILES && !APPEND) || active, active);  // every live lane
       } else if (__all_sync(FULL_MASK, tier2_candidate<INT_OPT>(s, active && room && steady, delta, fb, v, c2) ||
                                            !active)) {
         // second tier: small delta-of-delta + (float XOR | float repeat | int diff | int
@@ -1651,7 +1766,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   }
   flush_out(true);
   const uint64_t my_len = (total_bits + 7) >> 3;
-  if (valid && IN == 2 && p.n_tiles_out) p.n_tiles_out[sidx] = s.n_enc;
+  if (valid && TILES && p.n_tiles_out) p.n_tiles_out[sidx] = s.n_enc;
   if (valid && p.out_bits) p.out_bits[sidx] = total_bits;  // incl. the end-of-stream marker, before padding
   if (valid && p.last_value) {
     // Encoder.LastEncoded().Value (encoder.go:305-319): the float when the encoder is in float
@@ -1685,6 +1800,9 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       p.packed_off[sidx] = my_off;
       if (p.out_len) p.out_len[sidx] = fits ? my_len : 0ull;
       if (p.status) p.status[sidx] = (!fits && s.err == 0) ? M3TSZ_ERR_CAPACITY : s.err;
+      // the transformation state moves on only with a written series (status OK: no source error, no CAPACITY)
+      if (IN == 4 && p.xf_state && fits && s.err == 0 && !(p.tile_src_status && p.tile_src_status[sidx] != 0))
+        p.xf_state[sidx] = *xs;
     }
     __syncwarp();  // the flushes' stores to the slots are visible to the whole warp's copy below
     if (fits && total) {
@@ -1849,12 +1967,16 @@ uint64_t encode_packed_scratch_slots(uint64_t n_series) {
   return blocks * per_block;
 }
 
-// in_mode 0: series-major inputs; 1: point-major inputs; 2: Gauge aggregates
-// (packed output only)
+// in_mode 0: series-major inputs; 1: point-major inputs; 2: Gauge aggregates; 4: the aggregates through the
+// transformations (2 and 4: packed output only)
 cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_t stream) {
   if (p.in_mode == 2) {
     if (!p.packed) return cudaErrorInvalidValue;
     return int_optimized ? launch_encode_one<true, true, 2>(p, stream) : launch_encode_one<false, true, 2>(p, stream);
+  }
+  if (p.in_mode == 4) {
+    if (!p.packed) return cudaErrorInvalidValue;
+    return int_optimized ? launch_encode_one<true, true, 4>(p, stream) : launch_encode_one<false, true, 4>(p, stream);
   }
   if (p.in_mode == 1) {
     if (p.packed)

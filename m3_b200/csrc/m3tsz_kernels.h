@@ -63,11 +63,15 @@ struct EncodeParams {
   const uint32_t *n_points;  // optional
   const int64_t *start;
   int unit;
+  // IN = 4 (tile stage with transformations): the op list, op k in bits 4k .. 4k + 3, 0 ends it (in the padding
+  // after `unit`, so no other field moves)
+  uint32_t xf_ops;
   const uint8_t *units;  // optional per-datapoint units
   const uint64_t *ann_series_off;
   const m3tsz_annotation_entry *ann_entries;
   const uint8_t *ann_bytes;
   int default_unit;
+  int xf_discard_nan;  // IN = 4: a NaN result writes nothing of its window (in the padding after default_unit)
   uint8_t *out;
   uint64_t out_stride;
   uint64_t *out_len;
@@ -81,7 +85,8 @@ struct EncodeParams {
   unsigned long long *packed_cursor;   // bytes allocated so far (zero on entry)
   unsigned long long *batch_counter;   // work counter (zero on entry)
   uint32_t align;
-  // input stage (see encode_kernel): 0 series-major ts/val, 1 point-major ts/val, 2 Gauge aggregates
+  // input stage (see encode_kernel): 0 series-major ts/val, 1 point-major ts/val, 2 Gauge aggregates, 4 the
+  // aggregates through the transformations
   int in_mode;
   // window-major [points_stride][n_series]; a Counter's (metric_type M3TSZ_METRIC_COUNTER) are int64
   union { const double *tile_sum; const int64_t *tile_isum; };
@@ -98,8 +103,12 @@ struct EncodeParams {
   int agg_type;
   int metric_type;        // M3TSZ_METRIC_COUNTER, or the Gauge (M3TSZ_METRIC_GAUGE, or 0)
   uint32_t *n_tiles_out;  // optional [n_series]
-  // encoder-set append (launch_encode_append): per-series state in, updated in place; datapoints taken
-  m3tsz_encoder_state *state;
+  // encoder-set append (launch_encode_append): per-series state in, updated in place; datapoints taken.  The tile
+  // stage with transformations (IN = 4) keeps its per-series transformation state (optional) in the same pointer.
+  union {
+    m3tsz_encoder_state *state;
+    m3tsz_transform_state *xf_state;
+  };
   uint32_t *n_appended;
 };
 

@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
 """Transcribes the reference's own golden vectors for the M3TSZ path into
 tests/golden/m3tsz_goldens.json, those of the aggregator's Gauge / Counter arithmetic into
-tests/golden/m3tsz_agg_goldens.json, and the buffer bucket's write tables into
-tests/golden/m3tsz_buffer_goldens.json.
+tests/golden/m3tsz_agg_goldens.json, the buffer bucket's write tables into
+tests/golden/m3tsz_buffer_goldens.json, and the aggregator's transformations of a flushed window into
+tests/golden/m3tsz_transform_goldens.json.
 
 Run in the build container only (it reads /root/reference, which does not exist
 on the GPU box):   python scripts/make_goldens.py
@@ -23,6 +24,8 @@ OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "g
 OUT_AGG = os.path.join(os.path.dirname(OUT), "m3tsz_agg_goldens.json")
 # BufferBucket.write (storage/series/buffer.go:1261-1364): the write tables of storage/series/buffer_test.go
 OUT_BUFFER = os.path.join(os.path.dirname(OUT), "m3tsz_buffer_goldens.json")
+# the transformations of a flushed window (metrics/transformation, GenericElem.processValue)
+OUT_XF = os.path.join(os.path.dirname(OUT), "m3tsz_transform_goldens.json")
 
 SEC = 1_000_000_000
 MS = 1_000_000
@@ -487,6 +490,63 @@ def main():
         ],
     }
 
+    # ---- transformations: metrics/transformation/{binary,unary,unary_multi}_test.go and the flush sequences of
+    # aggregator/aggregator/elem_test.go up to their first resend / update.  A case is one element: `ops`
+    # (transformation.Type ids: 1 Absolute, 2 PerSecond, 3 Increase, 4 Add, 5 Reset), the resolution `step_ns`,
+    # DiscardNaNAggregatedValues, an optional starting state (the binary op's previous window) and its flushes
+    # ("calls"), each the non-empty windows (end, value) it consumes and the datapoints it writes, in order.
+    # Values are numbers, or "NaN:<64-bit hex>" for an exact NaN ("NaN:7ff8000000000001" is emptyDatapoint).
+    EMPTY = "NaN:7ff8000000000001"
+    NOW = 1_600_000_000_123_456_789  # the reset tests' time.Now()
+
+    def per_second(i, prev, curr, want):
+        return {"name": "TestPerSecond/%d" % i, "src_line": "metrics/transformation/binary_test.go:30-78",
+                "ops": [2], "step_ns": 10 * SEC, "discard_nan": False,
+                "state": {"has_prev": 1, "prev_t": prev[0] * SEC, "prev_v": prev[1]},
+                "calls": [{"windows": [[curr[0] * SEC, curr[1]]], "want": [[curr[0] * SEC, want]]}]}
+
+    def absolute(i, t, v, want):
+        return {"name": "TestAbsolute/%d" % i, "src_line": "metrics/transformation/unary_test.go:29-51",
+                "ops": [1], "step_ns": 10 * SEC, "discard_nan": False, "state": None,
+                "calls": [{"windows": [[t, v]], "want": [[t, want]]}]}
+
+    ps = [((1230, 25.0), (1240, 30.0), 0.5), ((1230, 25.0), (1240, 30.0), 0.5), ((1230, 25.0), (1230, 20.0), EMPTY),
+          ((1230, "NaN:7ff8000000000001"), (1240, 20.0), EMPTY), ((1230, 20.0), (1240, "NaN:7ff8000000000001"), EMPTY),
+          ((1230, 30.0), (1240, 20.0), EMPTY)]
+    xf = {
+        "src": "metrics/transformation/{binary,unary,unary_multi}_test.go, aggregator/aggregator/elem_test.go",
+        "cases": [per_second(i, *c) for i, c in enumerate(ps)] +
+                 [absolute(i, *c) for i, c in enumerate([(0, 1.2, 1.2), (0, -1.2, 1.2), (1234, -1.2, 1.2)])] + [
+            {"name": "TestReset", "src_line": "metrics/transformation/unary_multi_test.go:29-38", "ops": [5],
+             "step_ns": 30 * SEC, "discard_nan": False, "state": None,
+             "calls": [{"windows": [[NOW, 1000.0]], "want": [[NOW, 1000.0], [NOW + 15 * SEC, 0.0]]}]},
+            {"name": "TestResetAtLeast1Nanosecond", "src_line": "metrics/transformation/unary_multi_test.go:40-49",
+             "ops": [5], "step_ns": 1, "discard_nan": False, "state": None,
+             "calls": [{"windows": [[NOW, 1000.0]], "want": [[NOW, 1000.0], [NOW + 1, 0.0]]}]},
+            # Sum of one value per window, resolution 10 s (testStoragePolicy), Consume(0) / (220 s) / (240 s)
+            {"name": "TestGaugeElemReset", "src_line": "aggregator/aggregator/elem_test.go:2238-2305", "ops": [5],
+             "step_ns": 10 * SEC, "discard_nan": False, "state": None,
+             "calls": [{"windows": [], "want": []},
+                       {"windows": [[220 * SEC, 123.0]], "want": [[220 * SEC, 123.0], [225 * SEC, 0.0]]},
+                       {"windows": [[230 * SEC, 456.0], [240 * SEC, 589.0]],
+                        "want": [[230 * SEC, 456.0], [235 * SEC, 0.0], [240 * SEC, 589.0], [245 * SEC, 0.0]]}]},
+            # the default Gauge type (Last) of testGauge (123.456) in two windows, Increase
+            {"name": "TestGaugeElemConsumeResendBuffer", "src_line": "aggregator/aggregator/elem_test.go:1709-1765",
+             "ops": [3], "step_ns": 10 * SEC, "discard_nan": True, "state": None,
+             "calls": [{"windows": [[220 * SEC, 123.456]], "want": [[220 * SEC, 123.456]]},
+                       {"windows": [[230 * SEC, 123.456]], "want": [[230 * SEC, 0.0]]}]},
+            # Last, Increase (then a rollup: the forwarded values are the transformation's)
+            {"name": "TestGaugeElemResendBufferForwarding",
+             "src_line": "aggregator/aggregator/elem_test.go:2095-2199", "ops": [3], "step_ns": 10 * SEC,
+             "discard_nan": True, "state": None,
+             "calls": [{"windows": [], "want": []},
+                       {"windows": [[220 * SEC, 123.0]], "want": [[220 * SEC, 123.0]]},
+                       {"windows": [[230 * SEC, 456.0], [240 * SEC, 589.0]],
+                        "want": [[230 * SEC, 333.0], [240 * SEC, 133.0]]}],
+             "consumed": [123.0, 456.0, 589.0]},
+        ],
+    }
+
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f, indent=1)
@@ -497,6 +557,9 @@ def main():
     with open(OUT_BUFFER, "w") as f:
         json.dump(buffer, f, indent=1)
     print("wrote", OUT_BUFFER)
+    with open(OUT_XF, "w") as f:
+        json.dump(xf, f, indent=1)
+    print("wrote", OUT_XF)
 
 
 if __name__ == "__main__":
