@@ -693,7 +693,8 @@ int m3tsz_aggregate_tiles_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const ui
  * series' slot bound is m3tsz_encode_bound(2 * n_windows).  n_ops == 0 gives exactly
  * m3tsz_aggregate_tiles_ex's bytes.  One aggregation type per call: the reference's Add
  * op is one closure shared by all of an element's aggregation types; here each call's
- * type keeps its own sums. */
+ * type keeps its own sums (m3tsz_aggregate_tiles_types runs an element's types together
+ * and shares them). */
 enum { /* transformation.Type ids, src/metrics/transformation/type.go:36-43 */
   M3TSZ_TRANSFORM_ABSOLUTE = 1,
   M3TSZ_TRANSFORM_PERSECOND = 2,
@@ -718,6 +719,48 @@ int m3tsz_aggregate_tiles_transform(m3tsz_ctx *ctx, const m3tsz_options *opts, c
                                     uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
                                     uint64_t *d_total_bytes, const int32_t *ops, uint32_t n_ops,
                                     int32_t discard_nan, m3tsz_transform_state *d_state, void *stream);
+
+/* Tile aggregation of an element with several aggregation types (GenericElem.processValue's
+ * loop over e.aggTypes, generic_elem.go:830-889): one decode + windows for the whole set,
+ * one output stream per (type, series).  agg_types (host, 1 .. M3TSZ_MAX_ELEMENT_TYPES
+ * entries) must be strictly ascending, as idDecompressor.Decompress returns an element's
+ * types (metrics/aggregation/id_compress.go:110-135), and every entry must be valid for
+ * metric_type as in m3tsz_aggregate_tiles_ex; `ops` is checked as in
+ * m3tsz_aggregate_tiles_transform.  Else M3TSZ_ERR_INVALID_ARG before any launch.
+ * Per non-empty window, for type j = 0 .. n_types - 1 in order, ValueOf(agg_types[j]) runs
+ * through `ops` exactly as in m3tsz_aggregate_tiles_transform, except that:
+ *   - the Add op at position i updates one sum shared by every type (the reference's one
+ *     transformAdd closure, transformation/unary.go:46-54): type 0 adds before type 1;
+ *   - the binary op's previous value is type j's own input in the previous non-empty
+ *     window (consumedValues[j]); the previous window's end is the element's;
+ *   - discard_nan drops type j's datapoint (and its Reset datapoint) only.
+ * Output row j * n_series + s is series s, type j: d_out_offsets, d_out_len, d_status and
+ * d_n_tiles have n_types * n_series entries, the rows packed into d_packed as
+ * m3tsz_encode_batch_packed packs streams (slot bound as in m3tsz_aggregate_tiles_transform).
+ * A source decode error goes to all n_types rows of its series, with no output.
+ * d_state (optional, [n_series], caller-owned, all zeros = a new element) carries the
+ * element from one call to the next.  A series' record is written only when its source
+ * decoded and all n_types rows are M3TSZ_OK, so re-running the series after an error or
+ * M3TSZ_ERR_CAPACITY gives the unstopped result for every type.  NULL: every series starts
+ * new and nothing is saved.  With n_types == 1 the call writes the bytes, lengths, tile
+ * counts, status and (in the first 96 bytes of the record) the state of
+ * m3tsz_aggregate_tiles_transform (m3tsz_aggregate_tiles_ex when n_ops == 0).  Without an
+ * Add op, row j equals m3tsz_aggregate_tiles_transform's for agg_types[j]. */
+#define M3TSZ_MAX_ELEMENT_TYPES 8
+typedef struct m3tsz_element_state {
+  m3tsz_transform_state head; /* has_prev, prev_t, prev_v = type 0's binary-op input, sum[8] (shared) */
+  double prev_v_more[M3TSZ_MAX_ELEMENT_TYPES - 1]; /* the binary op's input of types 1..7 */
+  uint64_t reserved;
+} m3tsz_element_state;        /* 160 bytes */
+int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                int32_t metric_type, const int32_t *agg_types, uint32_t n_types,
+                                int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+                                uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
+                                uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
+                                uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
+                                void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

@@ -32,6 +32,8 @@ METRIC_COUNTER, METRIC_GAUGE = 1, 3  # metric.Type ids
 TRANSFORM_ABSOLUTE, TRANSFORM_PERSECOND, TRANSFORM_INCREASE, TRANSFORM_ADD, TRANSFORM_RESET = 1, 2, 3, 4, 5
 MAX_TRANSFORMS = 8  # M3TSZ_MAX_TRANSFORMS
 TRANSFORM_STATE_BYTES = 96  # sizeof(m3tsz_transform_state)
+MAX_ELEMENT_TYPES = 8  # M3TSZ_MAX_ELEMENT_TYPES (m3tsz_aggregate_tiles_types)
+ELEMENT_STATE_BYTES = 160  # sizeof(m3tsz_element_state)
 
 UNIT_NONE, UNIT_S, UNIT_MS, UNIT_US, UNIT_NS, UNIT_MIN, UNIT_HOUR, UNIT_DAY, UNIT_YEAR = range(9)
 
@@ -111,7 +113,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_iter_pool_create", "m3tsz_iter_pool_get", "m3tsz_iter_pool_destroy",
     "m3tsz_encoder_set_reset", "m3tsz_encoder_set_append", "m3tsz_encoder_set_stream",
     "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex", "m3tsz_encoder_set_write",
-    "m3tsz_aggregate_tiles_transform",
+    "m3tsz_aggregate_tiles_transform", "m3tsz_aggregate_tiles_types",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -276,6 +278,10 @@ def lib():
     L.m3tsz_aggregate_tiles_transform.argtypes = [vp, po, vp, u64, vp, vp, u64, i64, i64, u32, i32, i32, i32, u32,
                                                   vp, u64, vp, vp, vp, vp, vp, C.POINTER(C.c_int32), u32, i32, vp,
                                                   vp]
+    L.m3tsz_aggregate_tiles_types.restype = C.c_int
+    L.m3tsz_aggregate_tiles_types.argtypes = [vp, po, vp, u64, vp, vp, u64, i64, i64, u32, i32, C.POINTER(C.c_int32),
+                                              u32, i32, u32, vp, u64, vp, vp, vp, vp, vp, C.POINTER(C.c_int32), u32,
+                                              i32, vp, vp]
     _lib = L
     return L
 

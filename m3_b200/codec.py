@@ -387,6 +387,53 @@ class BatchCodec:
         aggregate_tiles(..., transforms=..., state=...)."""
         return torch.zeros((n_series, capi.TRANSFORM_STATE_BYTES), dtype=torch.uint8, device=self.device)
 
+    def aggregate_tiles_types(self, streams, offsets, start_ns, step_ns, n_windows, agg_types,
+                              metric_type=capi.METRIC_GAUGE, out_unit=capi.UNIT_S, lengths=None, align=64,
+                              capacity=None, transforms=(), discard_nan=True, state: Optional[torch.Tensor] = None):
+        """An element with several aggregation types (m3tsz_aggregate_tiles_types): one decode + windows, then one
+        stream per (type, series).  agg_types: strictly ascending aggregation.Type ids (capi.AGG_*), 1..8 of them;
+        transforms / discard_nan as in aggregate_tiles, except that the Add op's sums are shared by the types, as in
+        the reference's element.  state (element_state(S)) carries each series' element from one call to the next.
+        Returns (PackedResult, n_tiles int32 [k, S]); the result's offsets / out_len / status are [k, S] views, row j
+        being agg_types[j]."""
+        S = offsets.numel() - 1 if lengths is None else lengths.numel()
+        dev = self.device
+        types = [int(t) for t in agg_types]
+        transforms = [int(t) for t in transforms]
+        k = len(types)
+        if capacity is None:
+            rows = 2 * n_windows if capi.TRANSFORM_RESET in transforms else n_windows
+            capacity = max(1, k * S * self.encode_bound(rows))
+        n = max(1, k) * S
+        out = PackedResult(
+            packed=torch.empty(capacity, dtype=torch.uint8, device=dev),
+            offsets=torch.empty(n, dtype=torch.int64, device=dev),
+            out_len=torch.empty(n, dtype=torch.int64, device=dev),
+            status=torch.empty(n, dtype=torch.int32, device=dev),
+            total=torch.zeros(1, dtype=torch.int64, device=dev))
+        n_tiles = torch.empty(n, dtype=torch.int32, device=dev)
+        if state is not None:
+            assert state.is_cuda and state.is_contiguous() and state.dtype == torch.uint8
+            assert state.shape == (S, capi.ELEMENT_STATE_BYTES)
+        types_a = (C.c_int32 * max(1, k))(*types)
+        ops = (C.c_int32 * max(1, len(transforms)))(*transforms)
+        rc = capi.lib().m3tsz_aggregate_tiles_types(
+            self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), _ptr(lengths), S,
+            int(start_ns), int(step_ns), int(n_windows), int(metric_type), types_a, k, int(out_unit), int(align),
+            _ptr(out.packed), out.packed.numel(), _ptr(out.offsets), _ptr(out.out_len), _ptr(out.status),
+            _ptr(n_tiles), _ptr(out.total), ops, len(transforms), 1 if discard_nan else 0, _ptr(state),
+            _cuda_stream_ptr(dev))
+        self.ctx.check(rc, "m3tsz_aggregate_tiles_types")
+        out.offsets = out.offsets.view(k, S)
+        out.out_len = out.out_len.view(k, S)
+        out.status = out.status.view(k, S)
+        return out, n_tiles.view(k, S)
+
+    def element_state(self, n_series: int) -> torch.Tensor:
+        """A zeroed m3tsz_element_state per series (uint8 [S, 160]): every series a new element, for
+        aggregate_tiles_types(..., state=...)."""
+        return torch.zeros((n_series, capi.ELEMENT_STATE_BYTES), dtype=torch.uint8, device=self.device)
+
     def segment_checksums(self, streams, offsets, lengths=None, expected=None):
         """Adler-32 of every stream (ts.Segment.CalculateChecksum, src/dbnode/ts/segment.go:60-76)
         over the decoder's CSR layout; with `lengths` (int64 [S]) stream s = offsets[s] .. +lengths[s]

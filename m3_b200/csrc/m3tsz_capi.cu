@@ -656,10 +656,16 @@ struct TileTransforms {
   bool reset = false;  // a Reset op: two rows per window
   int32_t discard_nan = 0;
   m3tsz_transform_state *state = nullptr;
+  // m3tsz_aggregate_tiles_types: the element's types (n_types > 0: the multi-type stage, whatever `ops` is; the
+  // call's agg_type is then unused) and its records
+  const int32_t *types = nullptr;
+  uint32_t n_types = 0;
+  m3tsz_element_state *elem_state = nullptr;
 };
 
-// Every tile call, after the caller checked ctx, opts, d_total_bytes, d_status, the (metric, type) pair and the
-// transformation list (xf.ops == 0: none, the stage of m3tsz_aggregate_tiles_ex).
+// Every tile call, after the caller checked ctx, opts, d_total_bytes, d_status, the (metric, type) pairs and the
+// transformation list (xf.ops == 0: none, the stage of m3tsz_aggregate_tiles_ex).  One decode + windows serves every
+// type of xf.types; output row j * n_series + s is series s, type j.
 static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                                 uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
                                 uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
@@ -689,10 +695,15 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   if ((rc = ensure(ctx, kSlotWinLast, wb, &d_last))) return rc;
   if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_np))) return rc;
   if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_sst))) return rc;
-  // 1. fused decode + windows: the Gauge with `last` (mode 2), + sumSq for SumSq / Stdev (mode 4), or the Counter
-  //    (mode 5, its int64 sum / min / max in the Gauge's slots)
+  // 1. fused decode + windows: the Gauge with `last` (mode 2), + sumSq if a type is SumSq / Stdev (mode 4), or the
+  //    Counter (mode 5, its int64 sum / min / max in the Gauge's slots)
+  const bool multi = xf.n_types > 0;
+  const uint32_t n_types = multi ? xf.n_types : 1u;
+  const int32_t *types = multi ? xf.types : &agg_type;
+  const uint64_t n_rows = (uint64_t)n_types * n_series;
   const bool counter = metric_type == M3TSZ_METRIC_COUNTER;
-  const bool sq = counter || agg_type == M3TSZ_AGG_SUMSQ || agg_type == M3TSZ_AGG_STDEV;
+  bool sq = counter;
+  for (uint32_t j = 0; j < n_types; j++) sq |= types[j] == M3TSZ_AGG_SUMSQ || types[j] == M3TSZ_AGG_STDEV;
   void *d_sq = nullptr;
   if (!sq) {
     rc = downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
@@ -730,13 +741,13 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   memset(&p, 0, sizeof(p));
   // (a Reset op writes up to two datapoints per window)
   const uint64_t rows = xf.reset ? 2ull * n_windows : (uint64_t)n_windows;
-  if ((rc = packed_params(ctx, n_series, m3tsz_encode_bound(rows), align, d_packed, packed_capacity,
+  if ((rc = packed_params(ctx, n_rows, m3tsz_encode_bound(rows), align, d_packed, packed_capacity,
                           d_out_offsets, d_total_bytes, st, p)))
     return rc;
-  // every series' encoder starts at the tile range's start (the target block's start)
-  if ((rc = ensure(ctx, kSlotTileStarts, n_series * 8, &d_es))) return rc;
-  CK(launch_fill_i64((int64_t *)d_es, start_ns, n_series, st));
-  p.n_series = n_series;
+  // every row's encoder starts at the tile range's start (the target block's start)
+  if ((rc = ensure(ctx, kSlotTileStarts, n_rows * 8, &d_es))) return rc;
+  CK(launch_fill_i64((int64_t *)d_es, start_ns, n_rows, st));
+  p.n_series = n_rows;
   p.points_stride = n_windows;
   p.start = (const int64_t *)d_es;
   p.unit = out_unit;
@@ -762,7 +773,20 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   p.agg_type = agg_type;
   p.metric_type = metric_type;
   p.n_tiles_out = d_n_tiles;
-  if (xf.ops) {
+  void *d_rec = nullptr;
+  if (multi) {
+    // lanes write their parts of each series' new record to scratch; the status pass commits whole records
+    if (xf.elem_state && (rc = ensure(ctx, kSlotElementScratch, n_series * sizeof(m3tsz_element_state), &d_rec)))
+      return rc;
+    p.in_mode = 5;
+    p.xf_ops = xf.ops;
+    p.xf_discard_nan = (xf.ops && xf.discard_nan) ? 1 : 0;  // (an empty list discards nothing, as tiles_ex)
+    p.xf_elem = xf.elem_state;
+    p.xf_elem_out = (m3tsz_element_state *)d_rec;
+    p.tile_n_src = n_series;
+    p.tile_n_types = n_types;
+    for (uint32_t j = 0; j < n_types; j++) p.tile_types |= (uint32_t)types[j] << (4 * j);
+  } else if (xf.ops) {
     p.in_mode = 4;
     p.xf_ops = xf.ops;
     p.xf_discard_nan = xf.discard_nan ? 1 : 0;
@@ -770,7 +794,11 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   }
   CK(launch_encode(p, opts->int_optimized != 0, st));
   ctx->launches += 2;
-  CK(launch_tiles_status((const int32_t *)d_sst, d_status, n_series, st));
+  if (multi)
+    CK(launch_tiles_types_status((const int32_t *)d_sst, d_status, n_series, n_types,
+                                 (const m3tsz_element_state *)d_rec, xf.elem_state, st));
+  else
+    CK(launch_tiles_status((const int32_t *)d_sst, d_status, n_series, st));
   ctx->launches++;
   return M3TSZ_OK;
 }
@@ -816,6 +844,19 @@ int m3tsz_aggregate_tiles_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const ui
                               d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream);
 }
 
+// newParsedPipeline (aggregator/elem_base.go:682-752): known types, derivative order <= 1
+static bool parse_transforms(const int32_t *ops, uint32_t n_ops, TileTransforms &xf) {
+  if (n_ops > M3TSZ_MAX_TRANSFORMS || (n_ops && !ops)) return false;
+  int binary = 0;
+  for (uint32_t k = 0; k < n_ops; k++) {
+    if (ops[k] < M3TSZ_TRANSFORM_ABSOLUTE || ops[k] > M3TSZ_TRANSFORM_RESET) return false;
+    binary += ops[k] == M3TSZ_TRANSFORM_PERSECOND || ops[k] == M3TSZ_TRANSFORM_INCREASE;
+    xf.reset |= ops[k] == M3TSZ_TRANSFORM_RESET;
+    xf.ops |= (uint32_t)ops[k] << (4 * k);
+  }
+  return binary <= 1;
+}
+
 int m3tsz_aggregate_tiles_transform(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                                     uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
                                     uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
@@ -826,21 +867,39 @@ int m3tsz_aggregate_tiles_transform(m3tsz_ctx *ctx, const m3tsz_options *opts, c
                                     int32_t discard_nan, m3tsz_transform_state *d_state, void *stream) {
   if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !valid_tile_pair(metric_type, agg_type))
     return M3TSZ_ERR_INVALID_ARG;
-  // newParsedPipeline (aggregator/elem_base.go:682-752): known types, derivative order <= 1
-  if (n_ops > M3TSZ_MAX_TRANSFORMS || (n_ops && !ops)) return M3TSZ_ERR_INVALID_ARG;
   TileTransforms xf;
-  int binary = 0;
-  for (uint32_t k = 0; k < n_ops; k++) {
-    if (ops[k] < M3TSZ_TRANSFORM_ABSOLUTE || ops[k] > M3TSZ_TRANSFORM_RESET) return M3TSZ_ERR_INVALID_ARG;
-    binary += ops[k] == M3TSZ_TRANSFORM_PERSECOND || ops[k] == M3TSZ_TRANSFORM_INCREASE;
-    xf.reset |= ops[k] == M3TSZ_TRANSFORM_RESET;
-    xf.ops |= (uint32_t)ops[k] << (4 * k);
-  }
-  if (binary > 1) return M3TSZ_ERR_INVALID_ARG;
+  if (!parse_transforms(ops, n_ops, xf)) return M3TSZ_ERR_INVALID_ARG;
   xf.discard_nan = discard_nan;
   xf.state = d_state;
   return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                               n_windows, metric_type, agg_type, out_unit, align, d_packed, packed_capacity,
+                              d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream, xf);
+}
+
+int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                int32_t metric_type, const int32_t *agg_types, uint32_t n_types,
+                                int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+                                uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
+                                uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
+                                uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
+                                void *stream) {
+  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !agg_types || n_types == 0 ||
+      n_types > M3TSZ_MAX_ELEMENT_TYPES)
+    return M3TSZ_ERR_INVALID_ARG;
+  // an element's types: strictly ascending (idDecompressor.Decompress walks a bitset), each valid for the metric
+  for (uint32_t j = 0; j < n_types; j++)
+    if (!valid_tile_pair(metric_type, agg_types[j]) || (j && agg_types[j] <= agg_types[j - 1]))
+      return M3TSZ_ERR_INVALID_ARG;
+  TileTransforms xf;
+  if (!parse_transforms(ops, n_ops, xf)) return M3TSZ_ERR_INVALID_ARG;
+  xf.discard_nan = discard_nan;
+  xf.types = agg_types;
+  xf.n_types = n_types;
+  xf.elem_state = d_state;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, metric_type, agg_types[0], out_unit, align, d_packed, packed_capacity,
                               d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream, xf);
 }
 

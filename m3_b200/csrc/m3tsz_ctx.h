@@ -40,9 +40,8 @@ struct Scratch {
 //   36, 37        packed slot sets, batch counter                packed encode, tiles
 //   38, 39        window last, tile encoder starts               tiles, downsample_ex (38, NULL d_last); tiles
 //   40-47         streaming handles, under handle_mu             m3tsz_stream.cu
+//   35            element records of the multi-type tile stage   tiles (aggregate_tiles_types)
 //   48-50         route targets, touched records, their count    encoder_set_write
-//
-// Slot 35 is unused.
 enum Slot : int {
   kSlotStreams = 0,
   kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
@@ -63,6 +62,7 @@ enum Slot : int {
   kSlotCompactTmp = 15,
   kSlotLaneBase = 16,
   kSlotWinSumSq = 25,  // between the two pipeline lanes' slot ranges
+  kSlotElementScratch = 35,
   kSlotPackedSlots = 36,
   kSlotBatchCounter = 37,
   kSlotWinLast = 38,

@@ -91,12 +91,29 @@ struct XfSlot {
   uint64_t pad;
 };
 static_assert(sizeof(XfSlot) == 104 && (ENC_OUT_TILE_WORDS * 4) % 8 == 0, "transformation state slots");
+// The multi-type stage (IN = 5) keeps an element's record there instead, rearranged for the chain: `w` is the
+// m3tsz_transform_state xf_window runs on (its prev_v is loaded with the type that runs), pv[j] is type j's
+// binary-op input, and `reserved` the record's last word.  The lane's source series and type sit behind it, out of
+// the registers (in them the int-optimised kernel spilled).  184 bytes (23 8-byte words, an odd number): the 16
+// lanes of a half-warp's 8-byte access hit distinct bank pairs, as in XfSlot.
+struct XfElem {
+  m3tsz_transform_state w;
+  double pv[M3TSZ_MAX_ELEMENT_TYPES];
+};
+struct XfElemSlot {
+  XfElem e;
+  uint64_t reserved;
+  uint64_t src;  // the lane's source series (row % tile_n_src)
+  uint32_t ty;   // its type (row / tile_n_src)
+  uint32_t all;  // the list has an Add op: the lane runs every type
+};
+static_assert(sizeof(XfElemSlot) == 184, "element state slots");
 template <int IN>
 __host__ __device__ constexpr size_t enc_warp_smem() {
   const size_t raw =
       ((IN == 0 || IN == 1) ? 2 * (size_t)enc_nstage<IN>() * (enc_in_t<IN>() * enc_in_stride<IN>()) * 8 : 0) +
       (size_t)ENC_OUT_TILE_WORDS * 4 + (enc_bulk<IN>() ? 8 * enc_nstage<IN>() : 0) +  // (+ one mbarrier per stage)
-      (IN == 4 ? 32 * sizeof(XfSlot) : 0);
+      (IN == 4 ? 32 * sizeof(XfSlot) : 0) + (IN == 5 ? 32 * sizeof(XfElemSlot) : 0);
   return enc_bulk<IN>() ? ((raw + 127) & ~(size_t)127) : raw;  // tensor copies land on 128-byte boundaries
 }
 
@@ -1074,6 +1091,69 @@ __device__ __forceinline__ void xf_window(uint32_t ops, int64_t step, m3tsz_tran
   }
 }
 
+// One non-empty window (end t) of an element with several aggregation types (generic_elem.go:830-889, the loop over
+// e.aggTypes): types i0 .. i1 - 1 in order each take their value value_of(i) through xf_window, with the element's
+// Add sums (e.w.sum: a type adds after the types before it), the previous window as it was before this window (the
+// element's has_prev / prev_t) and the type's own binary-op input e.pv[i] (consumedValues[i]), which the type then
+// records.  take(i, v, extra_t) gets each type's result and Reset timestamp.  A lane whose list has an Add op runs
+// every type (i0 = 0, i1 = n_types) to keep the sums; without one, a type depends on nothing of the others.
+template <class ValueOf, class Take>
+__device__ __forceinline__ void xf_element_window(uint32_t ops, int64_t step, XfElem &e, uint32_t i0, uint32_t i1,
+                                                  int64_t t, ValueOf value_of, Take take) {
+  const int32_t has_prev = e.w.has_prev;
+  const int64_t prev_t = e.w.prev_t;
+#pragma unroll 1
+  for (uint32_t i = i0; i < i1; i++) {
+    double v = value_of(i);
+    int64_t extra_t = 0;
+    e.w.has_prev = has_prev;
+    e.w.prev_t = prev_t;
+    e.w.prev_v = e.pv[i];
+    xf_window(ops, step, e.w, t, v, extra_t);
+    e.pv[i] = e.w.prev_v;
+    take(i, v, extra_t);
+  }
+}
+
+// The window value of the tile stages (IN = 2 / 4 / 5): ValueOf(agg) of window-major element o with count c.  The
+// switches are uniform across a warp, except in an IN = 5 warp whose 32 rows straddle two types.
+__device__ __forceinline__ double tile_value_of(const EncodeParams &p, bool counter, int agg, uint64_t o, int64_t c) {
+  double v = 0.0;
+  if (counter) {
+    // Counter.ValueOf, counter.go:112-134: float64() of the int64 aggregates (uniform switch)
+    switch (agg) {
+      case M3TSZ_AGG_MIN: v = __ll2double_rn(__ldg(p.tile_imin + o)); break;
+      case M3TSZ_AGG_MAX: v = __ll2double_rn(__ldg(p.tile_imax + o)); break;
+      case M3TSZ_AGG_MEAN:
+        v = c == 0 ? 0.0 : __ddiv_rn(__ll2double_rn(__ldg(p.tile_isum + o)), __ll2double_rn(c));
+        break;
+      case M3TSZ_AGG_COUNT: v = __ll2double_rn(c); break;
+      case M3TSZ_AGG_SUM: v = __ll2double_rn(__ldg(p.tile_isum + o)); break;
+      case M3TSZ_AGG_SUMSQ: v = __ll2double_rn(__ldg(static_cast<const int64_t *>(p.tile_sum_sq) + o)); break;
+      case M3TSZ_AGG_STDEV:
+        v = agg_stdev(c, __ll2double_rn(__ldg(static_cast<const int64_t *>(p.tile_sum_sq) + o)),
+                      __ll2double_rn(__ldg(p.tile_isum + o)));
+        break;
+      default: break;
+    }
+  } else {
+    switch (agg) {  // Gauge.ValueOf, gauge.go:144-165 (uniform switch)
+      case M3TSZ_AGG_LAST: v = __ldg(p.tile_last + o); break;
+      case M3TSZ_AGG_MIN: v = __ldg(p.tile_min + o); break;
+      case M3TSZ_AGG_MAX: v = __ldg(p.tile_max + o); break;
+      case M3TSZ_AGG_MEAN: v = c == 0 ? 0.0 : __ddiv_rn(__ldg(p.tile_sum + o), __ll2double_rn(c)); break;
+      case M3TSZ_AGG_COUNT: v = __ll2double_rn(c); break;
+      case M3TSZ_AGG_SUM: v = __ldg(p.tile_sum + o); break;
+      case M3TSZ_AGG_SUMSQ: v = __ldg(static_cast<const double *>(p.tile_sum_sq) + o); break;
+      case M3TSZ_AGG_STDEV:
+        v = agg_stdev(c, __ldg(static_cast<const double *>(p.tile_sum_sq) + o), __ldg(p.tile_sum + o));
+        break;
+      default: break;
+    }
+  }
+  return v;
+}
+
 // PACKED = false: one warp per 32-series batch, every series writes its own slot
 //   p.out + s * p.out_stride (fixed stride).
 // PACKED = true : persistent warps fetch batches from a counter, encode into a per-warp
@@ -1096,6 +1176,10 @@ __device__ __forceinline__ void xf_window(uint32_t ops, int64_t step, m3tsz_tran
 //         With a Reset op a window takes two rows: 2i its datapoint, 2i + 1 the Reset datapoint (or skipped).  The
 //         prologue loads the series' p.xf_state record (zeros without one), the epilogue saves it when the
 //         series' status is OK.
+// IN = 5: IN = 4 for an element's several aggregation types (xf_element_window): lane row r is source series
+//         r % p.tile_n_src under type r / p.tile_n_src; with an Add op the lane runs every type of the window to
+//         keep the shared sums and writes its own.  The prologue loads the series' p.xf_elem record, the epilogue
+//         writes the lane's part of the new one to p.xf_elem_out (launch_tiles_types_status commits it).
 // APPEND: encoder-set append (DESIGN.md §4.6).  Every lane continues the open encoder p.state[s] in slot p.out +
 //   s * out_stride: the prologue loads the state (leftover words into the output tile), each datapoint is checked
 //   before anything of it is written, and the epilogue flushes whole sectors and saves the state instead of
@@ -1104,8 +1188,10 @@ template <bool INT_OPT, bool PACKED, int IN, bool APPEND = false>
 __global__ void __launch_bounds__(ENC_WARPS * 32,
                                   IN >= 2 ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
     encode_kernel(const EncodeParams p, const __grid_constant__ EncTensorMaps tmaps) {
-  static_assert(!APPEND || (!PACKED && IN != 2 && IN != 4), "append mode writes its own slots from staged inputs");
-  constexpr bool TILES = IN == 2 || IN == 4;  // the tile aggregation's re-encode (IN = 4: with transformations)
+  static_assert(!APPEND || (!PACKED && IN != 2 && IN != 4 && IN != 5),
+                "append mode writes its own slots from staged inputs");
+  // the tile aggregation's re-encode (IN = 4: with transformations, IN = 5: an element's several types)
+  constexpr bool TILES = IN == 2 || IN == 4 || IN == 5;
   static_assert(IN != 3 || APPEND, "the routed input stage continues open encoders");
   extern __shared__ __align__(128) uint32_t smem[];
   const int lane = threadIdx.x & 31;
@@ -1215,6 +1301,35 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
     else
       memset(xs, 0, sizeof(*xs));
   }
+  // IN = 5 only: the lane's element record, source series and type (its slot behind the output tile)
+  XfElemSlot *xe = nullptr;
+  if constexpr (IN == 5) {
+    xe = reinterpret_cast<XfElemSlot *>(wbase + ENC_OUT_TILE_WORDS * 4) + lane;
+    bool all = false;
+    for (int k = 0; k < M3TSZ_MAX_TRANSFORMS; k++) {
+      const uint32_t op = (p.xf_ops >> (4 * k)) & 0xfu;
+      xf_reset |= op == M3TSZ_TRANSFORM_RESET;
+      all |= op == M3TSZ_TRANSFORM_ADD;
+    }
+    uint32_t ty = 0;
+    uint64_t src = sidx;
+    if (valid) {
+      ty = (uint32_t)(sidx / p.tile_n_src);
+      src = sidx - (uint64_t)ty * p.tile_n_src;
+    }
+    if (valid && p.xf_elem) {
+      const m3tsz_element_state &r = p.xf_elem[src];
+      xe->e.w = r.head;
+      xe->e.pv[0] = r.head.prev_v;
+      for (int j = 1; j < M3TSZ_MAX_ELEMENT_TYPES; j++) xe->e.pv[j] = r.prev_v_more[j - 1];
+      xe->reserved = r.reserved;
+    } else {
+      memset(xe, 0, sizeof(*xe));
+    }
+    xe->src = src;
+    xe->ty = ty;
+    xe->all = all ? 1u : 0u;
+  }
   if constexpr (APPEND) {
     if (valid) {
       n_pts = p.n_points ? p.n_points[in_s] : (uint32_t)p.points_stride;
@@ -1231,12 +1346,17 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
     }
   } else if (valid) {
     n_pts = (!TILES && p.n_points) ? p.n_points[sidx] : (uint32_t)p.points_stride;
-    if (TILES && p.tile_src_status && p.tile_src_status[sidx] != 0) n_pts = 0;  // failed source stream: no tiles
+    // failed source stream: no tiles
+    if constexpr (IN == 5) {
+      if (p.tile_src_status && p.tile_src_status[xe->src] != 0) n_pts = 0;
+    } else if (TILES && p.tile_src_status && p.tile_src_status[sidx] != 0) {
+      n_pts = 0;
+    }
     if (n_pts > p.points_stride) {
       s.err = M3TSZ_ERR_INVALID_ARG;
       n_pts = 0;
     }
-    if (IN == 4 && xf_reset) n_pts *= 2;  // two rows per window
+    if ((IN == 4 || IN == 5) && xf_reset) n_pts *= 2;  // two rows per window
     const int64_t start = p.start[sidx];
     s.prev_time = start;
     s.unit = initial_time_unit(start, p.default_unit);  // encoder.reset :268-272
@@ -1385,7 +1505,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       v_o = (uint64_t)__double_as_longlong(__ldg(p.val + o));
       return;
     }
-    if constexpr (IN == 4) {
+    if constexpr (IN == 4 || IN == 5) {
       if (xf_reset && (row & 1u)) {  // the Reset datapoint of window row / 2 (0: none, or its window was skipped)
         skip_o = xf_extra_t == 0;
         t_o = xf_extra_t;  // (value +0)
@@ -1393,44 +1513,43 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       }
       if (xf_reset) row >>= 1;
     }
-    const uint64_t o = (uint64_t)row * p.n_series + sidx;
-    if (TILES) {
+    if constexpr (IN == 5) {
+      const uint64_t o = (uint64_t)row * p.tile_n_src + xe->src;  // the lane's source series
       const int64_t c = __ldg(p.tile_count + o);
       skip_o = (c == 0);
       t_o = p.tile_start + (int64_t)(row + 1) * p.tile_step;  // the window's end boundary
       double v = 0.0;
-      if (p.metric_type == M3TSZ_METRIC_COUNTER) {
-        // Counter.ValueOf, counter.go:112-134: float64() of the int64 aggregates (uniform switch)
-        switch (p.agg_type) {
-          case M3TSZ_AGG_MIN: v = __ll2double_rn(__ldg(p.tile_imin + o)); break;
-          case M3TSZ_AGG_MAX: v = __ll2double_rn(__ldg(p.tile_imax + o)); break;
-          case M3TSZ_AGG_MEAN:
-            v = c == 0 ? 0.0 : __ddiv_rn(__ll2double_rn(__ldg(p.tile_isum + o)), __ll2double_rn(c));
-            break;
-          case M3TSZ_AGG_COUNT: v = __ll2double_rn(c); break;
-          case M3TSZ_AGG_SUM: v = __ll2double_rn(__ldg(p.tile_isum + o)); break;
-          case M3TSZ_AGG_SUMSQ: v = __ll2double_rn(__ldg(static_cast<const int64_t *>(p.tile_sum_sq) + o)); break;
-          case M3TSZ_AGG_STDEV:
-            v = agg_stdev(c, __ll2double_rn(__ldg(static_cast<const int64_t *>(p.tile_sum_sq) + o)),
-                          __ll2double_rn(__ldg(p.tile_isum + o)));
-            break;
-          default: break;
-        }
-      } else {
-        switch (p.agg_type) {  // Gauge.ValueOf, gauge.go:144-165 (uniform switch)
-          case M3TSZ_AGG_LAST: v = __ldg(p.tile_last + o); break;
-          case M3TSZ_AGG_MIN: v = __ldg(p.tile_min + o); break;
-          case M3TSZ_AGG_MAX: v = __ldg(p.tile_max + o); break;
-          case M3TSZ_AGG_MEAN: v = c == 0 ? 0.0 : __ddiv_rn(__ldg(p.tile_sum + o), __ll2double_rn(c)); break;
-          case M3TSZ_AGG_COUNT: v = __ll2double_rn(c); break;
-          case M3TSZ_AGG_SUM: v = __ldg(p.tile_sum + o); break;
-          case M3TSZ_AGG_SUMSQ: v = __ldg(static_cast<const double *>(p.tile_sum_sq) + o); break;
-          case M3TSZ_AGG_STDEV:
-            v = agg_stdev(c, __ldg(static_cast<const double *>(p.tile_sum_sq) + o), __ldg(p.tile_sum + o));
-            break;
-          default: break;
+      xf_extra_t = 0;
+      if (!skip_o) {
+        const bool counter = p.metric_type == M3TSZ_METRIC_COUNTER;
+        const uint32_t ty = xe->ty;
+        xf_element_window(
+            p.xf_ops, p.tile_step, xe->e, xe->all ? 0u : ty, xe->all ? p.tile_n_types : ty + 1, t_o,
+            [&](uint32_t i) {
+              // (o laundered per type: hoisting the eight arrays' addresses out of the loop spilled registers)
+              uint64_t oi;
+              asm volatile("mov.b64 %0, %1;" : "=l"(oi) : "l"(o));
+              return tile_value_of(p, counter, (int)((p.tile_types >> (4 * i)) & 0xfu), oi, c);
+            },
+            [&](uint32_t i, double r, int64_t extra_t) {
+              if (i == ty) {
+                v = r;
+                xf_extra_t = extra_t;
+              }
+            });
+        if (p.xf_discard_nan && xf_isnan(v)) {  // DiscardNaNAggregatedValues: nothing of this type's window
+          skip_o = true;
+          xf_extra_t = 0;
         }
       }
+      v_o = (uint64_t)__double_as_longlong(v);
+    } else if (TILES) {
+      const uint64_t o = (uint64_t)row * p.n_series + sidx;
+      const int64_t c = __ldg(p.tile_count + o);
+      skip_o = (c == 0);
+      t_o = p.tile_start + (int64_t)(row + 1) * p.tile_step;  // the window's end boundary
+      double v = 0.0;
+      v = tile_value_of(p, p.metric_type == M3TSZ_METRIC_COUNTER, p.agg_type, o, c);
       if constexpr (IN == 4) {
         xf_extra_t = 0;
         if (!skip_o) {
@@ -1803,6 +1922,23 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       // the transformation state moves on only with a written series (status OK: no source error, no CAPACITY)
       if (IN == 4 && p.xf_state && fits && s.err == 0 && !(p.tile_src_status && p.tile_src_status[sidx] != 0))
         p.xf_state[sidx] = *xs;
+      // IN = 5: this lane's part of its series' new record (launch_tiles_types_status commits it when the source and
+      // every type's row are OK).  Type 0's lane writes the element's fields and the inputs of types the call does
+      // not have; type j's lane its own input
+      if constexpr (IN == 5) {
+        if (p.xf_elem_out) {
+          m3tsz_element_state &r = p.xf_elem_out[xe->src];
+          const uint32_t ty = xe->ty;
+          if (ty == 0) {
+            r.head = xe->e.w;
+            r.head.prev_v = xe->e.pv[0];
+            for (uint32_t j = p.tile_n_types; j < M3TSZ_MAX_ELEMENT_TYPES; j++) r.prev_v_more[j - 1] = xe->e.pv[j];
+            r.reserved = xe->reserved;
+          } else {
+            r.prev_v_more[ty - 1] = xe->e.pv[ty];
+          }
+        }
+      }
     }
     __syncwarp();  // the flushes' stores to the slots are visible to the whole warp's copy below
     if (fits && total) {
@@ -1968,7 +2104,7 @@ uint64_t encode_packed_scratch_slots(uint64_t n_series) {
 }
 
 // in_mode 0: series-major inputs; 1: point-major inputs; 2: Gauge aggregates; 4: the aggregates through the
-// transformations (2 and 4: packed output only)
+// transformations; 5: an element's several types through them (2, 4 and 5: packed output only)
 cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_t stream) {
   if (p.in_mode == 2) {
     if (!p.packed) return cudaErrorInvalidValue;
@@ -1977,6 +2113,10 @@ cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_
   if (p.in_mode == 4) {
     if (!p.packed) return cudaErrorInvalidValue;
     return int_optimized ? launch_encode_one<true, true, 4>(p, stream) : launch_encode_one<false, true, 4>(p, stream);
+  }
+  if (p.in_mode == 5) {
+    if (!p.packed || p.tile_n_src == 0) return cudaErrorInvalidValue;
+    return int_optimized ? launch_encode_one<true, true, 5>(p, stream) : launch_encode_one<false, true, 5>(p, stream);
   }
   if (p.in_mode == 1) {
     if (p.packed)

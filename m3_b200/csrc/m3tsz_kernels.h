@@ -86,7 +86,7 @@ struct EncodeParams {
   unsigned long long *batch_counter;   // work counter (zero on entry)
   uint32_t align;
   // input stage (see encode_kernel): 0 series-major ts/val, 1 point-major ts/val, 2 Gauge aggregates, 4 the
-  // aggregates through the transformations
+  // aggregates through the transformations, 5 an element's several types through them
   int in_mode;
   // window-major [points_stride][n_series]; a Counter's (metric_type M3TSZ_METRIC_COUNTER) are int64
   union { const double *tile_sum; const int64_t *tile_isum; };
@@ -104,12 +104,26 @@ struct EncodeParams {
   int metric_type;        // M3TSZ_METRIC_COUNTER, or the Gauge (M3TSZ_METRIC_GAUGE, or 0)
   uint32_t *n_tiles_out;  // optional [n_series]
   // encoder-set append (launch_encode_append): per-series state in, updated in place; datapoints taken.  The tile
-  // stage with transformations (IN = 4) keeps its per-series transformation state (optional) in the same pointer.
+  // stage with transformations (IN = 4) keeps its per-series transformation state (optional) in the same pointer,
+  // and the multi-type stage (IN = 5) reads its per-series element state (optional) from it.
   union {
     m3tsz_encoder_state *state;
     m3tsz_transform_state *xf_state;
+    const m3tsz_element_state *xf_elem;
   };
-  uint32_t *n_appended;
+  // IN = 5: xf_elem_out (optional, [tile_n_src]) takes each lane's part of its series' new element record, which
+  // launch_tiles_types_status commits
+  union {
+    uint32_t *n_appended;
+    m3tsz_element_state *xf_elem_out;
+  };
+  // IN = 5 (an element's several aggregation types; after every older field, which keep their parameter offsets,
+  // and inside the alignment gap before the tensor maps, which keep theirs): the launch's n_series rows are
+  // tile_n_types * tile_n_src, row r is source series r % tile_n_src and type r / tile_n_src, type j's id is
+  // (tile_types >> 4j) & 0xf
+  uint64_t tile_n_src;
+  uint32_t tile_types;
+  uint32_t tile_n_types;
 };
 
 // an overflow record that a bucket write gave datapoints: pool record, its series, its encoder index (1..K-1)
@@ -145,7 +159,9 @@ struct RouteParams {
   RouteTouched *touched;  // [pool_capacity]
   uint32_t *n_touched;
 };
-static_assert(sizeof(EncodeParams) == 288, "the tensor maps follow EncodeParams: its size fixes their offset");
+// The tensor maps follow EncodeParams at the next 64-byte boundary of the constant bank, whose parameters start at
+// 0x210: 304 bytes is the most EncodeParams can take without moving them (and every kernel's SASS with them).
+static_assert(sizeof(EncodeParams) == 304, "the tensor maps follow EncodeParams: its size fixes their offset");
 
 uint64_t encode_packed_resident_blocks();
 // encoder sets (m3tsz_encode.cu): append runs encode_kernel's append mode over p.state / p.out (the slots)
@@ -216,6 +232,11 @@ cudaError_t launch_prom(const PromParams &p, cudaStream_t stream);
 // tile aggregation glue (m3tsz_query.cu)
 cudaError_t launch_fill_i64(int64_t *dst, int64_t v, uint64_t n, cudaStream_t stream);
 cudaError_t launch_tiles_status(const int32_t *src_status, int32_t *status, uint64_t n, cudaStream_t stream);
+// the multi-type stage's: a failed source's error goes to all n_types rows of its series; with `state`, a series
+// whose source and rows are all OK takes its new record from `scratch`
+cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status, uint64_t n, uint32_t n_types,
+                                      const m3tsz_element_state *scratch, m3tsz_element_state *state,
+                                      cudaStream_t stream);
 
 // exclusive scan of aligned lengths + gather into a packed buffer
 cudaError_t launch_compact(const uint8_t *slots, uint64_t slot_stride, const uint64_t *len,

@@ -154,4 +154,32 @@ cudaError_t launch_tiles_status(const int32_t *src_status, int32_t *status, uint
   return cudaGetLastError();
 }
 
+// The multi-type stage's status merge and state commit (one thread per source series): a failed source's error goes
+// to all n_types rows of the series; a series whose source and rows are all OK takes the record its lanes wrote to
+// `scratch` (the encode kernel's IN = 5 epilogue)
+__global__ void tiles_types_status_kernel(const int32_t *src_status, int32_t *status, uint64_t n, uint32_t n_types,
+                                          const m3tsz_element_state *scratch, m3tsz_element_state *state) {
+  const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  const int32_t e = src_status[s];
+  bool ok = e == 0;
+  for (uint32_t j = 0; j < n_types; j++) {
+    int32_t *row = status + (uint64_t)j * n + s;
+    if (e != 0)
+      *row = e;
+    else
+      ok = ok && *row == M3TSZ_OK;
+  }
+  if (state && ok) state[s] = scratch[s];
+}
+cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status, uint64_t n, uint32_t n_types,
+                                      const m3tsz_element_state *scratch, m3tsz_element_state *state,
+                                      cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  const unsigned tb = 256;
+  tiles_types_status_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, stream>>>(src_status, status, n, n_types, scratch,
+                                                                              state);
+  return cudaGetLastError();
+}
+
 }  // namespace m3tsz

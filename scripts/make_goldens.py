@@ -2,8 +2,9 @@
 """Transcribes the reference's own golden vectors for the M3TSZ path into
 tests/golden/m3tsz_goldens.json, those of the aggregator's Gauge / Counter arithmetic into
 tests/golden/m3tsz_agg_goldens.json, the buffer bucket's write tables into
-tests/golden/m3tsz_buffer_goldens.json, and the aggregator's transformations of a flushed window into
-tests/golden/m3tsz_transform_goldens.json.
+tests/golden/m3tsz_buffer_goldens.json, the aggregator's transformations of a flushed window into
+tests/golden/m3tsz_transform_goldens.json, and the flushes of an element with several aggregation types into
+tests/golden/m3tsz_element_types_goldens.json.
 
 Run in the build container only (it reads /root/reference, which does not exist
 on the GPU box):   python scripts/make_goldens.py
@@ -26,6 +27,8 @@ OUT_AGG = os.path.join(os.path.dirname(OUT), "m3tsz_agg_goldens.json")
 OUT_BUFFER = os.path.join(os.path.dirname(OUT), "m3tsz_buffer_goldens.json")
 # the transformations of a flushed window (metrics/transformation, GenericElem.processValue)
 OUT_XF = os.path.join(os.path.dirname(OUT), "m3tsz_transform_goldens.json")
+# an element's several aggregation types (GenericElem.processValue's loop over aggTypes)
+OUT_ELEM = os.path.join(os.path.dirname(OUT), "m3tsz_element_types_goldens.json")
 
 SEC = 1_000_000_000
 MS = 1_000_000
@@ -547,6 +550,30 @@ def main():
         ],
     }
 
+    # ---- an element's several aggregation types: the flushes of elem_test.go's custom-aggregation tests with the
+    # default pipeline (testAggregationTypes = {Mean, Sum}, elem_test.go:58; one value per window, resolution 10 s,
+    # windows starting at 210 s and 220 s, Consume(0) / (220 s) / (230 s)).  A case is one element: its metric type
+    # (1 Counter, 3 Gauge), its aggregation.Type ids in order, `ops` as above, and its flushes, each the non-empty
+    # windows (end, [value of every type]) and what every type writes (want[j]: type j's datapoints).
+    def types_case(name, src_line, metric_type, val):
+        return {"name": name, "src_line": src_line, "metric_type": metric_type, "agg_types": [4, 7], "ops": [],
+                "step_ns": 10 * SEC, "discard_nan": True,
+                "calls": [{"windows": [], "want": [[], []]},
+                          {"windows": [[220 * SEC, [val, val]]], "want": [[[220 * SEC, val]], [[220 * SEC, val]]]},
+                          {"windows": [[230 * SEC, [val, val]]], "want": [[[230 * SEC, val]], [[230 * SEC, val]]]}]}
+
+    elem = {
+        "src": "aggregator/aggregator/elem_test.go",
+        "cases": [
+            # testCounter.CounterVal = 1234 (elem_test.go:79-83): Mean and Sum of one value
+            types_case("TestCounterElemConsumeCustomAggregationDefaultPipeline", "aggregator/aggregator/elem_test.go:532",
+                       1, 1234.0),
+            # testGauge.GaugeVal = 123.456 (elem_test.go:89-93)
+            types_case("TestGaugeElemConsumeCustomAggregationDefaultPipeline", "aggregator/aggregator/elem_test.go:1826",
+                       3, 123.456),
+        ],
+    }
+
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f, indent=1)
@@ -560,6 +587,9 @@ def main():
     with open(OUT_XF, "w") as f:
         json.dump(xf, f, indent=1)
     print("wrote", OUT_XF)
+    with open(OUT_ELEM, "w") as f:
+        json.dump(elem, f, indent=1)
+    print("wrote", OUT_ELEM)
 
 
 if __name__ == "__main__":
