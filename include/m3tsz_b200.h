@@ -762,6 +762,38 @@ int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const
                                 uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
                                 void *stream);
 
+/* m3tsz_aggregate_tiles_types that keeps annotations, as the aggregator's flush does: the
+ * same parameters, contract and outputs, plus each window's annotation.  A window keeps the
+ * last non-empty annotation it was given (MaybeReplaceAnnotation, aggregation/common.go:47-61)
+ * and is flushed with it alone (consumeState.annotation, aggregator/generic_elem.go:567 and
+ * 915-931); nothing carries over from earlier windows or calls.  So the annotation of series s
+ * in window w is that of the last datapoint, in stream order, whose timestamp lies in window w
+ * and that carries one (an annotation marker directly before it: Current() reports it on that
+ * datapoint only); none if there is no such datapoint.  Out-of-order datapoints count for the
+ * window they fall in; datapoints outside [start_ns, start_ns + n_windows * step_ns) count for
+ * nothing.  Every datapoint a window writes carries the window's annotation, in every type's
+ * row and the Reset datapoint included; the encoder writes it only when it is non-empty and its
+ * bytes differ from the last annotation written to that row (timestamp_encoder.go:164-195), so
+ * the Reset datapoint and later windows with the same annotation add no marker.  A window that
+ * discard_nan drops writes nothing, its annotation included.
+ * Room: every annotation a row writes is a copy of a different annotation of its source stream,
+ * so a row takes at most m3tsz_encode_bound(rows) + its source stream's length; the scratch
+ * slots are sized for the longest source stream of the call (one 8-byte read back to the host).
+ * A row that does not fit gets M3TSZ_ERR_CAPACITY, never a truncated stream.
+ * Limits: a window's annotation is kept on the device as (bit offset from the stream's first
+ * bit) << 32 | length in bytes; a stream of 2^28 bytes or more, whose offsets would not fit, is
+ * already refused by the decode (M3TSZ_ERR_STREAM_TOO_LARGE on all of its rows).
+ * Sources without annotations give exactly m3tsz_aggregate_tiles_types' outputs. */
+int m3tsz_aggregate_tiles_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                    uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                    uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                    int32_t metric_type, const int32_t *agg_types, uint32_t n_types,
+                                    int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+                                    uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
+                                    uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
+                                    uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
+                                    void *stream);
+
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the
  * reference's interfaces (INTEGRATION.md §2 is that shim):

@@ -113,7 +113,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_iter_pool_create", "m3tsz_iter_pool_get", "m3tsz_iter_pool_destroy",
     "m3tsz_encoder_set_reset", "m3tsz_encoder_set_append", "m3tsz_encoder_set_stream",
     "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex", "m3tsz_encoder_set_write",
-    "m3tsz_aggregate_tiles_transform", "m3tsz_aggregate_tiles_types",
+    "m3tsz_aggregate_tiles_transform", "m3tsz_aggregate_tiles_types", "m3tsz_aggregate_tiles_annotated",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -282,6 +282,8 @@ def lib():
     L.m3tsz_aggregate_tiles_types.argtypes = [vp, po, vp, u64, vp, vp, u64, i64, i64, u32, i32, C.POINTER(C.c_int32),
                                               u32, i32, u32, vp, u64, vp, vp, vp, vp, vp, C.POINTER(C.c_int32), u32,
                                               i32, vp, vp]
+    L.m3tsz_aggregate_tiles_annotated.restype = C.c_int
+    L.m3tsz_aggregate_tiles_annotated.argtypes = L.m3tsz_aggregate_tiles_types.argtypes
     _lib = L
     return L
 

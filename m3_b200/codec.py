@@ -389,13 +389,16 @@ class BatchCodec:
 
     def aggregate_tiles_types(self, streams, offsets, start_ns, step_ns, n_windows, agg_types,
                               metric_type=capi.METRIC_GAUGE, out_unit=capi.UNIT_S, lengths=None, align=64,
-                              capacity=None, transforms=(), discard_nan=True, state: Optional[torch.Tensor] = None):
+                              capacity=None, transforms=(), discard_nan=True, state: Optional[torch.Tensor] = None,
+                              annotations=False):
         """An element with several aggregation types (m3tsz_aggregate_tiles_types): one decode + windows, then one
         stream per (type, series).  agg_types: strictly ascending aggregation.Type ids (capi.AGG_*), 1..8 of them;
         transforms / discard_nan as in aggregate_tiles, except that the Add op's sums are shared by the types, as in
         the reference's element.  state (element_state(S)) carries each series' element from one call to the next.
         Returns (PackedResult, n_tiles int32 [k, S]); the result's offsets / out_len / status are [k, S] views, row j
-        being agg_types[j]."""
+        being agg_types[j].  annotations=True (m3tsz_aggregate_tiles_annotated): every window's datapoints also carry
+        the window's annotation, that of the last datapoint in stream order inside the window that has one; the
+        default capacity then adds each source stream's length to every row's bound."""
         S = offsets.numel() - 1 if lengths is None else lengths.numel()
         dev = self.device
         types = [int(t) for t in agg_types]
@@ -403,7 +406,12 @@ class BatchCodec:
         k = len(types)
         if capacity is None:
             rows = 2 * n_windows if capi.TRANSFORM_RESET in transforms else n_windows
-            capacity = max(1, k * S * self.encode_bound(rows))
+            capacity = k * S * self.encode_bound(rows)
+            if annotations:  # a row's annotations are copies of different ones of its source stream
+                src_bytes = (int(offsets[-1].item() - offsets[0].item()) if lengths is None
+                             else int(lengths.sum().item()))
+                capacity += k * (src_bytes + 16 * S)
+            capacity = max(1, capacity)
         n = max(1, k) * S
         out = PackedResult(
             packed=torch.empty(capacity, dtype=torch.uint8, device=dev),
@@ -417,13 +425,14 @@ class BatchCodec:
             assert state.shape == (S, capi.ELEMENT_STATE_BYTES)
         types_a = (C.c_int32 * max(1, k))(*types)
         ops = (C.c_int32 * max(1, len(transforms)))(*transforms)
-        rc = capi.lib().m3tsz_aggregate_tiles_types(
+        fn = capi.lib().m3tsz_aggregate_tiles_annotated if annotations else capi.lib().m3tsz_aggregate_tiles_types
+        rc = fn(
             self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), _ptr(lengths), S,
             int(start_ns), int(step_ns), int(n_windows), int(metric_type), types_a, k, int(out_unit), int(align),
             _ptr(out.packed), out.packed.numel(), _ptr(out.offsets), _ptr(out.out_len), _ptr(out.status),
             _ptr(n_tiles), _ptr(out.total), ops, len(transforms), 1 if discard_nan else 0, _ptr(state),
             _cuda_stream_ptr(dev))
-        self.ctx.check(rc, "m3tsz_aggregate_tiles_types")
+        self.ctx.check(rc, "m3tsz_aggregate_tiles_annotated" if annotations else "m3tsz_aggregate_tiles_types")
         out.offsets = out.offsets.view(k, S)
         out.out_len = out.out_len.view(k, S)
         out.status = out.status.view(k, S)

@@ -240,13 +240,13 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
                            int64_t range_start_ns, int64_t window_ns, uint32_t n_windows, double *d_sum,
                            int64_t *d_count, double *d_min, double *d_max, double *d_last,
                            int64_t *d_last_at, bool want_last, uint32_t *d_n_points, int32_t *d_status,
-                           void *stream) {
+                           void *stream, uint64_t *d_win_ann = nullptr) {
   if (!ctx || !valid_opts(opts)) return M3TSZ_ERR_INVALID_ARG;
   if (n_series == 0) return M3TSZ_OK;
   DecodeParams p;
   if (!decode_params(opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, d_n_points, d_status, p) ||
       !d_sum || !d_count || !d_min || !d_max || window_ns <= 0 || n_windows == 0 || n_windows > 0x7fffffffu ||
-      (want_last && !d_last))
+      (want_last && !d_last) || (d_win_ann && !want_last))
     return M3TSZ_ERR_INVALID_ARG;
   // range_start + n_windows*window must not overflow int64
   if ((__int128)range_start_ns + (__int128)n_windows * (__int128)window_ns > (__int128)INT64_MAX)
@@ -268,17 +268,20 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
   p.ds_max = d_max;
   p.ds_last = d_last;
   p.ds_last_at = d_last_at;
-  CK(launch_decode(p, opts->int_optimized != 0, want_last ? 2 : 1, (cudaStream_t)stream));
+  p.ds_ann = d_win_ann;  // (mode 6: mode 2 + each window's annotation reference)
+  CK(launch_decode(p, opts->int_optimized != 0, d_win_ann ? 6 : (want_last ? 2 : 1), (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
 }
 
 // m3tsz_decode_downsample_ex: a Gauge without sumSq is downsample_impl (modes 1 / 2, today's kernels); a Gauge
-// with sumSq is mode 4, a Counter mode 5.
-int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                               uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
-                               uint64_t n_series, int64_t range_start_ns, int64_t window_ns, uint32_t n_windows,
-                               const m3tsz_downsample_outputs *o, void *stream) {
+// with sumSq is mode 4, a Counter mode 5.  With d_win_ann (the annotated tile calls' window annotation references,
+// not part of the public outputs) they are modes 6, 7 and 8.
+static int decode_downsample_ex_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                     uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                     uint64_t n_series, int64_t range_start_ns, int64_t window_ns,
+                                     uint32_t n_windows, const m3tsz_downsample_outputs *o, void *stream,
+                                     uint64_t *d_win_ann) {
   if (!ctx || !valid_opts(opts) || !o || o->reserved != 0) return M3TSZ_ERR_INVALID_ARG;
   const bool gauge = o->metric_type == M3TSZ_METRIC_GAUGE, counter = o->metric_type == M3TSZ_METRIC_COUNTER;
   if (gauge) {
@@ -288,7 +291,7 @@ int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
     if (!o->d_sum_sq)
       return downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, range_start_ns,
                              window_ns, n_windows, o->d_sum, o->d_count, o->d_min, o->d_max, o->d_last,
-                             o->d_last_at, o->d_last != nullptr, o->d_n_points, o->d_status, stream);
+                             o->d_last_at, o->d_last != nullptr, o->d_n_points, o->d_status, stream, d_win_ann);
   } else if (counter) {
     if (o->d_sum || o->d_min || o->d_max || o->d_sum_sq || o->d_last || o->d_last_at) return M3TSZ_ERR_INVALID_ARG;
   } else {
@@ -339,9 +342,18 @@ int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
       p.ds_isum_sq = (int64_t *)sc;
     }
   }
-  CK(launch_decode(p, opts->int_optimized != 0, gauge ? 4 : 5, (cudaStream_t)stream));
+  p.ds_ann = d_win_ann;
+  CK(launch_decode(p, opts->int_optimized != 0, d_win_ann ? (gauge ? 7 : 8) : (gauge ? 4 : 5), (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
+}
+
+int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                               uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                               uint64_t n_series, int64_t range_start_ns, int64_t window_ns, uint32_t n_windows,
+                               const m3tsz_downsample_outputs *o, void *stream) {
+  return decode_downsample_ex_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series,
+                                   range_start_ns, window_ns, n_windows, o, stream, nullptr);
 }
 
 int m3tsz_decode_downsample_batch(m3tsz_ctx *ctx, const m3tsz_options *opts,
@@ -661,6 +673,7 @@ struct TileTransforms {
   const int32_t *types = nullptr;
   uint32_t n_types = 0;
   m3tsz_element_state *elem_state = nullptr;
+  bool annotated = false;  // m3tsz_aggregate_tiles_annotated (multi-type stage only): each window's annotation
 };
 
 // Every tile call, after the caller checked ctx, opts, d_total_bytes, d_status, the (metric, type) pairs and the
@@ -685,7 +698,7 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   // context scratch: window-major aggregates, then series-major tiles
   const size_t wb = (size_t)n_series * n_windows * 8;
-  void *d_sum, *d_cnt, *d_min, *d_max, *d_last, *d_lat, *d_sst, *d_np, *d_es = nullptr;
+  void *d_sum, *d_cnt, *d_min, *d_max, *d_last, *d_lat, *d_sst, *d_np, *d_es = nullptr, *d_ann = nullptr;
   int rc;
   if ((rc = ensure(ctx, kSlotWinSum, wb, &d_sum))) return rc;
   if ((rc = ensure(ctx, kSlotWinCount, wb, &d_cnt))) return rc;
@@ -695,6 +708,7 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   if ((rc = ensure(ctx, kSlotWinLast, wb, &d_last))) return rc;
   if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_np))) return rc;
   if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_sst))) return rc;
+  if (xf.annotated && (rc = ensure(ctx, kSlotWinAnn, wb, &d_ann))) return rc;
   // 1. fused decode + windows: the Gauge with `last` (mode 2), + sumSq if a type is SumSq / Stdev (mode 4), or the
   //    Counter (mode 5, its int64 sum / min / max in the Gauge's slots)
   const bool multi = xf.n_types > 0;
@@ -708,7 +722,8 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   if (!sq) {
     rc = downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                          n_windows, (double *)d_sum, (int64_t *)d_cnt, (double *)d_min, (double *)d_max,
-                         (double *)d_last, (int64_t *)d_lat, true, (uint32_t *)d_np, (int32_t *)d_sst, st);
+                         (double *)d_last, (int64_t *)d_lat, true, (uint32_t *)d_np, (int32_t *)d_sst, st,
+                         (uint64_t *)d_ann);
   } else {
     if ((rc = ensure(ctx, kSlotWinSumSq, wb, &d_sq))) return rc;
     m3tsz_downsample_outputs o;
@@ -730,8 +745,8 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
     }
     o.d_n_points = (uint32_t *)d_np;
     o.d_status = (int32_t *)d_sst;
-    rc = m3tsz_decode_downsample_ex(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
-                                    step_ns, n_windows, &o, st);
+    rc = decode_downsample_ex_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
+                                   step_ns, n_windows, &o, st, (uint64_t *)d_ann);
   }
   if (rc) return rc;
   // 2. re-encode straight from the window-major aggregates (the encoder's input stage skips empty
@@ -741,7 +756,21 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   memset(&p, 0, sizeof(p));
   // (a Reset op writes up to two datapoints per window)
   const uint64_t rows = xf.reset ? 2ull * n_windows : (uint64_t)n_windows;
-  if ((rc = packed_params(ctx, n_rows, m3tsz_encode_bound(rows), align, d_packed, packed_capacity,
+  uint64_t slot_bytes = m3tsz_encode_bound(rows);
+  if (xf.annotated) {
+    // a row's annotations are copies of different annotations of its source stream: the slots also take the longest
+    // source stream of the call
+    void *d_mx = nullptr;
+    if ((rc = ensure(ctx, kSlotSrcMaxLen, 8, &d_mx))) return rc;
+    CK(cudaMemsetAsync(d_mx, 0, 8, st));
+    CK(launch_max_stream_len(d_offsets, d_lengths, n_series, streams_bytes, (unsigned long long *)d_mx, st));
+    ctx->launches++;
+    uint64_t mx = 0;
+    CK(cudaMemcpyAsync(&mx, d_mx, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    slot_bytes = (slot_bytes + mx + 15) & ~15ull;
+  }
+  if ((rc = packed_params(ctx, n_rows, slot_bytes, align, d_packed, packed_capacity,
                           d_out_offsets, d_total_bytes, st, p)))
     return rc;
   // every row's encoder starts at the tile range's start (the target block's start)
@@ -779,6 +808,12 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
     if (xf.elem_state && (rc = ensure(ctx, kSlotElementScratch, n_series * sizeof(m3tsz_element_state), &d_rec)))
       return rc;
     p.in_mode = 5;
+    if (xf.annotated) {
+      p.in_mode = 6;
+      p.tile_ann = (const uint64_t *)d_ann;
+      p.tile_src_streams = d_streams;
+      p.tile_src_off = d_offsets;
+    }
     p.xf_ops = xf.ops;
     p.xf_discard_nan = (xf.ops && xf.discard_nan) ? 1 : 0;  // (an empty list discards nothing, as tiles_ex)
     p.xf_elem = xf.elem_state;
@@ -876,15 +911,16 @@ int m3tsz_aggregate_tiles_transform(m3tsz_ctx *ctx, const m3tsz_options *opts, c
                               d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream, xf);
 }
 
-int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                                uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
-                                uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
-                                int32_t metric_type, const int32_t *agg_types, uint32_t n_types,
-                                int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
-                                uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
-                                uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
-                                uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
-                                void *stream) {
+// m3tsz_aggregate_tiles_types and m3tsz_aggregate_tiles_annotated
+static int aggregate_tiles_types_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                      uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                      uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                      int32_t metric_type, const int32_t *agg_types, uint32_t n_types,
+                                      int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+                                      uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
+                                      uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
+                                      uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
+                                      void *stream, bool annotated) {
   if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !agg_types || n_types == 0 ||
       n_types > M3TSZ_MAX_ELEMENT_TYPES)
     return M3TSZ_ERR_INVALID_ARG;
@@ -898,9 +934,40 @@ int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   xf.types = agg_types;
   xf.n_types = n_types;
   xf.elem_state = d_state;
+  xf.annotated = annotated;
   return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                               n_windows, metric_type, agg_types[0], out_unit, align, d_packed, packed_capacity,
                               d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream, xf);
+}
+
+int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                int32_t metric_type, const int32_t *agg_types, uint32_t n_types,
+                                int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+                                uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
+                                uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
+                                uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
+                                void *stream) {
+  return aggregate_tiles_types_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
+                                    step_ns, n_windows, metric_type, agg_types, n_types, out_unit, align, d_packed,
+                                    packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes,
+                                    ops, n_ops, discard_nan, d_state, stream, false);
+}
+
+int m3tsz_aggregate_tiles_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                    uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                    uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                    int32_t metric_type, const int32_t *agg_types, uint32_t n_types,
+                                    int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+                                    uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
+                                    uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
+                                    uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
+                                    void *stream) {
+  return aggregate_tiles_types_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
+                                    step_ns, n_windows, metric_type, agg_types, n_types, out_unit, align, d_packed,
+                                    packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes,
+                                    ops, n_ops, discard_nan, d_state, stream, true);
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

@@ -42,6 +42,8 @@ struct Scratch {
 //   40-47         streaming handles, under handle_mu             m3tsz_stream.cu
 //   35            element records of the multi-type tile stage   tiles (aggregate_tiles_types)
 //   48-50         route targets, touched records, their count    encoder_set_write
+//   51, 52        window annotation references, the longest     tiles (aggregate_tiles_annotated)
+//                 source stream
 enum Slot : int {
   kSlotStreams = 0,
   kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
@@ -84,7 +86,10 @@ enum Slot : int {
   kSlotRouteTarget = 48,
   kSlotRouteTouched = 49,
   kSlotRouteCount = 50,
-  kNumSlots = 51
+  // tile aggregation with annotations
+  kSlotWinAnn = 51,
+  kSlotSrcMaxLen = 52,
+  kNumSlots = 53
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

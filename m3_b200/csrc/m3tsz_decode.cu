@@ -14,6 +14,8 @@
 // Format: SURVEY.md Appendix A; reference decode path
 //   m3tsz/iterator.go:81-219, m3tsz/timestamp_iterator.go:80-326,
 //   m3tsz/float_encoder_iterator.go:105-165, istream.go:73-115.
+#include <type_traits>
+
 #include "m3tsz_common.cuh"
 #include "m3tsz_kernels.h"
 
@@ -392,6 +394,36 @@ __device__ __noinline__ bool decode_dp_slow(DecState &s, const SlowSrc src, int 
 }
 #undef M3_RD
 
+// The annotation a datapoint carries when decode_dp_slow read `count` > 1 annotation markers before it (it keeps the
+// first in *bit / *len): the last of them, as Current() reports it (readAnnotation replaces PrevAnt,
+// timestamp_iterator.go:328-356).  The slow path has checked every marker, varint and payload up to the datapoint,
+// which are annotation and time-unit markers only, so the walk reads them without checks.
+__device__ __forceinline__ void dec_last_annotation(const SlowSrc src, uint64_t wbase, uint32_t count, uint32_t *bit,
+                                                    uint32_t *len) {
+  uint32_t pos = *bit + *len * 8u;
+  for (uint32_t k = 1; k < count;) {
+    const int m = (int)((gpeek64(src, wbase, pos) >> 53) & 3u);
+    pos += kMarkerBits;
+    if (m == kMarkerTimeUnit) {
+      pos += 8;
+      continue;
+    }
+    uint64_t ux = 0;
+    for (int i = 0, shift = 0; i < 10; i++, shift += 7) {  // binary.ReadUvarint
+      const uint32_t b = (uint32_t)(gpeek64(src, wbase, pos) >> 56);
+      pos += 8;
+      ux |= shl64((uint64_t)(b & 0x7f), shift);
+      if (b < 0x80) break;
+    }
+    int64_t alen = (int64_t)(ux >> 1);
+    if (ux & 1) alen = ~alen;
+    *bit = pos;
+    *len = (uint32_t)(alen + 1);
+    pos += *len * 8u;
+    k++;
+  }
+}
+
 __device__ __forceinline__ uint32_t smem_addr(const void *p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -436,11 +468,20 @@ __device__ __forceinline__ void ring_fill(uint32_t ring_lane_addr, const uint8_t
 }
 
 // The fused-downsample modes: 1 Gauge (sum, count, min, max), 2 + last / lastAt, 4 + sumSq (the Gauge with
-// expensive aggregations), 5 Counter (int64 sum, count, min, max, sumSq).
-__host__ __device__ constexpr bool dec_ds_mode(int mode) { return mode == 1 || mode == 2 || mode == 4 || mode == 5; }
+// expensive aggregations), 5 Counter (int64 sum, count, min, max, sumSq); 6, 7, 8: modes 2, 4, 5 that also write
+// each window's annotation reference (ds_ann).
+__host__ __device__ constexpr bool dec_ds_mode(int mode) {
+  return mode == 1 || mode == 2 || mode == 4 || mode == 5 || mode == 6 || mode == 7 || mode == 8;
+}
+__host__ __device__ constexpr int dec_base_mode(int mode) {
+  return mode == 6 ? 2 : (mode == 7 ? 4 : (mode == 8 ? 5 : mode));
+}
 // 4 and 5 carry two more 64-bit accumulators than mode 2 and start from the same budget (-Xptxas -v reports no
-// spills at 96 registers)
-__host__ __device__ constexpr int dec_min_blocks(int mode) { return dec_ds_mode(mode) ? DEC_MIN_BLOCKS_DS : DEC_MIN_BLOCKS; }
+// spills at 96 registers).  6-8 add the window's annotation reference and the walk to a datapoint's last annotation:
+// at 96 registers mode 7 spilled, so they take the plain decode's 4 blocks
+__host__ __device__ constexpr int dec_min_blocks(int mode) {
+  return (dec_ds_mode(mode) && mode < 6) ? DEC_MIN_BLOCKS_DS : DEC_MIN_BLOCKS;
+}
 
 // window accumulator type: the Gauge's float64, the Counter's int64 (counter.go:31-41)
 template <bool COUNTER> struct DsVal { using T = double; };
@@ -468,6 +509,12 @@ struct DsAcc {
   int64_t last_t;    // MODE 2: lastAt / last (gauge.go:74-81)
   uint64_t last_v;
 };
+// Modes 6-8: the open window's annotation, the last one a datapoint of the window carried (MaybeReplaceAnnotation,
+// aggregation/common.go:47-61), as a packed reference (m3tsz_aggregate_tiles_annotated): 0 none
+struct DsAnn {
+  uint64_t ref;
+};
+struct DsNoAnn {};
 
 // MODE 0: plain decode (ts, value) ; 1: fused 5-tuple-less downsample (sum, count, min, max);
 // 2: downsample + last (+ lastAt scratch); 4: + sumSq; 5: Counter downsample.
@@ -480,10 +527,12 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
   // aggregations); 5: Counter (int64(value): sum, count, min, max, sumSq; no last, no NaN vote)
   // The fused-downsample and point-major kernels read the ring as 8-byte pairs; series-major decode keeps the
   // 16-byte reads (the pairs cost more shared-memory wavefronts, see the parse).
+  constexpr int BASE = dec_base_mode(MODE);
+  constexpr bool ANN = BASE != MODE;  // modes 6-8: + each window's annotation reference
   constexpr bool RING64 = (MODE != 0);
-  constexpr bool DS = dec_ds_mode(MODE), LAST = (MODE == 2 || MODE == 4), PLAIN = (MODE == 0 || MODE == 3),
+  constexpr bool DS = dec_ds_mode(MODE), LAST = (BASE == 2 || BASE == 4), PLAIN = (MODE == 0 || MODE == 3),
                  PM = (MODE == 3);
-  constexpr bool SQ = (MODE == 4), CTR = (MODE == 5);  // Gauge sumSq / Counter
+  constexpr bool SQ = (BASE == 4), CTR = (BASE == 5);  // Gauge sumSq / Counter
   using V = typename DsVal<CTR>::T;
   extern __shared__ __align__(16) uint32_t smem[];
   const int lane = threadIdx.x & 31;
@@ -570,6 +619,8 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
   acc.n_sync = 0;
   acc.last_t = 0;
   acc.last_v = 0;
+  std::conditional_t<ANN, DsAnn, DsNoAnn> wa;  // (modes 6-8 only)
+  if constexpr (ANN) wa.ref = 0;
   const int64_t range_end = p.range_start + (int64_t)p.n_windows * p.window;
   (void)range_end;
 
@@ -596,6 +647,7 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
       }
       if constexpr (SQ) p.ds_sum_sq[o] = acc.sq;
     }
+    if constexpr (ANN) p.ds_ann[o] = wa.ref;
   };
   auto ds_store_empty = [&](int32_t w) {  // NewGauge: sum 0, count 0, min/max NaN, last 0 (gauge.go:45-51)
     const uint64_t o = (uint64_t)(uint32_t)w * p.n_series + sidx;
@@ -616,8 +668,10 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
       }
       if constexpr (SQ) p.ds_sum_sq[o] = 0.0;
     }
+    if constexpr (ANN) p.ds_ann[o] = 0;
   };
   auto ds_reset = [&]() {
+    if constexpr (ANN) wa.ref = 0;
     if constexpr (CTR) {
       acc.sum = 0;
       acc.cnt = 0;
@@ -765,6 +819,8 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
       int64_t t = 0;
       uint64_t v = 0;
       bool emitted = false;
+      uint64_t dp_ann = 0;  // modes 6-8: the annotation reference this datapoint carries (slow path only)
+      (void)dp_ann;
       // ---------------- parse: the 128-bit window at the current word ----------------
       const uint32_t sh = s.pos & 31u;
       // the window = words cw .. cw+3 of the lane's ring column (16-byte cells, [quad][lane]), as the five
@@ -1041,7 +1097,18 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
           evs.count = p.event_count;
           evs.series = sidx;
           evs.pos0 = pos0;
+          if constexpr (ANN) tmp.ann_count = 0;  // (no per-series annotation output in these modes)
           const bool em = decode_dp_slow<INT_OPT>(tmp, src, p.default_unit, st, sv, &evs);
+          if constexpr (ANN) {
+            // the annotation of this datapoint, the last marker before it, as (bit offset from the stream's first
+            // bit) << 32 | length in bytes: the stream limit of 2^28 bytes keeps both in 32 bits, and a length is at
+            // least 1
+            if (em && tmp.ann_count) {
+              uint32_t abit = tmp.ann_bit, alen = tmp.ann_len;
+              if (tmp.ann_count > 1) dec_last_annotation(src, tmp.wbase, tmp.ann_count, &abit, &alen);
+              dp_ann = ((uint64_t)(abit - pos0) << 32) | alen;
+            }
+          }
           s = tmp;
           t = st;
           v = sv;
@@ -1115,6 +1182,7 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
                 }
                 if constexpr (SQ) acc.sq = p.ds_sum_sq[o];
               }
+              if constexpr (ANN) wa.ref = p.ds_ann[o];
             }
             acc.cur_w = (int32_t)nw;
             acc.w_end = p.range_start + (nw + 1) * p.window;
@@ -1122,6 +1190,8 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
           }
           acc.in_open = in_win;
           if (in_win) {
+            if constexpr (ANN)
+              if (dp_ann) wa.ref = dp_ann;  // an empty annotation keeps the window's earlier one
             // lastAt.IsZero() || timestamp.After(lastAt), gauge.go:74-81 (NaN values included)
             if (LAST && (acc.cnt == 0 || t > acc.last_t)) {
               acc.last_t = t;
@@ -1227,7 +1297,7 @@ static cudaError_t launch_one(const DecodeParams &p, cudaStream_t stream) {
 }
 
 // mode: 0 plain decode (series-major), 1 fused downsample (sum/count/min/max), 2 + last, 3 plain decode (point-major),
-// 4 fused downsample + last + sumSq, 5 fused Counter downsample
+// 4 fused downsample + last + sumSq, 5 fused Counter downsample, 6 / 7 / 8: 2 / 4 / 5 + window annotations
 cudaError_t launch_decode(const DecodeParams &p, bool int_optimized, int mode, cudaStream_t stream) {
   switch (mode) {
     case 0: return int_optimized ? launch_one<true, 0>(p, stream) : launch_one<false, 0>(p, stream);
@@ -1236,6 +1306,9 @@ cudaError_t launch_decode(const DecodeParams &p, bool int_optimized, int mode, c
     case 3: return int_optimized ? launch_one<true, 3>(p, stream) : launch_one<false, 3>(p, stream);
     case 4: return int_optimized ? launch_one<true, 4>(p, stream) : launch_one<false, 4>(p, stream);
     case 5: return int_optimized ? launch_one<true, 5>(p, stream) : launch_one<false, 5>(p, stream);
+    case 6: return int_optimized ? launch_one<true, 6>(p, stream) : launch_one<false, 6>(p, stream);
+    case 7: return int_optimized ? launch_one<true, 7>(p, stream) : launch_one<false, 7>(p, stream);
+    case 8: return int_optimized ? launch_one<true, 8>(p, stream) : launch_one<false, 8>(p, stream);
     default: return cudaErrorInvalidValue;
   }
 }

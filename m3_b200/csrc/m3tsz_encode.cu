@@ -113,7 +113,7 @@ __host__ __device__ constexpr size_t enc_warp_smem() {
   const size_t raw =
       ((IN == 0 || IN == 1) ? 2 * (size_t)enc_nstage<IN>() * (enc_in_t<IN>() * enc_in_stride<IN>()) * 8 : 0) +
       (size_t)ENC_OUT_TILE_WORDS * 4 + (enc_bulk<IN>() ? 8 * enc_nstage<IN>() : 0) +  // (+ one mbarrier per stage)
-      (IN == 4 ? 32 * sizeof(XfSlot) : 0) + (IN == 5 ? 32 * sizeof(XfElemSlot) : 0);
+      (IN == 4 ? 32 * sizeof(XfSlot) : 0) + ((IN == 5 || IN == 6) ? 32 * sizeof(XfElemSlot) : 0);
   return enc_bulk<IN>() ? ((raw + 127) & ~(size_t)127) : raw;  // tensor copies land on 128-byte boundaries
 }
 
@@ -1188,10 +1188,12 @@ template <bool INT_OPT, bool PACKED, int IN, bool APPEND = false>
 __global__ void __launch_bounds__(ENC_WARPS * 32,
                                   IN >= 2 ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
     encode_kernel(const EncodeParams p, const __grid_constant__ EncTensorMaps tmaps) {
-  static_assert(!APPEND || (!PACKED && IN != 2 && IN != 4 && IN != 5),
+  static_assert(!APPEND || (!PACKED && IN != 2 && IN != 4 && IN != 5 && IN != 6),
                 "append mode writes its own slots from staged inputs");
   // the tile aggregation's re-encode (IN = 4: with transformations, IN = 5: an element's several types)
-  constexpr bool TILES = IN == 2 || IN == 4 || IN == 5;
+  constexpr bool TILES = IN == 2 || IN == 4 || IN == 5 || IN == 6;
+  // IN = 6: IN = 5 that writes each window's annotation (p.tile_ann), read from the source streams
+  constexpr bool ELEM = IN == 5 || IN == 6, TANN = IN == 6;
   static_assert(IN != 3 || APPEND, "the routed input stage continues open encoders");
   extern __shared__ __align__(128) uint32_t smem[];
   const int lane = threadIdx.x & 31;
@@ -1303,7 +1305,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   }
   // IN = 5 only: the lane's element record, source series and type (its slot behind the output tile)
   XfElemSlot *xe = nullptr;
-  if constexpr (IN == 5) {
+  if constexpr (ELEM) {
     xe = reinterpret_cast<XfElemSlot *>(wbase + ENC_OUT_TILE_WORDS * 4) + lane;
     bool all = false;
     for (int k = 0; k < M3TSZ_MAX_TRANSFORMS; k++) {
@@ -1347,7 +1349,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
   } else if (valid) {
     n_pts = (!TILES && p.n_points) ? p.n_points[sidx] : (uint32_t)p.points_stride;
     // failed source stream: no tiles
-    if constexpr (IN == 5) {
+    if constexpr (ELEM) {
       if (p.tile_src_status && p.tile_src_status[xe->src] != 0) n_pts = 0;
     } else if (TILES && p.tile_src_status && p.tile_src_status[sidx] != 0) {
       n_pts = 0;
@@ -1356,7 +1358,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       s.err = M3TSZ_ERR_INVALID_ARG;
       n_pts = 0;
     }
-    if ((IN == 4 || IN == 5) && xf_reset) n_pts *= 2;  // two rows per window
+    if ((IN == 4 || ELEM) && xf_reset) n_pts *= 2;  // two rows per window
     const int64_t start = p.start[sidx];
     s.prev_time = start;
     s.unit = initial_time_unit(start, p.default_unit);  // encoder.reset :268-272
@@ -1505,7 +1507,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       v_o = (uint64_t)__double_as_longlong(__ldg(p.val + o));
       return;
     }
-    if constexpr (IN == 4 || IN == 5) {
+    if constexpr (IN == 4 || ELEM) {
       if (xf_reset && (row & 1u)) {  // the Reset datapoint of window row / 2 (0: none, or its window was skipped)
         skip_o = xf_extra_t == 0;
         t_o = xf_extra_t;  // (value +0)
@@ -1513,7 +1515,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       }
       if (xf_reset) row >>= 1;
     }
-    if constexpr (IN == 5) {
+    if constexpr (ELEM) {
       const uint64_t o = (uint64_t)row * p.tile_n_src + xe->src;  // the lane's source series
       const int64_t c = __ldg(p.tile_count + o);
       skip_o = (c == 0);
@@ -1670,8 +1672,36 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
     bool want_ann = false;
     uint64_t a_off = 0;
     uint32_t a_len = 0;
-    if (p.ann_series_off) {
-      if (active && ann_i < ann_end) {
+    // byte i of the annotation at a_off: the annotation inputs' bytes, or (IN = 6) the source stream's, bit-aligned
+    // at bit a_off of the batch (inside the source stream, which the decode checked: the next byte is there too
+    // whenever the annotation does not start on a byte)
+    auto ann_byte = [&](uint64_t off, uint32_t i) -> uint32_t {
+      if constexpr (TANN) {
+        const uint64_t b = off + 8ull * i;
+        const uint32_t sh = (uint32_t)(b & 7u);
+        const uint8_t *q = p.tile_src_streams + (b >> 3);
+        return sh ? (((uint32_t)q[0] << sh) | ((uint32_t)q[1] >> (8u - sh))) & 0xffu : (uint32_t)q[0];
+      } else {
+        return p.ann_bytes[off + i];
+      }
+    };
+    if (TANN || p.ann_series_off) {
+      if constexpr (TANN) {
+        // the window's annotation (every row of the window carries it, the Reset row included), rewritten only when
+        // its bytes differ from the last one written
+        if (active) {
+          const uint32_t w = xf_reset ? iter >> 1 : iter;
+          const uint64_t ref = __ldg(p.tile_ann + (uint64_t)w * p.tile_n_src + xe->src);
+          if (ref) {
+            a_off = __ldg(p.tile_src_off + xe->src) * 8ull + (ref >> 32);
+            a_len = (uint32_t)ref;
+            bool same = a_len == last_ann_len;
+            if (same && a_off != last_ann_off)
+              for (uint32_t i = 0; same && i < a_len; i++) same = ann_byte(a_off, i) == ann_byte(last_ann_off, i);
+            want_ann = !same;
+          }
+        }
+      } else if (active && ann_i < ann_end) {
         const m3tsz_annotation_entry e = p.ann_entries[ann_i];
         if (e.dp_index == iter) {
           ann_i++;
@@ -1718,7 +1748,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
             }
           }
           while (rem > 0 && s.k < (uint32_t)(ENC_OUT_W - ENC_GUARD)) {
-            put32(s, out_tile, lane, (uint32_t)p.ann_bytes[a_off + done_bytes], 8);
+            put32(s, out_tile, lane, ann_byte(a_off, done_bytes), 8);
             done_bytes++;
             rem--;
           }
@@ -1925,7 +1955,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
       // IN = 5: this lane's part of its series' new record (launch_tiles_types_status commits it when the source and
       // every type's row are OK).  Type 0's lane writes the element's fields and the inputs of types the call does
       // not have; type j's lane its own input
-      if constexpr (IN == 5) {
+      if constexpr (ELEM) {
         if (p.xf_elem_out) {
           m3tsz_element_state &r = p.xf_elem_out[xe->src];
           const uint32_t ty = xe->ty;
@@ -2104,7 +2134,8 @@ uint64_t encode_packed_scratch_slots(uint64_t n_series) {
 }
 
 // in_mode 0: series-major inputs; 1: point-major inputs; 2: Gauge aggregates; 4: the aggregates through the
-// transformations; 5: an element's several types through them (2, 4 and 5: packed output only)
+// transformations; 5: an element's several types through them; 6: 5 with the windows' annotations (2, 4, 5 and 6:
+// packed output only)
 cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_t stream) {
   if (p.in_mode == 2) {
     if (!p.packed) return cudaErrorInvalidValue;
@@ -2117,6 +2148,11 @@ cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_
   if (p.in_mode == 5) {
     if (!p.packed || p.tile_n_src == 0) return cudaErrorInvalidValue;
     return int_optimized ? launch_encode_one<true, true, 5>(p, stream) : launch_encode_one<false, true, 5>(p, stream);
+  }
+  if (p.in_mode == 6) {
+    if (!p.packed || p.tile_n_src == 0 || !p.tile_ann || !p.tile_src_streams || !p.tile_src_off)
+      return cudaErrorInvalidValue;
+    return int_optimized ? launch_encode_one<true, true, 6>(p, stream) : launch_encode_one<false, true, 6>(p, stream);
   }
   if (p.in_mode == 1) {
     if (p.packed)

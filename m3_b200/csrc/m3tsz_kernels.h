@@ -42,10 +42,13 @@ struct DecodeParams {
   // modes 4 and 5 (after every older field, which keep their parameter offsets; window-major like the above)
   double *ds_sum_sq;    // mode 4: Gauge sumSq (+ the mode 2 outputs)
   int64_t *ds_isum, *ds_imin, *ds_imax, *ds_isum_sq;  // mode 5: Counter (+ ds_count)
+  // modes 6-8 (after every older field): window-major annotation references, (bit offset of the payload from the
+  // stream's first bit) << 32 | length in bytes, 0 for a window without one
+  uint64_t *ds_ann;
 };
 
 // mode: 0 plain decode, 1 fused downsample (sum/count/min/max), 2 fused downsample + last, 3 point-major decode,
-// 4 fused downsample + last + sumSq, 5 fused Counter downsample
+// 4 fused downsample + last + sumSq, 5 fused Counter downsample; 6 / 7 / 8: modes 2 / 4 / 5 + ds_ann
 cudaError_t launch_decode(const DecodeParams &p, bool int_optimized, int mode, cudaStream_t stream);
 
 // The layout stays what it was before the tile stage's Counter and sumSq inputs: the kernel's second parameter (the
@@ -57,10 +60,18 @@ struct EncodeParams {
     const int64_t *ts;
     const void *tile_sum_sq;  // IN = 2, SumSq / Stdev: window-major sumSq, double (Gauge) or int64 (Counter)
   };
-  const double *val;
+  // IN = 6 (the multi-type stage with annotations) reads no val / n_points / annotation entries: the source streams,
+  // their offsets and the window-major annotation references of the fused decode (DecodeParams::ds_ann) share them
+  union {
+    const double *val;
+    const uint8_t *tile_src_streams;
+  };
   uint64_t n_series;
   uint64_t points_stride;
-  const uint32_t *n_points;  // optional
+  union {
+    const uint32_t *n_points;  // optional
+    const uint64_t *tile_src_off;
+  };
   const int64_t *start;
   int unit;
   // IN = 4 (tile stage with transformations): the op list, op k in bits 4k .. 4k + 3, 0 ends it (in the padding
@@ -68,7 +79,10 @@ struct EncodeParams {
   uint32_t xf_ops;
   const uint8_t *units;  // optional per-datapoint units
   const uint64_t *ann_series_off;
-  const m3tsz_annotation_entry *ann_entries;
+  union {
+    const m3tsz_annotation_entry *ann_entries;
+    const uint64_t *tile_ann;  // [points_stride][tile_n_src]
+  };
   const uint8_t *ann_bytes;
   int default_unit;
   int xf_discard_nan;  // IN = 4: a NaN result writes nothing of its window (in the padding after default_unit)
@@ -86,7 +100,8 @@ struct EncodeParams {
   unsigned long long *batch_counter;   // work counter (zero on entry)
   uint32_t align;
   // input stage (see encode_kernel): 0 series-major ts/val, 1 point-major ts/val, 2 Gauge aggregates, 4 the
-  // aggregates through the transformations, 5 an element's several types through them
+  // aggregates through the transformations, 5 an element's several types through them, 6 the same with the
+  // windows' annotations
   int in_mode;
   // window-major [points_stride][n_series]; a Counter's (metric_type M3TSZ_METRIC_COUNTER) are int64
   union { const double *tile_sum; const int64_t *tile_isum; };
@@ -232,6 +247,10 @@ cudaError_t launch_prom(const PromParams &p, cudaStream_t stream);
 // tile aggregation glue (m3tsz_query.cu)
 cudaError_t launch_fill_i64(int64_t *dst, int64_t v, uint64_t n, cudaStream_t stream);
 cudaError_t launch_tiles_status(const int32_t *src_status, int32_t *status, uint64_t n, cudaStream_t stream);
+// the longest stream of a batch (offsets + lengths, or CSR offsets) into *out (zeroed by the caller); streams the
+// decode refuses (outside the buffer, 2^28 bytes or more) are left out
+cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, uint64_t n, uint64_t streams_bytes,
+                                  unsigned long long *out, cudaStream_t stream);
 // the multi-type stage's: a failed source's error goes to all n_types rows of its series; with `state`, a series
 // whose source and rows are all OK takes its new record from `scratch`
 cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status, uint64_t n, uint32_t n_types,

@@ -182,4 +182,28 @@ cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status
   return cudaGetLastError();
 }
 
+// The longest source stream of a tile call with annotations: the bound of an annotated row adds it (one warp-wide max
+// and one atomic per warp)
+__global__ void max_stream_len_kernel(const uint64_t *offsets, const uint64_t *lengths, uint64_t n,
+                                      uint64_t streams_bytes, unsigned long long *out) {
+  const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long len = 0;
+  if (s < n) {
+    const uint64_t o0 = offsets[s], o1 = lengths ? o0 + lengths[s] : offsets[s + 1];
+    if (o1 >= o0 && o1 <= streams_bytes && o1 - o0 < (1ull << 28)) len = o1 - o0;
+  }
+  for (int d = 16; d > 0; d >>= 1) {
+    const unsigned long long o = __shfl_xor_sync(0xffffffffu, len, d);
+    len = o > len ? o : len;
+  }
+  if ((threadIdx.x & 31) == 0 && len) atomicMax(out, len);
+}
+cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, uint64_t n, uint64_t streams_bytes,
+                                  unsigned long long *out, cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  const unsigned tb = 256;
+  max_stream_len_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, stream>>>(offsets, lengths, n, streams_bytes, out);
+  return cudaGetLastError();
+}
+
 }  // namespace m3tsz

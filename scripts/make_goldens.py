@@ -29,6 +29,7 @@ OUT_BUFFER = os.path.join(os.path.dirname(OUT), "m3tsz_buffer_goldens.json")
 OUT_XF = os.path.join(os.path.dirname(OUT), "m3tsz_transform_goldens.json")
 # an element's several aggregation types (GenericElem.processValue's loop over aggTypes)
 OUT_ELEM = os.path.join(os.path.dirname(OUT), "m3tsz_element_types_goldens.json")
+OUT_ANN = os.path.join(os.path.dirname(OUT), "m3tsz_tile_annotation_goldens.json")
 
 SEC = 1_000_000_000
 MS = 1_000_000
@@ -574,6 +575,42 @@ def main():
         ],
     }
 
+    # ---- the annotation a window is flushed with (aggregation/common.go:47-61 MaybeReplaceAnnotation, called by
+    # Gauge.Update / Counter.Update; consumeState.annotation, aggregator/generic_elem.go:567): the datapoints as they
+    # reach the element, in order, and each window's annotation ("" for none).  time.Now() in the aggregation tests
+    # is a timestamp inside one window here.
+    def ann_case(name, source, metric_type, start_ns, step_ns, n_windows, dps, want):
+        return {"name": name, "source": source, "metric_type": metric_type, "start_ns": start_ns,
+                "step_ns": step_ns, "n_windows": n_windows,
+                "datapoints": [[t, v, a.hex()] for t, v, a in dps], "want_windows": [a.hex() for a in want]}
+
+    # elem_test.go:56 (10 s resolution), :120-125 (testTimestamps, testAlignedStarts), :79-83 (CounterVal 1234)
+    ts3 = [216 * SEC, 217 * SEC, 221 * SEC]
+    ann = {
+        "description": "The annotation each aggregation window keeps: the last non-empty one of its datapoints "
+                       "(aggregation/common.go:47-61, gauge.go:54-57, counter.go:77), transcribed from the "
+                       "reference's annotation tests by scripts/make_goldens.py.  datapoints: [t_ns, value, "
+                       "annotation hex] in stream order; want_windows: each window's annotation hex, \"\" for none.",
+        "cases": [
+            ann_case("TestGaugeReturnsLastNonEmptyAnnotation", "aggregator/aggregation/gauge_test.go:99-106", 3,
+                     210 * SEC, 10 * SEC, 1,
+                     [(216 * SEC, 1.1, b"first"), (217 * SEC, 2.1, b"second"), (218 * SEC, 3.1, b"")],
+                     [b"second"]),
+            ann_case("TestCounterReturnsLastNonEmptyAnnotation", "aggregator/aggregation/counter_test.go:45-52", 1,
+                     210 * SEC, 10 * SEC, 1,
+                     [(216 * SEC, 1.0, b"first"), (217 * SEC, 2.0, b"second"), (218 * SEC, 3.0, b"")],
+                     [b"second"]),
+            ann_case("TestCounterElemAddUnion", "aggregator/aggregator/elem_test.go:215-252", 1, 210 * SEC,
+                     10 * SEC, 2,
+                     [(ts3[0], 1234.0, b"\x01"), (ts3[1], 1234.0, b""), (ts3[2], 1234.0, b"\x02")],
+                     [b"\x01", b"\x02"]),
+            ann_case("TestCounterElemAddUnionWithCustomAggregation", "aggregator/aggregator/elem_test.go:254-300", 1,
+                     210 * SEC, 10 * SEC, 2,
+                     [(ts3[0], 1234.0, b"\x01"), (ts3[1], 1234.0, b""), (ts3[2], 1234.0, b"")],
+                     [b"\x01", b""]),
+        ],
+    }
+
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f, indent=1)
@@ -590,6 +627,9 @@ def main():
     with open(OUT_ELEM, "w") as f:
         json.dump(elem, f, indent=1)
     print("wrote", OUT_ELEM)
+    with open(OUT_ANN, "w") as f:
+        json.dump(ann, f, indent=1)
+    print("wrote", OUT_ANN)
 
 
 if __name__ == "__main__":
