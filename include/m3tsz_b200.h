@@ -794,6 +794,47 @@ int m3tsz_aggregate_tiles_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, c
                                     uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
                                     void *stream);
 
+/* Tile aggregation of a range inside one target block that spans many source blocks
+ * (AggregateTiles, dbnode/storage/namespace.go:1775-1786): each series has one stream per
+ * source block, and comes out as one stream per aggregation type.
+ * Addressing: segment q is [d_offsets[q], d_offsets[q] + d_lengths[q]), or, with d_lengths
+ * NULL, [d_offsets[q], d_offsets[q + 1]).  Series s is segments [d_block_off[s],
+ * d_block_off[s + 1]) (n_series + 1 entries), in the order listed (block-start order).  A
+ * series whose range decreases or runs past n_segments gets M3TSZ_ERR_INVALID_ARG on all its
+ * rows; the other series are unaffected.
+ * Each segment is decoded on its own (its own first timestamp, time unit, int / float state
+ * and annotation markers), and series s's datapoints are those of its segments, concatenated
+ * in the listed order.  From there every rule is m3tsz_aggregate_tiles_types' (annotations
+ * == 0) or m3tsz_aggregate_tiles_annotated's (annotations != 0) on that sequence: windows,
+ * out-of-order datapoints, datapoints outside the range, types, ops, discard_nan, d_state, the
+ * row layout j * n_series + s and d_n_tiles.  Equal timestamps in different segments are not
+ * deduplicated.  With one segment per series the outputs are exactly those calls' outputs.
+ * With annotations, a segment's stream writes its first annotation even when it equals the
+ * previous segment's last, so a window whose only annotated datapoint is a segment's first
+ * keeps that annotation, where one stream re-encoding the concatenation would not carry it.
+ * Errors: a decode error of any segment, the first in listed order, is the series' error on
+ * all its rows, with no output and no record saved.  An empty segment adds no datapoints, and
+ * a series with no segments, or only empty ones, has every window empty and status M3TSZ_OK
+ * (where the single-stream calls report an empty stream as M3TSZ_ERR_EOF, as the reference
+ * iterator does).
+ * Room: a row takes at most m3tsz_encode_bound(rows), plus, with annotations, the sum of its
+ * series' segment lengths; the slots are sized for the largest such sum of the call (one
+ * 8-byte read back).  A row that does not fit gets M3TSZ_ERR_CAPACITY.
+ * Limits: with annotations, a window's annotation is kept on the device as (bit offset of the
+ * payload from d_streams' first bit) << 27 | length in bytes, so a series in which a datapoint
+ * carries an annotation of 2^27 bytes or more gets M3TSZ_ERR_STREAM_TOO_LARGE on all its rows.
+ * d_block_off NULL, or any check of m3tsz_aggregate_tiles_types: M3TSZ_ERR_INVALID_ARG before
+ * any launch. */
+int m3tsz_aggregate_tiles_blocks(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                 uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                 uint64_t n_segments, const uint64_t *d_block_off, uint64_t n_series, int64_t start_ns,
+                                 int64_t step_ns, uint32_t n_windows, int32_t metric_type, const int32_t *agg_types,
+                                 uint32_t n_types, int32_t out_unit, uint32_t align, uint8_t *d_packed,
+                                 uint64_t packed_capacity, uint64_t *d_out_offsets, uint64_t *d_out_len,
+                                 int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
+                                 uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
+                                 int32_t annotations, void *stream);
+
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the
  * reference's interfaces (INTEGRATION.md §2 is that shim):

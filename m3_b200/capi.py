@@ -114,6 +114,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_encoder_set_reset", "m3tsz_encoder_set_append", "m3tsz_encoder_set_stream",
     "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex", "m3tsz_encoder_set_write",
     "m3tsz_aggregate_tiles_transform", "m3tsz_aggregate_tiles_types", "m3tsz_aggregate_tiles_annotated",
+    "m3tsz_aggregate_tiles_blocks",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -284,6 +285,10 @@ def lib():
                                               i32, vp, vp]
     L.m3tsz_aggregate_tiles_annotated.restype = C.c_int
     L.m3tsz_aggregate_tiles_annotated.argtypes = L.m3tsz_aggregate_tiles_types.argtypes
+    L.m3tsz_aggregate_tiles_blocks.restype = C.c_int
+    L.m3tsz_aggregate_tiles_blocks.argtypes = [vp, po, vp, u64, vp, vp, u64, vp, u64, i64, i64, u32, i32,
+                                               C.POINTER(C.c_int32), u32, i32, u32, vp, u64, vp, vp, vp, vp, vp,
+                                               C.POINTER(C.c_int32), u32, i32, vp, i32, vp]
     _lib = L
     return L
 

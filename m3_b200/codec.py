@@ -390,7 +390,7 @@ class BatchCodec:
     def aggregate_tiles_types(self, streams, offsets, start_ns, step_ns, n_windows, agg_types,
                               metric_type=capi.METRIC_GAUGE, out_unit=capi.UNIT_S, lengths=None, align=64,
                               capacity=None, transforms=(), discard_nan=True, state: Optional[torch.Tensor] = None,
-                              annotations=False):
+                              annotations=False, blocks: Optional[torch.Tensor] = None):
         """An element with several aggregation types (m3tsz_aggregate_tiles_types): one decode + windows, then one
         stream per (type, series).  agg_types: strictly ascending aggregation.Type ids (capi.AGG_*), 1..8 of them;
         transforms / discard_nan as in aggregate_tiles, except that the Add op's sums are shared by the types, as in
@@ -398,8 +398,13 @@ class BatchCodec:
         Returns (PackedResult, n_tiles int32 [k, S]); the result's offsets / out_len / status are [k, S] views, row j
         being agg_types[j].  annotations=True (m3tsz_aggregate_tiles_annotated): every window's datapoints also carry
         the window's annotation, that of the last datapoint in stream order inside the window that has one; the
-        default capacity then adds each source stream's length to every row's bound."""
-        S = offsets.numel() - 1 if lengths is None else lengths.numel()
+        default capacity then adds each source stream's length to every row's bound.
+        blocks (int64 [S + 1] device tensor; m3tsz_aggregate_tiles_blocks): offsets / lengths then describe segments,
+        one per (series, source block), and series s is segments blocks[s] .. blocks[s + 1] - 1, decoded one after
+        another as one datapoint sequence (fileset.read_block_range returns these inputs); with annotations the
+        default capacity adds each series' summed segment lengths."""
+        n_seg = offsets.numel() - 1 if lengths is None else lengths.numel()
+        S = n_seg if blocks is None else blocks.numel() - 1
         dev = self.device
         types = [int(t) for t in agg_types]
         transforms = [int(t) for t in transforms]
@@ -407,7 +412,13 @@ class BatchCodec:
         if capacity is None:
             rows = 2 * n_windows if capi.TRANSFORM_RESET in transforms else n_windows
             capacity = k * S * self.encode_bound(rows)
-            if annotations:  # a row's annotations are copies of different ones of its source stream
+            if annotations and blocks is not None:  # ... of different ones of its series' segments
+                seg = (offsets[1:] - offsets[:-1]) if lengths is None else lengths
+                cs = torch.cat([torch.zeros(1, dtype=torch.int64, device=seg.device), torch.cumsum(seg, 0)])
+                b = blocks.clamp(0, n_seg)
+                src_bytes = int((cs[b[1:]] - cs[b[:-1]]).clamp(min=0).sum().item())
+                capacity += k * (src_bytes + 16 * S)
+            elif annotations:  # a row's annotations are copies of different ones of its source stream
                 src_bytes = (int(offsets[-1].item() - offsets[0].item()) if lengths is None
                              else int(lengths.sum().item()))
                 capacity += k * (src_bytes + 16 * S)
@@ -425,6 +436,16 @@ class BatchCodec:
             assert state.shape == (S, capi.ELEMENT_STATE_BYTES)
         types_a = (C.c_int32 * max(1, k))(*types)
         ops = (C.c_int32 * max(1, len(transforms)))(*transforms)
+        if blocks is not None:
+            assert blocks.is_cuda and blocks.dtype == torch.int64 and blocks.is_contiguous()
+            rc = capi.lib().m3tsz_aggregate_tiles_blocks(
+                self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), _ptr(lengths),
+                n_seg, _ptr(blocks), S, int(start_ns), int(step_ns), int(n_windows), int(metric_type), types_a, k,
+                int(out_unit), int(align), _ptr(out.packed), out.packed.numel(), _ptr(out.offsets), _ptr(out.out_len),
+                _ptr(out.status), _ptr(n_tiles), _ptr(out.total), ops, len(transforms), 1 if discard_nan else 0,
+                _ptr(state), 1 if annotations else 0, _cuda_stream_ptr(dev))
+            self.ctx.check(rc, "m3tsz_aggregate_tiles_blocks")
+            return self._types_views(out, n_tiles, k, S)
         fn = capi.lib().m3tsz_aggregate_tiles_annotated if annotations else capi.lib().m3tsz_aggregate_tiles_types
         rc = fn(
             self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), _ptr(lengths), S,
@@ -433,6 +454,10 @@ class BatchCodec:
             _ptr(n_tiles), _ptr(out.total), ops, len(transforms), 1 if discard_nan else 0, _ptr(state),
             _cuda_stream_ptr(dev))
         self.ctx.check(rc, "m3tsz_aggregate_tiles_annotated" if annotations else "m3tsz_aggregate_tiles_types")
+        return self._types_views(out, n_tiles, k, S)
+
+    @staticmethod
+    def _types_views(out, n_tiles, k, S):
         out.offsets = out.offsets.view(k, S)
         out.out_len = out.out_len.view(k, S)
         out.status = out.status.view(k, S)

@@ -240,7 +240,8 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
                            int64_t range_start_ns, int64_t window_ns, uint32_t n_windows, double *d_sum,
                            int64_t *d_count, double *d_min, double *d_max, double *d_last,
                            int64_t *d_last_at, bool want_last, uint32_t *d_n_points, int32_t *d_status,
-                           void *stream, uint64_t *d_win_ann = nullptr) {
+                           void *stream, uint64_t *d_win_ann = nullptr, const uint64_t *d_block_off = nullptr,
+                           uint64_t n_segments = 0) {
   if (!ctx || !valid_opts(opts)) return M3TSZ_ERR_INVALID_ARG;
   if (n_series == 0) return M3TSZ_OK;
   DecodeParams p;
@@ -269,6 +270,8 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
   p.ds_last = d_last;
   p.ds_last_at = d_last_at;
   p.ds_ann = d_win_ann;  // (mode 6: mode 2 + each window's annotation reference)
+  p.block_off = d_block_off;
+  p.n_segments = n_segments;
   CK(launch_decode(p, opts->int_optimized != 0, d_win_ann ? 6 : (want_last ? 2 : 1), (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
@@ -276,12 +279,14 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
 
 // m3tsz_decode_downsample_ex: a Gauge without sumSq is downsample_impl (modes 1 / 2, today's kernels); a Gauge
 // with sumSq is mode 4, a Counter mode 5.  With d_win_ann (the annotated tile calls' window annotation references,
-// not part of the public outputs) they are modes 6, 7 and 8.
+// not part of the public outputs) they are modes 6, 7 and 8.  With d_block_off, over source blocks (the tile call
+// m3tsz_aggregate_tiles_blocks).
 static int decode_downsample_ex_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                                      uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
                                      uint64_t n_series, int64_t range_start_ns, int64_t window_ns,
                                      uint32_t n_windows, const m3tsz_downsample_outputs *o, void *stream,
-                                     uint64_t *d_win_ann) {
+                                     uint64_t *d_win_ann, const uint64_t *d_block_off = nullptr,
+                                     uint64_t n_segments = 0) {
   if (!ctx || !valid_opts(opts) || !o || o->reserved != 0) return M3TSZ_ERR_INVALID_ARG;
   const bool gauge = o->metric_type == M3TSZ_METRIC_GAUGE, counter = o->metric_type == M3TSZ_METRIC_COUNTER;
   if (gauge) {
@@ -291,7 +296,8 @@ static int decode_downsample_ex_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, 
     if (!o->d_sum_sq)
       return downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, range_start_ns,
                              window_ns, n_windows, o->d_sum, o->d_count, o->d_min, o->d_max, o->d_last,
-                             o->d_last_at, o->d_last != nullptr, o->d_n_points, o->d_status, stream, d_win_ann);
+                             o->d_last_at, o->d_last != nullptr, o->d_n_points, o->d_status, stream, d_win_ann,
+                             d_block_off, n_segments);
   } else if (counter) {
     if (o->d_sum || o->d_min || o->d_max || o->d_sum_sq || o->d_last || o->d_last_at) return M3TSZ_ERR_INVALID_ARG;
   } else {
@@ -343,6 +349,8 @@ static int decode_downsample_ex_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, 
     }
   }
   p.ds_ann = d_win_ann;
+  p.block_off = d_block_off;
+  p.n_segments = n_segments;
   CK(launch_decode(p, opts->int_optimized != 0, d_win_ann ? (gauge ? 7 : 8) : (gauge ? 4 : 5), (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
@@ -674,6 +682,10 @@ struct TileTransforms {
   uint32_t n_types = 0;
   m3tsz_element_state *elem_state = nullptr;
   bool annotated = false;  // m3tsz_aggregate_tiles_annotated (multi-type stage only): each window's annotation
+  // m3tsz_aggregate_tiles_blocks (multi-type stage only): offsets / lengths address n_segments segments, and series s
+  // is segments [block_off[s], block_off[s + 1])
+  const uint64_t *block_off = nullptr;
+  uint64_t n_segments = 0;
 };
 
 // Every tile call, after the caller checked ctx, opts, d_total_bytes, d_status, the (metric, type) pairs and the
@@ -723,7 +735,7 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
     rc = downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                          n_windows, (double *)d_sum, (int64_t *)d_cnt, (double *)d_min, (double *)d_max,
                          (double *)d_last, (int64_t *)d_lat, true, (uint32_t *)d_np, (int32_t *)d_sst, st,
-                         (uint64_t *)d_ann);
+                         (uint64_t *)d_ann, xf.block_off, xf.n_segments);
   } else {
     if ((rc = ensure(ctx, kSlotWinSumSq, wb, &d_sq))) return rc;
     m3tsz_downsample_outputs o;
@@ -746,7 +758,7 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
     o.d_n_points = (uint32_t *)d_np;
     o.d_status = (int32_t *)d_sst;
     rc = decode_downsample_ex_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
-                                   step_ns, n_windows, &o, st, (uint64_t *)d_ann);
+                                   step_ns, n_windows, &o, st, (uint64_t *)d_ann, xf.block_off, xf.n_segments);
   }
   if (rc) return rc;
   // 2. re-encode straight from the window-major aggregates (the encoder's input stage skips empty
@@ -759,11 +771,15 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   uint64_t slot_bytes = m3tsz_encode_bound(rows);
   if (xf.annotated) {
     // a row's annotations are copies of different annotations of its source stream: the slots also take the longest
-    // source stream of the call
+    // source stream of the call (over source blocks: the largest sum of a series' block lengths)
     void *d_mx = nullptr;
     if ((rc = ensure(ctx, kSlotSrcMaxLen, 8, &d_mx))) return rc;
     CK(cudaMemsetAsync(d_mx, 0, 8, st));
-    CK(launch_max_stream_len(d_offsets, d_lengths, n_series, streams_bytes, (unsigned long long *)d_mx, st));
+    if (xf.block_off)
+      CK(launch_max_series_blocks_len(d_offsets, d_lengths, xf.block_off, n_series, xf.n_segments, streams_bytes,
+                                      (unsigned long long *)d_mx, st));
+    else
+      CK(launch_max_stream_len(d_offsets, d_lengths, n_series, streams_bytes, (unsigned long long *)d_mx, st));
     ctx->launches++;
     uint64_t mx = 0;
     CK(cudaMemcpyAsync(&mx, d_mx, 8, cudaMemcpyDeviceToHost, st));
@@ -809,10 +825,10 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
       return rc;
     p.in_mode = 5;
     if (xf.annotated) {
-      p.in_mode = 6;
+      p.in_mode = xf.block_off ? 7 : 6;  // (7: the references hold the payload's bit offset in the whole batch)
       p.tile_ann = (const uint64_t *)d_ann;
       p.tile_src_streams = d_streams;
-      p.tile_src_off = d_offsets;
+      if (!xf.block_off) p.tile_src_off = d_offsets;
     }
     p.xf_ops = xf.ops;
     p.xf_discard_nan = (xf.ops && xf.discard_nan) ? 1 : 0;  // (an empty list discards nothing, as tiles_ex)
@@ -920,7 +936,8 @@ static int aggregate_tiles_types_impl(m3tsz_ctx *ctx, const m3tsz_options *opts,
                                       uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
                                       uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
                                       uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
-                                      void *stream, bool annotated) {
+                                      void *stream, bool annotated, const uint64_t *d_block_off = nullptr,
+                                      uint64_t n_segments = 0) {
   if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !agg_types || n_types == 0 ||
       n_types > M3TSZ_MAX_ELEMENT_TYPES)
     return M3TSZ_ERR_INVALID_ARG;
@@ -935,6 +952,8 @@ static int aggregate_tiles_types_impl(m3tsz_ctx *ctx, const m3tsz_options *opts,
   xf.n_types = n_types;
   xf.elem_state = d_state;
   xf.annotated = annotated;
+  xf.block_off = d_block_off;
+  xf.n_segments = n_segments;
   return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                               n_windows, metric_type, agg_types[0], out_unit, align, d_packed, packed_capacity,
                               d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream, xf);
@@ -968,6 +987,24 @@ int m3tsz_aggregate_tiles_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, c
                                     step_ns, n_windows, metric_type, agg_types, n_types, out_unit, align, d_packed,
                                     packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes,
                                     ops, n_ops, discard_nan, d_state, stream, true);
+}
+
+int m3tsz_aggregate_tiles_blocks(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                 uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                 uint64_t n_segments, const uint64_t *d_block_off, uint64_t n_series, int64_t start_ns,
+                                 int64_t step_ns, uint32_t n_windows, int32_t metric_type, const int32_t *agg_types,
+                                 uint32_t n_types, int32_t out_unit, uint32_t align, uint8_t *d_packed,
+                                 uint64_t packed_capacity, uint64_t *d_out_offsets, uint64_t *d_out_len,
+                                 int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
+                                 uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
+                                 int32_t annotations, void *stream) {
+  // (the block table's ranges are checked per series on the device: a bad one is that series' INVALID_ARG)
+  if (!d_block_off) return M3TSZ_ERR_INVALID_ARG;
+  return aggregate_tiles_types_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
+                                    step_ns, n_windows, metric_type, agg_types, n_types, out_unit, align, d_packed,
+                                    packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes,
+                                    ops, n_ops, discard_nan, d_state, stream, annotations != 0, d_block_off,
+                                    n_segments);
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

@@ -478,9 +478,10 @@ __host__ __device__ constexpr int dec_base_mode(int mode) {
 }
 // 4 and 5 carry two more 64-bit accumulators than mode 2 and start from the same budget (-Xptxas -v reports no
 // spills at 96 registers).  6-8 add the window's annotation reference and the walk to a datapoint's last annotation:
-// at 96 registers mode 7 spilled, so they take the plain decode's 4 blocks
-__host__ __device__ constexpr int dec_min_blocks(int mode) {
-  return (dec_ds_mode(mode) && mode < 6) ? DEC_MIN_BLOCKS_DS : DEC_MIN_BLOCKS;
+// at 96 registers mode 7 spilled, so they take the plain decode's 4 blocks.  The block loop (BLK) keeps its
+// counterpart's budget, except mode 4, whose int-optimised kernel spilled at 96 registers
+__host__ __device__ constexpr int dec_min_blocks(int mode, bool blk = false) {
+  return (dec_ds_mode(mode) && mode < 6 && !(blk && mode == 4)) ? DEC_MIN_BLOCKS_DS : DEC_MIN_BLOCKS;
 }
 
 // window accumulator type: the Gauge's float64, the Counter's int64 (counter.go:31-41)
@@ -518,8 +519,10 @@ struct DsNoAnn {};
 
 // MODE 0: plain decode (ts, value) ; 1: fused 5-tuple-less downsample (sum, count, min, max);
 // 2: downsample + last (+ lastAt scratch); 4: + sumSq; 5: Counter downsample.
-template <bool INT_OPT, int MODE>
-__global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
+// BLK (modes 2 and 4-8): the lane decodes its series' source blocks, segments [block_off[s], block_off[s + 1]), one
+// after another into the same windows (m3tsz_aggregate_tiles_blocks).
+template <bool INT_OPT, int MODE, bool BLK = false>
+__global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE, BLK))
     decode_kernel(const DecodeParams p) {
   // MODE 0: plain decode, series-major output [series][point]; 3: plain decode, point-major output
   // [point][series] (every step's 32 lanes store 32 consecutive elements: coalesced 256-byte rows);
@@ -571,27 +574,79 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
   s.ann_len = 0;
   s.ann_bit = 0;
   uint32_t pos0 = 0;
-  if (valid) {
-    const uint64_t o0 = p.offsets[sidx];
-    const uint64_t o1 = p.lengths ? o0 + p.lengths[sidx] : p.offsets[sidx + 1];
-    if (o1 < o0 || o1 > p.streams_bytes) {
-      s.err = M3TSZ_ERR_INVALID_ARG;
-    } else if (o1 - o0 >= (1ull << 28)) {
-      s.err = M3TSZ_ERR_STREAM_TOO_LARGE;
-    } else {
-      // base = the stream's first word rounded down to a DEC_FILL-word boundary
+  // BLK: the series' next segment and the end of its range
+  uint64_t blk = 0, blk_end = 0;
+  // BLK: opens the series' next non-empty segment with a fresh stream state (the window accumulator carries on);
+  // false when none is left, or with s.err on a segment outside the buffer or too large
+  auto next_block = [&]() -> bool {
+    while (blk < blk_end) {
+      const uint64_t q = blk++;
+      const uint64_t o0 = p.offsets[q];
+      const uint64_t o1 = p.lengths ? o0 + p.lengths[q] : p.offsets[q + 1];
+      if (o1 < o0 || o1 > p.streams_bytes) {
+        s.err = M3TSZ_ERR_INVALID_ARG;
+        return false;
+      }
+      if (o1 - o0 >= (1ull << 28)) {
+        s.err = M3TSZ_ERR_STREAM_TOO_LARGE;
+        return false;
+      }
+      if (o1 == o0) continue;  // an empty segment adds no datapoints
       const uint64_t w = o0 >> 2;
       s.wbase = w & ~(uint64_t)(DEC_FILL - 1);
       s.pos = (uint32_t)(w - s.wbase) * 32u + (uint32_t)(o0 & 3) * 8u;
       s.end = s.pos + (uint32_t)(o1 - o0) * 8u;
       pos0 = s.pos;
+      s.prev_time = 0;  // the block's first timestamp, unit and int / float state come from its own stream
+      s.prev_delta = 0;
+      s.prev_bits = 0;
+      s.prev_xor = 0;
+      s.int_val = 0.0;
+      s.unit_ns = 0;
+      s.sig = 0;
+      s.mult = 0;
+      s.unit = 0;
+      s.scheme = kSchemeNone;
+      s.is_float = false;
+      s.done = false;
+      s.ann_count = 0;
+      s.ann_len = 0;
+      s.ann_bit = 0;
+      return true;
+    }
+    return false;
+  };
+  if (valid) {
+    if constexpr (BLK) {
+      blk = p.block_off[sidx];
+      blk_end = p.block_off[sidx + 1];
+      if (blk > blk_end || blk_end > p.n_segments)
+        s.err = M3TSZ_ERR_INVALID_ARG;
+      else if (!next_block() && s.err == 0)
+        s.done = true;  // no datapoints: every window empty, status OK
+    } else {
+      const uint64_t o0 = p.offsets[sidx];
+      const uint64_t o1 = p.lengths ? o0 + p.lengths[sidx] : p.offsets[sidx + 1];
+      if (o1 < o0 || o1 > p.streams_bytes) {
+        s.err = M3TSZ_ERR_INVALID_ARG;
+      } else if (o1 - o0 >= (1ull << 28)) {
+        s.err = M3TSZ_ERR_STREAM_TOO_LARGE;
+      } else {
+        // base = the stream's first word rounded down to a DEC_FILL-word boundary
+        const uint64_t w = o0 >> 2;
+        s.wbase = w & ~(uint64_t)(DEC_FILL - 1);
+        s.pos = (uint32_t)(w - s.wbase) * 32u + (uint32_t)(o0 & 3) * 8u;
+        s.end = s.pos + (uint32_t)(o1 - o0) * 8u;
+        pos0 = s.pos;
+      }
     }
   }
-  if (DS && valid && s.err != 0) {  // rejected before its first datapoint: publish now (see the sink)
+  // rejected before its first datapoint (BLK: or without any): publish now (see the sink)
+  if (DS && valid && (s.err != 0 || (BLK && s.done))) {
     if (p.n_points) p.n_points[sidx] = 0;
     if (p.status) p.status[sidx] = s.err;
   }
-  const uint32_t gbase = (uint32_t)s.wbase;  // streams_bytes < 16 GiB (checked by the host)
+  uint32_t gbase = (uint32_t)s.wbase;  // streams_bytes < 16 GiB (checked by the host); BLK: the current block's
   // previous XOR's leading / trailing zero counts, kept eagerly (float path)
   int plz = 64, ptz = 0;
 
@@ -1098,15 +1153,25 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
           evs.series = sidx;
           evs.pos0 = pos0;
           if constexpr (ANN) tmp.ann_count = 0;  // (no per-series annotation output in these modes)
-          const bool em = decode_dp_slow<INT_OPT>(tmp, src, p.default_unit, st, sv, &evs);
+          bool em = decode_dp_slow<INT_OPT>(tmp, src, p.default_unit, st, sv, &evs);
           if constexpr (ANN) {
             // the annotation of this datapoint, the last marker before it, as (bit offset from the stream's first
             // bit) << 32 | length in bytes: the stream limit of 2^28 bytes keeps both in 32 bits, and a length is at
-            // least 1
+            // least 1.  BLK: (bit offset from the first bit of the batch) << kBlockAnnLenBits | length, so that the
+            // encoder needs no block table; a longer annotation rejects the series
             if (em && tmp.ann_count) {
               uint32_t abit = tmp.ann_bit, alen = tmp.ann_len;
               if (tmp.ann_count > 1) dec_last_annotation(src, tmp.wbase, tmp.ann_count, &abit, &alen);
-              dp_ann = ((uint64_t)(abit - pos0) << 32) | alen;
+              if constexpr (BLK) {
+                if (alen >> kBlockAnnLenBits) {
+                  tmp.err = M3TSZ_ERR_STREAM_TOO_LARGE;
+                  em = false;
+                } else {
+                  dp_ann = ((tmp.wbase * 32ull + abit) << kBlockAnnLenBits) | alen;
+                }
+              } else {
+                dp_ann = ((uint64_t)(abit - pos0) << 32) | alen;
+              }
             }
           }
           s = tmp;
@@ -1115,6 +1180,19 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
           emitted = em;
           lz_tz(s.prev_xor, plz, ptz);
           su_ok = (s.scheme == kScheme32 || s.scheme == kScheme64) && (s.unit >= 1 && s.unit <= 4);
+          if constexpr (BLK) {
+            // the end of a block opens the next one in this step; its first datapoint takes the slow path (prev_time
+            // 0), which reads global memory until the next refill event fills the ring from the new block (that
+            // event first waits for the copies still in flight from the old one)
+            if (s.done && s.err == 0 && next_block()) {
+              plz = 64;
+              ptz = 0;
+              su_ok = false;
+              gbase = (uint32_t)s.wbase;
+              filled = (s.pos >> 5) & ~(uint32_t)(DEC_FILL - 1);
+              safe = filled;
+            }
+          }
         }
         live = !s.done && s.err == 0;
         fast_en = live && su_ok;
@@ -1273,10 +1351,10 @@ __global__ void __launch_bounds__(DEC_WARPS * 32, dec_min_blocks(MODE))
 
 #undef M3_FIELD64
 
-template <bool INT_OPT, int MODE>
+template <bool INT_OPT, int MODE, bool BLK = false>
 static cudaError_t launch_one(const DecodeParams &p, cudaStream_t stream) {
   constexpr size_t smem = DEC_WARP_SMEM_PLAIN * DEC_WARPS;
-  cudaError_t e = cudaFuncSetAttribute(decode_kernel<INT_OPT, MODE>,
+  cudaError_t e = cudaFuncSetAttribute(decode_kernel<INT_OPT, MODE, BLK>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   // Shared-memory carveout = resident blocks x 35.8 KB; the rest of the SM's 256 KB of L1 + shared memory is
@@ -1285,20 +1363,31 @@ static cudaError_t launch_one(const DecodeParams &p, cudaStream_t stream) {
   // 7.60 / 7.58 / 8.57, fused downsample 6.36 / 5.37 / 5.00 / 4.98 / 5.78.  So: plain decode 4 blocks + 92 KB
   // of L1, fused downsample 5 blocks + 60 KB.
   constexpr int carveout_kb = dec_ds_mode(MODE) ? 196 : 164;
-  e = cudaFuncSetAttribute(decode_kernel<INT_OPT, MODE>, cudaFuncAttributePreferredSharedMemoryCarveout,
+  e = cudaFuncSetAttribute(decode_kernel<INT_OPT, MODE, BLK>, cudaFuncAttributePreferredSharedMemoryCarveout,
                            carveout_kb * 100 / 228);
   if (e != cudaSuccess) return e;
   const uint64_t per_block = (uint64_t)DEC_WARPS * 32ull;
   const uint64_t blocks = (p.n_series + per_block - 1) / per_block;
   if (blocks == 0) return cudaSuccess;
   if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
-  decode_kernel<INT_OPT, MODE><<<(unsigned)blocks, DEC_WARPS * 32, smem, stream>>>(p);
+  decode_kernel<INT_OPT, MODE, BLK><<<(unsigned)blocks, DEC_WARPS * 32, smem, stream>>>(p);
   return cudaGetLastError();
 }
 
 // mode: 0 plain decode (series-major), 1 fused downsample (sum/count/min/max), 2 + last, 3 plain decode (point-major),
 // 4 fused downsample + last + sumSq, 5 fused Counter downsample, 6 / 7 / 8: 2 / 4 / 5 + window annotations
 cudaError_t launch_decode(const DecodeParams &p, bool int_optimized, int mode, cudaStream_t stream) {
+  if (p.block_off) {  // several source blocks per series: the tile calls' modes only
+    switch (mode) {
+      case 2: return int_optimized ? launch_one<true, 2, true>(p, stream) : launch_one<false, 2, true>(p, stream);
+      case 4: return int_optimized ? launch_one<true, 4, true>(p, stream) : launch_one<false, 4, true>(p, stream);
+      case 5: return int_optimized ? launch_one<true, 5, true>(p, stream) : launch_one<false, 5, true>(p, stream);
+      case 6: return int_optimized ? launch_one<true, 6, true>(p, stream) : launch_one<false, 6, true>(p, stream);
+      case 7: return int_optimized ? launch_one<true, 7, true>(p, stream) : launch_one<false, 7, true>(p, stream);
+      case 8: return int_optimized ? launch_one<true, 8, true>(p, stream) : launch_one<false, 8, true>(p, stream);
+      default: return cudaErrorInvalidValue;
+    }
+  }
   switch (mode) {
     case 0: return int_optimized ? launch_one<true, 0>(p, stream) : launch_one<false, 0>(p, stream);
     case 1: return int_optimized ? launch_one<true, 1>(p, stream) : launch_one<false, 1>(p, stream);

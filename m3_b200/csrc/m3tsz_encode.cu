@@ -113,7 +113,7 @@ __host__ __device__ constexpr size_t enc_warp_smem() {
   const size_t raw =
       ((IN == 0 || IN == 1) ? 2 * (size_t)enc_nstage<IN>() * (enc_in_t<IN>() * enc_in_stride<IN>()) * 8 : 0) +
       (size_t)ENC_OUT_TILE_WORDS * 4 + (enc_bulk<IN>() ? 8 * enc_nstage<IN>() : 0) +  // (+ one mbarrier per stage)
-      (IN == 4 ? 32 * sizeof(XfSlot) : 0) + ((IN == 5 || IN == 6) ? 32 * sizeof(XfElemSlot) : 0);
+      (IN == 4 ? 32 * sizeof(XfSlot) : 0) + ((IN == 5 || IN == 6 || IN == 7) ? 32 * sizeof(XfElemSlot) : 0);
   return enc_bulk<IN>() ? ((raw + 127) & ~(size_t)127) : raw;  // tensor copies land on 128-byte boundaries
 }
 
@@ -1188,12 +1188,13 @@ template <bool INT_OPT, bool PACKED, int IN, bool APPEND = false>
 __global__ void __launch_bounds__(ENC_WARPS * 32,
                                   IN >= 2 ? ENC_MIN_BLOCKS_AGG : (IN == 1 ? ENC_MIN_BLOCKS_PM : ENC_MIN_BLOCKS))
     encode_kernel(const EncodeParams p, const __grid_constant__ EncTensorMaps tmaps) {
-  static_assert(!APPEND || (!PACKED && IN != 2 && IN != 4 && IN != 5 && IN != 6),
+  static_assert(!APPEND || (!PACKED && IN != 2 && IN != 4 && IN != 5 && IN != 6 && IN != 7),
                 "append mode writes its own slots from staged inputs");
   // the tile aggregation's re-encode (IN = 4: with transformations, IN = 5: an element's several types)
-  constexpr bool TILES = IN == 2 || IN == 4 || IN == 5 || IN == 6;
-  // IN = 6: IN = 5 that writes each window's annotation (p.tile_ann), read from the source streams
-  constexpr bool ELEM = IN == 5 || IN == 6, TANN = IN == 6;
+  constexpr bool TILES = IN == 2 || IN == 4 || IN == 5 || IN == 6 || IN == 7;
+  // IN = 6: IN = 5 that writes each window's annotation (p.tile_ann), read from the source streams; IN = 7: the same
+  // over several source blocks per series, whose references hold the payload's bit offset in the whole batch
+  constexpr bool ELEM = IN == 5 || IN == 6 || IN == 7, TANN = IN == 6 || IN == 7, TBLK = IN == 7;
   static_assert(IN != 3 || APPEND, "the routed input stage continues open encoders");
   extern __shared__ __align__(128) uint32_t smem[];
   const int lane = threadIdx.x & 31;
@@ -1693,8 +1694,13 @@ __global__ void __launch_bounds__(ENC_WARPS * 32,
           const uint32_t w = xf_reset ? iter >> 1 : iter;
           const uint64_t ref = __ldg(p.tile_ann + (uint64_t)w * p.tile_n_src + xe->src);
           if (ref) {
-            a_off = __ldg(p.tile_src_off + xe->src) * 8ull + (ref >> 32);
-            a_len = (uint32_t)ref;
+            if constexpr (TBLK) {
+              a_off = ref >> kBlockAnnLenBits;
+              a_len = (uint32_t)(ref & ((1ull << kBlockAnnLenBits) - 1));
+            } else {
+              a_off = __ldg(p.tile_src_off + xe->src) * 8ull + (ref >> 32);
+              a_len = (uint32_t)ref;
+            }
             bool same = a_len == last_ann_len;
             if (same && a_off != last_ann_off)
               for (uint32_t i = 0; same && i < a_len; i++) same = ann_byte(a_off, i) == ann_byte(last_ann_off, i);
@@ -2134,8 +2140,8 @@ uint64_t encode_packed_scratch_slots(uint64_t n_series) {
 }
 
 // in_mode 0: series-major inputs; 1: point-major inputs; 2: Gauge aggregates; 4: the aggregates through the
-// transformations; 5: an element's several types through them; 6: 5 with the windows' annotations (2, 4, 5 and 6:
-// packed output only)
+// transformations; 5: an element's several types through them; 6: 5 with the windows' annotations; 7: 6 over
+// several source blocks per series (2, 4, 5, 6 and 7: packed output only)
 cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_t stream) {
   if (p.in_mode == 2) {
     if (!p.packed) return cudaErrorInvalidValue;
@@ -2153,6 +2159,10 @@ cudaError_t launch_encode(const EncodeParams &p, bool int_optimized, cudaStream_
     if (!p.packed || p.tile_n_src == 0 || !p.tile_ann || !p.tile_src_streams || !p.tile_src_off)
       return cudaErrorInvalidValue;
     return int_optimized ? launch_encode_one<true, true, 6>(p, stream) : launch_encode_one<false, true, 6>(p, stream);
+  }
+  if (p.in_mode == 7) {
+    if (!p.packed || p.tile_n_src == 0 || !p.tile_ann || !p.tile_src_streams) return cudaErrorInvalidValue;
+    return int_optimized ? launch_encode_one<true, true, 7>(p, stream) : launch_encode_one<false, true, 7>(p, stream);
   }
   if (p.in_mode == 1) {
     if (p.packed)

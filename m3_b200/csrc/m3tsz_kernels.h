@@ -45,10 +45,21 @@ struct DecodeParams {
   // modes 6-8 (after every older field): window-major annotation references, (bit offset of the payload from the
   // stream's first bit) << 32 | length in bytes, 0 for a window without one
   uint64_t *ds_ann;
+  // several source blocks per series (m3tsz_aggregate_tiles_blocks; modes 2 and 4-8, after every older field):
+  // offsets / lengths address n_segments segments, and series s decodes segments [block_off[s], block_off[s + 1])
+  // one after another as one datapoint sequence.  ds_ann then holds (bit offset of the payload from the first bit of
+  // `streams`) << kBlockAnnLenBits | length in bytes.
+  const uint64_t *block_off;
+  uint64_t n_segments;
 };
 
+// The length field of a block-mode annotation reference: an annotation of 2^27 bytes or more is refused
+// (M3TSZ_ERR_STREAM_TOO_LARGE), so that a 37-bit bit offset (streams_bytes < 16 GiB) fits above it.
+constexpr int kBlockAnnLenBits = 27;
+
 // mode: 0 plain decode, 1 fused downsample (sum/count/min/max), 2 fused downsample + last, 3 point-major decode,
-// 4 fused downsample + last + sumSq, 5 fused Counter downsample; 6 / 7 / 8: modes 2 / 4 / 5 + ds_ann
+// 4 fused downsample + last + sumSq, 5 fused Counter downsample; 6 / 7 / 8: modes 2 / 4 / 5 + ds_ann.  With
+// p.block_off (modes 2 and 4-8 only) the kernels that decode several source blocks per series.
 cudaError_t launch_decode(const DecodeParams &p, bool int_optimized, int mode, cudaStream_t stream);
 
 // The layout stays what it was before the tile stage's Counter and sumSq inputs: the kernel's second parameter (the
@@ -61,7 +72,8 @@ struct EncodeParams {
     const void *tile_sum_sq;  // IN = 2, SumSq / Stdev: window-major sumSq, double (Gauge) or int64 (Counter)
   };
   // IN = 6 (the multi-type stage with annotations) reads no val / n_points / annotation entries: the source streams,
-  // their offsets and the window-major annotation references of the fused decode (DecodeParams::ds_ann) share them
+  // their offsets and the window-major annotation references of the fused decode (DecodeParams::ds_ann) share them.
+  // IN = 7 (the same over source blocks) reads the streams and the references only
   union {
     const double *val;
     const uint8_t *tile_src_streams;
@@ -251,6 +263,11 @@ cudaError_t launch_tiles_status(const int32_t *src_status, int32_t *status, uint
 // decode refuses (outside the buffer, 2^28 bytes or more) are left out
 cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, uint64_t n, uint64_t streams_bytes,
                                   unsigned long long *out, cudaStream_t stream);
+// the same over source blocks: the largest sum, over series s, of the lengths of segments [block_off[s],
+// block_off[s + 1]) (segments the decode refuses count 0, and so does a series with an invalid range)
+cudaError_t launch_max_series_blocks_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
+                                         uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
+                                         unsigned long long *out, cudaStream_t stream);
 // the multi-type stage's: a failed source's error goes to all n_types rows of its series; with `state`, a series
 // whose source and rows are all OK takes its new record from `scratch`
 cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status, uint64_t n, uint32_t n_types,

@@ -206,4 +206,36 @@ cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengt
   return cudaGetLastError();
 }
 
+// The room of an annotated tile call over source blocks: a row's annotations are copies of different annotations of
+// any of its series' blocks, so its bound adds the sum of their lengths
+__global__ void max_series_blocks_len_kernel(const uint64_t *offsets, const uint64_t *lengths,
+                                             const uint64_t *block_off, uint64_t n, uint64_t n_segments,
+                                             uint64_t streams_bytes, unsigned long long *out) {
+  const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long len = 0;
+  if (s < n) {
+    const uint64_t q0 = block_off[s], q1 = block_off[s + 1];
+    if (q0 <= q1 && q1 <= n_segments) {
+      for (uint64_t q = q0; q < q1; q++) {
+        const uint64_t o0 = offsets[q], o1 = lengths ? o0 + lengths[q] : offsets[q + 1];
+        if (o1 >= o0 && o1 <= streams_bytes && o1 - o0 < (1ull << 28)) len += o1 - o0;
+      }
+    }
+  }
+  for (int d = 16; d > 0; d >>= 1) {
+    const unsigned long long o = __shfl_xor_sync(0xffffffffu, len, d);
+    len = o > len ? o : len;
+  }
+  if ((threadIdx.x & 31) == 0 && len) atomicMax(out, len);
+}
+cudaError_t launch_max_series_blocks_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
+                                         uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
+                                         unsigned long long *out, cudaStream_t stream) {
+  if (n_series == 0) return cudaSuccess;
+  const unsigned tb = 256;
+  max_series_blocks_len_kernel<<<(unsigned)((n_series + tb - 1) / tb), tb, 0, stream>>>(
+      offsets, lengths, block_off, n_series, n_segments, streams_bytes, out);
+  return cudaGetLastError();
+}
+
 }  // namespace m3tsz

@@ -315,3 +315,77 @@ def decode_fileset(codec, fs: FilesetData, max_points: int, verify_checksums: bo
                                             expected=torch.from_numpy(fs.data_checksums.view(np.int32)).to(dev))
     res = codec.decode(d_data[:nbytes], d_off, max_points, lengths=d_len, want_events=want_events)
     return res, status
+
+
+# ------------------------------------------------------------------ a block range (tile aggregation)
+@dataclass
+class BlockRange:
+    """The inputs of m3tsz_aggregate_tiles_blocks for a range of source blocks: `data` holds the blocks' data files,
+    each at a 16-byte-aligned offset; segment q is data[offsets[q]: offsets[q] + sizes[q]] with the expected Adler-32
+    data_checksums[q]; series s (ids[s], in ID order) is segments block_off[s] .. block_off[s + 1] - 1, one per block
+    that lists the series, in block order."""
+    block_starts: List[int]
+    volumes: List[int]
+    ids: List[bytes]
+    tags: List[bytes]           # from the last block that lists the series
+    data: np.ndarray            # uint8
+    offsets: np.ndarray         # int64 [n_segments]
+    sizes: np.ndarray           # int64 [n_segments]
+    data_checksums: np.ndarray  # uint32 [n_segments]
+    block_off: np.ndarray       # int64 [n_series + 1]
+
+
+def latest_volume(prefix: str, namespace: str, shard: int, block_start_ns: int) -> int:
+    """The highest volume index of a block that has a checkpoint file (a complete volume)."""
+    d = os.path.dirname(fileset_path(prefix, namespace, shard, block_start_ns, 0, "checkpoint"))
+    head = "fileset-%d-" % block_start_ns
+    vols = []
+    for f in os.listdir(d) if os.path.isdir(d) else ():
+        if f.startswith(head) and f.endswith("-checkpoint.db"):
+            v = f[len(head):-len("-checkpoint.db")]
+            if v.isdigit():
+                vols.append(int(v))
+    if not vols:
+        raise FileNotFoundError("fileset: no complete volume of block %d in %s" % (block_start_ns, d))
+    return max(vols)
+
+
+def read_block_range(prefix: str, namespace: str, shard: int, block_starts: Sequence[int],
+                     volumes: Optional[Sequence[int]] = None) -> BlockRange:
+    """Reads one volume per source block (default: each block's latest complete volume) and lays the blocks out as
+    m3tsz_aggregate_tiles_blocks reads them: the union of the series IDs in ID order, and for each series one
+    segment per block that lists it, in the order of `block_starts`.  The data files are copied as they are; the
+    caller uploads `data` and verifies the segments with BatchCodec.segment_checksums against data_checksums."""
+    block_starts = [int(b) for b in block_starts]
+    if volumes is None:
+        volumes = [latest_volume(prefix, namespace, shard, b) for b in block_starts]
+    volumes = [int(v) for v in volumes]
+    if len(volumes) != len(block_starts):
+        raise ValueError("fileset: one volume per block")
+    sets = [read_fileset(prefix, namespace, shard, b, v) for b, v in zip(block_starts, volumes)]
+    base, pos = [], 0
+    for fs in sets:
+        pos = (pos + 15) & ~15
+        base.append(pos)
+        pos += int(fs.data.shape[0])
+    data = np.zeros((pos + 15) & ~15, dtype=np.uint8)
+    for b, fs in zip(base, sets):
+        data[b: b + fs.data.shape[0]] = fs.data
+    where = [{id_: k for k, id_ in enumerate(fs.ids)} for fs in sets]
+    ids = sorted(set().union(*where)) if where else []
+    tags, offsets, sizes, checks, block_off = [], [], [], [], [0]
+    for id_ in ids:
+        tag = b""
+        for j, fs in enumerate(sets):
+            k = where[j].get(id_)
+            if k is None:
+                continue
+            offsets.append(base[j] + int(fs.offsets[k]))
+            sizes.append(int(fs.sizes[k]))
+            checks.append(int(fs.data_checksums[k]))
+            tag = fs.tags[k]
+        tags.append(tag)
+        block_off.append(len(offsets))
+    return BlockRange(block_starts, volumes, ids, tags, data, np.array(offsets, dtype=np.int64),
+                      np.array(sizes, dtype=np.int64), np.array(checks, dtype=np.uint32),
+                      np.array(block_off, dtype=np.int64))

@@ -2,7 +2,8 @@
 """Checks that two builds compiled every batch encode_kernel and every decode_kernel instantiation to the same SASS,
 instruction for instruction (cuobjdump -sass; addresses and encodings dropped).  The encoder sets added a fourth
 template argument, APPEND, to encode_kernel: an old build's <INT_OPT, PACKED, IN> is compared with a new build's
-<INT_OPT, PACKED, IN, false>.  decode_kernel<INT_OPT, MODE> is compared by name.  Instantiations only one build has
+<INT_OPT, PACKED, IN, false>.  decode_kernel<INT_OPT, MODE> is compared by name; the source-block loop added a third
+argument, BLK, so an old build's <INT_OPT, MODE> is compared with a new build's <INT_OPT, MODE, false>.  Instantiations only one build has
 (the append mode, new decode modes) are listed, not compared.
 
     python scripts/compare_encode_sass.py OLD.(o|so) NEW.(o|so)     # exit code 1 on any difference
@@ -28,7 +29,7 @@ def kernels(path):
                 cur = re.sub(r"(encode_kernelILb[01]ELb[01]ELi[0-9]+E)Lb0E", r"\1", name)
                 out[cur] = []
             elif "decode_kernel" in name:
-                cur = name
+                cur = re.sub(r"(decode_kernelILb[01]ELi[0-9]+E)Lb0E", r"\1", name)
                 out[cur] = []
             continue
         m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;", line)
