@@ -835,6 +835,62 @@ int m3tsz_aggregate_tiles_blocks(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
                                  uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
                                  int32_t annotations, void *stream);
 
+/* Tile aggregation through a rollup (the pipeline "transformations, Rollup, remainder" of
+ * newParsedPipeline, aggregator/elem_base.go:682-752): each group's source series are folded
+ * into one element per group, which writes one stream per rollup type.
+ * Sources: as in m3tsz_aggregate_tiles_blocks with d_block_off; with d_block_off NULL, one
+ * stream per series (n_segments must then equal n_series).  Every source series is one element
+ * of (metric_type, src_type): its non-empty windows' values Gauge/Counter.ValueOf(src_type)
+ * run through pre_ops (d_src_state [n_series], optional, carries the chain from call to call)
+ * and are forwarded with the window's end as timestamp; only the value is forwarded (a Reset
+ * op here forwards no extra datapoint, generic_elem.go:912-937).
+ * Groups: group g is the sources d_members[d_group_off[g] .. d_group_off[g + 1]) (n_groups + 1
+ * offsets, n_members members), folded in that listed order: a source may be in several groups,
+ * in none, or twice in one.  Window w of group g takes every forwarded value of window w of
+ * its members, all at one timestamp, through AddUnique (generic_elem.go:246-281):
+ *   - Gauge: Gauge.Update (gauge.go:74-101); Last is the first member's value, count counts
+ *     NaNs, sum / min / max / sumSq skip them, min and max keep the first of +-0;
+ *   - Counter: Counter.Update(int64(value)) with amd64's conversion (NaN and out of range give
+ *     MinInt64), int64 sum / sumSq that wrap.
+ * From there the group is the element of m3tsz_aggregate_tiles_types with rollup_types (1..8,
+ * strictly ascending, each valid for metric_type), post_ops and d_group_state [n_groups]
+ * (optional): output row j * n_groups + g is group g under rollup_types[j], with the tile
+ * timestamps of the other calls (start_ns + (w + 1) * step_ns).  A window that no member
+ * forwarded a value to writes nothing.
+ * discard_nan (DiscardNaNAggregatedValues) applies on both sides whether or not that side
+ * has ops, as processValue does (generic_elem.go:892-894): a source window whose value is NaN
+ * after pre_ops is not forwarded (so it adds nothing to the group's window, Count included),
+ * and a rollup row value that is NaN after post_ops is not written.  (The single-element tile
+ * calls discard only with ops, to keep m3tsz_aggregate_tiles_ex's bytes.)
+ * Statuses: d_status / d_n_tiles / d_out_offsets / d_out_len have n_rollup_types * n_groups
+ * entries.  A group whose range decreases or runs past n_members, or that lists a source index
+ * >= n_series, gets M3TSZ_ERR_INVALID_ARG on its rows; a member that fails to decode gives its
+ * error to every group that lists it (the first failing member in listed order).  A group
+ * without members, or without values, writes empty rows with M3TSZ_OK.  d_src_status
+ * (optional, [n_series]) takes each source's decode status.  Room: a row takes at most
+ * m3tsz_encode_bound(n_windows), twice that with a Reset in post_ops; a row that does not fit
+ * gets M3TSZ_ERR_CAPACITY.
+ * Records: a group's record is saved when its rows are all OK and all its members decoded; a
+ * source's when it decoded and every group that lists it was saved (a source in no group: when
+ * it decoded).  So re-running exactly the failed groups with their members gives the result of
+ * one unstopped call, and consecutive calls over a split window range give one call's bytes.
+ * A rollup in post_ops (a chained rollup) is not taken: run the next level as another call.
+ * Invalid metric / source type pair, type list, op lists (parse as in
+ * m3tsz_aggregate_tiles_transform), or NULL d_group_off / d_members where needed:
+ * M3TSZ_ERR_INVALID_ARG before any launch. */
+int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                 uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                 uint64_t n_segments, const uint64_t *d_block_off, uint64_t n_series, int64_t start_ns,
+                                 int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t src_type,
+                                 const int32_t *pre_ops, uint32_t n_pre_ops, const uint64_t *d_group_off,
+                                 const uint32_t *d_members, uint64_t n_members, uint64_t n_groups,
+                                 const int32_t *rollup_types, uint32_t n_rollup_types, const int32_t *post_ops,
+                                 uint32_t n_post_ops, int32_t discard_nan, m3tsz_transform_state *d_src_state,
+                                 m3tsz_element_state *d_group_state, int32_t out_unit, uint32_t align,
+                                 uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                                 uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
+                                 int32_t *d_src_status, void *stream);
+
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the
  * reference's interfaces (INTEGRATION.md §2 is that shim):

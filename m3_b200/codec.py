@@ -463,6 +463,61 @@ class BatchCodec:
         out.status = out.status.view(k, S)
         return out, n_tiles.view(k, S)
 
+    def aggregate_tiles_rollup(self, streams, offsets, start_ns, step_ns, n_windows, src_type, group_off, members,
+                               rollup_types, metric_type=capi.METRIC_GAUGE, pre_transforms=(), post_transforms=(),
+                               discard_nan=True, src_state: Optional[torch.Tensor] = None,
+                               group_state: Optional[torch.Tensor] = None, lengths=None,
+                               blocks: Optional[torch.Tensor] = None, capacity=None, out_unit=capi.UNIT_S, align=64):
+        """Tile aggregation through a rollup (m3tsz_aggregate_tiles_rollup): every source series is an element of
+        (metric_type, src_type) whose window values run through pre_transforms and are forwarded; group g is the
+        sources members[group_off[g] .. group_off[g + 1]) (int64 [G + 1] and int32 [n] device tensors), whose
+        forwarded values are folded in that order into one element per group with rollup_types (strictly ascending,
+        1..8) and post_transforms.  src_state (transform_state(S)) and group_state (element_state(G)) carry the
+        chains from call to call.  offsets / lengths / blocks address the sources as in aggregate_tiles_types.
+        Returns (PackedResult with [k, G] views, n_tiles int32 [k, G], source statuses int32 [S])."""
+        n_seg = offsets.numel() - 1 if lengths is None else lengths.numel()
+        S = n_seg if blocks is None else blocks.numel() - 1
+        assert group_off.numel() >= 1, "group_off has G + 1 entries"
+        G = group_off.numel() - 1
+        dev = self.device
+        types = [int(t) for t in rollup_types]
+        pre = [int(t) for t in pre_transforms]
+        post = [int(t) for t in post_transforms]
+        k = len(types)
+        if capacity is None:
+            rows = 2 * n_windows if capi.TRANSFORM_RESET in post else n_windows
+            capacity = max(1, k * G * self.encode_bound(rows))
+        n = k * G
+        out = PackedResult(
+            packed=torch.empty(capacity, dtype=torch.uint8, device=dev),
+            offsets=torch.empty(n, dtype=torch.int64, device=dev),
+            out_len=torch.empty(n, dtype=torch.int64, device=dev),
+            status=torch.empty(n, dtype=torch.int32, device=dev),
+            total=torch.zeros(1, dtype=torch.int64, device=dev))
+        n_tiles = torch.empty(n, dtype=torch.int32, device=dev)
+        src_status = torch.empty(max(1, S), dtype=torch.int32, device=dev)
+        assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
+        assert members.is_cuda and members.dtype == torch.int32 and members.is_contiguous()
+        if blocks is not None:
+            assert blocks.is_cuda and blocks.dtype == torch.int64 and blocks.is_contiguous()
+        if src_state is not None:
+            assert src_state.is_cuda and src_state.is_contiguous() and src_state.dtype == torch.uint8
+            assert src_state.shape == (S, capi.TRANSFORM_STATE_BYTES)
+        if group_state is not None:
+            assert group_state.is_cuda and group_state.is_contiguous() and group_state.dtype == torch.uint8
+            assert group_state.shape == (G, capi.ELEMENT_STATE_BYTES)
+        i32s = lambda xs: (C.c_int32 * max(1, len(xs)))(*xs)
+        rc = capi.lib().m3tsz_aggregate_tiles_rollup(
+            self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), _ptr(lengths),
+            n_seg, _ptr(blocks), S, int(start_ns), int(step_ns), int(n_windows), int(metric_type), int(src_type),
+            i32s(pre), len(pre), _ptr(group_off), _ptr(members), members.numel(), G, i32s(types), k, i32s(post),
+            len(post), 1 if discard_nan else 0, _ptr(src_state), _ptr(group_state), int(out_unit), int(align),
+            _ptr(out.packed), out.packed.numel(), _ptr(out.offsets), _ptr(out.out_len), _ptr(out.status),
+            _ptr(n_tiles), _ptr(out.total), _ptr(src_status), _cuda_stream_ptr(dev))
+        self.ctx.check(rc, "m3tsz_aggregate_tiles_rollup")
+        out, n_tiles = self._types_views(out, n_tiles, k, G)
+        return out, n_tiles, src_status[:S]
+
     def element_state(self, n_series: int) -> torch.Tensor:
         """A zeroed m3tsz_element_state per series (uint8 [S, 160]): every series a new element, for
         aggregate_tiles_types(..., state=...)."""

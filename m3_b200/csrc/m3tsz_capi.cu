@@ -688,6 +688,80 @@ struct TileTransforms {
   uint64_t n_segments = 0;
 };
 
+// The window-major aggregates of a tile call's fused decode, in context scratch ([n_windows][n_series] each)
+struct TileWindows {
+  void *sum = nullptr, *cnt = nullptr, *min = nullptr, *max = nullptr, *last = nullptr, *lat = nullptr;
+  void *sst = nullptr, *np = nullptr, *sq = nullptr, *ann = nullptr;
+};
+
+// Step 1 of every tile call: the fused decode + windows of the types' metric: the Gauge with `last` (mode 2), + sumSq
+// if a type is SumSq / Stdev (mode 4), or the Counter (mode 5, its int64 sum / min / max in the Gauge's slots);
+// `annotated`: + each window's annotation reference (modes 6-8).
+static int tiles_decode(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams, uint64_t streams_bytes,
+                        const uint64_t *d_offsets, const uint64_t *d_lengths, uint64_t n_series, int64_t start_ns,
+                        int64_t step_ns, uint32_t n_windows, bool counter, const int32_t *types, uint32_t n_types,
+                        bool annotated, const uint64_t *block_off, uint64_t n_segments, cudaStream_t st,
+                        TileWindows &w) {
+  const size_t wb = (size_t)n_series * n_windows * 8;
+  int rc;
+  if ((rc = ensure(ctx, kSlotWinSum, wb, &w.sum))) return rc;
+  if ((rc = ensure(ctx, kSlotWinCount, wb, &w.cnt))) return rc;
+  if ((rc = ensure(ctx, kSlotWinMin, wb, &w.min))) return rc;
+  if ((rc = ensure(ctx, kSlotWinMax, wb, &w.max))) return rc;
+  if ((rc = ensure(ctx, kSlotWinLastAt, wb, &w.lat))) return rc;
+  if ((rc = ensure(ctx, kSlotWinLast, wb, &w.last))) return rc;
+  if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &w.np))) return rc;
+  if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &w.sst))) return rc;
+  if (annotated && (rc = ensure(ctx, kSlotWinAnn, wb, &w.ann))) return rc;
+  bool sq = counter;
+  for (uint32_t j = 0; j < n_types; j++) sq |= types[j] == M3TSZ_AGG_SUMSQ || types[j] == M3TSZ_AGG_STDEV;
+  if (!sq)
+    return downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                           n_windows, (double *)w.sum, (int64_t *)w.cnt, (double *)w.min, (double *)w.max,
+                           (double *)w.last, (int64_t *)w.lat, true, (uint32_t *)w.np, (int32_t *)w.sst, st,
+                           (uint64_t *)w.ann, block_off, n_segments);
+  if ((rc = ensure(ctx, kSlotWinSumSq, wb, &w.sq))) return rc;
+  m3tsz_downsample_outputs o;
+  memset(&o, 0, sizeof(o));
+  o.metric_type = counter ? M3TSZ_METRIC_COUNTER : M3TSZ_METRIC_GAUGE;
+  o.d_count = (int64_t *)w.cnt;
+  if (counter) {
+    o.d_counter_sum = (int64_t *)w.sum;
+    o.d_counter_min = (int64_t *)w.min;
+    o.d_counter_max = (int64_t *)w.max;
+    o.d_counter_sum_sq = (int64_t *)w.sq;
+  } else {
+    o.d_sum = (double *)w.sum;
+    o.d_min = (double *)w.min;
+    o.d_max = (double *)w.max;
+    o.d_sum_sq = (double *)w.sq;
+    o.d_last = (double *)w.last;
+    o.d_last_at = (int64_t *)w.lat;
+  }
+  o.d_n_points = (uint32_t *)w.np;
+  o.d_status = (int32_t *)w.sst;
+  return decode_downsample_ex_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
+                                   step_ns, n_windows, &o, st, (uint64_t *)w.ann, block_off, n_segments);
+}
+
+// The window aggregates of a tile call as the tile stages read them: window-major [n_windows][n_src] (IN = 2 / 4
+// read n_src = p.n_series, the multi-type stage p.tile_n_src)
+static void tile_inputs(EncodeParams &p, bool counter, void *sum, void *cnt, void *min, void *max, void *last,
+                        void *sq) {
+  p.tile_count = (const int64_t *)cnt;
+  if (counter) {
+    p.tile_isum = (const int64_t *)sum;
+    p.tile_imin = (const int64_t *)min;
+    p.tile_imax = (const int64_t *)max;
+  } else {
+    p.tile_sum = (const double *)sum;
+    p.tile_min = (const double *)min;
+    p.tile_max = (const double *)max;
+    p.tile_last = (const double *)last;
+  }
+  p.tile_sum_sq = sq;  // (NULL unless SumSq / Stdev / Counter)
+}
+
 // Every tile call, after the caller checked ctx, opts, d_total_bytes, d_status, the (metric, type) pairs and the
 // transformation list (xf.ops == 0: none, the stage of m3tsz_aggregate_tiles_ex).  One decode + windows serves every
 // type of xf.types; output row j * n_series + s is series s, type j.
@@ -709,58 +783,19 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   // context scratch: window-major aggregates, then series-major tiles
-  const size_t wb = (size_t)n_series * n_windows * 8;
-  void *d_sum, *d_cnt, *d_min, *d_max, *d_last, *d_lat, *d_sst, *d_np, *d_es = nullptr, *d_ann = nullptr;
+  void *d_es = nullptr;
   int rc;
-  if ((rc = ensure(ctx, kSlotWinSum, wb, &d_sum))) return rc;
-  if ((rc = ensure(ctx, kSlotWinCount, wb, &d_cnt))) return rc;
-  if ((rc = ensure(ctx, kSlotWinMin, wb, &d_min))) return rc;
-  if ((rc = ensure(ctx, kSlotWinMax, wb, &d_max))) return rc;
-  if ((rc = ensure(ctx, kSlotWinLastAt, wb, &d_lat))) return rc;
-  if ((rc = ensure(ctx, kSlotWinLast, wb, &d_last))) return rc;
-  if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_np))) return rc;
-  if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_sst))) return rc;
-  if (xf.annotated && (rc = ensure(ctx, kSlotWinAnn, wb, &d_ann))) return rc;
-  // 1. fused decode + windows: the Gauge with `last` (mode 2), + sumSq if a type is SumSq / Stdev (mode 4), or the
-  //    Counter (mode 5, its int64 sum / min / max in the Gauge's slots)
+  // 1. fused decode + windows (one decode for all the types)
   const bool multi = xf.n_types > 0;
   const uint32_t n_types = multi ? xf.n_types : 1u;
   const int32_t *types = multi ? xf.types : &agg_type;
   const uint64_t n_rows = (uint64_t)n_types * n_series;
   const bool counter = metric_type == M3TSZ_METRIC_COUNTER;
-  bool sq = counter;
-  for (uint32_t j = 0; j < n_types; j++) sq |= types[j] == M3TSZ_AGG_SUMSQ || types[j] == M3TSZ_AGG_STDEV;
-  void *d_sq = nullptr;
-  if (!sq) {
-    rc = downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                         n_windows, (double *)d_sum, (int64_t *)d_cnt, (double *)d_min, (double *)d_max,
-                         (double *)d_last, (int64_t *)d_lat, true, (uint32_t *)d_np, (int32_t *)d_sst, st,
-                         (uint64_t *)d_ann, xf.block_off, xf.n_segments);
-  } else {
-    if ((rc = ensure(ctx, kSlotWinSumSq, wb, &d_sq))) return rc;
-    m3tsz_downsample_outputs o;
-    memset(&o, 0, sizeof(o));
-    o.metric_type = counter ? M3TSZ_METRIC_COUNTER : M3TSZ_METRIC_GAUGE;
-    o.d_count = (int64_t *)d_cnt;
-    if (counter) {
-      o.d_counter_sum = (int64_t *)d_sum;
-      o.d_counter_min = (int64_t *)d_min;
-      o.d_counter_max = (int64_t *)d_max;
-      o.d_counter_sum_sq = (int64_t *)d_sq;
-    } else {
-      o.d_sum = (double *)d_sum;
-      o.d_min = (double *)d_min;
-      o.d_max = (double *)d_max;
-      o.d_sum_sq = (double *)d_sq;
-      o.d_last = (double *)d_last;
-      o.d_last_at = (int64_t *)d_lat;
-    }
-    o.d_n_points = (uint32_t *)d_np;
-    o.d_status = (int32_t *)d_sst;
-    rc = decode_downsample_ex_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
-                                   step_ns, n_windows, &o, st, (uint64_t *)d_ann, xf.block_off, xf.n_segments);
-  }
-  if (rc) return rc;
+  TileWindows win;
+  if ((rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                         n_windows, counter, types, n_types, xf.annotated, xf.block_off, xf.n_segments, st, win)))
+    return rc;
+  void *d_sst = win.sst, *d_ann = win.ann;
   // 2. re-encode straight from the window-major aggregates (the encoder's input stage skips empty
   //    windows, stamps the window end and takes Gauge.ValueOf(agg_type)) into the packed buffer
   CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
@@ -800,18 +835,7 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   p.out_len = d_out_len;
   p.status = d_status;
   p.in_mode = 2;
-  p.tile_count = (const int64_t *)d_cnt;
-  if (counter) {
-    p.tile_isum = (const int64_t *)d_sum;
-    p.tile_imin = (const int64_t *)d_min;
-    p.tile_imax = (const int64_t *)d_max;
-  } else {
-    p.tile_sum = (const double *)d_sum;
-    p.tile_min = (const double *)d_min;
-    p.tile_max = (const double *)d_max;
-    p.tile_last = (const double *)d_last;
-  }
-  p.tile_sum_sq = d_sq;  // (NULL unless SumSq / Stdev / Counter)
+  tile_inputs(p, counter, win.sum, win.cnt, win.min, win.max, win.last, win.sq);
   p.tile_src_status = (const int32_t *)d_sst;
   p.tile_start = start_ns;
   p.tile_step = step_ns;
@@ -1005,6 +1029,161 @@ int m3tsz_aggregate_tiles_blocks(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
                                     packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes,
                                     ops, n_ops, discard_nan, d_state, stream, annotations != 0, d_block_off,
                                     n_segments);
+}
+
+// Tile aggregation through a rollup (DESIGN.md §4.8): the fused decode of the sources under src_type, the forward
+// stage (each source's pre_ops chain), the fold into the groups' windows, then the multi-type element stage over
+// n_rollup_types * n_groups rows, its status pass, and the source records.
+int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                 uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                 uint64_t n_segments, const uint64_t *d_block_off, uint64_t n_series, int64_t start_ns,
+                                 int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t src_type,
+                                 const int32_t *pre_ops, uint32_t n_pre_ops, const uint64_t *d_group_off,
+                                 const uint32_t *d_members, uint64_t n_members, uint64_t n_groups,
+                                 const int32_t *rollup_types, uint32_t n_rollup_types, const int32_t *post_ops,
+                                 uint32_t n_post_ops, int32_t discard_nan, m3tsz_transform_state *d_src_state,
+                                 m3tsz_element_state *d_group_state, int32_t out_unit, uint32_t align,
+                                 uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                                 uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
+                                 int32_t *d_src_status, void *stream) {
+  if (!ctx || !valid_opts(opts) || !d_total_bytes || !valid_tile_pair(metric_type, src_type) || !rollup_types ||
+      n_rollup_types == 0 || n_rollup_types > M3TSZ_MAX_ELEMENT_TYPES || (!d_block_off && n_segments != n_series) ||
+      (n_groups && (!d_group_off || !d_status)) || (n_members && !d_members))
+    return M3TSZ_ERR_INVALID_ARG;
+  for (uint32_t j = 0; j < n_rollup_types; j++)
+    if (!valid_tile_pair(metric_type, rollup_types[j]) || (j && rollup_types[j] <= rollup_types[j - 1]))
+      return M3TSZ_ERR_INVALID_ARG;
+  TileTransforms pre, post;
+  if (!parse_transforms(pre_ops, n_pre_ops, pre) || !parse_transforms(post_ops, n_post_ops, post))
+    return M3TSZ_ERR_INVALID_ARG;
+  const uint64_t n_rows = (uint64_t)n_rollup_types * n_groups;
+  if (n_rows && (!valid_align(align) || !d_packed || !d_out_offsets || !d_out_len || ((uintptr_t)d_packed & 63u)))
+    return M3TSZ_ERR_INVALID_ARG;
+  if (n_windows == 0 || n_windows > 0x7fffffffu || step_ns <= 0 ||
+      (__int128)start_ns + (__int128)n_windows * (__int128)step_ns > (__int128)INT64_MAX)
+    return M3TSZ_ERR_INVALID_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  const bool counter = metric_type == M3TSZ_METRIC_COUNTER;
+  int rc;
+  // 1. fused decode + windows of the sources under their one type
+  TileWindows win;
+  if (n_series &&
+      (rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                         n_windows, counter, &src_type, 1, false, d_block_off, n_segments, st, win)))
+    return rc;
+  // 2. forward stage: series-major forwarded values and presence words, each source's new record to scratch
+  const uint32_t n_words = (n_windows + 31) / 32;
+  void *d_fwd, *d_pres, *d_srec, *d_mark;
+  if ((rc = ensure(ctx, kSlotFwdVal, (size_t)n_series * n_windows * 8, &d_fwd))) return rc;
+  if ((rc = ensure(ctx, kSlotFwdPresent, (size_t)n_series * n_words * 4, &d_pres))) return rc;
+  if ((rc = ensure(ctx, kSlotSrcRecScratch, n_series * sizeof(m3tsz_transform_state), &d_srec))) return rc;
+  if ((rc = ensure(ctx, kSlotSrcMark, n_series, &d_mark))) return rc;
+  RollupForwardParams fp;
+  memset(&fp, 0, sizeof(fp));
+  tile_inputs(fp.tiles, counter, win.sum, win.cnt, win.min, win.max, win.last, win.sq);
+  fp.tiles.metric_type = metric_type;
+  fp.tiles.tile_start = start_ns;
+  fp.tiles.tile_step = step_ns;
+  fp.src_status = (const int32_t *)win.sst;
+  fp.n_src = n_series;
+  fp.n_windows = n_windows;
+  fp.n_words = n_words;
+  fp.src_type = src_type;
+  fp.ops = pre.ops;
+  fp.discard_nan = discard_nan ? 1 : 0;  // (generic_elem.go:892-894: with or without transformations)
+  fp.state = d_src_state;
+  fp.state_out = (m3tsz_transform_state *)d_srec;
+  fp.fwd = (double *)d_fwd;
+  fp.present = (uint32_t *)d_pres;
+  CK(launch_rollup_forward(fp, st));
+  ctx->launches++;
+  // 3. fold: the groups' window-major aggregates, in the fused decode's representation, and their statuses
+  const size_t gb = (size_t)n_groups * n_windows * 8;
+  bool sq = counter;
+  for (uint32_t j = 0; j < n_rollup_types; j++)
+    sq |= rollup_types[j] == M3TSZ_AGG_SUMSQ || rollup_types[j] == M3TSZ_AGG_STDEV;
+  void *g_sum, *g_cnt, *g_min, *g_max, *g_last = nullptr, *g_sq = nullptr, *g_st;
+  if ((rc = ensure(ctx, kSlotGroupSum, gb, &g_sum))) return rc;
+  if ((rc = ensure(ctx, kSlotGroupCount, gb, &g_cnt))) return rc;
+  if ((rc = ensure(ctx, kSlotGroupMin, gb, &g_min))) return rc;
+  if ((rc = ensure(ctx, kSlotGroupMax, gb, &g_max))) return rc;
+  if (!counter && (rc = ensure(ctx, kSlotGroupLast, gb, &g_last))) return rc;
+  if (sq && (rc = ensure(ctx, kSlotGroupSumSq, gb, &g_sq))) return rc;
+  if ((rc = ensure(ctx, kSlotGroupStatus, n_groups * 4, &g_st))) return rc;
+  RollupFoldParams gp;
+  memset(&gp, 0, sizeof(gp));
+  gp.fwd = (const double *)d_fwd;
+  gp.present = (const uint32_t *)d_pres;
+  gp.src_status = (const int32_t *)win.sst;
+  gp.n_src = n_series;
+  gp.n_windows = n_windows;
+  gp.n_words = n_words;
+  gp.group_off = d_group_off;
+  gp.members = d_members;
+  gp.n_members = n_members;
+  gp.n_groups = n_groups;
+  gp.counter = counter ? 1 : 0;
+  gp.sum = g_sum;
+  gp.count = (int64_t *)g_cnt;
+  gp.min = g_min;
+  gp.max = g_max;
+  gp.last = (double *)g_last;
+  gp.sum_sq = g_sq;
+  gp.group_status = (int32_t *)g_st;
+  CK(launch_rollup_fold(gp, st));
+  ctx->launches++;
+  // 4. the rollup element: the multi-type stage over n_rollup_types * n_groups rows, the groups as its sources
+  CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
+  void *d_grec = nullptr;
+  if (n_rows) {
+    EncodeParams p;
+    memset(&p, 0, sizeof(p));
+    const uint64_t rows = post.reset ? 2ull * n_windows : (uint64_t)n_windows;
+    if ((rc = packed_params(ctx, n_rows, m3tsz_encode_bound(rows), align, d_packed, packed_capacity, d_out_offsets,
+                            d_total_bytes, st, p)))
+      return rc;
+    void *d_es = nullptr;
+    if ((rc = ensure(ctx, kSlotTileStarts, n_rows * 8, &d_es))) return rc;
+    CK(launch_fill_i64((int64_t *)d_es, start_ns, n_rows, st));
+    if (d_group_state &&
+        (rc = ensure(ctx, kSlotElementScratch, n_groups * sizeof(m3tsz_element_state), &d_grec)))
+      return rc;
+    p.n_series = n_rows;
+    p.points_stride = n_windows;
+    p.start = (const int64_t *)d_es;
+    p.unit = out_unit;
+    p.default_unit = opts->default_time_unit;
+    p.out_len = d_out_len;
+    p.status = d_status;
+    p.in_mode = 5;
+    tile_inputs(p, counter, g_sum, g_cnt, g_min, g_max, g_last, g_sq);
+    p.tile_src_status = (const int32_t *)g_st;
+    p.tile_start = start_ns;
+    p.tile_step = step_ns;
+    p.agg_type = rollup_types[0];
+    p.metric_type = metric_type;
+    p.n_tiles_out = d_n_tiles;
+    p.xf_ops = post.ops;
+    p.xf_discard_nan = discard_nan ? 1 : 0;
+    p.xf_elem = d_group_state;
+    p.xf_elem_out = (m3tsz_element_state *)d_grec;
+    p.tile_n_src = n_groups;
+    p.tile_n_types = n_rollup_types;
+    for (uint32_t j = 0; j < n_rollup_types; j++) p.tile_types |= (uint32_t)rollup_types[j] << (4 * j);
+    CK(launch_encode(p, opts->int_optimized != 0, st));
+    ctx->launches += 2;
+    CK(launch_tiles_types_status((const int32_t *)g_st, d_status, n_groups, n_rollup_types,
+                                 (const m3tsz_element_state *)d_grec, d_group_state, st));
+    ctx->launches++;
+  }
+  // 5. the source records: a source is saved when it decoded and every group that lists it was saved
+  CK(launch_rollup_commit(d_group_off, d_members, n_members, n_groups, d_status, n_rollup_types,
+                          (const int32_t *)win.sst, n_series, (uint8_t *)d_mark, (const m3tsz_transform_state *)d_srec,
+                          d_src_state, d_src_status, st));
+  ctx->launches += 2;
+  return M3TSZ_OK;
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

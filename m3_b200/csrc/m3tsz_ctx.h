@@ -44,6 +44,10 @@ struct Scratch {
 //   48-50         route targets, touched records, their count    encoder_set_write
 //   51, 52        window annotation references, the longest     tiles (aggregate_tiles_annotated)
 //                 source stream
+//   53-56         forwarded values, presence words, source      tiles (aggregate_tiles_rollup)
+//                 records, source marks
+//   57-63         group window sum / count / min / max / last   tiles (aggregate_tiles_rollup)
+//                 / sumSq, group statuses
 enum Slot : int {
   kSlotStreams = 0,
   kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
@@ -89,7 +93,19 @@ enum Slot : int {
   // tile aggregation with annotations
   kSlotWinAnn = 51,
   kSlotSrcMaxLen = 52,
-  kNumSlots = 53
+  // tile aggregation through a rollup
+  kSlotFwdVal = 53,
+  kSlotFwdPresent = 54,
+  kSlotSrcRecScratch = 55,
+  kSlotSrcMark = 56,
+  kSlotGroupSum = 57,
+  kSlotGroupCount = 58,
+  kSlotGroupMin = 59,
+  kSlotGroupMax = 60,
+  kSlotGroupLast = 61,
+  kSlotGroupSumSq = 62,
+  kSlotGroupStatus = 63,
+  kNumSlots = 64
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

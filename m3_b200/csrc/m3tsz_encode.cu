@@ -2258,6 +2258,208 @@ cudaError_t launch_encoder_set_stream(const m3tsz_encoder_state *state, uint64_t
 }
 
 // ---------------------------------------------------------------------------
+// tile aggregation through a rollup (DESIGN.md §4.8): forward stage, then the fold into the group element's windows
+// ---------------------------------------------------------------------------
+// One window of a rollup element: every value AddUnique gives it arrives at the same timestamp (the source windows'
+// common end), so Gauge.updateTotals (gauge.go:74-101) keeps the FIRST value as Last (timestamp.After(lastAt) is
+// false for equal times), counts NaNs and skips them in sum / min / max / sumSq; min and max start as math.NaN()
+// and keep the first of +-0.  Counter.Update (counter.go:52-78) takes int64(value) (amd64's conversion) and wraps.
+struct RollupGaugeAcc {
+  double sum, mn, mx, last, sq;
+  int64_t cnt;
+};
+struct RollupCounterAcc {
+  int64_t sum, mn, mx, sq, cnt;
+};
+__device__ __forceinline__ void rollup_gauge_init(RollupGaugeAcc &a) {  // NewGauge, gauge.go:45-51
+  a.sum = 0.0;
+  a.mn = xf_bits(kXfEmptyNaN);
+  a.mx = xf_bits(kXfEmptyNaN);
+  a.last = 0.0;
+  a.sq = 0.0;
+  a.cnt = 0;
+}
+__device__ __forceinline__ void rollup_counter_init(RollupCounterAcc &a) {  // NewCounter, counter.go:44-50
+  a.sum = 0;
+  a.mn = (int64_t)0x7fffffffffffffffull;
+  a.mx = (int64_t)0x8000000000000000ull;
+  a.sq = 0;
+  a.cnt = 0;
+}
+// amd64's ADDSD of a running total and a non-NaN value: a NaN total keeps its payload (quieted), Inf + -Inf gives
+// the default NaN
+__device__ __forceinline__ double rollup_add(double a, double x) {
+  const double r = __dadd_rn(a, x);
+  if (!xf_isnan(r)) return r;
+  return xf_isnan(a) ? xf_bits((uint64_t)__double_as_longlong(a) | 0x0008000000000000ull) : xf_bits(kXfOpNaN);
+}
+__device__ __forceinline__ void rollup_gauge_add(RollupGaugeAcc &a, double x) {
+  if (a.cnt == 0) a.last = x;
+  a.cnt++;
+  if (xf_isnan(x)) return;
+  a.sum = rollup_add(a.sum, x);
+  if (xf_isnan(a.mx) || a.mx < x) a.mx = x;
+  if (xf_isnan(a.mn) || a.mn > x) a.mn = x;
+  a.sq = rollup_add(a.sq, __dmul_rn(x, x));
+}
+__device__ __forceinline__ void rollup_counter_add(RollupCounterAcc &a, double x) {
+  const int64_t v = go_f64_to_i64(x);
+  a.sum = (int64_t)((uint64_t)a.sum + (uint64_t)v);
+  a.cnt++;
+  if (a.mx < v) a.mx = v;
+  if (a.mn > v) a.mn = v;
+  a.sq = (int64_t)((uint64_t)a.sq + (uint64_t)v * (uint64_t)v);
+}
+
+// Forward stage: one lane per source series, windows in order (the chain is a recurrence over them), 32 windows at a
+// time staged in shared memory so that the series-major rows are written as whole 256-byte runs; the presence words
+// of those 32 windows are one word-major row, written by the warp as 128-byte runs.
+constexpr int ROLLUP_FWD_WARPS = 4;
+__global__ void __launch_bounds__(ROLLUP_FWD_WARPS * 32) rollup_forward_kernel(const RollupForwardParams p) {
+  __shared__ double tile[ROLLUP_FWD_WARPS][32][33];
+  const uint32_t lane = threadIdx.x & 31u, wi = threadIdx.x >> 5;
+  const uint64_t s0 = ((uint64_t)blockIdx.x * ROLLUP_FWD_WARPS + wi) * 32ull, s = s0 + lane;
+  const bool valid = s < p.n_src;
+  const bool ok = valid && p.src_status[s] == M3TSZ_OK;
+  const bool counter = p.tiles.metric_type == M3TSZ_METRIC_COUNTER;
+  m3tsz_transform_state st;
+  if (valid && p.state)
+    st = p.state[s];
+  else
+    memset(&st, 0, sizeof(st));
+  double(*const tl)[33] = tile[wi];
+  for (uint32_t w0 = 0; w0 < p.n_windows; w0 += 32) {
+    uint32_t bits = 0;
+#pragma unroll 1
+    for (uint32_t i = 0; i < 32; i++) {
+      const uint32_t w = w0 + i;
+      double v = 0.0;
+      if (ok && w < p.n_windows) {
+        const uint64_t o = (uint64_t)w * p.n_src + s;
+        const int64_t c = __ldg(p.tiles.tile_count + o);
+        if (c != 0) {
+          v = tile_value_of(p.tiles, counter, p.src_type, o, c);
+          int64_t extra_t = 0;  // (a Reset datapoint is not forwarded)
+          xf_window(p.ops, p.tiles.tile_step, st, p.tiles.tile_start + (int64_t)(w + 1) * p.tiles.tile_step, v,
+                    extra_t);
+          if (!(p.discard_nan && xf_isnan(v))) bits |= 1u << i;
+        }
+      }
+      tl[lane][i] = v;
+    }
+    __syncwarp();
+    const uint32_t w = w0 + lane;
+    for (uint32_t j = 0; j < 32; j++)
+      if (s0 + j < p.n_src && w < p.n_windows) p.fwd[(s0 + j) * p.n_windows + w] = tl[j][lane];
+    if (valid) p.present[(uint64_t)(w0 >> 5) * p.n_src + s] = bits;
+    __syncwarp();
+  }
+  if (valid) p.state_out[s] = st;
+}
+
+// Fold: one warp per group, lane l over windows w0 + l; members in listed order (each lane folds its own window, so
+// the order is the same in every window), their present words read once per 32 windows, their values as 256-byte
+// runs.  A block's groups write their window rows through shared memory, ROLLUP_FOLD_WARPS adjacent slots at a time.
+constexpr int ROLLUP_FOLD_WARPS = 8;
+__global__ void __launch_bounds__(ROLLUP_FOLD_WARPS * 32) rollup_fold_kernel(const RollupFoldParams p) {
+  __shared__ uint64_t out[6][32][ROLLUP_FOLD_WARPS];
+  const uint32_t lane = threadIdx.x & 31u, wi = threadIdx.x >> 5;
+  const uint64_t g0 = (uint64_t)blockIdx.x * ROLLUP_FOLD_WARPS, g = g0 + wi;
+  const bool valid = g < p.n_groups;
+  // the group's status: its range, then its members in listed order (the first failing one)
+  int32_t gst = M3TSZ_OK;
+  uint64_t lo = 0, hi = 0;
+  if (valid) {
+    lo = p.group_off[g];
+    hi = p.group_off[g + 1];
+    if (lo > hi || hi > p.n_members) {
+      gst = M3TSZ_ERR_INVALID_ARG;
+    } else {
+      for (uint64_t i0 = lo; i0 < hi && gst == M3TSZ_OK; i0 += 32) {
+        int32_t e = M3TSZ_OK;
+        if (i0 + lane < hi) {
+          const uint32_t m = p.members[i0 + lane];
+          e = m >= p.n_src ? M3TSZ_ERR_INVALID_ARG : p.src_status[m];
+        }
+        const uint32_t bad = __ballot_sync(FULL_MASK, e != M3TSZ_OK);
+        if (bad) gst = __shfl_sync(FULL_MASK, e, __ffs(bad) - 1);
+      }
+    }
+    if (lane == 0) p.group_status[g] = gst;
+  }
+  const bool fold = valid && gst == M3TSZ_OK;
+  for (uint32_t w0 = 0; w0 < p.n_windows; w0 += 32) {
+    const uint32_t w = w0 + lane, word = w0 >> 5;  // (a window past the range has no present bit)
+    uint64_t r[6];
+    if (p.counter) {
+      RollupCounterAcc a;
+      rollup_counter_init(a);
+      if (fold) {
+        for (uint64_t i = lo; i < hi; i++) {
+          const uint64_t m = __ldg(p.members + i);
+          const uint32_t bits = __ldg(p.present + (uint64_t)word * p.n_src + m);
+          if ((bits >> lane) & 1u) rollup_counter_add(a, __ldg(p.fwd + m * p.n_windows + w));
+        }
+      }
+      r[0] = (uint64_t)a.sum;
+      r[1] = (uint64_t)a.cnt;
+      r[2] = (uint64_t)a.mn;
+      r[3] = (uint64_t)a.mx;
+      r[4] = 0;
+      r[5] = (uint64_t)a.sq;
+    } else {
+      RollupGaugeAcc a;
+      rollup_gauge_init(a);
+      if (fold) {
+        for (uint64_t i = lo; i < hi; i++) {
+          const uint64_t m = __ldg(p.members + i);
+          const uint32_t bits = __ldg(p.present + (uint64_t)word * p.n_src + m);
+          if ((bits >> lane) & 1u) rollup_gauge_add(a, __ldg(p.fwd + m * p.n_windows + w));
+        }
+      }
+      r[0] = (uint64_t)__double_as_longlong(a.sum);
+      r[1] = (uint64_t)a.cnt;
+      r[2] = (uint64_t)__double_as_longlong(a.mn);
+      r[3] = (uint64_t)__double_as_longlong(a.mx);
+      r[4] = (uint64_t)__double_as_longlong(a.last);
+      r[5] = (uint64_t)__double_as_longlong(a.sq);
+    }
+#pragma unroll
+    for (int k = 0; k < 6; k++) out[k][lane][wi] = r[k];
+    __syncthreads();
+    // row rr of this window block, group column c: ROLLUP_FOLD_WARPS adjacent 8-byte slots of one window row
+    for (uint32_t t = threadIdx.x; t < 32u * ROLLUP_FOLD_WARPS; t += blockDim.x) {
+      const uint32_t rr = t / ROLLUP_FOLD_WARPS, c = t % ROLLUP_FOLD_WARPS;
+      if (w0 + rr >= p.n_windows || g0 + c >= p.n_groups) continue;
+      const uint64_t o = (uint64_t)(w0 + rr) * p.n_groups + g0 + c;
+      reinterpret_cast<uint64_t *>(p.sum)[o] = out[0][rr][c];
+      p.count[o] = (int64_t)out[1][rr][c];
+      reinterpret_cast<uint64_t *>(p.min)[o] = out[2][rr][c];
+      reinterpret_cast<uint64_t *>(p.max)[o] = out[3][rr][c];
+      if (!p.counter) reinterpret_cast<uint64_t *>(p.last)[o] = out[4][rr][c];
+      if (p.sum_sq) reinterpret_cast<uint64_t *>(p.sum_sq)[o] = out[5][rr][c];
+    }
+    __syncthreads();
+  }
+}
+
+cudaError_t launch_rollup_forward(const RollupForwardParams &p, cudaStream_t stream) {
+  if (p.n_src == 0 || p.n_windows == 0) return cudaSuccess;
+  const uint64_t per_block = 32ull * ROLLUP_FWD_WARPS, blocks = (p.n_src + per_block - 1) / per_block;
+  if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
+  rollup_forward_kernel<<<(unsigned)blocks, ROLLUP_FWD_WARPS * 32, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_rollup_fold(const RollupFoldParams &p, cudaStream_t stream) {
+  if (p.n_groups == 0) return cudaSuccess;
+  const uint64_t blocks = (p.n_groups + ROLLUP_FOLD_WARPS - 1) / ROLLUP_FOLD_WARPS;
+  if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
+  rollup_fold_kernel<<<(unsigned)blocks, ROLLUP_FOLD_WARPS * 32, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------
 // compaction: slots -> packed buffer with CSR offsets
 // ---------------------------------------------------------------------------
 __global__ void compact_lens_kernel(const uint64_t *len, uint64_t n, uint64_t mask, uint64_t *out) {

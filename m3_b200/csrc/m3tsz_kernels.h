@@ -274,6 +274,54 @@ cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status
                                       const m3tsz_element_state *scratch, m3tsz_element_state *state,
                                       cudaStream_t stream);
 
+// tile aggregation through a rollup (m3tsz_aggregate_tiles_rollup; m3tsz_encode.cu).  The forward stage: the lane
+// that owns source series s runs its non-empty windows' values through the op list and writes the forwarded values
+// series-major, fwd[s][w], with a presence bit per window, present[w / 32][s] bit w % 32 (NaN payloads are values).
+struct RollupForwardParams {
+  // the fused decode's window-major [n_windows][n_src] aggregates, in the fields the tile stages read them from
+  // (tile_sum .. tile_count, tile_sum_sq, metric_type, tile_start, tile_step); tile_value_of takes them from here
+  EncodeParams tiles;
+  const int32_t *src_status;  // [n_src]: a failed source forwards nothing
+  uint64_t n_src;
+  uint32_t n_windows;
+  uint32_t n_words;  // presence rows, ceil(n_windows / 32), of n_src words each
+  int src_type;
+  uint32_t ops;  // as EncodeParams::xf_ops
+  int discard_nan;
+  const m3tsz_transform_state *state;  // optional [n_src]
+  m3tsz_transform_state *state_out;    // [n_src]: each source's new record (committed by launch_rollup_commit)
+  double *fwd;
+  uint32_t *present;
+};
+// The fold: window w of group g takes the forwarded values of its members, in listed order, and writes the aggregate
+// slots of the fused decode over n_groups "series" (window-major [n_windows][n_groups], the same representation)
+struct RollupFoldParams {
+  const double *fwd;
+  const uint32_t *present;
+  const int32_t *src_status;
+  uint64_t n_src;
+  uint32_t n_windows;
+  uint32_t n_words;
+  const uint64_t *group_off;  // [n_groups + 1]
+  const uint32_t *members;    // [n_members]
+  uint64_t n_members;
+  uint64_t n_groups;
+  int counter;  // Counter.Update(int64(v)) into int64 slots, else Gauge.Update into double slots
+  void *sum, *min, *max, *sum_sq;  // sum_sq optional
+  int64_t *count;
+  double *last;           // Gauge only
+  int32_t *group_status;  // [n_groups]: INVALID_ARG for a bad range or index, else the first failing member's error
+};
+cudaError_t launch_rollup_forward(const RollupForwardParams &p, cudaStream_t stream);
+cudaError_t launch_rollup_fold(const RollupFoldParams &p, cudaStream_t stream);
+// The source records (m3tsz_query.cu): a source takes its new record from `scratch` when it decoded and every group
+// that lists it has all n_types rows OK; src_status_out (optional) takes each source's decode status.  `mark` is
+// [n_src] bytes of scratch.
+cudaError_t launch_rollup_commit(const uint64_t *group_off, const uint32_t *members, uint64_t n_members,
+                                 uint64_t n_groups, const int32_t *status, uint32_t n_types, const int32_t *src_status,
+                                 uint64_t n_src, uint8_t *mark, const m3tsz_transform_state *scratch,
+                                 m3tsz_transform_state *state, int32_t *src_status_out, cudaStream_t stream);
+
 // exclusive scan of aligned lengths + gather into a packed buffer
 cudaError_t launch_compact(const uint8_t *slots, uint64_t slot_stride, const uint64_t *len,
                            uint64_t n_series, uint32_t align, uint8_t *packed,

@@ -182,6 +182,53 @@ cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status
   return cudaGetLastError();
 }
 
+// The rollup's source records.  First every group that was not saved (a row not OK: its members failed, its range or
+// an index was invalid, or a row hit CAPACITY) marks the members its range names inside d_members; then a source that
+// decoded and is unmarked takes its new record.  (Concurrent marks store the same byte.)
+__global__ void rollup_mark_kernel(const uint64_t *group_off, const uint32_t *members, uint64_t n_members,
+                                   uint64_t n_groups, const int32_t *status, uint32_t n_types, uint64_t n_src,
+                                   uint8_t *mark) {
+  // one warp per group, its lanes over the members: a large group costs its length / 32 steps
+  const uint64_t g = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31u;
+  if (g >= n_groups) return;
+  bool ok = true;
+  for (uint32_t j = 0; j < n_types; j++) ok = ok && status[(uint64_t)j * n_groups + g] == M3TSZ_OK;
+  if (ok) return;
+  const uint64_t lo = group_off[g], hi = group_off[g + 1] < n_members ? group_off[g + 1] : n_members;
+  for (uint64_t i = lo + lane; i < hi; i += 32) {
+    const uint32_t m = members[i];
+    if (m < n_src) mark[m] = 1;
+  }
+}
+__global__ void rollup_commit_kernel(const int32_t *src_status, const uint8_t *mark, uint64_t n,
+                                     const m3tsz_transform_state *scratch, m3tsz_transform_state *state,
+                                     int32_t *src_status_out) {
+  const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  const int32_t e = src_status[s];
+  if (src_status_out) src_status_out[s] = e;
+  if (state && e == M3TSZ_OK && !mark[s]) state[s] = scratch[s];
+}
+cudaError_t launch_rollup_commit(const uint64_t *group_off, const uint32_t *members, uint64_t n_members,
+                                 uint64_t n_groups, const int32_t *status, uint32_t n_types, const int32_t *src_status,
+                                 uint64_t n_src, uint8_t *mark, const m3tsz_transform_state *scratch,
+                                 m3tsz_transform_state *state, int32_t *src_status_out, cudaStream_t stream) {
+  if (n_src == 0) return cudaSuccess;
+  const unsigned tb = 256;
+  if ((n_groups * 32 + tb - 1) / tb > 0x7fffffffull || (n_src + tb - 1) / tb > 0x7fffffffull)
+    return cudaErrorInvalidValue;
+  cudaError_t e = cudaMemsetAsync(mark, 0, n_src, stream);
+  if (e != cudaSuccess) return e;
+  if (n_groups)
+    rollup_mark_kernel<<<(unsigned)((n_groups * 32 + tb - 1) / tb), tb, 0, stream>>>(group_off, members, n_members,
+                                                                                    n_groups, status, n_types, n_src,
+                                                                                    mark);
+  rollup_commit_kernel<<<(unsigned)((n_src + tb - 1) / tb), tb, 0, stream>>>(src_status, mark, n_src, scratch, state,
+                                                                            src_status_out);
+  return cudaGetLastError();
+}
+
 // The longest source stream of a tile call with annotations: the bound of an annotated row adds it (one warp-wide max
 // and one atomic per warp)
 __global__ void max_stream_len_kernel(const uint64_t *offsets, const uint64_t *lengths, uint64_t n,

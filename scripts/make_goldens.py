@@ -4,7 +4,8 @@ tests/golden/m3tsz_goldens.json, those of the aggregator's Gauge / Counter arith
 tests/golden/m3tsz_agg_goldens.json, the buffer bucket's write tables into
 tests/golden/m3tsz_buffer_goldens.json, the aggregator's transformations of a flushed window into
 tests/golden/m3tsz_transform_goldens.json, and the flushes of an element with several aggregation types into
-tests/golden/m3tsz_element_types_goldens.json.
+tests/golden/m3tsz_element_types_goldens.json, and the steps of a rollup (the values a source element forwards, what
+the rollup element folds, when the forwarded list flushes) into tests/golden/m3tsz_rollup_goldens.json.
 
 Run in the build container only (it reads /root/reference, which does not exist
 on the GPU box):   python scripts/make_goldens.py
@@ -30,6 +31,8 @@ OUT_XF = os.path.join(os.path.dirname(OUT), "m3tsz_transform_goldens.json")
 # an element's several aggregation types (GenericElem.processValue's loop over aggTypes)
 OUT_ELEM = os.path.join(os.path.dirname(OUT), "m3tsz_element_types_goldens.json")
 OUT_ANN = os.path.join(os.path.dirname(OUT), "m3tsz_tile_annotation_goldens.json")
+# a rollup: the source element's forwarded values, the rollup element's folds and the forwarded list's flush times
+OUT_ROLLUP = os.path.join(os.path.dirname(OUT), "m3tsz_rollup_goldens.json")
 
 SEC = 1_000_000_000
 MS = 1_000_000
@@ -611,6 +614,64 @@ def main():
         ],
     }
 
+    # ---- a rollup.  testPipeline (elem_test.go:94-117) is Absolute, PerSecond, then a rollup: the source element
+    # forwards only each window's value through the two transformations (generic_elem.go:912-937), at the window's
+    # end (10 s resolution, windows starting at 210, 220, 230 s with one value each, elem_test.go:597-607 and
+    # :1891-1901, DiscardNaNAggregatedValues off).  "windows": (end, ValueOf(type)) of the non-empty windows; "want":
+    # the forwarded (timestamp, value), "NaN" for a NaN; "consumed": the binary op's input after the last window.
+    def fwd_case(name, src_line, metric_type, src_type):
+        return {"name": name, "src_line": src_line, "metric_type": metric_type, "src_type": src_type,
+                "ops": [1, 2], "step_ns": 10 * SEC, "discard_nan": False,
+                "windows": [[220 * SEC, -123.0], [230 * SEC, -456.0], [240 * SEC, -589.0]],
+                "want": [[220 * SEC, "NaN"], [230 * SEC, 33.3], [240 * SEC, 13.3]], "consumed": 589.0}
+
+    # The rollup element's AddUnique (generic_elem.go:246-281): the values each window received, in order, and what
+    # the test asserts after them ("eps": the test's relative tolerance; sum_sq only where the element's types are
+    # expensive, testAggregationTypesExpensive = {SumSq}, elem_test.go:59).  The resends (Version > 0) and the
+    # duplicate-source errors of these tests are not part of the fold.
+    def fold(values, **want):
+        return {"values": values, "want": want}
+
+    rollup = {
+        "description": "The steps of a rollup, transcribed from the reference's aggregator tests by "
+                       "scripts/make_goldens.py: the values a source element forwards (forward), the rollup "
+                       "element's fold of the values a window receives (folds), and the forwarded list's flush "
+                       "timestamps (flush).",
+        "forward": [
+            fwd_case("TestCounterElemConsumeCustomAggregationCustomPipeline",
+                     "aggregator/aggregator/elem_test.go:596-724", 1, 7),
+            fwd_case("TestGaugeElemConsumeCustomAggregationCustomPipeline",
+                     "aggregator/aggregator/elem_test.go:1890-2012", 3, 1),
+        ],
+        "folds": [
+            {"name": "TestCounterElemAddUnique", "src_line": "aggregator/aggregator/elem_test.go:308-390",
+             "metric_type": 1,
+             "steps": [fold([345.0], sum=345, count=1), fold([345.0, 500.0], sum=845, count=2),
+                       fold([278.0], sum=278, count=1)]},
+            {"name": "TestCounterElemAddUniqueWithCustomAggregation",
+             "src_line": "aggregator/aggregator/elem_test.go:392-466", "metric_type": 1,
+             "steps": [fold([12.0], sum=12, max=12, sum_sq=144), fold([12.0, 14.0], sum=26, max=14),
+                       fold([20.0], sum=20, max=20, sum_sq=400, count=1)]},
+            {"name": "TestGaugeElemAddUnique", "src_line": "aggregator/aggregator/elem_test.go:1473-1570",
+             "metric_type": 3,
+             "steps": [fold([12.3, 34.5], sum=46.8, count=2), fold([12.3, 34.5, 50.0], sum=96.8, count=3),
+                       fold([27.8], sum=27.8, count=1)]},
+            {"name": "TestGaugeElemAddUniqueWithCustomAggregation",
+             "src_line": "aggregator/aggregator/elem_test.go:1572-1643", "metric_type": 3,
+             "steps": [fold([1.2], sum=1.2, max=1.2, sum_sq=1.44),
+                       fold([1.2, 1.4], sum=2.6, max=1.4, eps=1e-10),
+                       fold([2.0], sum=2.0, max=2.0, sum_sq=4.0)]},
+        ],
+        # list_test.go:815-1022: a counter (123) and a gauge (1.762) element with pipeline Rollup [Max] each take
+        # AddUnique at the aligned 210 s and 220 s (10 s resolution); the list flushes each window's value with the
+        # window's START as its timestamp (forwardedMetricTimestampNanos, list.go:621-623)
+        "flush": {"name": "TestForwardedMetricListFlushConsumingAndCollectingForwardedMetrics",
+                  "src_line": "aggregator/aggregator/list_test.go:815-1022", "resolution_ns": 10 * SEC,
+                  "agg_type": 3,
+                  "elements": [{"metric_type": 1, "value": 123.0}, {"metric_type": 3, "value": 1.762}],
+                  "added_at_ns": [210 * SEC, 220 * SEC], "want_flush_ns": [210 * SEC, 220 * SEC]},
+    }
+
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f, indent=1)
@@ -630,6 +691,9 @@ def main():
     with open(OUT_ANN, "w") as f:
         json.dump(ann, f, indent=1)
     print("wrote", OUT_ANN)
+    with open(OUT_ROLLUP, "w") as f:
+        json.dump(rollup, f, indent=1)
+    print("wrote", OUT_ROLLUP)
 
 
 if __name__ == "__main__":
