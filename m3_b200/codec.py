@@ -21,6 +21,13 @@ def _cuda_stream_ptr(device):
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def _check_records(t: Optional[torch.Tensor], n: int, nbytes: int):
+    """A tile call's optional record tensor: uint8 [n, nbytes], contiguous, on the device."""
+    if t is not None:
+        assert t.is_cuda and t.is_contiguous() and t.dtype == torch.uint8
+        assert t.shape == (n, nbytes)
+
+
 @dataclass
 class DecodeResult:
     ts: torch.Tensor        # int64  [S, max_points]
@@ -342,21 +349,12 @@ class BatchCodec:
         S = offsets.numel() - 1 if lengths is None else lengths.numel()
         dev = self.device
         transforms = [int(t) for t in transforms]
-        if out is None:
-            if capacity is None:
-                rows = 2 * n_windows if capi.TRANSFORM_RESET in transforms else n_windows
-                capacity = S * self.encode_bound(rows)
-            out = PackedResult(
-                packed=torch.empty(capacity, dtype=torch.uint8, device=dev),
-                offsets=torch.empty(S, dtype=torch.int64, device=dev),
-                out_len=torch.empty(S, dtype=torch.int64, device=dev),
-                status=torch.empty(S, dtype=torch.int32, device=dev),
-                total=torch.zeros(1, dtype=torch.int64, device=dev))
-        n_tiles = torch.empty(S, dtype=torch.int32, device=dev)
+        if out is None and capacity is None:
+            rows = 2 * n_windows if capi.TRANSFORM_RESET in transforms else n_windows
+            capacity = S * self.encode_bound(rows)
+        out, n_tiles = self._tile_outputs(S, capacity, out)
         if transforms:
-            if state is not None:
-                assert state.is_cuda and state.is_contiguous() and state.dtype == torch.uint8
-                assert state.shape == (S, capi.TRANSFORM_STATE_BYTES)
+            _check_records(state, S, capi.TRANSFORM_STATE_BYTES)
             ops = (C.c_int32 * len(transforms))(*transforms)
             rc = capi.lib().m3tsz_aggregate_tiles_transform(
                 self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets),
@@ -423,17 +421,8 @@ class BatchCodec:
                              else int(lengths.sum().item()))
                 capacity += k * (src_bytes + 16 * S)
             capacity = max(1, capacity)
-        n = max(1, k) * S
-        out = PackedResult(
-            packed=torch.empty(capacity, dtype=torch.uint8, device=dev),
-            offsets=torch.empty(n, dtype=torch.int64, device=dev),
-            out_len=torch.empty(n, dtype=torch.int64, device=dev),
-            status=torch.empty(n, dtype=torch.int32, device=dev),
-            total=torch.zeros(1, dtype=torch.int64, device=dev))
-        n_tiles = torch.empty(n, dtype=torch.int32, device=dev)
-        if state is not None:
-            assert state.is_cuda and state.is_contiguous() and state.dtype == torch.uint8
-            assert state.shape == (S, capi.ELEMENT_STATE_BYTES)
+        out, n_tiles = self._tile_outputs(max(1, k) * S, capacity)
+        _check_records(state, S, capi.ELEMENT_STATE_BYTES)
         types_a = (C.c_int32 * max(1, k))(*types)
         ops = (C.c_int32 * max(1, len(transforms)))(*transforms)
         if blocks is not None:
@@ -455,6 +444,18 @@ class BatchCodec:
             _cuda_stream_ptr(dev))
         self.ctx.check(rc, "m3tsz_aggregate_tiles_annotated" if annotations else "m3tsz_aggregate_tiles_types")
         return self._types_views(out, n_tiles, k, S)
+
+    def _tile_outputs(self, n, capacity, out: Optional["PackedResult"] = None):
+        """The packed outputs of a tile call with n rows (unless the caller passes them) and its n_tiles."""
+        dev = self.device
+        if out is None:
+            out = PackedResult(
+                packed=torch.empty(capacity, dtype=torch.uint8, device=dev),
+                offsets=torch.empty(n, dtype=torch.int64, device=dev),
+                out_len=torch.empty(n, dtype=torch.int64, device=dev),
+                status=torch.empty(n, dtype=torch.int32, device=dev),
+                total=torch.zeros(1, dtype=torch.int64, device=dev))
+        return out, torch.empty(n, dtype=torch.int32, device=dev)
 
     @staticmethod
     def _types_views(out, n_tiles, k, S):
@@ -487,25 +488,14 @@ class BatchCodec:
         if capacity is None:
             rows = 2 * n_windows if capi.TRANSFORM_RESET in post else n_windows
             capacity = max(1, k * G * self.encode_bound(rows))
-        n = k * G
-        out = PackedResult(
-            packed=torch.empty(capacity, dtype=torch.uint8, device=dev),
-            offsets=torch.empty(n, dtype=torch.int64, device=dev),
-            out_len=torch.empty(n, dtype=torch.int64, device=dev),
-            status=torch.empty(n, dtype=torch.int32, device=dev),
-            total=torch.zeros(1, dtype=torch.int64, device=dev))
-        n_tiles = torch.empty(n, dtype=torch.int32, device=dev)
+        out, n_tiles = self._tile_outputs(k * G, capacity)
         src_status = torch.empty(max(1, S), dtype=torch.int32, device=dev)
         assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
         assert members.is_cuda and members.dtype == torch.int32 and members.is_contiguous()
         if blocks is not None:
             assert blocks.is_cuda and blocks.dtype == torch.int64 and blocks.is_contiguous()
-        if src_state is not None:
-            assert src_state.is_cuda and src_state.is_contiguous() and src_state.dtype == torch.uint8
-            assert src_state.shape == (S, capi.TRANSFORM_STATE_BYTES)
-        if group_state is not None:
-            assert group_state.is_cuda and group_state.is_contiguous() and group_state.dtype == torch.uint8
-            assert group_state.shape == (G, capi.ELEMENT_STATE_BYTES)
+        _check_records(src_state, S, capi.TRANSFORM_STATE_BYTES)
+        _check_records(group_state, G, capi.ELEMENT_STATE_BYTES)
         i32s = lambda xs: (C.c_int32 * max(1, len(xs)))(*xs)
         rc = capi.lib().m3tsz_aggregate_tiles_rollup(
             self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), _ptr(lengths),

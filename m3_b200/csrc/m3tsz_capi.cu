@@ -234,23 +234,26 @@ int m3tsz_decode_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t 
                                max_points, d_n_points, d_status, d_unit, d_ann, nullptr, stream);
 }
 
+// The window range of every downsample and tile call: 1 .. 2^31 - 1 windows of step > 0 ns, and
+// start + n_windows * step inside int64
+static bool valid_windows(int64_t start_ns, int64_t step_ns, uint32_t n_windows) {
+  return step_ns > 0 && n_windows != 0 && n_windows <= 0x7fffffffu &&
+         (__int128)start_ns + (__int128)n_windows * (__int128)step_ns <= (__int128)INT64_MAX;
+}
+
 static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                            uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
                            uint64_t n_series,
                            int64_t range_start_ns, int64_t window_ns, uint32_t n_windows, double *d_sum,
                            int64_t *d_count, double *d_min, double *d_max, double *d_last,
                            int64_t *d_last_at, bool want_last, uint32_t *d_n_points, int32_t *d_status,
-                           void *stream, uint64_t *d_win_ann = nullptr, const uint64_t *d_block_off = nullptr,
-                           uint64_t n_segments = 0) {
+                           void *stream) {
   if (!ctx || !valid_opts(opts)) return M3TSZ_ERR_INVALID_ARG;
   if (n_series == 0) return M3TSZ_OK;
   DecodeParams p;
   if (!decode_params(opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, d_n_points, d_status, p) ||
-      !d_sum || !d_count || !d_min || !d_max || window_ns <= 0 || n_windows == 0 || n_windows > 0x7fffffffu ||
-      (want_last && !d_last) || (d_win_ann && !want_last))
-    return M3TSZ_ERR_INVALID_ARG;
-  // range_start + n_windows*window must not overflow int64
-  if ((__int128)range_start_ns + (__int128)n_windows * (__int128)window_ns > (__int128)INT64_MAX)
+      !d_sum || !d_count || !d_min || !d_max || !valid_windows(range_start_ns, window_ns, n_windows) ||
+      (want_last && !d_last))
     return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
@@ -269,24 +272,16 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
   p.ds_max = d_max;
   p.ds_last = d_last;
   p.ds_last_at = d_last_at;
-  p.ds_ann = d_win_ann;  // (mode 6: mode 2 + each window's annotation reference)
-  p.block_off = d_block_off;
-  p.n_segments = n_segments;
-  CK(launch_decode(p, opts->int_optimized != 0, d_win_ann ? 6 : (want_last ? 2 : 1), (cudaStream_t)stream));
+  CK(launch_decode(p, opts->int_optimized != 0, want_last ? 2 : 1, (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
 }
 
-// m3tsz_decode_downsample_ex: a Gauge without sumSq is downsample_impl (modes 1 / 2, today's kernels); a Gauge
-// with sumSq is mode 4, a Counter mode 5.  With d_win_ann (the annotated tile calls' window annotation references,
-// not part of the public outputs) they are modes 6, 7 and 8.  With d_block_off, over source blocks (the tile call
-// m3tsz_aggregate_tiles_blocks).
-static int decode_downsample_ex_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                                     uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
-                                     uint64_t n_series, int64_t range_start_ns, int64_t window_ns,
-                                     uint32_t n_windows, const m3tsz_downsample_outputs *o, void *stream,
-                                     uint64_t *d_win_ann, const uint64_t *d_block_off = nullptr,
-                                     uint64_t n_segments = 0) {
+// A Gauge without sumSq is downsample_impl (modes 1 / 2); a Gauge with sumSq is mode 4, a Counter mode 5.
+int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                               uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                               uint64_t n_series, int64_t range_start_ns, int64_t window_ns, uint32_t n_windows,
+                               const m3tsz_downsample_outputs *o, void *stream) {
   if (!ctx || !valid_opts(opts) || !o || o->reserved != 0) return M3TSZ_ERR_INVALID_ARG;
   const bool gauge = o->metric_type == M3TSZ_METRIC_GAUGE, counter = o->metric_type == M3TSZ_METRIC_COUNTER;
   if (gauge) {
@@ -296,8 +291,7 @@ static int decode_downsample_ex_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, 
     if (!o->d_sum_sq)
       return downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, range_start_ns,
                              window_ns, n_windows, o->d_sum, o->d_count, o->d_min, o->d_max, o->d_last,
-                             o->d_last_at, o->d_last != nullptr, o->d_n_points, o->d_status, stream, d_win_ann,
-                             d_block_off, n_segments);
+                             o->d_last_at, o->d_last != nullptr, o->d_n_points, o->d_status, stream);
   } else if (counter) {
     if (o->d_sum || o->d_min || o->d_max || o->d_sum_sq || o->d_last || o->d_last_at) return M3TSZ_ERR_INVALID_ARG;
   } else {
@@ -307,11 +301,9 @@ static int decode_downsample_ex_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, 
   DecodeParams p;
   if (!decode_params(opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, o->d_n_points, o->d_status,
                      p) ||
-      !o->d_count || window_ns <= 0 || n_windows == 0 || n_windows > 0x7fffffffu ||
+      !o->d_count || !valid_windows(range_start_ns, window_ns, n_windows) ||
       (gauge && (!o->d_sum || !o->d_min || !o->d_max)) ||
       (counter && (!o->d_counter_sum || !o->d_counter_min || !o->d_counter_max)))
-    return M3TSZ_ERR_INVALID_ARG;
-  if ((__int128)range_start_ns + (__int128)n_windows * (__int128)window_ns > (__int128)INT64_MAX)
     return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
@@ -348,20 +340,9 @@ static int decode_downsample_ex_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, 
       p.ds_isum_sq = (int64_t *)sc;
     }
   }
-  p.ds_ann = d_win_ann;
-  p.block_off = d_block_off;
-  p.n_segments = n_segments;
-  CK(launch_decode(p, opts->int_optimized != 0, d_win_ann ? (gauge ? 7 : 8) : (gauge ? 4 : 5), (cudaStream_t)stream));
+  CK(launch_decode(p, opts->int_optimized != 0, gauge ? 4 : 5, (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
-}
-
-int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                               uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
-                               uint64_t n_series, int64_t range_start_ns, int64_t window_ns, uint32_t n_windows,
-                               const m3tsz_downsample_outputs *o, void *stream) {
-  return decode_downsample_ex_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series,
-                                   range_start_ns, window_ns, n_windows, o, stream, nullptr);
 }
 
 int m3tsz_decode_downsample_batch(m3tsz_ctx *ctx, const m3tsz_options *opts,
@@ -669,39 +650,68 @@ int m3tsz_prom_convert_batch(m3tsz_ctx *ctx, const int64_t *d_ts, const double *
   return M3TSZ_OK;
 }
 
-// The transformation list of m3tsz_aggregate_tiles_transform, as the tile stage reads it: op k in bits 4k .. 4k + 3
-// of one word, 0 ending the list (a non-empty list is never 0).
+// The element a tile call writes, as the tile stages read it, and how its sources are addressed.  The
+// transformations: op k in bits 4k .. 4k + 3 of one word, 0 ending the list (a non-empty list is never 0).
 struct TileTransforms {
+  const int32_t *types = nullptr;  // output row j * n_src + s is source s under types[j]
+  uint32_t n_types = 0;
+  // the multi-type stage (m3tsz_aggregate_tiles_types and the calls built on it) with its element records, whatever
+  // n_types is; else the single-type stage of m3tsz_aggregate_tiles_ex / _transform
+  bool multi = false;
   uint32_t ops = 0;
   bool reset = false;  // a Reset op: two rows per window
-  int32_t discard_nan = 0;
-  m3tsz_transform_state *state = nullptr;
-  // m3tsz_aggregate_tiles_types: the element's types (n_types > 0: the multi-type stage, whatever `ops` is; the
-  // call's agg_type is then unused) and its records
-  const int32_t *types = nullptr;
-  uint32_t n_types = 0;
-  m3tsz_element_state *elem_state = nullptr;
-  bool annotated = false;  // m3tsz_aggregate_tiles_annotated (multi-type stage only): each window's annotation
-  // m3tsz_aggregate_tiles_blocks (multi-type stage only): offsets / lengths address n_segments segments, and series s
-  // is segments [block_off[s], block_off[s + 1])
+  // a NaN result writes nothing of its window.  The single-element calls discard only with a non-empty op list,
+  // which keeps m3tsz_aggregate_tiles_ex's bytes; the rollup whatever its lists are (DESIGN.md §4.8).
+  bool discard = false;
+  m3tsz_transform_state *state = nullptr;     // the single-type stage's records
+  m3tsz_element_state *elem_state = nullptr;  // the multi-type stage's records
+  bool annotated = false;                     // (multi-type stage only) each window's annotation
+  // over source blocks: offsets / lengths address n_segments segments, and series s is segments
+  // [block_off[s], block_off[s + 1])
   const uint64_t *block_off = nullptr;
   uint64_t n_segments = 0;
 };
 
-// The window-major aggregates of a tile call's fused decode, in context scratch ([n_windows][n_series] each)
+// The packed outputs of a tile call (m3tsz_aggregate_tiles_batch's align .. d_total_bytes)
+struct TileOutputs {
+  uint32_t align;
+  uint8_t *packed;
+  uint64_t capacity;
+  uint64_t *offsets, *len;
+  int32_t *status;
+  uint32_t *n_tiles;
+  uint64_t *total_bytes;
+};
+
+static bool valid_packing(const TileOutputs &o) {
+  return valid_align(o.align) && o.packed && o.offsets && o.len && !((uintptr_t)o.packed & 63u);
+}
+
+// Window-major aggregates ([n_windows][n_src] each) in context scratch: the fused decode's of the sources, or the
+// rollup's of its groups, in the same representation.  sst: each source's status.
 struct TileWindows {
   void *sum = nullptr, *cnt = nullptr, *min = nullptr, *max = nullptr, *last = nullptr, *lat = nullptr;
   void *sst = nullptr, *np = nullptr, *sq = nullptr, *ann = nullptr;
 };
 
-// Step 1 of every tile call: the fused decode + windows of the types' metric: the Gauge with `last` (mode 2), + sumSq
-// if a type is SumSq / Stdev (mode 4), or the Counter (mode 5, its int64 sum / min / max in the Gauge's slots);
-// `annotated`: + each window's annotation reference (modes 6-8).
+// the windows keep sumSq for SumSq / Stdev, and always for the Counter
+static bool needs_sum_sq(bool counter, const int32_t *types, uint32_t n) {
+  bool sq = counter;
+  for (uint32_t j = 0; j < n; j++) sq |= types[j] == M3TSZ_AGG_SUMSQ || types[j] == M3TSZ_AGG_STDEV;
+  return sq;
+}
+
+// Step 1 of every tile call: the fused decode + windows of the sources: the Gauge with `last` (mode 2), + sumSq if a
+// type needs it (mode 4), or the Counter (mode 5, its int64 sum / min / max in the Gauge's slots); xf.annotated:
+// + each window's annotation reference (modes 6-8).
 static int tiles_decode(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams, uint64_t streams_bytes,
                         const uint64_t *d_offsets, const uint64_t *d_lengths, uint64_t n_series, int64_t start_ns,
-                        int64_t step_ns, uint32_t n_windows, bool counter, const int32_t *types, uint32_t n_types,
-                        bool annotated, const uint64_t *block_off, uint64_t n_segments, cudaStream_t st,
+                        int64_t step_ns, uint32_t n_windows, bool counter, const TileTransforms &xf, cudaStream_t st,
                         TileWindows &w) {
+  DecodeParams p;
+  if (!decode_params(opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, nullptr, nullptr, p))
+    return M3TSZ_ERR_INVALID_ARG;
+  const bool sq = needs_sum_sq(counter, xf.types, xf.n_types);
   const size_t wb = (size_t)n_series * n_windows * 8;
   int rc;
   if ((rc = ensure(ctx, kSlotWinSum, wb, &w.sum))) return rc;
@@ -712,186 +722,160 @@ static int tiles_decode(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t
   if ((rc = ensure(ctx, kSlotWinLast, wb, &w.last))) return rc;
   if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &w.np))) return rc;
   if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &w.sst))) return rc;
-  if (annotated && (rc = ensure(ctx, kSlotWinAnn, wb, &w.ann))) return rc;
-  bool sq = counter;
-  for (uint32_t j = 0; j < n_types; j++) sq |= types[j] == M3TSZ_AGG_SUMSQ || types[j] == M3TSZ_AGG_STDEV;
-  if (!sq)
-    return downsample_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                           n_windows, (double *)w.sum, (int64_t *)w.cnt, (double *)w.min, (double *)w.max,
-                           (double *)w.last, (int64_t *)w.lat, true, (uint32_t *)w.np, (int32_t *)w.sst, st,
-                           (uint64_t *)w.ann, block_off, n_segments);
-  if ((rc = ensure(ctx, kSlotWinSumSq, wb, &w.sq))) return rc;
-  m3tsz_downsample_outputs o;
-  memset(&o, 0, sizeof(o));
-  o.metric_type = counter ? M3TSZ_METRIC_COUNTER : M3TSZ_METRIC_GAUGE;
-  o.d_count = (int64_t *)w.cnt;
+  if (xf.annotated && (rc = ensure(ctx, kSlotWinAnn, wb, &w.ann))) return rc;
+  if (sq && (rc = ensure(ctx, kSlotWinSumSq, wb, &w.sq))) return rc;
+  p.n_points = (uint32_t *)w.np;
+  p.status = (int32_t *)w.sst;
+  p.range_start = start_ns;
+  p.window = step_ns;
+  p.n_windows = n_windows;
+  p.ds_count = (int64_t *)w.cnt;
   if (counter) {
-    o.d_counter_sum = (int64_t *)w.sum;
-    o.d_counter_min = (int64_t *)w.min;
-    o.d_counter_max = (int64_t *)w.max;
-    o.d_counter_sum_sq = (int64_t *)w.sq;
+    p.ds_isum = (int64_t *)w.sum;
+    p.ds_imin = (int64_t *)w.min;
+    p.ds_imax = (int64_t *)w.max;
+    p.ds_isum_sq = (int64_t *)w.sq;
   } else {
-    o.d_sum = (double *)w.sum;
-    o.d_min = (double *)w.min;
-    o.d_max = (double *)w.max;
-    o.d_sum_sq = (double *)w.sq;
-    o.d_last = (double *)w.last;
-    o.d_last_at = (int64_t *)w.lat;
+    p.ds_sum = (double *)w.sum;
+    p.ds_min = (double *)w.min;
+    p.ds_max = (double *)w.max;
+    p.ds_sum_sq = (double *)w.sq;
+    p.ds_last = (double *)w.last;
+    p.ds_last_at = (int64_t *)w.lat;
   }
-  o.d_n_points = (uint32_t *)w.np;
-  o.d_status = (int32_t *)w.sst;
-  return decode_downsample_ex_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
-                                   step_ns, n_windows, &o, st, (uint64_t *)w.ann, block_off, n_segments);
+  p.ds_ann = (uint64_t *)w.ann;
+  p.block_off = xf.block_off;
+  p.n_segments = xf.n_segments;
+  const int mode = xf.annotated ? (counter ? 8 : sq ? 7 : 6) : (counter ? 5 : sq ? 4 : 2);
+  CK(launch_decode(p, opts->int_optimized != 0, mode, st));
+  ctx->launches++;
+  return M3TSZ_OK;
 }
 
-// The window aggregates of a tile call as the tile stages read them: window-major [n_windows][n_src] (IN = 2 / 4
-// read n_src = p.n_series, the multi-type stage p.tile_n_src)
-static void tile_inputs(EncodeParams &p, bool counter, void *sum, void *cnt, void *min, void *max, void *last,
-                        void *sq) {
-  p.tile_count = (const int64_t *)cnt;
+// The window aggregates as the tile stages read them: window-major [n_windows][n_src] (IN = 2 / 4 read
+// n_src = p.n_series, the multi-type stage p.tile_n_src)
+static void tile_inputs(EncodeParams &p, bool counter, const TileWindows &w) {
+  p.tile_count = (const int64_t *)w.cnt;
   if (counter) {
-    p.tile_isum = (const int64_t *)sum;
-    p.tile_imin = (const int64_t *)min;
-    p.tile_imax = (const int64_t *)max;
+    p.tile_isum = (const int64_t *)w.sum;
+    p.tile_imin = (const int64_t *)w.min;
+    p.tile_imax = (const int64_t *)w.max;
   } else {
-    p.tile_sum = (const double *)sum;
-    p.tile_min = (const double *)min;
-    p.tile_max = (const double *)max;
-    p.tile_last = (const double *)last;
+    p.tile_sum = (const double *)w.sum;
+    p.tile_min = (const double *)w.min;
+    p.tile_max = (const double *)w.max;
+    p.tile_last = (const double *)w.last;
   }
-  p.tile_sum_sq = sq;  // (NULL unless SumSq / Stdev / Counter)
+  p.tile_sum_sq = w.sq;  // (NULL unless SumSq / Stdev / Counter)
 }
 
-// Every tile call, after the caller checked ctx, opts, d_total_bytes, d_status, the (metric, type) pairs and the
-// transformation list (xf.ops == 0: none, the stage of m3tsz_aggregate_tiles_ex).  One decode + windows serves every
-// type of xf.types; output row j * n_series + s is series s, type j.
-static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                                uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
-                                uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
-                                int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
-                                uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
-                                uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
-                                uint64_t *d_total_bytes, void *stream, const TileTransforms &xf = TileTransforms()) {
-  cudaStream_t st = (cudaStream_t)stream;
-  if (n_series == 0) {
-    DeviceGuard guard(ctx->device);
-    CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
-    return M3TSZ_OK;
-  }
-  if (!valid_align(align) || !d_packed || !d_out_offsets || !d_out_len || ((uintptr_t)d_packed & 63u))
-    return M3TSZ_ERR_INVALID_ARG;
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
-  // context scratch: window-major aggregates, then series-major tiles
-  void *d_es = nullptr;
+// Step 2 of every tile call: the element xf over the windows w of n_src sources, re-encoded straight into the packed
+// outputs (the encoder's input stage skips empty windows, stamps the window end and takes Gauge.ValueOf(type)), then
+// the status pass: a failed source's error goes to all its rows.  With xf.annotated the rows copy annotations of the
+// source streams d_streams / d_offsets / d_lengths.
+static int tiles_encode(m3tsz_ctx *ctx, const m3tsz_options *opts, const TileWindows &w, uint64_t n_src,
+                        int64_t start_ns, int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t out_unit,
+                        const TileTransforms &xf, const uint8_t *d_streams, uint64_t streams_bytes,
+                        const uint64_t *d_offsets, const uint64_t *d_lengths, const TileOutputs &out,
+                        cudaStream_t st) {
+  CK(cudaMemsetAsync(out.total_bytes, 0, sizeof(uint64_t), st));
+  const uint64_t n_rows = (uint64_t)xf.n_types * n_src;
+  if (n_rows == 0) return M3TSZ_OK;  // (a rollup without groups)
   int rc;
-  // 1. fused decode + windows (one decode for all the types)
-  const bool multi = xf.n_types > 0;
-  const uint32_t n_types = multi ? xf.n_types : 1u;
-  const int32_t *types = multi ? xf.types : &agg_type;
-  const uint64_t n_rows = (uint64_t)n_types * n_series;
-  const bool counter = metric_type == M3TSZ_METRIC_COUNTER;
-  TileWindows win;
-  if ((rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                         n_windows, counter, types, n_types, xf.annotated, xf.block_off, xf.n_segments, st, win)))
-    return rc;
-  void *d_sst = win.sst, *d_ann = win.ann;
-  // 2. re-encode straight from the window-major aggregates (the encoder's input stage skips empty
-  //    windows, stamps the window end and takes Gauge.ValueOf(agg_type)) into the packed buffer
-  CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
-  EncodeParams p;
-  memset(&p, 0, sizeof(p));
   // (a Reset op writes up to two datapoints per window)
-  const uint64_t rows = xf.reset ? 2ull * n_windows : (uint64_t)n_windows;
-  uint64_t slot_bytes = m3tsz_encode_bound(rows);
+  uint64_t slot_bytes = m3tsz_encode_bound(xf.reset ? 2ull * n_windows : (uint64_t)n_windows);
   if (xf.annotated) {
     // a row's annotations are copies of different annotations of its source stream: the slots also take the longest
     // source stream of the call (over source blocks: the largest sum of a series' block lengths)
     void *d_mx = nullptr;
     if ((rc = ensure(ctx, kSlotSrcMaxLen, 8, &d_mx))) return rc;
     CK(cudaMemsetAsync(d_mx, 0, 8, st));
-    if (xf.block_off)
-      CK(launch_max_series_blocks_len(d_offsets, d_lengths, xf.block_off, n_series, xf.n_segments, streams_bytes,
-                                      (unsigned long long *)d_mx, st));
-    else
-      CK(launch_max_stream_len(d_offsets, d_lengths, n_series, streams_bytes, (unsigned long long *)d_mx, st));
+    CK(launch_max_stream_len(d_offsets, d_lengths, xf.block_off, n_src, xf.n_segments, streams_bytes,
+                             (unsigned long long *)d_mx, st));
     ctx->launches++;
     uint64_t mx = 0;
     CK(cudaMemcpyAsync(&mx, d_mx, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     slot_bytes = (slot_bytes + mx + 15) & ~15ull;
   }
-  if ((rc = packed_params(ctx, n_rows, slot_bytes, align, d_packed, packed_capacity,
-                          d_out_offsets, d_total_bytes, st, p)))
+  EncodeParams p;
+  memset(&p, 0, sizeof(p));
+  if ((rc = packed_params(ctx, n_rows, slot_bytes, out.align, out.packed, out.capacity, out.offsets,
+                          out.total_bytes, st, p)))
     return rc;
   // every row's encoder starts at the tile range's start (the target block's start)
+  void *d_es = nullptr, *d_rec = nullptr;
   if ((rc = ensure(ctx, kSlotTileStarts, n_rows * 8, &d_es))) return rc;
   CK(launch_fill_i64((int64_t *)d_es, start_ns, n_rows, st));
+  // lanes write their parts of each source's new element record to scratch; the status pass commits whole records
+  if (xf.elem_state && (rc = ensure(ctx, kSlotElementScratch, n_src * sizeof(m3tsz_element_state), &d_rec)))
+    return rc;
   p.n_series = n_rows;
   p.points_stride = n_windows;
   p.start = (const int64_t *)d_es;
   p.unit = out_unit;
   p.default_unit = opts->default_time_unit;
-  p.out_len = d_out_len;
-  p.status = d_status;
-  p.in_mode = 2;
-  tile_inputs(p, counter, win.sum, win.cnt, win.min, win.max, win.last, win.sq);
-  p.tile_src_status = (const int32_t *)d_sst;
+  p.out_len = out.len;
+  p.status = out.status;
+  tile_inputs(p, metric_type == M3TSZ_METRIC_COUNTER, w);
+  p.tile_src_status = (const int32_t *)w.sst;
   p.tile_start = start_ns;
   p.tile_step = step_ns;
-  p.agg_type = agg_type;
+  p.agg_type = xf.types[0];
   p.metric_type = metric_type;
-  p.n_tiles_out = d_n_tiles;
-  void *d_rec = nullptr;
-  if (multi) {
-    // lanes write their parts of each series' new record to scratch; the status pass commits whole records
-    if (xf.elem_state && (rc = ensure(ctx, kSlotElementScratch, n_series * sizeof(m3tsz_element_state), &d_rec)))
-      return rc;
+  p.n_tiles_out = out.n_tiles;
+  p.xf_ops = xf.ops;
+  p.xf_discard_nan = xf.discard ? 1 : 0;
+  if (xf.multi) {
     p.in_mode = 5;
     if (xf.annotated) {
       p.in_mode = xf.block_off ? 7 : 6;  // (7: the references hold the payload's bit offset in the whole batch)
-      p.tile_ann = (const uint64_t *)d_ann;
+      p.tile_ann = (const uint64_t *)w.ann;
       p.tile_src_streams = d_streams;
       if (!xf.block_off) p.tile_src_off = d_offsets;
     }
-    p.xf_ops = xf.ops;
-    p.xf_discard_nan = (xf.ops && xf.discard_nan) ? 1 : 0;  // (an empty list discards nothing, as tiles_ex)
     p.xf_elem = xf.elem_state;
     p.xf_elem_out = (m3tsz_element_state *)d_rec;
-    p.tile_n_src = n_series;
-    p.tile_n_types = n_types;
-    for (uint32_t j = 0; j < n_types; j++) p.tile_types |= (uint32_t)types[j] << (4 * j);
+    p.tile_n_src = n_src;
+    p.tile_n_types = xf.n_types;
+    for (uint32_t j = 0; j < xf.n_types; j++) p.tile_types |= (uint32_t)xf.types[j] << (4 * j);
   } else if (xf.ops) {
     p.in_mode = 4;
-    p.xf_ops = xf.ops;
-    p.xf_discard_nan = xf.discard_nan ? 1 : 0;
     p.xf_state = xf.state;
+  } else {
+    p.in_mode = 2;
   }
   CK(launch_encode(p, opts->int_optimized != 0, st));
   ctx->launches += 2;
-  if (multi)
-    CK(launch_tiles_types_status((const int32_t *)d_sst, d_status, n_series, n_types,
-                                 (const m3tsz_element_state *)d_rec, xf.elem_state, st));
-  else
-    CK(launch_tiles_status((const int32_t *)d_sst, d_status, n_series, st));
+  CK(launch_tiles_types_status((const int32_t *)w.sst, out.status, n_src, xf.n_types,
+                               (const m3tsz_element_state *)d_rec, xf.elem_state, st));
   ctx->launches++;
   return M3TSZ_OK;
 }
 
-int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                                uint64_t streams_bytes, const uint64_t *d_offsets,
-                                const uint64_t *d_lengths, uint64_t n_series, int64_t start_ns,
-                                int64_t step_ns, uint32_t n_windows, int32_t agg_type, int32_t out_unit,
-                                uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
-                                uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
-                                uint32_t *d_n_tiles, uint64_t *d_total_bytes, void *stream) {
-  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status) return M3TSZ_ERR_INVALID_ARG;
-  if (!(agg_type == M3TSZ_AGG_LAST || agg_type == M3TSZ_AGG_MIN || agg_type == M3TSZ_AGG_MAX ||
-        agg_type == M3TSZ_AGG_MEAN || agg_type == M3TSZ_AGG_COUNT || agg_type == M3TSZ_AGG_SUM))
-    return M3TSZ_ERR_INVALID_ARG;
-  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                              n_windows, M3TSZ_METRIC_GAUGE, agg_type, out_unit, align, d_packed, packed_capacity,
-                              d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream);
+// Every tile call but the rollup, after the caller checked its element: the fused decode, then the element stage.
+static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                                int32_t metric_type, int32_t out_unit, const TileTransforms &xf,
+                                const TileOutputs &out, void *stream) {
+  if (!ctx || !valid_opts(opts) || !out.total_bytes || !out.status) return M3TSZ_ERR_INVALID_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n_series == 0) {
+    DeviceGuard guard(ctx->device);
+    CK(cudaMemsetAsync(out.total_bytes, 0, sizeof(uint64_t), st));
+    return M3TSZ_OK;
+  }
+  if (!valid_packing(out) || !valid_windows(start_ns, step_ns, n_windows)) return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  TileWindows win;
+  int rc;
+  if ((rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                         n_windows, metric_type == M3TSZ_METRIC_COUNTER, xf, st, win)))
+    return rc;
+  return tiles_encode(ctx, opts, win, n_series, start_ns, step_ns, n_windows, metric_type, out_unit, xf, d_streams,
+                      streams_bytes, d_offsets, d_lengths, out, st);
 }
 
 // aggregation.Type.IsValidForGauge / IsValidForCounter, src/metrics/aggregation/type.go:178-196
@@ -903,20 +887,6 @@ static bool valid_tile_pair(int32_t metric_type, int32_t agg_type) {
       return metric_type == M3TSZ_METRIC_GAUGE || metric_type == M3TSZ_METRIC_COUNTER;
     default: return false;
   }
-}
-
-int m3tsz_aggregate_tiles_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                             uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
-                             uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
-                             int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
-                             uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
-                             uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
-                             uint64_t *d_total_bytes, void *stream) {
-  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !valid_tile_pair(metric_type, agg_type))
-    return M3TSZ_ERR_INVALID_ARG;
-  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                              n_windows, metric_type, agg_type, out_unit, align, d_packed, packed_capacity,
-                              d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream);
 }
 
 // newParsedPipeline (aggregator/elem_base.go:682-752): known types, derivative order <= 1
@@ -932,6 +902,58 @@ static bool parse_transforms(const int32_t *ops, uint32_t n_ops, TileTransforms 
   return binary <= 1;
 }
 
+// An element of the multi-type stage: its types strictly ascending (idDecompressor.Decompress walks a bitset), each
+// valid for the metric, its transformations, and its records
+static bool parse_element(int32_t metric_type, const int32_t *types, uint32_t n_types, const int32_t *ops,
+                          uint32_t n_ops, m3tsz_element_state *state, TileTransforms &xf) {
+  if (!types || n_types == 0 || n_types > M3TSZ_MAX_ELEMENT_TYPES) return false;
+  for (uint32_t j = 0; j < n_types; j++)
+    if (!valid_tile_pair(metric_type, types[j]) || (j && types[j] <= types[j - 1])) return false;
+  xf.types = types;
+  xf.n_types = n_types;
+  xf.multi = true;
+  xf.elem_state = state;
+  return parse_transforms(ops, n_ops, xf);
+}
+
+int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                uint64_t streams_bytes, const uint64_t *d_offsets,
+                                const uint64_t *d_lengths, uint64_t n_series, int64_t start_ns,
+                                int64_t step_ns, uint32_t n_windows, int32_t agg_type, int32_t out_unit,
+                                uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+                                uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
+                                uint32_t *d_n_tiles, uint64_t *d_total_bytes, void *stream) {
+  if (!(agg_type == M3TSZ_AGG_LAST || agg_type == M3TSZ_AGG_MIN || agg_type == M3TSZ_AGG_MAX ||
+        agg_type == M3TSZ_AGG_MEAN || agg_type == M3TSZ_AGG_COUNT || agg_type == M3TSZ_AGG_SUM))
+    return M3TSZ_ERR_INVALID_ARG;
+  TileTransforms xf;
+  xf.types = &agg_type;
+  xf.n_types = 1;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, M3TSZ_METRIC_GAUGE, out_unit, xf,
+                              {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles,
+                               d_total_bytes},
+                              stream);
+}
+
+int m3tsz_aggregate_tiles_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                             uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                             uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
+                             int32_t metric_type, int32_t agg_type, int32_t out_unit, uint32_t align,
+                             uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                             uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
+                             uint64_t *d_total_bytes, void *stream) {
+  if (!valid_tile_pair(metric_type, agg_type)) return M3TSZ_ERR_INVALID_ARG;
+  TileTransforms xf;
+  xf.types = &agg_type;
+  xf.n_types = 1;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, metric_type, out_unit, xf,
+                              {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles,
+                               d_total_bytes},
+                              stream);
+}
+
 int m3tsz_aggregate_tiles_transform(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                                     uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
                                     uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
@@ -940,47 +962,17 @@ int m3tsz_aggregate_tiles_transform(m3tsz_ctx *ctx, const m3tsz_options *opts, c
                                     uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles,
                                     uint64_t *d_total_bytes, const int32_t *ops, uint32_t n_ops,
                                     int32_t discard_nan, m3tsz_transform_state *d_state, void *stream) {
-  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !valid_tile_pair(metric_type, agg_type))
-    return M3TSZ_ERR_INVALID_ARG;
   TileTransforms xf;
-  if (!parse_transforms(ops, n_ops, xf)) return M3TSZ_ERR_INVALID_ARG;
-  xf.discard_nan = discard_nan;
+  if (!valid_tile_pair(metric_type, agg_type) || !parse_transforms(ops, n_ops, xf)) return M3TSZ_ERR_INVALID_ARG;
+  xf.types = &agg_type;
+  xf.n_types = 1;
+  xf.discard = xf.ops && discard_nan;
   xf.state = d_state;
   return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                              n_windows, metric_type, agg_type, out_unit, align, d_packed, packed_capacity,
-                              d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream, xf);
-}
-
-// m3tsz_aggregate_tiles_types and m3tsz_aggregate_tiles_annotated
-static int aggregate_tiles_types_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                                      uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
-                                      uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
-                                      int32_t metric_type, const int32_t *agg_types, uint32_t n_types,
-                                      int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
-                                      uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status,
-                                      uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
-                                      uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
-                                      void *stream, bool annotated, const uint64_t *d_block_off = nullptr,
-                                      uint64_t n_segments = 0) {
-  if (!ctx || !valid_opts(opts) || !d_total_bytes || !d_status || !agg_types || n_types == 0 ||
-      n_types > M3TSZ_MAX_ELEMENT_TYPES)
-    return M3TSZ_ERR_INVALID_ARG;
-  // an element's types: strictly ascending (idDecompressor.Decompress walks a bitset), each valid for the metric
-  for (uint32_t j = 0; j < n_types; j++)
-    if (!valid_tile_pair(metric_type, agg_types[j]) || (j && agg_types[j] <= agg_types[j - 1]))
-      return M3TSZ_ERR_INVALID_ARG;
-  TileTransforms xf;
-  if (!parse_transforms(ops, n_ops, xf)) return M3TSZ_ERR_INVALID_ARG;
-  xf.discard_nan = discard_nan;
-  xf.types = agg_types;
-  xf.n_types = n_types;
-  xf.elem_state = d_state;
-  xf.annotated = annotated;
-  xf.block_off = d_block_off;
-  xf.n_segments = n_segments;
-  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                              n_windows, metric_type, agg_types[0], out_unit, align, d_packed, packed_capacity,
-                              d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes, stream, xf);
+                              n_windows, metric_type, out_unit, xf,
+                              {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles,
+                               d_total_bytes},
+                              stream);
 }
 
 int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
@@ -992,10 +984,14 @@ int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const
                                 uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
                                 uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
                                 void *stream) {
-  return aggregate_tiles_types_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
-                                    step_ns, n_windows, metric_type, agg_types, n_types, out_unit, align, d_packed,
-                                    packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes,
-                                    ops, n_ops, discard_nan, d_state, stream, false);
+  TileTransforms xf;
+  if (!parse_element(metric_type, agg_types, n_types, ops, n_ops, d_state, xf)) return M3TSZ_ERR_INVALID_ARG;
+  xf.discard = xf.ops && discard_nan;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, metric_type, out_unit, xf,
+                              {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles,
+                               d_total_bytes},
+                              stream);
 }
 
 int m3tsz_aggregate_tiles_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
@@ -1007,10 +1003,15 @@ int m3tsz_aggregate_tiles_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, c
                                     uint32_t *d_n_tiles, uint64_t *d_total_bytes, const int32_t *ops,
                                     uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
                                     void *stream) {
-  return aggregate_tiles_types_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
-                                    step_ns, n_windows, metric_type, agg_types, n_types, out_unit, align, d_packed,
-                                    packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes,
-                                    ops, n_ops, discard_nan, d_state, stream, true);
+  TileTransforms xf;
+  if (!parse_element(metric_type, agg_types, n_types, ops, n_ops, d_state, xf)) return M3TSZ_ERR_INVALID_ARG;
+  xf.discard = xf.ops && discard_nan;
+  xf.annotated = true;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, metric_type, out_unit, xf,
+                              {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles,
+                               d_total_bytes},
+                              stream);
 }
 
 int m3tsz_aggregate_tiles_blocks(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
@@ -1023,12 +1024,18 @@ int m3tsz_aggregate_tiles_blocks(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
                                  uint32_t n_ops, int32_t discard_nan, m3tsz_element_state *d_state,
                                  int32_t annotations, void *stream) {
   // (the block table's ranges are checked per series on the device: a bad one is that series' INVALID_ARG)
-  if (!d_block_off) return M3TSZ_ERR_INVALID_ARG;
-  return aggregate_tiles_types_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
-                                    step_ns, n_windows, metric_type, agg_types, n_types, out_unit, align, d_packed,
-                                    packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes,
-                                    ops, n_ops, discard_nan, d_state, stream, annotations != 0, d_block_off,
-                                    n_segments);
+  TileTransforms xf;
+  if (!d_block_off || !parse_element(metric_type, agg_types, n_types, ops, n_ops, d_state, xf))
+    return M3TSZ_ERR_INVALID_ARG;
+  xf.discard = xf.ops && discard_nan;
+  xf.annotated = annotations != 0;
+  xf.block_off = d_block_off;
+  xf.n_segments = n_segments;
+  return aggregate_tiles_impl(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+                              n_windows, metric_type, out_unit, xf,
+                              {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles,
+                               d_total_bytes},
+                              stream);
 }
 
 // Tile aggregation through a rollup (DESIGN.md §4.8): the fused decode of the sources under src_type, the forward
@@ -1046,21 +1053,15 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
                                  uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
                                  uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
                                  int32_t *d_src_status, void *stream) {
-  if (!ctx || !valid_opts(opts) || !d_total_bytes || !valid_tile_pair(metric_type, src_type) || !rollup_types ||
-      n_rollup_types == 0 || n_rollup_types > M3TSZ_MAX_ELEMENT_TYPES || (!d_block_off && n_segments != n_series) ||
-      (n_groups && (!d_group_off || !d_status)) || (n_members && !d_members))
+  TileTransforms pre, post;  // the sources' element and the groups'
+  if (!ctx || !valid_opts(opts) || !d_total_bytes || !valid_tile_pair(metric_type, src_type) ||
+      (!d_block_off && n_segments != n_series) || (n_groups && (!d_group_off || !d_status)) ||
+      (n_members && !d_members) || !parse_transforms(pre_ops, n_pre_ops, pre) ||
+      !parse_element(metric_type, rollup_types, n_rollup_types, post_ops, n_post_ops, d_group_state, post))
     return M3TSZ_ERR_INVALID_ARG;
-  for (uint32_t j = 0; j < n_rollup_types; j++)
-    if (!valid_tile_pair(metric_type, rollup_types[j]) || (j && rollup_types[j] <= rollup_types[j - 1]))
-      return M3TSZ_ERR_INVALID_ARG;
-  TileTransforms pre, post;
-  if (!parse_transforms(pre_ops, n_pre_ops, pre) || !parse_transforms(post_ops, n_post_ops, post))
-    return M3TSZ_ERR_INVALID_ARG;
-  const uint64_t n_rows = (uint64_t)n_rollup_types * n_groups;
-  if (n_rows && (!valid_align(align) || !d_packed || !d_out_offsets || !d_out_len || ((uintptr_t)d_packed & 63u)))
-    return M3TSZ_ERR_INVALID_ARG;
-  if (n_windows == 0 || n_windows > 0x7fffffffu || step_ns <= 0 ||
-      (__int128)start_ns + (__int128)n_windows * (__int128)step_ns > (__int128)INT64_MAX)
+  const TileOutputs out{align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles,
+                        d_total_bytes};
+  if (((uint64_t)n_rollup_types * n_groups != 0 && !valid_packing(out)) || !valid_windows(start_ns, step_ns, n_windows))
     return M3TSZ_ERR_INVALID_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   DeviceGuard guard(ctx->device);
@@ -1068,10 +1069,13 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   const bool counter = metric_type == M3TSZ_METRIC_COUNTER;
   int rc;
   // 1. fused decode + windows of the sources under their one type
+  pre.types = &src_type;
+  pre.n_types = 1;
+  pre.block_off = d_block_off;
+  pre.n_segments = n_segments;
   TileWindows win;
-  if (n_series &&
-      (rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
-                         n_windows, counter, &src_type, 1, false, d_block_off, n_segments, st, win)))
+  if (n_series && (rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
+                                     step_ns, n_windows, counter, pre, st, win)))
     return rc;
   // 2. forward stage: series-major forwarded values and presence words, each source's new record to scratch
   const uint32_t n_words = (n_windows + 31) / 32;
@@ -1082,7 +1086,7 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   if ((rc = ensure(ctx, kSlotSrcMark, n_series, &d_mark))) return rc;
   RollupForwardParams fp;
   memset(&fp, 0, sizeof(fp));
-  tile_inputs(fp.tiles, counter, win.sum, win.cnt, win.min, win.max, win.last, win.sq);
+  tile_inputs(fp.tiles, counter, win);
   fp.tiles.metric_type = metric_type;
   fp.tiles.tile_start = start_ns;
   fp.tiles.tile_step = step_ns;
@@ -1101,17 +1105,15 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   ctx->launches++;
   // 3. fold: the groups' window-major aggregates, in the fused decode's representation, and their statuses
   const size_t gb = (size_t)n_groups * n_windows * 8;
-  bool sq = counter;
-  for (uint32_t j = 0; j < n_rollup_types; j++)
-    sq |= rollup_types[j] == M3TSZ_AGG_SUMSQ || rollup_types[j] == M3TSZ_AGG_STDEV;
-  void *g_sum, *g_cnt, *g_min, *g_max, *g_last = nullptr, *g_sq = nullptr, *g_st;
-  if ((rc = ensure(ctx, kSlotGroupSum, gb, &g_sum))) return rc;
-  if ((rc = ensure(ctx, kSlotGroupCount, gb, &g_cnt))) return rc;
-  if ((rc = ensure(ctx, kSlotGroupMin, gb, &g_min))) return rc;
-  if ((rc = ensure(ctx, kSlotGroupMax, gb, &g_max))) return rc;
-  if (!counter && (rc = ensure(ctx, kSlotGroupLast, gb, &g_last))) return rc;
-  if (sq && (rc = ensure(ctx, kSlotGroupSumSq, gb, &g_sq))) return rc;
-  if ((rc = ensure(ctx, kSlotGroupStatus, n_groups * 4, &g_st))) return rc;
+  TileWindows grp;
+  if ((rc = ensure(ctx, kSlotGroupSum, gb, &grp.sum))) return rc;
+  if ((rc = ensure(ctx, kSlotGroupCount, gb, &grp.cnt))) return rc;
+  if ((rc = ensure(ctx, kSlotGroupMin, gb, &grp.min))) return rc;
+  if ((rc = ensure(ctx, kSlotGroupMax, gb, &grp.max))) return rc;
+  if (!counter && (rc = ensure(ctx, kSlotGroupLast, gb, &grp.last))) return rc;
+  if (needs_sum_sq(counter, rollup_types, n_rollup_types) && (rc = ensure(ctx, kSlotGroupSumSq, gb, &grp.sq)))
+    return rc;
+  if ((rc = ensure(ctx, kSlotGroupStatus, n_groups * 4, &grp.sst))) return rc;
   RollupFoldParams gp;
   memset(&gp, 0, sizeof(gp));
   gp.fwd = (const double *)d_fwd;
@@ -1125,59 +1127,20 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   gp.n_members = n_members;
   gp.n_groups = n_groups;
   gp.counter = counter ? 1 : 0;
-  gp.sum = g_sum;
-  gp.count = (int64_t *)g_cnt;
-  gp.min = g_min;
-  gp.max = g_max;
-  gp.last = (double *)g_last;
-  gp.sum_sq = g_sq;
-  gp.group_status = (int32_t *)g_st;
+  gp.sum = grp.sum;
+  gp.count = (int64_t *)grp.cnt;
+  gp.min = grp.min;
+  gp.max = grp.max;
+  gp.last = (double *)grp.last;
+  gp.sum_sq = grp.sq;
+  gp.group_status = (int32_t *)grp.sst;
   CK(launch_rollup_fold(gp, st));
   ctx->launches++;
-  // 4. the rollup element: the multi-type stage over n_rollup_types * n_groups rows, the groups as its sources
-  CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
-  void *d_grec = nullptr;
-  if (n_rows) {
-    EncodeParams p;
-    memset(&p, 0, sizeof(p));
-    const uint64_t rows = post.reset ? 2ull * n_windows : (uint64_t)n_windows;
-    if ((rc = packed_params(ctx, n_rows, m3tsz_encode_bound(rows), align, d_packed, packed_capacity, d_out_offsets,
-                            d_total_bytes, st, p)))
-      return rc;
-    void *d_es = nullptr;
-    if ((rc = ensure(ctx, kSlotTileStarts, n_rows * 8, &d_es))) return rc;
-    CK(launch_fill_i64((int64_t *)d_es, start_ns, n_rows, st));
-    if (d_group_state &&
-        (rc = ensure(ctx, kSlotElementScratch, n_groups * sizeof(m3tsz_element_state), &d_grec)))
-      return rc;
-    p.n_series = n_rows;
-    p.points_stride = n_windows;
-    p.start = (const int64_t *)d_es;
-    p.unit = out_unit;
-    p.default_unit = opts->default_time_unit;
-    p.out_len = d_out_len;
-    p.status = d_status;
-    p.in_mode = 5;
-    tile_inputs(p, counter, g_sum, g_cnt, g_min, g_max, g_last, g_sq);
-    p.tile_src_status = (const int32_t *)g_st;
-    p.tile_start = start_ns;
-    p.tile_step = step_ns;
-    p.agg_type = rollup_types[0];
-    p.metric_type = metric_type;
-    p.n_tiles_out = d_n_tiles;
-    p.xf_ops = post.ops;
-    p.xf_discard_nan = discard_nan ? 1 : 0;
-    p.xf_elem = d_group_state;
-    p.xf_elem_out = (m3tsz_element_state *)d_grec;
-    p.tile_n_src = n_groups;
-    p.tile_n_types = n_rollup_types;
-    for (uint32_t j = 0; j < n_rollup_types; j++) p.tile_types |= (uint32_t)rollup_types[j] << (4 * j);
-    CK(launch_encode(p, opts->int_optimized != 0, st));
-    ctx->launches += 2;
-    CK(launch_tiles_types_status((const int32_t *)g_st, d_status, n_groups, n_rollup_types,
-                                 (const m3tsz_element_state *)d_grec, d_group_state, st));
-    ctx->launches++;
-  }
+  // 4. the rollup element over n_rollup_types * n_groups rows, the groups as its sources
+  post.discard = discard_nan != 0;
+  if ((rc = tiles_encode(ctx, opts, grp, n_groups, start_ns, step_ns, n_windows, metric_type, out_unit, post, nullptr,
+                         0, nullptr, nullptr, out, st)))
+    return rc;
   // 5. the source records: a source is saved when it decoded and every group that lists it was saved
   CK(launch_rollup_commit(d_group_off, d_members, n_members, n_groups, d_status, n_rollup_types,
                           (const int32_t *)win.sst, n_series, (uint8_t *)d_mark, (const m3tsz_transform_state *)d_srec,

@@ -258,18 +258,15 @@ cudaError_t launch_prom(const PromParams &p, cudaStream_t stream);
 
 // tile aggregation glue (m3tsz_query.cu)
 cudaError_t launch_fill_i64(int64_t *dst, int64_t v, uint64_t n, cudaStream_t stream);
-cudaError_t launch_tiles_status(const int32_t *src_status, int32_t *status, uint64_t n, cudaStream_t stream);
 // the longest stream of a batch (offsets + lengths, or CSR offsets) into *out (zeroed by the caller); streams the
-// decode refuses (outside the buffer, 2^28 bytes or more) are left out
-cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, uint64_t n, uint64_t streams_bytes,
+// decode refuses (outside the buffer, 2^28 bytes or more) are left out.  With block_off, over source blocks: the
+// largest sum, over series s, of the lengths of segments [block_off[s], block_off[s + 1]) (a series with an invalid
+// range counts 0); without, segment s is series s.
+cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
+                                  uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
                                   unsigned long long *out, cudaStream_t stream);
-// the same over source blocks: the largest sum, over series s, of the lengths of segments [block_off[s],
-// block_off[s + 1]) (segments the decode refuses count 0, and so does a series with an invalid range)
-cudaError_t launch_max_series_blocks_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
-                                         uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
-                                         unsigned long long *out, cudaStream_t stream);
-// the multi-type stage's: a failed source's error goes to all n_types rows of its series; with `state`, a series
-// whose source and rows are all OK takes its new record from `scratch`
+// a failed source's error goes to all n_types rows of its series; with `state`, a series whose source and rows are
+// all OK takes its new record from `scratch`
 cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status, uint64_t n, uint32_t n_types,
                                       const m3tsz_element_state *scratch, m3tsz_element_state *state,
                                       cudaStream_t stream);

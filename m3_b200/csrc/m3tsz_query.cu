@@ -142,21 +142,9 @@ cudaError_t launch_fill_i64(int64_t *dst, int64_t v, uint64_t n, cudaStream_t st
   return cudaGetLastError();
 }
 
-// status merge: a series whose source stream failed to decode reports that error
-__global__ void tiles_status_kernel(const int32_t *src_status, int32_t *status, uint64_t n) {
-  const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (s < n && src_status[s] != 0) status[s] = src_status[s];
-}
-cudaError_t launch_tiles_status(const int32_t *src_status, int32_t *status, uint64_t n, cudaStream_t stream) {
-  if (n == 0) return cudaSuccess;
-  const unsigned tb = 256;
-  tiles_status_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, stream>>>(src_status, status, n);
-  return cudaGetLastError();
-}
-
-// The multi-type stage's status merge and state commit (one thread per source series): a failed source's error goes
-// to all n_types rows of the series; a series whose source and rows are all OK takes the record its lanes wrote to
-// `scratch` (the encode kernel's IN = 5 epilogue)
+// Every tile call's status merge, and the multi-type stage's state commit (one thread per source series): a failed
+// source's error goes to all n_types rows of the series; a series whose source and rows are all OK takes the record
+// its lanes wrote to `scratch` (the encode kernel's IN = 5 epilogue)
 __global__ void tiles_types_status_kernel(const int32_t *src_status, int32_t *status, uint64_t n, uint32_t n_types,
                                           const m3tsz_element_state *scratch, m3tsz_element_state *state) {
   const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -229,44 +217,24 @@ cudaError_t launch_rollup_commit(const uint64_t *group_off, const uint32_t *memb
   return cudaGetLastError();
 }
 
-// The longest source stream of a tile call with annotations: the bound of an annotated row adds it (one warp-wide max
-// and one atomic per warp)
-__global__ void max_stream_len_kernel(const uint64_t *offsets, const uint64_t *lengths, uint64_t n,
-                                      uint64_t streams_bytes, unsigned long long *out) {
+// The room of a tile call with annotations: a row's annotations are copies of different annotations of its source
+// stream, or of any of its series' source blocks, so its bound adds the largest sum of a series' segment lengths (one
+// warp-wide max and one atomic per warp)
+__global__ void max_stream_len_kernel(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
+                                      uint64_t n, uint64_t n_segments, uint64_t streams_bytes,
+                                      unsigned long long *out) {
   const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   unsigned long long len = 0;
   if (s < n) {
-    const uint64_t o0 = offsets[s], o1 = lengths ? o0 + lengths[s] : offsets[s + 1];
-    if (o1 >= o0 && o1 <= streams_bytes && o1 - o0 < (1ull << 28)) len = o1 - o0;
-  }
-  for (int d = 16; d > 0; d >>= 1) {
-    const unsigned long long o = __shfl_xor_sync(0xffffffffu, len, d);
-    len = o > len ? o : len;
-  }
-  if ((threadIdx.x & 31) == 0 && len) atomicMax(out, len);
-}
-cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, uint64_t n, uint64_t streams_bytes,
-                                  unsigned long long *out, cudaStream_t stream) {
-  if (n == 0) return cudaSuccess;
-  const unsigned tb = 256;
-  max_stream_len_kernel<<<(unsigned)((n + tb - 1) / tb), tb, 0, stream>>>(offsets, lengths, n, streams_bytes, out);
-  return cudaGetLastError();
-}
-
-// The room of an annotated tile call over source blocks: a row's annotations are copies of different annotations of
-// any of its series' blocks, so its bound adds the sum of their lengths
-__global__ void max_series_blocks_len_kernel(const uint64_t *offsets, const uint64_t *lengths,
-                                             const uint64_t *block_off, uint64_t n, uint64_t n_segments,
-                                             uint64_t streams_bytes, unsigned long long *out) {
-  const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  unsigned long long len = 0;
-  if (s < n) {
-    const uint64_t q0 = block_off[s], q1 = block_off[s + 1];
-    if (q0 <= q1 && q1 <= n_segments) {
-      for (uint64_t q = q0; q < q1; q++) {
-        const uint64_t o0 = offsets[q], o1 = lengths ? o0 + lengths[q] : offsets[q + 1];
-        if (o1 >= o0 && o1 <= streams_bytes && o1 - o0 < (1ull << 28)) len += o1 - o0;
-      }
+    uint64_t q0 = s, q1 = s + 1;
+    if (block_off) {
+      q0 = block_off[s];
+      q1 = block_off[s + 1];
+      if (q0 > q1 || q1 > n_segments) q1 = q0;
+    }
+    for (uint64_t q = q0; q < q1; q++) {
+      const uint64_t o0 = offsets[q], o1 = lengths ? o0 + lengths[q] : offsets[q + 1];
+      if (o1 >= o0 && o1 <= streams_bytes && o1 - o0 < (1ull << 28)) len += o1 - o0;
     }
   }
   for (int d = 16; d > 0; d >>= 1) {
@@ -275,12 +243,12 @@ __global__ void max_series_blocks_len_kernel(const uint64_t *offsets, const uint
   }
   if ((threadIdx.x & 31) == 0 && len) atomicMax(out, len);
 }
-cudaError_t launch_max_series_blocks_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
-                                         uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
-                                         unsigned long long *out, cudaStream_t stream) {
+cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
+                                  uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
+                                  unsigned long long *out, cudaStream_t stream) {
   if (n_series == 0) return cudaSuccess;
   const unsigned tb = 256;
-  max_series_blocks_len_kernel<<<(unsigned)((n_series + tb - 1) / tb), tb, 0, stream>>>(
+  max_stream_len_kernel<<<(unsigned)((n_series + tb - 1) / tb), tb, 0, stream>>>(
       offsets, lengths, block_off, n_series, n_segments, streams_bytes, out);
   return cudaGetLastError();
 }
