@@ -891,6 +891,38 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
                                  uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
                                  int32_t *d_src_status, void *stream);
 
+/* Tile aggregation through a rollup that keeps annotations: the parameters and every rule of
+ * m3tsz_aggregate_tiles_rollup, plus the annotations the reference's rollup element keeps
+ * (Gauge / Counter Update's MaybeReplaceAnnotation, reached through AddUnique with the
+ * annotation each source window forwards).
+ *   - A source window forwards the annotation of m3tsz_aggregate_tiles_annotated (over source
+ *     blocks, of m3tsz_aggregate_tiles_blocks with annotations): the last one among its
+ *     datapoints, none if they carry none.
+ *   - The annotation of window w of group g is the last non-empty one, in listed member order,
+ *     among the members whose value for w was forwarded (a NaN that discard_nan drops is not;
+ *     one forwarded with discard_nan 0 is).  Every row of the group, a Reset op's extra
+ *     datapoint included, writes its datapoints of w with that annotation, which the encoder
+ *     writes only when it differs from the last one written.  No annotation crosses calls.
+ *   - Values, counts, statuses and records are those of m3tsz_aggregate_tiles_rollup; with no
+ *     annotated source the bytes are too.
+ *   - A source window annotation of 2^27 bytes or more gives that source
+ *     M3TSZ_ERR_STREAM_TOO_LARGE, which goes to every group that lists it.
+ *   - Room: a row also takes, for copies of its members' annotations, the largest sum over
+ *     groups of the members' source stream lengths (summed over their blocks); a row that does
+ *     not fit gets M3TSZ_ERR_CAPACITY.  Every encode scratch slot takes that room, so one wide
+ *     group raises the call's device scratch (DESIGN.md §4.8); a call that cannot allocate it
+ *     returns M3TSZ_ERR_CUDA. */
+int m3tsz_aggregate_tiles_rollup_annotated(
+    m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams, uint64_t streams_bytes,
+    const uint64_t *d_offsets, const uint64_t *d_lengths, uint64_t n_segments, const uint64_t *d_block_off,
+    uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t src_type,
+    const int32_t *pre_ops, uint32_t n_pre_ops, const uint64_t *d_group_off, const uint32_t *d_members,
+    uint64_t n_members, uint64_t n_groups, const int32_t *rollup_types, uint32_t n_rollup_types,
+    const int32_t *post_ops, uint32_t n_post_ops, int32_t discard_nan, m3tsz_transform_state *d_src_state,
+    m3tsz_element_state *d_group_state, int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+    uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
+    int32_t *d_src_status, void *stream);
+
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the
  * reference's interfaces (INTEGRATION.md §2 is that shim):

@@ -114,7 +114,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_encoder_set_reset", "m3tsz_encoder_set_append", "m3tsz_encoder_set_stream",
     "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex", "m3tsz_encoder_set_write",
     "m3tsz_aggregate_tiles_transform", "m3tsz_aggregate_tiles_types", "m3tsz_aggregate_tiles_annotated",
-    "m3tsz_aggregate_tiles_blocks", "m3tsz_aggregate_tiles_rollup",
+    "m3tsz_aggregate_tiles_blocks", "m3tsz_aggregate_tiles_rollup", "m3tsz_aggregate_tiles_rollup_annotated",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -294,6 +294,8 @@ def lib():
     L.m3tsz_aggregate_tiles_rollup.argtypes = [vp, po, vp, u64, vp, vp, u64, vp, u64, i64, i64, u32, i32, i32,
                                                pi32, u32, vp, vp, u64, u64, pi32, u32, pi32, u32, i32, vp, vp,
                                                i32, u32, vp, u64, vp, vp, vp, vp, vp, vp, vp]
+    L.m3tsz_aggregate_tiles_rollup_annotated.restype = C.c_int
+    L.m3tsz_aggregate_tiles_rollup_annotated.argtypes = L.m3tsz_aggregate_tiles_rollup.argtypes
     _lib = L
     return L
 

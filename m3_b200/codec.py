@@ -468,13 +468,17 @@ class BatchCodec:
                                rollup_types, metric_type=capi.METRIC_GAUGE, pre_transforms=(), post_transforms=(),
                                discard_nan=True, src_state: Optional[torch.Tensor] = None,
                                group_state: Optional[torch.Tensor] = None, lengths=None,
-                               blocks: Optional[torch.Tensor] = None, capacity=None, out_unit=capi.UNIT_S, align=64):
+                               blocks: Optional[torch.Tensor] = None, capacity=None, out_unit=capi.UNIT_S, align=64,
+                               annotations=False):
         """Tile aggregation through a rollup (m3tsz_aggregate_tiles_rollup): every source series is an element of
         (metric_type, src_type) whose window values run through pre_transforms and are forwarded; group g is the
         sources members[group_off[g] .. group_off[g + 1]) (int64 [G + 1] and int32 [n] device tensors), whose
         forwarded values are folded in that order into one element per group with rollup_types (strictly ascending,
         1..8) and post_transforms.  src_state (transform_state(S)) and group_state (element_state(G)) carry the
         chains from call to call.  offsets / lengths / blocks address the sources as in aggregate_tiles_types.
+        annotations=True (m3tsz_aggregate_tiles_rollup_annotated): each group window also carries the last non-empty
+        annotation, in listed order, of the members that forwarded a value to it, and its rows write it; the default
+        capacity then adds, per rollup type, the source bytes of every listed member.
         Returns (PackedResult with [k, G] views, n_tiles int32 [k, G], source statuses int32 [S])."""
         n_seg = offsets.numel() - 1 if lengths is None else lengths.numel()
         S = n_seg if blocks is None else blocks.numel() - 1
@@ -487,7 +491,20 @@ class BatchCodec:
         k = len(types)
         if capacity is None:
             rows = 2 * n_windows if capi.TRANSFORM_RESET in post else n_windows
-            capacity = max(1, k * G * self.encode_bound(rows))
+            capacity = k * G * self.encode_bound(rows)
+            if annotations and members.numel():  # a group row's annotations are copies of different ones of its members'
+                seg = (offsets[1:] - offsets[:-1]) if lengths is None else lengths
+                if blocks is None:
+                    src_len = seg
+                else:
+                    cs = torch.cat([torch.zeros(1, dtype=torch.int64, device=seg.device), torch.cumsum(seg, 0)])
+                    b = blocks.clamp(0, n_seg)
+                    src_len = (cs[b[1:]] - cs[b[:-1]]).clamp(min=0)
+                m = members.long()
+                ok = (m >= 0) & (m < S)
+                member_bytes = int(src_len[m.clamp(0, max(0, S - 1))][ok].clamp(min=0).sum().item()) if S else 0
+                capacity += k * (member_bytes + 16 * G)
+            capacity = max(1, capacity)
         out, n_tiles = self._tile_outputs(k * G, capacity)
         src_status = torch.empty(max(1, S), dtype=torch.int32, device=dev)
         assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
@@ -497,14 +514,15 @@ class BatchCodec:
         _check_records(src_state, S, capi.TRANSFORM_STATE_BYTES)
         _check_records(group_state, G, capi.ELEMENT_STATE_BYTES)
         i32s = lambda xs: (C.c_int32 * max(1, len(xs)))(*xs)
-        rc = capi.lib().m3tsz_aggregate_tiles_rollup(
+        fn = "m3tsz_aggregate_tiles_rollup_annotated" if annotations else "m3tsz_aggregate_tiles_rollup"
+        rc = getattr(capi.lib(), fn)(
             self.ctx.handle, C.byref(self.opts), _ptr(streams), streams.numel(), _ptr(offsets), _ptr(lengths),
             n_seg, _ptr(blocks), S, int(start_ns), int(step_ns), int(n_windows), int(metric_type), int(src_type),
             i32s(pre), len(pre), _ptr(group_off), _ptr(members), members.numel(), G, i32s(types), k, i32s(post),
             len(post), 1 if discard_nan else 0, _ptr(src_state), _ptr(group_state), int(out_unit), int(align),
             _ptr(out.packed), out.packed.numel(), _ptr(out.offsets), _ptr(out.out_len), _ptr(out.status),
             _ptr(n_tiles), _ptr(out.total), _ptr(src_status), _cuda_stream_ptr(dev))
-        self.ctx.check(rc, "m3tsz_aggregate_tiles_rollup")
+        self.ctx.check(rc, fn)
         out, n_tiles = self._types_views(out, n_tiles, k, G)
         return out, n_tiles, src_status[:S]
 

@@ -769,35 +769,41 @@ static void tile_inputs(EncodeParams &p, bool counter, const TileWindows &w) {
   p.tile_sum_sq = w.sq;  // (NULL unless SumSq / Stdev / Counter)
 }
 
+// The room a row's slot adds for its annotations with xf.annotated: `launch` writes the bound (launch_max_stream_len
+// or launch_group_max_stream_len) into a zeroed device word, which is read back.
+extern "C++" {
+template <typename Launch>
+static int annotation_room(m3tsz_ctx *ctx, cudaStream_t st, const Launch &launch, uint64_t &room) {
+  void *d_mx = nullptr;
+  int rc;
+  if ((rc = ensure(ctx, kSlotSrcMaxLen, 8, &d_mx))) return rc;
+  CK(cudaMemsetAsync(d_mx, 0, 8, st));
+  CK(launch((unsigned long long *)d_mx));
+  ctx->launches++;
+  CK(cudaMemcpyAsync(&room, d_mx, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return M3TSZ_OK;
+}
+}
+
 // Step 2 of every tile call: the element xf over the windows w of n_src sources, re-encoded straight into the packed
 // outputs (the encoder's input stage skips empty windows, stamps the window end and takes Gauge.ValueOf(type)), then
 // the status pass: a failed source's error goes to all its rows.  With xf.annotated the rows copy annotations of the
-// source streams d_streams / d_offsets / d_lengths.
+// streams d_streams, and every slot adds ann_room bytes for them (annotation_room).  The references w.ann hold the
+// payload's bit offset in its stream, whose byte offset is d_offsets[source], or, with xf.block_off or a NULL
+// d_offsets, in the whole batch.
 static int tiles_encode(m3tsz_ctx *ctx, const m3tsz_options *opts, const TileWindows &w, uint64_t n_src,
                         int64_t start_ns, int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t out_unit,
-                        const TileTransforms &xf, const uint8_t *d_streams, uint64_t streams_bytes,
-                        const uint64_t *d_offsets, const uint64_t *d_lengths, const TileOutputs &out,
-                        cudaStream_t st) {
+                        const TileTransforms &xf, const uint8_t *d_streams, const uint64_t *d_offsets,
+                        uint64_t ann_room, const TileOutputs &out, cudaStream_t st) {
   CK(cudaMemsetAsync(out.total_bytes, 0, sizeof(uint64_t), st));
   const uint64_t n_rows = (uint64_t)xf.n_types * n_src;
   if (n_rows == 0) return M3TSZ_OK;  // (a rollup without groups)
   int rc;
   // (a Reset op writes up to two datapoints per window)
   uint64_t slot_bytes = m3tsz_encode_bound(xf.reset ? 2ull * n_windows : (uint64_t)n_windows);
-  if (xf.annotated) {
-    // a row's annotations are copies of different annotations of its source stream: the slots also take the longest
-    // source stream of the call (over source blocks: the largest sum of a series' block lengths)
-    void *d_mx = nullptr;
-    if ((rc = ensure(ctx, kSlotSrcMaxLen, 8, &d_mx))) return rc;
-    CK(cudaMemsetAsync(d_mx, 0, 8, st));
-    CK(launch_max_stream_len(d_offsets, d_lengths, xf.block_off, n_src, xf.n_segments, streams_bytes,
-                             (unsigned long long *)d_mx, st));
-    ctx->launches++;
-    uint64_t mx = 0;
-    CK(cudaMemcpyAsync(&mx, d_mx, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    slot_bytes = (slot_bytes + mx + 15) & ~15ull;
-  }
+  // a row's annotations are copies of different annotations of its source streams
+  if (xf.annotated) slot_bytes = (slot_bytes + ann_room + 15) & ~15ull;
   EncodeParams p;
   memset(&p, 0, sizeof(p));
   if ((rc = packed_params(ctx, n_rows, slot_bytes, out.align, out.packed, out.capacity, out.offsets,
@@ -829,10 +835,10 @@ static int tiles_encode(m3tsz_ctx *ctx, const m3tsz_options *opts, const TileWin
   if (xf.multi) {
     p.in_mode = 5;
     if (xf.annotated) {
-      p.in_mode = xf.block_off ? 7 : 6;  // (7: the references hold the payload's bit offset in the whole batch)
+      p.tile_src_off = xf.block_off ? nullptr : d_offsets;
+      p.in_mode = p.tile_src_off ? 6 : 7;  // (7: the references hold the payload's bit offset in the whole batch)
       p.tile_ann = (const uint64_t *)w.ann;
       p.tile_src_streams = d_streams;
-      if (!xf.block_off) p.tile_src_off = d_offsets;
     }
     p.xf_elem = xf.elem_state;
     p.xf_elem_out = (m3tsz_element_state *)d_rec;
@@ -874,8 +880,15 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   if ((rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                          n_windows, metric_type == M3TSZ_METRIC_COUNTER, xf, st, win)))
     return rc;
+  // the longest source stream of the call (over source blocks: the largest sum of a series' block lengths)
+  uint64_t room = 0;
+  if (xf.annotated && (rc = annotation_room(ctx, st, [&](unsigned long long *mx) {
+        return launch_max_stream_len(d_offsets, d_lengths, xf.block_off, n_series, xf.n_segments, streams_bytes, mx,
+                                     st);
+      }, room)))
+    return rc;
   return tiles_encode(ctx, opts, win, n_series, start_ns, step_ns, n_windows, metric_type, out_unit, xf, d_streams,
-                      streams_bytes, d_offsets, d_lengths, out, st);
+                      d_offsets, room, out, st);
 }
 
 // aggregation.Type.IsValidForGauge / IsValidForCounter, src/metrics/aggregation/type.go:178-196
@@ -1040,27 +1053,25 @@ int m3tsz_aggregate_tiles_blocks(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
 
 // Tile aggregation through a rollup (DESIGN.md §4.8): the fused decode of the sources under src_type, the forward
 // stage (each source's pre_ops chain), the fold into the groups' windows, then the multi-type element stage over
-// n_rollup_types * n_groups rows, its status pass, and the source records.
-int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
-                                 uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
-                                 uint64_t n_segments, const uint64_t *d_block_off, uint64_t n_series, int64_t start_ns,
-                                 int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t src_type,
-                                 const int32_t *pre_ops, uint32_t n_pre_ops, const uint64_t *d_group_off,
-                                 const uint32_t *d_members, uint64_t n_members, uint64_t n_groups,
-                                 const int32_t *rollup_types, uint32_t n_rollup_types, const int32_t *post_ops,
-                                 uint32_t n_post_ops, int32_t discard_nan, m3tsz_transform_state *d_src_state,
-                                 m3tsz_element_state *d_group_state, int32_t out_unit, uint32_t align,
-                                 uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
-                                 uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
-                                 int32_t *d_src_status, void *stream) {
+// n_rollup_types * n_groups rows, its status pass, and the source records.  annotated: the annotated decode, forward
+// and fold variants carry each group window's annotation to its rows.
+static int aggregate_tiles_rollup_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                       uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                       uint64_t n_segments, const uint64_t *d_block_off, uint64_t n_series,
+                                       int64_t start_ns, int64_t step_ns, uint32_t n_windows, int32_t metric_type,
+                                       int32_t src_type, const int32_t *pre_ops, uint32_t n_pre_ops,
+                                       const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                       uint64_t n_groups, const int32_t *rollup_types, uint32_t n_rollup_types,
+                                       const int32_t *post_ops, uint32_t n_post_ops, int32_t discard_nan,
+                                       m3tsz_transform_state *d_src_state, m3tsz_element_state *d_group_state,
+                                       int32_t out_unit, const TileOutputs &out, int32_t *d_src_status, bool annotated,
+                                       void *stream) {
   TileTransforms pre, post;  // the sources' element and the groups'
-  if (!ctx || !valid_opts(opts) || !d_total_bytes || !valid_tile_pair(metric_type, src_type) ||
-      (!d_block_off && n_segments != n_series) || (n_groups && (!d_group_off || !d_status)) ||
+  if (!ctx || !valid_opts(opts) || !out.total_bytes || !valid_tile_pair(metric_type, src_type) ||
+      (!d_block_off && n_segments != n_series) || (n_groups && (!d_group_off || !out.status)) ||
       (n_members && !d_members) || !parse_transforms(pre_ops, n_pre_ops, pre) ||
       !parse_element(metric_type, rollup_types, n_rollup_types, post_ops, n_post_ops, d_group_state, post))
     return M3TSZ_ERR_INVALID_ARG;
-  const TileOutputs out{align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles,
-                        d_total_bytes};
   if (((uint64_t)n_rollup_types * n_groups != 0 && !valid_packing(out)) || !valid_windows(start_ns, step_ns, n_windows))
     return M3TSZ_ERR_INVALID_ARG;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1073,6 +1084,7 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   pre.n_types = 1;
   pre.block_off = d_block_off;
   pre.n_segments = n_segments;
+  pre.annotated = annotated;
   TileWindows win;
   if (n_series && (rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
                                      step_ns, n_windows, counter, pre, st, win)))
@@ -1101,7 +1113,15 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   fp.state_out = (m3tsz_transform_state *)d_srec;
   fp.fwd = (double *)d_fwd;
   fp.present = (uint32_t *)d_pres;
-  CK(launch_rollup_forward(fp, st));
+  void *d_apres = nullptr;
+  if (annotated) {
+    if ((rc = ensure(ctx, kSlotFwdAnnPresent, (size_t)n_series * n_words * 4, &d_apres))) return rc;
+    fp.ann = (uint64_t *)win.ann;
+    fp.src_off = d_block_off ? nullptr : d_offsets;  // (the block decode's references are batch-addressed already)
+    fp.src_status_out = (int32_t *)win.sst;
+    fp.ann_present = (uint32_t *)d_apres;
+  }
+  CK(launch_rollup_forward(fp, annotated, st));
   ctx->launches++;
   // 3. fold: the groups' window-major aggregates, in the fused decode's representation, and their statuses
   const size_t gb = (size_t)n_groups * n_windows * 8;
@@ -1114,6 +1134,7 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   if (needs_sum_sq(counter, rollup_types, n_rollup_types) && (rc = ensure(ctx, kSlotGroupSumSq, gb, &grp.sq)))
     return rc;
   if ((rc = ensure(ctx, kSlotGroupStatus, n_groups * 4, &grp.sst))) return rc;
+  if (annotated && (rc = ensure(ctx, kSlotGroupAnn, gb, &grp.ann))) return rc;
   RollupFoldParams gp;
   memset(&gp, 0, sizeof(gp));
   gp.fwd = (const double *)d_fwd;
@@ -1134,19 +1155,70 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   gp.last = (double *)grp.last;
   gp.sum_sq = grp.sq;
   gp.group_status = (int32_t *)grp.sst;
-  CK(launch_rollup_fold(gp, st));
+  gp.ann_present = (const uint32_t *)d_apres;
+  gp.ann = (const uint64_t *)win.ann;
+  gp.group_ann = (uint64_t *)grp.ann;
+  CK(launch_rollup_fold(gp, annotated, st));
   ctx->launches++;
-  // 4. the rollup element over n_rollup_types * n_groups rows, the groups as its sources
+  // 4. the rollup element over n_rollup_types * n_groups rows, the groups as its sources.  With annotations a group
+  // row copies annotations of its members' streams (batch-addressed references: IN = 7), so its slot adds the largest
+  // sum, over groups, of the members' source lengths
   post.discard = discard_nan != 0;
-  if ((rc = tiles_encode(ctx, opts, grp, n_groups, start_ns, step_ns, n_windows, metric_type, out_unit, post, nullptr,
-                         0, nullptr, nullptr, out, st)))
+  post.annotated = annotated;
+  uint64_t room = 0;
+  if (annotated && (uint64_t)n_rollup_types * n_groups != 0 &&
+      (rc = annotation_room(ctx, st, [&](unsigned long long *mx) {
+         return launch_group_max_stream_len(d_offsets, d_lengths, d_block_off, n_series, n_segments, streams_bytes,
+                                            d_group_off, d_members, n_members, n_groups, mx, st);
+       }, room)))
+    return rc;
+  if ((rc = tiles_encode(ctx, opts, grp, n_groups, start_ns, step_ns, n_windows, metric_type, out_unit, post,
+                         d_streams, nullptr, room, out, st)))
     return rc;
   // 5. the source records: a source is saved when it decoded and every group that lists it was saved
-  CK(launch_rollup_commit(d_group_off, d_members, n_members, n_groups, d_status, n_rollup_types,
+  CK(launch_rollup_commit(d_group_off, d_members, n_members, n_groups, out.status, n_rollup_types,
                           (const int32_t *)win.sst, n_series, (uint8_t *)d_mark, (const m3tsz_transform_state *)d_srec,
                           d_src_state, d_src_status, st));
   ctx->launches += 2;
   return M3TSZ_OK;
+}
+
+int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
+                                 uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
+                                 uint64_t n_segments, const uint64_t *d_block_off, uint64_t n_series, int64_t start_ns,
+                                 int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t src_type,
+                                 const int32_t *pre_ops, uint32_t n_pre_ops, const uint64_t *d_group_off,
+                                 const uint32_t *d_members, uint64_t n_members, uint64_t n_groups,
+                                 const int32_t *rollup_types, uint32_t n_rollup_types, const int32_t *post_ops,
+                                 uint32_t n_post_ops, int32_t discard_nan, m3tsz_transform_state *d_src_state,
+                                 m3tsz_element_state *d_group_state, int32_t out_unit, uint32_t align,
+                                 uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_out_offsets,
+                                 uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
+                                 int32_t *d_src_status, void *stream) {
+  return aggregate_tiles_rollup_impl(
+      ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_segments, d_block_off, n_series, start_ns, step_ns,
+      n_windows, metric_type, src_type, pre_ops, n_pre_ops, d_group_off, d_members, n_members, n_groups, rollup_types,
+      n_rollup_types, post_ops, n_post_ops, discard_nan, d_src_state, d_group_state, out_unit,
+      {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes}, d_src_status,
+      false, stream);
+}
+
+int m3tsz_aggregate_tiles_rollup_annotated(
+    m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams, uint64_t streams_bytes,
+    const uint64_t *d_offsets, const uint64_t *d_lengths, uint64_t n_segments, const uint64_t *d_block_off,
+    uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t src_type,
+    const int32_t *pre_ops, uint32_t n_pre_ops, const uint64_t *d_group_off, const uint32_t *d_members,
+    uint64_t n_members, uint64_t n_groups, const int32_t *rollup_types, uint32_t n_rollup_types,
+    const int32_t *post_ops, uint32_t n_post_ops, int32_t discard_nan, m3tsz_transform_state *d_src_state,
+    m3tsz_element_state *d_group_state, int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
+    uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
+    int32_t *d_src_status, void *stream) {
+  return aggregate_tiles_rollup_impl(
+      ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_segments, d_block_off, n_series, start_ns, step_ns,
+      n_windows, metric_type, src_type, pre_ops, n_pre_ops, d_group_off, d_members, n_members, n_groups, rollup_types,
+      n_rollup_types, post_ops, n_post_ops, discard_nan, d_src_state, d_group_state, out_unit,
+      {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes}, d_src_status,
+      true, stream);
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

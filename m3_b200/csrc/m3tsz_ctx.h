@@ -48,6 +48,8 @@ struct Scratch {
 //                 records, source marks
 //   57-63         group window sum / count / min / max / last   tiles (aggregate_tiles_rollup)
 //                 / sumSq, group statuses
+//   64, 65        forwarded-annotation words, group annotation   tiles (aggregate_tiles_rollup_annotated)
+//                 references
 enum Slot : int {
   kSlotStreams = 0,
   kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
@@ -105,7 +107,10 @@ enum Slot : int {
   kSlotGroupLast = 61,
   kSlotGroupSumSq = 62,
   kSlotGroupStatus = 63,
-  kNumSlots = 64
+  // the rollup that keeps annotations
+  kSlotFwdAnnPresent = 64,
+  kSlotGroupAnn = 65,
+  kNumSlots = 66
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

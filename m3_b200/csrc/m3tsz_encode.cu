@@ -2311,10 +2311,31 @@ __device__ __forceinline__ void rollup_counter_add(RollupCounterAcc &a, double x
   a.sq = (int64_t)((uint64_t)a.sq + (uint64_t)v * (uint64_t)v);
 }
 
+// The annotated forward stage's step for a window of source s with datapoints: the fused decode's reference `ref`
+// (0: none) in the batch-addressed form the multi-type stage's IN = 7 reads, (bit offset from the batch's first bit)
+// << kBlockAnnLenBits | length.  src_off NULL: the decode over source blocks already wrote it so.  false: a payload
+// of 2^27 bytes or more, which rejects the source (the limit of that form, as over source blocks)
+__device__ __forceinline__ bool rollup_ann_ref(uint64_t &ref, const uint64_t *src_off, uint64_t s) {
+  if (!ref || !src_off) return true;
+  const uint64_t len = ref & 0xffffffffull;
+  if (len >> kBlockAnnLenBits) return false;
+  ref = ((src_off[s] * 8ull + (ref >> 32)) << kBlockAnnLenBits) | len;
+  return true;
+}
+// The annotated fold's step for one member (MaybeReplaceAnnotation in Gauge / Counter Update, reached through
+// AddUnique): a window the member forwarded with a non-empty annotation (its ann_present bit) replaces the group's
+// reference, and any other keeps it
+__device__ __forceinline__ void rollup_ann_add(uint64_t &g, uint32_t ann_bits, uint32_t lane, const uint64_t *ref) {
+  if ((ann_bits >> lane) & 1u) g = *ref;
+}
+
 // Forward stage: one lane per source series, windows in order (the chain is a recurrence over them), 32 windows at a
 // time staged in shared memory so that the series-major rows are written as whole 256-byte runs; the presence words
-// of those 32 windows are one word-major row, written by the warp as 128-byte runs.
+// of those 32 windows are one word-major row, written by the warp as 128-byte runs.  ANN: also the ann_present row
+// the same way; the references stay window-major where the decode wrote them (a lane's read of window w is one
+// 256-byte run per warp), rewritten in place only where a forwarded window has one.
 constexpr int ROLLUP_FWD_WARPS = 4;
+template <bool ANN>
 __global__ void __launch_bounds__(ROLLUP_FWD_WARPS * 32) rollup_forward_kernel(const RollupForwardParams p) {
   __shared__ double tile[ROLLUP_FWD_WARPS][32][33];
   const uint32_t lane = threadIdx.x & 31u, wi = threadIdx.x >> 5;
@@ -2328,8 +2349,9 @@ __global__ void __launch_bounds__(ROLLUP_FWD_WARPS * 32) rollup_forward_kernel(c
   else
     memset(&st, 0, sizeof(st));
   double(*const tl)[33] = tile[wi];
+  bool too_large = false;  // (ANN)
   for (uint32_t w0 = 0; w0 < p.n_windows; w0 += 32) {
-    uint32_t bits = 0;
+    uint32_t bits = 0, abits = 0;
 #pragma unroll 1
     for (uint32_t i = 0; i < 32; i++) {
       const uint32_t w = w0 + i;
@@ -2343,6 +2365,15 @@ __global__ void __launch_bounds__(ROLLUP_FWD_WARPS * 32) rollup_forward_kernel(c
           xf_window(p.ops, p.tiles.tile_step, st, p.tiles.tile_start + (int64_t)(w + 1) * p.tiles.tile_step, v,
                     extra_t);
           if (!(p.discard_nan && xf_isnan(v))) bits |= 1u << i;
+          if constexpr (ANN) {
+            uint64_t ref = p.ann[o];
+            if (!rollup_ann_ref(ref, p.src_off, s)) {
+              too_large = true;
+            } else if (ref && ((bits >> i) & 1u)) {
+              abits |= 1u << i;
+              if (p.src_off) p.ann[o] = ref;
+            }
+          }
         }
       }
       tl[lane][i] = v;
@@ -2352,17 +2383,25 @@ __global__ void __launch_bounds__(ROLLUP_FWD_WARPS * 32) rollup_forward_kernel(c
     for (uint32_t j = 0; j < 32; j++)
       if (s0 + j < p.n_src && w < p.n_windows) p.fwd[(s0 + j) * p.n_windows + w] = tl[j][lane];
     if (valid) p.present[(uint64_t)(w0 >> 5) * p.n_src + s] = bits;
+    if constexpr (ANN)
+      if (valid) p.ann_present[(uint64_t)(w0 >> 5) * p.n_src + s] = abits;
     __syncwarp();
   }
   if (valid) p.state_out[s] = st;
+  if constexpr (ANN)
+    if (too_large) p.src_status_out[s] = M3TSZ_ERR_STREAM_TOO_LARGE;  // (the fold then fails every group listing s)
 }
 
 // Fold: one warp per group, lane l over windows w0 + l; members in listed order (each lane folds its own window, so
 // the order is the same in every window), their present words read once per 32 windows, their values as 256-byte
 // runs.  A block's groups write their window rows through shared memory, ROLLUP_FOLD_WARPS adjacent slots at a time.
+// ANN: also each group window's annotation reference, a seventh row; a member's ann_present word is read with its
+// present word, and its window-major reference only where that bit is set.
 constexpr int ROLLUP_FOLD_WARPS = 8;
+template <bool ANN>
 __global__ void __launch_bounds__(ROLLUP_FOLD_WARPS * 32) rollup_fold_kernel(const RollupFoldParams p) {
-  __shared__ uint64_t out[6][32][ROLLUP_FOLD_WARPS];
+  constexpr int NR = ANN ? 7 : 6;
+  __shared__ uint64_t out[NR][32][ROLLUP_FOLD_WARPS];
   const uint32_t lane = threadIdx.x & 31u, wi = threadIdx.x >> 5;
   const uint64_t g0 = (uint64_t)blockIdx.x * ROLLUP_FOLD_WARPS, g = g0 + wi;
   const bool valid = g < p.n_groups;
@@ -2390,7 +2429,8 @@ __global__ void __launch_bounds__(ROLLUP_FOLD_WARPS * 32) rollup_fold_kernel(con
   const bool fold = valid && gst == M3TSZ_OK;
   for (uint32_t w0 = 0; w0 < p.n_windows; w0 += 32) {
     const uint32_t w = w0 + lane, word = w0 >> 5;  // (a window past the range has no present bit)
-    uint64_t r[6];
+    uint64_t r[NR];
+    uint64_t gann = 0;  // (ANN)
     if (p.counter) {
       RollupCounterAcc a;
       rollup_counter_init(a);
@@ -2399,6 +2439,9 @@ __global__ void __launch_bounds__(ROLLUP_FOLD_WARPS * 32) rollup_fold_kernel(con
           const uint64_t m = __ldg(p.members + i);
           const uint32_t bits = __ldg(p.present + (uint64_t)word * p.n_src + m);
           if ((bits >> lane) & 1u) rollup_counter_add(a, __ldg(p.fwd + m * p.n_windows + w));
+          if constexpr (ANN)
+            rollup_ann_add(gann, __ldg(p.ann_present + (uint64_t)word * p.n_src + m), lane,
+                           p.ann + (uint64_t)w * p.n_src + m);
         }
       }
       r[0] = (uint64_t)a.sum;
@@ -2415,6 +2458,9 @@ __global__ void __launch_bounds__(ROLLUP_FOLD_WARPS * 32) rollup_fold_kernel(con
           const uint64_t m = __ldg(p.members + i);
           const uint32_t bits = __ldg(p.present + (uint64_t)word * p.n_src + m);
           if ((bits >> lane) & 1u) rollup_gauge_add(a, __ldg(p.fwd + m * p.n_windows + w));
+          if constexpr (ANN)
+            rollup_ann_add(gann, __ldg(p.ann_present + (uint64_t)word * p.n_src + m), lane,
+                           p.ann + (uint64_t)w * p.n_src + m);
         }
       }
       r[0] = (uint64_t)__double_as_longlong(a.sum);
@@ -2424,8 +2470,9 @@ __global__ void __launch_bounds__(ROLLUP_FOLD_WARPS * 32) rollup_fold_kernel(con
       r[4] = (uint64_t)__double_as_longlong(a.last);
       r[5] = (uint64_t)__double_as_longlong(a.sq);
     }
+    if constexpr (ANN) r[6] = gann;
 #pragma unroll
-    for (int k = 0; k < 6; k++) out[k][lane][wi] = r[k];
+    for (int k = 0; k < NR; k++) out[k][lane][wi] = r[k];
     __syncthreads();
     // row rr of this window block, group column c: ROLLUP_FOLD_WARPS adjacent 8-byte slots of one window row
     for (uint32_t t = threadIdx.x; t < 32u * ROLLUP_FOLD_WARPS; t += blockDim.x) {
@@ -2438,24 +2485,35 @@ __global__ void __launch_bounds__(ROLLUP_FOLD_WARPS * 32) rollup_fold_kernel(con
       reinterpret_cast<uint64_t *>(p.max)[o] = out[3][rr][c];
       if (!p.counter) reinterpret_cast<uint64_t *>(p.last)[o] = out[4][rr][c];
       if (p.sum_sq) reinterpret_cast<uint64_t *>(p.sum_sq)[o] = out[5][rr][c];
+      if constexpr (ANN) p.group_ann[o] = out[6][rr][c];
     }
     __syncthreads();
   }
 }
 
-cudaError_t launch_rollup_forward(const RollupForwardParams &p, cudaStream_t stream) {
+cudaError_t launch_rollup_forward(const RollupForwardParams &p, bool annotated, cudaStream_t stream) {
   if (p.n_src == 0 || p.n_windows == 0) return cudaSuccess;
   const uint64_t per_block = 32ull * ROLLUP_FWD_WARPS, blocks = (p.n_src + per_block - 1) / per_block;
   if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
-  rollup_forward_kernel<<<(unsigned)blocks, ROLLUP_FWD_WARPS * 32, 0, stream>>>(p);
+  if (annotated) {
+    if (!p.ann || !p.ann_present || !p.src_status_out) return cudaErrorInvalidValue;
+    rollup_forward_kernel<true><<<(unsigned)blocks, ROLLUP_FWD_WARPS * 32, 0, stream>>>(p);
+  } else {
+    rollup_forward_kernel<false><<<(unsigned)blocks, ROLLUP_FWD_WARPS * 32, 0, stream>>>(p);
+  }
   return cudaGetLastError();
 }
 
-cudaError_t launch_rollup_fold(const RollupFoldParams &p, cudaStream_t stream) {
+cudaError_t launch_rollup_fold(const RollupFoldParams &p, bool annotated, cudaStream_t stream) {
   if (p.n_groups == 0) return cudaSuccess;
   const uint64_t blocks = (p.n_groups + ROLLUP_FOLD_WARPS - 1) / ROLLUP_FOLD_WARPS;
   if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
-  rollup_fold_kernel<<<(unsigned)blocks, ROLLUP_FOLD_WARPS * 32, 0, stream>>>(p);
+  if (annotated) {
+    if (!p.group_ann) return cudaErrorInvalidValue;  // (ann / ann_present: read only where a bit is set)
+    rollup_fold_kernel<true><<<(unsigned)blocks, ROLLUP_FOLD_WARPS * 32, 0, stream>>>(p);
+  } else {
+    rollup_fold_kernel<false><<<(unsigned)blocks, ROLLUP_FOLD_WARPS * 32, 0, stream>>>(p);
+  }
   return cudaGetLastError();
 }
 

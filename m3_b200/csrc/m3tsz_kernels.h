@@ -265,6 +265,12 @@ cudaError_t launch_fill_i64(int64_t *dst, int64_t v, uint64_t n, cudaStream_t st
 cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
                                   uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
                                   unsigned long long *out, cudaStream_t stream);
+// The same room for the rollup's group rows: the largest sum, over groups g, of the segment lengths above of each
+// member m < n_series listed in members[group_off[g] .. group_off[g + 1]) (a group with an invalid range counts 0)
+cudaError_t launch_group_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
+                                        uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
+                                        const uint64_t *group_off, const uint32_t *members, uint64_t n_members,
+                                        uint64_t n_groups, unsigned long long *out, cudaStream_t stream);
 // a failed source's error goes to all n_types rows of its series; with `state`, a series whose source and rows are
 // all OK takes its new record from `scratch`
 cudaError_t launch_tiles_types_status(const int32_t *src_status, int32_t *status, uint64_t n, uint32_t n_types,
@@ -289,6 +295,16 @@ struct RollupForwardParams {
   m3tsz_transform_state *state_out;    // [n_src]: each source's new record (committed by launch_rollup_commit)
   double *fwd;
   uint32_t *present;
+  // the annotated variant (after every older field, which keep their offsets): `ann` is the fused decode's window-major
+  // [n_windows][n_src] references.  Without a block table (src_off = the sources' byte offsets) a reference holds
+  // (bit offset from the stream's first bit) << 32 | length, and the stage rewrites a forwarded window's in place as
+  // (bit offset from the batch's first bit) << kBlockAnnLenBits | length; with one it already has that form.  A
+  // source with a window annotation of 2^27 bytes or more gets src_status_out[s] = M3TSZ_ERR_STREAM_TOO_LARGE.
+  // ann_present[w / 32][s] bit w % 32: window w was forwarded and carries an annotation.
+  uint64_t *ann;
+  const uint64_t *src_off;
+  int32_t *src_status_out;
+  uint32_t *ann_present;
 };
 // The fold: window w of group g takes the forwarded values of its members, in listed order, and writes the aggregate
 // slots of the fused decode over n_groups "series" (window-major [n_windows][n_groups], the same representation)
@@ -308,9 +324,16 @@ struct RollupFoldParams {
   int64_t *count;
   double *last;           // Gauge only
   int32_t *group_status;  // [n_groups]: INVALID_ARG for a bad range or index, else the first failing member's error
+  // the annotated variant (after every older field): the forward stage's ann_present words and batch-addressed
+  // references, and each group window's reference, window-major [n_windows][n_groups]: the last non-zero one of the
+  // members, in listed order, whose window was forwarded (0: none, or the group failed)
+  const uint32_t *ann_present;
+  const uint64_t *ann;
+  uint64_t *group_ann;
 };
-cudaError_t launch_rollup_forward(const RollupForwardParams &p, cudaStream_t stream);
-cudaError_t launch_rollup_fold(const RollupFoldParams &p, cudaStream_t stream);
+// annotated: the variants that carry the annotation references (p.ann / ann_present / group_ann)
+cudaError_t launch_rollup_forward(const RollupForwardParams &p, bool annotated, cudaStream_t stream);
+cudaError_t launch_rollup_fold(const RollupFoldParams &p, bool annotated, cudaStream_t stream);
 // The source records (m3tsz_query.cu): a source takes its new record from `scratch` when it decoded and every group
 // that lists it has all n_types rows OK; src_status_out (optional) takes each source's decode status.  `mark` is
 // [n_src] bytes of scratch.

@@ -220,23 +220,28 @@ cudaError_t launch_rollup_commit(const uint64_t *group_off, const uint32_t *memb
 // The room of a tile call with annotations: a row's annotations are copies of different annotations of its source
 // stream, or of any of its series' source blocks, so its bound adds the largest sum of a series' segment lengths (one
 // warp-wide max and one atomic per warp)
+__device__ __forceinline__ unsigned long long series_stream_len(const uint64_t *offsets, const uint64_t *lengths,
+                                                                const uint64_t *block_off, uint64_t s,
+                                                                uint64_t n_segments, uint64_t streams_bytes) {
+  unsigned long long len = 0;
+  uint64_t q0 = s, q1 = s + 1;
+  if (block_off) {
+    q0 = block_off[s];
+    q1 = block_off[s + 1];
+    if (q0 > q1 || q1 > n_segments) q1 = q0;
+  }
+  for (uint64_t q = q0; q < q1; q++) {
+    const uint64_t o0 = offsets[q], o1 = lengths ? o0 + lengths[q] : offsets[q + 1];
+    if (o1 >= o0 && o1 <= streams_bytes && o1 - o0 < (1ull << 28)) len += o1 - o0;
+  }
+  return len;
+}
 __global__ void max_stream_len_kernel(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
                                       uint64_t n, uint64_t n_segments, uint64_t streams_bytes,
                                       unsigned long long *out) {
   const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   unsigned long long len = 0;
-  if (s < n) {
-    uint64_t q0 = s, q1 = s + 1;
-    if (block_off) {
-      q0 = block_off[s];
-      q1 = block_off[s + 1];
-      if (q0 > q1 || q1 > n_segments) q1 = q0;
-    }
-    for (uint64_t q = q0; q < q1; q++) {
-      const uint64_t o0 = offsets[q], o1 = lengths ? o0 + lengths[q] : offsets[q + 1];
-      if (o1 >= o0 && o1 <= streams_bytes && o1 - o0 < (1ull << 28)) len += o1 - o0;
-    }
-  }
+  if (s < n) len = series_stream_len(offsets, lengths, block_off, s, n_segments, streams_bytes);
   for (int d = 16; d > 0; d >>= 1) {
     const unsigned long long o = __shfl_xor_sync(0xffffffffu, len, d);
     len = o > len ? o : len;
@@ -250,6 +255,37 @@ cudaError_t launch_max_stream_len(const uint64_t *offsets, const uint64_t *lengt
   const unsigned tb = 256;
   max_stream_len_kernel<<<(unsigned)((n_series + tb - 1) / tb), tb, 0, stream>>>(
       offsets, lengths, block_off, n_series, n_segments, streams_bytes, out);
+  return cudaGetLastError();
+}
+
+// The same for the rollup's group rows, whose annotations are copies of annotations of any member's stream: one warp
+// per group, its lanes over the members, then a warp-wide sum and one atomic per group
+__global__ void group_max_stream_len_kernel(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
+                                            uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
+                                            const uint64_t *group_off, const uint32_t *members, uint64_t n_members,
+                                            uint64_t n_groups, unsigned long long *out) {
+  const uint64_t g = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t lane = threadIdx.x & 31u;
+  if (g >= n_groups) return;
+  const uint64_t lo = group_off[g], hi = group_off[g + 1];
+  if (lo > hi || hi > n_members) return;
+  unsigned long long len = 0;
+  for (uint64_t i = lo + lane; i < hi; i += 32) {
+    const uint32_t m = members[i];
+    if (m < n_series) len += series_stream_len(offsets, lengths, block_off, m, n_segments, streams_bytes);
+  }
+  for (int d = 16; d > 0; d >>= 1) len += __shfl_xor_sync(0xffffffffu, len, d);
+  if (lane == 0 && len) atomicMax(out, len);
+}
+cudaError_t launch_group_max_stream_len(const uint64_t *offsets, const uint64_t *lengths, const uint64_t *block_off,
+                                        uint64_t n_series, uint64_t n_segments, uint64_t streams_bytes,
+                                        const uint64_t *group_off, const uint32_t *members, uint64_t n_members,
+                                        uint64_t n_groups, unsigned long long *out, cudaStream_t stream) {
+  if (n_groups == 0 || n_series == 0) return cudaSuccess;
+  const unsigned tb = 256;
+  if ((n_groups * 32 + tb - 1) / tb > 0x7fffffffull) return cudaErrorInvalidValue;
+  group_max_stream_len_kernel<<<(unsigned)((n_groups * 32 + tb - 1) / tb), tb, 0, stream>>>(
+      offsets, lengths, block_off, n_series, n_segments, streams_bytes, group_off, members, n_members, n_groups, out);
   return cudaGetLastError();
 }
 

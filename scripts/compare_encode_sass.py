@@ -3,7 +3,9 @@
 instruction for instruction (cuobjdump -sass; addresses and encodings dropped).  The encoder sets added a fourth
 template argument, APPEND, to encode_kernel: an old build's <INT_OPT, PACKED, IN> is compared with a new build's
 <INT_OPT, PACKED, IN, false>.  decode_kernel<INT_OPT, MODE> is compared by name; the source-block loop added a third
-argument, BLK, so an old build's <INT_OPT, MODE> is compared with a new build's <INT_OPT, MODE, false>.  Instantiations only one build has
+argument, BLK, so an old build's <INT_OPT, MODE> is compared with a new build's <INT_OPT, MODE, false>.  The rollup's
+rollup_forward_kernel and rollup_fold_kernel are compared too; the annotated rollup made them templates over ANN, so an
+old build's untemplated kernel is compared with a new build's <false>.  Instantiations only one build has
 (the append mode, new decode modes) are listed, not compared.
 
     python scripts/compare_encode_sass.py OLD.(o|so) NEW.(o|so)     # exit code 1 on any difference
@@ -30,6 +32,9 @@ def kernels(path):
                 out[cur] = []
             elif "decode_kernel" in name:
                 cur = re.sub(r"(decode_kernelILb[01]ELi[0-9]+E)Lb0E", r"\1", name)
+                out[cur] = []
+            elif "rollup_forward_kernel" in name or "rollup_fold_kernel" in name:
+                cur = re.sub(r"(rollup_(?:forward|fold)_kernel)ILb0EEEvNS_", r"\1ENS_", name)
                 out[cur] = []
             continue
         m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;", line)

@@ -5,7 +5,8 @@ tests/golden/m3tsz_agg_goldens.json, the buffer bucket's write tables into
 tests/golden/m3tsz_buffer_goldens.json, the aggregator's transformations of a flushed window into
 tests/golden/m3tsz_transform_goldens.json, and the flushes of an element with several aggregation types into
 tests/golden/m3tsz_element_types_goldens.json, and the steps of a rollup (the values a source element forwards, what
-the rollup element folds, when the forwarded list flushes) into tests/golden/m3tsz_rollup_goldens.json.
+the rollup element folds, when the forwarded list flushes) into tests/golden/m3tsz_rollup_goldens.json, and the
+annotations a rollup element keeps from what it is forwarded into tests/golden/m3tsz_rollup_annotation_goldens.json.
 
 Run in the build container only (it reads /root/reference, which does not exist
 on the GPU box):   python scripts/make_goldens.py
@@ -33,6 +34,8 @@ OUT_ELEM = os.path.join(os.path.dirname(OUT), "m3tsz_element_types_goldens.json"
 OUT_ANN = os.path.join(os.path.dirname(OUT), "m3tsz_tile_annotation_goldens.json")
 # a rollup: the source element's forwarded values, the rollup element's folds and the forwarded list's flush times
 OUT_ROLLUP = os.path.join(os.path.dirname(OUT), "m3tsz_rollup_goldens.json")
+# the annotation a rollup element keeps: AddUnique passes metric.Annotation to Gauge / Counter Update
+OUT_ROLLUP_ANN = os.path.join(os.path.dirname(OUT), "m3tsz_rollup_annotation_goldens.json")
 
 SEC = 1_000_000_000
 MS = 1_000_000
@@ -672,6 +675,46 @@ def main():
                   "added_at_ns": [210 * SEC, 220 * SEC], "want_flush_ns": [210 * SEC, 220 * SEC]},
     }
 
+    # ---- annotations through a rollup.  The rollup element's AddUnique (generic_elem.go:246-281) passes
+    # metric.Annotation to Add, and Gauge / Counter Update keep the last non-empty one (MaybeReplaceAnnotation,
+    # aggregation/common.go:49-61).  Each step is one AddUnique: the forwarding source, the time it is added at,
+    # the forwarded values, their annotation (hex, null for none), and what the test asserts after it about the
+    # windows (index into window_starts_ns; "annotation" null is the test's require.Nil).  testAnnot is
+    # []byte("testAnnotation") (elem_test.go:55), testTimestamps 216 / 217 / 221 s (:120-122), testAlignedStarts
+    # 210 / 220 s (:123-125), 10 s resolution.  The resend with versions (:1547-1559) is left out.
+    test_annot = hx(b"testAnnotation")
+
+    def add_unique(source, at_s, values, annotation, *want):
+        return {"source": source, "at_ns": at_s * SEC, "values": values, "annotation": annotation,
+                "want": list(want)}
+
+    rollup_ann = {
+        "description": "The annotation a rollup element keeps, transcribed from the reference's AddUnique tests "
+                       "by scripts/make_goldens.py: each step's forwarded values and annotation, and what the "
+                       "test asserts after it (sum, count, Annotation()) about each window.",
+        "cases": [
+            {"name": "TestCounterElemAddUnique", "src_line": "aggregator/aggregator/elem_test.go:312-364",
+             "metric_type": 1, "resolution_ns": 10 * SEC, "window_starts_ns": [210 * SEC, 220 * SEC],
+             "steps": [
+                 add_unique(1234, 216, [345.0], None, {"window": 0, "sum": 345, "count": 1, "annotation": None}),
+                 add_unique(5678, 217, [500.0], test_annot,
+                            {"window": 0, "sum": 845, "count": 2, "annotation": test_annot}),
+                 add_unique(1234, 221, [278.0], None, {"window": 1, "sum": 278, "count": 1},
+                            {"window": 0, "annotation": test_annot}),
+             ]},
+            {"name": "TestGaugeElemAddUnique", "src_line": "aggregator/aggregator/elem_test.go:1478-1526",
+             "metric_type": 3, "resolution_ns": 10 * SEC, "window_starts_ns": [210 * SEC, 220 * SEC],
+             "steps": [
+                 add_unique(1234, 216, [12.3, 34.5], None,
+                            {"window": 0, "sum": 46.8, "count": 2, "annotation": None}),
+                 add_unique(5678, 217, [50.0], test_annot,
+                            {"window": 0, "sum": 96.8, "count": 3, "annotation": test_annot}),
+                 add_unique(1234, 221, [27.8], None, {"window": 0, "annotation": test_annot},
+                            {"window": 1, "sum": 27.8, "count": 1}),
+             ]},
+        ],
+    }
+
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f, indent=1)
@@ -694,6 +737,9 @@ def main():
     with open(OUT_ROLLUP, "w") as f:
         json.dump(rollup, f, indent=1)
     print("wrote", OUT_ROLLUP)
+    with open(OUT_ROLLUP_ANN, "w") as f:
+        json.dump(rollup_ann, f, indent=1)
+    print("wrote", OUT_ROLLUP_ANN)
 
 
 if __name__ == "__main__":
