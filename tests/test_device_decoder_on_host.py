@@ -73,8 +73,8 @@ static inline void lz_tz(uint64_t v, int &lz, int &tz) {
 DRIVER = r"""
 template <bool INT_OPT>
 static int drive(const uint8_t *buf, uint64_t nbytes, uint64_t o0, uint64_t o1, int default_unit, int64_t *ts,
-                 uint64_t *vals, uint32_t cap, uint32_t *n_out, m3tsz_dp_event *events, uint64_t ev_cap,
-                 unsigned long long *ev_count, int *last_unit, int *first_unit) {
+                 uint64_t *vals, uint32_t *bitpos, uint32_t cap, uint32_t *n_out, m3tsz_dp_event *events,
+                 uint64_t ev_cap, unsigned long long *ev_count, int *units, uint32_t *ann) {
   DecState s;
   memset(&s, 0, sizeof(s));
   s.scheme = kSchemeNone;
@@ -83,6 +83,7 @@ static int drive(const uint8_t *buf, uint64_t nbytes, uint64_t o0, uint64_t o1, 
   s.wbase = w & ~(uint64_t)15;
   s.pos = (uint32_t)(w - s.wbase) * 32u + (uint32_t)(o0 & 3) * 8u;
   s.end = s.pos + (uint32_t)(o1 - o0) * 8u;
+  const uint32_t pos0 = s.pos;
   SlowSrc src;
   src.base = buf;
   src.nbytes = nbytes;
@@ -93,34 +94,41 @@ static int drive(const uint8_t *buf, uint64_t nbytes, uint64_t o0, uint64_t o1, 
   ev.capacity = ev_cap;
   ev.count = ev_count;
   ev.series = 0;
-  ev.pos0 = s.pos;
+  ev.pos0 = pos0;
   while (!s.done && s.err == 0 && s.n < cap) {
     int64_t t = 0;
     uint64_t v = 0;
     if (decode_dp_slow<INT_OPT>(s, src, default_unit, t, v, &ev)) {
       ts[s.n] = t;
       vals[s.n] = v;
+      bitpos[s.n] = s.pos - pos0;  // the stream bit after the datapoint
       s.n++;
     }
   }
   *n_out = s.n;
-  *last_unit = s.emit_unit;
-  *first_unit = s.first_unit;
+  units[0] = s.emit_unit;  // unit at the last datapoint produced
+  units[1] = s.first_unit;  // ... at the first
+  units[2] = s.unit;        // unit in force when the decode stopped
+  // the first annotation, as the kernel's m3tsz_annotation_ref holds it
+  ann[0] = s.ann_count ? s.ann_bit - pos0 : 0u;
+  ann[1] = s.ann_len;
+  ann[2] = s.ann_count;
   return s.err;
 }
 extern "C" int dev_decode(const uint8_t *buf, uint64_t nbytes, uint64_t o0, uint64_t o1, int int_opt, int default_unit,
-                          int64_t *ts, uint64_t *vals, uint32_t cap, uint32_t *n_out, m3tsz_dp_event *events,
-                          uint64_t ev_cap, unsigned long long *ev_count, int *last_unit, int *first_unit) {
-  return int_opt ? drive<true>(buf, nbytes, o0, o1, default_unit, ts, vals, cap, n_out, events, ev_cap, ev_count,
-                               last_unit, first_unit)
-                 : drive<false>(buf, nbytes, o0, o1, default_unit, ts, vals, cap, n_out, events, ev_cap, ev_count,
-                                last_unit, first_unit);
+                          int64_t *ts, uint64_t *vals, uint32_t *bitpos, uint32_t cap, uint32_t *n_out,
+                          m3tsz_dp_event *events, uint64_t ev_cap, unsigned long long *ev_count, int *units,
+                          uint32_t *ann) {
+  return int_opt ? drive<true>(buf, nbytes, o0, o1, default_unit, ts, vals, bitpos, cap, n_out, events, ev_cap,
+                               ev_count, units, ann)
+                 : drive<false>(buf, nbytes, o0, o1, default_unit, ts, vals, bitpos, cap, n_out, events, ev_cap,
+                                ev_count, units, ann);
 }
 """
 
 
-@pytest.fixture(scope="module")
-def dev():
+def build_dev_decoder():
+    """Compiles the decoder's complete grammar for the host (g++ only) and returns the loaded library."""
     dec = open(os.path.join(CSRC, "m3tsz_decode.cu")).read()
     com = open(os.path.join(CSRC, "m3tsz_common.cuh")).read()
     consts = "\n".join(re.findall(r"^constexpr [^\n]*\bk(?:Marker|MaxMult)[^\n]*$", com, flags=re.M))
@@ -146,24 +154,48 @@ def dev():
     return lib
 
 
+@pytest.fixture(scope="module")
+def dev():
+    return build_dev_decoder()
+
+
+class DevDecode:
+    """One stream through the complete grammar: `status`, `dps` [(ts, value bits)], `bitpos` (the stream bit after
+    each datapoint), `emit_unit` / `first_unit` / `unit` (at the last and first datapoint, and when the decode
+    stopped), `ann` (the first annotation: bit offset from the stream's first bit, length, count) and `events`
+    (uint8 [E, 32] rows of m3tsz_dp_event, series 0)."""
+
+    def __init__(self, dev, stream, int_opt, lead=0, cap=4096, default_unit=1, ev_cap=256):
+        buf = np.zeros(lead + len(stream) + 64, dtype=np.uint8)
+        buf[lead: lead + len(stream)] = np.frombuffer(stream, dtype=np.uint8)
+        ts = np.zeros(cap, dtype=np.int64)
+        vals = np.zeros(cap, dtype=np.uint64)
+        bitpos = np.zeros(cap, dtype=np.uint32)
+        n = C.c_uint32()
+        events = np.zeros((ev_cap, 32), dtype=np.uint8)
+        evc = C.c_ulonglong(0)
+        units = np.zeros(3, dtype=np.int32)
+        ann = np.zeros(3, dtype=np.uint32)
+        p = lambda a: C.c_void_p(a.ctypes.data)
+        self.status = dev.dev_decode(p(buf), C.c_uint64(lead + len(stream)), C.c_uint64(lead),
+                                     C.c_uint64(lead + len(stream)), int(int_opt), int(default_unit), p(ts), p(vals),
+                                     p(bitpos), C.c_uint32(cap), C.byref(n), p(events), C.c_uint64(ev_cap),
+                                     C.byref(evc), p(units), p(ann))
+        k = n.value
+        self.ts, self.vals, self.bitpos = ts[:k], vals[:k], bitpos[:k]
+        self.dps = list(zip(self.ts.tolist(), self.vals.tolist()))
+        self.emit_unit, self.first_unit, self.unit = (int(u) for u in units)
+        self.ann = tuple(int(a) for a in ann)
+        assert evc.value <= ev_cap
+        self.events = events[: evc.value]
+
+
 def _dev_decode(dev, stream, int_opt, lead=0, cap=4096, want_events=False):
     """the stream placed `lead` bytes into a zero-padded buffer (any byte offset, like a packed data file)"""
-    buf = np.zeros(lead + len(stream) + 64, dtype=np.uint8)
-    buf[lead: lead + len(stream)] = np.frombuffer(stream, dtype=np.uint8)
-    ts = np.zeros(cap, dtype=np.int64)
-    vals = np.zeros(cap, dtype=np.uint64)
-    n = C.c_uint32()
-    events = np.zeros((256, 32), dtype=np.uint8)
-    evc = C.c_ulonglong(0)
-    lu, fu = C.c_int(), C.c_int()
-    err = dev.dev_decode(C.c_void_p(buf.ctypes.data), C.c_uint64(lead + len(stream)), C.c_uint64(lead),
-                         C.c_uint64(lead + len(stream)), int(int_opt), 1, C.c_void_p(ts.ctypes.data),
-                         C.c_void_p(vals.ctypes.data), C.c_uint32(cap), C.byref(n), C.c_void_p(events.ctypes.data),
-                         C.c_uint64(256), C.byref(evc), C.byref(lu), C.byref(fu))
-    out = list(zip(ts[: n.value].tolist(), vals[: n.value].tolist()))
+    r = DevDecode(dev, stream, int_opt, lead=lead, cap=cap)
     if want_events:
-        return out, err, events[: min(256, evc.value)], lu.value, fu.value
-    return out, err
+        return r.dps, r.status, r.events, r.emit_unit, r.first_unit
+    return r.dps, r.status
 
 
 def _oracle(stream, int_opt):
