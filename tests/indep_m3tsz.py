@@ -66,10 +66,18 @@ def _read_varint(b):  # encoding/binary.ReadVarint over whole bytes read through
     return ~x if ux & 1 else x
 
 
-def decode(data, int_optimized, default_unit=1):
-    """-> list of (timestamp_ns, value_bits_as_uint64, unit, annotation bytes or b"")"""
+def decode(data, int_optimized, default_unit=1, trace=None):
+    """-> list of (timestamp_ns, value_bits_as_uint64, unit, annotation bytes or b"").
+
+    `trace` (a list) receives one dict per datapoint, what the stream said about it: `dod` (in the unit; None after
+    a unit change) and its `bucket` (0, 7, 9, 12, 32 or 64 value bits; "tu64" for the 64-bit nanoseconds after a
+    unit change), `unit_changed`; the value code `kind` ("full", "zero", "contained", "new" for XOR codes; int mode
+    also "float_first", "int_first", "repeat", "float_switch", "int_update", "int_diff"), with `xor` and `nbits`
+    (payload bits) for XOR codes, `payload` and `neg` (the sign bit: 1 adds) for int codes, `sig_code` / `mult_code`
+    (None, "same", "zero", "set") of a header, and `sig`, `mult`, `is_float`, `t` and `bits` after the datapoint."""
     b = Bits(bytes(data))
     out = []
+    cur = {}
     prev_time = prev_delta = 0
     unit, unit_changed = 0, False
     prev_bits = prev_xor = 0
@@ -102,50 +110,68 @@ def decode(data, int_optimized, default_unit=1):
                     unit = tu
                     continue
             break
+        cur.update(unit_changed=unit_changed, dod=None, bucket="tu64")
         if unit_changed:  # readFullTimestamp: 64 bits of nanoseconds
             return _sign_extend(b.read(64), 64), False, ann
         assert unit in DEFAULT_BUCKET_BITS, "no time encoding scheme for unit %d" % unit
         if b.read(1) == 0:
+            cur.update(dod=0, bucket=0)
             return 0, False, ann
         for ones, vbits in ((1, 7), (2, 9), (3, 12)):  # opcodes 10, 110, 1110
             if b.read(1) == 0:
-                return _sign_extend(b.read(vbits), vbits) * UNIT_NANOS[unit], False, ann
+                d = _sign_extend(b.read(vbits), vbits)
+                cur.update(dod=d, bucket=vbits)
+                return d * UNIT_NANOS[unit], False, ann
         vbits = DEFAULT_BUCKET_BITS[unit]
-        return _sign_extend(b.read(vbits), vbits) * UNIT_NANOS[unit], False, ann
+        d = _sign_extend(b.read(vbits), vbits)
+        cur.update(dod=d, bucket=vbits)
+        return d * UNIT_NANOS[unit], False, ann
 
-    def read_full_float():
+    def read_full_float(kind="full"):
         nonlocal prev_bits, prev_xor
         prev_bits = prev_xor = b.read(64)
+        cur.update(kind=kind, xor=prev_xor, nbits=64)
 
     def read_next_float():  # float_encoder_iterator.go:117-165
         nonlocal prev_bits, prev_xor
         if b.read(1) == 0:
             prev_xor = 0
+            cur.update(kind="zero", xor=0, nbits=0)
             return
         if b.read(1) == 0:  # '10' contained
             pl, pt = _lz_tz(prev_xor)
             prev_xor = b.read(64 - pl - pt) << pt
+            cur.update(kind="contained", nbits=64 - pl - pt)
         else:  # '11' uncontained
             hdr = b.read(12)
             lead, nbits = hdr >> 6, (hdr & 63) + 1
             prev_xor = b.read(nbits) << (64 - lead - nbits)
+            cur.update(kind="new", nbits=nbits)
+        cur["xor"] = prev_xor
         prev_bits ^= prev_xor
 
     def read_sig_mult():  # iterator.go:178-193
         nonlocal sig, mult
+        cur.update(sig_code="same", mult_code="same")
         if b.read(1) == 1:
             sig = 0 if b.read(1) == 0 else b.read(6) + 1
+            cur["sig_code"] = "set" if sig else "zero"
         if b.read(1) == 1:
             mult = b.read(3)
+            cur["mult_code"] = "set"
             assert mult <= 6, "invalid multiplier"
 
     def read_int_diff():  # iterator.go:195-219 (sign bit 1 = add)
         nonlocal int_val
-        sign = 1.0 if b.read(1) == 1 else -1.0
-        int_val += sign * float(b.read(sig))
+        neg = b.read(1)
+        sign = 1.0 if neg == 1 else -1.0
+        payload = b.read(sig)
+        cur.update(neg=neg, payload=payload)
+        int_val += sign * float(payload)
 
     first = True
     while True:
+        cur = {"kind": None, "sig_code": None, "mult_code": None}
         if first:
             nt = _sign_extend(b.read(64), 64)
             if unit == 0:
@@ -168,25 +194,28 @@ def decode(data, int_optimized, default_unit=1):
             read_full_float() if first else read_next_float()
         elif first:
             if b.read(1) == 1:
-                read_full_float()
+                read_full_float("float_first")
                 is_float = True
             else:
+                cur["kind"] = "int_first"
                 read_sig_mult()
                 read_int_diff()
         else:
             if b.read(1) == 0:  # update
                 if b.read(1) == 1:
-                    pass  # repeat
+                    cur["kind"] = "repeat"
                 elif b.read(1) == 1:
-                    read_full_float()
+                    read_full_float("float_switch")
                     is_float = True
                 else:
+                    cur["kind"] = "int_update"
                     read_sig_mult()
                     read_int_diff()
                     is_float = False
             elif is_float:
                 read_next_float()
             else:
+                cur["kind"] = "int_diff"
                 read_int_diff()
         if not int_optimized or is_float:
             vbits = prev_bits
@@ -194,6 +223,9 @@ def decode(data, int_optimized, default_unit=1):
             v = int_val if mult == 0 else int_val / (10.0 ** mult)
             vbits = struct.unpack("<Q", struct.pack("<d", v))[0]
         out.append((prev_time, vbits, unit, ann))
+        if trace is not None:
+            cur.update(t=prev_time, bits=vbits, sig=sig, mult=mult, is_float=is_float)
+            trace.append(cur)
         first = False
         # the reference keys "first" on PrevTime == 0 (timestamp_iterator.go:89); same thing for real timestamps
         assert prev_time != 0

@@ -71,7 +71,7 @@ inline void emit_code_p(EncLane &s, uint32_t *tile, int lane, uint32_t hdr, int 
 DRIVER = r"""
 template <bool INT_OPT>
 static long long drive(const int64_t *ts, const double *vals, const uint8_t *units, size_t n, int64_t start, int unit,
-                       int default_unit, int use_tier2, uint8_t *out, size_t cap, int *n_tier2) {
+                       int default_unit, int use_tier2, uint8_t *out, size_t cap, int *n_tier2, uint8_t *tiers) {
   std::vector<uint32_t> tile((n * 6 + 64) * ENC_STRIDE, 0u);
   EncLane s;
   memset(&s, 0, sizeof(s));
@@ -95,6 +95,7 @@ static long long drive(const int64_t *ts, const double *vals, const uint8_t *uni
       tier2_commit<INT_OPT>(s, tile.data(), 0, fb, c2);
       s.n_enc++;
       (*n_tier2)++;
+      if (tiers) tiers[i] = 2;
     } else {
       uint32_t hdr;
       int hb;
@@ -106,6 +107,7 @@ static long long drive(const int64_t *ts, const double *vals, const uint8_t *uni
         emit_code(s, tile.data(), 0, hdr, hb, payload, plen);
         s.n_enc++;
       }
+      if (tiers) tiers[i] = 1;
     }
     steady = (u == s.unit) && (s.unit >= 1 && s.unit <= 4) && s.n_enc > 0;
   }
@@ -124,9 +126,9 @@ static long long drive(const int64_t *ts, const double *vals, const uint8_t *uni
 }
 extern "C" long long dev_encode_series(const int64_t *ts, const double *vals, const uint8_t *units, size_t n,
                                        int64_t start, int unit, int int_opt, int default_unit, int use_tier2,
-                                       uint8_t *out, size_t cap, int *n_tier2) {
-  return int_opt ? drive<true>(ts, vals, units, n, start, unit, default_unit, use_tier2, out, cap, n_tier2)
-                 : drive<false>(ts, vals, units, n, start, unit, default_unit, use_tier2, out, cap, n_tier2);
+                                       uint8_t *out, size_t cap, int *n_tier2, uint8_t *tiers) {
+  return int_opt ? drive<true>(ts, vals, units, n, start, unit, default_unit, use_tier2, out, cap, n_tier2, tiers)
+                 : drive<false>(ts, vals, units, n, start, unit, default_unit, use_tier2, out, cap, n_tier2, tiers);
 }
 """
 
@@ -159,8 +161,11 @@ def _fn(name):
     return r"__device__[^\n;{]*\b%s\s*\(" % re.escape(name)
 
 
-@pytest.fixture(scope="module")
-def dev():
+def build_dev_encoder():
+    """Compiles the encoder's general path and second tier for the host (g++ only) and returns the loaded library:
+    `dev_encode_series(ts, vals, units, n, start, unit, int_opt, default_unit, use_tier2, out, cap, &n_tier2,
+    tiers)` returns the stream's length, or minus the status; `tiers` (may be NULL) receives per datapoint 1 for
+    the general path and 2 for the second tier."""
     enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
     com = open(os.path.join(CSRC, "m3tsz_common.cuh")).read()
     consts = "\n".join(re.findall(r"^constexpr [^\n]*\bk(?:Marker|MaxMult)[^\n]*$", com, flags=re.M))
@@ -187,8 +192,13 @@ def dev():
     lib = C.CDLL(so)
     lib.dev_encode_series.restype = C.c_longlong
     lib.dev_encode_series.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int64, C.c_int, C.c_int,
-                                      C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_int)]
+                                      C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.c_void_p]
     return lib
+
+
+@pytest.fixture(scope="module")
+def dev():
+    return build_dev_encoder()
 
 
 def _dev_encode(dev, ts, vals, start, unit, int_opt, use_tier2, units=None):
@@ -199,7 +209,7 @@ def _dev_encode(dev, ts, vals, start, unit, int_opt, use_tier2, units=None):
     nt = C.c_int()
     n = dev.dev_encode_series(ts.ctypes.data, vals.ctypes.data, None if un is None else un.ctypes.data, len(ts),
                               int(start), int(unit), int(int_opt), 1, int(use_tier2), out.ctypes.data, len(out),
-                              C.byref(nt))
+                              C.byref(nt), None)
     assert n >= 0, n
     return out[:n].tobytes(), nt.value
 
