@@ -1,24 +1,12 @@
 """ctypes binding of the aggregation oracle (tests/agg_oracle.c -> tests/libm3tsz_agg_oracle.so): the aggregator's
 Gauge with expensive aggregations (sumSq, Stdev), its Counter and stdev, src/aggregator/aggregation/{gauge,counter,
 common}.go.  Test infrastructure only, like oracle_lib.py; __graft_entry__.build() compiles the library, and
-build_agg_oracle() rebuilds it when the source is newer."""
+build_c_oracle() rebuilds it when the source is newer."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(_HERE, "agg_oracle.c")
-LIB_PATH = os.path.join(_HERE, "libm3tsz_agg_oracle.so")
-CFLAGS = ["-O2", "-g", "-fPIC", "-std=c11", "-Wall", "-Wextra", "-ffp-contract=off", "-fno-strict-aliasing"]
-
-
-def build_agg_oracle(force=False):
-    if not force and os.path.exists(LIB_PATH) and os.path.getmtime(LIB_PATH) >= os.path.getmtime(SRC):
-        return LIB_PATH
-    subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", LIB_PATH, SRC, "-lm"])
-    return LIB_PATH
+from host_build import build_c_oracle
 
 
 def _ptr(a):
@@ -36,7 +24,7 @@ METRIC_COUNTER, METRIC_GAUGE = 1, 3  # metric.Type ids
 def _agg_lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(build_agg_oracle())
+        L = C.CDLL(build_c_oracle("agg"))
         vp = C.c_void_p
         sigs = {
             "m3o_go_int64": (C.c_int64, [C.c_double]),

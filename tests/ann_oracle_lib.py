@@ -2,29 +2,17 @@
 path of m3tsz_aggregate_tiles_annotated composed from the oracles: the reference iterator's per-datapoint annotations
 (oracle_lib), the window rule (ann_oracle.c), the element (elem_oracle_lib over the aggregation oracle's windows) and
 the reference encoder writing every datapoint of a window with the window's annotation.  Test infrastructure only,
-like elem_oracle_lib.py; __graft_entry__.build() compiles the library, and build_ann_oracle() rebuilds it when the
+like elem_oracle_lib.py; __graft_entry__.build() compiles the library, and build_c_oracle() rebuilds it when the
 source is newer."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 import elem_oracle_lib as E
 import oracle_lib as O
+from host_build import build_c_oracle
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(_HERE, "ann_oracle.c")
-LIB_PATH = os.path.join(_HERE, "libm3tsz_ann_oracle.so")
-CFLAGS = ["-O2", "-g", "-fPIC", "-std=c11", "-Wall", "-Wextra", "-ffp-contract=off", "-fno-strict-aliasing"]
 TRANSFORM_RESET = 5
-
-
-def build_ann_oracle(force=False):
-    if not force and os.path.exists(LIB_PATH) and os.path.getmtime(LIB_PATH) >= os.path.getmtime(SRC):
-        return LIB_PATH
-    subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", LIB_PATH, SRC])
-    return LIB_PATH
 
 
 def _ptr(a):
@@ -37,7 +25,7 @@ _lib = None
 def _ann_lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(build_ann_oracle())
+        L = C.CDLL(build_c_oracle("ann"))
         vp = C.c_void_p
         L.m3o_window_annotations.restype = None
         L.m3o_window_annotations.argtypes = [vp, vp, C.c_size_t, C.c_int64, C.c_int64, C.c_size_t, vp]

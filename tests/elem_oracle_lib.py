@@ -1,33 +1,20 @@
 """ctypes binding of the multi-type element oracle (tests/elem_oracle.c -> tests/libm3tsz_elem_oracle.so): what an
 element with several aggregation types writes for its flushed windows, GenericElem.processValue's loop over
 e.aggTypes.  Test infrastructure only, like xf_oracle_lib.py; __graft_entry__.build() compiles the library, and
-build_elem_oracle() rebuilds it when the source is newer.  The tile path (decode -> downsample -> ValueOf of every
+build_c_oracle() rebuilds it when the source is newer.  The tile path (decode -> downsample -> ValueOf of every
 type -> the element) composes this oracle with the aggregation oracle (agg_oracle_lib.aggregate_tiles_series_ex)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 import agg_oracle_lib as A
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(_HERE, "elem_oracle.c")
-LIB_PATH = os.path.join(_HERE, "libm3tsz_elem_oracle.so")
-CFLAGS = ["-O2", "-g", "-fPIC", "-std=c11", "-Wall", "-Wextra", "-ffp-contract=off", "-fno-strict-aliasing"]
+from host_build import build_c_oracle
 
 # m3tsz_element_state: m3tsz_transform_state (type 0's binary-op input in prev_v), then types 1..7's (160 bytes)
 ELEM_STATE_DTYPE = np.dtype([("has_prev", "<i4"), ("reserved0", "<i4"), ("prev_t", "<i8"), ("prev_v", "<f8"),
                              ("sum", "<f8", (8,)), ("reserved1", "<u8"), ("prev_v_more", "<f8", (7,)),
                              ("reserved", "<u8")])
 assert ELEM_STATE_DTYPE.itemsize == 160
-
-
-def build_elem_oracle(force=False):
-    if not force and os.path.exists(LIB_PATH) and os.path.getmtime(LIB_PATH) >= os.path.getmtime(SRC):
-        return LIB_PATH
-    subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", LIB_PATH, SRC, "-lm"])
-    return LIB_PATH
 
 
 def _ptr(a):
@@ -40,7 +27,7 @@ _lib = None
 def _elem_lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(build_elem_oracle())
+        L = C.CDLL(build_c_oracle("elem"))
         vp = C.c_void_p
         L.m3o_element_series.restype = None
         L.m3o_element_series.argtypes = [vp, C.c_size_t, C.c_int, C.c_int64, C.c_size_t, vp, vp, vp, C.c_size_t,

@@ -2,11 +2,9 @@
 (agg_oracle_lib), each source's chain through the transformation oracle with its record (xf_oracle_lib), the fold of
 every group window in listed order (tests/rollup_oracle.c -> tests/libm3tsz_rollup_oracle.so), the element oracle
 for the rollup element with the post-ops and its record (elem_oracle_lib) and the reference encoder.  Test
-infrastructure only; __graft_entry__.build() compiles the library, and build_rollup_oracle() rebuilds it when the
+infrastructure only; __graft_entry__.build() compiles the library, and build_c_oracle() rebuilds it when the
 source is newer."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
@@ -15,20 +13,9 @@ import blocks_oracle_lib as B
 import elem_oracle_lib as E
 import oracle_lib as O
 import xf_oracle_lib as X
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(_HERE, "rollup_oracle.c")
-LIB_PATH = os.path.join(_HERE, "libm3tsz_rollup_oracle.so")
-CFLAGS = ["-O2", "-g", "-fPIC", "-std=c11", "-Wall", "-Wextra", "-ffp-contract=off", "-fno-strict-aliasing"]
+from host_build import build_c_oracle
 
 ERR_INVALID_ARG = 101  # M3TSZ_ERR_INVALID_ARG
-
-
-def build_rollup_oracle(force=False):
-    if not force and os.path.exists(LIB_PATH) and os.path.getmtime(LIB_PATH) >= os.path.getmtime(SRC):
-        return LIB_PATH
-    subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", LIB_PATH, SRC, "-lm"])
-    return LIB_PATH
 
 
 def _ptr(a):
@@ -41,7 +28,7 @@ _lib = None
 def _rollup_lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(build_rollup_oracle())
+        L = C.CDLL(build_c_oracle("rollup"))
         vp = C.c_void_p
         L.m3o_rollup_gauge.restype = None
         L.m3o_rollup_gauge.argtypes = [vp, C.c_size_t, vp, vp]

@@ -1,5 +1,5 @@
 """The encoder sets' APPEND path, compiled for the host from the .cu source text and driven one open encoder at a
-time the way a lane of the append kernel drives it: the encoder functions of test_device_encoder_on_host plus
+time the way a lane of the append kernel drives it: the encoder functions of the encoder harness plus
 `EncStateInternal`, `enc_state_reset`, `enc_state_load<INT_OPT>` / `enc_state_save<INT_OPT>`, `enc_check_time`,
 `enc_snapshot_words` (m3tsz_encode.cu) and `xxh64` (m3tsz_common.cuh) are cut out of the source at test time.
 Between two calls only the 128-byte state and the slot's whole sectors survive, as on the device.
@@ -11,151 +11,19 @@ reference's value families, Gaussian walks, special values, unit changes at call
 repeated across a boundary (not rewritten) and long annotations (XXH64's 32-byte path).  A CPU regression
 harness for the device source; nothing of it ships."""
 import ctypes as C
-import os
 import random
-import re
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import oracle_lib as O
-from test_device_encoder_on_host import CSRC, EMIT, ROOT, SEC, SHIM, _cut, _fn, _series
-
-ERRS = "enum { M3TSZ_ERR_CAPACITY = 100, M3TSZ_ERR_INVALID_ARG = 101 };\n"
-
-DRIVER = r"""
-// one append call on one encoder: what a lane of encode_kernel<., false, ., true> does with its series
-template <bool INT_OPT>
-static long long append_call(m3tsz_encoder_state *st, uint8_t *slot, const int64_t *ts, const double *vals,
-                             const uint8_t *units, int unit, size_t n, const uint32_t *ann_off,
-                             const uint32_t *ann_len, const uint8_t *ann_bytes, int use_tier2, int *err) {
-  std::vector<uint32_t> tile((n * 40 + 64) * ENC_STRIDE, 0u);
-  EncLane s;
-  memset(&s, 0, sizeof(s));
-  uint64_t ann_cs = 0;
-  *err = enc_state_load<INT_OPT>(*st, s, tile.data(), 0, ann_cs);
-  if (*err) return 0;
-  const uint32_t n0 = s.n_enc;
-  if (n && s.n_enc == 0) put64(s, tile.data(), 0, (uint64_t)s.prev_time, 64);
-  for (size_t i = 0; i < n; i++) {
-    const int64_t t = ts[i];
-    const double v = vals[i];
-    const int u = units ? (int)units[i] : unit;
-    *err = enc_check_time(s, t, u);
-    if (*err) break;
-    if (ann_len[i]) {  // timestamp_encoder.go:166-195 with the checksum carried in the state
-      const uint64_t h = xxh64(ann_bytes + ann_off[i], ann_len[i]);
-      if (h != ann_cs) {
-        put32(s, tile.data(), 0, (kMarkerOpcode << 2) | (uint32_t)kMarkerAnnotation, kMarkerBits);
-        uint64_t ux = ((uint64_t)(ann_len[i] - 1)) << 1;
-        while (ux >= 0x80) {
-          put32(s, tile.data(), 0, (uint32_t)(ux & 0x7f) | 0x80u, 8);
-          ux >>= 7;
-        }
-        put32(s, tile.data(), 0, (uint32_t)ux, 8);
-        for (uint32_t b = 0; b < ann_len[i]; b++) put32(s, tile.data(), 0, ann_bytes[ann_off[i] + b], 8);
-      }
-      ann_cs = h;
-    }
-    const bool steady = (u == s.unit) && (s.unit >= 1 && s.unit <= 4) && s.n_enc > 0;
-    uint64_t fb;
-    memcpy(&fb, &v, 8);
-    const int64_t delta = (int64_t)((uint64_t)t - (uint64_t)s.prev_time);
-    Tier2 c2;
-    if (use_tier2 && tier2_candidate<INT_OPT>(s, steady, delta, fb, v, c2)) {
-      s.prev_time = t;
-      s.prev_delta = delta;
-      tier2_commit<INT_OPT>(s, tile.data(), 0, fb, c2);
-    } else {
-      uint32_t hdr;
-      int hb;
-      encode_time(s, tile.data(), 0, t, u, hdr, hb);
-      if (s.err) {  // enc_check_time let through a datapoint encode_time refuses
-        *err = -1;
-        return -1;
-      }
-      uint64_t payload;
-      int plen;
-      encode_value<INT_OPT>(s, v, hdr, hb, payload, plen);
-      emit_code(s, tile.data(), 0, hdr, hb, payload, plen);
-    }
-    s.n_enc++;
-  }
-  // the epilogue's flush: whole sectors to the slot, <= 7 words stay
-  const uint32_t done = s.k & ~7u;
-  for (uint32_t w = 0; w < done; w++)
-    for (int b = 0; b < 4; b++) slot[(s.words_out + w) * 4ull + b] = (uint8_t)(tile[w * ENC_STRIDE] >> (24 - 8 * b));
-  for (uint32_t w = done; w < s.k; w++) tile[(w - done) * ENC_STRIDE] = tile[w * ENC_STRIDE];
-  s.words_out += done;
-  s.k -= done;
-  if (s.n_enc != n0) enc_state_save<INT_OPT>(*st, s, tile.data(), 0, ann_cs);
-  return (long long)(s.n_enc - n0);
-}
-extern "C" long long dev_append(m3tsz_encoder_state *st, uint8_t *slot, const int64_t *ts, const double *vals,
-                                const uint8_t *units, int unit, size_t n, const uint32_t *ann_off,
-                                const uint32_t *ann_len, const uint8_t *ann_bytes, int int_opt, int use_tier2,
-                                int *err) {
-  return int_opt ? append_call<true>(st, slot, ts, vals, units, unit, n, ann_off, ann_len, ann_bytes, use_tier2, err)
-                 : append_call<false>(st, slot, ts, vals, units, unit, n, ann_off, ann_len, ann_bytes, use_tier2, err);
-}
-extern "C" void dev_reset(m3tsz_encoder_state *st, int64_t start, int default_unit, int int_opt) {
-  enc_state_reset(*st, start, default_unit, int_opt != 0);
-}
-// the snapshot kernel's work for one encoder; returns Len()
-extern "C" uint64_t dev_snapshot(const m3tsz_encoder_state *st, uint8_t *slot) {
-  uint32_t w[12];
-  uint64_t at = 0;
-  const uint32_t n = enc_snapshot_words(*st, w, at);
-  for (uint32_t i = 0; i < n; i++)
-    for (int b = 0; b < 4; b++) slot[(at + i) * 4 + b] = (uint8_t)(w[i] >> (24 - 8 * b));
-  return st->num_encoded ? (st->bits + kMarkerBits + 7) / 8 : 0;
-}
-"""
+from host_build import build_dev_append
+from test_device_encoder_on_host import SEC, _series
 
 
 @pytest.fixture(scope="module")
 def dev():
-    enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
-    com = open(os.path.join(CSRC, "m3tsz_common.cuh")).read()
-    hdr = open(os.path.join(ROOT, "include", "m3tsz_b200.h")).read()
-    state = re.search(r"typedef struct m3tsz_encoder_state \{.*?\} m3tsz_encoder_state;", hdr, flags=re.S).group(0)
-    consts = "\n".join(re.findall(r"^constexpr [^\n]*\bk(?:Marker|MaxMult)[^\n]*$", com, flags=re.M))
-    parts = [ERRS, state, consts, _cut(com, r"enum SchemeKind"),
-             _cut(com, r"__host__ __device__[^\n{;]*\bunit_is_valid\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\bunit_nanos\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\bscheme_kind_for_unit\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\binitial_time_unit\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\bxxh64\s*\("),
-             _cut(com, _fn("num_sig")), _cut(com, _fn("mult_pow10")),
-             _cut(enc, r"struct EncLane"), _cut(enc, _fn("put32")), _cut(enc, _fn("put64")), EMIT,
-             _cut(enc, _fn("emit_code"))]
-    for name in ("maybe_int", "go_f64_to_u64_via_i64", "convert_to_int_float", "track_new_sig", "sig_mult_hdr",
-                 "xor_code", "encode_value", "encode_time"):
-        parts.append(_cut(enc, _fn(name)))
-    parts += [_cut(enc, r"struct Tier2"), _cut(enc, _fn("div_unit")), _cut(enc, _fn("tier2_candidate")),
-              _cut(enc, _fn("tier2_commit")), _cut(enc, r"struct EncStateInternal")]
-    for name in ("enc_state_tag", "enc_state_reset", "enc_state_load", "enc_state_save", "enc_check_time",
-                 "enc_snapshot_words"):
-        parts.append(_cut(enc, _fn(name)))
-    body = "\n".join(parts)
-    assert "asm" not in body, "a PTX block slipped into the host build"
-    d = tempfile.mkdtemp(prefix="m3dev_append_host_")
-    path = os.path.join(d, "dev_append_host.cpp")
-    open(path, "w").write(SHIM + body + DRIVER)
-    so = os.path.join(d, "dev_append_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
-    vp = C.c_void_p
-    lib.dev_append.restype = C.c_longlong
-    lib.dev_append.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_size_t, vp, vp, vp, C.c_int, C.c_int,
-                               C.POINTER(C.c_int)]
-    lib.dev_reset.restype = None
-    lib.dev_reset.argtypes = [vp, C.c_int64, C.c_int, C.c_int]
-    lib.dev_snapshot.restype = C.c_uint64
-    lib.dev_snapshot.argtypes = [vp, vp]
-    return lib
+    return build_dev_append()
 
 
 class HostEncoder:

@@ -5,37 +5,16 @@ lane-strided chunking, the dp4a partial sums, the head / tail handling and the f
 device source.  Compared with zlib.adler32 (= ts.Segment.CalculateChecksum, src/dbnode/ts/segment.go:60-76) for
 every alignment and a range of lengths, CSR and (offset, size) addressing, expected-checksum mismatches."""
 import ctypes as C
-import os
-import subprocess
-import tempfile
 import zlib
 
 import numpy as np
 import pytest
 
-from test_device_encoder_on_host import _cut
+from host_build import compile, constants, cut, source_text
 
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-CSRC = os.path.join(ROOT, "m3_b200", "csrc")
-
-SHIM = r"""
-#include <cstdint>
-#include <cstring>
-#include "%s"
-#define __device__
-#define __global__
-#define __forceinline__ inline
-#define __launch_bounds__(...)
-struct Dim3 { unsigned x, y, z; };
-static thread_local Dim3 threadIdx, blockIdx, blockDim;
-struct uint4 { uint32_t x, y, z, w; };
-static inline uint4 __ldg(const uint4 *p) { return *p; }
-static inline uint32_t __dp4a(uint32_t a, uint32_t b, uint32_t c) {
-  for (int i = 0; i < 4; i++) c += ((a >> (8 * i)) & 0xffu) * ((b >> (8 * i)) & 0xffu);
-  return c;
-}
+# warp_sum_u64's contract -- lane 0 ends up with the sum over the warp -- for lanes executed 31, 30, .. 0
+WARP_SUM = r"""
 namespace m3tsz {
-// warp_sum_u64's contract -- lane 0 ends up with the sum over the warp -- for lanes executed 31, 30, .. 0
 static thread_local uint64_t g_acc[2];
 static thread_local int g_call;
 static inline uint64_t warp_sum_u64(uint64_t v) { g_acc[g_call] += v; return g_acc[g_call++]; }
@@ -57,7 +36,7 @@ extern "C" void dev_checksum(const uint8_t *streams, uint64_t streams_bytes, con
     for (int lane = 31; lane >= 0; lane--) {
       const uint64_t t = s * 32 + (uint64_t)lane;
       blockIdx.x = (unsigned)(t / blockDim.x);
-      threadIdx.x = (unsigned)(t %% blockDim.x);
+      threadIdx.x = (unsigned)(t % blockDim.x);
       g_call = 0;
       checksum_kernel(p);
     }
@@ -68,22 +47,14 @@ extern "C" void dev_checksum(const uint8_t *streams, uint64_t streams_bytes, con
 
 @pytest.fixture(scope="module")
 def dev():
-    src = open(os.path.join(CSRC, "m3tsz_checksum.cu")).read()
-    ker = open(os.path.join(CSRC, "m3tsz_kernels.h")).read()
-    a = src.index("namespace m3tsz {")
-    b = src.index("cudaError_t launch_checksum")
-    body = src[a:b] + "\n}  // namespace m3tsz\n"
-    ws = _cut(body, r"__device__[^\n;{]*\bwarp_sum_u64\s*\(")
-    body = body.replace(ws, "// (warp_sum_u64: see the shim)\n")
+    src = source_text("m3tsz_checksum.cu")
+    body = src[src.index("namespace m3tsz {"): src.index("cudaError_t launch_checksum")] + "\n}  // namespace m3tsz\n"
+    body = body.replace(cut(body, r"__device__[^\n;{]*\bwarp_sum_u64\s*\("), "// (warp_sum_u64: see WARP_SUM)\n")
     body = body.replace("#pragma unroll", "")
-    params = "namespace m3tsz {\nconstexpr unsigned FULL_MASK = 0xffffffffu;\n" + _cut(ker, r"struct ChecksumParams") + "\n}\n"
+    params = "namespace m3tsz {\n%s\n%s\n}\n" % (constants(source_text("m3tsz_common.cuh"), "FULL_MASK"),
+                                                 cut(source_text("m3tsz_kernels.h"), r"struct ChecksumParams"))
     assert "__shfl" not in body and "<<<" not in body
-    d = tempfile.mkdtemp(prefix="m3dev_ck_host_")
-    path = os.path.join(d, "dev_ck_host.cpp")
-    open(path, "w").write(SHIM % os.path.join(ROOT, "include", "m3tsz_b200.h") + params + body + DRIVER.replace("%%", "%"))
-    so = os.path.join(d, "dev_ck_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
+    lib = compile("dev_ck_host", WARP_SUM + params + body, DRIVER)
     lib.dev_checksum.restype = None
     return lib
 

@@ -11,183 +11,24 @@ identical in float mode (datapoints and error), and in int mode never more datap
 difference being the documented one (DESIGN.md §6, difference 1: the reference's `readBits` may overwrite an earlier
 error and carry on; the kernel stops at the first failed read)."""
 import base64
-import ctypes as C
 import json
 import os
 import random
-import re
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import oracle_lib as O
-from test_device_encoder_on_host import _cut, _fn
+from host_build import DevDecode, build_dev_decoder
 
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-CSRC = os.path.join(ROOT, "m3_b200", "csrc")
 G = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "m3tsz_goldens.json")))
 SEC = 10 ** 9
-
-SHIM = r"""
-#include <cmath>
-#include <cstdint>
-#include <cstring>
-#include "%s"
-#define __device__
-#define __host__
-#define __forceinline__ inline
-#define __noinline__
-static inline double __dsub_rn(double a, double b) { return a - b; }
-static inline double __dadd_rn(double a, double b) { return a + b; }
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline double __ull2double_rn(unsigned long long a) { return (double)a; }
-static inline long long __double_as_longlong(double a) { long long r; memcpy(&r, &a, 8); return r; }
-static inline uint32_t __ldg(const uint32_t *p) { return *p; }
-static inline uint32_t __byte_perm(uint32_t v, uint32_t, uint32_t sel) {  // only the byte swap is used
-  if (sel != 0x0123) __builtin_trap();
-  return __builtin_bswap32(v);
-}
-// funnel shift left by (sh & 31): the high word of (hi:lo) << sh  (PTX shf.l.wrap)
-static inline uint32_t __funnelshift_l(uint32_t lo, uint32_t hi, uint32_t sh) {
-  sh &= 31;
-  return sh ? ((hi << sh) | (lo >> (32 - sh))) : hi;
-}
-static inline unsigned long long atomicAdd(unsigned long long *p, unsigned long long v) {
-  const unsigned long long o = *p;
-  *p += v;
-  return o;
-}
-constexpr int DEC_QUADS = 16;
-// ---- PTX helpers of m3tsz_common.cuh restated ----
-static inline uint64_t shl64(uint64_t x, int n) { return n >= 64 ? 0ull : x << n; }
-static inline void lz_tz(uint64_t v, int &lz, int &tz) {
-  if (!v) { lz = 64; tz = 0; return; }
-  lz = __builtin_clzll(v);
-  tz = __builtin_ctzll(v);
-}
-"""
-
-DRIVER = r"""
-template <bool INT_OPT>
-static int drive(const uint8_t *buf, uint64_t nbytes, uint64_t o0, uint64_t o1, int default_unit, int64_t *ts,
-                 uint64_t *vals, uint32_t *bitpos, uint32_t cap, uint32_t *n_out, m3tsz_dp_event *events,
-                 uint64_t ev_cap, unsigned long long *ev_count, int *units, uint32_t *ann) {
-  DecState s;
-  memset(&s, 0, sizeof(s));
-  s.scheme = kSchemeNone;
-  // the kernel's addressing: base = the stream's first word rounded down to a 16-word boundary
-  const uint64_t w = o0 >> 2;
-  s.wbase = w & ~(uint64_t)15;
-  s.pos = (uint32_t)(w - s.wbase) * 32u + (uint32_t)(o0 & 3) * 8u;
-  s.end = s.pos + (uint32_t)(o1 - o0) * 8u;
-  const uint32_t pos0 = s.pos;
-  SlowSrc src;
-  src.base = buf;
-  src.nbytes = nbytes;
-  src.ring_lane = nullptr;
-  src.ring_safe = 0;
-  EventSink ev;
-  ev.events = events;
-  ev.capacity = ev_cap;
-  ev.count = ev_count;
-  ev.series = 0;
-  ev.pos0 = pos0;
-  while (!s.done && s.err == 0 && s.n < cap) {
-    int64_t t = 0;
-    uint64_t v = 0;
-    if (decode_dp_slow<INT_OPT>(s, src, default_unit, t, v, &ev)) {
-      ts[s.n] = t;
-      vals[s.n] = v;
-      bitpos[s.n] = s.pos - pos0;  // the stream bit after the datapoint
-      s.n++;
-    }
-  }
-  *n_out = s.n;
-  units[0] = s.emit_unit;  // unit at the last datapoint produced
-  units[1] = s.first_unit;  // ... at the first
-  units[2] = s.unit;        // unit in force when the decode stopped
-  // the first annotation, as the kernel's m3tsz_annotation_ref holds it
-  ann[0] = s.ann_count ? s.ann_bit - pos0 : 0u;
-  ann[1] = s.ann_len;
-  ann[2] = s.ann_count;
-  return s.err;
-}
-extern "C" int dev_decode(const uint8_t *buf, uint64_t nbytes, uint64_t o0, uint64_t o1, int int_opt, int default_unit,
-                          int64_t *ts, uint64_t *vals, uint32_t *bitpos, uint32_t cap, uint32_t *n_out,
-                          m3tsz_dp_event *events, uint64_t ev_cap, unsigned long long *ev_count, int *units,
-                          uint32_t *ann) {
-  return int_opt ? drive<true>(buf, nbytes, o0, o1, default_unit, ts, vals, bitpos, cap, n_out, events, ev_cap,
-                               ev_count, units, ann)
-                 : drive<false>(buf, nbytes, o0, o1, default_unit, ts, vals, bitpos, cap, n_out, events, ev_cap,
-                                ev_count, units, ann);
-}
-"""
-
-
-def build_dev_decoder():
-    """Compiles the decoder's complete grammar for the host (g++ only) and returns the loaded library."""
-    dec = open(os.path.join(CSRC, "m3tsz_decode.cu")).read()
-    com = open(os.path.join(CSRC, "m3tsz_common.cuh")).read()
-    consts = "\n".join(re.findall(r"^constexpr [^\n]*\bk(?:Marker|MaxMult)[^\n]*$", com, flags=re.M))
-    m = re.search(r"#define M3_RD\(nbits, var\).*?\n  \}\n", dec, flags=re.S)
-    assert m
-    parts = [consts, _cut(com, r"enum SchemeKind"),
-             _cut(com, r"__host__ __device__[^\n{;]*\bunit_is_valid\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\bunit_nanos\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\bscheme_kind_for_unit\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\binitial_time_unit\s*\("),
-             _cut(com, _fn("sign_extend")), _cut(com, _fn("mult_pow10")), _cut(com, _fn("load_be32")),
-             _cut(dec, r"struct DecState"), _cut(dec, r"struct SlowSrc"), _cut(dec, r"struct EventSink"),
-             _cut(dec, _fn("push_event")), _cut(dec, _fn("gpeek64")), m.group(0), _cut(dec, _fn("decode_dp_slow"))]
-    body = "\n".join(parts)
-    assert "asm" not in body
-    d = tempfile.mkdtemp(prefix="m3dev_dec_host_")
-    path = os.path.join(d, "dev_dec_host.cpp")
-    open(path, "w").write(SHIM % os.path.join(ROOT, "include", "m3tsz_b200.h") + body + DRIVER)
-    so = os.path.join(d, "dev_dec_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
-    lib.dev_decode.restype = C.c_int
-    return lib
 
 
 @pytest.fixture(scope="module")
 def dev():
     return build_dev_decoder()
-
-
-class DevDecode:
-    """One stream through the complete grammar: `status`, `dps` [(ts, value bits)], `bitpos` (the stream bit after
-    each datapoint), `emit_unit` / `first_unit` / `unit` (at the last and first datapoint, and when the decode
-    stopped), `ann` (the first annotation: bit offset from the stream's first bit, length, count) and `events`
-    (uint8 [E, 32] rows of m3tsz_dp_event, series 0)."""
-
-    def __init__(self, dev, stream, int_opt, lead=0, cap=4096, default_unit=1, ev_cap=256):
-        buf = np.zeros(lead + len(stream) + 64, dtype=np.uint8)
-        buf[lead: lead + len(stream)] = np.frombuffer(stream, dtype=np.uint8)
-        ts = np.zeros(cap, dtype=np.int64)
-        vals = np.zeros(cap, dtype=np.uint64)
-        bitpos = np.zeros(cap, dtype=np.uint32)
-        n = C.c_uint32()
-        events = np.zeros((ev_cap, 32), dtype=np.uint8)
-        evc = C.c_ulonglong(0)
-        units = np.zeros(3, dtype=np.int32)
-        ann = np.zeros(3, dtype=np.uint32)
-        p = lambda a: C.c_void_p(a.ctypes.data)
-        self.status = dev.dev_decode(p(buf), C.c_uint64(lead + len(stream)), C.c_uint64(lead),
-                                     C.c_uint64(lead + len(stream)), int(int_opt), int(default_unit), p(ts), p(vals),
-                                     p(bitpos), C.c_uint32(cap), C.byref(n), p(events), C.c_uint64(ev_cap),
-                                     C.byref(evc), p(units), p(ann))
-        k = n.value
-        self.ts, self.vals, self.bitpos = ts[:k], vals[:k], bitpos[:k]
-        self.dps = list(zip(self.ts.tolist(), self.vals.tolist()))
-        self.emit_unit, self.first_unit, self.unit = (int(u) for u in units)
-        self.ann = tuple(int(a) for a in ann)
-        assert evc.value <= ev_cap
-        self.events = events[: evc.value]
 
 
 def _dev_decode(dev, stream, int_opt, lead=0, cap=4096, want_events=False):

@@ -7,23 +7,14 @@ record from the lanes' parts as the epilogue does.  Datapoints and record must e
 bit for bit, on the goldens and on random type sets, op lists and call splits.  A CPU regression harness for the
 device source; nothing of it ships."""
 import ctypes as C
-import os
-import re
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import elem_oracle_lib as E
-from test_device_encoder_on_host import CSRC, ROOT, SHIM, _cut, _fn
+from host_build import compile, constants, cut, fn, source_text
 from test_independent_element import _element_windows, _goldens, random_element_pipeline
 from test_independent_transforms import _splits, _val
-
-EXTRA = r"""
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline double __ll2double_rn(long long a) { return (double)a; }
-"""
 
 DRIVER = r"""
 // lane j of the IN = 5 stage for n non-empty windows (v: [n][k]) of one series, from record `rec`; its datapoints go
@@ -88,26 +79,11 @@ extern "C" void dev_element_series(const int32_t *ops, size_t n_ops, int discard
 
 @pytest.fixture(scope="module")
 def dev():
-    enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
-    hdr = open(os.path.join(ROOT, "include", "m3tsz_b200.h")).read()
-    ids = re.search(r"enum \{ /\* transformation\.Type ids.*?\};", hdr, flags=re.S).group(0)
-    maxk = re.search(r"^#define M3TSZ_MAX_TRANSFORMS \d+$", hdr, flags=re.M).group(0)
-    maxt = re.search(r"^#define M3TSZ_MAX_ELEMENT_TYPES \d+$", hdr, flags=re.M).group(0)
-    state = re.search(r"typedef struct m3tsz_transform_state \{.*?\} m3tsz_transform_state;", hdr,
-                      flags=re.S).group(0)
-    elem = re.search(r"typedef struct m3tsz_element_state \{.*?\} m3tsz_element_state;", hdr, flags=re.S).group(0)
-    consts = "\n".join(re.findall(r"^constexpr uint64_t kXf[^\n]*$", enc, flags=re.M))
-    parts = [EXTRA, ids, maxk, maxt, state, elem, consts, _cut(enc, r"struct XfElem \{")]
+    enc = source_text("m3tsz_encode.cu")
+    parts = [constants(enc, r"kXf\w*"), cut(enc, r"struct XfElem \{")]
     for name in ("xf_isnan", "xf_bits", "xf_per_second", "xf_increase", "xf_window", "xf_element_window"):
-        parts.append(_cut(enc, _fn(name)))
-    body = "\n".join(parts)
-    assert "asm" not in body, "a PTX block slipped into the host build"
-    d = tempfile.mkdtemp(prefix="m3dev_elem_host_")
-    path = os.path.join(d, "dev_elem_host.cpp")
-    open(path, "w").write(SHIM + body + DRIVER)
-    so = os.path.join(d, "dev_elem_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
+        parts.append(cut(enc, fn(name)))
+    lib = compile("dev_elem_host", "\n".join(parts), DRIVER)
     vp = C.c_void_p
     lib.dev_element_series.restype = None
     lib.dev_element_series.argtypes = [vp, C.c_size_t, C.c_int, C.c_int64, C.c_size_t, vp, vp, vp, C.c_size_t, vp,

@@ -1,5 +1,5 @@
 """A deterministic corpus of malformed M3TSZ streams, and the decoder's complete grammar (`decode_dp_slow`, compiled for
-the host by `test_device_decoder_on_host.build_dev_decoder`) against the oracle on every stream of it.
+the host by `host_build.build_dev_decoder`) against the oracle on every stream of it.
 
 The corpus (`corpus(int_opt)`) starts from well-formed base streams, most of them 240 datapoints at a steady cadence
 so that a warp of their variants is on the decoder's hot path when the damage arrives: the goldens and production
@@ -24,7 +24,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as O
-from test_device_decoder_on_host import DevDecode, build_dev_decoder
+from host_build import DevDecode, build_dev_decoder
 
 G = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "m3tsz_goldens.json")))
 SEC = 10 ** 9
@@ -139,14 +139,9 @@ def _base_streams(int_opt):
     return out
 
 
-@functools.lru_cache(maxsize=None)
-def _grammar():
-    return build_dev_decoder()
-
-
 def grammar(stream, int_opt, default_unit=O.UNIT_S):
     """the complete grammar's decode of one stream (a DevDecode)"""
-    return DevDecode(_grammar(), stream, int_opt, cap=CAP, default_unit=default_unit, ev_cap=1024)
+    return DevDecode(build_dev_decoder(), stream, int_opt, cap=CAP, default_unit=default_unit, ev_cap=1024)
 
 
 @functools.lru_cache(maxsize=None)

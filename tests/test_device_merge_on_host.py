@@ -6,33 +6,13 @@ kernel on the series it gave up on).  Compared with the merge oracle AND with th
 of tests/test_independent_merge.py on random fetch shapes (reader errors, out-of-order blocks, empty slices, range
 filters, all four strategies), series-major and point-major strides."""
 import ctypes as C
-import os
-import re
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import oracle_lib as O
 import test_independent_merge as M
-from test_device_encoder_on_host import _cut
-
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-CSRC = os.path.join(ROOT, "m3_b200", "csrc")
-
-SHIM = r"""
-#include <cstdint>
-#include <cstring>
-#include "%s"
-#define __device__
-#define __host__
-#define __global__
-#define __forceinline__ inline
-#define __launch_bounds__(...)
-struct Dim3 { unsigned x, y, z; };
-static thread_local Dim3 threadIdx, blockIdx, blockDim;
-"""
+from host_build import compile, cut, source_text
 
 DRIVER = r"""
 extern "C" void dev_merge(const int64_t *ts, const double *val, uint64_t cap, const uint32_t *n_points,
@@ -70,19 +50,11 @@ extern "C" void dev_merge(const int64_t *ts, const double *val, uint64_t cap, co
 
 @pytest.fixture(scope="module")
 def dev():
-    src = open(os.path.join(CSRC, "m3tsz_merge.cu")).read()
-    ker = open(os.path.join(CSRC, "m3tsz_kernels.h")).read()
-    a = src.index("namespace m3tsz {")
-    b = src.index("cudaError_t launch_merge")
-    body = src[a:b] + "\n}  // namespace m3tsz\n"
-    params = "namespace m3tsz {\n" + _cut(ker, r"struct MergeParams") + "\n}\n"
-    assert "asm" not in body and "<<<" not in body
-    d = tempfile.mkdtemp(prefix="m3dev_merge_host_")
-    path = os.path.join(d, "dev_merge_host.cpp")
-    open(path, "w").write(SHIM % os.path.join(ROOT, "include", "m3tsz_b200.h") + params + body + DRIVER)
-    so = os.path.join(d, "dev_merge_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
+    src = source_text("m3tsz_merge.cu")
+    body = src[src.index("namespace m3tsz {"): src.index("cudaError_t launch_merge")] + "\n}  // namespace m3tsz\n"
+    params = "namespace m3tsz {\n" + cut(source_text("m3tsz_kernels.h"), r"struct MergeParams") + "\n}\n"
+    assert "<<<" not in body
+    lib = compile("dev_merge_host", params + body, DRIVER)
     lib.dev_merge.restype = None
     return lib
 

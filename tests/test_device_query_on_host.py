@@ -4,34 +4,15 @@ the way `launch_prom` picks and shapes them; compared with the oracle's iterator
 independent Python one (tests/test_independent_query_rows.py) on random batches: counters with resets, tolerance
 clamps, NaN, empty series, output capacity overflow, and rows whose count exceeds their capacity (refused unread)."""
 import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import oracle_lib as O
-from test_device_encoder_on_host import _cut
+from host_build import compile, cut, source_text
 from test_independent_query_rows import prom_convert
 
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-CSRC = os.path.join(ROOT, "m3_b200", "csrc")
 SEC = 10 ** 9
-
-SHIM = r"""
-#include <cstdint>
-#include <cstring>
-#include "%s"
-#define __device__
-#define __global__
-#define __forceinline__ inline
-static inline double __dmul_rn(double a, double b) { return a * b; }
-static inline double __dsub_rn(double a, double b) { return a - b; }
-static inline double __dadd_rn(double a, double b) { return a + b; }
-struct Dim3 { unsigned x, y, z; };
-static thread_local Dim3 threadIdx, blockIdx, blockDim;
-"""
 
 DRIVER = r"""
 extern "C" int dev_prom(const int64_t *ts, const double *val, uint64_t cap, const uint32_t *n_points, uint64_t n_series,
@@ -58,19 +39,11 @@ extern "C" int dev_prom(const int64_t *ts, const double *val, uint64_t cap, cons
 
 @pytest.fixture(scope="module")
 def dev():
-    src = open(os.path.join(CSRC, "m3tsz_query.cu")).read()
-    ker = open(os.path.join(CSRC, "m3tsz_kernels.h")).read()
-    a = src.index("namespace m3tsz {")
-    b = src.index("cudaError_t launch_prom")
-    body = src[a:b] + "\n}  // namespace m3tsz\n"
-    params = "namespace m3tsz {\n" + _cut(ker, r"struct PromParams") + "\n}\n"
-    assert "asm" not in body and "<<<" not in body
-    d = tempfile.mkdtemp(prefix="m3dev_query_host_")
-    path = os.path.join(d, "dev_query_host.cpp")
-    open(path, "w").write(SHIM % os.path.join(ROOT, "include", "m3tsz_b200.h") + params + body + DRIVER)
-    so = os.path.join(d, "dev_query_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
+    src = source_text("m3tsz_query.cu")
+    body = src[src.index("namespace m3tsz {"): src.index("cudaError_t launch_prom")] + "\n}  // namespace m3tsz\n"
+    params = "namespace m3tsz {\n" + cut(source_text("m3tsz_kernels.h"), r"struct PromParams") + "\n}\n"
+    assert "<<<" not in body
+    lib = compile("dev_query_host", params + body, DRIVER)
     lib.dev_prom.restype = C.c_int
     return lib
 

@@ -6,17 +6,13 @@ the fold kernel's lane does, and must equal the oracle (tests/rollup_oracle.c) b
 regression harness for the device source; nothing of it ships."""
 import ctypes as C
 import math
-import os
-import re
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import rollup_oracle_lib as R
-from test_device_encoder_on_host import CSRC, SHIM, _cut, _fn
+from host_build import compile, constants, cut, fn, source_text
 
 DRIVER = r"""
 extern "C" void dev_fold_gauge(const double *v, size_t n, double *out5, int64_t *count) {
@@ -45,23 +41,14 @@ extern "C" void dev_fold_counter(const double *v, size_t n, int64_t *out5) {
 
 @pytest.fixture(scope="module")
 def dev():
-    enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
-    com = open(os.path.join(CSRC, "m3tsz_common.cuh")).read()
-    consts = "\n".join(re.findall(r"^constexpr uint64_t kXf[^\n]*$", enc, flags=re.M))
-    parts = [consts, _cut(com, _fn("go_f64_to_i64"))]
+    enc, com = source_text("m3tsz_encode.cu"), source_text("m3tsz_common.cuh")
+    parts = [constants(enc, r"kXf\w*"), cut(com, fn("go_f64_to_i64"))]
     for name in ("xf_isnan", "xf_bits"):
-        parts.append(_cut(enc, _fn(name)))
-    parts += [_cut(enc, r"struct RollupGaugeAcc\b"), _cut(enc, r"struct RollupCounterAcc\b")]
+        parts.append(cut(enc, fn(name)))
+    parts += [cut(enc, r"struct RollupGaugeAcc\b"), cut(enc, r"struct RollupCounterAcc\b")]
     for name in ("rollup_gauge_init", "rollup_counter_init", "rollup_add", "rollup_gauge_add", "rollup_counter_add"):
-        parts.append(_cut(enc, _fn(name)))
-    body = "\n".join(parts)
-    assert "asm" not in body, "a PTX block slipped into the host build"
-    d = tempfile.mkdtemp(prefix="m3dev_rollup_host_")
-    path = os.path.join(d, "dev_rollup_host.cpp")
-    open(path, "w").write(SHIM + body + DRIVER)
-    so = os.path.join(d, "dev_rollup_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
+        parts.append(cut(enc, fn(name)))
+    lib = compile("dev_rollup_host", "\n".join(parts), DRIVER)
     vp = C.c_void_p
     lib.dev_fold_gauge.restype = None
     lib.dev_fold_gauge.argtypes = [vp, C.c_size_t, vp, vp]

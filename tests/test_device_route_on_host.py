@@ -11,25 +11,13 @@ out-of-order writes, duplicates, upserts, annotations, unit changes, delta-of-de
 encoder limit and t == 0.  The append must take every datapoint the route sends it.  A CPU regression harness for
 the device source; nothing of it ships."""
 import ctypes as C
-import os
-import re
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import oracle_lib as O
 from bucket_model import ERR_CAPACITY, SEC, Bucket, random_calls
-from test_device_append_on_host import DRIVER as APPEND_DRIVER
-from test_device_encoder_on_host import CSRC, EMIT, ROOT, SHIM, _cut, _fn
-
-ERRS = """enum { M3TSZ_OK = 0, M3TSZ_ERR_NO_DATAPOINTS = 3, M3TSZ_ERR_TOO_MANY_ENCODERS = 16,
-       M3TSZ_ERR_CAPACITY = 100, M3TSZ_ERR_INVALID_ARG = 101 };
-#define M3TSZ_MAX_BUCKET_ENCODERS 12
-static inline uint32_t atomicAdd(uint32_t *a, uint32_t v) { const uint32_t o = *a; *a += v; return o; }
-static inline uint32_t atomicSub(uint32_t *a, uint32_t v) { const uint32_t o = *a; *a -= v; return o; }
-"""
+from host_build import build_dev_append, constants, cut, fn, source_text
 
 ROUTE_DRIVER = r"""
 // one call of one bucket (series 0 of a one-series batch, series-major)
@@ -77,52 +65,13 @@ extern "C" int dev_route(int int_opt, m3tsz_encoder_state *state, uint64_t slot_
 
 @pytest.fixture(scope="module")
 def dev():
-    enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
-    com = open(os.path.join(CSRC, "m3tsz_common.cuh")).read()
-    kh = open(os.path.join(CSRC, "m3tsz_kernels.h")).read()
-    hdr = open(os.path.join(ROOT, "include", "m3tsz_b200.h")).read()
-    state = re.search(r"typedef struct m3tsz_encoder_state \{.*?\} m3tsz_encoder_state;", hdr, flags=re.S).group(0)
-    entry = re.search(r"typedef struct m3tsz_annotation_entry \{.*?\} m3tsz_annotation_entry;", hdr,
-                      flags=re.S).group(0)
-    consts = "\n".join(re.findall(r"^constexpr [^\n]*\bk(?:Marker|MaxMult)[^\n]*$", com, flags=re.M))
-    guard = re.search(r"^constexpr int ENC_GUARD = \d+;", enc, flags=re.M).group(0)
-    parts = [ERRS, state, entry, guard, consts, _cut(kh, r"struct RouteTouched(?= \{)"),
-             _cut(kh, r"struct RouteParams(?= \{)"), _cut(com, r"enum SchemeKind"),
-             _cut(com, r"__host__ __device__[^\n{;]*\bunit_is_valid\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\bunit_nanos\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\bscheme_kind_for_unit\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\binitial_time_unit\s*\("),
-             _cut(com, r"__host__ __device__[^\n{;]*\bxxh64\s*\("),
-             _cut(com, _fn("num_sig")), _cut(com, _fn("mult_pow10")),
-             _cut(enc, r"struct EncLane"), _cut(enc, _fn("put32")), _cut(enc, _fn("put64")), EMIT,
-             _cut(enc, _fn("emit_code"))]
-    for name in ("maybe_int", "go_f64_to_u64_via_i64", "convert_to_int_float", "track_new_sig", "sig_mult_hdr",
-                 "xor_code", "encode_value", "encode_time"):
-        parts.append(_cut(enc, _fn(name)))
-    parts += [_cut(enc, r"struct Tier2"), _cut(enc, _fn("div_unit")), _cut(enc, _fn("tier2_candidate")),
-              _cut(enc, _fn("tier2_commit")), _cut(enc, r"struct EncStateInternal")]
-    for name in ("enc_state_tag", "enc_state_reset", "enc_state_load", "enc_state_save", "enc_check_time",
-                 "enc_snapshot_words"):
-        parts.append(_cut(enc, _fn(name)))
-    parts += [_cut(enc, r"struct RouteEnc(?= \{)")]
+    enc, kh = source_text("m3tsz_encode.cu"), source_text("m3tsz_kernels.h")
+    parts = [constants(enc, "ENC_GUARD"), cut(kh, r"struct RouteTouched(?= \{)"), cut(kh, r"struct RouteParams(?= \{)"),
+             cut(enc, r"struct RouteEnc(?= \{)")]
     for name in ("route_enc_load", "route_at", "route_last_value", "route_series"):
-        parts.append(_cut(enc, _fn(name)))
-    body = "\n".join(parts)
-    assert "asm" not in body, "a PTX block slipped into the host build"
-    d = tempfile.mkdtemp(prefix="m3dev_route_host_")
-    path = os.path.join(d, "dev_route_host.cpp")
-    open(path, "w").write(SHIM + body + APPEND_DRIVER + ROUTE_DRIVER)
-    so = os.path.join(d, "dev_route_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
+        parts.append(cut(enc, fn(name)))
+    lib = build_dev_append("dev_route_host", "\n".join(parts), ROUTE_DRIVER)
     vp = C.c_void_p
-    lib.dev_append.restype = C.c_longlong
-    lib.dev_append.argtypes = [vp, vp, vp, vp, vp, C.c_int, C.c_size_t, vp, vp, vp, C.c_int, C.c_int,
-                               C.POINTER(C.c_int)]
-    lib.dev_reset.restype = None
-    lib.dev_reset.argtypes = [vp, C.c_int64, C.c_int, C.c_int]
-    lib.dev_snapshot.restype = C.c_uint64
-    lib.dev_snapshot.argtypes = [vp, vp]
     lib.dev_route.restype = C.c_int
     lib.dev_route.argtypes = [C.c_int, vp, C.c_uint64, vp, C.c_uint64, C.c_uint64, vp, vp, C.c_int, vp, vp,
                               C.c_uint64, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp]

@@ -1,41 +1,19 @@
 """The value classifier the encode kernel runs -- `maybe_int`, `go_f64_to_u64_via_i64`, `convert_to_int_float`
 (m3_b200/csrc/m3tsz_encode.cu) and `mult_pow10` (m3tsz_common.cuh) -- compiled FOR THE HOST from the device source
 text itself (the function bodies are cut out of the .cu files at test time; CUDA's round-to-nearest intrinsics are
-mapped onto the IEEE operations they are, the build uses -ffp-contract=off like the kernels' -fmad=false) and
+mapped onto the IEEE operations they are, the build contracts no FMA, like the kernels' -fmad=false) and
 compared with the oracle's convertToIntFloat: same (value bits, multiplier, isFloat) for every current multiplier
 on the reference's families, ulp neighbourhoods of decimals, random bit patterns and the special values.  This is a
 CPU check of the DEVICE code's arithmetic, not a CPU path of the product: the shared object it builds lives in a
 temporary directory and only this test loads it."""
 import ctypes as C
-import os
 import random
-import re
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import oracle_lib as O
-
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-CSRC = os.path.join(ROOT, "m3_b200", "csrc")
-
-SHIM = r"""
-#include <cmath>
-#include <cstdint>
-#include <cstring>
-#define __device__
-#define __forceinline__ inline
-#define __noinline__
-constexpr int kMaxMult = 6;
-static inline double __dmul_rn(double a, double b) { return a * b; }
-static inline double __dsub_rn(double a, double b) { return a - b; }
-static inline double __dadd_rn(double a, double b) { return a + b; }
-static inline long long __double2ll_rz(double a) { return (long long)a; }
-static inline long long __double_as_longlong(double a) { long long r; memcpy(&r, &a, 8); return r; }
-static inline double __longlong_as_double(long long a) { double r; memcpy(&r, &a, 8); return r; }
-"""
+from host_build import compile, constants, cut, fn, source_text
 
 EXPORTS = r"""
 extern "C" {
@@ -50,34 +28,13 @@ void dev_convert(double v, int cur, double *val, int *mult, int *is_float) {
 """
 
 
-def _cut_function(src, name):
-    m = re.search(r"__device__[^\n;{]*\b%s\s*\(" % re.escape(name), src)
-    assert m, name
-    i = src.index("{", m.end())
-    depth = 0
-    for j in range(i, len(src)):
-        if src[j] == "{":
-            depth += 1
-        elif src[j] == "}":
-            depth -= 1
-            if depth == 0:
-                return src[m.start(): j + 1]
-    raise AssertionError(name)
-
-
 @pytest.fixture(scope="module")
 def dev():
-    enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
-    com = open(os.path.join(CSRC, "m3tsz_common.cuh")).read()
-    body = "\n".join([_cut_function(com, "mult_pow10"), _cut_function(enc, "maybe_int"),
-                      _cut_function(enc, "go_f64_to_u64_via_i64"), _cut_function(enc, "convert_to_int_float")])
+    enc, com = source_text("m3tsz_encode.cu"), source_text("m3tsz_common.cuh")
+    body = "\n".join([constants(com, "kMaxMult"), cut(com, fn("mult_pow10")), cut(enc, fn("maybe_int")),
+                      cut(enc, fn("go_f64_to_u64_via_i64")), cut(enc, fn("convert_to_int_float"))])
     assert "__dmul_rn" in body and "trunc(" in body  # still the separately rounded form
-    d = tempfile.mkdtemp(prefix="m3dev_host_")
-    path = os.path.join(d, "dev_host.cpp")
-    open(path, "w").write(SHIM + body + EXPORTS)
-    so = os.path.join(d, "dev_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", path, "-o", so])
-    lib = C.CDLL(so)
+    lib = compile("dev_host", body, EXPORTS)
     lib.dev_maybe_int.restype, lib.dev_maybe_int.argtypes = C.c_int, [C.c_double]
     lib.dev_f64_to_u64.restype, lib.dev_f64_to_u64.argtypes = C.c_uint64, [C.c_double]
     lib.dev_convert.restype = None

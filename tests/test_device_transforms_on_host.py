@@ -6,22 +6,13 @@ timestamp is 0) and must equal the oracle (tests/xf_oracle.c) bit for bit, state
 the random sequences of test_independent_transforms.py, calls split at random.  A CPU regression harness for the
 device source; nothing of it ships."""
 import ctypes as C
-import os
-import re
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import xf_oracle_lib as X
-from test_device_encoder_on_host import CSRC, ROOT, SHIM, _cut, _fn
+from host_build import compile, constants, cut, fn, source_text
 from test_independent_transforms import _goldens, _oracle_state, _splits, _val, random_pipeline, random_windows
-
-EXTRA = r"""
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline double __ll2double_rn(long long a) { return (double)a; }
-"""
 
 DRIVER = r"""
 // the kernel's IN = 4 rows for n non-empty windows of one series: the window's datapoint unless a discarded NaN,
@@ -51,24 +42,11 @@ extern "C" size_t dev_transform_series(const int32_t *ops, size_t n_ops, int dis
 
 @pytest.fixture(scope="module")
 def dev():
-    enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
-    hdr = open(os.path.join(ROOT, "include", "m3tsz_b200.h")).read()
-    ids = re.search(r"enum \{ /\* transformation\.Type ids.*?\};", hdr, flags=re.S).group(0)
-    maxk = re.search(r"^#define M3TSZ_MAX_TRANSFORMS \d+$", hdr, flags=re.M).group(0)
-    state = re.search(r"typedef struct m3tsz_transform_state \{.*?\} m3tsz_transform_state;", hdr,
-                      flags=re.S).group(0)
-    consts = "\n".join(re.findall(r"^constexpr uint64_t kXf[^\n]*$", enc, flags=re.M))
-    parts = [EXTRA, ids, maxk, state, consts]
+    enc = source_text("m3tsz_encode.cu")
+    parts = [constants(enc, r"kXf\w*")]
     for name in ("xf_isnan", "xf_bits", "xf_per_second", "xf_increase", "xf_window"):
-        parts.append(_cut(enc, _fn(name)))
-    body = "\n".join(parts)
-    assert "asm" not in body, "a PTX block slipped into the host build"
-    d = tempfile.mkdtemp(prefix="m3dev_xf_host_")
-    path = os.path.join(d, "dev_xf_host.cpp")
-    open(path, "w").write(SHIM + body + DRIVER)
-    so = os.path.join(d, "dev_xf_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
+        parts.append(cut(enc, fn(name)))
+    lib = compile("dev_xf_host", "\n".join(parts), DRIVER)
     vp = C.c_void_p
     lib.dev_transform_series.restype = C.c_size_t
     lib.dev_transform_series.argtypes = [vp, C.c_size_t, C.c_int, C.c_int64, vp, vp, vp, C.c_size_t, vp, vp]

@@ -18,8 +18,7 @@ import pytest
 import grammar_edges as G
 import indep_m3tsz as I
 import oracle_lib as O
-from test_device_decoder_on_host import DevDecode, build_dev_decoder
-from test_device_encoder_on_host import build_dev_encoder
+from host_build import DevDecode, build_dev_decoder, build_dev_encoder
 
 LANES = (0, 1)  # lane 1 negates the int series
 

@@ -8,21 +8,18 @@ import ctypes as C
 import json
 import math
 import os
-import re
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
 import agg_oracle_lib as A
 import oracle_lib as O
+from host_build import compile, cut, fn, source_text
 
 SEC = 1_000_000_000
 M64 = (1 << 64) - 1
 HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(HERE, "..", "m3_b200", "csrc")
 AMD64_NAN = 0xFFF8000000000000  # the invalid-operation NaN of SSE2 (Inf - Inf, sqrt(-x))
 
 
@@ -242,21 +239,6 @@ def test_tiles_every_valid_pair_match_restatement_and_independent_encoder(metric
 
 
 # ---- the device functions, compiled for the host ----
-SHIM = r"""
-#include <cmath>
-#include <cstdint>
-#include <cstring>
-#define __device__
-#define __forceinline__ inline
-static inline double __dmul_rn(double a, double b) { return a * b; }
-static inline double __dsub_rn(double a, double b) { return a - b; }
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline double __dsqrt_rn(double a) { return std::sqrt(a); }
-static inline double __ll2double_rn(long long a) { return (double)a; }
-static inline long long __double2ll_rz(double a) { return (long long)a; }
-static inline double __longlong_as_double(long long a) { double r; memcpy(&r, &a, 8); return r; }
-"""
-
 EXPORTS = r"""
 extern "C" {
 int64_t dev_i64(double v) { return go_f64_to_i64(v); }
@@ -266,27 +248,10 @@ double dev_stdev(int64_t c, double sq, double s) { return agg_stdev(c, sq, s); }
 """
 
 
-def _cut(src, name):
-    m = re.search(r"__device__[^\n;{]*\b%s\s*\(" % re.escape(name), src)
-    assert m, name
-    i, depth = src.index("{", m.end()), 0
-    for j in range(i, len(src)):
-        depth += {"{": 1, "}": -1}.get(src[j], 0)
-        if depth == 0:
-            return src[m.start(): j + 1]
-    raise AssertionError(name)
-
-
 def test_device_conversion_and_stdev_on_host():
-    com = open(os.path.join(CSRC, "m3tsz_common.cuh")).read()
-    enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
-    body = "\n".join([_cut(com, "go_f64_to_i64"), _cut(enc, "go_f64_to_u64_via_i64"), _cut(com, "agg_stdev")])
-    d = tempfile.mkdtemp(prefix="m3agg_host_")
-    path = os.path.join(d, "agg_host.cpp")
-    open(path, "w").write(SHIM + body + EXPORTS)
-    so = os.path.join(d, "agg_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", path, "-o", so])
-    L = C.CDLL(so)
+    com, enc = source_text("m3tsz_common.cuh"), source_text("m3tsz_encode.cu")
+    body = "\n".join([cut(com, fn("go_f64_to_i64")), cut(enc, fn("go_f64_to_u64_via_i64")), cut(com, fn("agg_stdev"))])
+    L = compile("agg_host", body, EXPORTS)
     L.dev_i64.restype, L.dev_i64.argtypes = C.c_int64, [C.c_double]
     L.dev_u64.restype, L.dev_u64.argtypes = C.c_uint64, [C.c_double]
     L.dev_stdev.restype, L.dev_stdev.argtypes = C.c_double, [C.c_int64, C.c_double, C.c_double]

@@ -8,10 +8,6 @@ the annotated forward stage's reference conversion and 2^27 check and the fold's
 host from the .cu source text."""
 import ctypes as C
 import math
-import os
-import re
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -24,7 +20,7 @@ import oracle_lib as O
 import rollup_ann_oracle_lib as RA
 import rollup_oracle_lib as R
 import xf_oracle_lib as X
-from test_device_encoder_on_host import CSRC, SHIM, _cut, _fn
+from host_build import compile, constants, cut, fn, source_text
 from test_independent_rollup import fold_counter, fold_gauge
 
 SEC = 10 ** 9
@@ -206,17 +202,10 @@ extern "C" uint64_t dev_ann_fold(const uint32_t *ann_bits, const uint64_t *refs,
 
 @pytest.fixture(scope="module")
 def dev():
-    enc = open(os.path.join(CSRC, "m3tsz_encode.cu")).read()
-    hdr = open(os.path.join(CSRC, "m3tsz_kernels.h")).read()
-    consts = re.search(r"^constexpr int kBlockAnnLenBits = \d+;$", hdr, flags=re.M).group(0)
-    body = "\n".join([consts, _cut(enc, _fn("rollup_ann_ref")), _cut(enc, _fn("rollup_ann_add"))])
-    assert "asm" not in body
-    d = tempfile.mkdtemp(prefix="m3dev_rollup_ann_host_")
-    path = os.path.join(d, "dev_rollup_ann_host.cpp")
-    open(path, "w").write(SHIM + body + DRIVER)
-    so = os.path.join(d, "dev_rollup_ann_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-w", path, "-o", so])
-    lib = C.CDLL(so)
+    enc = source_text("m3tsz_encode.cu")
+    body = "\n".join([constants(source_text("m3tsz_kernels.h"), "kBlockAnnLenBits"), cut(enc, fn("rollup_ann_ref")),
+                      cut(enc, fn("rollup_ann_add"))])
+    lib = compile("dev_rollup_ann_host", body, DRIVER)
     vp = C.c_void_p
     lib.dev_ann_ref.restype = C.c_int
     lib.dev_ann_ref.argtypes = [C.c_uint64, vp, C.c_uint64, vp]

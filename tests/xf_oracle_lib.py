@@ -1,33 +1,20 @@
 """ctypes binding of the transformation oracle (tests/xf_oracle.c -> tests/libm3tsz_xf_oracle.so): what the
 aggregator's transformations do to a flushed window's value, src/metrics/transformation and GenericElem.processValue.
 Test infrastructure only, like agg_oracle_lib.py; __graft_entry__.build() compiles the library, and
-build_xf_oracle() rebuilds it when the source is newer.  The tile path (decode -> downsample -> ValueOf ->
+build_c_oracle() rebuilds it when the source is newer.  The tile path (decode -> downsample -> ValueOf ->
 transformations) composes this oracle with the aggregation oracle (agg_oracle_lib.aggregate_tiles_series_ex)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 import agg_oracle_lib as A
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = os.path.join(_HERE, "xf_oracle.c")
-LIB_PATH = os.path.join(_HERE, "libm3tsz_xf_oracle.so")
-CFLAGS = ["-O2", "-g", "-fPIC", "-std=c11", "-Wall", "-Wextra", "-ffp-contract=off", "-fno-strict-aliasing"]
+from host_build import build_c_oracle
 
 XF_ABSOLUTE, XF_PERSECOND, XF_INCREASE, XF_ADD, XF_RESET = 1, 2, 3, 4, 5  # transformation.Type ids
 # m3tsz_transform_state: has_prev, reserved, prev_t, prev_v, sum[8], reserved (96 bytes)
 XF_STATE_DTYPE = np.dtype([("has_prev", "<i4"), ("reserved0", "<i4"), ("prev_t", "<i8"), ("prev_v", "<f8"),
                            ("sum", "<f8", (8,)), ("reserved1", "<u8")])
 assert XF_STATE_DTYPE.itemsize == 96
-
-
-def build_xf_oracle(force=False):
-    if not force and os.path.exists(LIB_PATH) and os.path.getmtime(LIB_PATH) >= os.path.getmtime(SRC):
-        return LIB_PATH
-    subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", "-o", LIB_PATH, SRC, "-lm"])
-    return LIB_PATH
 
 
 def _ptr(a):
@@ -40,7 +27,7 @@ _lib = None
 def _xf_lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(build_xf_oracle())
+        L = C.CDLL(build_c_oracle("xf"))
         vp = C.c_void_p
         L.m3o_transform_series.restype = C.c_size_t
         L.m3o_transform_series.argtypes = [vp, C.c_size_t, C.c_int, C.c_int64, vp, vp, vp, C.c_size_t, vp, vp]
