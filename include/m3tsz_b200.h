@@ -69,6 +69,7 @@ enum {
   M3TSZ_ERR_TOO_MANY_ITERATORS = 14, /* > 12 replicas per series or readers per block slice */
   M3TSZ_ERR_CHECKSUM_MISMATCH = 15, /* errSeekChecksumMismatch, persist/fs/seek.go:50-51, read.go:395-397 */
   M3TSZ_ERR_TOO_MANY_ENCODERS = 16, /* errTooManyEncoders, storage/series/buffer.go:57 */
+  M3TSZ_ERR_AGGREGATION_CLOSED = 17, /* errAggregationClosed, aggregator/elem_base.go:72 */
   /* library-level conditions */
   M3TSZ_ERR_CAPACITY = 100,        /* more datapoints / bytes than the caller's buffer holds */
   M3TSZ_ERR_INVALID_ARG = 101,
@@ -922,6 +923,85 @@ int m3tsz_aggregate_tiles_rollup_annotated(
     m3tsz_element_state *d_group_state, int32_t out_unit, uint32_t align, uint8_t *d_packed, uint64_t packed_capacity,
     uint64_t *d_out_offsets, uint64_t *d_out_len, int32_t *d_status, uint32_t *d_n_tiles, uint64_t *d_total_bytes,
     int32_t *d_src_status, void *stream);
+
+/* ------------------------------------------------------------------------
+ * Element sets: the aggregator's elements fed datapoint by datapoint (DESIGN.md §4.12).  GenericElem.AddUnion /
+ * AddValue add a datapoint to the open window it falls in (src/aggregator/aggregator/generic_elem.go:193-240);
+ * Consume(target) flushes every window whose end is at or before target, in order, through ValueOf of each aggregation
+ * type and the transformations, at the window's end (generic_elem.go:291-358, 804-950, list.go:531-543).  A set is
+ * n_elements Gauge or Counter elements with one resolution, one type list and one transformation list.
+ *
+ * The caller owns every array (device memory):
+ *   - open windows: n_windows (R) slots per element, window-slot-major [R][n_elements] (slot r of element s at
+ *     r * n_elements + s), 8-byte aligned: the window start, its datapoint count (0: the slot is free) and the
+ *     aggregates the fused decode keeps: Gauge sum, min, max, sumSq (float64), last (float64) and lastAt (int64 ns);
+ *     Counter sum, min, max, sumSq (int64; d_win_last / d_win_last_at unused, may be NULL);
+ *   - d_elem: one m3tsz_element_state per element (the record the tile calls carry), 16-byte aligned;
+ *   - d_watermark: one int64 per element, the end of the last window consumed (INT64_MIN: none yet);
+ *   - the output: an encoder set (m3tsz_encoder_set_*) of n_types * n_elements records, row j * n_elements + s
+ *     being element s under agg_types[j] (as m3tsz_aggregate_tiles_types numbers its rows); stream / grow / the
+ *     accessors work on it unchanged.
+ * agg_types (1 .. M3TSZ_MAX_ELEMENT_TYPES, strictly ascending, valid for metric_type) and ops / discard_nan are
+ * checked and applied as in m3tsz_aggregate_tiles_types.  Every call checks all of its arguments on the host before
+ * any launch (M3TSZ_ERR_INVALID_ARG).  Resetting or growing is a copy of these arrays: they hold no pointers.
+ * ---------------------------------------------------------------------- */
+#define M3TSZ_MAX_ELEMENT_WINDOWS 64
+typedef struct m3tsz_element_set {
+  uint64_t n_elements;
+  uint32_t n_windows;       /* R: open-window slots per element, 1 .. M3TSZ_MAX_ELEMENT_WINDOWS */
+  int32_t metric_type;      /* M3TSZ_METRIC_GAUGE or M3TSZ_METRIC_COUNTER */
+  int64_t resolution_ns;    /* > 0 */
+  const int32_t *agg_types; /* host */
+  uint32_t n_types;
+  uint32_t n_ops;
+  const int32_t *ops;       /* host */
+  int32_t discard_nan;
+  int32_t reserved;         /* 0 */
+  int64_t *d_win_start, *d_win_count;
+  void *d_win_sum, *d_win_min, *d_win_max, *d_win_sum_sq;
+  double *d_win_last;
+  int64_t *d_win_last_at;
+  m3tsz_element_state *d_elem;
+  int64_t *d_watermark;
+  m3tsz_encoder_state *d_out_state;
+  uint8_t *d_out_buf;
+  uint64_t out_stride;      /* bytes per output slot, a multiple of 16 */
+} m3tsz_element_set;
+
+/* Frees every window, zeroes every record, sets every watermark to INT64_MIN, and resets the output encoder set with
+ * d_start [n_elements] (element s's start for all of its rows). */
+int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                            const int64_t *d_start, void *stream);
+
+/* Adds datapoints to the elements' open windows, point-major d_ts / d_val [points_stride][n_elements]: element s
+ * takes d_n_points[s] (NULL: points_stride) of them, in row order.  Per datapoint, in that order:
+ *   - its window starts at t.Truncate(resolution_ns), Go's time.Time truncation (from the zero time, so negative times
+ *     round down);
+ *   - a window whose end is at or before the element's watermark is closed: M3TSZ_ERR_AGGREGATION_CLOSED, nothing
+ *     changes (the reference closes only the last window it consumed, DESIGN.md §6);
+ *   - else the datapoint updates its open window, or opens one: Gauge.Update / Counter.Update as the fused decode
+ *     runs them (gauge.go:74-106, counter.go:52-78);
+ *   - a new window with all R slots open is M3TSZ_ERR_CAPACITY for that datapoint and every later one of the element
+ *     in this call: nothing of them is added, so adding exactly those again after growing R gives the unstopped
+ *     result.
+ * d_result (int8, [points_stride][n_elements]): 0 added, else the status above (M3TSZ_ERR_INVALID_ARG for a time
+ * whose window start lies below INT64_MIN); rows past the element's count are not written.  d_status [n_elements]:
+ * M3TSZ_OK, M3TSZ_ERR_CAPACITY, or M3TSZ_ERR_INVALID_ARG (n_points > points_stride: the element is untouched). */
+int m3tsz_element_set_add(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                          const int64_t *d_ts, const double *d_val, uint64_t points_stride,
+                          const uint32_t *d_n_points, int8_t *d_result, int32_t *d_status, void *stream);
+
+/* Consume(target_ns) of every element: the open windows whose end is at or before target_ns, in ascending start
+ * order, each as one window of m3tsz_aggregate_tiles_types: every type's ValueOf, the transformations on the element
+ * record, the NaN discard and the Reset datapoint, appended to the type's output row at the window's end with unit
+ * out_unit (as m3tsz_encoder_set_append).  The flushed slots are freed and the watermark moves to the last one's end.
+ * d_status [n_elements]: M3TSZ_OK; M3TSZ_ERR_CAPACITY when a row's slot lacks room for the flush with every datapoint
+ * at its worst case (the append's bound: a slot of m3tsz_encode_bound_units(P, 1) bytes takes P datapoints) -- the element
+ * then keeps its windows, record and watermark and nothing is appended, so consuming again after growing the output
+ * gives the unstopped result; else the first failing row's append status (the element is consumed, and that row
+ * stops as m3tsz_encoder_set_append stops a series). */
+int m3tsz_element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                              int64_t target_ns, int32_t out_unit, int32_t *d_status, void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

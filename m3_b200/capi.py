@@ -20,6 +20,7 @@ ERR_INVALID_MULT = 7
 ERR_OUT_OF_ORDER = 13
 ERR_TOO_MANY_ITERATORS = 14
 ERR_TOO_MANY_ENCODERS = 16
+ERR_AGGREGATION_CLOSED = 17
 ERR_CAPACITY = 100
 ERR_INVALID_ARG = 101
 ERR_CUDA = 102
@@ -34,6 +35,7 @@ MAX_TRANSFORMS = 8  # M3TSZ_MAX_TRANSFORMS
 TRANSFORM_STATE_BYTES = 96  # sizeof(m3tsz_transform_state)
 MAX_ELEMENT_TYPES = 8  # M3TSZ_MAX_ELEMENT_TYPES (m3tsz_aggregate_tiles_types)
 ELEMENT_STATE_BYTES = 160  # sizeof(m3tsz_element_state)
+MAX_ELEMENT_WINDOWS = 64  # M3TSZ_MAX_ELEMENT_WINDOWS (element sets)
 
 UNIT_NONE, UNIT_S, UNIT_MS, UNIT_US, UNIT_NS, UNIT_MIN, UNIT_HOUR, UNIT_DAY, UNIT_YEAR = range(9)
 
@@ -55,6 +57,17 @@ class DpEvent(C.Structure):
 
 
 EVENT_TIME_UNIT, EVENT_ANNOTATION = 1, 2
+
+
+class ElementSet(C.Structure):
+    """m3tsz_element_set: an element set's settings (host lists) and its device arrays (include/m3tsz_b200.h)."""
+    _fields_ = [("n_elements", C.c_uint64), ("n_windows", C.c_uint32), ("metric_type", C.c_int32),
+                ("resolution_ns", C.c_int64), ("agg_types", C.POINTER(C.c_int32)), ("n_types", C.c_uint32),
+                ("n_ops", C.c_uint32), ("ops", C.POINTER(C.c_int32)), ("discard_nan", C.c_int32),
+                ("reserved", C.c_int32)] + [(f, C.c_void_p) for f in (
+                    "d_win_start", "d_win_count", "d_win_sum", "d_win_min", "d_win_max", "d_win_sum_sq", "d_win_last",
+                    "d_win_last_at", "d_elem", "d_watermark", "d_out_state", "d_out_buf")] + [
+                ("out_stride", C.c_uint64)]
 
 
 class DecodeExtras(C.Structure):
@@ -115,6 +128,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_decode_downsample_ex", "m3tsz_aggregate_tiles_ex", "m3tsz_encoder_set_write",
     "m3tsz_aggregate_tiles_transform", "m3tsz_aggregate_tiles_types", "m3tsz_aggregate_tiles_annotated",
     "m3tsz_aggregate_tiles_blocks", "m3tsz_aggregate_tiles_rollup", "m3tsz_aggregate_tiles_rollup_annotated",
+    "m3tsz_element_set_reset", "m3tsz_element_set_add", "m3tsz_element_set_consume",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -296,6 +310,13 @@ def lib():
                                                i32, u32, vp, u64, vp, vp, vp, vp, vp, vp, vp]
     L.m3tsz_aggregate_tiles_rollup_annotated.restype = C.c_int
     L.m3tsz_aggregate_tiles_rollup_annotated.argtypes = L.m3tsz_aggregate_tiles_rollup.argtypes
+    pes = C.POINTER(ElementSet)
+    L.m3tsz_element_set_reset.restype = C.c_int
+    L.m3tsz_element_set_reset.argtypes = [vp, po, pes, vp, vp]
+    L.m3tsz_element_set_add.restype = C.c_int
+    L.m3tsz_element_set_add.argtypes = [vp, po, pes, vp, vp, u64, vp, vp, vp, vp]
+    L.m3tsz_element_set_consume.restype = C.c_int
+    L.m3tsz_element_set_consume.argtypes = [vp, po, pes, i64, i32, vp, vp]
     _lib = L
     return L
 

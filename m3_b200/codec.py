@@ -287,6 +287,18 @@ class BatchCodec:
         bytes (a multiple of 16): the write path's encoders, appended to over many calls."""
         return EncoderSet(self, start, stride)
 
+    def element_set(self, start: torch.Tensor, metric_type, agg_types, resolution_ns, transforms=(),
+                    discard_nan=False, open_windows=4, stride: Optional[int] = None,
+                    out_unit=capi.UNIT_S) -> "ElementSet":
+        """N aggregator elements fed datapoint by datapoint (m3tsz_element_set_*, N = start.numel(), start int64
+        [N] ns): one metric type (capi.METRIC_GAUGE / METRIC_COUNTER), resolution, strictly ascending list of
+        aggregation types and transformation list, checked and applied as in aggregate_tiles_types (discard_nan
+        only with transformations).  Each element keeps up to `open_windows` open windows; its flushed windows go to
+        an encoder set of k * N rows (row j * N + s: element s under agg_types[j]) with slots of `stride` bytes
+        (default: room for 128 datapoints per row at their worst case), written with `out_unit`."""
+        return ElementSet(self, start, metric_type, agg_types, resolution_ns, transforms, discard_nan, open_windows,
+                          stride, out_unit)
+
     def bucket_set(self, start: torch.Tensor, stride: int, encoders=4, pool_records: Optional[int] = None,
                    pool_stride: Optional[int] = None) -> "BucketSet":
         """S buffer buckets (BufferBucket.write, m3tsz_encoder_set_write): encoder 0 of bucket s is an encoder set
@@ -848,3 +860,134 @@ class BucketSet:
         return self.codec.merge_series(ts[seq].contiguous(), vals[seq].contiguous(), npts[seq].contiguous(),
                                        st[seq].contiguous(), slice_off, ident, ident, out_cap, start_ns, end_ns,
                                        strategy=0)
+
+
+class ElementSet:
+    """Aggregator elements on the device (m3tsz_element_set_*, DESIGN.md §4.12).  The caller-side arrays: `win`, the
+    open-window slots window-slot-major [R, N] (start, count -- 0 for a free slot -- sum, min, max, sum_sq, and for
+    the Gauge last / last_at; a Counter's aggregates are int64), `elem` uint8 [N, 160] (m3tsz_element_state),
+    `watermark` int64 [N] (the end of the last window consumed, INT64_MIN for none) and `out`, the EncoderSet the
+    flushed windows are appended to.  add() puts datapoints into open windows, consume() flushes the windows that
+    ended by a target time."""
+
+    def __init__(self, codec: BatchCodec, start: torch.Tensor, metric_type, agg_types, resolution_ns, transforms,
+                 discard_nan, open_windows, stride, out_unit):
+        assert start.dtype == torch.int64 and start.is_cuda
+        self.codec = codec
+        self.metric_type = int(metric_type)
+        self.agg_types = [int(t) for t in agg_types]
+        self.transforms = [int(t) for t in transforms]
+        self.discard_nan = bool(discard_nan)
+        self.resolution_ns = int(resolution_ns)
+        self.out_unit = int(out_unit)
+        self.n_elements = start.numel()
+        k, N, R = len(self.agg_types), self.n_elements, int(open_windows)
+        assert k >= 1 and R >= 1
+        self._types = (C.c_int32 * k)(*self.agg_types)
+        self._ops = (C.c_int32 * max(1, len(self.transforms)))(*self.transforms)
+        dev = codec.device
+        counter = self.metric_type == capi.METRIC_COUNTER
+        agg = torch.int64 if counter else torch.float64
+        names = [("start", torch.int64), ("count", torch.int64), ("sum", agg), ("min", agg), ("max", agg),
+                 ("sum_sq", agg)] + ([] if counter else [("last", torch.float64), ("last_at", torch.int64)])
+        self.win = {f: torch.zeros((R, N), dtype=t, device=dev) for f, t in names}
+        self.elem = torch.zeros((N, capi.ELEMENT_STATE_BYTES), dtype=torch.uint8, device=dev)
+        self.watermark = torch.empty(N, dtype=torch.int64, device=dev)
+        if stride is None:
+            stride = int(capi.lib().m3tsz_encode_bound_units(128, 1))
+        start = start.contiguous()
+        self.out = EncoderSet(codec, start.repeat(k), stride)
+        self.reset(start)
+
+    @property
+    def open_windows(self) -> int:
+        return self.win["start"].shape[0]
+
+    def _desc(self):
+        w = self.win
+        d = capi.ElementSet()
+        d.n_elements = self.n_elements
+        d.n_windows = self.open_windows
+        d.metric_type = self.metric_type
+        d.resolution_ns = self.resolution_ns
+        d.agg_types = C.cast(self._types, C.POINTER(C.c_int32))
+        d.n_types = len(self.agg_types)
+        d.n_ops = len(self.transforms)
+        d.ops = C.cast(self._ops, C.POINTER(C.c_int32))
+        d.discard_nan = 1 if self.discard_nan else 0
+        for f in ("start", "count", "sum", "min", "max", "sum_sq", "last", "last_at"):
+            setattr(d, "d_win_" + f, w[f].data_ptr() if f in w else None)
+        d.d_elem = self.elem.data_ptr()
+        d.d_watermark = self.watermark.data_ptr()
+        d.d_out_state = self.out.state.data_ptr()
+        d.d_out_buf = self.out.buf.data_ptr()
+        d.out_stride = self.out.stride
+        return d
+
+    def reset(self, start: torch.Tensor):
+        """Every element new: windows free, records zero, nothing consumed, output rows Reset(start[s])."""
+        assert start.dtype == torch.int64 and start.is_cuda and start.numel() == self.n_elements
+        start = start.contiguous()
+        d = self._desc()
+        rc = capi.lib().m3tsz_element_set_reset(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
+                                                _ptr(start), _cuda_stream_ptr(self.codec.device))
+        self.codec.ctx.check(rc, "m3tsz_element_set_reset")
+
+    def add(self, ts: torch.Tensor, values: torch.Tensor, n_points: Optional[torch.Tensor] = None):
+        """AddUnion of point-major ts / values int64 / float64 [P, N]: element s takes n_points[s] (int32 [N]; all P
+        when None) of its column, in order.  Returns (result int8 [P, N]: 0 added, else ERR_AGGREGATION_CLOSED /
+        ERR_CAPACITY / ERR_INVALID_ARG, rows past an element's count left 0; status int32 [N]: OK, ERR_CAPACITY --
+        that datapoint and the element's later ones were not added: grow() and add them again -- or
+        ERR_INVALID_ARG)."""
+        assert ts.dtype == torch.int64 and values.dtype == torch.float64 and ts.shape == values.shape
+        assert ts.is_cuda and values.is_cuda and ts.is_contiguous() and values.is_contiguous()
+        assert ts.dim() == 2 and ts.shape[1] == self.n_elements
+        if n_points is not None:
+            assert n_points.dtype == torch.int32 and n_points.is_cuda and n_points.is_contiguous()
+            assert n_points.numel() == self.n_elements
+        dev = self.codec.device
+        P = ts.shape[0]
+        result = torch.zeros(ts.shape, dtype=torch.int8, device=dev)
+        status = torch.zeros(self.n_elements, dtype=torch.int32, device=dev)
+        if P == 0:
+            return result, status
+        d = self._desc()
+        rc = capi.lib().m3tsz_element_set_add(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), _ptr(ts),
+                                              _ptr(values), P, _ptr(n_points), _ptr(result), _ptr(status),
+                                              _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_add")
+        return result, status
+
+    def consume(self, target_ns) -> torch.Tensor:
+        """Consume(target_ns): every open window that ended by target_ns, in order, through the element and onto
+        the output rows.  Returns status int32 [N]: OK, ERR_CAPACITY (the element's output slots lack room: it is
+        unchanged; grow(stride=...) and consume again), or a row's append status."""
+        dev = self.codec.device
+        status = torch.empty(self.n_elements, dtype=torch.int32, device=dev)
+        d = self._desc()
+        rc = capi.lib().m3tsz_element_set_consume(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
+                                                  int(target_ns), self.out_unit, _ptr(status), _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_consume")
+        return status
+
+    def grow(self, open_windows: Optional[int] = None, stride: Optional[int] = None):
+        """More open-window slots per element (the slots are copied; the new ones are free) and / or larger output
+        slots (EncoderSet.grow)."""
+        if open_windows is not None and open_windows != self.open_windows:
+            R = self.open_windows
+            assert open_windows > R
+            for f, a in self.win.items():
+                b = torch.zeros((open_windows, self.n_elements), dtype=a.dtype, device=a.device)
+                b[:R] = a
+                self.win[f] = b
+        if stride is not None and stride != self.out.stride:
+            self.out.grow(stride)
+
+    def stream(self) -> EncodeResult:
+        """The output rows' snapshot (EncoderSet.stream): row j * N + s is element s under agg_types[j]."""
+        return self.out.stream()
+
+    def state(self):
+        """Copies of the element-side state: {"win": {field: [R, N]}, "elem": uint8 [N, 160], "watermark": [N]}."""
+        return {"win": {f: a.clone() for f, a in self.win.items()}, "elem": self.elem.clone(),
+                "watermark": self.watermark.clone()}

@@ -126,6 +126,7 @@ const char *m3tsz_status_string(int st) {
     case M3TSZ_ERR_OUT_OF_ORDER: return "values are out of order from inner iterator";
     case M3TSZ_ERR_TOO_MANY_ITERATORS: return "too many replicas / readers for one series";
     case M3TSZ_ERR_TOO_MANY_ENCODERS: return "too many encoders per block";
+    case M3TSZ_ERR_AGGREGATION_CLOSED: return "aggregation is closed";
     case M3TSZ_ERR_CHECKSUM_MISMATCH: return "checksum does not match expected checksum";
     case M3TSZ_ERR_CAPACITY: return "output capacity exceeded";
     case M3TSZ_ERR_INVALID_ARG: return "invalid argument";
@@ -1219,6 +1220,156 @@ int m3tsz_aggregate_tiles_rollup_annotated(
       n_rollup_types, post_ops, n_post_ops, discard_nan, d_src_state, d_group_state, out_unit,
       {align, d_packed, packed_capacity, d_out_offsets, d_out_len, d_status, d_n_tiles, d_total_bytes}, d_src_status,
       true, stream);
+}
+
+// ---- element sets (DESIGN.md §4.12) ----
+// The checks every element-set call makes on the set (its element as m3tsz_aggregate_tiles_types checks one, its
+// arrays' presence and alignment), and the parameters the kernels read; xf takes the parsed lists.
+static bool element_params(const m3tsz_options *opts, const m3tsz_element_set *set, ElementParams &p,
+                           TileTransforms &xf) {
+  if (!valid_opts(opts) || !set || set->reserved != 0) return false;
+  const m3tsz_element_set &e = *set;
+  const bool counter = e.metric_type == M3TSZ_METRIC_COUNTER;
+  if (e.n_windows == 0 || e.n_windows > M3TSZ_MAX_ELEMENT_WINDOWS || e.resolution_ns <= 0 ||
+      e.n_elements > (1ull << 40) ||
+      !parse_element(e.metric_type, e.agg_types, e.n_types, e.ops, e.n_ops, e.d_elem, xf))
+    return false;
+  auto a8 = [](const void *q) { return q && !((uintptr_t)q & 7u); };
+  auto a16 = [](const void *q) { return q && !((uintptr_t)q & 15u); };
+  if (!a8(e.d_win_start) || !a8(e.d_win_count) || !a8(e.d_win_sum) || !a8(e.d_win_min) || !a8(e.d_win_max) ||
+      !a8(e.d_win_sum_sq) || (!counter && (!a8(e.d_win_last) || !a8(e.d_win_last_at))) || !a16(e.d_elem) ||
+      !a8(e.d_watermark) || !a16(e.d_out_state) || !a16(e.d_out_buf) || (e.out_stride & 15u) || e.out_stride == 0 ||
+      e.out_stride > (1ull << 33))
+    return false;
+  memset(&p, 0, sizeof(p));
+  p.n = e.n_elements;
+  p.n_slots = e.n_windows;
+  p.counter = counter ? 1 : 0;
+  p.resolution = e.resolution_ns;
+  // time.Time.Truncate counts from the zero time, 62135596800 s before the Unix epoch
+  p.trunc_off = (int64_t)((unsigned __int128)62135596800ull * 1000000000ull % (unsigned __int128)e.resolution_ns);
+  p.start = e.d_win_start;
+  p.count = e.d_win_count;
+  p.sum = e.d_win_sum;
+  p.min = e.d_win_min;
+  p.max = e.d_win_max;
+  p.sum_sq = e.d_win_sum_sq;
+  p.last = e.d_win_last;
+  p.last_at = e.d_win_last_at;
+  p.elem = e.d_elem;
+  p.watermark = e.d_watermark;
+  for (uint32_t j = 0; j < xf.n_types; j++) p.types |= (uint32_t)xf.types[j] << (4 * j);
+  p.n_types = xf.n_types;
+  p.ops = xf.ops;
+  p.discard_nan = (xf.ops && e.discard_nan) ? 1 : 0;  // (as m3tsz_aggregate_tiles_types)
+  p.out_state = e.d_out_state;
+  p.out_slot_words = e.out_stride >> 2;
+  memset(&p.tiles, 0, sizeof(p.tiles));
+  TileWindows w;
+  w.sum = e.d_win_sum;
+  w.cnt = e.d_win_count;
+  w.min = e.d_win_min;
+  w.max = e.d_win_max;
+  w.last = e.d_win_last;
+  w.sq = e.d_win_sum_sq;
+  tile_inputs(p.tiles, counter, w);
+  p.tiles.metric_type = e.metric_type;
+  return true;
+}
+
+int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                            const int64_t *d_start, void *stream) {
+  ElementParams p;
+  TileTransforms xf;
+  if (!ctx || !element_params(opts, set, p, xf) || (p.n && !d_start)) return M3TSZ_ERR_INVALID_ARG;
+  if (p.n == 0) return M3TSZ_OK;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t wb = (size_t)p.n * p.n_slots * 8;
+  for (void *a : {(void *)p.start, (void *)p.count, p.sum, p.min, p.max, p.sum_sq, (void *)p.last, (void *)p.last_at})
+    if (a) CK(cudaMemsetAsync(a, 0, wb, st));
+  CK(cudaMemsetAsync(p.elem, 0, p.n * sizeof(m3tsz_element_state), st));
+  CK(launch_fill_i64(p.watermark, INT64_MIN, p.n, st));
+  // row j * n + s of the output starts at element s's start
+  const uint64_t kn = (uint64_t)p.n_types * p.n;
+  void *d_rs = nullptr;
+  int rc;
+  if ((rc = ensure(ctx, kSlotElemRowTs, kn * 8, &d_rs))) return rc;
+  for (uint32_t j = 0; j < p.n_types; j++)
+    CK(cudaMemcpyAsync((int64_t *)d_rs + (uint64_t)j * p.n, d_start, p.n * 8, cudaMemcpyDeviceToDevice, st));
+  CK(launch_encoder_set_reset(set->d_out_state, kn, (const int64_t *)d_rs, opts->default_time_unit,
+                              opts->int_optimized != 0, st));
+  ctx->launches += 2;
+  return M3TSZ_OK;
+}
+
+int m3tsz_element_set_add(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                          const int64_t *d_ts, const double *d_val, uint64_t points_stride,
+                          const uint32_t *d_n_points, int8_t *d_result, int32_t *d_status, void *stream) {
+  ElementParams p;
+  TileTransforms xf;
+  if (!ctx || !element_params(opts, set, p, xf) || points_stride > 0xffffffffull) return M3TSZ_ERR_INVALID_ARG;
+  if (p.n == 0) return M3TSZ_OK;
+  if (!d_ts || !d_val || !d_result || !d_status || ((uintptr_t)d_ts & 7u) || ((uintptr_t)d_val & 7u) ||
+      ((uintptr_t)d_n_points & 3u) || ((uintptr_t)d_status & 3u))
+    return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  p.ts = d_ts;
+  p.val = d_val;
+  p.points_stride = points_stride;
+  p.n_points = d_n_points;
+  p.result = d_result;
+  p.status = d_status;
+  CK(launch_element_add(p, (cudaStream_t)stream));
+  ctx->launches++;
+  return M3TSZ_OK;
+}
+
+// The consume kernel stages each element's flushed datapoints as rows, the encoder-set append writes them, and the
+// status pass folds each element's rows into its status.
+int m3tsz_element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                              int64_t target_ns, int32_t out_unit, int32_t *d_status, void *stream) {
+  ElementParams p;
+  TileTransforms xf;
+  if (!ctx || !element_params(opts, set, p, xf) || !unit_is_valid(out_unit)) return M3TSZ_ERR_INVALID_ARG;
+  if (p.n == 0) return M3TSZ_OK;
+  if (!d_status || ((uintptr_t)d_status & 3u)) return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  cudaStream_t st = (cudaStream_t)stream;
+  const uint64_t kn = (uint64_t)p.n_types * p.n;
+  const uint64_t rows = (uint64_t)p.n_slots * (xf.reset ? 2u : 1u);  // a Reset op writes two datapoints per window
+  void *d_ts = nullptr, *d_val = nullptr, *d_n = nullptr, *d_rst = nullptr, *d_app = nullptr;
+  int rc;
+  if ((rc = ensure(ctx, kSlotElemRowTs, kn * rows * 8, &d_ts))) return rc;
+  if ((rc = ensure(ctx, kSlotElemRowVal, kn * rows * 8, &d_val))) return rc;
+  if ((rc = ensure(ctx, kSlotElemRowN, kn * 4, &d_n))) return rc;
+  if ((rc = ensure(ctx, kSlotElemRowStatus, kn * 4, &d_rst))) return rc;
+  if ((rc = ensure(ctx, kSlotElemRowAppended, kn * 4, &d_app))) return rc;
+  p.target = target_ns;
+  p.row_ts = (int64_t *)d_ts;
+  p.row_val = (double *)d_val;
+  p.row_n = (uint32_t *)d_n;
+  p.rows_stride = rows;
+  p.status = d_status;
+  CK(launch_element_consume(p, st));
+  m3tsz_encode_extras ex;
+  memset(&ex, 0, sizeof(ex));
+  ex.point_major_input = 1;
+  EncodeParams ep;
+  if (!encode_params(opts, p.row_ts, p.row_val, kn, rows, p.row_n, nullptr, out_unit, nullptr, nullptr, nullptr,
+                     nullptr, nullptr, (int32_t *)d_rst, &ex, ep, true))
+    return M3TSZ_ERR_INVALID_ARG;
+  ep.out = set->d_out_buf;
+  ep.out_stride = set->out_stride;
+  ep.state = set->d_out_state;
+  ep.n_appended = (uint32_t *)d_app;
+  CK(launch_encode_append(ep, opts->int_optimized != 0, st));
+  CK(launch_element_status((const int32_t *)d_rst, p.n, p.n_types, d_status, st));
+  ctx->launches += 3;
+  return M3TSZ_OK;
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

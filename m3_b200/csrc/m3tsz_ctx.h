@@ -50,6 +50,8 @@ struct Scratch {
 //                 / sumSq, group statuses
 //   64, 65        forwarded-annotation words, group annotation   tiles (aggregate_tiles_rollup_annotated)
 //                 references
+//   66-70         staged row ts / values / counts, row statuses, element_set_consume; element_set_reset (66: the
+//                 datapoints appended                            output rows' starts)
 enum Slot : int {
   kSlotStreams = 0,
   kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
@@ -110,7 +112,13 @@ enum Slot : int {
   // the rollup that keeps annotations
   kSlotFwdAnnPresent = 64,
   kSlotGroupAnn = 65,
-  kNumSlots = 66
+  // element sets
+  kSlotElemRowTs = 66,
+  kSlotElemRowVal = 67,
+  kSlotElemRowN = 68,
+  kSlotElemRowStatus = 69,
+  kSlotElemRowAppended = 70,
+  kNumSlots = 71
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

@@ -2518,6 +2518,315 @@ cudaError_t launch_rollup_fold(const RollupFoldParams &p, bool annotated, cudaSt
 }
 
 // ---------------------------------------------------------------------------
+// element sets (DESIGN.md §4.12): the aggregator's elements fed datapoint by datapoint, one lane per element
+// ---------------------------------------------------------------------------
+// t.Truncate(resolution) of Go's time.Time, which truncates the time since the zero time (year 1): the start of t's
+// window, with off = that origin's distance to the Unix epoch modulo the resolution.  false: the start would lie
+// below INT64_MIN.
+__device__ __forceinline__ bool elem_window_start(int64_t t, int64_t res, int64_t off, int64_t &ws) {
+  int64_t r = t % res;
+  if (r < 0) r += res;
+  r += off;
+  if (r >= res) r -= res;
+  if (t < (int64_t)0x8000000000000000ull + r) return false;
+  ws = t - r;
+  return true;
+}
+// a window starting at ws ends at or before `at` (ws + res <= at without the overflow of ws + res)
+__device__ __forceinline__ bool elem_ends_by(int64_t ws, int64_t res, int64_t at) {
+  return ws < at && (uint64_t)at - (uint64_t)ws >= (uint64_t)res;
+}
+
+// The open window a lane holds in registers: its start and the aggregates of the fused decode's windows (the Gauge's
+// min / max as its running form, +inf / -inf with no value yet; the Counter's int64)
+template <bool CTR>
+struct ElemAcc {
+  using V = std::conditional_t<CTR, int64_t, double>;
+  int64_t start, cnt;
+  V sum, mn, mx, sq;
+  double last;  // Gauge only
+  int64_t last_at;
+};
+template <bool CTR>
+__device__ __forceinline__ void elem_init(ElemAcc<CTR> &a, int64_t ws) {  // NewGauge / NewCounter
+  a.start = ws;
+  a.cnt = 0;
+  if constexpr (CTR) {
+    a.sum = 0;
+    a.mn = (int64_t)0x7fffffffffffffffull;
+    a.mx = (int64_t)0x8000000000000000ull;
+    a.sq = 0;
+  } else {
+    a.sum = 0.0;
+    a.mn = xf_bits(0x7ff0000000000000ull);
+    a.mx = xf_bits(0xfff0000000000000ull);
+    a.sq = 0.0;
+  }
+  a.last = 0.0;
+  a.last_at = 0;
+}
+// slots hold what the fused decode publishes: a Gauge window without a non-NaN value has min = max = math.NaN()
+template <bool CTR>
+__device__ __forceinline__ void elem_load(const ElementParams &p, uint64_t o, ElemAcc<CTR> &a) {
+  using V = typename ElemAcc<CTR>::V;
+  a.start = p.start[o];
+  a.cnt = p.count[o];
+  a.sum = static_cast<const V *>(p.sum)[o];
+  a.mn = static_cast<const V *>(p.min)[o];
+  a.mx = static_cast<const V *>(p.max)[o];
+  a.sq = static_cast<const V *>(p.sum_sq)[o];
+  if constexpr (!CTR) {
+    if (xf_isnan(a.mn)) {
+      a.mn = xf_bits(0x7ff0000000000000ull);
+      a.mx = xf_bits(0xfff0000000000000ull);
+    }
+    a.last = p.last[o];
+    a.last_at = p.last_at[o];
+  }
+}
+template <bool CTR>
+__device__ __forceinline__ void elem_store(const ElementParams &p, uint64_t o, const ElemAcc<CTR> &a) {
+  using V = typename ElemAcc<CTR>::V;
+  p.start[o] = a.start;
+  p.count[o] = a.cnt;
+  static_cast<V *>(p.sum)[o] = a.sum;
+  static_cast<V *>(p.sum_sq)[o] = a.sq;
+  if constexpr (CTR) {
+    static_cast<V *>(p.min)[o] = a.mn;
+    static_cast<V *>(p.max)[o] = a.mx;
+  } else {
+    const bool none = a.mn == xf_bits(0x7ff0000000000000ull) && a.mx == xf_bits(0xfff0000000000000ull);
+    static_cast<V *>(p.min)[o] = none ? xf_bits(kXfEmptyNaN) : a.mn;
+    static_cast<V *>(p.max)[o] = none ? xf_bits(kXfEmptyNaN) : a.mx;
+    p.last[o] = a.last;
+    p.last_at[o] = a.last_at;
+  }
+}
+// Gauge.Update (gauge.go:74-106) / Counter.Update (counter.go:52-78) as the fused decode runs them
+template <bool CTR>
+__device__ __forceinline__ void elem_update(ElemAcc<CTR> &a, int64_t t, double v) {
+  if constexpr (CTR) {  // int64(value), int64 arithmetic that wraps
+    const int64_t x = go_f64_to_i64(v);
+    a.sum = (int64_t)((uint64_t)a.sum + (uint64_t)x);
+    if (a.mx < x) a.mx = x;
+    if (a.mn > x) a.mn = x;
+    a.sq = (int64_t)((uint64_t)a.sq + (uint64_t)x * (uint64_t)x);
+  } else {
+    if (a.cnt == 0 || t > a.last_at) {  // lastAt.IsZero() || timestamp.After(lastAt), NaN values included
+      a.last_at = t;
+      a.last = v;
+    }
+    if (v == v) {
+      a.sum = __dadd_rn(a.sum, v);
+      a.sq = __dadd_rn(a.sq, __dmul_rn(v, v));
+    }
+    if (v > a.mx) a.mx = v;
+    if (v < a.mn) a.mn = v;
+  }
+  a.cnt++;
+}
+
+// AddUnion of element s's datapoints in row order.  The window the last datapoint went to stays in registers (in-order
+// data almost never leaves it) and goes back to its slot when a datapoint needs another one, and at the end.
+template <bool CTR>
+__device__ __forceinline__ void elem_add_lane(const ElementParams &p, uint64_t s) {
+  const uint32_t n_pts = p.n_points ? p.n_points[s] : (uint32_t)p.points_stride;
+  if (n_pts > p.points_stride) {
+    p.status[s] = M3TSZ_ERR_INVALID_ARG;
+    return;
+  }
+  const int64_t wm = p.watermark[s];
+  ElemAcc<CTR> a;
+  elem_init(a, 0);
+  int cur = -1;  // the slot `a` belongs to, -1: none
+  int32_t status = M3TSZ_OK;
+  for (uint32_t i = 0; i < n_pts; i++) {
+    const uint64_t at = (uint64_t)i * p.n + s;
+    int res = M3TSZ_ERR_CAPACITY;  // (after a CAPACITY, the rest of the element's datapoints)
+    if (status == M3TSZ_OK) {
+      const int64_t t = p.ts[at];
+      const double v = p.val[at];
+      int64_t ws = 0;
+      if (!elem_window_start(t, p.resolution, p.trunc_off, ws)) {
+        res = M3TSZ_ERR_INVALID_ARG;
+      } else if (elem_ends_by(ws, p.resolution, wm)) {
+        res = M3TSZ_ERR_AGGREGATION_CLOSED;
+      } else {
+        res = M3TSZ_OK;
+        if (cur < 0 || ws != a.start) {  // the window's slot, or a free one
+          int hit = -1, fr = -1;
+          for (uint32_t r = 0; r < p.n_slots; r++) {
+            if ((int)r == cur) continue;
+            const uint64_t o = (uint64_t)r * p.n + s;
+            if (p.count[o] == 0) {
+              if (fr < 0) fr = (int)r;
+            } else if (p.start[o] == ws) {
+              hit = (int)r;
+              break;
+            }
+          }
+          if (hit < 0 && fr < 0) {
+            status = res = M3TSZ_ERR_CAPACITY;
+          } else {
+            if (cur >= 0) elem_store(p, (uint64_t)cur * p.n + s, a);
+            cur = hit >= 0 ? hit : fr;
+            if (hit >= 0)
+              elem_load(p, (uint64_t)hit * p.n + s, a);
+            else
+              elem_init(a, ws);
+          }
+        }
+        if (res == M3TSZ_OK) elem_update(a, t, v);
+      }
+    }
+    p.result[at] = (int8_t)res;
+  }
+  if (cur >= 0) elem_store(p, (uint64_t)cur * p.n + s, a);
+  p.status[s] = status;
+}
+
+// Consume(target) of element s: its windows ending at or before p.target, in start order, through the multi-type
+// stage's element step (xf_element_window over tile_value_of of the slot), staged as rows for the encoder-set append:
+// type j's datapoints in rows j * n + s of p.row_ts / p.row_val ([p.rows_stride][n_types * n]), their count in
+// p.row_n.  An element whose output rows lack room changes nothing and gets CAPACITY.  `e` is the lane's element record
+// while it runs (the kernel's is in shared memory: xf_element_window indexes its inputs by type).
+template <bool CTR>
+__device__ __forceinline__ void elem_consume_lane(const ElementParams &p, uint64_t s, XfElem &e) {
+  const uint64_t kn = (uint64_t)p.n_types * p.n;
+  uint32_t m = 0;
+  for (uint32_t r = 0; r < p.n_slots; r++) {
+    const uint64_t o = (uint64_t)r * p.n + s;
+    if (p.count[o] != 0 && elem_ends_by(p.start[o], p.resolution, p.target)) m++;
+  }
+  bool reset = false;
+  for (int k = 0; k < M3TSZ_MAX_TRANSFORMS; k++) reset |= ((p.ops >> (4 * k)) & 0xfu) == M3TSZ_TRANSFORM_RESET;
+  int32_t status = M3TSZ_OK;
+  if (m) {
+    // the append's room check before a row's last datapoint, every earlier one at its worst case (163 bits with a
+    // time-unit change, m3tsz_encode_bound_units) after an empty encoder's 64-bit start: stream words so far +
+    // ENC_GUARD + 4 <= slot words
+    const uint64_t per_row = (uint64_t)m * (reset ? 2u : 1u);
+    for (uint32_t j = 0; j < p.n_types; j++) {
+      const m3tsz_encoder_state &e = p.out_state[(uint64_t)j * p.n + s];
+      const uint64_t bits = e.bits + (e.num_encoded ? 0u : 64u) + (per_row - 1) * 163u;
+      if ((bits >> 5) + ENC_GUARD + 4 > p.out_slot_words) status = M3TSZ_ERR_CAPACITY;
+    }
+  }
+  if (m == 0 || status != M3TSZ_OK) {
+    for (uint32_t j = 0; j < p.n_types; j++) p.row_n[(uint64_t)j * p.n + s] = 0;
+    p.status[s] = status;
+    return;
+  }
+  {
+    const m3tsz_element_state &r = p.elem[s];
+    e.w = r.head;
+    e.pv[0] = r.head.prev_v;
+    for (int j = 1; j < M3TSZ_MAX_ELEMENT_TYPES; j++) e.pv[j] = r.prev_v_more[j - 1];
+  }
+  uint64_t rows = 0;  // type j's datapoints so far in bits 8j .. 8j + 7 (at most 2 * M3TSZ_MAX_ELEMENT_WINDOWS)
+  int64_t prev = 0;
+  for (uint32_t q = 0; q < m; q++) {
+    int best = -1;  // the next window in start order (starts are distinct)
+    int64_t bs = 0;
+    for (uint32_t r = 0; r < p.n_slots; r++) {
+      const uint64_t o = (uint64_t)r * p.n + s;
+      if (p.count[o] == 0) continue;
+      const int64_t ws = p.start[o];
+      if (!elem_ends_by(ws, p.resolution, p.target) || (q && ws <= prev)) continue;
+      if (best < 0 || ws < bs) {
+        best = (int)r;
+        bs = ws;
+      }
+    }
+    prev = bs;
+    const uint64_t o = (uint64_t)best * p.n + s;
+    const int64_t c = p.count[o];
+    const int64_t t = bs + p.resolution;  // the window's end
+    xf_element_window(
+        p.ops, p.resolution, e, 0u, p.n_types, t,
+        [&](uint32_t i) {
+          uint64_t oi;  // (laundered per type, as in the IN = 5 stage)
+          asm volatile("mov.b64 %0, %1;" : "=l"(oi) : "l"(o));
+          return tile_value_of(p.tiles, CTR, (int)((p.types >> (4 * i)) & 0xfu), oi, c);
+        },
+        [&](uint32_t i, double v, int64_t extra_t) {
+          if (p.discard_nan && xf_isnan(v)) return;  // nothing of this type's window, its Reset datapoint included
+          uint64_t at = ((rows >> (8 * i)) & 0xffu) * kn + (uint64_t)i * p.n + s;
+          p.row_ts[at] = t;
+          p.row_val[at] = v;
+          if (extra_t != 0) {
+            at += kn;
+            p.row_ts[at] = extra_t;
+            p.row_val[at] = 0.0;
+          }
+          rows += (uint64_t)(extra_t != 0 ? 2u : 1u) << (8 * i);
+        });
+    p.count[o] = 0;  // the slot is free
+  }
+  p.watermark[s] = prev + p.resolution;
+  m3tsz_element_state &r = p.elem[s];
+  r.head = e.w;
+  r.head.prev_v = e.pv[0];
+  for (int j = 1; j < M3TSZ_MAX_ELEMENT_TYPES; j++) r.prev_v_more[j - 1] = e.pv[j];
+  for (uint32_t j = 0; j < p.n_types; j++) p.row_n[(uint64_t)j * p.n + s] = (uint32_t)((rows >> (8 * j)) & 0xffu);
+  p.status[s] = M3TSZ_OK;
+}
+
+constexpr int ELEM_THREADS = 256;
+template <bool CTR>
+__global__ void __launch_bounds__(ELEM_THREADS) element_add_kernel(const ElementParams p) {
+  const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (s < p.n) elem_add_lane<CTR>(p, s);
+}
+template <bool CTR>
+__global__ void __launch_bounds__(ELEM_THREADS) element_consume_kernel(const ElementParams p) {
+  __shared__ XfElem rec[ELEM_THREADS];
+  const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (s < p.n) elem_consume_lane<CTR>(p, s, rec[threadIdx.x]);
+}
+__global__ void element_status_kernel(const int32_t *row_status, uint64_t n, uint32_t n_types, int32_t *status) {
+  const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n || status[s] != M3TSZ_OK) return;
+  for (uint32_t j = 0; j < n_types; j++) {
+    const int32_t st = row_status[(uint64_t)j * n + s];
+    if (st != M3TSZ_OK) {
+      status[s] = st;
+      return;
+    }
+  }
+}
+
+static unsigned elem_blocks(uint64_t n) { return (unsigned)((n + ELEM_THREADS - 1) / ELEM_THREADS); }
+
+cudaError_t launch_element_add(const ElementParams &p, cudaStream_t stream) {
+  if (p.n == 0) return cudaSuccess;
+  if ((p.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  if (p.counter)
+    element_add_kernel<true><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  else
+    element_add_kernel<false><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_element_consume(const ElementParams &p, cudaStream_t stream) {
+  if (p.n == 0) return cudaSuccess;
+  if ((p.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  if (p.counter)
+    element_consume_kernel<true><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  else
+    element_consume_kernel<false><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_element_status(const int32_t *row_status, uint64_t n, uint32_t n_types, int32_t *status,
+                                  cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  if ((n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  element_status_kernel<<<elem_blocks(n), ELEM_THREADS, 0, stream>>>(row_status, n, n_types, status);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------
 // compaction: slots -> packed buffer with CSR offsets
 // ---------------------------------------------------------------------------
 __global__ void compact_lens_kernel(const uint64_t *len, uint64_t n, uint64_t mask, uint64_t *out) {

@@ -342,6 +342,47 @@ cudaError_t launch_rollup_commit(const uint64_t *group_off, const uint32_t *memb
                                  uint64_t n_src, uint8_t *mark, const m3tsz_transform_state *scratch,
                                  m3tsz_transform_state *state, int32_t *src_status_out, cudaStream_t stream);
 
+// element sets (m3tsz_element_set_*; m3tsz_encode.cu): one lane per element over its open-window slots, window-slot
+// major [n_slots][n] (slot r of element s at r * n + s)
+struct ElementParams {
+  uint64_t n;
+  uint32_t n_slots;
+  int counter;          // Counter: int64 sum / min / max / sumSq, no last; else the Gauge
+  int64_t resolution;
+  int64_t trunc_off;    // Go's Truncate origin: (the zero time's distance to the Unix epoch) % resolution
+  int64_t *start, *count;
+  void *sum, *min, *max, *sum_sq;
+  double *last;
+  int64_t *last_at;
+  m3tsz_element_state *elem;
+  int64_t *watermark;
+  // add: point-major datapoints [points_stride][n]
+  const int64_t *ts;
+  const double *val;
+  uint64_t points_stride;
+  const uint32_t *n_points;  // optional
+  int8_t *result;
+  int32_t *status;
+  // consume: the windows ending at or before `target` go to rows staged point-major [rows_stride][n_types * n]
+  int64_t target;
+  uint32_t types, n_types;  // type j's id in bits 4j .. 4j + 3
+  uint32_t ops;             // as EncodeParams::xf_ops
+  int discard_nan;          // (only with ops, as the tile calls)
+  const m3tsz_encoder_state *out_state;  // [n_types * n]: the output rows' encoders (their room)
+  uint64_t out_slot_words;
+  int64_t *row_ts;
+  double *row_val;
+  uint32_t *row_n;
+  uint64_t rows_stride;
+  // the slots as tile_value_of reads them (tile_sum .. tile_count, tile_sum_sq, metric_type)
+  EncodeParams tiles;
+};
+cudaError_t launch_element_add(const ElementParams &p, cudaStream_t stream);
+cudaError_t launch_element_consume(const ElementParams &p, cudaStream_t stream);
+// an element consumed with status OK takes the first failing status of its n_types rows
+cudaError_t launch_element_status(const int32_t *row_status, uint64_t n, uint32_t n_types, int32_t *status,
+                                  cudaStream_t stream);
+
 // exclusive scan of aligned lengths + gather into a packed buffer
 cudaError_t launch_compact(const uint8_t *slots, uint64_t slot_stride, const uint64_t *len,
                            uint64_t n_series, uint32_t align, uint8_t *packed,

@@ -36,6 +36,7 @@ OUT_ANN = os.path.join(os.path.dirname(OUT), "m3tsz_tile_annotation_goldens.json
 OUT_ROLLUP = os.path.join(os.path.dirname(OUT), "m3tsz_rollup_goldens.json")
 # the annotation a rollup element keeps: AddUnique passes metric.Annotation to Gauge / Counter Update
 OUT_ROLLUP_ANN = os.path.join(os.path.dirname(OUT), "m3tsz_rollup_annotation_goldens.json")
+OUT_ELEM_CONSUME = os.path.join(os.path.dirname(OUT), "m3tsz_element_consume_goldens.json")
 
 SEC = 1_000_000_000
 MS = 1_000_000
@@ -715,6 +716,68 @@ def main():
         ],
     }
 
+    # ---- an element fed datapoint by datapoint (element sets): GenericElem.AddUnion's window contents and
+    # Consume(target)'s flushed datapoints, from elem_test.go.  testTimestamps are 216 / 217 / 221 s,
+    # testAlignedStarts 210 / 220 / 230 s (:120-125), resolution 10 s (:56), testGauge.GaugeVal 123.456 (:89-93),
+    # testCounter.CounterVal 1234 (:79-83), testAggregationTypesExpensive {SumSq} (:59).  The default types are Last
+    # (Gauge) and Sum (Counter).  An "adds" case adds its datapoints one per step and lists the windows the test
+    # asserts on after each (only the fields it asserts; the reference tracks sumSq only with an expensive type, so the
+    # default cases assert nothing of it here).  The Counter's datapoints are those of the case of the same name in
+    # m3tsz_tile_annotation_goldens.json ("datapoints_from").  A "consumes" case starts from the windows the test
+    # builds, one datapoint each ("windows": start, the value; testGaugeElemWithData stores its datapoint at the start
+    # minus 1 ns, :3135-3136, which only sets lastAt), and lists each Consume's target and each type's datapoints.
+    g_val, c_val = 123.456, 1234.0
+
+    def win(start_s, **fields):
+        return dict({"start_ns": start_s * SEC}, **fields)
+
+    elem_consume = {
+        "description": "An aggregator element fed datapoint by datapoint, transcribed from the reference's element "
+                       "tests by scripts/make_goldens.py: the windows AddUnion leaves (adds) and the datapoints each "
+                       "Consume(target) flushes at the window's end (consumes).",
+        "adds": [
+            {"name": "TestGaugeElemAddUnion", "src_line": "aggregator/aggregator/elem_test.go:1383-1424",
+             "metric_type": 3, "agg_types": [1], "resolution_ns": 10 * SEC,
+             "datapoints": [[216 * SEC, g_val], [217 * SEC, g_val], [221 * SEC, g_val]],
+             "want_windows": [[win(210, last=g_val, sum=g_val)],
+                              [win(210, last=g_val, sum=2 * g_val)],
+                              [win(210), win(220, last=g_val, sum=g_val)]]},
+            {"name": "TestGaugeElemAddUnionWithCustomAggregation",
+             "src_line": "aggregator/aggregator/elem_test.go:1426-1471", "metric_type": 3, "agg_types": [8],
+             "resolution_ns": 10 * SEC,
+             "datapoints": [[216 * SEC, g_val], [217 * SEC, g_val], [221 * SEC, g_val]],
+             "want_windows": [[win(210, last=g_val, sum=g_val, mean=g_val, sum_sq=g_val * g_val)],
+                              [win(210, last=g_val, max=g_val, sum=2 * g_val, sum_sq=2 * g_val * g_val)],
+                              [win(210), win(220, last=g_val, max=g_val)]]},
+            {"name": "TestCounterElemAddUnion", "src_line": "aggregator/aggregator/elem_test.go:215-259",
+             "metric_type": 1, "agg_types": [7], "resolution_ns": 10 * SEC,
+             "datapoints_from": "m3tsz_tile_annotation_goldens.json",
+             "want_windows": [[win(210, sum=1234, count=1)],
+                              [win(210, sum=2468, count=2)],
+                              [win(210, count=2), win(220, sum=1234)]]},
+            {"name": "TestCounterElemAddUnionWithCustomAggregation",
+             "src_line": "aggregator/aggregator/elem_test.go:261-306", "metric_type": 1, "agg_types": [8],
+             "resolution_ns": 10 * SEC, "datapoints_from": "m3tsz_tile_annotation_goldens.json",
+             "want_windows": [[win(210, sum=1234, max=1234, sum_sq=1234 * 1234)],
+                              [win(210, sum=2468, max=1234, sum_sq=2 * 1234 * 1234)],
+                              [win(210), win(220, sum=1234, max=1234, sum_sq=1234 * 1234)]]},
+        ],
+        "consumes": [
+            {"name": "TestCounterElemConsumeDefaultAggregationDefaultPipeline",
+             "src_line": "aggregator/aggregator/elem_test.go:468-530", "metric_type": 1, "agg_types": [7],
+             "resolution_ns": 10 * SEC, "windows": [[210 * SEC, c_val], [220 * SEC, c_val]],
+             "steps": [{"target_ns": 0, "want": [[]]},
+                       {"target_ns": 220 * SEC, "want": [[[220 * SEC, c_val]]]},
+                       {"target_ns": 230 * SEC, "want": [[[230 * SEC, c_val]]]}]},
+            {"name": "TestGaugeElemConsumeDefaultAggregationDefaultPipeline",
+             "src_line": "aggregator/aggregator/elem_test.go:1645-1707", "metric_type": 3, "agg_types": [1],
+             "resolution_ns": 10 * SEC, "windows": [[210 * SEC, g_val], [220 * SEC, g_val]],
+             "steps": [{"target_ns": 0, "want": [[]]},
+                       {"target_ns": 220 * SEC, "want": [[[220 * SEC, g_val]]]},
+                       {"target_ns": 230 * SEC, "want": [[[230 * SEC, g_val]]]}]},
+        ],
+    }
+
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     with open(OUT, "w") as f:
         json.dump(g, f, indent=1)
@@ -740,6 +803,9 @@ def main():
     with open(OUT_ROLLUP_ANN, "w") as f:
         json.dump(rollup_ann, f, indent=1)
     print("wrote", OUT_ROLLUP_ANN)
+    with open(OUT_ELEM_CONSUME, "w") as f:
+        json.dump(elem_consume, f, indent=1)
+    print("wrote", OUT_ELEM_CONSUME)
 
 
 if __name__ == "__main__":
