@@ -1003,6 +1003,53 @@ int m3tsz_element_set_add(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz
 int m3tsz_element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
                               int64_t target_ns, int32_t out_unit, int32_t *d_status, void *stream);
 
+/* Element sets that keep annotations (DESIGN.md §4.12): each open window holds the last non-empty annotation of the
+ * datapoints added to it, as Gauge.Update / Counter.Update keep it (aggregation/common.go:47-61), and every datapoint a
+ * consume flushes for the window carries it (generic_elem.go:567, 923-931), the Reset datapoint included.
+ *
+ * The window slots' annotations live in caller-owned device memory beside the other slot arrays, pointer-free like
+ * them (growing R or the capacity is a copy):
+ *   - d_len [R][n_elements], 4-byte aligned: the byte length of slot r's annotation, 0 for none;
+ *   - d_bytes, 8-byte aligned: slot r of element s's bytes at (r * n_elements + s) * capacity.
+ * capacity: bytes per slot, a multiple of 8 in 8 .. M3TSZ_MAX_ELEMENT_ANNOTATION.
+ *
+ * The lengths need no initial value.  The annotated add writes a slot's length whenever it opens a window there (0
+ * until a datapoint with an annotation arrives) and stores at most `capacity`; the annotated consume reads the lengths
+ * of open slots only, and takes a length above `capacity` as none.  The plain calls neither read nor write these
+ * arrays, so a window the plain add opened keeps whatever length its slot held, and an annotated consume writes it
+ * with that slot's stale annotation.  A set should therefore use one kind of call; to switch a set to the annotated
+ * calls, zero d_len after its last plain add.  The annotated calls write the same bytes as the plain calls where no
+ * datapoint carries an annotation. */
+#define M3TSZ_MAX_ELEMENT_ANNOTATION 65536
+typedef struct m3tsz_element_annotations {
+  uint32_t *d_len;   /* [R][n_elements]: bytes of window slot r's annotation, 0 = none */
+  uint8_t *d_bytes;  /* slot r of element s at (r * n_elements + s) * capacity */
+  uint32_t capacity; /* bytes per slot: a multiple of 8, 8 .. M3TSZ_MAX_ELEMENT_ANNOTATION */
+  uint32_t reserved; /* 0 */
+} m3tsz_element_annotations;
+
+/* m3tsz_element_set_add with annotations: the sparse list of m3tsz_encoder_set_append (entries
+ * [d_ann_series_off[s], d_ann_series_off[s+1]) belong to element s, sorted by dp_index, which counts rows of the
+ * element's point-major column in this call; length 0 is no annotation; d_ann_series_off NULL: none in this call).
+ * A datapoint the add accepts (d_result 0) with a non-empty annotation makes it its window's annotation, whatever its
+ * value (NaN included); a refused datapoint changes no annotation.  A datapoint that would be accepted but whose
+ * annotation is longer than `capacity` gets M3TSZ_ERR_CAPACITY under the rule of a new window with all R slots open:
+ * nothing of it or of the element's later datapoints in this call is added, so growing the capacity and adding exactly
+ * those again gives the unstopped result. */
+int m3tsz_element_set_add_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                    const m3tsz_element_annotations *ann, const int64_t *d_ts, const double *d_val,
+                                    uint64_t points_stride, const uint32_t *d_n_points,
+                                    const uint64_t *d_ann_series_off, const m3tsz_annotation_entry *d_ann_entries,
+                                    const uint8_t *d_ann_bytes, int8_t *d_result, int32_t *d_status, void *stream);
+
+/* m3tsz_element_set_consume where every datapoint flushed for a window carries the window's annotation; the output row
+ * writes it when its XXH64 differs from the row's last one written (as m3tsz_encoder_set_append does).  The room check
+ * also counts each flushed datapoint's annotation as the append's own check does, (len + 3) / 4 + 4 words for a
+ * non-empty one.  The flushed slots' bytes stay where they are until the next add. */
+int m3tsz_element_set_consume_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                        const m3tsz_element_annotations *ann, int64_t target_ns, int32_t out_unit,
+                                        int32_t *d_status, void *stream);
+
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the
  * reference's interfaces (INTEGRATION.md §2 is that shim):

@@ -36,6 +36,7 @@ TRANSFORM_STATE_BYTES = 96  # sizeof(m3tsz_transform_state)
 MAX_ELEMENT_TYPES = 8  # M3TSZ_MAX_ELEMENT_TYPES (m3tsz_aggregate_tiles_types)
 ELEMENT_STATE_BYTES = 160  # sizeof(m3tsz_element_state)
 MAX_ELEMENT_WINDOWS = 64  # M3TSZ_MAX_ELEMENT_WINDOWS (element sets)
+MAX_ELEMENT_ANNOTATION = 65536  # M3TSZ_MAX_ELEMENT_ANNOTATION (bytes per window slot of an annotated element set)
 
 UNIT_NONE, UNIT_S, UNIT_MS, UNIT_US, UNIT_NS, UNIT_MIN, UNIT_HOUR, UNIT_DAY, UNIT_YEAR = range(9)
 
@@ -68,6 +69,11 @@ class ElementSet(C.Structure):
                     "d_win_start", "d_win_count", "d_win_sum", "d_win_min", "d_win_max", "d_win_sum_sq", "d_win_last",
                     "d_win_last_at", "d_elem", "d_watermark", "d_out_state", "d_out_buf")] + [
                 ("out_stride", C.c_uint64)]
+
+
+class ElementAnnotations(C.Structure):
+    """m3tsz_element_annotations: the window slots' annotation lengths and bytes (include/m3tsz_b200.h)."""
+    _fields_ = [("d_len", C.c_void_p), ("d_bytes", C.c_void_p), ("capacity", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 class DecodeExtras(C.Structure):
@@ -129,6 +135,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_aggregate_tiles_transform", "m3tsz_aggregate_tiles_types", "m3tsz_aggregate_tiles_annotated",
     "m3tsz_aggregate_tiles_blocks", "m3tsz_aggregate_tiles_rollup", "m3tsz_aggregate_tiles_rollup_annotated",
     "m3tsz_element_set_reset", "m3tsz_element_set_add", "m3tsz_element_set_consume",
+    "m3tsz_element_set_add_annotated", "m3tsz_element_set_consume_annotated",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -317,6 +324,11 @@ def lib():
     L.m3tsz_element_set_add.argtypes = [vp, po, pes, vp, vp, u64, vp, vp, vp, vp]
     L.m3tsz_element_set_consume.restype = C.c_int
     L.m3tsz_element_set_consume.argtypes = [vp, po, pes, i64, i32, vp, vp]
+    pea = C.POINTER(ElementAnnotations)
+    L.m3tsz_element_set_add_annotated.restype = C.c_int
+    L.m3tsz_element_set_add_annotated.argtypes = [vp, po, pes, pea, vp, vp, u64, vp, vp, vp, vp, vp, vp, vp]
+    L.m3tsz_element_set_consume_annotated.restype = C.c_int
+    L.m3tsz_element_set_consume_annotated.argtypes = [vp, po, pes, pea, i64, i32, vp, vp]
     _lib = L
     return L
 

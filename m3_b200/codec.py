@@ -289,15 +289,17 @@ class BatchCodec:
 
     def element_set(self, start: torch.Tensor, metric_type, agg_types, resolution_ns, transforms=(),
                     discard_nan=False, open_windows=4, stride: Optional[int] = None,
-                    out_unit=capi.UNIT_S) -> "ElementSet":
+                    out_unit=capi.UNIT_S, annotation_capacity=0) -> "ElementSet":
         """N aggregator elements fed datapoint by datapoint (m3tsz_element_set_*, N = start.numel(), start int64
         [N] ns): one metric type (capi.METRIC_GAUGE / METRIC_COUNTER), resolution, strictly ascending list of
         aggregation types and transformation list, checked and applied as in aggregate_tiles_types (discard_nan
         only with transformations).  Each element keeps up to `open_windows` open windows; its flushed windows go to
         an encoder set of k * N rows (row j * N + s: element s under agg_types[j]) with slots of `stride` bytes
-        (default: room for 128 datapoints per row at their worst case), written with `out_unit`."""
+        (default: room for 128 datapoints per row at their worst case), written with `out_unit`.
+        annotation_capacity > 0 (a multiple of 8, at most capi.MAX_ELEMENT_ANNOTATION): the elements keep annotations
+        (m3tsz_element_set_*_annotated), each open window up to that many bytes of its last non-empty one."""
         return ElementSet(self, start, metric_type, agg_types, resolution_ns, transforms, discard_nan, open_windows,
-                          stride, out_unit)
+                          stride, out_unit, annotation_capacity)
 
     def bucket_set(self, start: torch.Tensor, stride: int, encoders=4, pool_records: Optional[int] = None,
                    pool_stride: Optional[int] = None) -> "BucketSet":
@@ -868,10 +870,11 @@ class ElementSet:
     the Gauge last / last_at; a Counter's aggregates are int64), `elem` uint8 [N, 160] (m3tsz_element_state),
     `watermark` int64 [N] (the end of the last window consumed, INT64_MIN for none) and `out`, the EncoderSet the
     flushed windows are appended to.  add() puts datapoints into open windows, consume() flushes the windows that
-    ended by a target time."""
+    ended by a target time.  With an annotation capacity the set keeps annotations: `ann_len` int32 [R, N] (bytes of
+    each slot's annotation, 0 for none) and `ann_bytes` uint8 [R, N, capacity], and every call is the annotated one."""
 
     def __init__(self, codec: BatchCodec, start: torch.Tensor, metric_type, agg_types, resolution_ns, transforms,
-                 discard_nan, open_windows, stride, out_unit):
+                 discard_nan, open_windows, stride, out_unit, annotation_capacity=0):
         assert start.dtype == torch.int64 and start.is_cuda
         self.codec = codec
         self.metric_type = int(metric_type)
@@ -893,6 +896,10 @@ class ElementSet:
         self.win = {f: torch.zeros((R, N), dtype=t, device=dev) for f, t in names}
         self.elem = torch.zeros((N, capi.ELEMENT_STATE_BYTES), dtype=torch.uint8, device=dev)
         self.watermark = torch.empty(N, dtype=torch.int64, device=dev)
+        self.ann_len = self.ann_bytes = None
+        if annotation_capacity:
+            self.ann_len = torch.zeros((R, N), dtype=torch.int32, device=dev)
+            self.ann_bytes = torch.zeros((R, N, int(annotation_capacity)), dtype=torch.uint8, device=dev)
         if stride is None:
             stride = int(capi.lib().m3tsz_encode_bound_units(128, 1))
         start = start.contiguous()
@@ -924,6 +931,17 @@ class ElementSet:
         d.out_stride = self.out.stride
         return d
 
+    @property
+    def annotation_capacity(self) -> int:
+        return 0 if self.ann_bytes is None else self.ann_bytes.shape[2]
+
+    def _ann(self):
+        a = capi.ElementAnnotations()
+        a.d_len = self.ann_len.data_ptr()
+        a.d_bytes = self.ann_bytes.data_ptr()
+        a.capacity = self.annotation_capacity
+        return a
+
     def reset(self, start: torch.Tensor):
         """Every element new: windows free, records zero, nothing consumed, output rows Reset(start[s])."""
         assert start.dtype == torch.int64 and start.is_cuda and start.numel() == self.n_elements
@@ -932,13 +950,19 @@ class ElementSet:
         rc = capi.lib().m3tsz_element_set_reset(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
                                                 _ptr(start), _cuda_stream_ptr(self.codec.device))
         self.codec.ctx.check(rc, "m3tsz_element_set_reset")
+        if self.ann_len is not None:
+            self.ann_len.zero_()
 
-    def add(self, ts: torch.Tensor, values: torch.Tensor, n_points: Optional[torch.Tensor] = None):
+    def add(self, ts: torch.Tensor, values: torch.Tensor, n_points: Optional[torch.Tensor] = None,
+            annotations=None):
         """AddUnion of point-major ts / values int64 / float64 [P, N]: element s takes n_points[s] (int32 [N]; all P
         when None) of its column, in order.  Returns (result int8 [P, N]: 0 added, else ERR_AGGREGATION_CLOSED /
         ERR_CAPACITY / ERR_INVALID_ARG, rows past an element's count left 0; status int32 [N]: OK, ERR_CAPACITY --
         that datapoint and the element's later ones were not added: grow() and add them again -- or
-        ERR_INVALID_ARG)."""
+        ERR_INVALID_ARG).  annotations (a set with an annotation capacity only): (series_off int64 [N + 1], entries
+        capi.AnnotationEntry rows as uint8 [E, 16], bytes uint8) as EncoderSet.append takes them, dp_index counting
+        rows of the element's column; an annotation longer than the capacity stops the element with ERR_CAPACITY
+        (grow(annotation_capacity=...) and add again)."""
         assert ts.dtype == torch.int64 and values.dtype == torch.float64 and ts.shape == values.shape
         assert ts.is_cuda and values.is_cuda and ts.is_contiguous() and values.is_contiguous()
         assert ts.dim() == 2 and ts.shape[1] == self.n_elements
@@ -952,10 +976,22 @@ class ElementSet:
         if P == 0:
             return result, status
         d = self._desc()
-        rc = capi.lib().m3tsz_element_set_add(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), _ptr(ts),
-                                              _ptr(values), P, _ptr(n_points), _ptr(result), _ptr(status),
-                                              _cuda_stream_ptr(dev))
-        self.codec.ctx.check(rc, "m3tsz_element_set_add")
+        if self.ann_len is None:
+            assert annotations is None, "a set without an annotation capacity takes no annotations"
+            rc = capi.lib().m3tsz_element_set_add(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
+                                                  _ptr(ts), _ptr(values), P, _ptr(n_points), _ptr(result),
+                                                  _ptr(status), _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_element_set_add")
+            return result, status
+        a_off = a_ent = a_bytes = None
+        if annotations is not None:
+            a_off, a_ent, a_bytes = annotations
+        a = self._ann()
+        rc = capi.lib().m3tsz_element_set_add_annotated(
+            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(a), _ptr(ts), _ptr(values), P,
+            _ptr(n_points), _ptr(a_off), _ptr(a_ent), _ptr(a_bytes), _ptr(result), _ptr(status),
+            _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_add_annotated")
         return result, status
 
     def consume(self, target_ns) -> torch.Tensor:
@@ -965,14 +1001,23 @@ class ElementSet:
         dev = self.codec.device
         status = torch.empty(self.n_elements, dtype=torch.int32, device=dev)
         d = self._desc()
-        rc = capi.lib().m3tsz_element_set_consume(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
-                                                  int(target_ns), self.out_unit, _ptr(status), _cuda_stream_ptr(dev))
-        self.codec.ctx.check(rc, "m3tsz_element_set_consume")
+        if self.ann_len is None:
+            rc = capi.lib().m3tsz_element_set_consume(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
+                                                      int(target_ns), self.out_unit, _ptr(status),
+                                                      _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_element_set_consume")
+            return status
+        a = self._ann()
+        rc = capi.lib().m3tsz_element_set_consume_annotated(self.codec.ctx.handle, C.byref(self.codec.opts),
+                                                            C.byref(d), C.byref(a), int(target_ns), self.out_unit,
+                                                            _ptr(status), _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_consume_annotated")
         return status
 
-    def grow(self, open_windows: Optional[int] = None, stride: Optional[int] = None):
-        """More open-window slots per element (the slots are copied; the new ones are free) and / or larger output
-        slots (EncoderSet.grow)."""
+    def grow(self, open_windows: Optional[int] = None, stride: Optional[int] = None,
+             annotation_capacity: Optional[int] = None):
+        """More open-window slots per element (the slots are copied; the new ones are free), larger output slots
+        (EncoderSet.grow) and / or, for a set that keeps annotations, more annotation bytes per slot (copied)."""
         if open_windows is not None and open_windows != self.open_windows:
             R = self.open_windows
             assert open_windows > R
@@ -980,6 +1025,19 @@ class ElementSet:
                 b = torch.zeros((open_windows, self.n_elements), dtype=a.dtype, device=a.device)
                 b[:R] = a
                 self.win[f] = b
+            if self.ann_len is not None:
+                ln = torch.zeros((open_windows, self.n_elements), dtype=torch.int32, device=self.ann_len.device)
+                ln[:R] = self.ann_len
+                by = torch.zeros((open_windows,) + tuple(self.ann_bytes.shape[1:]), dtype=torch.uint8,
+                                 device=self.ann_bytes.device)
+                by[:R] = self.ann_bytes
+                self.ann_len, self.ann_bytes = ln, by
+        if annotation_capacity is not None and annotation_capacity != self.annotation_capacity:
+            assert self.ann_bytes is not None and annotation_capacity > self.annotation_capacity
+            by = torch.zeros(tuple(self.ann_bytes.shape[:2]) + (int(annotation_capacity),), dtype=torch.uint8,
+                             device=self.ann_bytes.device)
+            by[:, :, : self.annotation_capacity] = self.ann_bytes
+            self.ann_bytes = by
         if stride is not None and stride != self.out.stride:
             self.out.grow(stride)
 
@@ -988,6 +1046,10 @@ class ElementSet:
         return self.out.stream()
 
     def state(self):
-        """Copies of the element-side state: {"win": {field: [R, N]}, "elem": uint8 [N, 160], "watermark": [N]}."""
-        return {"win": {f: a.clone() for f, a in self.win.items()}, "elem": self.elem.clone(),
-                "watermark": self.watermark.clone()}
+        """Copies of the element-side state: {"win": {field: [R, N]}, "elem": uint8 [N, 160], "watermark": [N]},
+        and with annotations "ann_len" [R, N] and "ann_bytes" [R, N, capacity]."""
+        st = {"win": {f: a.clone() for f, a in self.win.items()}, "elem": self.elem.clone(),
+              "watermark": self.watermark.clone()}
+        if self.ann_len is not None:
+            st["ann_len"], st["ann_bytes"] = self.ann_len.clone(), self.ann_bytes.clone()
+        return st

@@ -1304,12 +1304,31 @@ int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3t
   return M3TSZ_OK;
 }
 
-int m3tsz_element_set_add(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
-                          const int64_t *d_ts, const double *d_val, uint64_t points_stride,
-                          const uint32_t *d_n_points, int8_t *d_result, int32_t *d_status, void *stream) {
+// The annotated calls' slot arrays (m3tsz_element_annotations), checked as element_params checks the others; p gets
+// them.  The lengths and bytes cover R * n_elements slots: a capacity of at most 2^16 keeps every offset in 64 bits.
+static bool element_ann_params(const m3tsz_element_annotations *ann, ElementParams &p) {
+  if (!ann || ann->reserved != 0 || ann->capacity == 0 || (ann->capacity & 7u) ||
+      ann->capacity > M3TSZ_MAX_ELEMENT_ANNOTATION || !ann->d_len || ((uintptr_t)ann->d_len & 3u) || !ann->d_bytes ||
+      ((uintptr_t)ann->d_bytes & 7u))
+    return false;
+  p.ann_len = ann->d_len;
+  p.ann_slot = ann->d_bytes;
+  p.ann_cap = ann->capacity;
+  return true;
+}
+
+// m3tsz_element_set_add(_annotated): ann NULL is the plain add
+static int element_set_add(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                           const m3tsz_element_annotations *ann, const int64_t *d_ts, const double *d_val,
+                           uint64_t points_stride, const uint32_t *d_n_points, const uint64_t *d_ann_series_off,
+                           const m3tsz_annotation_entry *d_ann_entries, const uint8_t *d_ann_bytes, int8_t *d_result,
+                           int32_t *d_status, void *stream, bool annotated) {
   ElementParams p;
   TileTransforms xf;
   if (!ctx || !element_params(opts, set, p, xf) || points_stride > 0xffffffffull) return M3TSZ_ERR_INVALID_ARG;
+  if (annotated && (!element_ann_params(ann, p) || ((uintptr_t)d_ann_series_off & 7u) ||
+                    (d_ann_series_off && (!d_ann_entries || !d_ann_bytes || ((uintptr_t)d_ann_entries & 7u)))))
+    return M3TSZ_ERR_INVALID_ARG;
   if (p.n == 0) return M3TSZ_OK;
   if (!d_ts || !d_val || !d_result || !d_status || ((uintptr_t)d_ts & 7u) || ((uintptr_t)d_val & 7u) ||
       ((uintptr_t)d_n_points & 3u) || ((uintptr_t)d_status & 3u))
@@ -1322,18 +1341,43 @@ int m3tsz_element_set_add(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz
   p.n_points = d_n_points;
   p.result = d_result;
   p.status = d_status;
+  if (annotated) {
+    p.ann_series_off = d_ann_series_off;
+    p.ann_entries = d_ann_entries;
+    p.ann_bytes = d_ann_bytes;
+  }
   CK(launch_element_add(p, (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
 }
 
+int m3tsz_element_set_add(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                          const int64_t *d_ts, const double *d_val, uint64_t points_stride,
+                          const uint32_t *d_n_points, int8_t *d_result, int32_t *d_status, void *stream) {
+  return element_set_add(ctx, opts, set, nullptr, d_ts, d_val, points_stride, d_n_points, nullptr, nullptr, nullptr,
+                         d_result, d_status, stream, false);
+}
+
+int m3tsz_element_set_add_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                    const m3tsz_element_annotations *ann, const int64_t *d_ts, const double *d_val,
+                                    uint64_t points_stride, const uint32_t *d_n_points,
+                                    const uint64_t *d_ann_series_off, const m3tsz_annotation_entry *d_ann_entries,
+                                    const uint8_t *d_ann_bytes, int8_t *d_result, int32_t *d_status, void *stream) {
+  return element_set_add(ctx, opts, set, ann, d_ts, d_val, points_stride, d_n_points, d_ann_series_off,
+                         d_ann_entries, d_ann_bytes, d_result, d_status, stream, true);
+}
+
 // The consume kernel stages each element's flushed datapoints as rows, the encoder-set append writes them, and the
-// status pass folds each element's rows into its status.
-int m3tsz_element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
-                              int64_t target_ns, int32_t out_unit, int32_t *d_status, void *stream) {
+// status pass folds each element's rows into its status.  Annotated: the kernel also stages each row's annotation
+// entries (a fixed-stride list over the slots' bytes), which the append reads as it reads an encoder set's sparse
+// list; its lane code takes that list in the point-major stage too (dp_index counts a series' rows in either layout).
+static int element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                               const m3tsz_element_annotations *ann, int64_t target_ns, int32_t out_unit,
+                               int32_t *d_status, void *stream, bool annotated) {
   ElementParams p;
   TileTransforms xf;
   if (!ctx || !element_params(opts, set, p, xf) || !unit_is_valid(out_unit)) return M3TSZ_ERR_INVALID_ARG;
+  if (annotated && !element_ann_params(ann, p)) return M3TSZ_ERR_INVALID_ARG;
   if (p.n == 0) return M3TSZ_OK;
   if (!d_status || ((uintptr_t)d_status & 3u)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
@@ -1348,6 +1392,13 @@ int m3tsz_element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m
   if ((rc = ensure(ctx, kSlotElemRowN, kn * 4, &d_n))) return rc;
   if ((rc = ensure(ctx, kSlotElemRowStatus, kn * 4, &d_rst))) return rc;
   if ((rc = ensure(ctx, kSlotElemRowAppended, kn * 4, &d_app))) return rc;
+  if (annotated) {
+    void *d_aoff = nullptr, *d_aent = nullptr;
+    if ((rc = ensure(ctx, kSlotElemRowAnnOff, (kn + 1) * 8, &d_aoff))) return rc;
+    if ((rc = ensure(ctx, kSlotElemRowAnn, kn * rows * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
+    p.row_ann_off = (uint64_t *)d_aoff;
+    p.row_ann = (m3tsz_annotation_entry *)d_aent;
+  }
   p.target = target_ns;
   p.row_ts = (int64_t *)d_ts;
   p.row_val = (double *)d_val;
@@ -1362,6 +1413,11 @@ int m3tsz_element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m
   if (!encode_params(opts, p.row_ts, p.row_val, kn, rows, p.row_n, nullptr, out_unit, nullptr, nullptr, nullptr,
                      nullptr, nullptr, (int32_t *)d_rst, &ex, ep, true))
     return M3TSZ_ERR_INVALID_ARG;
+  if (annotated) {  // (the public calls take no annotations with point-major input; this list is the library's own)
+    ep.ann_series_off = p.row_ann_off;
+    ep.ann_entries = p.row_ann;
+    ep.ann_bytes = p.ann_slot;
+  }
   ep.out = set->d_out_buf;
   ep.out_stride = set->out_stride;
   ep.state = set->d_out_state;
@@ -1370,6 +1426,17 @@ int m3tsz_element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m
   CK(launch_element_status((const int32_t *)d_rst, p.n, p.n_types, d_status, st));
   ctx->launches += 3;
   return M3TSZ_OK;
+}
+
+int m3tsz_element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                              int64_t target_ns, int32_t out_unit, int32_t *d_status, void *stream) {
+  return element_set_consume(ctx, opts, set, nullptr, target_ns, out_unit, d_status, stream, false);
+}
+
+int m3tsz_element_set_consume_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                        const m3tsz_element_annotations *ann, int64_t target_ns, int32_t out_unit,
+                                        int32_t *d_status, void *stream) {
+  return element_set_consume(ctx, opts, set, ann, target_ns, out_unit, d_status, stream, true);
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

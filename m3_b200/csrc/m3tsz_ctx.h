@@ -52,6 +52,7 @@ struct Scratch {
 //                 references
 //   66-70         staged row ts / values / counts, row statuses, element_set_consume; element_set_reset (66: the
 //                 datapoints appended                            output rows' starts)
+//   71, 72        staged rows' annotation offsets and entries    element_set_consume_annotated
 enum Slot : int {
   kSlotStreams = 0,
   kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
@@ -118,7 +119,9 @@ enum Slot : int {
   kSlotElemRowN = 68,
   kSlotElemRowStatus = 69,
   kSlotElemRowAppended = 70,
-  kNumSlots = 71
+  kSlotElemRowAnnOff = 71,
+  kSlotElemRowAnn = 72,
+  kNumSlots = 73
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

@@ -2546,6 +2546,18 @@ struct ElemAcc {
   V sum, mn, mx, sq;
   double last;  // Gauge only
   int64_t last_at;
+  // an annotated set's window annotation to slot o: the a_len bytes at p.ann_bytes + a_off (the add's inputs) as whole
+  // 8-byte words, the last one zero-padded (a_len <= ann_cap, a multiple of 8)
+  __device__ static __forceinline__ void store_ann(const ElementParams &p, uint64_t o, uint64_t a_off, uint32_t a_len) {
+    p.ann_len[o] = a_len;
+    uint64_t *dst = reinterpret_cast<uint64_t *>(p.ann_slot + o * p.ann_cap);
+    const uint8_t *src = p.ann_bytes + a_off;
+    for (uint32_t w = 0; w < (a_len + 7u) / 8u; w++) {
+      uint64_t x = 0;
+      for (uint32_t b = 0; b < 8u && w * 8u + b < a_len; b++) x |= (uint64_t)src[w * 8u + b] << (8u * b);
+      dst[w] = x;
+    }
+  }
 };
 template <bool CTR>
 __device__ __forceinline__ void elem_init(ElemAcc<CTR> &a, int64_t ws) {  // NewGauge / NewCounter
@@ -2628,7 +2640,11 @@ __device__ __forceinline__ void elem_update(ElemAcc<CTR> &a, int64_t t, double v
 
 // AddUnion of element s's datapoints in row order.  The window the last datapoint went to stays in registers (in-order
 // data almost never leaves it) and goes back to its slot when a datapoint needs another one, and at the end.
-template <bool CTR>
+// ANN: so does the window's annotation, as a reference (a_off, a_len) into the call's annotation bytes: the last
+// non-empty one of the window's accepted datapoints (MaybeReplaceAnnotation, aggregation/common.go:47-61).  It goes to
+// the slot with the window, and only when it changed (a_dirty): a window opened here always writes its length, 0
+// without an annotation, so a slot never keeps the length of a window it held before.
+template <bool CTR, bool ANN = false>
 __device__ __forceinline__ void elem_add_lane(const ElementParams &p, uint64_t s) {
   const uint32_t n_pts = p.n_points ? p.n_points[s] : (uint32_t)p.points_stride;
   if (n_pts > p.points_stride) {
@@ -2640,6 +2656,13 @@ __device__ __forceinline__ void elem_add_lane(const ElementParams &p, uint64_t s
   elem_init(a, 0);
   int cur = -1;  // the slot `a` belongs to, -1: none
   int32_t status = M3TSZ_OK;
+  uint64_t a_off = 0, ann_i = 0, ann_end = 0;
+  uint32_t a_len = 0;
+  bool a_dirty = false;
+  if (ANN && p.ann_series_off) {
+    ann_i = p.ann_series_off[s];
+    ann_end = p.ann_series_off[s + 1];
+  }
   for (uint32_t i = 0; i < n_pts; i++) {
     const uint64_t at = (uint64_t)i * p.n + s;
     int res = M3TSZ_ERR_CAPACITY;  // (after a CAPACITY, the rest of the element's datapoints)
@@ -2647,10 +2670,21 @@ __device__ __forceinline__ void elem_add_lane(const ElementParams &p, uint64_t s
       const int64_t t = p.ts[at];
       const double v = p.val[at];
       int64_t ws = 0;
+      uint64_t d_off = 0;  // this datapoint's annotation, d_len 0: none
+      uint32_t d_len = 0;
+      if constexpr (ANN) {
+        while (ann_i < ann_end && p.ann_entries[ann_i].dp_index < i) ann_i++;
+        if (ann_i < ann_end && p.ann_entries[ann_i].dp_index == i) {
+          d_off = p.ann_entries[ann_i].byte_offset;
+          d_len = p.ann_entries[ann_i].length;
+        }
+      }
       if (!elem_window_start(t, p.resolution, p.trunc_off, ws)) {
         res = M3TSZ_ERR_INVALID_ARG;
       } else if (elem_ends_by(ws, p.resolution, wm)) {
         res = M3TSZ_ERR_AGGREGATION_CLOSED;
+      } else if (ANN && d_len > p.ann_cap) {
+        status = res = M3TSZ_ERR_CAPACITY;
       } else {
         res = M3TSZ_OK;
         if (cur < 0 || ws != a.start) {  // the window's slot, or a free one
@@ -2668,20 +2702,35 @@ __device__ __forceinline__ void elem_add_lane(const ElementParams &p, uint64_t s
           if (hit < 0 && fr < 0) {
             status = res = M3TSZ_ERR_CAPACITY;
           } else {
-            if (cur >= 0) elem_store(p, (uint64_t)cur * p.n + s, a);
+            if (cur >= 0) {
+              elem_store(p, (uint64_t)cur * p.n + s, a);
+              if (ANN && a_dirty) ElemAcc<CTR>::store_ann(p, (uint64_t)cur * p.n + s, a_off, a_len);
+            }
             cur = hit >= 0 ? hit : fr;
             if (hit >= 0)
               elem_load(p, (uint64_t)hit * p.n + s, a);
             else
               elem_init(a, ws);
+            a_len = 0;
+            a_dirty = hit < 0;
           }
         }
-        if (res == M3TSZ_OK) elem_update(a, t, v);
+        if (res == M3TSZ_OK) {
+          elem_update(a, t, v);
+          if (ANN && d_len) {
+            a_off = d_off;
+            a_len = d_len;
+            a_dirty = true;
+          }
+        }
       }
     }
     p.result[at] = (int8_t)res;
   }
-  if (cur >= 0) elem_store(p, (uint64_t)cur * p.n + s, a);
+  if (cur >= 0) {
+    elem_store(p, (uint64_t)cur * p.n + s, a);
+    if (ANN && a_dirty) ElemAcc<CTR>::store_ann(p, (uint64_t)cur * p.n + s, a_off, a_len);
+  }
   p.status[s] = status;
 }
 
@@ -2690,13 +2739,32 @@ __device__ __forceinline__ void elem_add_lane(const ElementParams &p, uint64_t s
 // type j's datapoints in rows j * n + s of p.row_ts / p.row_val ([p.rows_stride][n_types * n]), their count in
 // p.row_n.  An element whose output rows lack room changes nothing and gets CAPACITY.  `e` is the lane's element record
 // while it runs (the kernel's is in shared memory: xf_element_window indexes its inputs by type).
-template <bool CTR>
+// ANN: every staged datapoint of a window also gets an entry for the append, row i's at row_ann_off[i] =
+// i * rows_stride, referring to the window's slot bytes (length 0 without an annotation, which the append takes as
+// none); an entry past a row's count is never read.
+template <bool CTR, bool ANN = false>
 __device__ __forceinline__ void elem_consume_lane(const ElementParams &p, uint64_t s, XfElem &e) {
   const uint64_t kn = (uint64_t)p.n_types * p.n;
+  // a slot's annotation length (one above the capacity, which the library never stores, reads as none)
+  auto ann_len = [&](uint64_t o) -> uint32_t {
+    const uint32_t l = p.ann_len[o];
+    return l <= p.ann_cap ? l : 0u;
+  };
+  if constexpr (ANN) {
+    for (uint32_t j = 0; j < p.n_types; j++) p.row_ann_off[(uint64_t)j * p.n + s] = ((uint64_t)j * p.n + s) * p.rows_stride;
+    if (s + 1 == p.n) p.row_ann_off[kn] = kn * p.rows_stride;
+  }
   uint32_t m = 0;
+  uint64_t ann_words = 0;  // ANN: the flushed windows' annotations as the append's room check counts them
   for (uint32_t r = 0; r < p.n_slots; r++) {
     const uint64_t o = (uint64_t)r * p.n + s;
-    if (p.count[o] != 0 && elem_ends_by(p.start[o], p.resolution, p.target)) m++;
+    if (p.count[o] != 0 && elem_ends_by(p.start[o], p.resolution, p.target)) {
+      m++;
+      if constexpr (ANN) {
+        const uint32_t l = ann_len(o);
+        if (l) ann_words += (l + 3u) / 4u + 4u;
+      }
+    }
   }
   bool reset = false;
   for (int k = 0; k < M3TSZ_MAX_TRANSFORMS; k++) reset |= ((p.ops >> (4 * k)) & 0xfu) == M3TSZ_TRANSFORM_RESET;
@@ -2704,12 +2772,16 @@ __device__ __forceinline__ void elem_consume_lane(const ElementParams &p, uint64
   if (m) {
     // the append's room check before a row's last datapoint, every earlier one at its worst case (163 bits with a
     // time-unit change, m3tsz_encode_bound_units) after an empty encoder's 64-bit start: stream words so far +
-    // ENC_GUARD + 4 <= slot words
+    // ENC_GUARD + 4 <= slot words.  ANN: each datapoint's annotation adds (len + 3) / 4 + 4 words to its own check
+    // and at most that much to the stream (marker, varint and bytes), so the last check, with every datapoint's
+    // annotation words added, bounds all of them.
     const uint64_t per_row = (uint64_t)m * (reset ? 2u : 1u);
     for (uint32_t j = 0; j < p.n_types; j++) {
       const m3tsz_encoder_state &e = p.out_state[(uint64_t)j * p.n + s];
       const uint64_t bits = e.bits + (e.num_encoded ? 0u : 64u) + (per_row - 1) * 163u;
-      if ((bits >> 5) + ENC_GUARD + 4 > p.out_slot_words) status = M3TSZ_ERR_CAPACITY;
+      uint64_t words = (bits >> 5) + ENC_GUARD + 4;
+      if constexpr (ANN) words += ann_words * (reset ? 2u : 1u);
+      if (words > p.out_slot_words) status = M3TSZ_ERR_CAPACITY;
     }
   }
   if (m == 0 || status != M3TSZ_OK) {
@@ -2742,6 +2814,18 @@ __device__ __forceinline__ void elem_consume_lane(const ElementParams &p, uint64
     const uint64_t o = (uint64_t)best * p.n + s;
     const int64_t c = p.count[o];
     const int64_t t = bs + p.resolution;  // the window's end
+    uint32_t a_len = 0;
+    if constexpr (ANN) a_len = ann_len(o);
+    // ANN: the entry of staged datapoint d of row `row` (the same window annotation for the Reset datapoint)
+    auto stage_ann = [&](uint64_t row, uint64_t d) {
+      if constexpr (ANN) {
+        m3tsz_annotation_entry en;
+        en.dp_index = (uint32_t)d;
+        en.length = a_len;
+        en.byte_offset = o * p.ann_cap;
+        p.row_ann[row * p.rows_stride + d] = en;
+      }
+    };
     xf_element_window(
         p.ops, p.resolution, e, 0u, p.n_types, t,
         [&](uint32_t i) {
@@ -2751,13 +2835,16 @@ __device__ __forceinline__ void elem_consume_lane(const ElementParams &p, uint64
         },
         [&](uint32_t i, double v, int64_t extra_t) {
           if (p.discard_nan && xf_isnan(v)) return;  // nothing of this type's window, its Reset datapoint included
-          uint64_t at = ((rows >> (8 * i)) & 0xffu) * kn + (uint64_t)i * p.n + s;
+          const uint64_t d = (rows >> (8 * i)) & 0xffu;
+          uint64_t at = d * kn + (uint64_t)i * p.n + s;
           p.row_ts[at] = t;
           p.row_val[at] = v;
+          stage_ann((uint64_t)i * p.n + s, d);
           if (extra_t != 0) {
             at += kn;
             p.row_ts[at] = extra_t;
             p.row_val[at] = 0.0;
+            stage_ann((uint64_t)i * p.n + s, d + 1);
           }
           rows += (uint64_t)(extra_t != 0 ? 2u : 1u) << (8 * i);
         });
@@ -2773,16 +2860,16 @@ __device__ __forceinline__ void elem_consume_lane(const ElementParams &p, uint64
 }
 
 constexpr int ELEM_THREADS = 256;
-template <bool CTR>
+template <bool CTR, bool ANN>
 __global__ void __launch_bounds__(ELEM_THREADS) element_add_kernel(const ElementParams p) {
   const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
-  if (s < p.n) elem_add_lane<CTR>(p, s);
+  if (s < p.n) elem_add_lane<CTR, ANN>(p, s);
 }
-template <bool CTR>
+template <bool CTR, bool ANN>
 __global__ void __launch_bounds__(ELEM_THREADS) element_consume_kernel(const ElementParams p) {
   __shared__ XfElem rec[ELEM_THREADS];
   const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
-  if (s < p.n) elem_consume_lane<CTR>(p, s, rec[threadIdx.x]);
+  if (s < p.n) elem_consume_lane<CTR, ANN>(p, s, rec[threadIdx.x]);
 }
 __global__ void element_status_kernel(const int32_t *row_status, uint64_t n, uint32_t n_types, int32_t *status) {
   const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -2801,20 +2888,31 @@ static unsigned elem_blocks(uint64_t n) { return (unsigned)((n + ELEM_THREADS - 
 cudaError_t launch_element_add(const ElementParams &p, cudaStream_t stream) {
   if (p.n == 0) return cudaSuccess;
   if ((p.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
-  if (p.counter)
-    element_add_kernel<true><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  const bool ann = p.ann_len != nullptr;
+  if (p.counter && ann)
+    element_add_kernel<true, true><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  else if (p.counter)
+    element_add_kernel<true, false><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  else if (ann)
+    element_add_kernel<false, true><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
   else
-    element_add_kernel<false><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+    element_add_kernel<false, false><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
 cudaError_t launch_element_consume(const ElementParams &p, cudaStream_t stream) {
   if (p.n == 0) return cudaSuccess;
   if ((p.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
-  if (p.counter)
-    element_consume_kernel<true><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  const bool ann = p.ann_len != nullptr;
+  if (ann && (!p.row_ann_off || !p.row_ann)) return cudaErrorInvalidValue;
+  if (p.counter && ann)
+    element_consume_kernel<true, true><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  else if (p.counter)
+    element_consume_kernel<true, false><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+  else if (ann)
+    element_consume_kernel<false, true><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
   else
-    element_consume_kernel<false><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
+    element_consume_kernel<false, false><<<elem_blocks(p.n), ELEM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

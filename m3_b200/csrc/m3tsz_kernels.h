@@ -376,7 +376,20 @@ struct ElementParams {
   uint64_t rows_stride;
   // the slots as tile_value_of reads them (tile_sum .. tile_count, tile_sum_sq, metric_type)
   EncodeParams tiles;
+  // the annotated calls (ann_len set): each slot's annotation, its length in ann_len [n_slots][n] and slot r of
+  // element s's bytes at (r * n + s) * ann_cap
+  uint32_t *ann_len;
+  uint8_t *ann_slot;
+  uint64_t ann_cap;
+  // add: the call's sparse annotation list (optional; dp_index counts rows of the element's column)
+  const uint64_t *ann_series_off;
+  const m3tsz_annotation_entry *ann_entries;
+  const uint8_t *ann_bytes;
+  // consume: the staged rows' annotations for the append, row i's entries from row_ann_off[i] = i * rows_stride
+  uint64_t *row_ann_off;
+  m3tsz_annotation_entry *row_ann;
 };
+// (the annotated kernels when p.ann_len is set)
 cudaError_t launch_element_add(const ElementParams &p, cudaStream_t stream);
 cudaError_t launch_element_consume(const ElementParams &p, cudaStream_t stream);
 // an element consumed with status OK takes the first failing status of its n_types rows

@@ -5,8 +5,10 @@ template argument, APPEND, to encode_kernel: an old build's <INT_OPT, PACKED, IN
 <INT_OPT, PACKED, IN, false>.  decode_kernel<INT_OPT, MODE> is compared by name; the source-block loop added a third
 argument, BLK, so an old build's <INT_OPT, MODE> is compared with a new build's <INT_OPT, MODE, false>.  The rollup's
 rollup_forward_kernel and rollup_fold_kernel are compared too; the annotated rollup made them templates over ANN, so an
-old build's untemplated kernel is compared with a new build's <false>.  Instantiations only one build has
-(the append mode, new decode modes) are listed, not compared.
+old build's untemplated kernel is compared with a new build's <false>.  The element sets' element_add_kernel<CTR> and
+element_consume_kernel<CTR> are compared too; the annotated element sets added a second argument, ANN, so an old
+build's <CTR> is compared with a new build's <CTR, false>.  Instantiations only one build has (the append mode, new
+decode modes, the annotated element kernels) are listed, not compared.
 
     python scripts/compare_encode_sass.py OLD.(o|so) NEW.(o|so)     # exit code 1 on any difference
 
@@ -32,6 +34,9 @@ def kernels(path):
                 out[cur] = []
             elif "decode_kernel" in name:
                 cur = re.sub(r"(decode_kernelILb[01]ELi[0-9]+E)Lb0E", r"\1", name)
+                out[cur] = []
+            elif "element_add_kernel" in name or "element_consume_kernel" in name:
+                cur = re.sub(r"(element_(?:add|consume)_kernelILb[01]E)Lb0E", r"\1", name)
                 out[cur] = []
             elif "rollup_forward_kernel" in name or "rollup_fold_kernel" in name:
                 cur = re.sub(r"(rollup_(?:forward|fold)_kernel)ILb0EEEvNS_", r"\1ENS_", name)
