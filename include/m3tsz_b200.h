@@ -967,9 +967,13 @@ typedef struct m3tsz_element_set {
   uint8_t *d_out_buf;
   uint64_t out_stride;      /* bytes per output slot, a multiple of 16 */
 } m3tsz_element_set;
+/* A set without output (d_out_state and d_out_buf NULL, out_stride 0) has no encoder set: it is a rollup's source set
+ * (m3tsz_element_set_forward).  reset, add, add_annotated and forward take it and never touch an output;
+ * consume and consume_annotated refuse it (M3TSZ_ERR_INVALID_ARG). */
 
 /* Frees every window, zeroes every record, sets every watermark to INT64_MIN, and resets the output encoder set with
- * d_start [n_elements] (element s's start for all of its rows). */
+ * d_start [n_elements] (element s's start for all of its rows; a set without output reads nothing of d_start, which
+ * may then be NULL). */
 int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
                             const int64_t *d_start, void *stream);
 
@@ -1049,6 +1053,46 @@ int m3tsz_element_set_add_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, c
 int m3tsz_element_set_consume_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
                                         const m3tsz_element_annotations *ann, int64_t target_ns, int32_t out_unit,
                                         int32_t *d_status, void *stream);
+
+/* Element sets through a rollup (the pipeline "transformations, Rollup, remainder", DESIGN.md §4.12): each source's
+ * Consume(target_ns) forwards its windows' values to the groups that list it, and each group takes them through its
+ * rollup element's AddUnique (generic_elem.go:246-281, 912-937).
+ *   - src: the source set, of metric type M, with exactly one aggregation type (the rollup's source type, valid for M
+ *     as in m3tsz_aggregate_tiles_rollup: Counter Sum and Gauge Last are the usual ones), its ops the pipeline's
+ *     transformations before the rollup and its discard_nan the pipeline's.  It needs no output (see above).
+ *   - groups: an element set of the same M and resolution_ns with n_elements == n_groups, its type list the rollup's
+ *     types and its ops the remainder's; m3tsz_element_set_consume consumes it as any other set.
+ *   - group g is the sources d_members[d_group_off[g] .. d_group_off[g + 1]) (n_groups + 1 offsets, n_members
+ *     members), as in m3tsz_aggregate_tiles_rollup: a source may be in several groups, in none, or twice in one.
+ * Rules:
+ *   1. Forward: every source takes its open windows that end at or before target_ns, in ascending start order; each
+ *      window's value is ValueOf(the source type) through the ops on the source's record (a Reset forwards nothing
+ *      extra).  discard_nan drops a NaN value with or without ops (generic_elem.go:892-894): it is not forwarded.
+ *   2. Fold: every group takes its members in listed order, and each member's forwarded windows in start order, into
+ *      the group window with the same start as the source window, opening a slot if needed.  Every value of a window
+ *      arrives at one timestamp, so the fold is m3tsz_aggregate_tiles_rollup's: Gauge Last is the first value, count
+ *      counts NaNs, sum / min / max / sumSq skip them; Counter int64(value) with sums that wrap.  The slot holds the
+ *      result as an add leaves it (a Gauge's last_at is the window's end).  A member listed twice is folded twice.
+ *   3. A group window that ends at or before the group's watermark is closed: its values are dropped and the group
+ *      gets M3TSZ_ERR_AGGREGATION_CLOSED; its other windows still fold.
+ *   4. A group with fewer free slots than new windows gets M3TSZ_ERR_CAPACITY, and nothing is folded into it.
+ *   5. A group whose range decreases or runs past n_members, or that lists a source >= src->n_elements, gets
+ *      M3TSZ_ERR_INVALID_ARG (over CAPACITY), and nothing is folded into it.
+ *   6. Commit: a group that failed with CAPACITY or INVALID_ARG holds back every member its range names (up to
+ *      n_members): such a source keeps its windows, record and watermark, and d_src_status[s] is that group's status
+ *      (INVALID_ARG when groups of both kinds list it).  Every other source frees its due windows, saves its record
+ *      and moves its watermark to the last due window's end, with d_src_status[s] = M3TSZ_OK; a source in no group
+ *      drops its values.  So after growing the groups' open windows, calling again with exactly the failed groups
+ *      (d_group_off / d_members listing only them, the same group set) gives the result of one unstopped call.
+ * d_group_status [n_groups]: M3TSZ_OK or the status above.  The call reads and writes no annotation arrays (an
+ * annotated group set's new windows get no annotation lengths: consume it with the plain consume).  A metric type or
+ * resolution mismatch, a source type list of other than one type, an invalid type or op list, n_groups other than
+ * groups->n_elements, n_members above 2^40, src and groups sharing their slots, or NULL d_group_off / d_members /
+ * statuses where they are needed: M3TSZ_ERR_INVALID_ARG before any launch. */
+int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                              int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
+                              uint64_t n_members, uint64_t n_groups, const m3tsz_element_set *groups,
+                              int32_t *d_src_status, int32_t *d_group_status, void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

@@ -297,7 +297,9 @@ class BatchCodec:
         an encoder set of k * N rows (row j * N + s: element s under agg_types[j]) with slots of `stride` bytes
         (default: room for 128 datapoints per row at their worst case), written with `out_unit`.
         annotation_capacity > 0 (a multiple of 8, at most capi.MAX_ELEMENT_ANNOTATION): the elements keep annotations
-        (m3tsz_element_set_*_annotated), each open window up to that many bytes of its last non-empty one."""
+        (m3tsz_element_set_*_annotated), each open window up to that many bytes of its last non-empty one.
+        stride=0: a set without output rows, a rollup's source set (ElementSet.forward); consume() and stream()
+        refuse it."""
         return ElementSet(self, start, metric_type, agg_types, resolution_ns, transforms, discard_nan, open_windows,
                           stride, out_unit, annotation_capacity)
 
@@ -903,7 +905,7 @@ class ElementSet:
         if stride is None:
             stride = int(capi.lib().m3tsz_encode_bound_units(128, 1))
         start = start.contiguous()
-        self.out = EncoderSet(codec, start.repeat(k), stride)
+        self.out = EncoderSet(codec, start.repeat(k), stride) if stride else None
         self.reset(start)
 
     @property
@@ -926,10 +928,15 @@ class ElementSet:
             setattr(d, "d_win_" + f, w[f].data_ptr() if f in w else None)
         d.d_elem = self.elem.data_ptr()
         d.d_watermark = self.watermark.data_ptr()
-        d.d_out_state = self.out.state.data_ptr()
-        d.d_out_buf = self.out.buf.data_ptr()
-        d.out_stride = self.out.stride
+        if self.out is not None:
+            d.d_out_state = self.out.state.data_ptr()
+            d.d_out_buf = self.out.buf.data_ptr()
+            d.out_stride = self.out.stride
         return d
+
+    def _require_output(self):
+        if self.out is None:
+            raise ValueError("this element set has no output rows (stride=0): it is a rollup's source set")
 
     @property
     def annotation_capacity(self) -> int:
@@ -998,6 +1005,7 @@ class ElementSet:
         """Consume(target_ns): every open window that ended by target_ns, in order, through the element and onto
         the output rows.  Returns status int32 [N]: OK, ERR_CAPACITY (the element's output slots lack room: it is
         unchanged; grow(stride=...) and consume again), or a row's append status."""
+        self._require_output()
         dev = self.codec.device
         status = torch.empty(self.n_elements, dtype=torch.int32, device=dev)
         d = self._desc()
@@ -1038,12 +1046,41 @@ class ElementSet:
                              device=self.ann_bytes.device)
             by[:, :, : self.annotation_capacity] = self.ann_bytes
             self.ann_bytes = by
-        if stride is not None and stride != self.out.stride:
-            self.out.grow(stride)
+        if stride is not None:
+            self._require_output()
+            if stride != self.out.stride:
+                self.out.grow(stride)
 
     def stream(self) -> EncodeResult:
         """The output rows' snapshot (EncoderSet.stream): row j * N + s is element s under agg_types[j]."""
+        self._require_output()
         return self.out.stream()
+
+    def forward(self, target_ns, group_off: torch.Tensor, members: torch.Tensor, groups: "ElementSet"):
+        """This set as a rollup's source set (m3tsz_element_set_forward, DESIGN.md §4.12): every element's open
+        windows that ended by target_ns go, through ValueOf of the set's one type and its transformations, to the
+        groups that list it; group g of `groups` (an ElementSet of the same metric type and resolution, one element
+        per group, without annotations) takes the values of the sources members[group_off[g] .. group_off[g + 1])
+        (int64 [G + 1] and int32 [n] device tensors, as aggregate_tiles_rollup takes them), in that order, into its
+        window with the source window's start.  Returns (source statuses int32 [N]: OK, or the status of a failed
+        group that held the source back; group statuses int32 [G]: OK, ERR_AGGREGATION_CLOSED -- a window that ended
+        by the group's watermark was dropped --, ERR_CAPACITY -- too few open windows: groups.grow(open_windows=...)
+        and forward again with exactly the failed groups --, or ERR_INVALID_ARG)."""
+        assert isinstance(groups, ElementSet) and groups.ann_len is None, "the group set keeps no annotations"
+        assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
+        assert members.is_cuda and members.dtype == torch.int32 and members.is_contiguous()
+        G = group_off.numel() - 1
+        assert G >= 0, "group_off has G + 1 entries"
+        dev = self.codec.device
+        src_status = torch.empty(max(1, self.n_elements), dtype=torch.int32, device=dev)
+        group_status = torch.empty(max(1, G), dtype=torch.int32, device=dev)
+        d, gd = self._desc(), groups._desc()
+        rc = capi.lib().m3tsz_element_set_forward(
+            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), int(target_ns), _ptr(group_off),
+            _ptr(members), members.numel(), G, C.byref(gd), _ptr(src_status), _ptr(group_status),
+            _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_forward")
+        return src_status[: self.n_elements], group_status[:G]
 
     def state(self):
         """Copies of the element-side state: {"win": {field: [R, N]}, "elem": uint8 [N, 160], "watermark": [N]},

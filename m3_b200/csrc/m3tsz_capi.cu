@@ -1225,6 +1225,9 @@ int m3tsz_aggregate_tiles_rollup_annotated(
 // ---- element sets (DESIGN.md §4.12) ----
 // The checks every element-set call makes on the set (its element as m3tsz_aggregate_tiles_types checks one, its
 // arrays' presence and alignment), and the parameters the kernels read; xf takes the parsed lists.
+static bool element_set_no_output(const m3tsz_element_set *set) {
+  return !set->d_out_state && !set->d_out_buf && set->out_stride == 0;
+}
 static bool element_params(const m3tsz_options *opts, const m3tsz_element_set *set, ElementParams &p,
                            TileTransforms &xf) {
   if (!valid_opts(opts) || !set || set->reserved != 0) return false;
@@ -1238,8 +1241,12 @@ static bool element_params(const m3tsz_options *opts, const m3tsz_element_set *s
   auto a16 = [](const void *q) { return q && !((uintptr_t)q & 15u); };
   if (!a8(e.d_win_start) || !a8(e.d_win_count) || !a8(e.d_win_sum) || !a8(e.d_win_min) || !a8(e.d_win_max) ||
       !a8(e.d_win_sum_sq) || (!counter && (!a8(e.d_win_last) || !a8(e.d_win_last_at))) || !a16(e.d_elem) ||
-      !a8(e.d_watermark) || !a16(e.d_out_state) || !a16(e.d_out_buf) || (e.out_stride & 15u) || e.out_stride == 0 ||
-      e.out_stride > (1ull << 33))
+      !a8(e.d_watermark))
+    return false;
+  // a set without output (NULL output arrays, out_stride 0) is a rollup's source set: every call but the consume
+  // takes it
+  if (!element_set_no_output(set) && (!a16(e.d_out_state) || !a16(e.d_out_buf) || (e.out_stride & 15u) ||
+                                      e.out_stride == 0 || e.out_stride > (1ull << 33)))
     return false;
   memset(&p, 0, sizeof(p));
   p.n = e.n_elements;
@@ -1281,7 +1288,8 @@ int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3t
                             const int64_t *d_start, void *stream) {
   ElementParams p;
   TileTransforms xf;
-  if (!ctx || !element_params(opts, set, p, xf) || (p.n && !d_start)) return M3TSZ_ERR_INVALID_ARG;
+  if (!ctx || !element_params(opts, set, p, xf) || (p.n && !d_start && !element_set_no_output(set)))
+    return M3TSZ_ERR_INVALID_ARG;
   if (p.n == 0) return M3TSZ_OK;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
@@ -1291,6 +1299,8 @@ int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3t
     if (a) CK(cudaMemsetAsync(a, 0, wb, st));
   CK(cudaMemsetAsync(p.elem, 0, p.n * sizeof(m3tsz_element_state), st));
   CK(launch_fill_i64(p.watermark, INT64_MIN, p.n, st));
+  ctx->launches++;
+  if (element_set_no_output(set)) return M3TSZ_OK;
   // row j * n + s of the output starts at element s's start
   const uint64_t kn = (uint64_t)p.n_types * p.n;
   void *d_rs = nullptr;
@@ -1300,7 +1310,7 @@ int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3t
     CK(cudaMemcpyAsync((int64_t *)d_rs + (uint64_t)j * p.n, d_start, p.n * 8, cudaMemcpyDeviceToDevice, st));
   CK(launch_encoder_set_reset(set->d_out_state, kn, (const int64_t *)d_rs, opts->default_time_unit,
                               opts->int_optimized != 0, st));
-  ctx->launches += 2;
+  ctx->launches++;
   return M3TSZ_OK;
 }
 
@@ -1376,7 +1386,8 @@ static int element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
                                int32_t *d_status, void *stream, bool annotated) {
   ElementParams p;
   TileTransforms xf;
-  if (!ctx || !element_params(opts, set, p, xf) || !unit_is_valid(out_unit)) return M3TSZ_ERR_INVALID_ARG;
+  if (!ctx || !element_params(opts, set, p, xf) || element_set_no_output(set) || !unit_is_valid(out_unit))
+    return M3TSZ_ERR_INVALID_ARG;
   if (annotated && !element_ann_params(ann, p)) return M3TSZ_ERR_INVALID_ARG;
   if (p.n == 0) return M3TSZ_OK;
   if (!d_status || ((uintptr_t)d_status & 3u)) return M3TSZ_ERR_INVALID_ARG;
@@ -1437,6 +1448,73 @@ int m3tsz_element_set_consume_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
                                         const m3tsz_element_annotations *ann, int64_t target_ns, int32_t out_unit,
                                         int32_t *d_status, void *stream) {
   return element_set_consume(ctx, opts, set, ann, target_ns, out_unit, d_status, stream, true);
+}
+
+// The forward kernel writes each source's due windows to scratch, the fold kernel folds them into the groups' windows
+// and marks the members of the groups that failed, and the commit kernel frees the other sources' due windows
+int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                              int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
+                              uint64_t n_members, uint64_t n_groups, const m3tsz_element_set *groups,
+                              int32_t *d_src_status, int32_t *d_group_status, void *stream) {
+  ElementRollupParams rp;
+  memset(&rp, 0, sizeof(rp));
+  ElementParams gp;
+  TileTransforms sx, gx;
+  if (!ctx || !element_params(opts, src, rp.src, sx) || !element_params(opts, groups, gp, gx)) return M3TSZ_ERR_INVALID_ARG;
+  if (src->metric_type != groups->metric_type || src->resolution_ns != groups->resolution_ns || sx.n_types != 1 ||
+      src->d_win_start == groups->d_win_start || n_groups != groups->n_elements || n_members > (1ull << 40) ||
+      (n_groups && !d_group_off) || (n_members && !d_members) || ((uintptr_t)d_group_off & 7u) ||
+      ((uintptr_t)d_members & 3u))
+    return M3TSZ_ERR_INVALID_ARG;
+  const uint64_t S = rp.src.n;
+  if ((S && (!d_src_status || ((uintptr_t)d_src_status & 3u))) ||
+      (n_groups && (!d_group_status || ((uintptr_t)d_group_status & 3u))))
+    return M3TSZ_ERR_INVALID_ARG;
+  if (S == 0 && n_groups == 0) return M3TSZ_OK;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  cudaStream_t st = (cudaStream_t)stream;
+  const uint64_t sn = S ? S : 1;  // (the fold reads nothing of the sources when there are none)
+  void *d_fs, *d_fv, *d_fn, *d_fp, *d_fd, *d_rec, *d_mark;
+  int rc;
+  if ((rc = ensure(ctx, kSlotElemFwdStart, (size_t)sn * rp.src.n_slots * 8, &d_fs))) return rc;
+  if ((rc = ensure(ctx, kSlotElemFwdVal, (size_t)sn * rp.src.n_slots * 8, &d_fv))) return rc;
+  if ((rc = ensure(ctx, kSlotElemFwdN, sn * 4, &d_fn))) return rc;
+  if ((rc = ensure(ctx, kSlotElemFwdPresent, sn * 8, &d_fp))) return rc;
+  if ((rc = ensure(ctx, kSlotElemFwdDue, sn * 8, &d_fd))) return rc;
+  if ((rc = ensure(ctx, kSlotElemFwdRec, sn * sizeof(m3tsz_transform_state), &d_rec))) return rc;
+  if ((rc = ensure(ctx, kSlotElemFwdMark, sn * 4, &d_mark))) return rc;
+  rp.src.target = target_ns;
+  rp.discard_nan = src->discard_nan ? 1 : 0;  // (generic_elem.go:892-894: with or without transformations)
+  rp.fwd_start = (int64_t *)d_fs;
+  rp.fwd_val = (double *)d_fv;
+  rp.fwd_n = (uint32_t *)d_fn;
+  rp.fwd_present = (uint64_t *)d_fp;
+  rp.fwd_due = (uint64_t *)d_fd;
+  rp.rec = (m3tsz_transform_state *)d_rec;
+  rp.group_off = d_group_off;
+  rp.members = d_members;
+  rp.n_members = n_members;
+  rp.n_groups = n_groups;
+  rp.g_slots = gp.n_slots;
+  rp.g_start = gp.start;
+  rp.g_count = gp.count;
+  rp.g_sum = gp.sum;
+  rp.g_min = gp.min;
+  rp.g_max = gp.max;
+  rp.g_sum_sq = gp.sum_sq;
+  rp.g_last = gp.last;
+  rp.g_last_at = gp.last_at;
+  rp.g_watermark = gp.watermark;
+  rp.group_status = d_group_status;
+  rp.mark = (int32_t *)d_mark;
+  rp.src_status = d_src_status;
+  CK(cudaMemsetAsync(d_mark, 0, sn * 4, st));
+  CK(launch_element_forward(rp, st));
+  CK(launch_element_fold(rp, st));
+  CK(launch_element_commit(rp, st));
+  ctx->launches += 3;
+  return M3TSZ_OK;
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

@@ -53,6 +53,9 @@ struct Scratch {
 //   66-70         staged row ts / values / counts, row statuses, element_set_consume; element_set_reset (66: the
 //                 datapoints appended                            output rows' starts)
 //   71, 72        staged rows' annotation offsets and entries    element_set_consume_annotated
+//   73-79         forwarded window starts / values, due-window   element_set_forward
+//                 counts, presence and slot words, source
+//                 records, source marks
 enum Slot : int {
   kSlotStreams = 0,
   kSlotSeriesIndex = 1,  // per-series index input: stream offsets, or the encoder starts
@@ -121,7 +124,15 @@ enum Slot : int {
   kSlotElemRowAppended = 70,
   kSlotElemRowAnnOff = 71,
   kSlotElemRowAnn = 72,
-  kNumSlots = 73
+  // element sets through a rollup
+  kSlotElemFwdStart = 73,
+  kSlotElemFwdVal = 74,
+  kSlotElemFwdN = 75,
+  kSlotElemFwdPresent = 76,
+  kSlotElemFwdDue = 77,
+  kSlotElemFwdRec = 78,
+  kSlotElemFwdMark = 79,
+  kNumSlots = 80
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

@@ -2925,6 +2925,332 @@ cudaError_t launch_element_status(const int32_t *row_status, uint64_t n, uint32_
 }
 
 // ---------------------------------------------------------------------------
+// element sets through a rollup (DESIGN.md §4.12): forward, fold, commit
+// ---------------------------------------------------------------------------
+// Consume(target) of source s of a rollup pipeline (generic_elem.go:912-937): its windows ending at or before
+// p.src.target, in start order as elem_consume_lane selects them, each through tile_value_of of the source's one type
+// and the pre-ops on the record's head (xf_element_window with one type is xf_window on it; a Reset forwards nothing
+// extra).  The q-th window's start and value go to fwd_start / fwd_val at q * n + s, and bit q of fwd_present says
+// the value is forwarded (discard_nan drops a NaN with or without ops, as processValue does).  The slots, record and
+// watermark stay as they are: the commit frees the due slots (fwd_due) and saves the record (rec) unless a failed
+// group holds the source back.
+template <bool CTR>
+__device__ __forceinline__ void elem_forward_lane(const ElementRollupParams &p, uint64_t s) {
+  const ElementParams &e = p.src;
+  uint32_t m = 0;
+  uint64_t due = 0;
+  for (uint32_t r = 0; r < e.n_slots; r++) {
+    const uint64_t o = (uint64_t)r * e.n + s;
+    if (e.count[o] != 0 && elem_ends_by(e.start[o], e.resolution, e.target)) {
+      m++;
+      due |= 1ull << r;
+    }
+  }
+  m3tsz_transform_state st = e.elem[s].head;
+  uint64_t present = 0;
+  int64_t prev = 0;
+  for (uint32_t q = 0; q < m; q++) {
+    int best = -1;  // the next due window in start order (starts are distinct)
+    int64_t bs = 0;
+    for (uint32_t r = 0; r < e.n_slots; r++) {
+      if (!((due >> r) & 1u)) continue;
+      const int64_t ws = e.start[(uint64_t)r * e.n + s];
+      if (q && ws <= prev) continue;
+      if (best < 0 || ws < bs) {
+        best = (int)r;
+        bs = ws;
+      }
+    }
+    prev = bs;
+    const uint64_t o = (uint64_t)best * e.n + s;
+    double v = tile_value_of(e.tiles, CTR, (int)(e.types & 0xfu), o, e.count[o]);
+    int64_t extra_t = 0;
+    xf_window(e.ops, e.resolution, st, bs + e.resolution, v, extra_t);
+    if (!(p.discard_nan && xf_isnan(v))) present |= 1ull << q;
+    p.fwd_start[(uint64_t)q * e.n + s] = bs;
+    p.fwd_val[(uint64_t)q * e.n + s] = v;
+  }
+  p.fwd_n[s] = m;
+  p.fwd_present[s] = present;
+  p.fwd_due[s] = due;
+  p.rec[s] = st;
+}
+
+// A group window while the fold holds it: its start and the rollup fold's accumulator (every value arrives at one
+// timestamp, so rollup_gauge_add / rollup_counter_add: the first value is Last, NaNs are counted, sums wrap), loaded
+// from and stored to the slot form elem_store writes (a Gauge window without a non-NaN value has min = max =
+// math.NaN(), which is the fold's own empty form; last_at is the window's end, where the values arrive)
+template <bool CTR>
+struct ElemFoldAcc {
+  using A = std::conditional_t<CTR, RollupCounterAcc, RollupGaugeAcc>;
+  int64_t start;
+  A a;
+};
+template <bool CTR>
+__device__ __forceinline__ void elem_fold_load(const ElementRollupParams &p, uint64_t o, ElemFoldAcc<CTR> &f) {
+  f.start = p.g_start[o];
+  f.a.cnt = p.g_count[o];
+  if constexpr (CTR) {
+    f.a.sum = static_cast<const int64_t *>(p.g_sum)[o];
+    f.a.mn = static_cast<const int64_t *>(p.g_min)[o];
+    f.a.mx = static_cast<const int64_t *>(p.g_max)[o];
+    f.a.sq = static_cast<const int64_t *>(p.g_sum_sq)[o];
+  } else {
+    f.a.sum = static_cast<const double *>(p.g_sum)[o];
+    f.a.mn = static_cast<const double *>(p.g_min)[o];
+    f.a.mx = static_cast<const double *>(p.g_max)[o];
+    f.a.sq = static_cast<const double *>(p.g_sum_sq)[o];
+    f.a.last = p.g_last[o];
+  }
+}
+template <bool CTR>
+__device__ __forceinline__ void elem_fold_store(const ElementRollupParams &p, uint64_t o, const ElemFoldAcc<CTR> &f) {
+  using V = std::conditional_t<CTR, int64_t, double>;
+  p.g_start[o] = f.start;
+  p.g_count[o] = f.a.cnt;
+  static_cast<V *>(p.g_sum)[o] = f.a.sum;
+  static_cast<V *>(p.g_min)[o] = f.a.mn;
+  static_cast<V *>(p.g_max)[o] = f.a.mx;
+  static_cast<V *>(p.g_sum_sq)[o] = f.a.sq;
+  if constexpr (!CTR) {
+    p.g_last[o] = f.a.last;
+    p.g_last_at[o] = (int64_t)((uint64_t)f.start + (uint64_t)p.src.resolution);
+  }
+}
+
+// What the fold reads of the member at one listed position: its source index, its due windows, which of them are
+// forwarded, and its first due window's start and value (later ones are read from fwd_start / fwd_val)
+struct FwdMember {
+  uint64_t m;  // >= src.n: an invalid index (n = 0)
+  uint32_t n;
+  uint64_t present;
+  int64_t start0;
+  double val0;
+};
+__device__ __forceinline__ FwdMember fwd_member(const ElementRollupParams &p, uint64_t i) {
+  FwdMember a;
+  a.m = p.members[i];
+  a.n = 0;
+  a.present = 0;
+  a.start0 = 0;
+  a.val0 = 0.0;
+  if (a.m < p.src.n) {
+    a.n = p.fwd_n[a.m];
+    a.present = p.fwd_present[a.m];
+    if (a.n) {
+      a.start0 = p.fwd_start[a.m];
+      a.val0 = p.fwd_val[a.m];
+    }
+  }
+  return a;
+}
+
+// AddUnique of group g's members in listed order (generic_elem.go:246-281), each member's forwarded windows in start
+// order, into the group window with the source window's start.  member(i) gives listed position i (lo <= i < hi),
+// asked for in order.  First a pass that checks the range and the indices (INVALID_ARG) and counts the group's new
+// windows against its free slots (CAPACITY): a failed group changes nothing.  Then the fold, the current window in
+// registers (it goes back to its slot when a value needs another one, and at the end); a window that ends at or
+// before the group's watermark is dropped (AGGREGATION_CLOSED, the other windows still fold).  fresh: room for
+// g_slots starts.  Returns the group's status (also written to group_status[g]).
+template <bool CTR, class Member>
+__device__ __forceinline__ int32_t elem_fold_group(const ElementRollupParams &p, uint64_t g, int64_t *fresh,
+                                                   Member member) {
+  const uint64_t lo = p.group_off[g], hi = p.group_off[g + 1], G = p.n_groups;
+  const int64_t res = p.src.resolution, wm = p.g_watermark[g];
+  int32_t status = M3TSZ_OK;
+  auto window = [&](const FwdMember &a, uint32_t q, int64_t &ws, double &v) {
+    if (q == 0) {
+      ws = a.start0;
+      v = a.val0;
+    } else {
+      ws = p.fwd_start[(uint64_t)q * p.src.n + a.m];
+      v = p.fwd_val[(uint64_t)q * p.src.n + a.m];
+    }
+  };
+  if (lo > hi || hi > p.n_members) {
+    status = M3TSZ_ERR_INVALID_ARG;
+  } else {
+    uint32_t n_free = 0, n_fresh = 0;
+    for (uint32_t r = 0; r < p.g_slots; r++) n_free += p.g_count[(uint64_t)r * G + g] == 0;
+    bool bad = false, full = false, seen = false;
+    int64_t last = 0;  // the last start checked (a group's values mostly go to one window)
+    for (uint64_t i = lo; i < hi; i++) {
+      const FwdMember a = member(i);
+      if (a.m >= p.src.n) bad = true;
+      for (uint32_t q = 0; q < a.n; q++) {
+        if (!((a.present >> q) & 1u)) continue;
+        int64_t ws;
+        double v;
+        window(a, q, ws, v);
+        if ((seen && ws == last) || elem_ends_by(ws, res, wm)) continue;
+        seen = true;
+        last = ws;
+        bool known = false;
+        for (uint32_t r = 0; r < p.g_slots && !known; r++) {
+          const uint64_t o = (uint64_t)r * G + g;
+          known = p.g_count[o] != 0 && p.g_start[o] == ws;
+        }
+        for (uint32_t k = 0; k < n_fresh && !known; k++) known = fresh[k] == ws;
+        if (known) continue;
+        if (n_fresh < n_free)
+          fresh[n_fresh++] = ws;
+        else
+          full = true;
+      }
+    }
+    status = bad ? M3TSZ_ERR_INVALID_ARG : full ? M3TSZ_ERR_CAPACITY : M3TSZ_OK;
+  }
+  if (status == M3TSZ_OK) {
+    ElemFoldAcc<CTR> f;
+    int cur = -1;  // the slot `f` belongs to, -1: none
+    bool closed = false;
+    for (uint64_t i = lo; i < hi; i++) {
+      const FwdMember a = member(i);
+      for (uint32_t q = 0; q < a.n; q++) {
+        if (!((a.present >> q) & 1u)) continue;
+        int64_t ws;
+        double v;
+        window(a, q, ws, v);
+        if (elem_ends_by(ws, res, wm)) {
+          closed = true;
+          continue;
+        }
+        if (cur < 0 || ws != f.start) {  // the window's slot, or a free one (the first pass counted them)
+          if (cur >= 0) elem_fold_store(p, (uint64_t)cur * G + g, f);
+          int hit = -1, fr = -1;
+          for (uint32_t r = 0; r < p.g_slots; r++) {
+            const uint64_t o = (uint64_t)r * G + g;
+            if (p.g_count[o] == 0) {
+              if (fr < 0) fr = (int)r;
+            } else if (p.g_start[o] == ws) {
+              hit = (int)r;
+              break;
+            }
+          }
+          cur = hit >= 0 ? hit : fr;
+          if (hit >= 0) {
+            elem_fold_load(p, (uint64_t)hit * G + g, f);
+          } else {
+            f.start = ws;
+            if constexpr (CTR)
+              rollup_counter_init(f.a);
+            else
+              rollup_gauge_init(f.a);
+          }
+        }
+        if constexpr (CTR)
+          rollup_counter_add(f.a, v);
+        else
+          rollup_gauge_add(f.a, v);
+      }
+    }
+    if (cur >= 0) elem_fold_store(p, (uint64_t)cur * G + g, f);
+    if (closed) status = M3TSZ_ERR_AGGREGATION_CLOSED;
+  }
+  p.group_status[g] = status;
+  return status;
+}
+
+// The commit of source s: a source that a failed group holds back (mark[s], that group's status) keeps its windows,
+// record and watermark; every other one frees its due slots, saves its new record and moves its watermark to the last
+// due window's end
+__device__ __forceinline__ void elem_commit_lane(const ElementRollupParams &p, uint64_t s) {
+  const int32_t mk = p.mark[s];
+  p.src_status[s] = mk;
+  const uint32_t m = p.fwd_n[s];
+  if (mk != 0 || m == 0) return;
+  const uint64_t due = p.fwd_due[s];
+  for (uint32_t r = 0; r < p.src.n_slots; r++)
+    if ((due >> r) & 1u) p.src.count[(uint64_t)r * p.src.n + s] = 0;
+  p.src.watermark[s] = p.fwd_start[(uint64_t)(m - 1) * p.src.n + s] + p.src.resolution;
+  p.src.elem[s].head = p.rec[s];
+}
+
+template <bool CTR>
+__global__ void __launch_bounds__(ELEM_THREADS) element_forward_kernel(const ElementRollupParams p) {
+  const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (s < p.src.n) elem_forward_lane<CTR>(p, s);
+}
+
+// One warp per group.  The lanes gather 32 listed members at a time (their indices as one coalesced load, their due
+// counts, presence words and first forwarded windows as one gather); every lane then runs the group's fold on the
+// same values, shuffled from the lane that loaded them, so the fold is in listed order and its branches are uniform.
+// The lanes' stores to the group's slots are of equal values.  A group that failed with CAPACITY or INVALID_ARG marks
+// the members its range names for the commit.
+constexpr int ELEM_FOLD_WARPS = 8;
+template <bool CTR>
+__global__ void __launch_bounds__(ELEM_FOLD_WARPS * 32) element_fold_kernel(const ElementRollupParams p) {
+  __shared__ int64_t fresh[ELEM_FOLD_WARPS][M3TSZ_MAX_ELEMENT_WINDOWS];
+  const uint32_t lane = threadIdx.x & 31u, wi = threadIdx.x >> 5;
+  const uint64_t g = (uint64_t)blockIdx.x * ELEM_FOLD_WARPS + wi;
+  if (g >= p.n_groups) return;
+  const uint64_t lo = p.group_off[g], hi = p.group_off[g + 1];
+  uint64_t base = ~0ull;
+  FwdMember mine;
+  auto member = [&](uint64_t i) {
+    const uint64_t b = lo + ((i - lo) & ~31ull);
+    if (b != base) {
+      base = b;
+      mine.m = ~0ull;
+      mine.n = 0;
+      mine.present = 0;
+      mine.start0 = 0;
+      mine.val0 = 0.0;
+      if (b + lane < hi) mine = fwd_member(p, b + lane);
+    }
+    const int j = (int)((i - lo) & 31u);
+    FwdMember a;
+    a.m = __shfl_sync(FULL_MASK, mine.m, j);
+    a.n = __shfl_sync(FULL_MASK, mine.n, j);
+    a.present = __shfl_sync(FULL_MASK, mine.present, j);
+    a.start0 = __shfl_sync(FULL_MASK, mine.start0, j);
+    a.val0 = __shfl_sync(FULL_MASK, mine.val0, j);
+    return a;
+  };
+  const int32_t st = elem_fold_group<CTR>(p, g, fresh[wi], member);
+  if ((st == M3TSZ_ERR_CAPACITY || st == M3TSZ_ERR_INVALID_ARG) && lo <= hi) {
+    const uint64_t end = hi < p.n_members ? hi : p.n_members;
+    for (uint64_t i = lo + lane; i < end; i += 32) {
+      const uint32_t m = p.members[i];
+      if (m < p.src.n) atomicMax(p.mark + m, st);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(ELEM_THREADS) element_commit_kernel(const ElementRollupParams p) {
+  const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (s < p.src.n) elem_commit_lane(p, s);
+}
+
+cudaError_t launch_element_forward(const ElementRollupParams &p, cudaStream_t stream) {
+  if (p.src.n == 0) return cudaSuccess;
+  if ((p.src.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  if (p.src.counter)
+    element_forward_kernel<true><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
+  else
+    element_forward_kernel<false><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_element_fold(const ElementRollupParams &p, cudaStream_t stream) {
+  if (p.n_groups == 0) return cudaSuccess;
+  const uint64_t blocks = (p.n_groups + ELEM_FOLD_WARPS - 1) / ELEM_FOLD_WARPS;
+  if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
+  if (p.src.counter)
+    element_fold_kernel<true><<<(unsigned)blocks, ELEM_FOLD_WARPS * 32, 0, stream>>>(p);
+  else
+    element_fold_kernel<false><<<(unsigned)blocks, ELEM_FOLD_WARPS * 32, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_element_commit(const ElementRollupParams &p, cudaStream_t stream) {
+  if (p.src.n == 0) return cudaSuccess;
+  if ((p.src.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  element_commit_kernel<<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------
 // compaction: slots -> packed buffer with CSR offsets
 // ---------------------------------------------------------------------------
 __global__ void compact_lens_kernel(const uint64_t *len, uint64_t n, uint64_t mask, uint64_t *out) {

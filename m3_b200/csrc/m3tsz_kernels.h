@@ -396,6 +396,40 @@ cudaError_t launch_element_consume(const ElementParams &p, cudaStream_t stream);
 cudaError_t launch_element_status(const int32_t *row_status, uint64_t n, uint32_t n_types, int32_t *status,
                                   cudaStream_t stream);
 
+// element sets through a rollup (m3tsz_element_set_forward; m3tsz_encode.cu): the source set's forward (one lane per
+// source), the fold into the group set's windows (one warp per group) and the sources' commit (one lane per source)
+struct ElementRollupParams {
+  ElementParams src;  // the source set: its slots, records and watermarks, target, ops and its one type (types)
+  int discard_nan;    // the source side drops a NaN forwarded value with or without ops
+  // the forward's output: the q-th due window of source s (start order) at q * src.n + s, window-major
+  // [src.n_slots][src.n]; per source the number of due windows, which of them forward a value (bit q), which slots
+  // they are in (bit r) and the new record
+  int64_t *fwd_start;
+  double *fwd_val;
+  uint32_t *fwd_n;
+  uint64_t *fwd_present, *fwd_due;
+  m3tsz_transform_state *rec;
+  // the groups: group g is the sources members[group_off[g] .. group_off[g + 1])
+  const uint64_t *group_off;
+  const uint32_t *members;
+  uint64_t n_members, n_groups;
+  // the group set's slots, window-slot major [g_slots][n_groups], and watermarks
+  uint32_t g_slots;
+  int64_t *g_start, *g_count;
+  void *g_sum, *g_min, *g_max, *g_sum_sq;
+  double *g_last;
+  int64_t *g_last_at;
+  const int64_t *g_watermark;
+  int32_t *group_status;
+  // the commit: mark[s] is the largest status of a failed group listing s (0: none)
+  int32_t *mark;
+  int32_t *src_status;
+};
+cudaError_t launch_element_forward(const ElementRollupParams &p, cudaStream_t stream);
+// (p.mark must be zero)
+cudaError_t launch_element_fold(const ElementRollupParams &p, cudaStream_t stream);
+cudaError_t launch_element_commit(const ElementRollupParams &p, cudaStream_t stream);
+
 // exclusive scan of aligned lengths + gather into a packed buffer
 cudaError_t launch_compact(const uint8_t *slots, uint64_t slot_stride, const uint64_t *len,
                            uint64_t n_series, uint32_t align, uint8_t *packed,
