@@ -16,8 +16,34 @@
  * owns every buffer; the library owns only scratch held by an explicit
  * m3tsz_ctx.  "d_" pointers are CUDA device pointers, "h_" pointers are host
  * pointers.  `stream` is a cudaStream_t passed as void* (NULL = default stream).
- * Device entry points are asynchronous on `stream`; host entry points
- * synchronise before returning.
+ * Device entry points are asynchronous on `stream`: every launch and copy of the
+ * call is on `stream`, and the call returns before it runs, except as listed
+ * below.  Host entry points synchronise before returning.
+ *
+ * Streams and one context.  One context may serve device calls on several
+ * streams.  The context's scratch belongs to the context, not to a stream, so
+ * the calls that use it (the tile calls, m3tsz_decode_downsample_ex and
+ * m3tsz_decode_downsample_last_batch with a NULL lastAt / sumSq / last output,
+ * m3tsz_encode_batch_packed(_ex), m3tsz_compact_streams,
+ * m3tsz_encoder_set_write, m3tsz_element_set_reset of a set with output rows,
+ * m3tsz_element_set_consume(_annotated), m3tsz_element_set_forward) are
+ * ordered in the order they are issued: each one's stream waits on the device
+ * for the context's previous such call, whatever stream that was on.  Two such
+ * calls on one context therefore never overlap; a caller who wants them to
+ * overlap uses two contexts.  A *_host call (and a streaming handle's call)
+ * waits for the context's earlier device calls of this kind before it touches
+ * the scratch.  The other device calls take no part in this ordering.
+ * Batch calls on one context must still come from one host thread at a time:
+ * the scratch and this ordering are not locked.
+ *
+ * Device entry points that block the host until their stream reaches a point of
+ * the call (each one's comment says so too): m3tsz_compact_streams,
+ * m3tsz_aggregate_tiles_annotated, m3tsz_aggregate_tiles_blocks (with
+ * annotations) and m3tsz_aggregate_tiles_rollup_annotated.
+ *
+ * Besides those, a scratch-using call that has to grow a scratch slot (the first
+ * call at a larger size) waits on the host for the context's previous
+ * scratch-using call to finish before it frees the smaller buffer.
  *
  * Bit-exactness contract: encoded streams are byte-identical to what the
  * reference m3tsz encoder produces for the same (start, datapoints, units,
@@ -402,7 +428,9 @@ int m3tsz_encode_batch_packed_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
  * d_offsets[n_series+1] (exclusive prefix sum of d_out_len, each start rounded
  * up to `align` bytes, align in {1,4,8,16,32,64}) and copies the bytes.  64-byte
  * aligned starts let the decoder's lanes read their staging rings in phase (fewer
- * shared-memory bank conflicts); any alignment decodes to the same result. */
+ * shared-memory bank conflicts); any alignment decodes to the same result.
+ * Blocks the host: it reads the capacity flag back, so it returns once `stream`
+ * has run the whole call. */
 int m3tsz_compact_streams(m3tsz_ctx *ctx, const uint8_t *d_slots, uint64_t slot_stride,
                           const uint64_t *d_len, uint64_t n_series, uint32_t align,
                           uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_offsets,
@@ -784,7 +812,9 @@ int m3tsz_aggregate_tiles_types(m3tsz_ctx *ctx, const m3tsz_options *opts, const
  * Limits: a window's annotation is kept on the device as (bit offset from the stream's first
  * bit) << 32 | length in bytes; a stream of 2^28 bytes or more, whose offsets would not fit, is
  * already refused by the decode (M3TSZ_ERR_STREAM_TOO_LARGE on all of its rows).
- * Sources without annotations give exactly m3tsz_aggregate_tiles_types' outputs. */
+ * Sources without annotations give exactly m3tsz_aggregate_tiles_types' outputs.
+ * Blocks the host: it waits for `stream` to reach the 8-byte read of the longest source
+ * stream (after the fused decode), then issues the encode stage and returns. */
 int m3tsz_aggregate_tiles_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                                     uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
                                     uint64_t n_series, int64_t start_ns, int64_t step_ns, uint32_t n_windows,
@@ -825,7 +855,9 @@ int m3tsz_aggregate_tiles_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, c
  * payload from d_streams' first bit) << 27 | length in bytes, so a series in which a datapoint
  * carries an annotation of 2^27 bytes or more gets M3TSZ_ERR_STREAM_TOO_LARGE on all its rows.
  * d_block_off NULL, or any check of m3tsz_aggregate_tiles_types: M3TSZ_ERR_INVALID_ARG before
- * any launch. */
+ * any launch.
+ * With annotations this call blocks the host, as m3tsz_aggregate_tiles_annotated does (the
+ * read of the largest sum); without, it does not. */
 int m3tsz_aggregate_tiles_blocks(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
                                  uint64_t streams_bytes, const uint64_t *d_offsets, const uint64_t *d_lengths,
                                  uint64_t n_segments, const uint64_t *d_block_off, uint64_t n_series, int64_t start_ns,
@@ -912,7 +944,9 @@ int m3tsz_aggregate_tiles_rollup(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
  *     groups of the members' source stream lengths (summed over their blocks); a row that does
  *     not fit gets M3TSZ_ERR_CAPACITY.  Every encode scratch slot takes that room, so one wide
  *     group raises the call's device scratch (DESIGN.md §4.8); a call that cannot allocate it
- *     returns M3TSZ_ERR_CUDA. */
+ *     returns M3TSZ_ERR_CUDA.
+ *   - Blocks the host: with rows to write it waits for `stream` to reach the read of that room
+ *     (after the fold), then issues the encode stage and returns. */
 int m3tsz_aggregate_tiles_rollup_annotated(
     m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams, uint64_t streams_bytes,
     const uint64_t *d_offsets, const uint64_t *d_lengths, uint64_t n_segments, const uint64_t *d_block_off,

@@ -83,15 +83,16 @@ static bool encode_params(const m3tsz_options *opts, const int64_t *d_ts, const 
 
 // Packed mode: the kernel encodes into a set of context slots of slot_bytes each and appends
 // every finished stream at an `align`ed cursor (*d_total_bytes, zeroed by the caller) in d_packed.
-static int packed_params(m3tsz_ctx *ctx, uint64_t n_series, uint64_t slot_bytes, uint32_t align,
+static int packed_params(m3tsz_ctx *ctx, const ScratchFence &fence, uint64_t n_series, uint64_t slot_bytes,
+                         uint32_t align,
                          uint8_t *d_packed, uint64_t packed_capacity, uint64_t *d_offsets,
                          uint64_t *d_total_bytes, cudaStream_t st, EncodeParams &p) {
   const uint64_t slots = encode_packed_scratch_slots(n_series);
   if (slots == 0) return set_cuda_error(ctx, cudaGetLastError(), "encode_packed_scratch_slots");
   void *scratch = nullptr, *ctr = nullptr;
   int rc;
-  if ((rc = ensure(ctx, kSlotPackedSlots, slots * slot_bytes, &scratch))) return rc;
-  if ((rc = ensure(ctx, kSlotBatchCounter, 64, &ctr))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotPackedSlots, slots * slot_bytes, &scratch))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotBatchCounter, 64, &ctr))) return rc;
   CK(cudaMemsetAsync(ctr, 0, 64, st));
   p.out = (uint8_t *)scratch;
   p.out_stride = slot_bytes;
@@ -154,6 +155,7 @@ int m3tsz_ctx_create(int device, m3tsz_ctx **out) {
       cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess ||
       cudaStreamCreateWithFlags(&ctx->stream2, cudaStreamNonBlocking) != cudaSuccess ||
       cudaEventCreateWithFlags(&ctx->ev, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&ctx->scratch_ev, cudaEventDisableTiming) != cudaSuccess ||
       cudaMalloc(&ctx->d_flag, 2 * sizeof(int32_t)) != cudaSuccess) {
     (void)cudaGetLastError();
     delete ctx;
@@ -172,6 +174,7 @@ void m3tsz_ctx_destroy(m3tsz_ctx *ctx) {
   for (int i = 0; i < 2; i++)
     if (ctx->h_stage[i]) cudaFreeHost(ctx->h_stage[i]);
   if (ctx->ev) cudaEventDestroy(ctx->ev);
+  if (ctx->scratch_ev) cudaEventDestroy(ctx->scratch_ev);
   if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
@@ -258,9 +261,10 @@ static int downsample_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
     return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx, (cudaStream_t)stream, want_last && !d_last_at);
   if (want_last && !d_last_at) {  // lastAt lives in context scratch
     void *sc = nullptr;
-    int rc = ensure(ctx, kSlotWinLastAt, (size_t)n_series * n_windows * 8, &sc);
+    int rc = ensure(ctx, fence, kSlotWinLastAt, (size_t)n_series * n_windows * 8, &sc);
     if (rc) return rc;
     d_last_at = (int64_t *)sc;
   }
@@ -308,6 +312,8 @@ int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
     return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx, (cudaStream_t)stream,
+                     gauge ? (!o->d_last || !o->d_last_at) : !o->d_counter_sum_sq);
   // what the caller leaves out but the kernel keeps (to re-open a committed window exactly) lives in scratch
   const size_t wb = (size_t)n_series * n_windows * 8;
   void *sc = nullptr;
@@ -324,11 +330,11 @@ int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
     p.ds_last = o->d_last;
     p.ds_last_at = o->d_last_at;
     if (!p.ds_last) {
-      if ((rc = ensure(ctx, kSlotWinLast, wb, &sc))) return rc;
+      if ((rc = ensure(ctx, fence, kSlotWinLast, wb, &sc))) return rc;
       p.ds_last = (double *)sc;
     }
     if (!p.ds_last_at) {
-      if ((rc = ensure(ctx, kSlotWinLastAt, wb, &sc))) return rc;
+      if ((rc = ensure(ctx, fence, kSlotWinLastAt, wb, &sc))) return rc;
       p.ds_last_at = (int64_t *)sc;
     }
   } else {
@@ -337,7 +343,7 @@ int m3tsz_decode_downsample_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
     p.ds_imax = o->d_counter_max;
     p.ds_isum_sq = o->d_counter_sum_sq;
     if (!p.ds_isum_sq) {
-      if ((rc = ensure(ctx, kSlotWinSumSq, wb, &sc))) return rc;
+      if ((rc = ensure(ctx, fence, kSlotWinSumSq, wb, &sc))) return rc;
       p.ds_isum_sq = (int64_t *)sc;
     }
   }
@@ -490,11 +496,12 @@ int m3tsz_encoder_set_write(m3tsz_ctx *ctx, const m3tsz_options *opts, m3tsz_enc
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   const cudaStream_t st = (cudaStream_t)stream;
+  ScratchFence fence(ctx, st);
   void *target = nullptr, *touched = nullptr, *count = nullptr;
   int rc;
-  if ((rc = ensure(ctx, kSlotRouteTarget, n_series * points_stride, &target))) return rc;
-  if ((rc = ensure(ctx, kSlotRouteTouched, pool_capacity * sizeof(RouteTouched), &touched))) return rc;
-  if ((rc = ensure(ctx, kSlotRouteCount, sizeof(uint32_t), &count))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotRouteTarget, n_series * points_stride, &target))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotRouteTouched, pool_capacity * sizeof(RouteTouched), &touched))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotRouteCount, sizeof(uint32_t), &count))) return rc;
   CK(cudaMemsetAsync(count, 0, sizeof(uint32_t), st));
   RouteParams r;
   memset(&r, 0, sizeof(r));
@@ -576,6 +583,7 @@ int m3tsz_encode_batch_packed_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   cudaStream_t st = (cudaStream_t)stream;
+  ScratchFence fence(ctx, st);
   CK(cudaMemsetAsync(d_total_bytes, 0, sizeof(uint64_t), st));
   if (n_series == 0) return M3TSZ_OK;
   EncodeParams p;
@@ -586,7 +594,7 @@ int m3tsz_encode_batch_packed_ex(m3tsz_ctx *ctx, const m3tsz_options *opts, cons
   if (slot_bytes == 0) slot_bytes = m3tsz_encode_bound_units(points_stride, d_units != nullptr);
   slot_bytes = (slot_bytes + 15) & ~15ull;
   if (slot_bytes > (1ull << 33)) return M3TSZ_ERR_INVALID_ARG;
-  int rc = packed_params(ctx, n_series, slot_bytes, align, d_packed, packed_capacity, d_offsets, d_total_bytes,
+  int rc = packed_params(ctx, fence, n_series, slot_bytes, align, d_packed, packed_capacity, d_offsets, d_total_bytes,
                          st, p);
   if (rc) return rc;
   CK(launch_encode(p, opts->int_optimized != 0, st));
@@ -603,9 +611,10 @@ int m3tsz_compact_streams(m3tsz_ctx *ctx, const uint8_t *d_slots, uint64_t slot_
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   cudaStream_t st = (cudaStream_t)stream;
+  ScratchFence fence(ctx, st);  // (scratch, and d_flag)
   size_t tmp_bytes = compact_scan_tmp_bytes(n_series);
   void *tmp = nullptr;
-  int rc = ensure(ctx, kSlotCompactTmp, tmp_bytes, &tmp);
+  int rc = ensure(ctx, fence, kSlotCompactTmp, tmp_bytes, &tmp);
   if (rc) return rc;
   CK(cudaMemsetAsync(ctx->d_flag, 0, sizeof(int32_t), st));
   CK(launch_compact(d_slots, slot_stride, d_len, n_series, align, d_packed, packed_capacity,
@@ -705,7 +714,8 @@ static bool needs_sum_sq(bool counter, const int32_t *types, uint32_t n) {
 // Step 1 of every tile call: the fused decode + windows of the sources: the Gauge with `last` (mode 2), + sumSq if a
 // type needs it (mode 4), or the Counter (mode 5, its int64 sum / min / max in the Gauge's slots); xf.annotated:
 // + each window's annotation reference (modes 6-8).
-static int tiles_decode(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams, uint64_t streams_bytes,
+static int tiles_decode(m3tsz_ctx *ctx, const ScratchFence &fence, const m3tsz_options *opts,
+                        const uint8_t *d_streams, uint64_t streams_bytes,
                         const uint64_t *d_offsets, const uint64_t *d_lengths, uint64_t n_series, int64_t start_ns,
                         int64_t step_ns, uint32_t n_windows, bool counter, const TileTransforms &xf, cudaStream_t st,
                         TileWindows &w) {
@@ -715,16 +725,16 @@ static int tiles_decode(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t
   const bool sq = needs_sum_sq(counter, xf.types, xf.n_types);
   const size_t wb = (size_t)n_series * n_windows * 8;
   int rc;
-  if ((rc = ensure(ctx, kSlotWinSum, wb, &w.sum))) return rc;
-  if ((rc = ensure(ctx, kSlotWinCount, wb, &w.cnt))) return rc;
-  if ((rc = ensure(ctx, kSlotWinMin, wb, &w.min))) return rc;
-  if ((rc = ensure(ctx, kSlotWinMax, wb, &w.max))) return rc;
-  if ((rc = ensure(ctx, kSlotWinLastAt, wb, &w.lat))) return rc;
-  if ((rc = ensure(ctx, kSlotWinLast, wb, &w.last))) return rc;
-  if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &w.np))) return rc;
-  if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &w.sst))) return rc;
-  if (xf.annotated && (rc = ensure(ctx, kSlotWinAnn, wb, &w.ann))) return rc;
-  if (sq && (rc = ensure(ctx, kSlotWinSumSq, wb, &w.sq))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinSum, wb, &w.sum))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinCount, wb, &w.cnt))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinMin, wb, &w.min))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinMax, wb, &w.max))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinLastAt, wb, &w.lat))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinLast, wb, &w.last))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotNPoints, n_series * 4, &w.np))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotStatus, n_series * 4, &w.sst))) return rc;
+  if (xf.annotated && (rc = ensure(ctx, fence, kSlotWinAnn, wb, &w.ann))) return rc;
+  if (sq && (rc = ensure(ctx, fence, kSlotWinSumSq, wb, &w.sq))) return rc;
   p.n_points = (uint32_t *)w.np;
   p.status = (int32_t *)w.sst;
   p.range_start = start_ns;
@@ -774,10 +784,11 @@ static void tile_inputs(EncodeParams &p, bool counter, const TileWindows &w) {
 // or launch_group_max_stream_len) into a zeroed device word, which is read back.
 extern "C++" {
 template <typename Launch>
-static int annotation_room(m3tsz_ctx *ctx, cudaStream_t st, const Launch &launch, uint64_t &room) {
+static int annotation_room(m3tsz_ctx *ctx, const ScratchFence &fence, cudaStream_t st, const Launch &launch,
+                           uint64_t &room) {
   void *d_mx = nullptr;
   int rc;
-  if ((rc = ensure(ctx, kSlotSrcMaxLen, 8, &d_mx))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotSrcMaxLen, 8, &d_mx))) return rc;
   CK(cudaMemsetAsync(d_mx, 0, 8, st));
   CK(launch((unsigned long long *)d_mx));
   ctx->launches++;
@@ -793,7 +804,8 @@ static int annotation_room(m3tsz_ctx *ctx, cudaStream_t st, const Launch &launch
 // streams d_streams, and every slot adds ann_room bytes for them (annotation_room).  The references w.ann hold the
 // payload's bit offset in its stream, whose byte offset is d_offsets[source], or, with xf.block_off or a NULL
 // d_offsets, in the whole batch.
-static int tiles_encode(m3tsz_ctx *ctx, const m3tsz_options *opts, const TileWindows &w, uint64_t n_src,
+static int tiles_encode(m3tsz_ctx *ctx, const ScratchFence &fence, const m3tsz_options *opts, const TileWindows &w,
+                        uint64_t n_src,
                         int64_t start_ns, int64_t step_ns, uint32_t n_windows, int32_t metric_type, int32_t out_unit,
                         const TileTransforms &xf, const uint8_t *d_streams, const uint64_t *d_offsets,
                         uint64_t ann_room, const TileOutputs &out, cudaStream_t st) {
@@ -807,15 +819,15 @@ static int tiles_encode(m3tsz_ctx *ctx, const m3tsz_options *opts, const TileWin
   if (xf.annotated) slot_bytes = (slot_bytes + ann_room + 15) & ~15ull;
   EncodeParams p;
   memset(&p, 0, sizeof(p));
-  if ((rc = packed_params(ctx, n_rows, slot_bytes, out.align, out.packed, out.capacity, out.offsets,
+  if ((rc = packed_params(ctx, fence, n_rows, slot_bytes, out.align, out.packed, out.capacity, out.offsets,
                           out.total_bytes, st, p)))
     return rc;
   // every row's encoder starts at the tile range's start (the target block's start)
   void *d_es = nullptr, *d_rec = nullptr;
-  if ((rc = ensure(ctx, kSlotTileStarts, n_rows * 8, &d_es))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotTileStarts, n_rows * 8, &d_es))) return rc;
   CK(launch_fill_i64((int64_t *)d_es, start_ns, n_rows, st));
   // lanes write their parts of each source's new element record to scratch; the status pass commits whole records
-  if (xf.elem_state && (rc = ensure(ctx, kSlotElementScratch, n_src * sizeof(m3tsz_element_state), &d_rec)))
+  if (xf.elem_state && (rc = ensure(ctx, fence, kSlotElementScratch, n_src * sizeof(m3tsz_element_state), &d_rec)))
     return rc;
   p.n_series = n_rows;
   p.points_stride = n_windows;
@@ -876,20 +888,21 @@ static int aggregate_tiles_impl(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   if (!valid_packing(out) || !valid_windows(start_ns, step_ns, n_windows)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx, st);
   TileWindows win;
   int rc;
-  if ((rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
+  if ((rc = tiles_decode(ctx, fence, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns, step_ns,
                          n_windows, metric_type == M3TSZ_METRIC_COUNTER, xf, st, win)))
     return rc;
   // the longest source stream of the call (over source blocks: the largest sum of a series' block lengths)
   uint64_t room = 0;
-  if (xf.annotated && (rc = annotation_room(ctx, st, [&](unsigned long long *mx) {
+  if (xf.annotated && (rc = annotation_room(ctx, fence, st, [&](unsigned long long *mx) {
         return launch_max_stream_len(d_offsets, d_lengths, xf.block_off, n_series, xf.n_segments, streams_bytes, mx,
                                      st);
       }, room)))
     return rc;
-  return tiles_encode(ctx, opts, win, n_series, start_ns, step_ns, n_windows, metric_type, out_unit, xf, d_streams,
-                      d_offsets, room, out, st);
+  return tiles_encode(ctx, fence, opts, win, n_series, start_ns, step_ns, n_windows, metric_type, out_unit, xf,
+                      d_streams, d_offsets, room, out, st);
 }
 
 // aggregation.Type.IsValidForGauge / IsValidForCounter, src/metrics/aggregation/type.go:178-196
@@ -1078,6 +1091,7 @@ static int aggregate_tiles_rollup_impl(m3tsz_ctx *ctx, const m3tsz_options *opts
   cudaStream_t st = (cudaStream_t)stream;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx, st);
   const bool counter = metric_type == M3TSZ_METRIC_COUNTER;
   int rc;
   // 1. fused decode + windows of the sources under their one type
@@ -1087,16 +1101,16 @@ static int aggregate_tiles_rollup_impl(m3tsz_ctx *ctx, const m3tsz_options *opts
   pre.n_segments = n_segments;
   pre.annotated = annotated;
   TileWindows win;
-  if (n_series && (rc = tiles_decode(ctx, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series, start_ns,
-                                     step_ns, n_windows, counter, pre, st, win)))
+  if (n_series && (rc = tiles_decode(ctx, fence, opts, d_streams, streams_bytes, d_offsets, d_lengths, n_series,
+                                     start_ns, step_ns, n_windows, counter, pre, st, win)))
     return rc;
   // 2. forward stage: series-major forwarded values and presence words, each source's new record to scratch
   const uint32_t n_words = (n_windows + 31) / 32;
   void *d_fwd, *d_pres, *d_srec, *d_mark;
-  if ((rc = ensure(ctx, kSlotFwdVal, (size_t)n_series * n_windows * 8, &d_fwd))) return rc;
-  if ((rc = ensure(ctx, kSlotFwdPresent, (size_t)n_series * n_words * 4, &d_pres))) return rc;
-  if ((rc = ensure(ctx, kSlotSrcRecScratch, n_series * sizeof(m3tsz_transform_state), &d_srec))) return rc;
-  if ((rc = ensure(ctx, kSlotSrcMark, n_series, &d_mark))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotFwdVal, (size_t)n_series * n_windows * 8, &d_fwd))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotFwdPresent, (size_t)n_series * n_words * 4, &d_pres))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotSrcRecScratch, n_series * sizeof(m3tsz_transform_state), &d_srec))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotSrcMark, n_series, &d_mark))) return rc;
   RollupForwardParams fp;
   memset(&fp, 0, sizeof(fp));
   tile_inputs(fp.tiles, counter, win);
@@ -1116,7 +1130,7 @@ static int aggregate_tiles_rollup_impl(m3tsz_ctx *ctx, const m3tsz_options *opts
   fp.present = (uint32_t *)d_pres;
   void *d_apres = nullptr;
   if (annotated) {
-    if ((rc = ensure(ctx, kSlotFwdAnnPresent, (size_t)n_series * n_words * 4, &d_apres))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotFwdAnnPresent, (size_t)n_series * n_words * 4, &d_apres))) return rc;
     fp.ann = (uint64_t *)win.ann;
     fp.src_off = d_block_off ? nullptr : d_offsets;  // (the block decode's references are batch-addressed already)
     fp.src_status_out = (int32_t *)win.sst;
@@ -1127,15 +1141,15 @@ static int aggregate_tiles_rollup_impl(m3tsz_ctx *ctx, const m3tsz_options *opts
   // 3. fold: the groups' window-major aggregates, in the fused decode's representation, and their statuses
   const size_t gb = (size_t)n_groups * n_windows * 8;
   TileWindows grp;
-  if ((rc = ensure(ctx, kSlotGroupSum, gb, &grp.sum))) return rc;
-  if ((rc = ensure(ctx, kSlotGroupCount, gb, &grp.cnt))) return rc;
-  if ((rc = ensure(ctx, kSlotGroupMin, gb, &grp.min))) return rc;
-  if ((rc = ensure(ctx, kSlotGroupMax, gb, &grp.max))) return rc;
-  if (!counter && (rc = ensure(ctx, kSlotGroupLast, gb, &grp.last))) return rc;
-  if (needs_sum_sq(counter, rollup_types, n_rollup_types) && (rc = ensure(ctx, kSlotGroupSumSq, gb, &grp.sq)))
+  if ((rc = ensure(ctx, fence, kSlotGroupSum, gb, &grp.sum))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotGroupCount, gb, &grp.cnt))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotGroupMin, gb, &grp.min))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotGroupMax, gb, &grp.max))) return rc;
+  if (!counter && (rc = ensure(ctx, fence, kSlotGroupLast, gb, &grp.last))) return rc;
+  if (needs_sum_sq(counter, rollup_types, n_rollup_types) && (rc = ensure(ctx, fence, kSlotGroupSumSq, gb, &grp.sq)))
     return rc;
-  if ((rc = ensure(ctx, kSlotGroupStatus, n_groups * 4, &grp.sst))) return rc;
-  if (annotated && (rc = ensure(ctx, kSlotGroupAnn, gb, &grp.ann))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotGroupStatus, n_groups * 4, &grp.sst))) return rc;
+  if (annotated && (rc = ensure(ctx, fence, kSlotGroupAnn, gb, &grp.ann))) return rc;
   RollupFoldParams gp;
   memset(&gp, 0, sizeof(gp));
   gp.fwd = (const double *)d_fwd;
@@ -1168,12 +1182,12 @@ static int aggregate_tiles_rollup_impl(m3tsz_ctx *ctx, const m3tsz_options *opts
   post.annotated = annotated;
   uint64_t room = 0;
   if (annotated && (uint64_t)n_rollup_types * n_groups != 0 &&
-      (rc = annotation_room(ctx, st, [&](unsigned long long *mx) {
+      (rc = annotation_room(ctx, fence, st, [&](unsigned long long *mx) {
          return launch_group_max_stream_len(d_offsets, d_lengths, d_block_off, n_series, n_segments, streams_bytes,
                                             d_group_off, d_members, n_members, n_groups, mx, st);
        }, room)))
     return rc;
-  if ((rc = tiles_encode(ctx, opts, grp, n_groups, start_ns, step_ns, n_windows, metric_type, out_unit, post,
+  if ((rc = tiles_encode(ctx, fence, opts, grp, n_groups, start_ns, step_ns, n_windows, metric_type, out_unit, post,
                          d_streams, nullptr, room, out, st)))
     return rc;
   // 5. the source records: a source is saved when it decoded and every group that lists it was saved
@@ -1294,6 +1308,7 @@ int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3t
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   cudaStream_t st = (cudaStream_t)stream;
+  ScratchFence fence(ctx, st, !element_set_no_output(set));  // (the output rows' starts)
   const size_t wb = (size_t)p.n * p.n_slots * 8;
   for (void *a : {(void *)p.start, (void *)p.count, p.sum, p.min, p.max, p.sum_sq, (void *)p.last, (void *)p.last_at})
     if (a) CK(cudaMemsetAsync(a, 0, wb, st));
@@ -1305,7 +1320,7 @@ int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3t
   const uint64_t kn = (uint64_t)p.n_types * p.n;
   void *d_rs = nullptr;
   int rc;
-  if ((rc = ensure(ctx, kSlotElemRowTs, kn * 8, &d_rs))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowTs, kn * 8, &d_rs))) return rc;
   for (uint32_t j = 0; j < p.n_types; j++)
     CK(cudaMemcpyAsync((int64_t *)d_rs + (uint64_t)j * p.n, d_start, p.n * 8, cudaMemcpyDeviceToDevice, st));
   CK(launch_encoder_set_reset(set->d_out_state, kn, (const int64_t *)d_rs, opts->default_time_unit,
@@ -1394,19 +1409,20 @@ static int element_set_consume(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   cudaStream_t st = (cudaStream_t)stream;
+  ScratchFence fence(ctx, st);
   const uint64_t kn = (uint64_t)p.n_types * p.n;
   const uint64_t rows = (uint64_t)p.n_slots * (xf.reset ? 2u : 1u);  // a Reset op writes two datapoints per window
   void *d_ts = nullptr, *d_val = nullptr, *d_n = nullptr, *d_rst = nullptr, *d_app = nullptr;
   int rc;
-  if ((rc = ensure(ctx, kSlotElemRowTs, kn * rows * 8, &d_ts))) return rc;
-  if ((rc = ensure(ctx, kSlotElemRowVal, kn * rows * 8, &d_val))) return rc;
-  if ((rc = ensure(ctx, kSlotElemRowN, kn * 4, &d_n))) return rc;
-  if ((rc = ensure(ctx, kSlotElemRowStatus, kn * 4, &d_rst))) return rc;
-  if ((rc = ensure(ctx, kSlotElemRowAppended, kn * 4, &d_app))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowTs, kn * rows * 8, &d_ts))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowVal, kn * rows * 8, &d_val))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowN, kn * 4, &d_n))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowStatus, kn * 4, &d_rst))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowAppended, kn * 4, &d_app))) return rc;
   if (annotated) {
     void *d_aoff = nullptr, *d_aent = nullptr;
-    if ((rc = ensure(ctx, kSlotElemRowAnnOff, (kn + 1) * 8, &d_aoff))) return rc;
-    if ((rc = ensure(ctx, kSlotElemRowAnn, kn * rows * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotElemRowAnnOff, (kn + 1) * 8, &d_aoff))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotElemRowAnn, kn * rows * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
     p.row_ann_off = (uint64_t *)d_aoff;
     p.row_ann = (m3tsz_annotation_entry *)d_aent;
   }
@@ -1474,16 +1490,17 @@ int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   cudaStream_t st = (cudaStream_t)stream;
+  ScratchFence fence(ctx, st);
   const uint64_t sn = S ? S : 1;  // (the fold reads nothing of the sources when there are none)
   void *d_fs, *d_fv, *d_fn, *d_fp, *d_fd, *d_rec, *d_mark;
   int rc;
-  if ((rc = ensure(ctx, kSlotElemFwdStart, (size_t)sn * rp.src.n_slots * 8, &d_fs))) return rc;
-  if ((rc = ensure(ctx, kSlotElemFwdVal, (size_t)sn * rp.src.n_slots * 8, &d_fv))) return rc;
-  if ((rc = ensure(ctx, kSlotElemFwdN, sn * 4, &d_fn))) return rc;
-  if ((rc = ensure(ctx, kSlotElemFwdPresent, sn * 8, &d_fp))) return rc;
-  if ((rc = ensure(ctx, kSlotElemFwdDue, sn * 8, &d_fd))) return rc;
-  if ((rc = ensure(ctx, kSlotElemFwdRec, sn * sizeof(m3tsz_transform_state), &d_rec))) return rc;
-  if ((rc = ensure(ctx, kSlotElemFwdMark, sn * 4, &d_mark))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdStart, (size_t)sn * rp.src.n_slots * 8, &d_fs))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdVal, (size_t)sn * rp.src.n_slots * 8, &d_fv))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdN, sn * 4, &d_fn))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdPresent, sn * 8, &d_fp))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdDue, sn * 8, &d_fd))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdRec, sn * sizeof(m3tsz_transform_state), &d_rec))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdMark, sn * 4, &d_mark))) return rc;
   rp.src.target = target_ns;
   rp.discard_nan = src->discard_nan ? 1 : 0;  // (generic_elem.go:892-894: with or without transformations)
   rp.fwd_start = (int64_t *)d_fs;
@@ -1610,17 +1627,18 @@ int m3tsz_decode_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uin
   if (!h_streams || !h_offsets || !h_ts || !h_val || max_points == 0) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx);  // (after earlier device calls on this context, whatever their streams)
   DrainStreams drain{ctx};
   void *d_streams, *d_off, *d_ts, *d_val, *d_n, *d_st, *d_unit = nullptr, *d_ann = nullptr;
   int rc;
-  if ((rc = ensure(ctx, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
-  if ((rc = ensure(ctx, kSlotSeriesIndex, (n_series + 1) * 8, &d_off))) return rc;
-  if ((rc = ensure(ctx, kSlotTs, n_series * max_points * 8, &d_ts))) return rc;
-  if ((rc = ensure(ctx, kSlotVal, n_series * max_points * 8, &d_val))) return rc;
-  if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_n))) return rc;
-  if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_st))) return rc;
-  if (h_unit && (rc = ensure(ctx, kSlotUnit, n_series, &d_unit))) return rc;
-  if (h_ann && (rc = ensure(ctx, kSlotAnnRefs, n_series * sizeof(m3tsz_annotation_ref), &d_ann))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotSeriesIndex, (n_series + 1) * 8, &d_off))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotTs, n_series * max_points * 8, &d_ts))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotVal, n_series * max_points * 8, &d_val))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotNPoints, n_series * 4, &d_n))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotStatus, n_series * 4, &d_st))) return rc;
+  if (h_unit && (rc = ensure(ctx, fence, kSlotUnit, n_series, &d_unit))) return rc;
+  if (h_ann && (rc = ensure(ctx, fence, kSlotAnnRefs, n_series * sizeof(m3tsz_annotation_ref), &d_ann))) return rc;
   // Chunked pipeline over two streams: the H2D copy of chunk c+1 overlaps the
   // kernel and the D2H copy of chunk c (PCIe is full duplex).
   cudaStream_t sts[2] = {ctx->stream, ctx->stream2};
@@ -1671,19 +1689,20 @@ int m3tsz_decode_downsample_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts
   if (!h_streams || !h_offsets || !h_sum || !h_count || !h_min || !h_max) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx);  // (after earlier device calls on this context, whatever their streams)
   DrainStreams drain{ctx};
   cudaStream_t st = ctx->stream;
   const size_t wb = (size_t)n_series * n_windows * 8;
   void *d_streams, *d_off, *d_sum, *d_cnt, *d_min, *d_max, *d_n, *d_st;
   int rc;
-  if ((rc = ensure(ctx, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
-  if ((rc = ensure(ctx, kSlotSeriesIndex, (n_series + 1) * 8, &d_off))) return rc;
-  if ((rc = ensure(ctx, kSlotWinSum, wb, &d_sum))) return rc;
-  if ((rc = ensure(ctx, kSlotWinCount, wb, &d_cnt))) return rc;
-  if ((rc = ensure(ctx, kSlotWinMin, wb, &d_min))) return rc;
-  if ((rc = ensure(ctx, kSlotWinMax, wb, &d_max))) return rc;
-  if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_n))) return rc;
-  if ((rc = ensure(ctx, kSlotStatus, n_series * 4, &d_st))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotSeriesIndex, (n_series + 1) * 8, &d_off))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinSum, wb, &d_sum))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinCount, wb, &d_cnt))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinMin, wb, &d_min))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotWinMax, wb, &d_max))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotNPoints, n_series * 4, &d_n))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotStatus, n_series * 4, &d_st))) return rc;
   CK(cudaMemcpyAsync(d_streams, h_streams, streams_bytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_off, h_offsets, (n_series + 1) * 8, cudaMemcpyHostToDevice, st));
   rc = m3tsz_decode_downsample_batch(ctx, opts, (const uint8_t *)d_streams, streams_bytes,
@@ -1717,6 +1736,7 @@ int m3tsz_encode_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const int
   if (!valid_align(align)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx);  // (after earlier device calls on this context, whatever their streams)
   DrainStreams drain{ctx};
   cudaStream_t sts[2] = {ctx->stream, ctx->stream2};
   const uint64_t ann_total = h_ann_series_off ? ann_bytes_len + 16 * h_ann_series_off[n_series] : 0;
@@ -1726,18 +1746,18 @@ int m3tsz_encode_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const int
   int rc;
   // whole-batch device inputs that are small: start, n_points, annotations
   void *d_start, *d_np = nullptr, *d_aoff = nullptr, *d_aent = nullptr, *d_abytes = nullptr;
-  if ((rc = ensure(ctx, kSlotSeriesIndex, (n_series + 1) * 8, &d_start))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotSeriesIndex, (n_series + 1) * 8, &d_start))) return rc;
   CK(cudaMemcpyAsync(d_start, h_start, n_series * 8, cudaMemcpyHostToDevice, sts[0]));
   if (h_n_points) {
-    if ((rc = ensure(ctx, kSlotNPoints, n_series * 4, &d_np))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotNPoints, n_series * 4, &d_np))) return rc;
     CK(cudaMemcpyAsync(d_np, h_n_points, n_series * 4, cudaMemcpyHostToDevice, sts[0]));
   }
   if (h_ann_series_off) {
     if (!h_ann_entries || (!h_ann_bytes && ann_bytes_len)) return M3TSZ_ERR_INVALID_ARG;
     const uint64_t n_ent = h_ann_series_off[n_series];
-    if ((rc = ensure(ctx, kSlotAnnSeriesOff, (n_series + 1) * 8, &d_aoff))) return rc;
-    if ((rc = ensure(ctx, kSlotAnnEntries, n_ent * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
-    if ((rc = ensure(ctx, kSlotAnnBytes, ann_bytes_len, &d_abytes))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotAnnSeriesOff, (n_series + 1) * 8, &d_aoff))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotAnnEntries, n_ent * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotAnnBytes, ann_bytes_len, &d_abytes))) return rc;
     CK(cudaMemcpyAsync(d_aoff, h_ann_series_off, (n_series + 1) * 8, cudaMemcpyHostToDevice, sts[0]));
     if (n_ent)
       CK(cudaMemcpyAsync(d_aent, h_ann_entries, n_ent * sizeof(m3tsz_annotation_entry),
@@ -1759,15 +1779,15 @@ int m3tsz_encode_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const int
   for (int i = 0; i < 2; i++) {
     ln[i].units = nullptr;
     ln[i].busy = false;
-    if ((rc = ensure(ctx, lane_slot(i, 0), ch * row_bytes, &ln[i].ts))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 1), ch * row_bytes, &ln[i].val))) return rc;
-    if (h_units && (rc = ensure(ctx, lane_slot(i, 2), ch * points_stride, &ln[i].units))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 3), ch * out_stride, &ln[i].out))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 4), ch * 8, &ln[i].len))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 5), ch * 4, &ln[i].st))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 6), ch * packed_stride + 64, &ln[i].packed))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 7), (ch + 1) * 8, &ln[i].off))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 8), tmp_bytes, &ln[i].tmp))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 0), ch * row_bytes, &ln[i].ts))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 1), ch * row_bytes, &ln[i].val))) return rc;
+    if (h_units && (rc = ensure(ctx, fence, lane_slot(i, 2), ch * points_stride, &ln[i].units))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 3), ch * out_stride, &ln[i].out))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 4), ch * 8, &ln[i].len))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 5), ch * 4, &ln[i].st))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 6), ch * packed_stride + 64, &ln[i].packed))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 7), (ch + 1) * 8, &ln[i].off))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 8), tmp_bytes, &ln[i].tmp))) return rc;
     if ((rc = ensure_stage(ctx, i, (ch + 1) * 8 + 8))) return rc;
   }
   CK(cudaMemsetAsync(ctx->d_flag, 0, 2 * sizeof(int32_t), sts[0]));
@@ -1856,6 +1876,7 @@ int m3tsz_fetch_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
     return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx);  // (after earlier device calls on this context, whatever their streams)
   DrainStreams drain{ctx};
   cudaStream_t sts[2] = {ctx->stream, ctx->stream2};
   // series per chunk: ~8 chunks, whole sequences of whole series
@@ -1883,22 +1904,22 @@ int m3tsz_fetch_batch_host(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint
   }
   void *d_streams, *d_off;
   int rc;
-  if ((rc = ensure(ctx, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
-  if ((rc = ensure(ctx, kSlotSeriesIndex, (n_seq + 1) * 8, &d_off))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotStreams, streams_bytes + 16, &d_streams))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotSeriesIndex, (n_seq + 1) * 8, &d_off))) return rc;
   struct Lane {
     void *ts, *val, *n, *st, *meta, *ots, *oval, *on, *ost;
   } ln[2];
   const size_t meta_words = (max_k + 1) + (max_r + 1) + (ch + 1);
   for (int i = 0; i < 2; i++) {
-    if ((rc = ensure(ctx, lane_slot(i, 0), max_q * max_points * 8, &ln[i].ts))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 1), max_q * max_points * 8, &ln[i].val))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 2), max_q * 4, &ln[i].n))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 3), max_q * 4, &ln[i].st))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 4), meta_words * 8, &ln[i].meta))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 5), ch * out_cap * 8, &ln[i].ots))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 6), ch * out_cap * 8, &ln[i].oval))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 7), ch * 4, &ln[i].on))) return rc;
-    if ((rc = ensure(ctx, lane_slot(i, 8), ch * 4, &ln[i].ost))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 0), max_q * max_points * 8, &ln[i].ts))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 1), max_q * max_points * 8, &ln[i].val))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 2), max_q * 4, &ln[i].n))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 3), max_q * 4, &ln[i].st))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 4), meta_words * 8, &ln[i].meta))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 5), ch * out_cap * 8, &ln[i].ots))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 6), ch * out_cap * 8, &ln[i].oval))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 7), ch * 4, &ln[i].on))) return rc;
+    if ((rc = ensure(ctx, fence, lane_slot(i, 8), ch * 4, &ln[i].ost))) return rc;
     if ((rc = ensure_stage(ctx, i, meta_words * 8))) return rc;
   }
   CK(cudaMemcpyAsync(d_off, h_offsets, (n_seq + 1) * 8, cudaMemcpyHostToDevice, sts[0]));

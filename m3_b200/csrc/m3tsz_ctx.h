@@ -143,6 +143,8 @@ struct m3tsz_ctx {
   cudaStream_t stream = nullptr;   // used by the *_host entry points
   cudaStream_t stream2 = nullptr;  // second lane of the chunked H2D / kernel / D2H pipeline
   cudaEvent_t ev = nullptr;
+  // recorded by every call that uses the scratch below or d_flag, on the stream it ran on (ScratchFence)
+  cudaEvent_t scratch_ev = nullptr;
   uint64_t launches = 0;
   char last_error[256] = {0};
   Scratch s[kNumSlots];
@@ -165,26 +167,6 @@ inline int set_cuda_error(m3tsz_ctx *ctx, cudaError_t e, const char *where) {
     cudaError_t _e = (call);                                     \
     if (_e != cudaSuccess) return set_cuda_error(ctx, _e, #call); \
   } while (0)
-
-inline int ensure(m3tsz_ctx *ctx, Slot slot, size_t bytes, void **out) {
-  Scratch &sc = ctx->s[slot];
-  if (bytes == 0) bytes = 16;
-  if (sc.bytes < bytes) {
-    if (sc.ptr) CK(cudaFree(sc.ptr));
-    sc.ptr = nullptr;
-    sc.bytes = 0;
-    size_t want = bytes + bytes / 8;  // grow-only with slack
-    cudaError_t e = cudaMalloc(&sc.ptr, want);
-    if (e != cudaSuccess) {
-      (void)cudaGetLastError();
-      want = bytes;
-      CK(cudaMalloc(&sc.ptr, want));
-    }
-    sc.bytes = want;
-  }
-  *out = sc.ptr;
-  return M3TSZ_OK;
-}
 
 inline int ensure_stage(m3tsz_ctx *ctx, int i, size_t bytes) {
   if (ctx->h_stage_bytes[i] >= bytes) return M3TSZ_OK;
@@ -227,7 +209,63 @@ struct DeviceGuard {
   }
 };
 
-// Declared right after a *_host call's DeviceGuard: however the call returns, it does not
+// Declared right after the DeviceGuard of every call that uses context scratch or d_flag.  The scratch belongs to
+// the context, not to a stream, so these calls are ordered in the order they are issued, whatever streams they run
+// on: the call's stream (for the *_host calls and the streaming handles, both context streams) waits for the last
+// such call's work, and on every exit path the call's own work is recorded as the new last.  Neither this nor
+// ensure() is locked: batch calls on one context come from one host thread at a time.  `active` false: the call
+// uses no scratch this time (e.g. the caller passed every output), and the fence does nothing.
+struct ScratchFence {
+  m3tsz_ctx *ctx;
+  cudaStream_t st, st2 = nullptr;
+  bool active;
+  ScratchFence(m3tsz_ctx *c, cudaStream_t s, bool use = true) : ctx(c), st(s), active(use) {
+    if (active) cudaStreamWaitEvent(st, ctx->scratch_ev, 0);
+  }
+  explicit ScratchFence(m3tsz_ctx *c) : ctx(c), st(c->stream), st2(c->stream2), active(true) {
+    cudaStreamWaitEvent(st, ctx->scratch_ev, 0);
+    cudaStreamWaitEvent(st2, ctx->scratch_ev, 0);
+  }
+  ~ScratchFence() {
+    if (!active) return;
+    if (st2) {  // one event, two streams: the second joins the first
+      cudaEventRecord(ctx->ev, st2);
+      cudaStreamWaitEvent(st, ctx->ev, 0);
+    }
+    cudaEventRecord(ctx->scratch_ev, st);
+  }
+  ScratchFence(const ScratchFence &) = delete;
+  ScratchFence &operator=(const ScratchFence &) = delete;
+};
+
+// A scratch slot of at least `bytes`, under the call's fence.  Growing a slot frees the old buffer, so it first waits
+// for the last scratch-using call to finish.
+inline int ensure(m3tsz_ctx *ctx, const ScratchFence &fence, Slot slot, size_t bytes, void **out) {
+  if (!fence.active) {
+    snprintf(ctx->last_error, sizeof(ctx->last_error), "scratch slot %d used without its fence", (int)slot);
+    return M3TSZ_ERR_CUDA;
+  }
+  Scratch &sc = ctx->s[slot];
+  if (bytes == 0) bytes = 16;
+  if (sc.bytes < bytes) {
+    CK(cudaEventSynchronize(ctx->scratch_ev));
+    if (sc.ptr) CK(cudaFree(sc.ptr));
+    sc.ptr = nullptr;
+    sc.bytes = 0;
+    size_t want = bytes + bytes / 8;  // grow-only with slack
+    cudaError_t e = cudaMalloc(&sc.ptr, want);
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();
+      want = bytes;
+      CK(cudaMalloc(&sc.ptr, want));
+    }
+    sc.bytes = want;
+  }
+  *out = sc.ptr;
+  return M3TSZ_OK;
+}
+
+// Declared right after a *_host call's ScratchFence: however the call returns, it does not
 // leave copies from or into the caller's buffers in flight on the context's streams.
 struct DrainStreams {
   m3tsz_ctx *ctx;

@@ -119,16 +119,17 @@ int encoder_materialise(m3tsz_encoder *e) {
   std::lock_guard<std::mutex> lock(ctx->handle_mu);
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx);
   cudaStream_t st = ctx->stream;
   const uint64_t stride = m3tsz_encode_bound_units(n, 1) + ((e->ann_bytes.size() + 16 * e->ann.size() + 15) & ~15ull);
   void *d_ts, *d_val, *d_unit, *d_start, *d_out, *d_len, *d_st, *d_bits, *d_last, *d_aoff = nullptr,
        *d_aent = nullptr, *d_ab = nullptr;
   int rc;
-  if ((rc = ensure(ctx, kSlotEncTs, n * 8, &d_ts))) return rc;
-  if ((rc = ensure(ctx, kSlotEncVal, n * 8, &d_val))) return rc;
-  if ((rc = ensure(ctx, kSlotEncUnit, n, &d_unit))) return rc;
-  if ((rc = ensure(ctx, kSlotHandleMeta, 64, &d_start))) return rc;
-  if ((rc = ensure(ctx, kSlotEncOut, stride, &d_out))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotEncTs, n * 8, &d_ts))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotEncVal, n * 8, &d_val))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotEncUnit, n, &d_unit))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotHandleMeta, 64, &d_start))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotEncOut, stride, &d_out))) return rc;
   d_len = (uint8_t *)d_start + 8;
   d_st = (uint8_t *)d_start + 16;
   d_bits = (uint8_t *)d_start + 24;
@@ -139,9 +140,10 @@ int encoder_materialise(m3tsz_encoder *e) {
   CK(cudaMemcpyAsync(d_start, &e->start, 8, cudaMemcpyHostToDevice, st));
   uint64_t aoff[2] = {0, e->ann.size()};
   if (!e->ann.empty()) {
-    if ((rc = ensure(ctx, kSlotEncAnnOff, 16, &d_aoff))) return rc;
-    if ((rc = ensure(ctx, kSlotEncAnnEntries, e->ann.size() * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
-    if ((rc = ensure(ctx, kSlotEncAnnBytes, e->ann_bytes.size(), &d_ab))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotEncAnnOff, 16, &d_aoff))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotEncAnnEntries, e->ann.size() * sizeof(m3tsz_annotation_entry), &d_aent)))
+      return rc;
+    if ((rc = ensure(ctx, fence, kSlotEncAnnBytes, e->ann_bytes.size(), &d_ab))) return rc;
     CK(cudaMemcpyAsync(d_aoff, aoff, 16, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_aent, e->ann.data(), e->ann.size() * sizeof(m3tsz_annotation_entry),
                        cudaMemcpyHostToDevice, st));
@@ -223,13 +225,14 @@ int iter_materialise(m3tsz_iter *it) {
   std::lock_guard<std::mutex> lock(ctx->handle_mu);
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  ScratchFence fence(ctx);
   cudaStream_t st = ctx->stream;
   const size_t nbytes = it->data.size();
   uint64_t cap = 1024, ev_cap = 64;
   void *d_stream, *d_meta;
   int rc;
-  if ((rc = ensure(ctx, kSlotIterStream, nbytes + 16, &d_stream))) return rc;
-  if ((rc = ensure(ctx, kSlotHandleMeta, 64, &d_meta))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotIterStream, nbytes + 16, &d_stream))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotHandleMeta, 64, &d_meta))) return rc;
   CK(cudaMemcpyAsync(d_stream, it->data.data(), nbytes, cudaMemcpyHostToDevice, st));
   struct Meta {
     uint64_t off[2];
@@ -241,9 +244,9 @@ int iter_materialise(m3tsz_iter *it) {
   std::vector<m3tsz_dp_event> events;
   for (int attempt = 0; attempt < 8; attempt++) {
     void *d_ts, *d_val, *d_ev;
-    if ((rc = ensure(ctx, kSlotIterTs, cap * 8, &d_ts))) return rc;
-    if ((rc = ensure(ctx, kSlotIterVal, cap * 8, &d_val))) return rc;
-    if ((rc = ensure(ctx, kSlotIterEvents, ev_cap * sizeof(m3tsz_dp_event), &d_ev))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotIterTs, cap * 8, &d_ts))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotIterVal, cap * 8, &d_val))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotIterEvents, ev_cap * sizeof(m3tsz_dp_event), &d_ev))) return rc;
     memset(&meta, 0, sizeof(meta));
     meta.off[1] = nbytes;
     CK(cudaMemcpyAsync(d_meta, &meta, sizeof(meta), cudaMemcpyHostToDevice, st));
