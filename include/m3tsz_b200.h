@@ -26,7 +26,7 @@
  * m3tsz_decode_downsample_last_batch with a NULL lastAt / sumSq / last output,
  * m3tsz_encode_batch_packed(_ex), m3tsz_compact_streams,
  * m3tsz_encoder_set_write, m3tsz_element_set_reset of a set with output rows,
- * m3tsz_element_set_consume(_annotated), m3tsz_element_set_forward) are
+ * m3tsz_element_set_consume(_annotated), m3tsz_element_set_forward(_annotated)) are
  * ordered in the order they are issued: each one's stream waits on the device
  * for the context's previous such call, whatever stream that was on.  Two such
  * calls on one context therefore never overlap; a caller who wants them to
@@ -1119,7 +1119,8 @@ int m3tsz_element_set_consume_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
  *      drops its values.  So after growing the groups' open windows, calling again with exactly the failed groups
  *      (d_group_off / d_members listing only them, the same group set) gives the result of one unstopped call.
  * d_group_status [n_groups]: M3TSZ_OK or the status above.  The call reads and writes no annotation arrays (an
- * annotated group set's new windows get no annotation lengths: consume it with the plain consume).  A metric type or
+ * annotated group set's new windows get no annotation lengths: consume it with the plain consume, or forward with
+ * m3tsz_element_set_forward_annotated).  A metric type or
  * resolution mismatch, a source type list of other than one type, an invalid type or op list, n_groups other than
  * groups->n_elements, n_members above 2^40, src and groups sharing their slots, or NULL d_group_off / d_members /
  * statuses where they are needed: M3TSZ_ERR_INVALID_ARG before any launch. */
@@ -1127,6 +1128,35 @@ int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m
                               int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
                               uint64_t n_members, uint64_t n_groups, const m3tsz_element_set *groups,
                               int32_t *d_src_status, int32_t *d_group_status, void *stream);
+
+/* m3tsz_element_set_forward for sets that keep annotations: src_ann holds the source set's window annotations and
+ * group_ann the group set's (m3tsz_element_annotations, both required).  Values, counts, statuses, records, watermarks
+ * and the commit rule are those of m3tsz_element_set_forward; in addition:
+ *   1. A forwarded source window carries its slot's annotation: src_ann->d_len and the slot's bytes, a length of 0 or
+ *      above src_ann->capacity being none (as m3tsz_element_set_consume_annotated reads it).
+ *   2. A group window's annotation follows MaybeReplaceAnnotation through AddUnique (generic_elem.go:278-281,
+ *      aggregation/common.go:47-61): members in listed order, each member's forwarded windows in start order, every
+ *      forwarded value with a non-empty annotation replaces its group window's annotation.  A NaN that discard_nan
+ *      drops is not forwarded, so its annotation is not taken; a NaN forwarded without discard_nan carries its
+ *      annotation; a value dropped because its group window is closed changes nothing.  The order is the listed
+ *      member order, not arrival order (DESIGN.md §6).
+ *   3. A group window already open keeps its annotation unless a forwarded value replaces it; a window the call opens
+ *      writes its length (the annotation it took, or 0), so the group set's lengths need no initial value either.
+ *   4. A group one of whose values that would fold (its group window not closed) carries an annotation longer than
+ *      group_ann->capacity gets M3TSZ_ERR_CAPACITY under rule 4 above: nothing is folded into it and its members are
+ *      held back (INVALID_ARG over CAPACITY), so growing the group set's capacity and calling again with exactly the
+ *      failed groups gives the unstopped result.
+ *   5. The source annotation arrays are read, never written: a committed source's slot bytes stay until its next add.
+ * Besides the checks of m3tsz_element_set_forward: a NULL src_ann or group_ann, a capacity that is not a multiple of 8
+ * in 8 .. M3TSZ_MAX_ELEMENT_ANNOTATION, a non-zero reserved, misaligned pointers, or source and group annotation
+ * arrays that overlap: M3TSZ_ERR_INVALID_ARG before any launch.  Consume the group set with
+ * m3tsz_element_set_consume_annotated. */
+int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                        const m3tsz_element_annotations *src_ann, int64_t target_ns,
+                                        const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                        uint64_t n_groups, const m3tsz_element_set *groups,
+                                        const m3tsz_element_annotations *group_ann, int32_t *d_src_status,
+                                        int32_t *d_group_status, void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

@@ -136,6 +136,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_aggregate_tiles_blocks", "m3tsz_aggregate_tiles_rollup", "m3tsz_aggregate_tiles_rollup_annotated",
     "m3tsz_element_set_reset", "m3tsz_element_set_add", "m3tsz_element_set_consume",
     "m3tsz_element_set_add_annotated", "m3tsz_element_set_consume_annotated", "m3tsz_element_set_forward",
+    "m3tsz_element_set_forward_annotated",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -331,6 +332,8 @@ def lib():
     L.m3tsz_element_set_consume_annotated.argtypes = [vp, po, pes, pea, i64, i32, vp, vp]
     L.m3tsz_element_set_forward.restype = C.c_int
     L.m3tsz_element_set_forward.argtypes = [vp, po, pes, i64, vp, vp, u64, u64, pes, vp, vp, vp]
+    L.m3tsz_element_set_forward_annotated.restype = C.c_int
+    L.m3tsz_element_set_forward_annotated.argtypes = [vp, po, pes, pea, i64, vp, vp, u64, u64, pes, pea, vp, vp, vp]
     _lib = L
     return L
 

@@ -1060,13 +1060,20 @@ class ElementSet:
         """This set as a rollup's source set (m3tsz_element_set_forward, DESIGN.md §4.12): every element's open
         windows that ended by target_ns go, through ValueOf of the set's one type and its transformations, to the
         groups that list it; group g of `groups` (an ElementSet of the same metric type and resolution, one element
-        per group, without annotations) takes the values of the sources members[group_off[g] .. group_off[g + 1])
+        per group) takes the values of the sources members[group_off[g] .. group_off[g + 1])
         (int64 [G + 1] and int32 [n] device tensors, as aggregate_tiles_rollup takes them), in that order, into its
         window with the source window's start.  Returns (source statuses int32 [N]: OK, or the status of a failed
         group that held the source back; group statuses int32 [G]: OK, ERR_AGGREGATION_CLOSED -- a window that ended
         by the group's watermark was dropped --, ERR_CAPACITY -- too few open windows: groups.grow(open_windows=...)
-        and forward again with exactly the failed groups --, or ERR_INVALID_ARG)."""
-        assert isinstance(groups, ElementSet) and groups.ann_len is None, "the group set keeps no annotations"
+        and forward again with exactly the failed groups --, or ERR_INVALID_ARG).
+        When `groups` keeps annotations (m3tsz_element_set_forward_annotated) this set must keep them too: each
+        forwarded window carries its annotation, and each value with one replaces its group window's annotation, in
+        the listed member order.  A group whose forwarded annotation is longer than its capacity gets ERR_CAPACITY
+        too: groups.grow(annotation_capacity=...) and forward again with exactly the failed groups.  A group set
+        without annotations takes the plain call, whatever this set keeps."""
+        assert isinstance(groups, ElementSet)
+        if groups.ann_len is not None and self.ann_len is None:
+            raise ValueError("a group set that keeps annotations needs a source set that keeps them")
         assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
         assert members.is_cuda and members.dtype == torch.int32 and members.is_contiguous()
         G = group_off.numel() - 1
@@ -1075,11 +1082,19 @@ class ElementSet:
         src_status = torch.empty(max(1, self.n_elements), dtype=torch.int32, device=dev)
         group_status = torch.empty(max(1, G), dtype=torch.int32, device=dev)
         d, gd = self._desc(), groups._desc()
-        rc = capi.lib().m3tsz_element_set_forward(
-            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), int(target_ns), _ptr(group_off),
-            _ptr(members), members.numel(), G, C.byref(gd), _ptr(src_status), _ptr(group_status),
+        if groups.ann_len is None:
+            rc = capi.lib().m3tsz_element_set_forward(
+                self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), int(target_ns), _ptr(group_off),
+                _ptr(members), members.numel(), G, C.byref(gd), _ptr(src_status), _ptr(group_status),
+                _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_element_set_forward")
+            return src_status[: self.n_elements], group_status[:G]
+        a, ga = self._ann(), groups._ann()
+        rc = capi.lib().m3tsz_element_set_forward_annotated(
+            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(a), int(target_ns), _ptr(group_off),
+            _ptr(members), members.numel(), G, C.byref(gd), C.byref(ga), _ptr(src_status), _ptr(group_status),
             _cuda_stream_ptr(dev))
-        self.codec.ctx.check(rc, "m3tsz_element_set_forward")
+        self.codec.ctx.check(rc, "m3tsz_element_set_forward_annotated")
         return src_status[: self.n_elements], group_status[:G]
 
     def state(self):

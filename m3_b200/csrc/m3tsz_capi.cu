@@ -1467,11 +1467,15 @@ int m3tsz_element_set_consume_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
 }
 
 // The forward kernel writes each source's due windows to scratch, the fold kernel folds them into the groups' windows
-// and marks the members of the groups that failed, and the commit kernel frees the other sources' due windows
-int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
-                              int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
-                              uint64_t n_members, uint64_t n_groups, const m3tsz_element_set *groups,
-                              int32_t *d_src_status, int32_t *d_group_status, void *stream) {
+// and marks the members of the groups that failed, and the commit kernel frees the other sources' due windows.
+// m3tsz_element_set_forward(_annotated): annotated, the forward also writes which forwarded windows carry an
+// annotation and their references, and the fold copies each group window's into its slot.
+static int element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                               const m3tsz_element_annotations *src_ann, int64_t target_ns,
+                               const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                               uint64_t n_groups, const m3tsz_element_set *groups,
+                               const m3tsz_element_annotations *group_ann, int32_t *d_src_status,
+                               int32_t *d_group_status, void *stream, bool annotated) {
   ElementRollupParams rp;
   memset(&rp, 0, sizeof(rp));
   ElementParams gp;
@@ -1482,6 +1486,19 @@ int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m
       (n_groups && !d_group_off) || (n_members && !d_members) || ((uintptr_t)d_group_off & 7u) ||
       ((uintptr_t)d_members & 3u))
     return M3TSZ_ERR_INVALID_ARG;
+  if (annotated) {
+    if (!element_ann_params(src_ann, rp.src) || !element_ann_params(group_ann, gp)) return M3TSZ_ERR_INVALID_ARG;
+    // the source and group annotation arrays must not overlap: the fold copies source slot bytes into group slots
+    auto overlap = [](const void *a, uint64_t na, const void *b, uint64_t nb) {
+      return na && nb && (uintptr_t)a < (uintptr_t)b + nb && (uintptr_t)b < (uintptr_t)a + na;
+    };
+    const uint64_t sl = (uint64_t)rp.src.n_slots * rp.src.n, gl = (uint64_t)gp.n_slots * gp.n;
+    const void *sa[2] = {rp.src.ann_len, rp.src.ann_slot}, *ga[2] = {gp.ann_len, gp.ann_slot};
+    const uint64_t sb[2] = {sl * 4, sl * rp.src.ann_cap}, gb[2] = {gl * 4, gl * gp.ann_cap};
+    for (int i = 0; i < 2; i++)
+      for (int j = 0; j < 2; j++)
+        if (overlap(sa[i], sb[i], ga[j], gb[j])) return M3TSZ_ERR_INVALID_ARG;
+  }
   const uint64_t S = rp.src.n;
   if ((S && (!d_src_status || ((uintptr_t)d_src_status & 3u))) ||
       (n_groups && (!d_group_status || ((uintptr_t)d_group_status & 3u))))
@@ -1501,6 +1518,16 @@ int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m
   if ((rc = ensure(ctx, fence, kSlotElemFwdDue, sn * 8, &d_fd))) return rc;
   if ((rc = ensure(ctx, fence, kSlotElemFwdRec, sn * sizeof(m3tsz_transform_state), &d_rec))) return rc;
   if ((rc = ensure(ctx, fence, kSlotElemFwdMark, sn * 4, &d_mark))) return rc;
+  if (annotated) {
+    void *d_fap, *d_fa;
+    if ((rc = ensure(ctx, fence, kSlotElemFwdAnnPresent, sn * 8, &d_fap))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotElemFwdAnn, (size_t)sn * rp.src.n_slots * 8, &d_fa))) return rc;
+    rp.fwd_ann_present = (uint64_t *)d_fap;
+    rp.fwd_ann = (uint64_t *)d_fa;
+    rp.g_ann_len = gp.ann_len;
+    rp.g_ann_slot = gp.ann_slot;
+    rp.g_ann_cap = gp.ann_cap;
+  }
   rp.src.target = target_ns;
   rp.discard_nan = src->discard_nan ? 1 : 0;  // (generic_elem.go:892-894: with or without transformations)
   rp.fwd_start = (int64_t *)d_fs;
@@ -1532,6 +1559,24 @@ int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m
   CK(launch_element_commit(rp, st));
   ctx->launches += 3;
   return M3TSZ_OK;
+}
+
+int m3tsz_element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                              int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
+                              uint64_t n_members, uint64_t n_groups, const m3tsz_element_set *groups,
+                              int32_t *d_src_status, int32_t *d_group_status, void *stream) {
+  return element_set_forward(ctx, opts, src, nullptr, target_ns, d_group_off, d_members, n_members, n_groups, groups,
+                             nullptr, d_src_status, d_group_status, stream, false);
+}
+
+int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                        const m3tsz_element_annotations *src_ann, int64_t target_ns,
+                                        const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                        uint64_t n_groups, const m3tsz_element_set *groups,
+                                        const m3tsz_element_annotations *group_ann, int32_t *d_src_status,
+                                        int32_t *d_group_status, void *stream) {
+  return element_set_forward(ctx, opts, src, src_ann, target_ns, d_group_off, d_members, n_members, n_groups, groups,
+                             group_ann, d_src_status, d_group_status, stream, true);
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

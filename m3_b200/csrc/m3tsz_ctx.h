@@ -132,7 +132,10 @@ enum Slot : int {
   kSlotElemFwdDue = 77,
   kSlotElemFwdRec = 78,
   kSlotElemFwdMark = 79,
-  kNumSlots = 80
+  // ... that keep annotations
+  kSlotElemFwdAnnPresent = 80,
+  kSlotElemFwdAnn = 81,
+  kNumSlots = 82
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

@@ -2934,7 +2934,10 @@ cudaError_t launch_element_status(const int32_t *row_status, uint64_t n, uint32_
 // the value is forwarded (discard_nan drops a NaN with or without ops, as processValue does).  The slots, record and
 // watermark stay as they are: the commit frees the due slots (fwd_due) and saves the record (rec) unless a failed
 // group holds the source back.
-template <bool CTR>
+// ANN: a forwarded window whose slot holds an annotation (a length of 1 .. src.ann_cap; above the capacity reads as
+// none, as the annotated consume reads it) sets bit q of fwd_ann_present and writes its reference to fwd_ann; the
+// slot's bytes stay where they are for the fold to copy.
+template <bool CTR, bool ANN = false>
 __device__ __forceinline__ void elem_forward_lane(const ElementRollupParams &p, uint64_t s) {
   const ElementParams &e = p.src;
   uint32_t m = 0;
@@ -2970,6 +2973,22 @@ __device__ __forceinline__ void elem_forward_lane(const ElementRollupParams &p, 
     p.fwd_start[(uint64_t)q * e.n + s] = bs;
     p.fwd_val[(uint64_t)q * e.n + s] = v;
   }
+  if constexpr (ANN) {  // (after the windows' loop, so that nothing more lives across xf_window's calls)
+    uint64_t ann = 0;
+    for (uint32_t r = 0; r < e.n_slots; r++) {
+      if (!((due >> r) & 1u)) continue;
+      const uint64_t o = (uint64_t)r * e.n + s;
+      const uint32_t l = e.ann_len[o];
+      if (l == 0 || l > e.ann_cap) continue;
+      const int64_t ws = e.start[o];
+      uint32_t q = 0;  // the window's place in start order
+      for (uint32_t r2 = 0; r2 < e.n_slots; r2++) q += ((due >> r2) & 1u) && e.start[(uint64_t)r2 * e.n + s] < ws;
+      if (!((present >> q) & 1u)) continue;
+      ann |= 1ull << q;
+      p.fwd_ann[(uint64_t)q * e.n + s] = (o << 17) | l;
+    }
+    p.fwd_ann_present[s] = ann;
+  }
   p.fwd_n[s] = m;
   p.fwd_present[s] = present;
   p.fwd_due[s] = due;
@@ -2985,6 +3004,17 @@ struct ElemFoldAcc {
   using A = std::conditional_t<CTR, RollupCounterAcc, RollupGaugeAcc>;
   int64_t start;
   A a;
+  // the annotated fold's group window annotation to group slot o: ref is the forward's reference to a source slot
+  // (0: none), whose bytes go over as whole 8-byte words (the annotated add zero-pads a slot's last word), lane
+  // `lane` of n_lanes copying words lane, lane + n_lanes, ...; every lane writes the length
+  __device__ static __forceinline__ void store_ann(const ElementRollupParams &p, uint64_t o, uint64_t ref,
+                                                   uint32_t lane, uint32_t n_lanes) {
+    const uint32_t len = (uint32_t)(ref & 0x1ffffu);
+    p.g_ann_len[o] = len;
+    const uint64_t *src = reinterpret_cast<const uint64_t *>(p.src.ann_slot + (ref >> 17) * p.src.ann_cap);
+    uint64_t *dst = reinterpret_cast<uint64_t *>(p.g_ann_slot + o * p.g_ann_cap);
+    for (uint32_t w = lane; w < (len + 7u) / 8u; w += n_lanes) dst[w] = src[w];
+  }
 };
 template <bool CTR>
 __device__ __forceinline__ void elem_fold_load(const ElementRollupParams &p, uint64_t o, ElemFoldAcc<CTR> &f) {
@@ -3019,14 +3049,17 @@ __device__ __forceinline__ void elem_fold_store(const ElementRollupParams &p, ui
 }
 
 // What the fold reads of the member at one listed position: its source index, its due windows, which of them are
-// forwarded, and its first due window's start and value (later ones are read from fwd_start / fwd_val)
+// forwarded, and its first due window's start and value (later ones are read from fwd_start / fwd_val); ANN: which
+// forwarded windows carry an annotation (their references are read from fwd_ann, those windows' only)
 struct FwdMember {
   uint64_t m;  // >= src.n: an invalid index (n = 0)
   uint32_t n;
   uint64_t present;
   int64_t start0;
   double val0;
+  uint64_t ann;
 };
+template <bool ANN = false>
 __device__ __forceinline__ FwdMember fwd_member(const ElementRollupParams &p, uint64_t i) {
   FwdMember a;
   a.m = p.members[i];
@@ -3034,9 +3067,11 @@ __device__ __forceinline__ FwdMember fwd_member(const ElementRollupParams &p, ui
   a.present = 0;
   a.start0 = 0;
   a.val0 = 0.0;
+  a.ann = 0;
   if (a.m < p.src.n) {
     a.n = p.fwd_n[a.m];
     a.present = p.fwd_present[a.m];
+    if constexpr (ANN) a.ann = p.fwd_ann_present[a.m];
     if (a.n) {
       a.start0 = p.fwd_start[a.m];
       a.val0 = p.fwd_val[a.m];
@@ -3052,12 +3087,19 @@ __device__ __forceinline__ FwdMember fwd_member(const ElementRollupParams &p, ui
 // registers (it goes back to its slot when a value needs another one, and at the end); a window that ends at or
 // before the group's watermark is dropped (AGGREGATION_CLOSED, the other windows still fold).  fresh: room for
 // g_slots starts.  Returns the group's status (also written to group_status[g]).
-template <bool CTR, class Member>
+// ANN: MaybeReplaceAnnotation through AddUnique (generic_elem.go:278-281): each folded value whose window carries an
+// annotation makes it its group window's, kept in registers as the forward's reference beside the accumulator.  It goes
+// to the slot with the window when it changed: a window opened here always writes its length (0 without one), one
+// already open keeps its annotation unless a value replaced it.  The first pass also fails the group with CAPACITY
+// for an annotation longer than g_ann_cap on a value that would fold.  The lanes lane .. of n_lanes split a copy.
+template <bool CTR, bool ANN = false, class Member>
 __device__ __forceinline__ int32_t elem_fold_group(const ElementRollupParams &p, uint64_t g, int64_t *fresh,
-                                                   Member member) {
+                                                   Member member, uint32_t lane = 0, uint32_t n_lanes = 1) {
   const uint64_t lo = p.group_off[g], hi = p.group_off[g + 1], G = p.n_groups;
   const int64_t res = p.src.resolution, wm = p.g_watermark[g];
   int32_t status = M3TSZ_OK;
+  // ANN: the reference of member a's q-th window (its bit of a.ann set)
+  auto ann_ref = [&](const FwdMember &a, uint32_t q) { return p.fwd_ann[(uint64_t)q * p.src.n + a.m]; };
   auto window = [&](const FwdMember &a, uint32_t q, int64_t &ws, double &v) {
     if (q == 0) {
       ws = a.start0;
@@ -3082,6 +3124,10 @@ __device__ __forceinline__ int32_t elem_fold_group(const ElementRollupParams &p,
         int64_t ws;
         double v;
         window(a, q, ws, v);
+        if constexpr (ANN) {
+          if (((a.ann >> q) & 1u) && !elem_ends_by(ws, res, wm) && (ann_ref(a, q) & 0x1ffffu) > p.g_ann_cap)
+            full = true;
+        }
         if ((seen && ws == last) || elem_ends_by(ws, res, wm)) continue;
         seen = true;
         last = ws;
@@ -3104,6 +3150,8 @@ __device__ __forceinline__ int32_t elem_fold_group(const ElementRollupParams &p,
     ElemFoldAcc<CTR> f;
     int cur = -1;  // the slot `f` belongs to, -1: none
     bool closed = false;
+    uint64_t a_ref = 0;  // ANN: the window's annotation taken in this call (0: none), and whether its slot needs it
+    bool a_dirty = false;
     for (uint64_t i = lo; i < hi; i++) {
       const FwdMember a = member(i);
       for (uint32_t q = 0; q < a.n; q++) {
@@ -3116,7 +3164,10 @@ __device__ __forceinline__ int32_t elem_fold_group(const ElementRollupParams &p,
           continue;
         }
         if (cur < 0 || ws != f.start) {  // the window's slot, or a free one (the first pass counted them)
-          if (cur >= 0) elem_fold_store(p, (uint64_t)cur * G + g, f);
+          if (cur >= 0) {
+            elem_fold_store(p, (uint64_t)cur * G + g, f);
+            if (ANN && a_dirty) ElemFoldAcc<CTR>::store_ann(p, (uint64_t)cur * G + g, a_ref, lane, n_lanes);
+          }
           int hit = -1, fr = -1;
           for (uint32_t r = 0; r < p.g_slots; r++) {
             const uint64_t o = (uint64_t)r * G + g;
@@ -3137,14 +3188,23 @@ __device__ __forceinline__ int32_t elem_fold_group(const ElementRollupParams &p,
             else
               rollup_gauge_init(f.a);
           }
+          a_ref = 0;
+          a_dirty = hit < 0;
         }
         if constexpr (CTR)
           rollup_counter_add(f.a, v);
         else
           rollup_gauge_add(f.a, v);
+        if (ANN && ((a.ann >> q) & 1u)) {
+          a_ref = ann_ref(a, q);
+          a_dirty = true;
+        }
       }
     }
-    if (cur >= 0) elem_fold_store(p, (uint64_t)cur * G + g, f);
+    if (cur >= 0) {
+      elem_fold_store(p, (uint64_t)cur * G + g, f);
+      if (ANN && a_dirty) ElemFoldAcc<CTR>::store_ann(p, (uint64_t)cur * G + g, a_ref, lane, n_lanes);
+    }
     if (closed) status = M3TSZ_ERR_AGGREGATION_CLOSED;
   }
   p.group_status[g] = status;
@@ -3166,19 +3226,20 @@ __device__ __forceinline__ void elem_commit_lane(const ElementRollupParams &p, u
   p.src.elem[s].head = p.rec[s];
 }
 
-template <bool CTR>
+template <bool CTR, bool ANN>
 __global__ void __launch_bounds__(ELEM_THREADS) element_forward_kernel(const ElementRollupParams p) {
   const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
-  if (s < p.src.n) elem_forward_lane<CTR>(p, s);
+  if (s < p.src.n) elem_forward_lane<CTR, ANN>(p, s);
 }
 
 // One warp per group.  The lanes gather 32 listed members at a time (their indices as one coalesced load, their due
 // counts, presence words and first forwarded windows as one gather); every lane then runs the group's fold on the
 // same values, shuffled from the lane that loaded them, so the fold is in listed order and its branches are uniform.
 // The lanes' stores to the group's slots are of equal values.  A group that failed with CAPACITY or INVALID_ARG marks
-// the members its range names for the commit.
+// the members its range names for the commit.  ANN: the presence words carry the annotation words with them, and the
+// lanes split each annotation copy.
 constexpr int ELEM_FOLD_WARPS = 8;
-template <bool CTR>
+template <bool CTR, bool ANN>
 __global__ void __launch_bounds__(ELEM_FOLD_WARPS * 32) element_fold_kernel(const ElementRollupParams p) {
   __shared__ int64_t fresh[ELEM_FOLD_WARPS][M3TSZ_MAX_ELEMENT_WINDOWS];
   const uint32_t lane = threadIdx.x & 31u, wi = threadIdx.x >> 5;
@@ -3196,7 +3257,8 @@ __global__ void __launch_bounds__(ELEM_FOLD_WARPS * 32) element_fold_kernel(cons
       mine.present = 0;
       mine.start0 = 0;
       mine.val0 = 0.0;
-      if (b + lane < hi) mine = fwd_member(p, b + lane);
+      mine.ann = 0;
+      if (b + lane < hi) mine = fwd_member<ANN>(p, b + lane);
     }
     const int j = (int)((i - lo) & 31u);
     FwdMember a;
@@ -3205,9 +3267,11 @@ __global__ void __launch_bounds__(ELEM_FOLD_WARPS * 32) element_fold_kernel(cons
     a.present = __shfl_sync(FULL_MASK, mine.present, j);
     a.start0 = __shfl_sync(FULL_MASK, mine.start0, j);
     a.val0 = __shfl_sync(FULL_MASK, mine.val0, j);
+    a.ann = 0;
+    if constexpr (ANN) a.ann = __shfl_sync(FULL_MASK, mine.ann, j);
     return a;
   };
-  const int32_t st = elem_fold_group<CTR>(p, g, fresh[wi], member);
+  const int32_t st = elem_fold_group<CTR, ANN>(p, g, fresh[wi], member, lane, 32u);
   if ((st == M3TSZ_ERR_CAPACITY || st == M3TSZ_ERR_INVALID_ARG) && lo <= hi) {
     const uint64_t end = hi < p.n_members ? hi : p.n_members;
     for (uint64_t i = lo + lane; i < end; i += 32) {
@@ -3225,10 +3289,16 @@ __global__ void __launch_bounds__(ELEM_THREADS) element_commit_kernel(const Elem
 cudaError_t launch_element_forward(const ElementRollupParams &p, cudaStream_t stream) {
   if (p.src.n == 0) return cudaSuccess;
   if ((p.src.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
-  if (p.src.counter)
-    element_forward_kernel<true><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
+  const bool ann = p.src.ann_len != nullptr;
+  if (ann && (!p.fwd_ann_present || !p.fwd_ann)) return cudaErrorInvalidValue;
+  if (p.src.counter && ann)
+    element_forward_kernel<true, true><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
+  else if (p.src.counter)
+    element_forward_kernel<true, false><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
+  else if (ann)
+    element_forward_kernel<false, true><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
   else
-    element_forward_kernel<false><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
+    element_forward_kernel<false, false><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
@@ -3236,10 +3306,16 @@ cudaError_t launch_element_fold(const ElementRollupParams &p, cudaStream_t strea
   if (p.n_groups == 0) return cudaSuccess;
   const uint64_t blocks = (p.n_groups + ELEM_FOLD_WARPS - 1) / ELEM_FOLD_WARPS;
   if (blocks > 0x7fffffffull) return cudaErrorInvalidValue;
-  if (p.src.counter)
-    element_fold_kernel<true><<<(unsigned)blocks, ELEM_FOLD_WARPS * 32, 0, stream>>>(p);
+  const bool ann = p.src.ann_len != nullptr;
+  if (ann && (!p.fwd_ann_present || !p.fwd_ann || !p.g_ann_len || !p.g_ann_slot)) return cudaErrorInvalidValue;
+  if (p.src.counter && ann)
+    element_fold_kernel<true, true><<<(unsigned)blocks, ELEM_FOLD_WARPS * 32, 0, stream>>>(p);
+  else if (p.src.counter)
+    element_fold_kernel<true, false><<<(unsigned)blocks, ELEM_FOLD_WARPS * 32, 0, stream>>>(p);
+  else if (ann)
+    element_fold_kernel<false, true><<<(unsigned)blocks, ELEM_FOLD_WARPS * 32, 0, stream>>>(p);
   else
-    element_fold_kernel<false><<<(unsigned)blocks, ELEM_FOLD_WARPS * 32, 0, stream>>>(p);
+    element_fold_kernel<false, false><<<(unsigned)blocks, ELEM_FOLD_WARPS * 32, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

@@ -424,7 +424,17 @@ struct ElementRollupParams {
   // the commit: mark[s] is the largest status of a failed group listing s (0: none)
   int32_t *mark;
   int32_t *src_status;
+  // the annotated forward (src.ann_len set; src.ann_len / ann_slot / ann_cap are the source slots' annotations): per
+  // source, bit q of fwd_ann_present says the q-th due window is forwarded and carries an annotation, and for those
+  // windows only fwd_ann[q * src.n + s] refers to it as (its slot r * src.n + s) << 17 | its length (1 .. 65536);
+  // the group slots' annotations, laid out as the source slots'
+  uint64_t *fwd_ann_present;
+  uint64_t *fwd_ann;
+  uint32_t *g_ann_len;
+  uint8_t *g_ann_slot;
+  uint64_t g_ann_cap;
 };
+// (the annotated kernels when p.src.ann_len is set)
 cudaError_t launch_element_forward(const ElementRollupParams &p, cudaStream_t stream);
 // (p.mark must be zero)
 cudaError_t launch_element_fold(const ElementRollupParams &p, cudaStream_t stream);

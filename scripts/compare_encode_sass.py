@@ -8,8 +8,9 @@ rollup_forward_kernel and rollup_fold_kernel are compared too; the annotated rol
 old build's untemplated kernel is compared with a new build's <false>.  The element sets' element_add_kernel<CTR> and
 element_consume_kernel<CTR> are compared too; the annotated element sets added a second argument, ANN, so an old
 build's <CTR> is compared with a new build's <CTR, false>.  The element rollup's element_forward_kernel,
-element_fold_kernel and element_commit_kernel are compared by name.  Instantiations only one build has (the append mode, new
-decode modes, the annotated element kernels) are listed, not compared.
+element_fold_kernel and element_commit_kernel are compared too; the annotated element rollup added a second argument,
+ANN, to the first two, so an old build's <CTR> is compared with a new build's <CTR, false>.  Instantiations only one
+build has (the append mode, new decode modes, the annotated element kernels) are listed, not compared.
 
     python scripts/compare_encode_sass.py OLD.(o|so) NEW.(o|so)     # exit code 1 on any difference
 
@@ -40,7 +41,7 @@ def kernels(path):
                 cur = re.sub(r"(element_(?:add|consume)_kernelILb[01]E)Lb0E", r"\1", name)
                 out[cur] = []
             elif re.search(r"element_(forward|fold|commit)_kernel", name):  # (element sets through a rollup)
-                cur = name
+                cur = re.sub(r"(element_(?:forward|fold)_kernelILb[01]E)Lb0E", r"\1", name)
                 out[cur] = []
             elif "rollup_forward_kernel" in name or "rollup_fold_kernel" in name:
                 cur = re.sub(r"(rollup_(?:forward|fold)_kernel)ILb0EEEvNS_", r"\1ENS_", name)
