@@ -515,6 +515,7 @@ int m3tsz_decode_downsample_last_batch(m3tsz_ctx *ctx, const m3tsz_options *opts
  * ---------------------------------------------------------------------- */
 enum { /* metric.Type ids, src/metrics/metric/types.go:35-38 */
   M3TSZ_METRIC_COUNTER = 1,
+  M3TSZ_METRIC_TIMER = 2, /* element sets only (m3tsz_element_set_add_timer); every other call refuses it */
   M3TSZ_METRIC_GAUGE = 3
 };
 typedef struct m3tsz_downsample_outputs {
@@ -660,10 +661,26 @@ enum { /* aggregation.Type ids, src/metrics/aggregation/type.go:31-38 */
   M3TSZ_AGG_MIN = 2,
   M3TSZ_AGG_MAX = 3,
   M3TSZ_AGG_MEAN = 4,
+  M3TSZ_AGG_MEDIAN = 5, /* Timer element sets only, as are the quantile types below */
   M3TSZ_AGG_COUNT = 6,
   M3TSZ_AGG_SUM = 7,
   M3TSZ_AGG_SUMSQ = 8, /* m3tsz_aggregate_tiles_ex only */
-  M3TSZ_AGG_STDEV = 9  /* m3tsz_aggregate_tiles_ex only */
+  M3TSZ_AGG_STDEV = 9, /* m3tsz_aggregate_tiles_ex only */
+  M3TSZ_AGG_P10 = 10,
+  M3TSZ_AGG_P20 = 11,
+  M3TSZ_AGG_P30 = 12,
+  M3TSZ_AGG_P40 = 13,
+  M3TSZ_AGG_P50 = 14,
+  M3TSZ_AGG_P60 = 15,
+  M3TSZ_AGG_P70 = 16,
+  M3TSZ_AGG_P80 = 17,
+  M3TSZ_AGG_P90 = 18,
+  M3TSZ_AGG_P95 = 19,
+  M3TSZ_AGG_P99 = 20,
+  M3TSZ_AGG_P999 = 21,
+  M3TSZ_AGG_P9999 = 22,
+  M3TSZ_AGG_P25 = 23,
+  M3TSZ_AGG_P75 = 24
 };
 /* Gauge with the six types above; SumSq / Stdev are rejected here (m3tsz_aggregate_tiles_ex has them). */
 int m3tsz_aggregate_tiles_batch(m3tsz_ctx *ctx, const m3tsz_options *opts, const uint8_t *d_streams,
@@ -983,7 +1000,7 @@ int m3tsz_aggregate_tiles_rollup_annotated(
 typedef struct m3tsz_element_set {
   uint64_t n_elements;
   uint32_t n_windows;       /* R: open-window slots per element, 1 .. M3TSZ_MAX_ELEMENT_WINDOWS */
-  int32_t metric_type;      /* M3TSZ_METRIC_GAUGE or M3TSZ_METRIC_COUNTER */
+  int32_t metric_type;      /* M3TSZ_METRIC_GAUGE, M3TSZ_METRIC_COUNTER or M3TSZ_METRIC_TIMER (the Timer calls) */
   int64_t resolution_ns;    /* > 0 */
   const int32_t *agg_types; /* host */
   uint32_t n_types;
@@ -1157,6 +1174,81 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
                                         uint64_t n_groups, const m3tsz_element_set *groups,
                                         const m3tsz_element_annotations *group_ann, int32_t *d_src_status,
                                         int32_t *d_group_status, void *stream);
+
+/* Timer element sets (DESIGN.md §4.12): an element set of metric_type M3TSZ_METRIC_TIMER, whose windows are
+ * aggregation.Timer (aggregation/timer.go) over the CM stream (aggregation/quantile/cm/stream.go).
+ *   - Types: strictly ascending, any but Last (IsValidForTimer); 1 .. 23 of them without ops, 1 ..
+ *     M3TSZ_MAX_ELEMENT_TYPES with ops.  The stream's quantile list is Types.PooledQuantiles over them: the quantile
+ *     types in the listed order (ascending id), Median and P50 one 0.5.  It is not sorted: P25 / P75 (ids 23 / 24)
+ *     come after P9999, and "first listed quantile >= q" is what Quantile(q) returns.
+ *   - Slots: d_win_start, d_win_count (values added; 0: the slot is free), d_win_sum, d_win_sum_sq (float64, summed
+ *     in add order, NaN included, no FMA); d_win_min / d_win_max / d_win_last / d_win_last_at are unused (may be NULL).
+ *   - ValueOf: Min / Max the flushed stream's first / last sample, Mean sum / count, Count, Sum, SumSq, Stdev as in
+ *     m3tsz_aggregate_tiles_ex, and each quantile type Quantile(q) of the stream after Flush.  A quantile that
+ *     calcQuantiles leaves unset reads 0, as a freshly made stream holds it.
+ *   - A set of more than M3TSZ_MAX_ELEMENT_TYPES types has no ops and leaves its records untouched; up to that many,
+ *     the records are kept as for the other sets.
+ * m3tsz_element_set_reset takes a Timer set as any other; add, consume, their annotated forms and forward refuse it
+ * (M3TSZ_ERR_INVALID_ARG before any launch), as the tile and downsample calls refuse metric type 2.
+ *
+ * Each window slot's stream lives in caller-owned device memory, pointer-free (growing R or the capacity is a copy).
+ * Slot o = r * n_elements + s; its sample i (list sample or pending heap entry) at (r * sample_capacity + i) *
+ * n_elements + s, so a warp's lanes touch adjacent words.  The header is written when an add opens the window, so
+ * nothing needs an initial value. */
+typedef struct m3tsz_timer_stream_header {
+  int64_t num_values;        /* numValues: values inserted into the sorted list */
+  int64_t compress_min_rank; /* compressMinRank */
+  int32_t head, tail;        /* the list's ends (sample indices), -1: none */
+  int32_t insert_cursor;     /* insertCursor, -1: nil */
+  int32_t compress_cursor;   /* compressCursor, -1: nil */
+  int32_t n_samples;         /* samples in the list */
+  int32_t n_used;            /* sample entries ever taken; freed ones are chained through d_next from free_head */
+  int32_t free_head;
+  int32_t counter;           /* insertAndCompressCounter */
+  int32_t n_a, n_b;          /* the pending heaps' lengths */
+  int32_t less_is_b;         /* bufLess is heap b (resetInsertCursor swaps the two) */
+  int32_t reserved;
+} m3tsz_timer_stream_header; /* 64 bytes */
+typedef struct m3tsz_element_timer_streams {
+  m3tsz_timer_stream_header *d_header; /* [R][n_elements], 8-byte aligned */
+  double *d_value;                     /* list samples: value, numRanks, delta, prev / next links (-1: none) */
+  int64_t *d_num_ranks;
+  int64_t *d_delta;
+  int32_t *d_prev, *d_next;
+  double *d_heap_a, *d_heap_b;         /* the pending minHeaps, as the reference's arrays */
+  uint32_t sample_capacity;            /* >= 1: values a slot holds, list samples and pending values together */
+  uint32_t insert_and_compress_every;  /* >= 1 (StreamOptions: 1024) */
+  double eps;                          /* finite, > 0 (StreamOptions: 1e-3) */
+  uint64_t reserved;                   /* 0 */
+} m3tsz_element_timer_streams;
+
+/* Timer.AddBatch of the elements' samples, point-major d_ts / d_val [points_stride][n_elements] with d_n_points as
+ * in m3tsz_element_set_add.  d_batch (optional, int8 [points_stride][n_elements]): a nonzero entry continues the
+ * previous row's batch (BatchTimer); NULL: every row is its own batch (AppendTimerSample).  Per batch, in order:
+ *   - its window is that of its first row's timestamp; a window at or before the watermark refuses the whole batch
+ *     (M3TSZ_ERR_AGGREGATION_CLOSED), a start below INT64_MIN too (M3TSZ_ERR_INVALID_ARG);
+ *   - capacity: a slot holds at most sample_capacity values, list samples and pending values together.  A batch that
+ *     would exceed it, or that needs a new window when all R slots are open, gets M3TSZ_ERR_CAPACITY, and so does
+ *     every later row of the element in this call: nothing of them is added, so adding exactly those rows again
+ *     after growing gives the unstopped result.  No insert and no consume-time Flush can then run out of room;
+ *   - else count += len, sum += v and sumSq += v * v in order, and the stream's AddBatch (the first value of a new
+ *     window straight into the list; the pending heaps; insert + compress every insert_and_compress_every values).
+ * d_result [points_stride][n_elements]: each row its batch's status.  d_status: M3TSZ_OK, M3TSZ_ERR_CAPACITY, or
+ * M3TSZ_ERR_INVALID_ARG when n_points > points_stride (nothing written) or when a continuation is in row 0 or has
+ * another timestamp than its batch's first row (every row M3TSZ_ERR_INVALID_ARG; the element is untouched).
+ * Host checks (M3TSZ_ERR_INVALID_ARG before any launch): the set's, NULL streams, sample_capacity of 0 or above 2^30,
+ * eps not finite or <= 0, insert_and_compress_every of 0 or above 2^31 - 1, a non-zero reserved, misaligned arrays. */
+int m3tsz_element_set_add_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                const m3tsz_element_timer_streams *streams, const int64_t *d_ts, const double *d_val,
+                                uint64_t points_stride, const uint32_t *d_n_points, const int8_t *d_batch,
+                                int8_t *d_result, int32_t *d_status, void *stream);
+
+/* m3tsz_element_set_consume of a Timer set: each due window, in start order, is flushed (Flush: insert + compress
+ * until both pending heaps are empty, then calcQuantiles), and ValueOf of each type goes through the ops, the NaN
+ * discard and the Reset row, onto the output rows, with the plain consume's room check and commit rule. */
+int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                    const m3tsz_element_timer_streams *streams, int64_t target_ns, int32_t out_unit,
+                                    int32_t *d_status, void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

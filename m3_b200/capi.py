@@ -28,7 +28,16 @@ ERR_NO_DEVICE = 103
 
 AGG_LAST, AGG_MIN, AGG_MAX, AGG_MEAN, AGG_COUNT, AGG_SUM = 1, 2, 3, 4, 6, 7  # aggregation.Type ids
 AGG_SUMSQ, AGG_STDEV = 8, 9  # the expensive aggregations (m3tsz_aggregate_tiles_ex only)
-METRIC_COUNTER, METRIC_GAUGE = 1, 3  # metric.Type ids
+METRIC_COUNTER, METRIC_TIMER, METRIC_GAUGE = 1, 2, 3  # metric.Type ids (the Timer: element sets only)
+# the Timer's further aggregation.Type ids (Timer element sets)
+AGG_MEDIAN = 5
+AGG_P10, AGG_P20, AGG_P30, AGG_P40, AGG_P50, AGG_P60, AGG_P70, AGG_P80, AGG_P90 = range(10, 19)
+AGG_P95, AGG_P99, AGG_P999, AGG_P9999, AGG_P25, AGG_P75 = range(19, 25)
+# the aggregator's default Timer types (types_options.go): Sum, SumSq, Mean, Min, Max, Count, Stdev, Median, P50, P95,
+# P99, in ascending id order
+DEFAULT_TIMER_TYPES = (AGG_MIN, AGG_MAX, AGG_MEAN, AGG_MEDIAN, AGG_COUNT, AGG_SUM, AGG_SUMSQ, AGG_STDEV, AGG_P50,
+                       AGG_P95, AGG_P99)
+MAX_TIMER_TYPES = 23  # a Timer set without transformations: every type but Last
 # transformation.Type ids (m3tsz_aggregate_tiles_transform)
 TRANSFORM_ABSOLUTE, TRANSFORM_PERSECOND, TRANSFORM_INCREASE, TRANSFORM_ADD, TRANSFORM_RESET = 1, 2, 3, 4, 5
 MAX_TRANSFORMS = 8  # M3TSZ_MAX_TRANSFORMS
@@ -74,6 +83,17 @@ class ElementSet(C.Structure):
 class ElementAnnotations(C.Structure):
     """m3tsz_element_annotations: the window slots' annotation lengths and bytes (include/m3tsz_b200.h)."""
     _fields_ = [("d_len", C.c_void_p), ("d_bytes", C.c_void_p), ("capacity", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class ElementTimerStreams(C.Structure):
+    """m3tsz_element_timer_streams: the window slots' CM streams (include/m3tsz_b200.h)."""
+    _fields_ = [(f, C.c_void_p) for f in ("d_header", "d_value", "d_num_ranks", "d_delta", "d_prev", "d_next",
+                                          "d_heap_a", "d_heap_b")] + [
+        ("sample_capacity", C.c_uint32), ("insert_and_compress_every", C.c_uint32), ("eps", C.c_double),
+        ("reserved", C.c_uint64)]
+
+
+TIMER_STREAM_HEADER_BYTES = 64  # sizeof(m3tsz_timer_stream_header)
 
 
 class DecodeExtras(C.Structure):
@@ -136,7 +156,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_aggregate_tiles_blocks", "m3tsz_aggregate_tiles_rollup", "m3tsz_aggregate_tiles_rollup_annotated",
     "m3tsz_element_set_reset", "m3tsz_element_set_add", "m3tsz_element_set_consume",
     "m3tsz_element_set_add_annotated", "m3tsz_element_set_consume_annotated", "m3tsz_element_set_forward",
-    "m3tsz_element_set_forward_annotated",
+    "m3tsz_element_set_forward_annotated", "m3tsz_element_set_add_timer", "m3tsz_element_set_consume_timer",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -334,6 +354,11 @@ def lib():
     L.m3tsz_element_set_forward.argtypes = [vp, po, pes, i64, vp, vp, u64, u64, pes, vp, vp, vp]
     L.m3tsz_element_set_forward_annotated.restype = C.c_int
     L.m3tsz_element_set_forward_annotated.argtypes = [vp, po, pes, pea, i64, vp, vp, u64, u64, pes, pea, vp, vp, vp]
+    pts = C.POINTER(ElementTimerStreams)
+    L.m3tsz_element_set_add_timer.restype = C.c_int
+    L.m3tsz_element_set_add_timer.argtypes = [vp, po, pes, pts, vp, vp, u64, vp, vp, vp, vp, vp]
+    L.m3tsz_element_set_consume_timer.restype = C.c_int
+    L.m3tsz_element_set_consume_timer.argtypes = [vp, po, pes, pts, i64, i32, vp, vp]
     _lib = L
     return L
 

@@ -289,7 +289,8 @@ class BatchCodec:
 
     def element_set(self, start: torch.Tensor, metric_type, agg_types, resolution_ns, transforms=(),
                     discard_nan=False, open_windows=4, stride: Optional[int] = None,
-                    out_unit=capi.UNIT_S, annotation_capacity=0) -> "ElementSet":
+                    out_unit=capi.UNIT_S, annotation_capacity=0, sample_capacity: Optional[int] = None, eps=1e-3,
+                    insert_and_compress_every=1024) -> "ElementSet":
         """N aggregator elements fed datapoint by datapoint (m3tsz_element_set_*, N = start.numel(), start int64
         [N] ns): one metric type (capi.METRIC_GAUGE / METRIC_COUNTER), resolution, strictly ascending list of
         aggregation types and transformation list, checked and applied as in aggregate_tiles_types (discard_nan
@@ -299,9 +300,13 @@ class BatchCodec:
         annotation_capacity > 0 (a multiple of 8, at most capi.MAX_ELEMENT_ANNOTATION): the elements keep annotations
         (m3tsz_element_set_*_annotated), each open window up to that many bytes of its last non-empty one.
         stride=0: a set without output rows, a rollup's source set (ElementSet.forward); consume() and stream()
-        refuse it."""
+        refuse it.
+        capi.METRIC_TIMER (m3tsz_element_set_*_timer): every type but Last (up to capi.MAX_TIMER_TYPES without
+        transformations), each open window an aggregation.Timer over the CM stream with `eps` and
+        `insert_and_compress_every` (the aggregator's StreamOptions), holding at most `sample_capacity` values (list
+        samples and pending values together; required).  A Timer set takes no annotations and no forward."""
         return ElementSet(self, start, metric_type, agg_types, resolution_ns, transforms, discard_nan, open_windows,
-                          stride, out_unit, annotation_capacity)
+                          stride, out_unit, annotation_capacity, sample_capacity, eps, insert_and_compress_every)
 
     def bucket_set(self, start: torch.Tensor, stride: int, encoders=4, pool_records: Optional[int] = None,
                    pool_stride: Optional[int] = None) -> "BucketSet":
@@ -873,10 +878,14 @@ class ElementSet:
     `watermark` int64 [N] (the end of the last window consumed, INT64_MIN for none) and `out`, the EncoderSet the
     flushed windows are appended to.  add() puts datapoints into open windows, consume() flushes the windows that
     ended by a target time.  With an annotation capacity the set keeps annotations: `ann_len` int32 [R, N] (bytes of
-    each slot's annotation, 0 for none) and `ann_bytes` uint8 [R, N, capacity], and every call is the annotated one."""
+    each slot's annotation, 0 for none) and `ann_bytes` uint8 [R, N, capacity], and every call is the annotated one.
+    A Timer set (metric_type capi.METRIC_TIMER) keeps start, count, sum and sum_sq (float64) per slot, and each slot's
+    CM stream in `streams`: "header" uint8 [R, N, 64] and the sample arrays [R, sample_capacity, N] ("value",
+    "num_ranks", "delta", "prev", "next", "heap_a", "heap_b"); every call is the Timer one."""
 
     def __init__(self, codec: BatchCodec, start: torch.Tensor, metric_type, agg_types, resolution_ns, transforms,
-                 discard_nan, open_windows, stride, out_unit, annotation_capacity=0):
+                 discard_nan, open_windows, stride, out_unit, annotation_capacity=0, sample_capacity=None, eps=1e-3,
+                 insert_and_compress_every=1024):
         assert start.dtype == torch.int64 and start.is_cuda
         self.codec = codec
         self.metric_type = int(metric_type)
@@ -895,6 +904,19 @@ class ElementSet:
         agg = torch.int64 if counter else torch.float64
         names = [("start", torch.int64), ("count", torch.int64), ("sum", agg), ("min", agg), ("max", agg),
                  ("sum_sq", agg)] + ([] if counter else [("last", torch.float64), ("last_at", torch.int64)])
+        self.streams = None
+        if self.timer:
+            if annotation_capacity:
+                raise ValueError("a Timer set takes no annotations")
+            if sample_capacity is None or int(sample_capacity) < 1:
+                raise ValueError("a Timer set needs sample_capacity >= 1")
+            names = [("start", torch.int64), ("count", torch.int64), ("sum", torch.float64),
+                     ("sum_sq", torch.float64)]
+            self.eps, self.insert_and_compress_every = float(eps), int(insert_and_compress_every)
+            self.streams = {"header": torch.zeros((R, N, capi.TIMER_STREAM_HEADER_BYTES), dtype=torch.uint8,
+                                                  device=dev)}
+            for f, t in self._STREAM_ARRAYS:
+                self.streams[f] = torch.zeros((R, int(sample_capacity), N), dtype=t, device=dev)
         self.win = {f: torch.zeros((R, N), dtype=t, device=dev) for f, t in names}
         self.elem = torch.zeros((N, capi.ELEMENT_STATE_BYTES), dtype=torch.uint8, device=dev)
         self.watermark = torch.empty(N, dtype=torch.int64, device=dev)
@@ -908,9 +930,31 @@ class ElementSet:
         self.out = EncoderSet(codec, start.repeat(k), stride) if stride else None
         self.reset(start)
 
+    _STREAM_ARRAYS = (("value", torch.float64), ("num_ranks", torch.int64), ("delta", torch.int64),
+                      ("prev", torch.int32), ("next", torch.int32), ("heap_a", torch.float64),
+                      ("heap_b", torch.float64))
+
+    @property
+    def timer(self) -> bool:
+        return self.metric_type == capi.METRIC_TIMER
+
     @property
     def open_windows(self) -> int:
         return self.win["start"].shape[0]
+
+    @property
+    def sample_capacity(self) -> int:
+        return 0 if self.streams is None else self.streams["value"].shape[1]
+
+    def _streams(self):
+        st = capi.ElementTimerStreams()
+        st.d_header = self.streams["header"].data_ptr()
+        for f, _ in self._STREAM_ARRAYS:
+            setattr(st, "d_" + f, self.streams[f].data_ptr())
+        st.sample_capacity = self.sample_capacity
+        st.insert_and_compress_every = self.insert_and_compress_every
+        st.eps = self.eps
+        return st
 
     def _desc(self):
         w = self.win
@@ -961,7 +1005,7 @@ class ElementSet:
             self.ann_len.zero_()
 
     def add(self, ts: torch.Tensor, values: torch.Tensor, n_points: Optional[torch.Tensor] = None,
-            annotations=None):
+            annotations=None, batch: Optional[torch.Tensor] = None):
         """AddUnion of point-major ts / values int64 / float64 [P, N]: element s takes n_points[s] (int32 [N]; all P
         when None) of its column, in order.  Returns (result int8 [P, N]: 0 added, else ERR_AGGREGATION_CLOSED /
         ERR_CAPACITY / ERR_INVALID_ARG, rows past an element's count left 0; status int32 [N]: OK, ERR_CAPACITY --
@@ -969,7 +1013,12 @@ class ElementSet:
         ERR_INVALID_ARG).  annotations (a set with an annotation capacity only): (series_off int64 [N + 1], entries
         capi.AnnotationEntry rows as uint8 [E, 16], bytes uint8) as EncoderSet.append takes them, dp_index counting
         rows of the element's column; an annotation longer than the capacity stops the element with ERR_CAPACITY
-        (grow(annotation_capacity=...) and add again)."""
+        (grow(annotation_capacity=...) and add again).
+        A Timer set (m3tsz_element_set_add_timer): batch (int8 [P, N], optional) marks the rows that continue the
+        previous row's batch (BatchTimer; None: every row is its own, AppendTimerSample).  A batch is taken or refused
+        whole; ERR_CAPACITY (too few open windows, or more than sample_capacity values in its window's slot) stops the
+        element: grow() and add exactly the refused rows again.  A continuation in row 0, or one with another
+        timestamp than its batch's first row, refuses the element (ERR_INVALID_ARG, untouched)."""
         assert ts.dtype == torch.int64 and values.dtype == torch.float64 and ts.shape == values.shape
         assert ts.is_cuda and values.is_cuda and ts.is_contiguous() and values.is_contiguous()
         assert ts.dim() == 2 and ts.shape[1] == self.n_elements
@@ -983,6 +1032,17 @@ class ElementSet:
         if P == 0:
             return result, status
         d = self._desc()
+        if self.timer:
+            assert annotations is None, "a Timer set takes no annotations"
+            if batch is not None:
+                assert batch.dtype == torch.int8 and batch.is_cuda and batch.is_contiguous()
+                assert batch.shape == ts.shape
+            rc = capi.lib().m3tsz_element_set_add_timer(
+                self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()), _ptr(ts),
+                _ptr(values), P, _ptr(n_points), _ptr(batch), _ptr(result), _ptr(status), _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_element_set_add_timer")
+            return result, status
+        assert batch is None, "only a Timer set takes batches"
         if self.ann_len is None:
             assert annotations is None, "a set without an annotation capacity takes no annotations"
             rc = capi.lib().m3tsz_element_set_add(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
@@ -1009,6 +1069,12 @@ class ElementSet:
         dev = self.codec.device
         status = torch.empty(self.n_elements, dtype=torch.int32, device=dev)
         d = self._desc()
+        if self.timer:
+            rc = capi.lib().m3tsz_element_set_consume_timer(self.codec.ctx.handle, C.byref(self.codec.opts),
+                                                            C.byref(d), C.byref(self._streams()), int(target_ns),
+                                                            self.out_unit, _ptr(status), _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_element_set_consume_timer")
+            return status
         if self.ann_len is None:
             rc = capi.lib().m3tsz_element_set_consume(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
                                                       int(target_ns), self.out_unit, _ptr(status),
@@ -1023,9 +1089,18 @@ class ElementSet:
         return status
 
     def grow(self, open_windows: Optional[int] = None, stride: Optional[int] = None,
-             annotation_capacity: Optional[int] = None):
+             annotation_capacity: Optional[int] = None, sample_capacity: Optional[int] = None):
         """More open-window slots per element (the slots are copied; the new ones are free), larger output slots
-        (EncoderSet.grow) and / or, for a set that keeps annotations, more annotation bytes per slot (copied)."""
+        (EncoderSet.grow) and / or, for a set that keeps annotations, more annotation bytes per slot (copied), or for a
+        Timer set more stream samples per slot (copied)."""
+        if sample_capacity is not None and sample_capacity != self.sample_capacity:
+            assert self.timer and sample_capacity > self.sample_capacity
+            C0 = self.sample_capacity
+            for f, a in self.streams.items():
+                if f != "header":
+                    b = torch.zeros((a.shape[0], int(sample_capacity), a.shape[2]), dtype=a.dtype, device=a.device)
+                    b[:, :C0] = a
+                    self.streams[f] = b
         if open_windows is not None and open_windows != self.open_windows:
             R = self.open_windows
             assert open_windows > R
@@ -1040,6 +1115,11 @@ class ElementSet:
                                  device=self.ann_bytes.device)
                 by[:R] = self.ann_bytes
                 self.ann_len, self.ann_bytes = ln, by
+            if self.streams is not None:
+                for f, a in self.streams.items():
+                    b = torch.zeros((open_windows,) + tuple(a.shape[1:]), dtype=a.dtype, device=a.device)
+                    b[:R] = a
+                    self.streams[f] = b
         if annotation_capacity is not None and annotation_capacity != self.annotation_capacity:
             assert self.ann_bytes is not None and annotation_capacity > self.annotation_capacity
             by = torch.zeros(tuple(self.ann_bytes.shape[:2]) + (int(annotation_capacity),), dtype=torch.uint8,
@@ -1072,6 +1152,8 @@ class ElementSet:
         too: groups.grow(annotation_capacity=...) and forward again with exactly the failed groups.  A group set
         without annotations takes the plain call, whatever this set keeps."""
         assert isinstance(groups, ElementSet)
+        if self.timer or groups.timer:
+            raise ValueError("Timer sets take no forward")
         if groups.ann_len is not None and self.ann_len is None:
             raise ValueError("a group set that keeps annotations needs a source set that keeps them")
         assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
@@ -1099,9 +1181,11 @@ class ElementSet:
 
     def state(self):
         """Copies of the element-side state: {"win": {field: [R, N]}, "elem": uint8 [N, 160], "watermark": [N]},
-        and with annotations "ann_len" [R, N] and "ann_bytes" [R, N, capacity]."""
+        with annotations "ann_len" [R, N] and "ann_bytes" [R, N, capacity], and for a Timer set "streams"."""
         st = {"win": {f: a.clone() for f, a in self.win.items()}, "elem": self.elem.clone(),
               "watermark": self.watermark.clone()}
         if self.ann_len is not None:
             st["ann_len"], st["ann_bytes"] = self.ann_len.clone(), self.ann_bytes.clone()
+        if self.streams is not None:
+            st["streams"] = {f: a.clone() for f, a in self.streams.items()}
         return st

@@ -6,6 +6,7 @@
 // m3tsz_ctx_create fails with M3TSZ_ERR_NO_DEVICE.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1242,21 +1243,44 @@ int m3tsz_aggregate_tiles_rollup_annotated(
 static bool element_set_no_output(const m3tsz_element_set *set) {
   return !set->d_out_state && !set->d_out_buf && set->out_stride == 0;
 }
+// A Timer's type list (IsValidForTimer: all but Last), strictly ascending, up to M3TSZ_MAX_TIMER_TYPES without ops
+static bool parse_timer_element(const int32_t *types, uint32_t n_types, const int32_t *ops, uint32_t n_ops,
+                                TileTransforms &xf) {
+  if (!types || n_types == 0 || n_types > (n_ops ? M3TSZ_MAX_ELEMENT_TYPES : M3TSZ_MAX_TIMER_TYPES)) return false;
+  for (uint32_t j = 0; j < n_types; j++)
+    if (types[j] < M3TSZ_AGG_MIN || types[j] > M3TSZ_AGG_P75 || (j && types[j] <= types[j - 1])) return false;
+  xf.types = types;
+  xf.n_types = n_types;
+  xf.multi = true;
+  return parse_transforms(ops, n_ops, xf);
+}
+
+// timer: the set must be a Timer set (the Timer calls), else it must not be one (every other call but the reset)
 static bool element_params(const m3tsz_options *opts, const m3tsz_element_set *set, ElementParams &p,
-                           TileTransforms &xf) {
+                           TileTransforms &xf, bool timer = false) {
   if (!valid_opts(opts) || !set || set->reserved != 0) return false;
   const m3tsz_element_set &e = *set;
   const bool counter = e.metric_type == M3TSZ_METRIC_COUNTER;
+  if (timer != (e.metric_type == M3TSZ_METRIC_TIMER)) return false;
   if (e.n_windows == 0 || e.n_windows > M3TSZ_MAX_ELEMENT_WINDOWS || e.resolution_ns <= 0 ||
       e.n_elements > (1ull << 40) ||
-      !parse_element(e.metric_type, e.agg_types, e.n_types, e.ops, e.n_ops, e.d_elem, xf))
+      !(timer ? parse_timer_element(e.agg_types, e.n_types, e.ops, e.n_ops, xf)
+              : parse_element(e.metric_type, e.agg_types, e.n_types, e.ops, e.n_ops, e.d_elem, xf)))
     return false;
   auto a8 = [](const void *q) { return q && !((uintptr_t)q & 7u); };
   auto a16 = [](const void *q) { return q && !((uintptr_t)q & 15u); };
-  if (!a8(e.d_win_start) || !a8(e.d_win_count) || !a8(e.d_win_sum) || !a8(e.d_win_min) || !a8(e.d_win_max) ||
-      !a8(e.d_win_sum_sq) || (!counter && (!a8(e.d_win_last) || !a8(e.d_win_last_at))) || !a16(e.d_elem) ||
-      !a8(e.d_watermark))
+  if (timer) {  // (a Timer's slots: start, count, sum, sum_sq)
+    if (!a8(e.d_win_start) || !a8(e.d_win_count) || !a8(e.d_win_sum) || !a8(e.d_win_sum_sq) || !a16(e.d_elem) ||
+        !a8(e.d_watermark))
+      return false;
+    for (const void *q : {(const void *)e.d_win_min, (const void *)e.d_win_max, (const void *)e.d_win_last,
+                          (const void *)e.d_win_last_at})
+      if ((uintptr_t)q & 7u) return false;
+  } else if (!a8(e.d_win_start) || !a8(e.d_win_count) || !a8(e.d_win_sum) || !a8(e.d_win_min) ||
+             !a8(e.d_win_max) || !a8(e.d_win_sum_sq) || (!counter && (!a8(e.d_win_last) || !a8(e.d_win_last_at))) ||
+             !a16(e.d_elem) || !a8(e.d_watermark)) {
     return false;
+  }
   // a set without output (NULL output arrays, out_stride 0) is a rollup's source set: every call but the consume
   // takes it
   if (!element_set_no_output(set) && (!a16(e.d_out_state) || !a16(e.d_out_buf) || (e.out_stride & 15u) ||
@@ -1279,7 +1303,8 @@ static bool element_params(const m3tsz_options *opts, const m3tsz_element_set *s
   p.last_at = e.d_win_last_at;
   p.elem = e.d_elem;
   p.watermark = e.d_watermark;
-  for (uint32_t j = 0; j < xf.n_types; j++) p.types |= (uint32_t)xf.types[j] << (4 * j);
+  if (!timer)
+    for (uint32_t j = 0; j < xf.n_types; j++) p.types |= (uint32_t)xf.types[j] << (4 * j);
   p.n_types = xf.n_types;
   p.ops = xf.ops;
   p.discard_nan = (xf.ops && e.discard_nan) ? 1 : 0;  // (as m3tsz_aggregate_tiles_types)
@@ -1302,7 +1327,8 @@ int m3tsz_element_set_reset(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3t
                             const int64_t *d_start, void *stream) {
   ElementParams p;
   TileTransforms xf;
-  if (!ctx || !element_params(opts, set, p, xf) || (p.n && !d_start && !element_set_no_output(set)))
+  if (!ctx || !set || !element_params(opts, set, p, xf, set->metric_type == M3TSZ_METRIC_TIMER) ||
+      (p.n && !d_start && !element_set_no_output(set)))
     return M3TSZ_ERR_INVALID_ARG;
   if (p.n == 0) return M3TSZ_OK;
   DeviceGuard guard(ctx->device);
@@ -1464,6 +1490,127 @@ int m3tsz_element_set_consume_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
                                         const m3tsz_element_annotations *ann, int64_t target_ns, int32_t out_unit,
                                         int32_t *d_status, void *stream) {
   return element_set_consume(ctx, opts, set, ann, target_ns, out_unit, d_status, stream, true);
+}
+
+// ---- Timer element sets ----
+// aggregation.Type.Quantile()
+static double timer_quantile(int32_t t) {
+  static const double q[] = {0.1, 0.2, 0.3, 0.4, 0.5, 0.6, 0.7, 0.8, 0.9, 0.95, 0.99, 0.999, 0.9999, 0.25, 0.75};
+  if (t == M3TSZ_AGG_MEDIAN) return 0.5;
+  return t >= M3TSZ_AGG_P10 && t <= M3TSZ_AGG_P75 ? q[t - M3TSZ_AGG_P10] : 0.0;
+}
+
+// The Timer calls' checks: the set's (element_params), the streams' arrays and options; tp takes the set's
+// parameters, the streams, the types and their PooledQuantiles list (listed order, Median and P50 once)
+static bool timer_params(const m3tsz_options *opts, const m3tsz_element_set *set,
+                         const m3tsz_element_timer_streams *ts, ElementTimerParams &tp, TileTransforms &xf) {
+  memset(&tp, 0, sizeof(tp));
+  if (!element_params(opts, set, tp.e, xf, true) || !ts || ts->reserved != 0 || ts->sample_capacity == 0 ||
+      ts->sample_capacity > (1u << 30) || !std::isfinite(ts->eps) || !(ts->eps > 0.0) ||
+      ts->insert_and_compress_every == 0 || ts->insert_and_compress_every > 0x7fffffffu)
+    return false;
+  auto a = [](const void *q, uintptr_t m) { return q && !((uintptr_t)q & m); };
+  if (!a(ts->d_header, 7) || !a(ts->d_value, 7) || !a(ts->d_num_ranks, 7) || !a(ts->d_delta, 7) ||
+      !a(ts->d_prev, 3) || !a(ts->d_next, 3) || !a(ts->d_heap_a, 7) || !a(ts->d_heap_b, 7))
+    return false;
+  tp.hdr = ts->d_header;
+  tp.value = ts->d_value;
+  tp.num_ranks = ts->d_num_ranks;
+  tp.delta = ts->d_delta;
+  tp.prev = ts->d_prev;
+  tp.next = ts->d_next;
+  tp.heap_a = ts->d_heap_a;
+  tp.heap_b = ts->d_heap_b;
+  tp.cap = ts->sample_capacity;
+  tp.every = (int32_t)ts->insert_and_compress_every;
+  tp.eps = ts->eps;
+  tp.n_types = xf.n_types;
+  bool median = false;
+  for (uint32_t j = 0; j < xf.n_types; j++) {
+    const int32_t t = xf.types[j];
+    tp.type[j] = t;
+    const double q = timer_quantile(t);
+    if (q == 0.0) continue;
+    if (t == M3TSZ_AGG_P50 || t == M3TSZ_AGG_MEDIAN) {
+      if (median) continue;
+      median = true;
+    }
+    tp.q[tp.n_q++] = q;
+  }
+  return true;
+}
+
+int m3tsz_element_set_add_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                const m3tsz_element_timer_streams *streams, const int64_t *d_ts, const double *d_val,
+                                uint64_t points_stride, const uint32_t *d_n_points, const int8_t *d_batch,
+                                int8_t *d_result, int32_t *d_status, void *stream) {
+  ElementTimerParams tp;
+  TileTransforms xf;
+  if (!ctx || !timer_params(opts, set, streams, tp, xf) || points_stride > 0xffffffffull) return M3TSZ_ERR_INVALID_ARG;
+  if (tp.e.n == 0) return M3TSZ_OK;
+  if (!d_ts || !d_val || !d_result || !d_status || ((uintptr_t)d_ts & 7u) || ((uintptr_t)d_val & 7u) ||
+      ((uintptr_t)d_n_points & 3u) || ((uintptr_t)d_status & 3u))
+    return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  tp.e.ts = d_ts;
+  tp.e.val = d_val;
+  tp.e.points_stride = points_stride;
+  tp.e.n_points = d_n_points;
+  tp.e.result = d_result;
+  tp.e.status = d_status;
+  tp.batch = d_batch;
+  CK(launch_element_timer_add(tp, (cudaStream_t)stream));
+  ctx->launches++;
+  return M3TSZ_OK;
+}
+
+// element_set_consume with the Timer's consume kernel: the same scratch rows, append and status pass
+int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                    const m3tsz_element_timer_streams *streams, int64_t target_ns, int32_t out_unit,
+                                    int32_t *d_status, void *stream) {
+  ElementTimerParams tp;
+  TileTransforms xf;
+  if (!ctx || !timer_params(opts, set, streams, tp, xf) || element_set_no_output(set) || !unit_is_valid(out_unit))
+    return M3TSZ_ERR_INVALID_ARG;
+  ElementParams &p = tp.e;
+  if (p.n == 0) return M3TSZ_OK;
+  if (!d_status || ((uintptr_t)d_status & 3u)) return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  cudaStream_t st = (cudaStream_t)stream;
+  ScratchFence fence(ctx, st);
+  const uint64_t kn = (uint64_t)tp.n_types * p.n;
+  const uint64_t rows = (uint64_t)p.n_slots * (xf.reset ? 2u : 1u);
+  void *d_ts = nullptr, *d_val = nullptr, *d_n = nullptr, *d_rst = nullptr, *d_app = nullptr;
+  int rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowTs, kn * rows * 8, &d_ts))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowVal, kn * rows * 8, &d_val))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowN, kn * 4, &d_n))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowStatus, kn * 4, &d_rst))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemRowAppended, kn * 4, &d_app))) return rc;
+  p.target = target_ns;
+  p.row_ts = (int64_t *)d_ts;
+  p.row_val = (double *)d_val;
+  p.row_n = (uint32_t *)d_n;
+  p.rows_stride = rows;
+  p.status = d_status;
+  CK(launch_element_timer_consume(tp, st));
+  m3tsz_encode_extras ex;
+  memset(&ex, 0, sizeof(ex));
+  ex.point_major_input = 1;
+  EncodeParams ep;
+  if (!encode_params(opts, p.row_ts, p.row_val, kn, rows, p.row_n, nullptr, out_unit, nullptr, nullptr, nullptr,
+                     nullptr, nullptr, (int32_t *)d_rst, &ex, ep, true))
+    return M3TSZ_ERR_INVALID_ARG;
+  ep.out = set->d_out_buf;
+  ep.out_stride = set->out_stride;
+  ep.state = set->d_out_state;
+  ep.n_appended = (uint32_t *)d_app;
+  CK(launch_encode_append(ep, opts->int_optimized != 0, st));
+  CK(launch_element_status((const int32_t *)d_rst, p.n, tp.n_types, d_status, st));
+  ctx->launches += 3;
+  return M3TSZ_OK;
 }
 
 // The forward kernel writes each source's due windows to scratch, the fold kernel folds them into the groups' windows

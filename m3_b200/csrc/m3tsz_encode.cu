@@ -2925,6 +2925,557 @@ cudaError_t launch_element_status(const int32_t *row_status, uint64_t n, uint32_
 }
 
 // ---------------------------------------------------------------------------
+// Timer element sets (DESIGN.md §4.12): aggregation.Timer over cm.Stream, one lane per element
+// ---------------------------------------------------------------------------
+// One window slot's cm.Stream (aggregation/quantile/cm/stream.go), its header in registers and its entries in the
+// slot's arena: entry i at at(i) = base + i * n.  The list (sampleList) is linked by index; its arena and free list
+// are not observable, only the logical list is.  The two pending minHeaps (heap.go) are kept as the reference's
+// arrays, pushed and sorted exactly as written there, since where -0 / +0 and NaN land depends on both.  Every
+// float -> int64 conversion is Go's (go_f64_to_i64) and every operation is rounded on its own.
+struct CmStream {
+  m3tsz_timer_stream_header h;
+  double *value, *ha, *hb;
+  int64_t *nr, *dl;
+  int32_t *prv, *nxt;
+  uint64_t base, n;
+  double eps;
+  int32_t every;
+  const double *q;
+  uint32_t nq;
+
+  __device__ __forceinline__ uint64_t at(int32_t i) const { return base + (uint64_t)i * n; }
+  __device__ __forceinline__ double *less() const { return h.less_is_b ? hb : ha; }
+  __device__ __forceinline__ double *more() const { return h.less_is_b ? ha : hb; }
+  __device__ __forceinline__ int32_t &n_less() { return h.less_is_b ? h.n_b : h.n_a; }
+  __device__ __forceinline__ int32_t &n_more() { return h.less_is_b ? h.n_a : h.n_b; }
+
+  // NewStream + ResetSetData: an empty stream
+  __device__ __forceinline__ void init() {
+    h.num_values = 0;
+    h.compress_min_rank = 0;
+    h.head = h.tail = h.insert_cursor = h.compress_cursor = -1;
+    h.n_samples = h.n_used = 0;
+    h.free_head = -1;
+    h.counter = 0;
+    h.n_a = h.n_b = 0;
+    h.less_is_b = 0;
+    h.reserved = 0;
+  }
+  __device__ __forceinline__ int32_t size() const { return h.n_samples + h.n_a + h.n_b; }
+  // minHeap.Push: append, then sift up
+  __device__ __forceinline__ static void heap_push(double *hp, uint64_t base, uint64_t n, int32_t &len, double v) {
+    int32_t i = len++;
+    hp[base + (uint64_t)i * n] = v;
+    while (i > 0) {
+      const int32_t parent = (i - 1) / 2;
+      const double pv = hp[base + (uint64_t)parent * n], iv = hp[base + (uint64_t)i * n];
+      if (pv <= iv) break;
+      hp[base + (uint64_t)parent * n] = iv;
+      hp[base + (uint64_t)i * n] = pv;
+      i = parent;
+    }
+  }
+  // minHeap.SortDesc: the in-place heapsort (Pop in a loop)
+  __device__ __forceinline__ void sort_desc(double *hp, int32_t len) const {
+    for (int32_t m = len - 1; m > 0; m--) {
+      double t = hp[at(0)];
+      hp[at(0)] = hp[at(m)];
+      hp[at(m)] = t;
+      int32_t i = 0, smallest = 0;
+      for (;;) {
+        const int32_t left = smallest * 2 + 1, right = left + 1;
+        if (left < m && hp[at(left)] < hp[at(smallest)]) smallest = left;
+        if (right < m && hp[at(right)] < hp[at(smallest)]) smallest = right;
+        if (smallest == i) break;
+        t = hp[at(i)];
+        hp[at(i)] = hp[at(smallest)];
+        hp[at(smallest)] = t;
+        i = smallest;
+      }
+    }
+  }
+  __device__ __forceinline__ int32_t acquire(double v, int64_t delta) {
+    int32_t k;
+    if (h.free_head >= 0) {
+      k = h.free_head;
+      h.free_head = nxt[at(k)];
+    } else {
+      k = h.n_used++;
+    }
+    value[at(k)] = v;
+    nr[at(k)] = 1;
+    dl[at(k)] = delta;
+    h.n_samples++;
+    return k;
+  }
+  __device__ __forceinline__ void push_back(int32_t k) {
+    prv[at(k)] = h.tail;
+    nxt[at(k)] = -1;
+    if (h.head < 0)
+      h.head = k;
+    else
+      nxt[at(h.tail)] = k;
+    h.tail = k;
+  }
+  __device__ __forceinline__ void insert_before(int32_t k, int32_t mark) {
+    const int32_t p = prv[at(mark)];
+    if (p < 0)
+      h.head = k;
+    else
+      nxt[at(p)] = k;
+    prv[at(mark)] = k;
+    nxt[at(k)] = mark;
+    prv[at(k)] = p;
+  }
+  __device__ __forceinline__ void remove(int32_t k) {
+    const int32_t p = prv[at(k)], x = nxt[at(k)];
+    nxt[at(k)] = h.free_head;
+    h.free_head = k;
+    h.n_samples--;
+    if (p < 0)
+      h.head = x;
+    else
+      nxt[at(p)] = x;
+    if (x < 0)
+      h.tail = p;
+    else
+      prv[at(x)] = p;
+  }
+  __device__ __forceinline__ void reset_insert_cursor() {
+    h.less_is_b ^= 1;
+    h.insert_cursor = h.head;
+  }
+  // the smallest allowed error over the quantile list at `rank` (threshold(); compress's inner loop at maxRank)
+  __device__ __forceinline__ int64_t min_threshold(int64_t rank) const {
+    int64_t mn = INT64_MAX;
+    const int64_t num = h.num_values;
+    const double e2 = __dmul_rn(2.0, eps);
+    for (uint32_t i = 0; i < nq; i++) {
+      int64_t qm;
+      if (rank >= go_f64_to_i64(__dmul_rn(q[i], (double)num)))
+        qm = go_f64_to_i64(__ddiv_rn(__dmul_rn(e2, (double)rank), q[i]));
+      else
+        qm = go_f64_to_i64(__ddiv_rn(__dmul_rn(e2, (double)(num - rank)), __dsub_rn(1.0, q[i])));
+      if (qm < mn) mn = qm;
+    }
+    return mn;
+  }
+  __device__ __forceinline__ void insert() {
+    const int32_t cc = h.compress_cursor;
+    const double comp_value = cc >= 0 ? value[at(cc)] : xf_bits(0x7ff8000000000001ull);
+    double *vals = more();
+    const int32_t len = n_more();
+    sort_desc(vals, len);
+    int32_t idx = len - 1;
+    while (h.insert_cursor >= 0 && idx >= 0) {  // (idx < 0 only walks the rest of the list)
+      const int32_t curr = h.insert_cursor;
+      const double ipv = value[at(curr)];
+      while (idx >= 0 && vals[at(idx)] <= ipv) {
+        const double v = vals[at(idx)];
+        idx--;
+        const int32_t k = acquire(v, nr[at(curr)] + dl[at(curr)] - 1);
+        insert_before(k, curr);
+        if (comp_value >= v) h.compress_min_rank++;
+        h.num_values++;
+      }
+      h.insert_cursor = nxt[at(curr)];
+    }
+    if (h.insert_cursor < 0) {
+      while (idx >= 0 && vals[at(idx)] >= value[at(h.tail)]) {
+        const int32_t k = acquire(vals[at(idx)], 0);
+        idx--;
+        push_back(k);
+        h.num_values++;
+      }
+    }
+    n_more() = 0;  // (values left over, a NaN's, are dropped)
+    reset_insert_cursor();
+  }
+  __device__ __forceinline__ void compress() {
+    if (h.n_samples < 3) return;
+    if (h.compress_cursor < 0) {
+      const int32_t c = prv[at(h.tail)];
+      h.compress_min_rank = h.num_values - 1 - nr[at(c)];
+      h.compress_cursor = prv[at(c)];
+    }
+    while (h.compress_cursor != h.head) {
+      const int32_t curr = h.compress_cursor, next = nxt[at(curr)], prev = prv[at(curr)];
+      const int64_t c_nr = nr[at(curr)];
+      const int64_t threshold = min_threshold(h.compress_min_rank + c_nr + dl[at(curr)]);
+      h.compress_min_rank -= c_nr;
+      const int64_t n_nr = nr[at(next)];
+      if (c_nr + n_nr + dl[at(next)] <= threshold) {
+        if (h.insert_cursor == curr) h.insert_cursor = next;
+        nr[at(next)] = n_nr + c_nr;
+        remove(curr);
+      }
+      h.compress_cursor = prev;
+    }
+    h.compress_cursor = -1;
+  }
+  // AddBatch of the values v(0) .. v(len - 1)
+  template <class V>
+  __device__ __forceinline__ void add_batch(uint32_t len, V v) {
+    uint32_t i = 0;
+    if (h.n_samples == 0) {
+      push_back(acquire(v(0), 0));
+      h.insert_cursor = h.head;
+      h.num_values++;
+      i = 1;
+    }
+    const double ipv = value[at(h.insert_cursor)];  // (read once: stale after an insert inside the batch)
+    int32_t counter = h.counter;
+    for (; i < len; i++) {
+      const double x = v(i);
+      if (x < ipv)
+        heap_push(less(), base, n, n_less(), x);
+      else
+        heap_push(more(), base, n, n_more(), x);
+      if (counter == every) {
+        insert();
+        compress();
+        counter = 0;
+      }
+      counter++;
+    }
+    h.counter = counter;
+  }
+  // Flush, then calcQuantiles into cq[0 .. nq) (0 where it sets nothing, as a new stream's buffer)
+  __device__ __forceinline__ void flush(double *cq, int64_t *rank, int64_t *thr) {
+    while (h.n_a > 0 || h.n_b > 0) {
+      if (n_more() == 0) reset_insert_cursor();
+      insert();
+      compress();
+    }
+    for (uint32_t i = 0; i < nq; i++) cq[i] = 0.0;
+    if (nq == 0 || h.num_values == 0) return;
+    if (h.num_values <= 3) {  // quantilesFromBuf
+      double buf[3];
+      int32_t m = 0;
+      for (int32_t c = h.head; c >= 0 && m < 3; c = nxt[at(c)]) buf[m++] = value[at(c)];
+      for (uint32_t i = 0; i < nq; i++) {
+        int64_t k = go_f64_to_i64(__dmul_rn(q[i], (double)m));
+        if (k >= m) k = m - 1;
+        cq[i] = buf[k];
+      }
+      return;
+    }
+    for (uint32_t i = 0; i < nq; i++) {
+      rank[i] = go_f64_to_i64(ceil(__dmul_rn(q[i], (double)h.num_values)));
+      thr[i] = go_f64_to_i64(ceil(__ddiv_rn((double)min_threshold(rank[i]), 2.0)));
+    }
+    int64_t min_rank = 0, max_rank = 0;
+    uint32_t idx = 0;
+    int32_t curr = h.head, prev = h.head;
+    while (curr >= 0 && idx < nq) {
+      max_rank = min_rank + nr[at(curr)] + dl[at(curr)];
+      if (max_rank > rank[idx] + thr[idx] || min_rank > rank[idx]) cq[idx++] = value[at(prev)];
+      min_rank += nr[at(curr)];
+      prev = curr;
+      curr = nxt[at(curr)];
+    }
+    for (uint32_t i = idx; i < nq; i++)
+      if (max_rank >= rank[i] + thr[i] || min_rank > rank[i]) cq[i] = value[at(prev)];
+  }
+};
+
+__device__ __forceinline__ CmStream timer_stream(const ElementTimerParams &p, uint32_t r, uint64_t s) {
+  CmStream c;
+  c.value = p.value;
+  c.ha = p.heap_a;
+  c.hb = p.heap_b;
+  c.nr = p.num_ranks;
+  c.dl = p.delta;
+  c.prv = p.prev;
+  c.nxt = p.next;
+  c.base = (uint64_t)r * p.cap * p.e.n + s;
+  c.n = p.e.n;
+  c.eps = p.eps;
+  c.every = p.every;
+  c.q = p.q;
+  c.nq = p.n_q;
+  return c;
+}
+
+// One amd64 SSE operation's result r = a op b as Go's Timer sees it (its sums take NaN samples, unlike the Gauge's):
+// a NaN operand comes through quieted, the first one when both are; an invalid operation on other operands gives
+// the default NaN 0xFFF8000000000000.  (The GPU would write its canonical NaN instead.)
+__device__ __forceinline__ double amd64_op(double r, double a, double b) {
+  if (r == r) return r;
+  if (a != a) return __longlong_as_double(__double_as_longlong(a) | 0x0008000000000000ll);
+  if (b != b) return __longlong_as_double(__double_as_longlong(b) | 0x0008000000000000ll);
+  return __longlong_as_double((long long)0xFFF8000000000000ull);
+}
+// aggregation.stdev over a Timer's sums, with amd64_op's NaN rule (math.Sqrt of a negative is the default NaN)
+__device__ __forceinline__ double timer_stdev(int64_t count, double sum_sq, double sum) {
+  const int64_t div = (int64_t)((uint64_t)count * (uint64_t)(count - 1));
+  if (div == 0) return 0.0;
+  const double cf = __ll2double_rn(count), df = __ll2double_rn(div);
+  const double a = amd64_op(__dmul_rn(cf, sum_sq), cf, sum_sq), b = amd64_op(__dmul_rn(sum, sum), sum, sum);
+  const double num = amd64_op(__dsub_rn(a, b), a, b);
+  const double x = amd64_op(__ddiv_rn(num, df), num, df);
+  if (x != x) return x;
+  return x < 0.0 ? __longlong_as_double((long long)0xFFF8000000000000ull) : __dsqrt_rn(x);
+}
+
+// aggregation.Type.Quantile(): the quantile of a quantile type, 0 for the others
+__device__ __forceinline__ double timer_type_quantile(int32_t t) {
+  switch (t) {
+    case M3TSZ_AGG_P10: return 0.1;
+    case M3TSZ_AGG_P20: return 0.2;
+    case M3TSZ_AGG_P25: return 0.25;
+    case M3TSZ_AGG_P30: return 0.3;
+    case M3TSZ_AGG_P40: return 0.4;
+    case M3TSZ_AGG_P50: case M3TSZ_AGG_MEDIAN: return 0.5;
+    case M3TSZ_AGG_P60: return 0.6;
+    case M3TSZ_AGG_P70: return 0.7;
+    case M3TSZ_AGG_P75: return 0.75;
+    case M3TSZ_AGG_P80: return 0.8;
+    case M3TSZ_AGG_P90: return 0.9;
+    case M3TSZ_AGG_P95: return 0.95;
+    case M3TSZ_AGG_P99: return 0.99;
+    case M3TSZ_AGG_P999: return 0.999;
+    case M3TSZ_AGG_P9999: return 0.9999;
+    default: return 0.0;
+  }
+}
+
+// Timer.ValueOf of a flushed window: count values, their sum / sumSq, the stream's ends and its quantiles cq
+__device__ __forceinline__ double timer_value_of(const ElementTimerParams &p, int32_t t, int64_t cnt, double sum,
+                                                 double sq, double front, double back, const double *cq) {
+  const double qt = timer_type_quantile(t);
+  if (qt > 0.0) {  // Quantile(q): the first listed quantile >= q
+    for (uint32_t i = 0; i < p.n_q; i++)
+      if (p.q[i] >= qt) return cq[i];
+    return xf_bits(0x7ff8000000000001ull);
+  }
+  switch (t) {
+    case M3TSZ_AGG_MIN: return front;
+    case M3TSZ_AGG_MAX: return back;
+    case M3TSZ_AGG_MEAN: return amd64_op(__ddiv_rn(sum, (double)cnt), sum, (double)cnt);
+    case M3TSZ_AGG_COUNT: return (double)cnt;
+    case M3TSZ_AGG_SUM: return sum;
+    case M3TSZ_AGG_SUMSQ: return sq;
+    case M3TSZ_AGG_STDEV: return timer_stdev(cnt, sq, sum);
+    default: return 0.0;
+  }
+}
+
+// Timer.AddBatch of element s's batches in row order (m3tsz_element_set_add_timer).  A first pass checks the batch
+// marks; each batch then finds its window's slot (or a free one), checks the slot's room and adds to it.
+__device__ __forceinline__ void elem_timer_add_lane(const ElementTimerParams &tp, uint64_t s) {
+  const ElementParams &p = tp.e;
+  const uint32_t n_pts = p.n_points ? p.n_points[s] : (uint32_t)p.points_stride;
+  if (n_pts > p.points_stride) {
+    p.status[s] = M3TSZ_ERR_INVALID_ARG;
+    return;
+  }
+  auto cont = [&](uint32_t i) { return tp.batch && tp.batch[(uint64_t)i * p.n + s] != 0; };
+  bool bad = n_pts && cont(0);
+  int64_t t0 = 0;
+  for (uint32_t i = 0; i < n_pts && !bad; i++) {
+    const int64_t t = p.ts[(uint64_t)i * p.n + s];
+    if (!cont(i))
+      t0 = t;
+    else if (t != t0)
+      bad = true;
+  }
+  if (bad) {
+    for (uint32_t i = 0; i < n_pts; i++) p.result[(uint64_t)i * p.n + s] = (int8_t)M3TSZ_ERR_INVALID_ARG;
+    p.status[s] = M3TSZ_ERR_INVALID_ARG;
+    return;
+  }
+  const int64_t wm = p.watermark[s];
+  int32_t status = M3TSZ_OK;
+  uint32_t i = 0;
+  while (i < n_pts) {
+    uint32_t j = i + 1;
+    while (j < n_pts && cont(j)) j++;
+    const uint32_t len = j - i;
+    int res = M3TSZ_ERR_CAPACITY;
+    if (status == M3TSZ_OK) {
+      const int64_t t = p.ts[(uint64_t)i * p.n + s];
+      int64_t ws = 0;
+      if (!elem_window_start(t, p.resolution, p.trunc_off, ws)) {
+        res = M3TSZ_ERR_INVALID_ARG;
+      } else if (elem_ends_by(ws, p.resolution, wm)) {
+        res = M3TSZ_ERR_AGGREGATION_CLOSED;
+      } else {
+        int hit = -1, fr = -1;
+        for (uint32_t r = 0; r < p.n_slots; r++) {
+          const uint64_t o = (uint64_t)r * p.n + s;
+          if (p.count[o] == 0) {
+            if (fr < 0) fr = (int)r;
+          } else if (p.start[o] == ws) {
+            hit = (int)r;
+            break;
+          }
+        }
+        const int r = hit >= 0 ? hit : fr;
+        CmStream c;
+        if (r >= 0) {
+          c = timer_stream(tp, (uint32_t)r, s);
+          if (hit >= 0)
+            c.h = tp.hdr[(uint64_t)r * p.n + s];
+          else
+            c.init();
+        }
+        if (r < 0 || (uint64_t)c.size() + len > tp.cap) {
+          status = res = M3TSZ_ERR_CAPACITY;
+        } else {
+          const uint64_t o = (uint64_t)r * p.n + s;
+          int64_t cnt = 0;
+          double sum = 0.0, sq = 0.0;
+          if (hit >= 0) {
+            cnt = p.count[o];
+            sum = static_cast<const double *>(p.sum)[o];
+            sq = static_cast<const double *>(p.sum_sq)[o];
+          }
+          for (uint32_t k = i; k < j; k++) {
+            const double v = p.val[(uint64_t)k * p.n + s];
+            sum = amd64_op(__dadd_rn(sum, v), sum, v);
+            const double v2 = amd64_op(__dmul_rn(v, v), v, v);
+            sq = amd64_op(__dadd_rn(sq, v2), sq, v2);
+          }
+          c.add_batch(len, [&](uint32_t k) { return p.val[(uint64_t)(i + k) * p.n + s]; });
+          p.start[o] = ws;
+          p.count[o] = cnt + len;
+          static_cast<double *>(p.sum)[o] = sum;
+          static_cast<double *>(p.sum_sq)[o] = sq;
+          tp.hdr[o] = c.h;
+          res = M3TSZ_OK;
+        }
+      }
+    }
+    for (uint32_t k = i; k < j; k++) p.result[(uint64_t)k * p.n + s] = (int8_t)res;
+    i = j;
+  }
+  p.status[s] = status;
+}
+
+// Consume(target) of Timer element s, as elem_consume_lane: the same room check, window order, staging and commit;
+// each due window's stream is flushed and its quantiles computed here.  More than M3TSZ_MAX_ELEMENT_TYPES types come
+// without ops: each type's row takes every window's value, and the record is not touched.
+__device__ __forceinline__ void elem_timer_consume_lane(const ElementTimerParams &tp, uint64_t s, XfElem &e) {
+  const ElementParams &p = tp.e;
+  const uint64_t kn = (uint64_t)tp.n_types * p.n;
+  uint32_t m = 0;
+  for (uint32_t r = 0; r < p.n_slots; r++) {
+    const uint64_t o = (uint64_t)r * p.n + s;
+    if (p.count[o] != 0 && elem_ends_by(p.start[o], p.resolution, p.target)) m++;
+  }
+  bool reset = false;
+  for (int k = 0; k < M3TSZ_MAX_TRANSFORMS; k++) reset |= ((p.ops >> (4 * k)) & 0xfu) == M3TSZ_TRANSFORM_RESET;
+  int32_t status = M3TSZ_OK;
+  if (m) {  // (elem_consume_lane's room check)
+    const uint64_t per_row = (uint64_t)m * (reset ? 2u : 1u);
+    for (uint32_t j = 0; j < tp.n_types; j++) {
+      const m3tsz_encoder_state &oe = p.out_state[(uint64_t)j * p.n + s];
+      const uint64_t bits = oe.bits + (oe.num_encoded ? 0u : 64u) + (per_row - 1) * 163u;
+      if ((bits >> 5) + ENC_GUARD + 4 > p.out_slot_words) status = M3TSZ_ERR_CAPACITY;
+    }
+  }
+  if (m == 0 || status != M3TSZ_OK) {
+    for (uint32_t j = 0; j < tp.n_types; j++) p.row_n[(uint64_t)j * p.n + s] = 0;
+    p.status[s] = status;
+    return;
+  }
+  const bool xf = tp.n_types <= M3TSZ_MAX_ELEMENT_TYPES;
+  if (xf) {
+    const m3tsz_element_state &r = p.elem[s];
+    e.w = r.head;
+    e.pv[0] = r.head.prev_v;
+    for (int j = 1; j < M3TSZ_MAX_ELEMENT_TYPES; j++) e.pv[j] = r.prev_v_more[j - 1];
+  }
+  uint64_t rows = 0;  // type j's datapoints so far in bits 8j .. 8j + 7 (xf)
+  int64_t prev = 0;
+  for (uint32_t w = 0; w < m; w++) {
+    int best = -1;
+    int64_t bs = 0;
+    for (uint32_t r = 0; r < p.n_slots; r++) {
+      const uint64_t o = (uint64_t)r * p.n + s;
+      if (p.count[o] == 0) continue;
+      const int64_t ws = p.start[o];
+      if (!elem_ends_by(ws, p.resolution, p.target) || (w && ws <= prev)) continue;
+      if (best < 0 || ws < bs) {
+        best = (int)r;
+        bs = ws;
+      }
+    }
+    prev = bs;
+    const uint64_t o = (uint64_t)best * p.n + s;
+    const int64_t cnt = p.count[o];
+    const double sum = static_cast<const double *>(p.sum)[o], sq = static_cast<const double *>(p.sum_sq)[o];
+    const int64_t t = bs + p.resolution;
+    CmStream c = timer_stream(tp, (uint32_t)best, s);
+    c.h = tp.hdr[o];
+    double cq[M3TSZ_MAX_TIMER_QUANTILES];
+    int64_t rank[M3TSZ_MAX_TIMER_QUANTILES], thr[M3TSZ_MAX_TIMER_QUANTILES];
+    c.flush(cq, rank, thr);
+    const double front = c.value[c.at(c.h.head)], back = c.value[c.at(c.h.tail)];
+    auto value_of = [&](uint32_t i) { return timer_value_of(tp, tp.type[i], cnt, sum, sq, front, back, cq); };
+    if (xf) {
+      xf_element_window(p.ops, p.resolution, e, 0u, tp.n_types, t, value_of, [&](uint32_t i, double v, int64_t extra_t) {
+        if (p.discard_nan && xf_isnan(v)) return;
+        const uint64_t d = (rows >> (8 * i)) & 0xffu;
+        uint64_t a = d * kn + (uint64_t)i * p.n + s;
+        p.row_ts[a] = t;
+        p.row_val[a] = v;
+        if (extra_t != 0) {
+          a += kn;
+          p.row_ts[a] = extra_t;
+          p.row_val[a] = 0.0;
+        }
+        rows += (uint64_t)(extra_t != 0 ? 2u : 1u) << (8 * i);
+      });
+    } else {
+      for (uint32_t i = 0; i < tp.n_types; i++) {
+        const uint64_t a = (uint64_t)w * kn + (uint64_t)i * p.n + s;
+        p.row_ts[a] = t;
+        p.row_val[a] = value_of(i);
+      }
+    }
+    p.count[o] = 0;  // the slot is free; its stream is made anew when an add opens it
+  }
+  p.watermark[s] = prev + p.resolution;
+  if (xf) {
+    m3tsz_element_state &r = p.elem[s];
+    r.head = e.w;
+    r.head.prev_v = e.pv[0];
+    for (int j = 1; j < M3TSZ_MAX_ELEMENT_TYPES; j++) r.prev_v_more[j - 1] = e.pv[j];
+  }
+  for (uint32_t j = 0; j < tp.n_types; j++)
+    p.row_n[(uint64_t)j * p.n + s] = xf ? (uint32_t)((rows >> (8 * j)) & 0xffu) : m;
+  p.status[s] = M3TSZ_OK;
+}
+
+// (__maxnreg__ rather than __launch_bounds__: under the latter ptxas held these two at 80 registers and spilled around
+// the double-division calls of the stream's thresholds; with 128 neither spills)
+__global__ void __maxnreg__(128) element_timer_add_kernel(const ElementTimerParams p) {
+  const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (s < p.e.n) elem_timer_add_lane(p, s);
+}
+__global__ void __maxnreg__(128) element_timer_consume_kernel(const ElementTimerParams p) {
+  __shared__ XfElem rec[ELEM_THREADS];
+  const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (s < p.e.n) elem_timer_consume_lane(p, s, rec[threadIdx.x]);
+}
+
+cudaError_t launch_element_timer_add(const ElementTimerParams &p, cudaStream_t stream) {
+  if (p.e.n == 0) return cudaSuccess;
+  if ((p.e.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  element_timer_add_kernel<<<elem_blocks(p.e.n), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_element_timer_consume(const ElementTimerParams &p, cudaStream_t stream) {
+  if (p.e.n == 0) return cudaSuccess;
+  if ((p.e.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  element_timer_consume_kernel<<<elem_blocks(p.e.n), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------
 // element sets through a rollup (DESIGN.md §4.12): forward, fold, commit
 // ---------------------------------------------------------------------------
 // Consume(target) of source s of a rollup pipeline (generic_elem.go:912-937): its windows ending at or before

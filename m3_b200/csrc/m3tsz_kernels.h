@@ -396,6 +396,29 @@ cudaError_t launch_element_consume(const ElementParams &p, cudaStream_t stream);
 cudaError_t launch_element_status(const int32_t *row_status, uint64_t n, uint32_t n_types, int32_t *status,
                                   cudaStream_t stream);
 
+// Timer element sets (m3tsz_element_set_*_timer; m3tsz_encode.cu): the set's slots and rows in `e` (its types and
+// n_types unused; e.ops / e.discard_nan as in the other sets), each slot's CM stream in the m3tsz_element_timer_streams
+// arrays (slot o = r * n + s, its entry i at (r * cap + i) * n + s), and the element's types and quantile list here
+#define M3TSZ_MAX_TIMER_TYPES 23
+#define M3TSZ_MAX_TIMER_QUANTILES 15
+struct ElementTimerParams {
+  ElementParams e;
+  m3tsz_timer_stream_header *hdr;
+  double *value;
+  int64_t *num_ranks, *delta;
+  int32_t *prev, *next;
+  double *heap_a, *heap_b;
+  uint32_t cap;
+  int32_t every;  // insertAndCompressEvery
+  double eps;
+  const int8_t *batch;  // add: optional [points_stride][n], nonzero continues the previous row's batch
+  uint32_t n_types, n_q;
+  int32_t type[M3TSZ_MAX_TIMER_TYPES];
+  double q[M3TSZ_MAX_TIMER_QUANTILES];  // Types.PooledQuantiles of type[]
+};
+cudaError_t launch_element_timer_add(const ElementTimerParams &p, cudaStream_t stream);
+cudaError_t launch_element_timer_consume(const ElementTimerParams &p, cudaStream_t stream);
+
 // element sets through a rollup (m3tsz_element_set_forward; m3tsz_encode.cu): the source set's forward (one lane per
 // source), the fold into the group set's windows (one warp per group) and the sources' commit (one lane per source)
 struct ElementRollupParams {

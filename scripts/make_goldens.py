@@ -806,6 +806,52 @@ def main():
     with open(OUT_ELEM_CONSUME, "w") as f:
         json.dump(elem_consume, f, indent=1)
     print("wrote", OUT_ELEM_CONSUME)
+    timer_goldens()
+
+
+def timer_goldens():
+    """tests/golden/m3tsz_timer_goldens.json: the reference's exact Timer and CM stream expectations, transcribed from
+    its tests (values as written there; the "tolerance" cases state a property instead of values).  Types are
+    aggregation.Type ids; "batches" lists [values, times]: AddBatch(values) `times` times, in order; eps / every are
+    the stream options."""
+    out = os.path.join(os.path.dirname(OUT), "m3tsz_timer_goldens.json")
+    default = [2, 3, 4, 5, 6, 7, 8, 9, 14, 19, 20]  # the default Timer types, ascending
+    batch_timer = [1.0, 3.5, 2.2, 6.5, 4.8]
+    cases = [
+        {"name": "TestTimerAggregations", "src_line": "aggregator/aggregation/timer_test.go:109-180",
+         "eps": 1e-3, "every": 1024, "batches": [[[float(i)], 1] for i in range(1, 101)],
+         "types": [2, 3, 4, 5, 6, 7, 8, 14, 19, 20],
+         "want": {"2": 1.0, "3": 100.0, "4": 50.5, "5": 50.0, "6": 100.0, "7": 5050.0, "8": 338350.0, "14": 50.0,
+                  "19": 95.0}},
+        {"name": "TestTimerElemBatchTimer", "src_line": "aggregator/aggregator/elem_test.go:84-88,3196-3210",
+         "eps": 1e-3, "every": 1024, "batches": [[batch_timer, 1]], "types": default,
+         "want": {"7": 18.0, "8": 83.38, "4": 3.6, "2": 1.0, "3": 6.5, "6": 5.0, "9": 2.15522620622523, "5": 3.5,
+                  "14": 3.5, "19": 6.5, "20": 6.5}},
+        {"name": "TestStreamWithOnePositiveSample", "src_line": "aggregator/aggregation/quantile/cm/stream_test.go:56-68",
+         "eps": 0.01, "every": 1024, "batches": [[[100.0], 1]], "types": [2, 3, 14, 18, 20],
+         "want": {"2": 100.0, "3": 100.0, "14": 100.0, "18": 100.0, "20": 100.0}},
+        {"name": "TestStreamWithOneNegativeSample", "src_line": "aggregator/aggregation/quantile/cm/stream_test.go:70-82",
+         "eps": 0.01, "every": 1024, "batches": [[[-100.0], 1]], "types": [2, 3, 14, 18, 20],
+         "want": {"2": -100.0, "3": -100.0, "14": -100.0, "18": -100.0, "20": -100.0}},
+        {"name": "TestStreamWithThreeSamples", "src_line": "aggregator/aggregation/quantile/cm/stream_test.go:84-99",
+         "eps": 0.01, "every": 1024, "batches": [[[100.0], 1], [[200.0], 1], [[300.0], 1]], "types": [2, 3, 14, 18, 20],
+         "want": {"2": 100.0, "3": 300.0, "14": 200.0, "18": 300.0, "20": 300.0}},
+    ]
+    for every in (1024, 100):
+        cases.append({"name": "TestStreamWithSkewedDistribution/every=%d" % every,
+                      "src_line": "aggregator/aggregation/quantile/cm/stream_test.go:206-221", "eps": 0.01,
+                      "every": every, "batches": [[[1.0], 10000], [[10000000.0], 1]], "types": [2, 3, 14, 18, 20],
+                      "want": {"2": 1.0, "3": 10000000.0, "14": 1.0, "18": 1.0, "20": 1.0}})
+    tolerance = []
+    for order in ("increasing", "decreasing"):
+        for every in (1024, 100):
+            tolerance.append({"name": "TestStreamWith%sSamples/every=%d" % (order.capitalize(), every),
+                              "src_line": "aggregator/aggregation/quantile/cm/stream_test.go:144-176",
+                              "order": order, "n": 100000, "eps": 0.01, "every": every, "types": [2, 3, 14, 18, 20],
+                              "quantiles": {"14": 0.5, "18": 0.9, "20": 0.99}})
+    with open(out, "w") as f:
+        json.dump({"cases": cases, "tolerance": tolerance}, f, indent=1)
+    print("wrote", out)
 
 
 if __name__ == "__main__":
