@@ -1189,7 +1189,8 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
  *   - A set of more than M3TSZ_MAX_ELEMENT_TYPES types has no ops and leaves its records untouched; up to that many,
  *     the records are kept as for the other sets.
  * m3tsz_element_set_reset takes a Timer set as any other; add, consume, their annotated forms and forward refuse it
- * (M3TSZ_ERR_INVALID_ARG before any launch), as the tile and downsample calls refuse metric type 2.
+ * (M3TSZ_ERR_INVALID_ARG before any launch), as the tile and downsample calls refuse metric type 2; a Timer rollup
+ * forwards with m3tsz_element_set_forward_timer.
  *
  * Each window slot's stream lives in caller-owned device memory, pointer-free (growing R or the capacity is a copy).
  * Slot o = r * n_elements + s; its sample i (list sample or pending heap entry) at (r * sample_capacity + i) *
@@ -1249,6 +1250,49 @@ int m3tsz_element_set_add_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const
 int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
                                     const m3tsz_element_timer_streams *streams, int64_t target_ns, int32_t out_unit,
                                     int32_t *d_status, void *stream);
+
+/* Timer element sets through a rollup (DESIGN.md §4.12): m3tsz_element_set_forward for Timer sets.  A Timer source
+ * with a rollup pipeline forwards ValueOf(its type) through its pre-rollup ops (generic_elem.go:860-937); the forwarded
+ * metric keeps its type, so each group window is a Timer and AddUnique is Timer.Add of each value
+ * (generic_elem.go:276-281, aggregation/timer.go:52-76).
+ *   - src: a Timer set with exactly one type (any but Last, e.g. P99, Max or Mean), its ops the pre-rollup ops and its
+ *     discard_nan the pipeline's; it usually has no output.  src_streams: its streams.
+ *   - groups: a Timer set of the same resolution_ns with n_elements == n_groups, the rollup's types and the
+ *     remainder's ops; m3tsz_element_set_consume_timer consumes it.  group_streams: its streams.
+ *   - group g is the sources d_members[d_group_off[g] .. d_group_off[g + 1]), as in m3tsz_element_set_forward.
+ * Rules:
+ *   1. Forward: every source takes its open windows that end at or before target_ns, in start order.  Each window's
+ *      stream is Flushed and gives ValueOf(the source type), which goes through the ops on the source's record as
+ *      m3tsz_element_set_consume_timer computes a type's value (a Reset forwards nothing extra).  discard_nan drops a
+ *      NaN value with or without ops.  Each flushed stream header is written back to its slot, since the flush
+ *      rewrote the slot's samples; a Flush with empty heaps only recomputes the quantiles, so a held-back source
+ *      forwards the same bits when called again.
+ *   2. Fold: every group takes its members in listed order, and each member's forwarded windows in start order, into
+ *      the group window with the same start as the source window, opening a slot if needed.  Each value is one
+ *      Timer.Add: count + 1, sum and sumSq in order (NaN included, as m3tsz_element_set_add_timer sums them), then
+ *      AddBatch of that one value.  k values into one window are k one-value batches, not one batch of k (each reads
+ *      the insertion point afresh, which changes the quantiles).  A member listed twice is folded twice.
+ *   3. A group window that ends at or before the group's watermark is closed: its values are dropped and the group
+ *      gets M3TSZ_ERR_AGGREGATION_CLOSED; its other windows still fold.
+ *   4. Capacity: a group with fewer free slots than new windows, or with a window this call touches whose list
+ *      samples + pending values + the values this call folds into it (0 + n for a new window) exceed
+ *      group_streams->sample_capacity, gets M3TSZ_ERR_CAPACITY, and nothing is folded into it.  The sample bound
+ *      ignores the room the fold's compressions free, so it is deterministic: growing and calling again gives the
+ *      unstopped result.
+ *   5. Invalid group and 6. commit: rules 5 and 6 of m3tsz_element_set_forward.  A held-back source keeps its
+ *      windows, counts, sums, record and watermark; its due streams stay flushed in place (rule 1).  So after
+ *      growing the group set's open windows and / or sample capacity, calling again with exactly the failed groups
+ *      gives the result of one unstopped call.
+ * Host checks (M3TSZ_ERR_INVALID_ARG before any launch): those of m3tsz_element_set_forward, those of
+ * m3tsz_element_set_add_timer for both sets and stream structs, either set not a Timer set, a source type list other
+ * than one type, and source and group sets sharing slot or stream arrays.  m3tsz_element_set_forward and
+ * m3tsz_element_set_forward_annotated keep refusing Timer sets. */
+int m3tsz_element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                    const m3tsz_element_timer_streams *src_streams, int64_t target_ns,
+                                    const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                    uint64_t n_groups, const m3tsz_element_set *groups,
+                                    const m3tsz_element_timer_streams *group_streams, int32_t *d_src_status,
+                                    int32_t *d_group_status, void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

@@ -304,7 +304,8 @@ class BatchCodec:
         capi.METRIC_TIMER (m3tsz_element_set_*_timer): every type but Last (up to capi.MAX_TIMER_TYPES without
         transformations), each open window an aggregation.Timer over the CM stream with `eps` and
         `insert_and_compress_every` (the aggregator's StreamOptions), holding at most `sample_capacity` values (list
-        samples and pending values together; required).  A Timer set takes no annotations and no forward."""
+        samples and pending values together; required).  A Timer set takes no annotations, and forwards through a
+        rollup with ElementSet.forward_timer, not forward."""
         return ElementSet(self, start, metric_type, agg_types, resolution_ns, transforms, discard_nan, open_windows,
                           stride, out_unit, annotation_capacity, sample_capacity, eps, insert_and_compress_every)
 
@@ -1150,7 +1151,7 @@ class ElementSet:
         forwarded window carries its annotation, and each value with one replaces its group window's annotation, in
         the listed member order.  A group whose forwarded annotation is longer than its capacity gets ERR_CAPACITY
         too: groups.grow(annotation_capacity=...) and forward again with exactly the failed groups.  A group set
-        without annotations takes the plain call, whatever this set keeps."""
+        without annotations takes the plain call, whatever this set keeps.  Timer sets forward with forward_timer."""
         assert isinstance(groups, ElementSet)
         if self.timer or groups.timer:
             raise ValueError("Timer sets take no forward")
@@ -1177,6 +1178,34 @@ class ElementSet:
             _ptr(members), members.numel(), G, C.byref(gd), C.byref(ga), _ptr(src_status), _ptr(group_status),
             _cuda_stream_ptr(dev))
         self.codec.ctx.check(rc, "m3tsz_element_set_forward_annotated")
+        return src_status[: self.n_elements], group_status[:G]
+
+    def forward_timer(self, target_ns, group_off: torch.Tensor, members: torch.Tensor, groups: "ElementSet"):
+        """forward for Timer sets (m3tsz_element_set_forward_timer, DESIGN.md §4.12), with the same arguments and
+        return values: this set (one type, any but Last; its transformations the pre-rollup ones) flushes each due
+        window's stream and forwards ValueOf(its type); group g of `groups` (a Timer set of the same resolution)
+        takes each value as one Timer.Add into its window with the source window's start, members in listed order.
+        A group gets ERR_CAPACITY when it needs more windows than it has free slots, or when a window it touches
+        would hold more than groups.sample_capacity values: its list samples and pending values plus every value
+        this call folds into it.  Nothing is then folded into the group and its members are held back:
+        groups.grow(open_windows=..., sample_capacity=...) and forward again with exactly the failed groups, which
+        gives the result of one unstopped call."""
+        assert isinstance(groups, ElementSet)
+        if not (self.timer and groups.timer):
+            raise ValueError("forward_timer takes Timer sets; other sets forward with forward")
+        assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
+        assert members.is_cuda and members.dtype == torch.int32 and members.is_contiguous()
+        G = group_off.numel() - 1
+        assert G >= 0, "group_off has G + 1 entries"
+        dev = self.codec.device
+        src_status = torch.empty(max(1, self.n_elements), dtype=torch.int32, device=dev)
+        group_status = torch.empty(max(1, G), dtype=torch.int32, device=dev)
+        d, gd = self._desc(), groups._desc()
+        rc = capi.lib().m3tsz_element_set_forward_timer(
+            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()), int(target_ns),
+            _ptr(group_off), _ptr(members), members.numel(), G, C.byref(gd), C.byref(groups._streams()),
+            _ptr(src_status), _ptr(group_status), _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_forward_timer")
         return src_status[: self.n_elements], group_status[:G]
 
     def state(self):

@@ -1613,6 +1613,57 @@ int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   return M3TSZ_OK;
 }
 
+// The forward calls' status arrays: present and aligned where there are sources / groups
+static bool forward_statuses_ok(uint64_t S, uint64_t n_groups, const int32_t *d_src_status,
+                                const int32_t *d_group_status) {
+  return !((S && (!d_src_status || ((uintptr_t)d_src_status & 3u))) ||
+           (n_groups && (!d_group_status || ((uintptr_t)d_group_status & 3u))));
+}
+
+// The forward calls' scratch (the forwarded windows, records and commit marks) and the rest of rp: the call's
+// groups and the group set gp's slots
+static int element_forward_scratch(m3tsz_ctx *ctx, ScratchFence &fence, ElementRollupParams &rp,
+                                   const ElementParams &gp, int64_t target_ns, const uint64_t *d_group_off,
+                                   const uint32_t *d_members, uint64_t n_members, uint64_t n_groups,
+                                   int32_t *d_src_status, int32_t *d_group_status, int32_t discard_nan) {
+  const uint64_t sn = rp.src.n ? rp.src.n : 1;  // (the fold reads nothing of the sources when there are none)
+  void *d_fs, *d_fv, *d_fn, *d_fp, *d_fd, *d_rec, *d_mark;
+  int rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdStart, (size_t)sn * rp.src.n_slots * 8, &d_fs))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdVal, (size_t)sn * rp.src.n_slots * 8, &d_fv))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdN, sn * 4, &d_fn))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdPresent, sn * 8, &d_fp))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdDue, sn * 8, &d_fd))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdRec, sn * sizeof(m3tsz_transform_state), &d_rec))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdMark, sn * 4, &d_mark))) return rc;
+  rp.src.target = target_ns;
+  rp.discard_nan = discard_nan ? 1 : 0;  // (generic_elem.go:892-894: with or without transformations)
+  rp.fwd_start = (int64_t *)d_fs;
+  rp.fwd_val = (double *)d_fv;
+  rp.fwd_n = (uint32_t *)d_fn;
+  rp.fwd_present = (uint64_t *)d_fp;
+  rp.fwd_due = (uint64_t *)d_fd;
+  rp.rec = (m3tsz_transform_state *)d_rec;
+  rp.group_off = d_group_off;
+  rp.members = d_members;
+  rp.n_members = n_members;
+  rp.n_groups = n_groups;
+  rp.g_slots = gp.n_slots;
+  rp.g_start = gp.start;
+  rp.g_count = gp.count;
+  rp.g_sum = gp.sum;
+  rp.g_min = gp.min;
+  rp.g_max = gp.max;
+  rp.g_sum_sq = gp.sum_sq;
+  rp.g_last = gp.last;
+  rp.g_last_at = gp.last_at;
+  rp.g_watermark = gp.watermark;
+  rp.group_status = d_group_status;
+  rp.mark = (int32_t *)d_mark;
+  rp.src_status = d_src_status;
+  return M3TSZ_OK;
+}
+
 // The forward kernel writes each source's due windows to scratch, the fold kernel folds them into the groups' windows
 // and marks the members of the groups that failed, and the commit kernel frees the other sources' due windows.
 // m3tsz_element_set_forward(_annotated): annotated, the forward also writes which forwarded windows carry an
@@ -1646,27 +1697,18 @@ static int element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
       for (int j = 0; j < 2; j++)
         if (overlap(sa[i], sb[i], ga[j], gb[j])) return M3TSZ_ERR_INVALID_ARG;
   }
-  const uint64_t S = rp.src.n;
-  if ((S && (!d_src_status || ((uintptr_t)d_src_status & 3u))) ||
-      (n_groups && (!d_group_status || ((uintptr_t)d_group_status & 3u))))
-    return M3TSZ_ERR_INVALID_ARG;
-  if (S == 0 && n_groups == 0) return M3TSZ_OK;
+  if (!forward_statuses_ok(rp.src.n, n_groups, d_src_status, d_group_status)) return M3TSZ_ERR_INVALID_ARG;
+  if (rp.src.n == 0 && n_groups == 0) return M3TSZ_OK;
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
   cudaStream_t st = (cudaStream_t)stream;
   ScratchFence fence(ctx, st);
-  const uint64_t sn = S ? S : 1;  // (the fold reads nothing of the sources when there are none)
-  void *d_fs, *d_fv, *d_fn, *d_fp, *d_fd, *d_rec, *d_mark;
-  int rc;
-  if ((rc = ensure(ctx, fence, kSlotElemFwdStart, (size_t)sn * rp.src.n_slots * 8, &d_fs))) return rc;
-  if ((rc = ensure(ctx, fence, kSlotElemFwdVal, (size_t)sn * rp.src.n_slots * 8, &d_fv))) return rc;
-  if ((rc = ensure(ctx, fence, kSlotElemFwdN, sn * 4, &d_fn))) return rc;
-  if ((rc = ensure(ctx, fence, kSlotElemFwdPresent, sn * 8, &d_fp))) return rc;
-  if ((rc = ensure(ctx, fence, kSlotElemFwdDue, sn * 8, &d_fd))) return rc;
-  if ((rc = ensure(ctx, fence, kSlotElemFwdRec, sn * sizeof(m3tsz_transform_state), &d_rec))) return rc;
-  if ((rc = ensure(ctx, fence, kSlotElemFwdMark, sn * 4, &d_mark))) return rc;
+  int rc = element_forward_scratch(ctx, fence, rp, gp, target_ns, d_group_off, d_members, n_members, n_groups,
+                                   d_src_status, d_group_status, src->discard_nan);
+  if (rc != M3TSZ_OK) return rc;
   if (annotated) {
     void *d_fap, *d_fa;
+    const uint64_t sn = rp.src.n ? rp.src.n : 1;
     if ((rc = ensure(ctx, fence, kSlotElemFwdAnnPresent, sn * 8, &d_fap))) return rc;
     if ((rc = ensure(ctx, fence, kSlotElemFwdAnn, (size_t)sn * rp.src.n_slots * 8, &d_fa))) return rc;
     rp.fwd_ann_present = (uint64_t *)d_fap;
@@ -1675,32 +1717,7 @@ static int element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
     rp.g_ann_slot = gp.ann_slot;
     rp.g_ann_cap = gp.ann_cap;
   }
-  rp.src.target = target_ns;
-  rp.discard_nan = src->discard_nan ? 1 : 0;  // (generic_elem.go:892-894: with or without transformations)
-  rp.fwd_start = (int64_t *)d_fs;
-  rp.fwd_val = (double *)d_fv;
-  rp.fwd_n = (uint32_t *)d_fn;
-  rp.fwd_present = (uint64_t *)d_fp;
-  rp.fwd_due = (uint64_t *)d_fd;
-  rp.rec = (m3tsz_transform_state *)d_rec;
-  rp.group_off = d_group_off;
-  rp.members = d_members;
-  rp.n_members = n_members;
-  rp.n_groups = n_groups;
-  rp.g_slots = gp.n_slots;
-  rp.g_start = gp.start;
-  rp.g_count = gp.count;
-  rp.g_sum = gp.sum;
-  rp.g_min = gp.min;
-  rp.g_max = gp.max;
-  rp.g_sum_sq = gp.sum_sq;
-  rp.g_last = gp.last;
-  rp.g_last_at = gp.last_at;
-  rp.g_watermark = gp.watermark;
-  rp.group_status = d_group_status;
-  rp.mark = (int32_t *)d_mark;
-  rp.src_status = d_src_status;
-  CK(cudaMemsetAsync(d_mark, 0, sn * 4, st));
+  CK(cudaMemsetAsync(rp.mark, 0, (rp.src.n ? rp.src.n : 1) * 4, st));
   CK(launch_element_forward(rp, st));
   CK(launch_element_fold(rp, st));
   CK(launch_element_commit(rp, st));
@@ -1724,6 +1741,55 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
                                         int32_t *d_group_status, void *stream) {
   return element_set_forward(ctx, opts, src, src_ann, target_ns, d_group_off, d_members, n_members, n_groups, groups,
                              group_ann, d_src_status, d_group_status, stream, true);
+}
+
+// element_set_forward with the Timer forward and fold kernels: the same groups, scratch and commit
+int m3tsz_element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                    const m3tsz_element_timer_streams *src_streams, int64_t target_ns,
+                                    const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                    uint64_t n_groups, const m3tsz_element_set *groups,
+                                    const m3tsz_element_timer_streams *group_streams, int32_t *d_src_status,
+                                    int32_t *d_group_status, void *stream) {
+  ElementTimerParams sp, gt;
+  TileTransforms sx, gx;
+  if (!ctx || !timer_params(opts, src, src_streams, sp, sx) || !timer_params(opts, groups, group_streams, gt, gx))
+    return M3TSZ_ERR_INVALID_ARG;
+  if (src->resolution_ns != groups->resolution_ns || sx.n_types != 1 || n_groups != groups->n_elements ||
+      n_members > (1ull << 40) || (n_groups && !d_group_off) || (n_members && !d_members) ||
+      ((uintptr_t)d_group_off & 7u) || ((uintptr_t)d_members & 3u))
+    return M3TSZ_ERR_INVALID_ARG;
+  // the two sets share no slot or stream array: the forward rewrites the source streams and the fold the group ones
+  const uint64_t sl = (uint64_t)sp.e.n_slots * sp.e.n, gl = (uint64_t)gt.e.n_slots * gt.e.n;
+  const uint64_t se = sl * sp.cap, ge = gl * gt.cap;
+  const void *sa[] = {sp.e.start, sp.e.count, sp.e.sum, sp.e.sum_sq, sp.hdr, sp.value, sp.num_ranks, sp.delta,
+                      sp.prev, sp.next, sp.heap_a, sp.heap_b};
+  const void *ga[] = {gt.e.start, gt.e.count, gt.e.sum, gt.e.sum_sq, gt.hdr, gt.value, gt.num_ranks, gt.delta,
+                      gt.prev, gt.next, gt.heap_a, gt.heap_b};
+  const uint64_t sb[] = {sl * 8, sl * 8, sl * 8, sl * 8, sl * 64, se * 8, se * 8, se * 8, se * 4, se * 4, se * 8, se * 8};
+  const uint64_t gb[] = {gl * 8, gl * 8, gl * 8, gl * 8, gl * 64, ge * 8, ge * 8, ge * 8, ge * 4, ge * 4, ge * 8, ge * 8};
+  for (int i = 0; i < 12; i++)
+    for (int j = 0; j < 12; j++)
+      if (sb[i] && gb[j] && (uintptr_t)sa[i] < (uintptr_t)ga[j] + gb[j] && (uintptr_t)ga[j] < (uintptr_t)sa[i] + sb[i])
+        return M3TSZ_ERR_INVALID_ARG;
+  if (!forward_statuses_ok(sp.e.n, n_groups, d_src_status, d_group_status)) return M3TSZ_ERR_INVALID_ARG;
+  if (sp.e.n == 0 && n_groups == 0) return M3TSZ_OK;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  cudaStream_t st = (cudaStream_t)stream;
+  ScratchFence fence(ctx, st);
+  ElementRollupParams rp;
+  memset(&rp, 0, sizeof(rp));
+  rp.src = sp.e;
+  int rc = element_forward_scratch(ctx, fence, rp, gt.e, target_ns, d_group_off, d_members, n_members, n_groups,
+                                   d_src_status, d_group_status, src->discard_nan);
+  if (rc != M3TSZ_OK) return rc;
+  sp.e = rp.src;
+  CK(cudaMemsetAsync(rp.mark, 0, (rp.src.n ? rp.src.n : 1) * 4, st));
+  CK(launch_element_timer_forward(rp, sp, st));
+  CK(launch_element_timer_fold(rp, gt, st));
+  CK(launch_element_commit(rp, st));
+  ctx->launches += 3;
+  return M3TSZ_OK;
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

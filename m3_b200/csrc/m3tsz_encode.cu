@@ -3878,6 +3878,250 @@ cudaError_t launch_element_commit(const ElementRollupParams &p, cudaStream_t str
 }
 
 // ---------------------------------------------------------------------------
+// Timer element sets through a rollup (DESIGN.md §4.12): the Timer forward and fold; the commit is the one above
+// ---------------------------------------------------------------------------
+// elem_forward_lane for Timer source s (tp: the source set's streams, tp.e = p.src): the same due windows in start
+// order and scratch, each window's value Flush + ValueOf(tp.type[0]) as elem_timer_consume_lane computes it, through
+// the pre-ops on the record's head.  Each flushed header goes back to its slot: the flush rewrote the slot's arena, and
+// a source held back keeps the flushed stream (a second Flush, its heaps empty, gives the same quantiles).
+__device__ __forceinline__ void elem_timer_forward_lane(const ElementRollupParams &p, const ElementTimerParams &tp,
+                                                        uint64_t s) {
+  const ElementParams &e = p.src;
+  uint32_t m = 0;
+  uint64_t due = 0;
+  for (uint32_t r = 0; r < e.n_slots; r++) {
+    const uint64_t o = (uint64_t)r * e.n + s;
+    if (e.count[o] != 0 && elem_ends_by(e.start[o], e.resolution, e.target)) {
+      m++;
+      due |= 1ull << r;
+    }
+  }
+  m3tsz_transform_state st = e.elem[s].head;
+  uint64_t present = 0;
+  int64_t prev = 0;
+  for (uint32_t q = 0; q < m; q++) {
+    int best = -1;
+    int64_t bs = 0;
+    for (uint32_t r = 0; r < e.n_slots; r++) {
+      if (!((due >> r) & 1u)) continue;
+      const int64_t ws = e.start[(uint64_t)r * e.n + s];
+      if (q && ws <= prev) continue;
+      if (best < 0 || ws < bs) {
+        best = (int)r;
+        bs = ws;
+      }
+    }
+    prev = bs;
+    const uint64_t o = (uint64_t)best * e.n + s;
+    CmStream c = timer_stream(tp, (uint32_t)best, s);
+    c.h = tp.hdr[o];
+    double cq[M3TSZ_MAX_TIMER_QUANTILES];
+    int64_t rank[M3TSZ_MAX_TIMER_QUANTILES], thr[M3TSZ_MAX_TIMER_QUANTILES];
+    c.flush(cq, rank, thr);
+    tp.hdr[o] = c.h;
+    double v = timer_value_of(tp, tp.type[0], e.count[o], static_cast<const double *>(e.sum)[o],
+                              static_cast<const double *>(e.sum_sq)[o], c.value[c.at(c.h.head)],
+                              c.value[c.at(c.h.tail)], cq);
+    int64_t extra_t = 0;
+    xf_window(e.ops, e.resolution, st, bs + e.resolution, v, extra_t);
+    if (!(p.discard_nan && xf_isnan(v))) present |= 1ull << q;
+    p.fwd_start[(uint64_t)q * e.n + s] = bs;
+    p.fwd_val[(uint64_t)q * e.n + s] = v;
+  }
+  p.fwd_n[s] = m;
+  p.fwd_present[s] = present;
+  p.fwd_due[s] = due;
+  p.rec[s] = st;
+}
+
+// elem_fold_group for a Timer group set (gt: its streams, gt.e.n = p.n_groups): the same checks, order and closed
+// rule, each value one Timer.Add into the group window (count + 1, the sums with amd64's NaN rule as
+// elem_timer_add_lane takes them, then AddBatch of the one value: k values are k batches, each reading the insertion
+// point afresh).  The first pass also counts each touched window's values, n_add[r] for group slot r and
+// n_add[g_slots + k] for fresh[k], and fails the group with CAPACITY where its list + pending + those values exceed
+// gt.cap (an upper bound: the fold's compressions only free room).
+template <class Member>
+__device__ __forceinline__ int32_t elem_timer_fold_group(const ElementRollupParams &p, const ElementTimerParams &gt,
+                                                         uint64_t g, int64_t *fresh, uint32_t *n_add, Member member) {
+  const uint64_t lo = p.group_off[g], hi = p.group_off[g + 1], G = p.n_groups;
+  const int64_t res = p.src.resolution, wm = p.g_watermark[g];
+  int32_t status = M3TSZ_OK;
+  auto window = [&](const FwdMember &a, uint32_t q, int64_t &ws, double &v) {
+    if (q == 0) {
+      ws = a.start0;
+      v = a.val0;
+    } else {
+      ws = p.fwd_start[(uint64_t)q * p.src.n + a.m];
+      v = p.fwd_val[(uint64_t)q * p.src.n + a.m];
+    }
+  };
+  if (lo > hi || hi > p.n_members) {
+    status = M3TSZ_ERR_INVALID_ARG;
+  } else {
+    for (uint32_t r = 0; r < 2 * p.g_slots; r++) n_add[r] = 0;
+    uint32_t n_free = 0, n_fresh = 0;
+    for (uint32_t r = 0; r < p.g_slots; r++) n_free += p.g_count[(uint64_t)r * G + g] == 0;
+    bool bad = false, full = false;
+    int last = -1;  // the n_add entry of the last window counted (a group's values mostly go to one window)
+    int64_t last_ws = 0;
+    for (uint64_t i = lo; i < hi; i++) {
+      const FwdMember a = member(i);
+      if (a.m >= p.src.n) bad = true;
+      for (uint32_t q = 0; q < a.n; q++) {
+        if (!((a.present >> q) & 1u)) continue;
+        int64_t ws;
+        double v;
+        window(a, q, ws, v);
+        if (elem_ends_by(ws, res, wm)) continue;
+        int at = -1;
+        if (last >= 0 && ws == last_ws) {
+          at = last;
+        } else {
+          for (uint32_t r = 0; r < p.g_slots && at < 0; r++) {
+            const uint64_t o = (uint64_t)r * G + g;
+            if (p.g_count[o] != 0 && p.g_start[o] == ws) at = (int)r;
+          }
+          for (uint32_t k = 0; k < n_fresh && at < 0; k++)
+            if (fresh[k] == ws) at = (int)(p.g_slots + k);
+          if (at < 0 && n_fresh < n_free) {
+            fresh[n_fresh] = ws;
+            at = (int)(p.g_slots + n_fresh++);
+          }
+        }
+        if (at < 0) {
+          full = true;
+          continue;
+        }
+        last = at;
+        last_ws = ws;
+        n_add[at]++;
+      }
+    }
+    if (!bad && !full) {
+      for (uint32_t r = 0; r < p.g_slots; r++) {
+        const uint64_t o = (uint64_t)r * G + g;
+        uint64_t size = 0;
+        if (p.g_count[o] != 0) {
+          const m3tsz_timer_stream_header &h = gt.hdr[o];
+          size = (uint64_t)h.n_samples + (uint64_t)h.n_a + (uint64_t)h.n_b;
+        }
+        if (size + n_add[r] > gt.cap) full = true;
+      }
+      for (uint32_t k = 0; k < n_fresh; k++) full |= n_add[p.g_slots + k] > gt.cap;
+    }
+    status = bad ? M3TSZ_ERR_INVALID_ARG : full ? M3TSZ_ERR_CAPACITY : M3TSZ_OK;
+  }
+  if (status == M3TSZ_OK) {
+    int cur = -1;  // the group slot the registers hold, -1: none
+    int64_t w_start = 0, cnt = 0;
+    double sum = 0.0, sq = 0.0;
+    CmStream c = timer_stream(gt, 0u, g);  // (set again for the slot whenever `cur` changes)
+    bool closed = false;
+    auto store = [&]() {
+      const uint64_t o = (uint64_t)cur * G + g;
+      p.g_start[o] = w_start;
+      p.g_count[o] = cnt;
+      static_cast<double *>(p.g_sum)[o] = sum;
+      static_cast<double *>(p.g_sum_sq)[o] = sq;
+      gt.hdr[o] = c.h;
+    };
+    for (uint64_t i = lo; i < hi; i++) {
+      const FwdMember a = member(i);
+      for (uint32_t q = 0; q < a.n; q++) {
+        if (!((a.present >> q) & 1u)) continue;
+        int64_t ws;
+        double v;
+        window(a, q, ws, v);
+        if (elem_ends_by(ws, res, wm)) {
+          closed = true;
+          continue;
+        }
+        if (cur < 0 || ws != w_start) {  // the window's slot, or a free one (the first pass counted them)
+          if (cur >= 0) store();
+          int hit = -1, fr = -1;
+          for (uint32_t r = 0; r < p.g_slots; r++) {
+            const uint64_t o = (uint64_t)r * G + g;
+            if (p.g_count[o] == 0) {
+              if (fr < 0) fr = (int)r;
+            } else if (p.g_start[o] == ws) {
+              hit = (int)r;
+              break;
+            }
+          }
+          cur = hit >= 0 ? hit : fr;
+          const uint64_t o = (uint64_t)cur * G + g;
+          w_start = ws;
+          cnt = 0;
+          sum = sq = 0.0;
+          if (hit >= 0) {
+            cnt = p.g_count[o];
+            sum = static_cast<const double *>(p.g_sum)[o];
+            sq = static_cast<const double *>(p.g_sum_sq)[o];
+          }
+          c = timer_stream(gt, (uint32_t)cur, g);
+          if (hit >= 0)
+            c.h = gt.hdr[o];
+          else
+            c.init();
+        }
+        cnt++;
+        sum = amd64_op(__dadd_rn(sum, v), sum, v);
+        const double v2 = amd64_op(__dmul_rn(v, v), v, v);
+        sq = amd64_op(__dadd_rn(sq, v2), sq, v2);
+        c.add_batch(1u, [&](uint32_t) { return v; });
+      }
+    }
+    if (cur >= 0) store();
+    if (closed) status = M3TSZ_ERR_AGGREGATION_CLOSED;
+  }
+  p.group_status[g] = status;
+  return status;
+}
+
+// (__maxnreg__ as the other Timer kernels: the stream's code is the same)
+__global__ void __maxnreg__(128) element_timer_forward_kernel(const ElementRollupParams p,
+                                                              const ElementTimerParams tp) {
+  const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (s < p.src.n) elem_timer_forward_lane(p, tp, s);
+}
+
+// One lane per group, unlike element_fold_kernel's warp per group: a group's values go through the serial stream one
+// Timer.Add at a time, so a warp that ran one group would leave 31 lanes idle; with a lane per group the warp runs 32
+// groups' folds at once (DESIGN.md §4.12 has both mappings measured).  The fresh-window starts and per-window tallies
+// are the lane's own (local memory; a group touches few of the entries).
+__global__ void __maxnreg__(128) element_timer_fold_kernel(const ElementRollupParams p, const ElementTimerParams gt) {
+  const uint64_t g = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (g >= p.n_groups) return;
+  int64_t fresh[M3TSZ_MAX_ELEMENT_WINDOWS];
+  uint32_t n_add[2 * M3TSZ_MAX_ELEMENT_WINDOWS];
+  const int32_t st = elem_timer_fold_group(p, gt, g, fresh, n_add, [&](uint64_t i) { return fwd_member(p, i); });
+  const uint64_t lo = p.group_off[g], hi = p.group_off[g + 1];
+  if ((st == M3TSZ_ERR_CAPACITY || st == M3TSZ_ERR_INVALID_ARG) && lo <= hi) {
+    const uint64_t end = hi < p.n_members ? hi : p.n_members;
+    for (uint64_t i = lo; i < end; i++) {
+      const uint32_t m = p.members[i];
+      if (m < p.src.n) atomicMax(p.mark + m, st);
+    }
+  }
+}
+
+cudaError_t launch_element_timer_forward(const ElementRollupParams &p, const ElementTimerParams &src,
+                                         cudaStream_t stream) {
+  if (p.src.n == 0) return cudaSuccess;
+  if ((p.src.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  element_timer_forward_kernel<<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p, src);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_element_timer_fold(const ElementRollupParams &p, const ElementTimerParams &groups,
+                                      cudaStream_t stream) {
+  if (p.n_groups == 0) return cudaSuccess;
+  if ((p.n_groups + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  element_timer_fold_kernel<<<elem_blocks(p.n_groups), ELEM_THREADS, 0, stream>>>(p, groups);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------
 // compaction: slots -> packed buffer with CSR offsets
 // ---------------------------------------------------------------------------
 __global__ void compact_lens_kernel(const uint64_t *len, uint64_t n, uint64_t mask, uint64_t *out) {

@@ -462,6 +462,13 @@ cudaError_t launch_element_forward(const ElementRollupParams &p, cudaStream_t st
 // (p.mark must be zero)
 cudaError_t launch_element_fold(const ElementRollupParams &p, cudaStream_t stream);
 cudaError_t launch_element_commit(const ElementRollupParams &p, cudaStream_t stream);
+// Timer sets through a rollup (m3tsz_element_set_forward_timer): p as above (its g_min / g_max / g_last unused), with
+// the source set's streams and one type in `src` and the group set's streams and quantile list in `groups`; the commit
+// is launch_element_commit's.  (p.mark must be zero for the fold.)
+cudaError_t launch_element_timer_forward(const ElementRollupParams &p, const ElementTimerParams &src,
+                                         cudaStream_t stream);
+cudaError_t launch_element_timer_fold(const ElementRollupParams &p, const ElementTimerParams &groups,
+                                      cudaStream_t stream);
 
 // exclusive scan of aligned lengths + gather into a packed buffer
 cudaError_t launch_compact(const uint8_t *slots, uint64_t slot_stride, const uint64_t *len,

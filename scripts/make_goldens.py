@@ -807,6 +807,7 @@ def main():
         json.dump(elem_consume, f, indent=1)
     print("wrote", OUT_ELEM_CONSUME)
     timer_goldens()
+    timer_rollup_goldens()
 
 
 def timer_goldens():
@@ -851,6 +852,36 @@ def timer_goldens():
                               "quantiles": {"14": 0.5, "18": 0.9, "20": 0.99}})
     with open(out, "w") as f:
         json.dump({"cases": cases, "tolerance": tolerance}, f, indent=1)
+    print("wrote", out)
+
+
+def timer_rollup_goldens():
+    """tests/golden/m3tsz_timer_rollup_goldens.json: the reference's Timer rollup expectations.  "add_unique" cases are
+    TimerElem.AddUnique calls in order ([at_s, value] each, a Timer.Add into the window of at_s) with what the reference
+    checks after a step ("count", "sum", "sum_sq", "q0.5": Quantile(0.5); sums as InEpsilon 1e-10, the rest exact).
+    "pipeline" cases are a Timer source's windows ([start_s, samples]) consumed at each target through its type and
+    pre-rollup transformations; "want" lists the forwarded [time_s, value] in order ("NaN" for a NaN), compared
+    exactly as verifyForwardedMetrics does."""
+    out = os.path.join(os.path.dirname(OUT), "m3tsz_timer_rollup_goldens.json")
+    default = [2, 3, 4, 5, 6, 7, 8, 9, 14, 19, 20]  # the default Timer types, ascending
+    add_unique = [
+        {"name": "TestTimerElemAddUnique", "src_line": "aggregator/aggregator/elem_test.go:120-125,927-999",
+         "resolution_s": 10, "types": default, "eps": 1e-3, "every": 1024,
+         "steps": [{"add": [216, 11.1]}, {"add": [216, 12.2]},
+                   {"add": [216, 13.3], "window_s": 210, "want": {"count": 3, "sum": 36.6, "q0.5": 12.2}},
+                   {"add": [217, 14.4], "window_s": 210, "want": {"count": 4, "sum": 51.0}},
+                   {"add": [221, 20.0], "window_s": 220, "want": {"count": 1, "sum": 20.0, "sum_sq": 400.0}}]},
+    ]
+    pipeline = [
+        {"name": "TestTimerElemConsumeCustomAggregationCustomPipeline",
+         "src_line": "aggregator/aggregator/elem_test.go:94-110,1138-1264", "resolution_s": 10, "src_type": 2,
+         "pre_ops": [1, 2], "discard_nan": False, "rollup_types": [3],
+         "windows": [[210, [123.0, 1245.0]], [220, [456.0]], [230, [589.0, 1120.0]]],
+         "consumes": [{"target_s": 0, "want": []}, {"target_s": 220, "want": [[220, "NaN"]]},
+                      {"target_s": 240, "want": [[230, 33.3], [240, 13.3]]}]},
+    ]
+    with open(out, "w") as f:
+        json.dump({"add_unique": add_unique, "pipeline": pipeline}, f, indent=1)
     print("wrote", out)
 
 
