@@ -1188,9 +1188,11 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
  *     calcQuantiles leaves unset reads 0, as a freshly made stream holds it.
  *   - A set of more than M3TSZ_MAX_ELEMENT_TYPES types has no ops and leaves its records untouched; up to that many,
  *     the records are kept as for the other sets.
- * m3tsz_element_set_reset takes a Timer set as any other; add, consume, their annotated forms and forward refuse it
- * (M3TSZ_ERR_INVALID_ARG before any launch), as the tile and downsample calls refuse metric type 2; a Timer rollup
- * forwards with m3tsz_element_set_forward_timer.
+ * m3tsz_element_set_reset takes a Timer set as any other; add, consume, their annotated forms, forward and
+ * forward_annotated refuse it (M3TSZ_ERR_INVALID_ARG before any launch), as the tile and downsample calls refuse metric
+ * type 2; a Timer rollup forwards with m3tsz_element_set_forward_timer.  A Timer set that keeps annotations takes
+ * m3tsz_element_set_add_timer_annotated, m3tsz_element_set_consume_timer_annotated and
+ * m3tsz_element_set_forward_timer_annotated, which refuse Gauge and Counter sets.
  *
  * Each window slot's stream lives in caller-owned device memory, pointer-free (growing R or the capacity is a copy).
  * Slot o = r * n_elements + s; its sample i (list sample or pending heap entry) at (r * sample_capacity + i) *
@@ -1293,6 +1295,53 @@ int m3tsz_element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, c
                                     uint64_t n_groups, const m3tsz_element_set *groups,
                                     const m3tsz_element_timer_streams *group_streams, int32_t *d_src_status,
                                     int32_t *d_group_status, void *stream);
+
+/* Timer element sets that keep annotations (DESIGN.md §4.12): the Timer calls with the set's window annotations in
+ * `ann` (m3tsz_element_annotations, laid out and checked as for the other sets; the lengths need no initial value).
+ * Each Timer window keeps one annotation, as aggregation.Timer does (MaybeReplaceAnnotation, timer.go:57-76).
+ *
+ * m3tsz_element_set_add_timer with annotations: the sparse list of m3tsz_element_set_add_annotated (dp_index counts
+ * rows of the element's column).  A batch has one annotation, its first row's entry, as a BatchTimer has one; with
+ * d_batch NULL every row is its own batch with its own annotation (AppendTimerSample).  An entry with a length on a
+ * continuation row breaks the batch rule: every row of the element gets M3TSZ_ERR_INVALID_ARG and it is untouched.  Per
+ * batch, after the closed and invalid-start checks (a closed batch is M3TSZ_ERR_AGGREGATION_CLOSED whatever its
+ * annotation), an annotation longer than ann->capacity gets M3TSZ_ERR_CAPACITY under the R rule: nothing of the batch
+ * or of the element's later rows in this call is added.  Then the slot and sample-room checks.  An accepted batch with
+ * a non-empty annotation replaces its window's annotation, NaN samples included; a refused batch changes none.  A
+ * window this call opens writes its slot's length (0 until an annotation arrives). */
+int m3tsz_element_set_add_timer_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                          const m3tsz_element_timer_streams *streams,
+                                          const m3tsz_element_annotations *ann, const int64_t *d_ts,
+                                          const double *d_val, uint64_t points_stride, const uint32_t *d_n_points,
+                                          const int8_t *d_batch, const uint64_t *d_ann_series_off,
+                                          const m3tsz_annotation_entry *d_ann_entries, const uint8_t *d_ann_bytes,
+                                          int8_t *d_result, int32_t *d_status, void *stream);
+
+/* m3tsz_element_set_consume_timer where every datapoint staged for a window carries the window's annotation: every
+ * type's datapoint, the Reset datapoint, and the rows of a set of more than M3TSZ_MAX_ELEMENT_TYPES types.  The room
+ * check counts each flushed datapoint's annotation as m3tsz_element_set_consume_annotated does. */
+int m3tsz_element_set_consume_timer_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                              const m3tsz_element_timer_streams *streams,
+                                              const m3tsz_element_annotations *ann, int64_t target_ns,
+                                              int32_t out_unit, int32_t *d_status, void *stream);
+
+/* m3tsz_element_set_forward_timer for Timer sets that keep annotations: src_ann and group_ann as in
+ * m3tsz_element_set_forward_annotated (both required).  Values, statuses, records, watermarks, the stream write-back
+ * and the commit are those of m3tsz_element_set_forward_timer; the annotations follow rules 1-5 of
+ * m3tsz_element_set_forward_annotated: a forwarded window carries its slot's annotation (a length of 0 or above
+ * src_ann->capacity being none); each folded value with one replaces its group window's (MaybeReplaceAnnotation
+ * through AddUnique), members in listed order and each member's windows in start order; a value that discard_nan drops
+ * carries nothing and one dropped at a closed group window changes nothing; a window the fold opens writes its length;
+ * a value that would fold with an annotation longer than group_ann->capacity fails its group with M3TSZ_ERR_CAPACITY
+ * beside the slot and sample counts (nothing folded, members held back; INVALID_ARG still wins); the source annotation
+ * arrays are only read.  Host checks: those of m3tsz_element_set_forward_timer and of
+ * m3tsz_element_set_forward_annotated's annotation structs. */
+int m3tsz_element_set_forward_timer_annotated(
+    m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+    const m3tsz_element_timer_streams *src_streams, const m3tsz_element_annotations *src_ann, int64_t target_ns,
+    const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members, uint64_t n_groups,
+    const m3tsz_element_set *groups, const m3tsz_element_timer_streams *group_streams,
+    const m3tsz_element_annotations *group_ann, int32_t *d_src_status, int32_t *d_group_status, void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

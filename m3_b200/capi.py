@@ -157,7 +157,8 @@ EXPORTED_SYMBOLS = [
     "m3tsz_element_set_reset", "m3tsz_element_set_add", "m3tsz_element_set_consume",
     "m3tsz_element_set_add_annotated", "m3tsz_element_set_consume_annotated", "m3tsz_element_set_forward",
     "m3tsz_element_set_forward_annotated", "m3tsz_element_set_add_timer", "m3tsz_element_set_consume_timer",
-    "m3tsz_element_set_forward_timer",
+    "m3tsz_element_set_forward_timer", "m3tsz_element_set_add_timer_annotated",
+    "m3tsz_element_set_consume_timer_annotated", "m3tsz_element_set_forward_timer_annotated",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -362,6 +363,14 @@ def lib():
     L.m3tsz_element_set_consume_timer.argtypes = [vp, po, pes, pts, i64, i32, vp, vp]
     L.m3tsz_element_set_forward_timer.restype = C.c_int
     L.m3tsz_element_set_forward_timer.argtypes = [vp, po, pes, pts, i64, vp, vp, u64, u64, pes, pts, vp, vp, vp]
+    L.m3tsz_element_set_add_timer_annotated.restype = C.c_int
+    L.m3tsz_element_set_add_timer_annotated.argtypes = [vp, po, pes, pts, pea, vp, vp, u64, vp, vp, vp, vp, vp, vp,
+                                                        vp, vp]
+    L.m3tsz_element_set_consume_timer_annotated.restype = C.c_int
+    L.m3tsz_element_set_consume_timer_annotated.argtypes = [vp, po, pes, pts, pea, i64, i32, vp, vp]
+    L.m3tsz_element_set_forward_timer_annotated.restype = C.c_int
+    L.m3tsz_element_set_forward_timer_annotated.argtypes = [vp, po, pes, pts, pea, i64, vp, vp, u64, u64, pes, pts,
+                                                            pea, vp, vp, vp]
     _lib = L
     return L
 

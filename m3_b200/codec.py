@@ -304,8 +304,9 @@ class BatchCodec:
         capi.METRIC_TIMER (m3tsz_element_set_*_timer): every type but Last (up to capi.MAX_TIMER_TYPES without
         transformations), each open window an aggregation.Timer over the CM stream with `eps` and
         `insert_and_compress_every` (the aggregator's StreamOptions), holding at most `sample_capacity` values (list
-        samples and pending values together; required).  A Timer set takes no annotations, and forwards through a
-        rollup with ElementSet.forward_timer, not forward."""
+        samples and pending values together; required).  With annotation_capacity a Timer set keeps annotations too
+        (m3tsz_element_set_*_timer_annotated: a batch's annotation is its first row's).  It forwards through a rollup
+        with ElementSet.forward_timer, not forward."""
         return ElementSet(self, start, metric_type, agg_types, resolution_ns, transforms, discard_nan, open_windows,
                           stride, out_unit, annotation_capacity, sample_capacity, eps, insert_and_compress_every)
 
@@ -907,8 +908,6 @@ class ElementSet:
                  ("sum_sq", agg)] + ([] if counter else [("last", torch.float64), ("last_at", torch.int64)])
         self.streams = None
         if self.timer:
-            if annotation_capacity:
-                raise ValueError("a Timer set takes no annotations")
             if sample_capacity is None or int(sample_capacity) < 1:
                 raise ValueError("a Timer set needs sample_capacity >= 1")
             names = [("start", torch.int64), ("count", torch.int64), ("sum", torch.float64),
@@ -1019,7 +1018,9 @@ class ElementSet:
         previous row's batch (BatchTimer; None: every row is its own, AppendTimerSample).  A batch is taken or refused
         whole; ERR_CAPACITY (too few open windows, or more than sample_capacity values in its window's slot) stops the
         element: grow() and add exactly the refused rows again.  A continuation in row 0, or one with another
-        timestamp than its batch's first row, refuses the element (ERR_INVALID_ARG, untouched)."""
+        timestamp than its batch's first row, refuses the element (ERR_INVALID_ARG, untouched).  With annotations
+        (m3tsz_element_set_add_timer_annotated) a batch's annotation is its first row's entry; an annotation on a
+        continuation row refuses the element the same way."""
         assert ts.dtype == torch.int64 and values.dtype == torch.float64 and ts.shape == values.shape
         assert ts.is_cuda and values.is_cuda and ts.is_contiguous() and values.is_contiguous()
         assert ts.dim() == 2 and ts.shape[1] == self.n_elements
@@ -1034,14 +1035,22 @@ class ElementSet:
             return result, status
         d = self._desc()
         if self.timer:
-            assert annotations is None, "a Timer set takes no annotations"
             if batch is not None:
                 assert batch.dtype == torch.int8 and batch.is_cuda and batch.is_contiguous()
                 assert batch.shape == ts.shape
-            rc = capi.lib().m3tsz_element_set_add_timer(
-                self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()), _ptr(ts),
-                _ptr(values), P, _ptr(n_points), _ptr(batch), _ptr(result), _ptr(status), _cuda_stream_ptr(dev))
-            self.codec.ctx.check(rc, "m3tsz_element_set_add_timer")
+            if self.ann_len is None:
+                assert annotations is None, "a set without an annotation capacity takes no annotations"
+                rc = capi.lib().m3tsz_element_set_add_timer(
+                    self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()), _ptr(ts),
+                    _ptr(values), P, _ptr(n_points), _ptr(batch), _ptr(result), _ptr(status), _cuda_stream_ptr(dev))
+                self.codec.ctx.check(rc, "m3tsz_element_set_add_timer")
+                return result, status
+            a_off, a_ent, a_bytes = annotations if annotations is not None else (None, None, None)
+            rc = capi.lib().m3tsz_element_set_add_timer_annotated(
+                self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()),
+                C.byref(self._ann()), _ptr(ts), _ptr(values), P, _ptr(n_points), _ptr(batch), _ptr(a_off),
+                _ptr(a_ent), _ptr(a_bytes), _ptr(result), _ptr(status), _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_element_set_add_timer_annotated")
             return result, status
         assert batch is None, "only a Timer set takes batches"
         if self.ann_len is None:
@@ -1070,11 +1079,17 @@ class ElementSet:
         dev = self.codec.device
         status = torch.empty(self.n_elements, dtype=torch.int32, device=dev)
         d = self._desc()
-        if self.timer:
+        if self.timer and self.ann_len is None:
             rc = capi.lib().m3tsz_element_set_consume_timer(self.codec.ctx.handle, C.byref(self.codec.opts),
                                                             C.byref(d), C.byref(self._streams()), int(target_ns),
                                                             self.out_unit, _ptr(status), _cuda_stream_ptr(dev))
             self.codec.ctx.check(rc, "m3tsz_element_set_consume_timer")
+            return status
+        if self.timer:
+            rc = capi.lib().m3tsz_element_set_consume_timer_annotated(
+                self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()),
+                C.byref(self._ann()), int(target_ns), self.out_unit, _ptr(status), _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_element_set_consume_timer_annotated")
             return status
         if self.ann_len is None:
             rc = capi.lib().m3tsz_element_set_consume(self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d),
@@ -1189,10 +1204,15 @@ class ElementSet:
         would hold more than groups.sample_capacity values: its list samples and pending values plus every value
         this call folds into it.  Nothing is then folded into the group and its members are held back:
         groups.grow(open_windows=..., sample_capacity=...) and forward again with exactly the failed groups, which
-        gives the result of one unstopped call."""
+        gives the result of one unstopped call.
+        Annotations follow forward's rule: when `groups` keeps them (m3tsz_element_set_forward_timer_annotated) this
+        set must keep them too, and a group whose forwarded annotation is longer than its capacity gets ERR_CAPACITY
+        (groups.grow(annotation_capacity=...)); a group set without annotations takes the plain call."""
         assert isinstance(groups, ElementSet)
         if not (self.timer and groups.timer):
             raise ValueError("forward_timer takes Timer sets; other sets forward with forward")
+        if groups.ann_len is not None and self.ann_len is None:
+            raise ValueError("a group set that keeps annotations needs a source set that keeps them")
         assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
         assert members.is_cuda and members.dtype == torch.int32 and members.is_contiguous()
         G = group_off.numel() - 1
@@ -1201,11 +1221,19 @@ class ElementSet:
         src_status = torch.empty(max(1, self.n_elements), dtype=torch.int32, device=dev)
         group_status = torch.empty(max(1, G), dtype=torch.int32, device=dev)
         d, gd = self._desc(), groups._desc()
-        rc = capi.lib().m3tsz_element_set_forward_timer(
-            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()), int(target_ns),
-            _ptr(group_off), _ptr(members), members.numel(), G, C.byref(gd), C.byref(groups._streams()),
-            _ptr(src_status), _ptr(group_status), _cuda_stream_ptr(dev))
-        self.codec.ctx.check(rc, "m3tsz_element_set_forward_timer")
+        if groups.ann_len is None:
+            rc = capi.lib().m3tsz_element_set_forward_timer(
+                self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()), int(target_ns),
+                _ptr(group_off), _ptr(members), members.numel(), G, C.byref(gd), C.byref(groups._streams()),
+                _ptr(src_status), _ptr(group_status), _cuda_stream_ptr(dev))
+            self.codec.ctx.check(rc, "m3tsz_element_set_forward_timer")
+            return src_status[: self.n_elements], group_status[:G]
+        rc = capi.lib().m3tsz_element_set_forward_timer_annotated(
+            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(d), C.byref(self._streams()),
+            C.byref(self._ann()), int(target_ns), _ptr(group_off), _ptr(members), members.numel(), G, C.byref(gd),
+            C.byref(groups._streams()), C.byref(groups._ann()), _ptr(src_status), _ptr(group_status),
+            _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_forward_timer_annotated")
         return src_status[: self.n_elements], group_status[:G]
 
     def state(self):

@@ -1540,13 +1540,19 @@ static bool timer_params(const m3tsz_options *opts, const m3tsz_element_set *set
   return true;
 }
 
-int m3tsz_element_set_add_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
-                                const m3tsz_element_timer_streams *streams, const int64_t *d_ts, const double *d_val,
-                                uint64_t points_stride, const uint32_t *d_n_points, const int8_t *d_batch,
-                                int8_t *d_result, int32_t *d_status, void *stream) {
+// m3tsz_element_set_add_timer(_annotated): ann NULL is the plain add
+static int element_set_add_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                 const m3tsz_element_timer_streams *streams, const m3tsz_element_annotations *ann,
+                                 const int64_t *d_ts, const double *d_val, uint64_t points_stride,
+                                 const uint32_t *d_n_points, const int8_t *d_batch, const uint64_t *d_ann_series_off,
+                                 const m3tsz_annotation_entry *d_ann_entries, const uint8_t *d_ann_bytes,
+                                 int8_t *d_result, int32_t *d_status, void *stream, bool annotated) {
   ElementTimerParams tp;
   TileTransforms xf;
   if (!ctx || !timer_params(opts, set, streams, tp, xf) || points_stride > 0xffffffffull) return M3TSZ_ERR_INVALID_ARG;
+  if (annotated && (!element_ann_params(ann, tp.e) || ((uintptr_t)d_ann_series_off & 7u) ||
+                    (d_ann_series_off && (!d_ann_entries || !d_ann_bytes || ((uintptr_t)d_ann_entries & 7u)))))
+    return M3TSZ_ERR_INVALID_ARG;
   if (tp.e.n == 0) return M3TSZ_OK;
   if (!d_ts || !d_val || !d_result || !d_status || ((uintptr_t)d_ts & 7u) || ((uintptr_t)d_val & 7u) ||
       ((uintptr_t)d_n_points & 3u) || ((uintptr_t)d_status & 3u))
@@ -1560,20 +1566,47 @@ int m3tsz_element_set_add_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const
   tp.e.result = d_result;
   tp.e.status = d_status;
   tp.batch = d_batch;
+  if (annotated) {
+    tp.e.ann_series_off = d_ann_series_off;
+    tp.e.ann_entries = d_ann_entries;
+    tp.e.ann_bytes = d_ann_bytes;
+  }
   CK(launch_element_timer_add(tp, (cudaStream_t)stream));
   ctx->launches++;
   return M3TSZ_OK;
 }
 
-// element_set_consume with the Timer's consume kernel: the same scratch rows, append and status pass
-int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
-                                    const m3tsz_element_timer_streams *streams, int64_t target_ns, int32_t out_unit,
-                                    int32_t *d_status, void *stream) {
+int m3tsz_element_set_add_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                const m3tsz_element_timer_streams *streams, const int64_t *d_ts, const double *d_val,
+                                uint64_t points_stride, const uint32_t *d_n_points, const int8_t *d_batch,
+                                int8_t *d_result, int32_t *d_status, void *stream) {
+  return element_set_add_timer(ctx, opts, set, streams, nullptr, d_ts, d_val, points_stride, d_n_points, d_batch,
+                               nullptr, nullptr, nullptr, d_result, d_status, stream, false);
+}
+
+int m3tsz_element_set_add_timer_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                          const m3tsz_element_timer_streams *streams,
+                                          const m3tsz_element_annotations *ann, const int64_t *d_ts,
+                                          const double *d_val, uint64_t points_stride, const uint32_t *d_n_points,
+                                          const int8_t *d_batch, const uint64_t *d_ann_series_off,
+                                          const m3tsz_annotation_entry *d_ann_entries, const uint8_t *d_ann_bytes,
+                                          int8_t *d_result, int32_t *d_status, void *stream) {
+  return element_set_add_timer(ctx, opts, set, streams, ann, d_ts, d_val, points_stride, d_n_points, d_batch,
+                               d_ann_series_off, d_ann_entries, d_ann_bytes, d_result, d_status, stream, true);
+}
+
+// element_set_consume with the Timer's consume kernel: the same scratch rows, annotation entries, append and status
+// pass.  m3tsz_element_set_consume_timer(_annotated): ann NULL is the plain consume
+static int element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                     const m3tsz_element_timer_streams *streams, const m3tsz_element_annotations *ann,
+                                     int64_t target_ns, int32_t out_unit, int32_t *d_status, void *stream,
+                                     bool annotated) {
   ElementTimerParams tp;
   TileTransforms xf;
   if (!ctx || !timer_params(opts, set, streams, tp, xf) || element_set_no_output(set) || !unit_is_valid(out_unit))
     return M3TSZ_ERR_INVALID_ARG;
   ElementParams &p = tp.e;
+  if (annotated && !element_ann_params(ann, p)) return M3TSZ_ERR_INVALID_ARG;
   if (p.n == 0) return M3TSZ_OK;
   if (!d_status || ((uintptr_t)d_status & 3u)) return M3TSZ_ERR_INVALID_ARG;
   DeviceGuard guard(ctx->device);
@@ -1589,6 +1622,13 @@ int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   if ((rc = ensure(ctx, fence, kSlotElemRowN, kn * 4, &d_n))) return rc;
   if ((rc = ensure(ctx, fence, kSlotElemRowStatus, kn * 4, &d_rst))) return rc;
   if ((rc = ensure(ctx, fence, kSlotElemRowAppended, kn * 4, &d_app))) return rc;
+  if (annotated) {
+    void *d_aoff = nullptr, *d_aent = nullptr;
+    if ((rc = ensure(ctx, fence, kSlotElemRowAnnOff, (kn + 1) * 8, &d_aoff))) return rc;
+    if ((rc = ensure(ctx, fence, kSlotElemRowAnn, kn * rows * sizeof(m3tsz_annotation_entry), &d_aent))) return rc;
+    p.row_ann_off = (uint64_t *)d_aoff;
+    p.row_ann = (m3tsz_annotation_entry *)d_aent;
+  }
   p.target = target_ns;
   p.row_ts = (int64_t *)d_ts;
   p.row_val = (double *)d_val;
@@ -1603,6 +1643,11 @@ int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   if (!encode_params(opts, p.row_ts, p.row_val, kn, rows, p.row_n, nullptr, out_unit, nullptr, nullptr, nullptr,
                      nullptr, nullptr, (int32_t *)d_rst, &ex, ep, true))
     return M3TSZ_ERR_INVALID_ARG;
+  if (annotated) {  // (as element_set_consume)
+    ep.ann_series_off = p.row_ann_off;
+    ep.ann_entries = p.row_ann;
+    ep.ann_bytes = p.ann_slot;
+  }
   ep.out = set->d_out_buf;
   ep.out_stride = set->out_stride;
   ep.state = set->d_out_state;
@@ -1611,6 +1656,19 @@ int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   CK(launch_element_status((const int32_t *)d_rst, p.n, tp.n_types, d_status, st));
   ctx->launches += 3;
   return M3TSZ_OK;
+}
+
+int m3tsz_element_set_consume_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                    const m3tsz_element_timer_streams *streams, int64_t target_ns, int32_t out_unit,
+                                    int32_t *d_status, void *stream) {
+  return element_set_consume_timer(ctx, opts, set, streams, nullptr, target_ns, out_unit, d_status, stream, false);
+}
+
+int m3tsz_element_set_consume_timer_annotated(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                              const m3tsz_element_timer_streams *streams,
+                                              const m3tsz_element_annotations *ann, int64_t target_ns,
+                                              int32_t out_unit, int32_t *d_status, void *stream) {
+  return element_set_consume_timer(ctx, opts, set, streams, ann, target_ns, out_unit, d_status, stream, true);
 }
 
 // The forward calls' status arrays: present and aligned where there are sources / groups
@@ -1664,6 +1722,39 @@ static int element_forward_scratch(m3tsz_ctx *ctx, ScratchFence &fence, ElementR
   return M3TSZ_OK;
 }
 
+// The annotated forward calls' annotation structs: both checked (element_ann_params) into the source and group set
+// parameters, and the source and group arrays must not overlap (the fold copies source slot bytes into group slots)
+static bool forward_ann_params(const m3tsz_element_annotations *src_ann, ElementParams &sp,
+                               const m3tsz_element_annotations *group_ann, ElementParams &gp) {
+  if (!element_ann_params(src_ann, sp) || !element_ann_params(group_ann, gp)) return false;
+  auto overlap = [](const void *a, uint64_t na, const void *b, uint64_t nb) {
+    return na && nb && (uintptr_t)a < (uintptr_t)b + nb && (uintptr_t)b < (uintptr_t)a + na;
+  };
+  const uint64_t sl = (uint64_t)sp.n_slots * sp.n, gl = (uint64_t)gp.n_slots * gp.n;
+  const void *sa[2] = {sp.ann_len, sp.ann_slot}, *ga[2] = {gp.ann_len, gp.ann_slot};
+  const uint64_t sb[2] = {sl * 4, sl * sp.ann_cap}, gb[2] = {gl * 4, gl * gp.ann_cap};
+  for (int i = 0; i < 2; i++)
+    for (int j = 0; j < 2; j++)
+      if (overlap(sa[i], sb[i], ga[j], gb[j])) return false;
+  return true;
+}
+
+// The annotated forward calls' scratch: which forwarded windows carry an annotation and their references; rp takes
+// them and the group set gp's annotation arrays
+static int forward_ann_scratch(m3tsz_ctx *ctx, ScratchFence &fence, ElementRollupParams &rp, const ElementParams &gp) {
+  void *d_fap, *d_fa;
+  const uint64_t sn = rp.src.n ? rp.src.n : 1;
+  int rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdAnnPresent, sn * 8, &d_fap))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdAnn, (size_t)sn * rp.src.n_slots * 8, &d_fa))) return rc;
+  rp.fwd_ann_present = (uint64_t *)d_fap;
+  rp.fwd_ann = (uint64_t *)d_fa;
+  rp.g_ann_len = gp.ann_len;
+  rp.g_ann_slot = gp.ann_slot;
+  rp.g_ann_cap = gp.ann_cap;
+  return M3TSZ_OK;
+}
+
 // The forward kernel writes each source's due windows to scratch, the fold kernel folds them into the groups' windows
 // and marks the members of the groups that failed, and the commit kernel frees the other sources' due windows.
 // m3tsz_element_set_forward(_annotated): annotated, the forward also writes which forwarded windows carry an
@@ -1684,19 +1775,7 @@ static int element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
       (n_groups && !d_group_off) || (n_members && !d_members) || ((uintptr_t)d_group_off & 7u) ||
       ((uintptr_t)d_members & 3u))
     return M3TSZ_ERR_INVALID_ARG;
-  if (annotated) {
-    if (!element_ann_params(src_ann, rp.src) || !element_ann_params(group_ann, gp)) return M3TSZ_ERR_INVALID_ARG;
-    // the source and group annotation arrays must not overlap: the fold copies source slot bytes into group slots
-    auto overlap = [](const void *a, uint64_t na, const void *b, uint64_t nb) {
-      return na && nb && (uintptr_t)a < (uintptr_t)b + nb && (uintptr_t)b < (uintptr_t)a + na;
-    };
-    const uint64_t sl = (uint64_t)rp.src.n_slots * rp.src.n, gl = (uint64_t)gp.n_slots * gp.n;
-    const void *sa[2] = {rp.src.ann_len, rp.src.ann_slot}, *ga[2] = {gp.ann_len, gp.ann_slot};
-    const uint64_t sb[2] = {sl * 4, sl * rp.src.ann_cap}, gb[2] = {gl * 4, gl * gp.ann_cap};
-    for (int i = 0; i < 2; i++)
-      for (int j = 0; j < 2; j++)
-        if (overlap(sa[i], sb[i], ga[j], gb[j])) return M3TSZ_ERR_INVALID_ARG;
-  }
+  if (annotated && !forward_ann_params(src_ann, rp.src, group_ann, gp)) return M3TSZ_ERR_INVALID_ARG;
   if (!forward_statuses_ok(rp.src.n, n_groups, d_src_status, d_group_status)) return M3TSZ_ERR_INVALID_ARG;
   if (rp.src.n == 0 && n_groups == 0) return M3TSZ_OK;
   DeviceGuard guard(ctx->device);
@@ -1706,17 +1785,7 @@ static int element_set_forward(m3tsz_ctx *ctx, const m3tsz_options *opts, const 
   int rc = element_forward_scratch(ctx, fence, rp, gp, target_ns, d_group_off, d_members, n_members, n_groups,
                                    d_src_status, d_group_status, src->discard_nan);
   if (rc != M3TSZ_OK) return rc;
-  if (annotated) {
-    void *d_fap, *d_fa;
-    const uint64_t sn = rp.src.n ? rp.src.n : 1;
-    if ((rc = ensure(ctx, fence, kSlotElemFwdAnnPresent, sn * 8, &d_fap))) return rc;
-    if ((rc = ensure(ctx, fence, kSlotElemFwdAnn, (size_t)sn * rp.src.n_slots * 8, &d_fa))) return rc;
-    rp.fwd_ann_present = (uint64_t *)d_fap;
-    rp.fwd_ann = (uint64_t *)d_fa;
-    rp.g_ann_len = gp.ann_len;
-    rp.g_ann_slot = gp.ann_slot;
-    rp.g_ann_cap = gp.ann_cap;
-  }
+  if (annotated && (rc = forward_ann_scratch(ctx, fence, rp, gp)) != M3TSZ_OK) return rc;
   CK(cudaMemsetAsync(rp.mark, 0, (rp.src.n ? rp.src.n : 1) * 4, st));
   CK(launch_element_forward(rp, st));
   CK(launch_element_fold(rp, st));
@@ -1743,13 +1812,16 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
                              group_ann, d_src_status, d_group_status, stream, true);
 }
 
-// element_set_forward with the Timer forward and fold kernels: the same groups, scratch and commit
-int m3tsz_element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
-                                    const m3tsz_element_timer_streams *src_streams, int64_t target_ns,
-                                    const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
-                                    uint64_t n_groups, const m3tsz_element_set *groups,
-                                    const m3tsz_element_timer_streams *group_streams, int32_t *d_src_status,
-                                    int32_t *d_group_status, void *stream) {
+// element_set_forward with the Timer forward and fold kernels: the same groups, scratch, annotation scratch and
+// commit.  m3tsz_element_set_forward_timer(_annotated): src_ann / group_ann NULL is the plain forward
+static int element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                     const m3tsz_element_timer_streams *src_streams,
+                                     const m3tsz_element_annotations *src_ann, int64_t target_ns,
+                                     const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                     uint64_t n_groups, const m3tsz_element_set *groups,
+                                     const m3tsz_element_timer_streams *group_streams,
+                                     const m3tsz_element_annotations *group_ann, int32_t *d_src_status,
+                                     int32_t *d_group_status, void *stream, bool annotated) {
   ElementTimerParams sp, gt;
   TileTransforms sx, gx;
   if (!ctx || !timer_params(opts, src, src_streams, sp, sx) || !timer_params(opts, groups, group_streams, gt, gx))
@@ -1771,6 +1843,7 @@ int m3tsz_element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, c
     for (int j = 0; j < 12; j++)
       if (sb[i] && gb[j] && (uintptr_t)sa[i] < (uintptr_t)ga[j] + gb[j] && (uintptr_t)ga[j] < (uintptr_t)sa[i] + sb[i])
         return M3TSZ_ERR_INVALID_ARG;
+  if (annotated && !forward_ann_params(src_ann, sp.e, group_ann, gt.e)) return M3TSZ_ERR_INVALID_ARG;
   if (!forward_statuses_ok(sp.e.n, n_groups, d_src_status, d_group_status)) return M3TSZ_ERR_INVALID_ARG;
   if (sp.e.n == 0 && n_groups == 0) return M3TSZ_OK;
   DeviceGuard guard(ctx->device);
@@ -1783,6 +1856,7 @@ int m3tsz_element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   int rc = element_forward_scratch(ctx, fence, rp, gt.e, target_ns, d_group_off, d_members, n_members, n_groups,
                                    d_src_status, d_group_status, src->discard_nan);
   if (rc != M3TSZ_OK) return rc;
+  if (annotated && (rc = forward_ann_scratch(ctx, fence, rp, gt.e)) != M3TSZ_OK) return rc;
   sp.e = rp.src;
   CK(cudaMemsetAsync(rp.mark, 0, (rp.src.n ? rp.src.n : 1) * 4, st));
   CK(launch_element_timer_forward(rp, sp, st));
@@ -1790,6 +1864,28 @@ int m3tsz_element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   CK(launch_element_commit(rp, st));
   ctx->launches += 3;
   return M3TSZ_OK;
+}
+
+int m3tsz_element_set_forward_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                    const m3tsz_element_timer_streams *src_streams, int64_t target_ns,
+                                    const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                    uint64_t n_groups, const m3tsz_element_set *groups,
+                                    const m3tsz_element_timer_streams *group_streams, int32_t *d_src_status,
+                                    int32_t *d_group_status, void *stream) {
+  return element_set_forward_timer(ctx, opts, src, src_streams, nullptr, target_ns, d_group_off, d_members,
+                                   n_members, n_groups, groups, group_streams, nullptr, d_src_status, d_group_status,
+                                   stream, false);
+}
+
+int m3tsz_element_set_forward_timer_annotated(
+    m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+    const m3tsz_element_timer_streams *src_streams, const m3tsz_element_annotations *src_ann, int64_t target_ns,
+    const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members, uint64_t n_groups,
+    const m3tsz_element_set *groups, const m3tsz_element_timer_streams *group_streams,
+    const m3tsz_element_annotations *group_ann, int32_t *d_src_status, int32_t *d_group_status, void *stream) {
+  return element_set_forward_timer(ctx, opts, src, src_streams, src_ann, target_ns, d_group_off, d_members,
+                                   n_members, n_groups, groups, group_streams, group_ann, d_src_status,
+                                   d_group_status, stream, true);
 }
 
 int m3tsz_merge_series_batch_ex(m3tsz_ctx *ctx, const int64_t *d_ts, const double *d_val, uint64_t cap,

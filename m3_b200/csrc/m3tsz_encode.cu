@@ -2546,17 +2546,9 @@ struct ElemAcc {
   V sum, mn, mx, sq;
   double last;  // Gauge only
   int64_t last_at;
-  // an annotated set's window annotation to slot o: the a_len bytes at p.ann_bytes + a_off (the add's inputs) as whole
-  // 8-byte words, the last one zero-padded (a_len <= ann_cap, a multiple of 8)
+  // an annotated set's window annotation to slot o (ElementParams::store_ann)
   __device__ static __forceinline__ void store_ann(const ElementParams &p, uint64_t o, uint64_t a_off, uint32_t a_len) {
-    p.ann_len[o] = a_len;
-    uint64_t *dst = reinterpret_cast<uint64_t *>(p.ann_slot + o * p.ann_cap);
-    const uint8_t *src = p.ann_bytes + a_off;
-    for (uint32_t w = 0; w < (a_len + 7u) / 8u; w++) {
-      uint64_t x = 0;
-      for (uint32_t b = 0; b < 8u && w * 8u + b < a_len; b++) x |= (uint64_t)src[w * 8u + b] << (8u * b);
-      dst[w] = x;
-    }
+    p.store_ann(o, a_off, a_len);
   }
 };
 template <bool CTR>
@@ -2745,12 +2737,9 @@ __device__ __forceinline__ void elem_add_lane(const ElementParams &p, uint64_t s
 template <bool CTR, bool ANN = false>
 __device__ __forceinline__ void elem_consume_lane(const ElementParams &p, uint64_t s, XfElem &e) {
   const uint64_t kn = (uint64_t)p.n_types * p.n;
-  // a slot's annotation length (one above the capacity, which the library never stores, reads as none)
-  auto ann_len = [&](uint64_t o) -> uint32_t {
-    const uint32_t l = p.ann_len[o];
-    return l <= p.ann_cap ? l : 0u;
-  };
-  if constexpr (ANN) {
+  // a slot's annotation length (ElementParams::slot_ann_len)
+  auto ann_len = [&](uint64_t o) -> uint32_t { return p.slot_ann_len(o); };
+  if constexpr (ANN) {  // (ElementParams::stage_ann_offsets, kept as written here so that this kernel's SASS stays)
     for (uint32_t j = 0; j < p.n_types; j++) p.row_ann_off[(uint64_t)j * p.n + s] = ((uint64_t)j * p.n + s) * p.rows_stride;
     if (s + 1 == p.n) p.row_ann_off[kn] = kn * p.rows_stride;
   }
@@ -2818,13 +2807,7 @@ __device__ __forceinline__ void elem_consume_lane(const ElementParams &p, uint64
     if constexpr (ANN) a_len = ann_len(o);
     // ANN: the entry of staged datapoint d of row `row` (the same window annotation for the Reset datapoint)
     auto stage_ann = [&](uint64_t row, uint64_t d) {
-      if constexpr (ANN) {
-        m3tsz_annotation_entry en;
-        en.dp_index = (uint32_t)d;
-        en.length = a_len;
-        en.byte_offset = o * p.ann_cap;
-        p.row_ann[row * p.rows_stride + d] = en;
-      }
+      if constexpr (ANN) p.stage_ann(row, d, o, a_len);
     };
     xf_element_window(
         p.ops, p.resolution, e, 0u, p.n_types, t,
@@ -3263,6 +3246,13 @@ __device__ __forceinline__ double timer_value_of(const ElementTimerParams &p, in
 
 // Timer.AddBatch of element s's batches in row order (m3tsz_element_set_add_timer).  A first pass checks the batch
 // marks; each batch then finds its window's slot (or a free one), checks the slot's room and adds to it.
+// ANN (m3tsz_element_set_add_timer_annotated): a batch's annotation is its first row's entry (a BatchTimer has one);
+// an entry with a length on a continuation row breaks the batch rule.  An accepted batch with one replaces its
+// window's annotation (MaybeReplaceAnnotation, aggregation/timer.go:57-76), kept as in elem_add_lane: a reference
+// (a_off, a_len) into the call's bytes for the slot `cur`, copied to the slot when the batches leave it, and only when
+// it changed (a window opened here always writes its length).  A batch whose annotation is longer than ann_cap gets
+// CAPACITY after the closed and invalid-start checks.
+template <bool ANN = false>
 __device__ __forceinline__ void elem_timer_add_lane(const ElementTimerParams &tp, uint64_t s) {
   const ElementParams &p = tp.e;
   const uint32_t n_pts = p.n_points ? p.n_points[s] : (uint32_t)p.points_stride;
@@ -3280,6 +3270,15 @@ __device__ __forceinline__ void elem_timer_add_lane(const ElementTimerParams &tp
     else if (t != t0)
       bad = true;
   }
+  uint64_t ann_i = 0, ann_end = 0;
+  if (ANN && p.ann_series_off) {
+    ann_i = p.ann_series_off[s];
+    ann_end = p.ann_series_off[s + 1];
+    for (uint64_t k = ann_i; k < ann_end && !bad; k++) {
+      const m3tsz_annotation_entry &en = p.ann_entries[k];
+      bad = en.length != 0 && en.dp_index < n_pts && cont(en.dp_index);
+    }
+  }
   if (bad) {
     for (uint32_t i = 0; i < n_pts; i++) p.result[(uint64_t)i * p.n + s] = (int8_t)M3TSZ_ERR_INVALID_ARG;
     p.status[s] = M3TSZ_ERR_INVALID_ARG;
@@ -3287,6 +3286,10 @@ __device__ __forceinline__ void elem_timer_add_lane(const ElementTimerParams &tp
   }
   const int64_t wm = p.watermark[s];
   int32_t status = M3TSZ_OK;
+  int cur = -1;  // ANN: the slot whose annotation (a_off, a_len) is held, -1: none
+  uint64_t a_off = 0;
+  uint32_t a_len = 0;
+  bool a_dirty = false;
   uint32_t i = 0;
   while (i < n_pts) {
     uint32_t j = i + 1;
@@ -3296,10 +3299,21 @@ __device__ __forceinline__ void elem_timer_add_lane(const ElementTimerParams &tp
     if (status == M3TSZ_OK) {
       const int64_t t = p.ts[(uint64_t)i * p.n + s];
       int64_t ws = 0;
+      uint64_t d_off = 0;  // ANN: this batch's annotation, d_len 0: none
+      uint32_t d_len = 0;
+      if constexpr (ANN) {
+        while (ann_i < ann_end && p.ann_entries[ann_i].dp_index < i) ann_i++;
+        if (ann_i < ann_end && p.ann_entries[ann_i].dp_index == i) {
+          d_off = p.ann_entries[ann_i].byte_offset;
+          d_len = p.ann_entries[ann_i].length;
+        }
+      }
       if (!elem_window_start(t, p.resolution, p.trunc_off, ws)) {
         res = M3TSZ_ERR_INVALID_ARG;
       } else if (elem_ends_by(ws, p.resolution, wm)) {
         res = M3TSZ_ERR_AGGREGATION_CLOSED;
+      } else if (ANN && d_len > p.ann_cap) {
+        status = res = M3TSZ_ERR_CAPACITY;
       } else {
         int hit = -1, fr = -1;
         for (uint32_t r = 0; r < p.n_slots; r++) {
@@ -3344,25 +3358,50 @@ __device__ __forceinline__ void elem_timer_add_lane(const ElementTimerParams &tp
           static_cast<double *>(p.sum_sq)[o] = sq;
           tp.hdr[o] = c.h;
           res = M3TSZ_OK;
+          if constexpr (ANN) {
+            if (r != cur) {
+              if (cur >= 0 && a_dirty) p.store_ann((uint64_t)cur * p.n + s, a_off, a_len);
+              cur = r;
+              a_len = 0;
+              a_dirty = hit < 0;
+            }
+            if (d_len) {
+              a_off = d_off;
+              a_len = d_len;
+              a_dirty = true;
+            }
+          }
         }
       }
     }
     for (uint32_t k = i; k < j; k++) p.result[(uint64_t)k * p.n + s] = (int8_t)res;
     i = j;
   }
+  if (ANN && cur >= 0 && a_dirty) p.store_ann((uint64_t)cur * p.n + s, a_off, a_len);
   p.status[s] = status;
 }
 
 // Consume(target) of Timer element s, as elem_consume_lane: the same room check, window order, staging and commit;
 // each due window's stream is flushed and its quantiles computed here.  More than M3TSZ_MAX_ELEMENT_TYPES types come
 // without ops: each type's row takes every window's value, and the record is not touched.
+// ANN (m3tsz_element_set_consume_timer_annotated): every staged datapoint also gets its window's entry, and the room
+// check counts the annotations, both as elem_consume_lane<CTR, true> does.
+template <bool ANN = false>
 __device__ __forceinline__ void elem_timer_consume_lane(const ElementTimerParams &tp, uint64_t s, XfElem &e) {
   const ElementParams &p = tp.e;
   const uint64_t kn = (uint64_t)tp.n_types * p.n;
+  if constexpr (ANN) p.stage_ann_offsets(s, tp.n_types);
   uint32_t m = 0;
+  uint64_t ann_words = 0;  // ANN: the flushed windows' annotations as the append's room check counts them
   for (uint32_t r = 0; r < p.n_slots; r++) {
     const uint64_t o = (uint64_t)r * p.n + s;
-    if (p.count[o] != 0 && elem_ends_by(p.start[o], p.resolution, p.target)) m++;
+    if (p.count[o] != 0 && elem_ends_by(p.start[o], p.resolution, p.target)) {
+      m++;
+      if constexpr (ANN) {
+        const uint32_t l = p.slot_ann_len(o);
+        if (l) ann_words += (l + 3u) / 4u + 4u;
+      }
+    }
   }
   bool reset = false;
   for (int k = 0; k < M3TSZ_MAX_TRANSFORMS; k++) reset |= ((p.ops >> (4 * k)) & 0xfu) == M3TSZ_TRANSFORM_RESET;
@@ -3372,7 +3411,9 @@ __device__ __forceinline__ void elem_timer_consume_lane(const ElementTimerParams
     for (uint32_t j = 0; j < tp.n_types; j++) {
       const m3tsz_encoder_state &oe = p.out_state[(uint64_t)j * p.n + s];
       const uint64_t bits = oe.bits + (oe.num_encoded ? 0u : 64u) + (per_row - 1) * 163u;
-      if ((bits >> 5) + ENC_GUARD + 4 > p.out_slot_words) status = M3TSZ_ERR_CAPACITY;
+      uint64_t words = (bits >> 5) + ENC_GUARD + 4;
+      if constexpr (ANN) words += ann_words * (reset ? 2u : 1u);
+      if (words > p.out_slot_words) status = M3TSZ_ERR_CAPACITY;
     }
   }
   if (m == 0 || status != M3TSZ_OK) {
@@ -3407,6 +3448,8 @@ __device__ __forceinline__ void elem_timer_consume_lane(const ElementTimerParams
     const int64_t cnt = p.count[o];
     const double sum = static_cast<const double *>(p.sum)[o], sq = static_cast<const double *>(p.sum_sq)[o];
     const int64_t t = bs + p.resolution;
+    uint32_t a_len = 0;
+    if constexpr (ANN) a_len = p.slot_ann_len(o);
     CmStream c = timer_stream(tp, (uint32_t)best, s);
     c.h = tp.hdr[o];
     double cq[M3TSZ_MAX_TIMER_QUANTILES];
@@ -3421,10 +3464,12 @@ __device__ __forceinline__ void elem_timer_consume_lane(const ElementTimerParams
         uint64_t a = d * kn + (uint64_t)i * p.n + s;
         p.row_ts[a] = t;
         p.row_val[a] = v;
+        if constexpr (ANN) p.stage_ann((uint64_t)i * p.n + s, d, o, a_len);
         if (extra_t != 0) {
           a += kn;
           p.row_ts[a] = extra_t;
           p.row_val[a] = 0.0;
+          if constexpr (ANN) p.stage_ann((uint64_t)i * p.n + s, d + 1, o, a_len);
         }
         rows += (uint64_t)(extra_t != 0 ? 2u : 1u) << (8 * i);
       });
@@ -3433,6 +3478,7 @@ __device__ __forceinline__ void elem_timer_consume_lane(const ElementTimerParams
         const uint64_t a = (uint64_t)w * kn + (uint64_t)i * p.n + s;
         p.row_ts[a] = t;
         p.row_val[a] = value_of(i);
+        if constexpr (ANN) p.stage_ann((uint64_t)i * p.n + s, w, o, a_len);
       }
     }
     p.count[o] = 0;  // the slot is free; its stream is made anew when an add opens it
@@ -3451,27 +3497,37 @@ __device__ __forceinline__ void elem_timer_consume_lane(const ElementTimerParams
 
 // (__maxnreg__ rather than __launch_bounds__: under the latter ptxas held these two at 80 registers and spilled around
 // the double-division calls of the stream's thresholds; with 128 neither spills)
+template <bool ANN>
 __global__ void __maxnreg__(128) element_timer_add_kernel(const ElementTimerParams p) {
   const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
-  if (s < p.e.n) elem_timer_add_lane(p, s);
+  if (s < p.e.n) elem_timer_add_lane<ANN>(p, s);
 }
+template <bool ANN>
 __global__ void __maxnreg__(128) element_timer_consume_kernel(const ElementTimerParams p) {
   __shared__ XfElem rec[ELEM_THREADS];
   const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
-  if (s < p.e.n) elem_timer_consume_lane(p, s, rec[threadIdx.x]);
+  if (s < p.e.n) elem_timer_consume_lane<ANN>(p, s, rec[threadIdx.x]);
 }
 
 cudaError_t launch_element_timer_add(const ElementTimerParams &p, cudaStream_t stream) {
   if (p.e.n == 0) return cudaSuccess;
   if ((p.e.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
-  element_timer_add_kernel<<<elem_blocks(p.e.n), ELEM_THREADS, 0, stream>>>(p);
+  if (p.e.ann_len)
+    element_timer_add_kernel<true><<<elem_blocks(p.e.n), ELEM_THREADS, 0, stream>>>(p);
+  else
+    element_timer_add_kernel<false><<<elem_blocks(p.e.n), ELEM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
 cudaError_t launch_element_timer_consume(const ElementTimerParams &p, cudaStream_t stream) {
   if (p.e.n == 0) return cudaSuccess;
   if ((p.e.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
-  element_timer_consume_kernel<<<elem_blocks(p.e.n), ELEM_THREADS, 0, stream>>>(p);
+  const bool ann = p.e.ann_len != nullptr;
+  if (ann && (!p.e.row_ann_off || !p.e.row_ann)) return cudaErrorInvalidValue;
+  if (ann)
+    element_timer_consume_kernel<true><<<elem_blocks(p.e.n), ELEM_THREADS, 0, stream>>>(p);
+  else
+    element_timer_consume_kernel<false><<<elem_blocks(p.e.n), ELEM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
@@ -3524,7 +3580,8 @@ __device__ __forceinline__ void elem_forward_lane(const ElementRollupParams &p, 
     p.fwd_start[(uint64_t)q * e.n + s] = bs;
     p.fwd_val[(uint64_t)q * e.n + s] = v;
   }
-  if constexpr (ANN) {  // (after the windows' loop, so that nothing more lives across xf_window's calls)
+  if constexpr (ANN) {  // (after the windows' loop, so that nothing more lives across xf_window's calls; the pass of
+                        // ElementRollupParams::forward_ann, kept as written here so that this kernel's SASS stays)
     uint64_t ann = 0;
     for (uint32_t r = 0; r < e.n_slots; r++) {
       if (!((due >> r) & 1u)) continue;
@@ -3555,16 +3612,10 @@ struct ElemFoldAcc {
   using A = std::conditional_t<CTR, RollupCounterAcc, RollupGaugeAcc>;
   int64_t start;
   A a;
-  // the annotated fold's group window annotation to group slot o: ref is the forward's reference to a source slot
-  // (0: none), whose bytes go over as whole 8-byte words (the annotated add zero-pads a slot's last word), lane
-  // `lane` of n_lanes copying words lane, lane + n_lanes, ...; every lane writes the length
+  // the annotated fold's group window annotation to group slot o (ElementRollupParams::store_group_ann)
   __device__ static __forceinline__ void store_ann(const ElementRollupParams &p, uint64_t o, uint64_t ref,
                                                    uint32_t lane, uint32_t n_lanes) {
-    const uint32_t len = (uint32_t)(ref & 0x1ffffu);
-    p.g_ann_len[o] = len;
-    const uint64_t *src = reinterpret_cast<const uint64_t *>(p.src.ann_slot + (ref >> 17) * p.src.ann_cap);
-    uint64_t *dst = reinterpret_cast<uint64_t *>(p.g_ann_slot + o * p.g_ann_cap);
-    for (uint32_t w = lane; w < (len + 7u) / 8u; w += n_lanes) dst[w] = src[w];
+    p.store_group_ann(o, ref, lane, n_lanes);
   }
 };
 template <bool CTR>
@@ -3884,6 +3935,8 @@ cudaError_t launch_element_commit(const ElementRollupParams &p, cudaStream_t str
 // order and scratch, each window's value Flush + ValueOf(tp.type[0]) as elem_timer_consume_lane computes it, through
 // the pre-ops on the record's head.  Each flushed header goes back to its slot: the flush rewrote the slot's arena, and
 // a source held back keeps the flushed stream (a second Flush, its heaps empty, gives the same quantiles).
+// ANN: the annotated forward's reference pass (ElementRollupParams::forward_ann), after the windows' loop.
+template <bool ANN = false>
 __device__ __forceinline__ void elem_timer_forward_lane(const ElementRollupParams &p, const ElementTimerParams &tp,
                                                         uint64_t s) {
   const ElementParams &e = p.src;
@@ -3928,6 +3981,7 @@ __device__ __forceinline__ void elem_timer_forward_lane(const ElementRollupParam
     p.fwd_start[(uint64_t)q * e.n + s] = bs;
     p.fwd_val[(uint64_t)q * e.n + s] = v;
   }
+  if constexpr (ANN) p.forward_ann(s, due, present);
   p.fwd_n[s] = m;
   p.fwd_present[s] = present;
   p.fwd_due[s] = due;
@@ -3940,7 +3994,10 @@ __device__ __forceinline__ void elem_timer_forward_lane(const ElementRollupParam
 // point afresh).  The first pass also counts each touched window's values, n_add[r] for group slot r and
 // n_add[g_slots + k] for fresh[k], and fails the group with CAPACITY where its list + pending + those values exceed
 // gt.cap (an upper bound: the fold's compressions only free room).
-template <class Member>
+// ANN: elem_fold_group's annotation rule: the first pass also fails the group with CAPACITY for an annotation longer
+// than g_ann_cap on a value that would fold, and the group window's reference stays in registers beside its stream and
+// sums, resolved into the slot (ElementRollupParams::store_group_ann, this lane copying every word) only when changed.
+template <bool ANN = false, class Member>
 __device__ __forceinline__ int32_t elem_timer_fold_group(const ElementRollupParams &p, const ElementTimerParams &gt,
                                                          uint64_t g, int64_t *fresh, uint32_t *n_add, Member member) {
   const uint64_t lo = p.group_off[g], hi = p.group_off[g + 1], G = p.n_groups;
@@ -3973,6 +4030,9 @@ __device__ __forceinline__ int32_t elem_timer_fold_group(const ElementRollupPara
         double v;
         window(a, q, ws, v);
         if (elem_ends_by(ws, res, wm)) continue;
+        if constexpr (ANN) {
+          if (((a.ann >> q) & 1u) && (p.fwd_ann[(uint64_t)q * p.src.n + a.m] & 0x1ffffu) > p.g_ann_cap) full = true;
+        }
         int at = -1;
         if (last >= 0 && ws == last_ws) {
           at = last;
@@ -4017,6 +4077,8 @@ __device__ __forceinline__ int32_t elem_timer_fold_group(const ElementRollupPara
     double sum = 0.0, sq = 0.0;
     CmStream c = timer_stream(gt, 0u, g);  // (set again for the slot whenever `cur` changes)
     bool closed = false;
+    uint64_t a_ref = 0;  // ANN: the window's annotation taken in this call (0: none), and whether its slot needs it
+    bool a_dirty = false;
     auto store = [&]() {
       const uint64_t o = (uint64_t)cur * G + g;
       p.g_start[o] = w_start;
@@ -4024,6 +4086,7 @@ __device__ __forceinline__ int32_t elem_timer_fold_group(const ElementRollupPara
       static_cast<double *>(p.g_sum)[o] = sum;
       static_cast<double *>(p.g_sum_sq)[o] = sq;
       gt.hdr[o] = c.h;
+      if (ANN && a_dirty) p.store_group_ann(o, a_ref, 0u, 1u);
     };
     for (uint64_t i = lo; i < hi; i++) {
       const FwdMember a = member(i);
@@ -4063,12 +4126,18 @@ __device__ __forceinline__ int32_t elem_timer_fold_group(const ElementRollupPara
             c.h = gt.hdr[o];
           else
             c.init();
+          a_ref = 0;
+          a_dirty = hit < 0;
         }
         cnt++;
         sum = amd64_op(__dadd_rn(sum, v), sum, v);
         const double v2 = amd64_op(__dmul_rn(v, v), v, v);
         sq = amd64_op(__dadd_rn(sq, v2), sq, v2);
         c.add_batch(1u, [&](uint32_t) { return v; });
+        if (ANN && ((a.ann >> q) & 1u)) {
+          a_ref = p.fwd_ann[(uint64_t)q * p.src.n + a.m];
+          a_dirty = true;
+        }
       }
     }
     if (cur >= 0) store();
@@ -4079,22 +4148,25 @@ __device__ __forceinline__ int32_t elem_timer_fold_group(const ElementRollupPara
 }
 
 // (__maxnreg__ as the other Timer kernels: the stream's code is the same)
+template <bool ANN>
 __global__ void __maxnreg__(128) element_timer_forward_kernel(const ElementRollupParams p,
                                                               const ElementTimerParams tp) {
   const uint64_t s = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
-  if (s < p.src.n) elem_timer_forward_lane(p, tp, s);
+  if (s < p.src.n) elem_timer_forward_lane<ANN>(p, tp, s);
 }
 
 // One lane per group, unlike element_fold_kernel's warp per group: a group's values go through the serial stream one
 // Timer.Add at a time, so a warp that ran one group would leave 31 lanes idle; with a lane per group the warp runs 32
 // groups' folds at once (DESIGN.md §4.12 has both mappings measured).  The fresh-window starts and per-window tallies
 // are the lane's own (local memory; a group touches few of the entries).
+template <bool ANN>
 __global__ void __maxnreg__(128) element_timer_fold_kernel(const ElementRollupParams p, const ElementTimerParams gt) {
   const uint64_t g = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
   if (g >= p.n_groups) return;
   int64_t fresh[M3TSZ_MAX_ELEMENT_WINDOWS];
   uint32_t n_add[2 * M3TSZ_MAX_ELEMENT_WINDOWS];
-  const int32_t st = elem_timer_fold_group(p, gt, g, fresh, n_add, [&](uint64_t i) { return fwd_member(p, i); });
+  const int32_t st =
+      elem_timer_fold_group<ANN>(p, gt, g, fresh, n_add, [&](uint64_t i) { return fwd_member<ANN>(p, i); });
   const uint64_t lo = p.group_off[g], hi = p.group_off[g + 1];
   if ((st == M3TSZ_ERR_CAPACITY || st == M3TSZ_ERR_INVALID_ARG) && lo <= hi) {
     const uint64_t end = hi < p.n_members ? hi : p.n_members;
@@ -4109,7 +4181,12 @@ cudaError_t launch_element_timer_forward(const ElementRollupParams &p, const Ele
                                          cudaStream_t stream) {
   if (p.src.n == 0) return cudaSuccess;
   if ((p.src.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
-  element_timer_forward_kernel<<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p, src);
+  const bool ann = p.src.ann_len != nullptr;
+  if (ann && (!p.fwd_ann_present || !p.fwd_ann)) return cudaErrorInvalidValue;
+  if (ann)
+    element_timer_forward_kernel<true><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p, src);
+  else
+    element_timer_forward_kernel<false><<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p, src);
   return cudaGetLastError();
 }
 
@@ -4117,7 +4194,12 @@ cudaError_t launch_element_timer_fold(const ElementRollupParams &p, const Elemen
                                       cudaStream_t stream) {
   if (p.n_groups == 0) return cudaSuccess;
   if ((p.n_groups + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
-  element_timer_fold_kernel<<<elem_blocks(p.n_groups), ELEM_THREADS, 0, stream>>>(p, groups);
+  const bool ann = p.src.ann_len != nullptr;
+  if (ann && (!p.fwd_ann_present || !p.fwd_ann || !p.g_ann_len || !p.g_ann_slot)) return cudaErrorInvalidValue;
+  if (ann)
+    element_timer_fold_kernel<true><<<elem_blocks(p.n_groups), ELEM_THREADS, 0, stream>>>(p, groups);
+  else
+    element_timer_fold_kernel<false><<<elem_blocks(p.n_groups), ELEM_THREADS, 0, stream>>>(p, groups);
   return cudaGetLastError();
 }
 

@@ -388,6 +388,41 @@ struct ElementParams {
   // consume: the staged rows' annotations for the append, row i's entries from row_ann_off[i] = i * rows_stride
   uint64_t *row_ann_off;
   m3tsz_annotation_entry *row_ann;
+
+  // The annotated lanes' slot helpers (the Gauge / Counter lanes and the Timer lanes share them).
+  // add: a window annotation to slot o, the a_len bytes at ann_bytes + a_off (the add's inputs) as whole 8-byte words,
+  // the last one zero-padded (a_len <= ann_cap, a multiple of 8)
+  __device__ __forceinline__ void store_ann(uint64_t o, uint64_t a_off, uint32_t a_len) const {
+    ann_len[o] = a_len;
+    uint64_t *dst = reinterpret_cast<uint64_t *>(ann_slot + o * ann_cap);
+    const uint8_t *src = ann_bytes + a_off;
+    for (uint32_t w = 0; w < (a_len + 7u) / 8u; w++) {
+      uint64_t x = 0;
+      for (uint32_t b = 0; b < 8u && w * 8u + b < a_len; b++) x |= (uint64_t)src[w * 8u + b] << (8u * b);
+      dst[w] = x;
+    }
+  }
+  // consume / forward: slot o's annotation length (one above the capacity, which the library never stores, reads as
+  // none)
+  __device__ __forceinline__ uint32_t slot_ann_len(uint64_t o) const {
+    const uint32_t l = ann_len[o];
+    return l <= ann_cap ? l : 0u;
+  }
+  // consume: element s's k rows' entry lists, row i's at row_ann_off[i] = i * rows_stride (the last element also
+  // writes the end)
+  __device__ __forceinline__ void stage_ann_offsets(uint64_t s, uint32_t k) const {
+    for (uint32_t j = 0; j < k; j++) row_ann_off[(uint64_t)j * n + s] = ((uint64_t)j * n + s) * rows_stride;
+    if (s + 1 == n) row_ann_off[(uint64_t)k * n] = (uint64_t)k * n * rows_stride;
+  }
+  // consume: the entry of staged datapoint d of row `row`, slot o's a_len bytes (length 0, which the append takes as
+  // none, without an annotation); an entry past a row's count is never read
+  __device__ __forceinline__ void stage_ann(uint64_t row, uint64_t d, uint64_t o, uint32_t a_len) const {
+    m3tsz_annotation_entry en;
+    en.dp_index = (uint32_t)d;
+    en.length = a_len;
+    en.byte_offset = o * ann_cap;
+    row_ann[row * rows_stride + d] = en;
+  }
 };
 // (the annotated kernels when p.ann_len is set)
 cudaError_t launch_element_add(const ElementParams &p, cudaStream_t stream);
@@ -416,6 +451,7 @@ struct ElementTimerParams {
   int32_t type[M3TSZ_MAX_TIMER_TYPES];
   double q[M3TSZ_MAX_TIMER_QUANTILES];  // Types.PooledQuantiles of type[]
 };
+// (the annotated kernels when p.e.ann_len is set, as for the other sets)
 cudaError_t launch_element_timer_add(const ElementTimerParams &p, cudaStream_t stream);
 cudaError_t launch_element_timer_consume(const ElementTimerParams &p, cudaStream_t stream);
 
@@ -456,6 +492,39 @@ struct ElementRollupParams {
   uint32_t *g_ann_len;
   uint8_t *g_ann_slot;
   uint64_t g_ann_cap;
+
+  // The annotated forward's and fold's helpers (the Gauge / Counter lanes and the Timer lanes share them).
+  // forward, after its windows' loop: source s's forwarded windows (bit q of `present`, due slots the bits of `due`)
+  // whose slot holds an annotation (a length of 1 .. src.ann_cap; above the capacity reads as none, as the annotated
+  // consume reads it) set bit q of fwd_ann_present and write their reference to fwd_ann; the slot's bytes stay where
+  // they are for the fold to copy
+  __device__ __forceinline__ void forward_ann(uint64_t s, uint64_t due, uint64_t present) const {
+    const ElementParams &e = src;
+    uint64_t ann = 0;
+    for (uint32_t r = 0; r < e.n_slots; r++) {
+      if (!((due >> r) & 1u)) continue;
+      const uint64_t o = (uint64_t)r * e.n + s;
+      const uint32_t l = e.ann_len[o];
+      if (l == 0 || l > e.ann_cap) continue;
+      const int64_t ws = e.start[o];
+      uint32_t q = 0;  // the window's place in start order
+      for (uint32_t r2 = 0; r2 < e.n_slots; r2++) q += ((due >> r2) & 1u) && e.start[(uint64_t)r2 * e.n + s] < ws;
+      if (!((present >> q) & 1u)) continue;
+      ann |= 1ull << q;
+      fwd_ann[(uint64_t)q * e.n + s] = (o << 17) | l;
+    }
+    fwd_ann_present[s] = ann;
+  }
+  // fold: a group window's annotation to group slot o.  ref is the forward's reference to a source slot (0: none),
+  // whose bytes go over as whole 8-byte words (the annotated add zero-pads a slot's last word), lane `lane` of n_lanes
+  // copying words lane, lane + n_lanes, ...; every lane writes the length
+  __device__ __forceinline__ void store_group_ann(uint64_t o, uint64_t ref, uint32_t lane, uint32_t n_lanes) const {
+    const uint32_t len = (uint32_t)(ref & 0x1ffffu);
+    g_ann_len[o] = len;
+    const uint64_t *from = reinterpret_cast<const uint64_t *>(src.ann_slot + (ref >> 17) * src.ann_cap);
+    uint64_t *dst = reinterpret_cast<uint64_t *>(g_ann_slot + o * g_ann_cap);
+    for (uint32_t w = lane; w < (len + 7u) / 8u; w += n_lanes) dst[w] = from[w];
+  }
 };
 // (the annotated kernels when p.src.ann_len is set)
 cudaError_t launch_element_forward(const ElementRollupParams &p, cudaStream_t stream);
@@ -464,7 +533,8 @@ cudaError_t launch_element_fold(const ElementRollupParams &p, cudaStream_t strea
 cudaError_t launch_element_commit(const ElementRollupParams &p, cudaStream_t stream);
 // Timer sets through a rollup (m3tsz_element_set_forward_timer): p as above (its g_min / g_max / g_last unused), with
 // the source set's streams and one type in `src` and the group set's streams and quantile list in `groups`; the commit
-// is launch_element_commit's.  (p.mark must be zero for the fold.)
+// is launch_element_commit's.  (p.mark must be zero for the fold.)  The annotated kernels when p.src.ann_len is set, with
+// the annotated forward's fields of p.
 cudaError_t launch_element_timer_forward(const ElementRollupParams &p, const ElementTimerParams &src,
                                          cudaStream_t stream);
 cudaError_t launch_element_timer_fold(const ElementRollupParams &p, const ElementTimerParams &groups,

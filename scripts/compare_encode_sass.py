@@ -10,9 +10,9 @@ element_consume_kernel<CTR> are compared too; the annotated element sets added a
 build's <CTR> is compared with a new build's <CTR, false>.  The element rollup's element_forward_kernel,
 element_fold_kernel and element_commit_kernel are compared too; the annotated element rollup added a second argument,
 ANN, to the first two, so an old build's <CTR> is compared with a new build's <CTR, false>.  The Timer element sets'
-element_timer_add_kernel and element_timer_consume_kernel are collected by their own names.  Instantiations only one
-build has (the append mode, new decode modes, the annotated element kernels, the Timer kernels) are listed, not
-compared.
+element_timer_{add,consume,forward,fold}_kernel are compared too; the annotated Timer element sets made them templates
+over ANN, so an old build's untemplated kernel is compared with a new build's <false>.  Instantiations only one build
+has (the append mode, new decode modes, the annotated element kernels) are listed, not compared.
 
     python scripts/compare_encode_sass.py OLD.(o|so) NEW.(o|so)     # exit code 1 on any difference
 
@@ -42,8 +42,8 @@ def kernels(path):
             elif "element_add_kernel" in name or "element_consume_kernel" in name:
                 cur = re.sub(r"(element_(?:add|consume)_kernelILb[01]E)Lb0E", r"\1", name)
                 out[cur] = []
-            elif "element_timer_" in name:  # (Timer element sets: new kernels, listed as new only)
-                cur = name
+            elif "element_timer_" in name:  # (Timer element sets)
+                cur = re.sub(r"(element_timer_(?:add|consume|forward|fold)_kernel)ILb0EEEvNS_", r"\1ENS_", name)
                 out[cur] = []
             elif re.search(r"element_(forward|fold|commit)_kernel", name):  # (element sets through a rollup)
                 cur = re.sub(r"(element_(?:forward|fold)_kernelILb[01]E)Lb0E", r"\1", name)

@@ -808,6 +808,7 @@ def main():
     print("wrote", OUT_ELEM_CONSUME)
     timer_goldens()
     timer_rollup_goldens()
+    timer_annotation_goldens()
 
 
 def timer_goldens():
@@ -882,6 +883,19 @@ def timer_rollup_goldens():
     ]
     with open(out, "w") as f:
         json.dump({"add_unique": add_unique, "pipeline": pipeline}, f, indent=1)
+    print("wrote", out)
+
+
+def timer_annotation_goldens():
+    """tests/golden/m3tsz_timer_annotation_goldens.json: the reference's Timer annotation expectation.  "adds" lists
+    Timer.Add calls in order as [value, annotation] (null for a nil annotation); "want" is Annotation() after them."""
+    out = os.path.join(os.path.dirname(OUT), "m3tsz_timer_annotation_goldens.json")
+    cases = [
+        {"name": "TestTimerReturnsLastNonEmptyAnnotation", "src_line": "aggregator/aggregation/timer_test.go:212-222",
+         "adds": [[1.1, "first"], [2.1, "second"], [3.1, None]], "want": "second"},
+    ]
+    with open(out, "w") as f:
+        json.dump({"cases": cases}, f, indent=1)
     print("wrote", out)
 
 
