@@ -26,7 +26,8 @@
  * m3tsz_decode_downsample_last_batch with a NULL lastAt / sumSq / last output,
  * m3tsz_encode_batch_packed(_ex), m3tsz_compact_streams,
  * m3tsz_encoder_set_write, m3tsz_element_set_reset of a set with output rows,
- * m3tsz_element_set_consume(_annotated), m3tsz_element_set_forward(_annotated)) are
+ * m3tsz_element_set_consume(_annotated), m3tsz_element_set_forward(_annotated),
+ * m3tsz_element_set_forward_write, m3tsz_element_set_add_forwarded) are
  * ordered in the order they are issued: each one's stream waits on the device
  * for the context's previous such call, whatever stream that was on.  Two such
  * calls on one context therefore never overlap; a caller who wants them to
@@ -96,6 +97,7 @@ enum {
   M3TSZ_ERR_CHECKSUM_MISMATCH = 15, /* errSeekChecksumMismatch, persist/fs/seek.go:50-51, read.go:395-397 */
   M3TSZ_ERR_TOO_MANY_ENCODERS = 16, /* errTooManyEncoders, storage/series/buffer.go:57 */
   M3TSZ_ERR_AGGREGATION_CLOSED = 17, /* errAggregationClosed, aggregator/elem_base.go:72 */
+  M3TSZ_ERR_DUPLICATE_SOURCE = 18, /* errDuplicateForwardingSource, aggregator/elem_base.go:74 */
   /* library-level conditions */
   M3TSZ_ERR_CAPACITY = 100,        /* more datapoints / bytes than the caller's buffer holds */
   M3TSZ_ERR_INVALID_ARG = 101,
@@ -1174,6 +1176,91 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
                                         uint64_t n_groups, const m3tsz_element_set *groups,
                                         const m3tsz_element_annotations *group_ann, int32_t *d_src_status,
                                         int32_t *d_group_status, void *stream);
+
+/* Element-set rollups across shards (DESIGN.md §4.12): the reference splits a rollup whose sources live on other
+ * shards in two.  The source shard's forwarded writer (aggregator/forwarded_writer.go) collects, per rollup key and
+ * window, the values of its local sources and sends one aggregated.ForwardedMetric with ForwardMetadata.SourceID; the
+ * group shard takes it through GenericElem.AddUnique (generic_elem.go:241-288), which refuses a (source, version) its
+ * window has already seen.  m3tsz_element_set_forward_write is the first half, m3tsz_element_set_add_forwarded the
+ * second.  Gauge and Counter sets only, without annotations.
+ *
+ * One forwarded metric, pointer-free so that a batch (records + one float64 values array) can be copied, concatenated
+ * or sent as bytes (40 bytes, 8-byte aligned): */
+typedef struct m3tsz_forwarded_metric {
+  uint64_t key;       /* the receiving group set's element index */
+  int64_t time_ns;    /* ForwardedMetric.TimeNanos: the source window's end */
+  uint64_t value_off; /* its first value in the batch's values array */
+  uint32_t n_values;  /* >= 1 */
+  uint32_t source_id; /* ForwardMetadata.SourceID: the writing shard */
+  uint32_t version;   /* ForwardedMetric.Version: 0 (a resend is not taken) */
+  uint32_t reserved;  /* 0 */
+} m3tsz_forwarded_metric;
+
+/* The sources a group set's windows have seen: `capacity` bits per window slot, one per source id, in caller-owned
+ * device memory beside the slot arrays, word-interleaved across elements (word w of slot r of element s at
+ * (r * (capacity / 32) + w) * n_elements + s), 4-byte aligned.  capacity: a multiple of 32 in 32 ..
+ * M3TSZ_MAX_FORWARD_SOURCES.  Pointer-free: growing R or the capacity is a copy.
+ * The bits need no initial value: m3tsz_element_set_add_forwarded zeroes a slot's bits when it opens a window there.
+ * Only m3tsz_element_set_add_forwarded reads or writes them, so a window opened by add or forward has stale bits: a
+ * group set fed by add_forwarded takes all of its values that way, the shard's own sources included (through its own
+ * forward_write records, as the reference's shard reaches its own groups through its client). */
+#define M3TSZ_MAX_FORWARD_SOURCES 65536
+typedef struct m3tsz_element_sources {
+  uint32_t *d_bits;
+  uint32_t capacity; /* bits per slot: a multiple of 32, 32 .. M3TSZ_MAX_FORWARD_SOURCES */
+  uint32_t reserved; /* 0 */
+} m3tsz_element_sources;
+
+/* The source shard's forwarded writer.  src, target_ns, d_group_off, d_members, n_members and n_groups are those of
+ * m3tsz_element_set_forward (there is no group set here: n_groups is the call's group count), and every source
+ * forwards its due windows by that call's rule 1.  Nothing is folded: for each group, in group order, one record per
+ * distinct forwarded window start, in ascending start order, with
+ *   key = d_group_key[g] (d_group_key NULL: g), time_ns = the window start + resolution, source_id as given,
+ *   version 0, and as values the window's forwarded values of the group's members in listed member order (a member
+ *   listed twice contributes twice).  A window to which no member forwards a value gets no record (onDone skips an
+ *   empty bucket).
+ * The records go to d_metrics [metric_capacity] and their values to d_values [value_capacity], groups in order.  A
+ * group whose range decreases or runs past n_members, or that lists a source >= src->n_elements, gets
+ * M3TSZ_ERR_INVALID_ARG and writes nothing.  The others' record and value counts are exclusive-scanned: the groups
+ * that fit inside metric_capacity and value_capacity are written, and every later group gets M3TSZ_ERR_CAPACITY (a
+ * prefix rule).  The commit is rule 6 of m3tsz_element_set_forward: a failed group holds back its members.  So
+ * calling again after growing, with exactly the failed groups, gives the remaining records; the two calls' records
+ * together are the unstopped call's.
+ * d_counts [4] (uint64): metrics written, values written, metrics needed, values needed (all groups but the invalid
+ * ones).  d_src_status [src->n_elements], d_group_status [n_groups]: as in m3tsz_element_set_forward.
+ * Host checks (M3TSZ_ERR_INVALID_ARG before any launch): those of m3tsz_element_set_forward on src, a Timer set, a
+ * source type list of other than one type, n_groups or n_members above 2^40, capacities above 2^40, NULL or
+ * misaligned required pointers. */
+int m3tsz_element_set_forward_write(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                    int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
+                                    uint64_t n_members, uint64_t n_groups, const uint64_t *d_group_key,
+                                    uint32_t source_id, m3tsz_forwarded_metric *d_metrics, uint64_t metric_capacity,
+                                    double *d_values, uint64_t value_capacity, uint64_t *d_counts,
+                                    int32_t *d_src_status, int32_t *d_group_status, void *stream);
+
+/* AddUnique of forwarded metrics into a group set (Entry.addForwardedWithLock -> GenericElem.AddUnique, entry.go:
+ * 1177-1191, generic_elem.go:241-288).  Each element takes its records in array order (which stands in for arrival
+ * order); per record, in that order:
+ *   1. key >= n_elements, n_values 0, a value range past n_values, version != 0 or reserved != 0:
+ *      M3TSZ_ERR_INVALID_ARG, nothing changes;
+ *   2. the group window starts at Truncate(time_ns, resolution) - resolution (Go's truncation, as in add): the slot
+ *      m3tsz_element_set_forward folds the same source window into.  A start below INT64_MIN is INVALID_ARG;
+ *   3. a window ending at or before the element's watermark: M3TSZ_ERR_AGGREGATION_CLOSED, nothing changes;
+ *   4. source_id >= sources->capacity, or a new window with all R slots open: M3TSZ_ERR_CAPACITY for the record and
+ *      every later record of the element in this call (add's stop rule);
+ *   5. the window has seen source_id: M3TSZ_ERR_DUPLICATE_SOURCE, nothing changes, later records continue;
+ *   6. else the source's bit is set and each value is folded in order with m3tsz_element_set_forward's fold (Gauge
+ *      Last = the first value; Counter int64(value), sums that wrap).
+ * d_result (int8 [n_metrics], input order): 0 or the status above.  d_status [n_elements]: M3TSZ_OK or
+ * M3TSZ_ERR_CAPACITY.  After a CAPACITY stop and a grow, sending exactly the refused records again gives the unstopped
+ * result, and so does sending the whole batch again: the accepted records come back DUPLICATE_SOURCE (at-least-once
+ * delivery).  The call reads and writes no annotation arrays and needs no output rows.
+ * Host checks (M3TSZ_ERR_INVALID_ARG before any launch): the set's (a Timer set is refused), a NULL or bad sources
+ * struct, n_metrics or n_values above 2^40, NULL or misaligned required pointers. */
+int m3tsz_element_set_add_forwarded(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                    const m3tsz_element_sources *sources, const m3tsz_forwarded_metric *d_metrics,
+                                    uint64_t n_metrics, const double *d_values, uint64_t n_values, int8_t *d_result,
+                                    int32_t *d_status, void *stream);
 
 /* Timer element sets (DESIGN.md §4.12): an element set of metric_type M3TSZ_METRIC_TIMER, whose windows are
  * aggregation.Timer (aggregation/timer.go) over the CM stream (aggregation/quantile/cm/stream.go).

@@ -21,6 +21,7 @@ ERR_OUT_OF_ORDER = 13
 ERR_TOO_MANY_ITERATORS = 14
 ERR_TOO_MANY_ENCODERS = 16
 ERR_AGGREGATION_CLOSED = 17
+ERR_DUPLICATE_SOURCE = 18
 ERR_CAPACITY = 100
 ERR_INVALID_ARG = 101
 ERR_CUDA = 102
@@ -46,6 +47,7 @@ MAX_ELEMENT_TYPES = 8  # M3TSZ_MAX_ELEMENT_TYPES (m3tsz_aggregate_tiles_types)
 ELEMENT_STATE_BYTES = 160  # sizeof(m3tsz_element_state)
 MAX_ELEMENT_WINDOWS = 64  # M3TSZ_MAX_ELEMENT_WINDOWS (element sets)
 MAX_ELEMENT_ANNOTATION = 65536  # M3TSZ_MAX_ELEMENT_ANNOTATION (bytes per window slot of an annotated element set)
+MAX_FORWARD_SOURCES = 65536  # M3TSZ_MAX_FORWARD_SOURCES (source ids per window slot of m3tsz_element_sources)
 
 UNIT_NONE, UNIT_S, UNIT_MS, UNIT_US, UNIT_NS, UNIT_MIN, UNIT_HOUR, UNIT_DAY, UNIT_YEAR = range(9)
 
@@ -78,6 +80,20 @@ class ElementSet(C.Structure):
                     "d_win_start", "d_win_count", "d_win_sum", "d_win_min", "d_win_max", "d_win_sum_sq", "d_win_last",
                     "d_win_last_at", "d_elem", "d_watermark", "d_out_state", "d_out_buf")] + [
                 ("out_stride", C.c_uint64)]
+
+
+class ForwardedMetric(C.Structure):
+    """m3tsz_forwarded_metric: one record of a forwarded batch, 40 bytes (include/m3tsz_b200.h)."""
+    _fields_ = [("key", C.c_uint64), ("time_ns", C.c_int64), ("value_off", C.c_uint64), ("n_values", C.c_uint32),
+                ("source_id", C.c_uint32), ("version", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+FORWARDED_METRIC_BYTES = 40
+
+
+class ElementSources(C.Structure):
+    """m3tsz_element_sources: the source ids each window slot of a group set has seen (include/m3tsz_b200.h)."""
+    _fields_ = [("d_bits", C.c_void_p), ("capacity", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 class ElementAnnotations(C.Structure):
@@ -159,6 +175,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_element_set_forward_annotated", "m3tsz_element_set_add_timer", "m3tsz_element_set_consume_timer",
     "m3tsz_element_set_forward_timer", "m3tsz_element_set_add_timer_annotated",
     "m3tsz_element_set_consume_timer_annotated", "m3tsz_element_set_forward_timer_annotated",
+    "m3tsz_element_set_forward_write", "m3tsz_element_set_add_forwarded",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -356,6 +373,12 @@ def lib():
     L.m3tsz_element_set_forward.argtypes = [vp, po, pes, i64, vp, vp, u64, u64, pes, vp, vp, vp]
     L.m3tsz_element_set_forward_annotated.restype = C.c_int
     L.m3tsz_element_set_forward_annotated.argtypes = [vp, po, pes, pea, i64, vp, vp, u64, u64, pes, pea, vp, vp, vp]
+    L.m3tsz_element_set_forward_write.restype = C.c_int
+    L.m3tsz_element_set_forward_write.argtypes = [vp, po, pes, i64, vp, vp, u64, u64, vp, C.c_uint32, vp, u64, vp,
+                                                  u64, vp, vp, vp, vp]
+    L.m3tsz_element_set_add_forwarded.restype = C.c_int
+    L.m3tsz_element_set_add_forwarded.argtypes = [vp, po, pes, C.POINTER(ElementSources), vp, u64, vp, u64, vp, vp,
+                                                  vp]
     pts = C.POINTER(ElementTimerStreams)
     L.m3tsz_element_set_add_timer.restype = C.c_int
     L.m3tsz_element_set_add_timer.argtypes = [vp, po, pes, pts, vp, vp, u64, vp, vp, vp, vp, vp]

@@ -290,7 +290,7 @@ class BatchCodec:
     def element_set(self, start: torch.Tensor, metric_type, agg_types, resolution_ns, transforms=(),
                     discard_nan=False, open_windows=4, stride: Optional[int] = None,
                     out_unit=capi.UNIT_S, annotation_capacity=0, sample_capacity: Optional[int] = None, eps=1e-3,
-                    insert_and_compress_every=1024) -> "ElementSet":
+                    insert_and_compress_every=1024, source_capacity=0) -> "ElementSet":
         """N aggregator elements fed datapoint by datapoint (m3tsz_element_set_*, N = start.numel(), start int64
         [N] ns): one metric type (capi.METRIC_GAUGE / METRIC_COUNTER), resolution, strictly ascending list of
         aggregation types and transformation list, checked and applied as in aggregate_tiles_types (discard_nan
@@ -306,9 +306,13 @@ class BatchCodec:
         `insert_and_compress_every` (the aggregator's StreamOptions), holding at most `sample_capacity` values (list
         samples and pending values together; required).  With annotation_capacity a Timer set keeps annotations too
         (m3tsz_element_set_*_timer_annotated: a batch's annotation is its first row's).  It forwards through a rollup
-        with ElementSet.forward_timer, not forward."""
+        with ElementSet.forward_timer, not forward.
+        source_capacity > 0 (a multiple of 32, at most capi.MAX_FORWARD_SOURCES): the set is a rollup's group set fed
+        across shards (ElementSet.add_forwarded), each open window keeping which of that many source ids it has
+        seen."""
         return ElementSet(self, start, metric_type, agg_types, resolution_ns, transforms, discard_nan, open_windows,
-                          stride, out_unit, annotation_capacity, sample_capacity, eps, insert_and_compress_every)
+                          stride, out_unit, annotation_capacity, sample_capacity, eps, insert_and_compress_every,
+                          source_capacity)
 
     def bucket_set(self, start: torch.Tensor, stride: int, encoders=4, pool_records: Optional[int] = None,
                    pool_stride: Optional[int] = None) -> "BucketSet":
@@ -873,6 +877,45 @@ class BucketSet:
                                        strategy=0)
 
 
+class ForwardedBatch:
+    """The records a shard's forwarded writer wrote (ElementSet.forward_write): `metrics` uint8 [M, 40] rows of
+    capi.ForwardedMetric (key, time_ns, value_off, n_values, source_id, version, reserved), `values` float64 [V], and
+    `counts` (metrics written, values written, metrics needed, values needed).  Pointer-free: a batch can be copied
+    or sent as bytes."""
+
+    def __init__(self, metrics: torch.Tensor, values: torch.Tensor, counts):
+        self.metrics, self.values, self.counts = metrics, values, tuple(int(c) for c in counts)
+
+    def fields(self):
+        """The records as numpy arrays {"key", "time_ns", "value_off", "n_values", "source_id", "version",
+        "reserved"}."""
+        import numpy as np
+        a = self.metrics.cpu().numpy().reshape(-1, capi.FORWARDED_METRIC_BYTES)
+        u64 = lambda o: a[:, o:o + 8].copy().view(np.uint64)[:, 0]
+        u32 = lambda o: a[:, o:o + 4].copy().view(np.uint32)[:, 0]
+        return {"key": u64(0), "time_ns": u64(8).view(np.int64), "value_off": u64(16), "n_values": u32(24),
+                "source_id": u32(28), "version": u32(32), "reserved": u32(36)}
+
+    @staticmethod
+    def concat(batches) -> "ForwardedBatch":
+        """One batch of the given batches' records in order, each batch's value offsets moved past the values
+        before it."""
+        batches = list(batches)
+        ms, vs, base = [], [], 0
+        for b in batches:
+            m = b.metrics.clone()
+            if m.shape[0]:
+                off = m[:, 16:24].contiguous().view(torch.int64).view(-1) + base
+                m[:, 16:24] = off.view(torch.uint8).view(-1, 8)
+            ms.append(m)
+            vs.append(b.values)
+            base += b.values.numel()
+        dev = batches[0].metrics.device if batches else "cuda"
+        metrics = torch.cat(ms) if ms else torch.zeros((0, capi.FORWARDED_METRIC_BYTES), dtype=torch.uint8, device=dev)
+        values = torch.cat(vs) if vs else torch.zeros(0, dtype=torch.float64, device=dev)
+        return ForwardedBatch(metrics, values, (metrics.shape[0], values.numel(), metrics.shape[0], values.numel()))
+
+
 class ElementSet:
     """Aggregator elements on the device (m3tsz_element_set_*, DESIGN.md §4.12).  The caller-side arrays: `win`, the
     open-window slots window-slot-major [R, N] (start, count -- 0 for a free slot -- sum, min, max, sum_sq, and for
@@ -887,7 +930,7 @@ class ElementSet:
 
     def __init__(self, codec: BatchCodec, start: torch.Tensor, metric_type, agg_types, resolution_ns, transforms,
                  discard_nan, open_windows, stride, out_unit, annotation_capacity=0, sample_capacity=None, eps=1e-3,
-                 insert_and_compress_every=1024):
+                 insert_and_compress_every=1024, source_capacity=0):
         assert start.dtype == torch.int64 and start.is_cuda
         self.codec = codec
         self.metric_type = int(metric_type)
@@ -924,6 +967,9 @@ class ElementSet:
         if annotation_capacity:
             self.ann_len = torch.zeros((R, N), dtype=torch.int32, device=dev)
             self.ann_bytes = torch.zeros((R, N, int(annotation_capacity)), dtype=torch.uint8, device=dev)
+        self.source_bits = None
+        if source_capacity:
+            self.source_bits = torch.zeros((R, int(source_capacity) // 32, N), dtype=torch.int32, device=dev)
         if stride is None:
             stride = int(capi.lib().m3tsz_encode_bound_units(128, 1))
         start = start.contiguous()
@@ -1105,10 +1151,18 @@ class ElementSet:
         return status
 
     def grow(self, open_windows: Optional[int] = None, stride: Optional[int] = None,
-             annotation_capacity: Optional[int] = None, sample_capacity: Optional[int] = None):
+             annotation_capacity: Optional[int] = None, sample_capacity: Optional[int] = None,
+             source_capacity: Optional[int] = None):
         """More open-window slots per element (the slots are copied; the new ones are free), larger output slots
         (EncoderSet.grow) and / or, for a set that keeps annotations, more annotation bytes per slot (copied), or for a
-        Timer set more stream samples per slot (copied)."""
+        Timer set more stream samples per slot (copied), or for a set fed by add_forwarded more source ids per slot
+        (copied)."""
+        if source_capacity is not None and source_capacity != self.source_capacity:
+            assert self.source_bits is not None and source_capacity > self.source_capacity
+            b = torch.zeros((self.open_windows, int(source_capacity) // 32, self.n_elements), dtype=torch.int32,
+                            device=self.source_bits.device)
+            b[:, : self.source_bits.shape[1]] = self.source_bits
+            self.source_bits = b
         if sample_capacity is not None and sample_capacity != self.sample_capacity:
             assert self.timer and sample_capacity > self.sample_capacity
             C0 = self.sample_capacity
@@ -1131,6 +1185,11 @@ class ElementSet:
                                  device=self.ann_bytes.device)
                 by[:R] = self.ann_bytes
                 self.ann_len, self.ann_bytes = ln, by
+            if self.source_bits is not None:
+                b = torch.zeros((open_windows,) + tuple(self.source_bits.shape[1:]), dtype=torch.int32,
+                                device=self.source_bits.device)
+                b[:R] = self.source_bits
+                self.source_bits = b
             if self.streams is not None:
                 for f, a in self.streams.items():
                     b = torch.zeros((open_windows,) + tuple(a.shape[1:]), dtype=a.dtype, device=a.device)
@@ -1236,13 +1295,88 @@ class ElementSet:
         self.codec.ctx.check(rc, "m3tsz_element_set_forward_timer_annotated")
         return src_status[: self.n_elements], group_status[:G]
 
+    @property
+    def source_capacity(self) -> int:
+        return 0 if self.source_bits is None else self.source_bits.shape[1] * 32
+
+    def forward_write(self, target_ns, group_off: torch.Tensor, members: torch.Tensor, source_id: int,
+                      keys: Optional[torch.Tensor] = None, metric_capacity: Optional[int] = None,
+                      value_capacity: Optional[int] = None):
+        """This set as a rollup's source set on shard `source_id` (m3tsz_element_set_forward_write, DESIGN.md
+        §4.12): every element's open windows that ended by target_ns are forwarded as in forward(), but instead of a
+        fold each group g (members[group_off[g] .. group_off[g + 1]), as forward() takes them) writes one record per
+        distinct forwarded window start, in ascending order: key keys[g] (int64 [G]; None: g), time_ns the window's
+        end, its members' values in listed order.  Groups are written in order while they fit metric_capacity /
+        value_capacity (default: room for every record); every later group gets ERR_CAPACITY and holds its members
+        back, so calling again with exactly the failed groups and more room gives the rest.  Returns (ForwardedBatch,
+        source statuses int32 [N], group statuses int32 [G]: OK, ERR_CAPACITY or ERR_INVALID_ARG)."""
+        if self.timer:
+            raise ValueError("Timer sets take no forward_write")
+        assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
+        assert members.is_cuda and members.dtype == torch.int32 and members.is_contiguous()
+        if keys is not None:
+            assert keys.is_cuda and keys.dtype == torch.int64 and keys.is_contiguous()
+            assert keys.numel() == group_off.numel() - 1
+        G = group_off.numel() - 1
+        assert G >= 0, "group_off has G + 1 entries"
+        if metric_capacity is None:
+            metric_capacity = members.numel() * self.open_windows
+        if value_capacity is None:
+            value_capacity = members.numel() * self.open_windows
+        dev = self.codec.device
+        metrics = torch.zeros((max(1, int(metric_capacity)), capi.FORWARDED_METRIC_BYTES), dtype=torch.uint8,
+                              device=dev)
+        values = torch.zeros(max(1, int(value_capacity)), dtype=torch.float64, device=dev)
+        counts = torch.zeros(4, dtype=torch.int64, device=dev)
+        src_status = torch.empty(max(1, self.n_elements), dtype=torch.int32, device=dev)
+        group_status = torch.empty(max(1, G), dtype=torch.int32, device=dev)
+        rc = capi.lib().m3tsz_element_set_forward_write(
+            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(self._desc()), int(target_ns), _ptr(group_off),
+            _ptr(members), members.numel(), G, _ptr(keys), int(source_id), metrics.data_ptr(), int(metric_capacity),
+            values.data_ptr(), int(value_capacity), counts.data_ptr(), _ptr(src_status), _ptr(group_status),
+            _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_forward_write")
+        c = counts.tolist()
+        batch = ForwardedBatch(metrics[: c[0]], values[: c[1]], c)
+        return batch, src_status[: self.n_elements], group_status[:G]
+
+    def add_forwarded(self, batches):
+        """AddUnique of forwarded metrics (m3tsz_element_set_add_forwarded, DESIGN.md §4.12) into this set, which
+        needs a source_capacity: one ForwardedBatch or a list, concatenated in the given order (value offsets
+        rebased), each element taking its records in that order.  Returns (result int8 [M] in record order: OK,
+        ERR_INVALID_ARG, ERR_AGGREGATION_CLOSED, ERR_CAPACITY -- the element stopped: grow() and send the refused
+        records again --, or ERR_DUPLICATE_SOURCE -- the window has seen that source --; status int32 [N]: OK or
+        ERR_CAPACITY)."""
+        if self.timer:
+            raise ValueError("Timer sets take no add_forwarded")
+        if self.source_bits is None:
+            raise ValueError("add_forwarded needs an element set with a source_capacity")
+        b = batches if isinstance(batches, ForwardedBatch) else ForwardedBatch.concat(batches)
+        metrics, values = b.metrics.contiguous(), b.values.contiguous()
+        M = metrics.shape[0]
+        dev = self.codec.device
+        result = torch.zeros(max(1, M), dtype=torch.int8, device=dev)
+        status = torch.zeros(max(1, self.n_elements), dtype=torch.int32, device=dev)
+        src = capi.ElementSources()
+        src.d_bits = self.source_bits.data_ptr()
+        src.capacity = self.source_capacity
+        rc = capi.lib().m3tsz_element_set_add_forwarded(
+            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(self._desc()), C.byref(src),
+            metrics.data_ptr() if M else None, M, values.data_ptr() if values.numel() else None, values.numel(),
+            result.data_ptr(), status.data_ptr(), _cuda_stream_ptr(dev))
+        self.codec.ctx.check(rc, "m3tsz_element_set_add_forwarded")
+        return result[:M], status[: self.n_elements]
+
     def state(self):
         """Copies of the element-side state: {"win": {field: [R, N]}, "elem": uint8 [N, 160], "watermark": [N]},
-        with annotations "ann_len" [R, N] and "ann_bytes" [R, N, capacity], and for a Timer set "streams"."""
+        with annotations "ann_len" [R, N] and "ann_bytes" [R, N, capacity], for a Timer set "streams", and with a
+        source capacity "source_bits" int32 [R, capacity / 32, N]."""
         st = {"win": {f: a.clone() for f, a in self.win.items()}, "elem": self.elem.clone(),
               "watermark": self.watermark.clone()}
         if self.ann_len is not None:
             st["ann_len"], st["ann_bytes"] = self.ann_len.clone(), self.ann_bytes.clone()
         if self.streams is not None:
             st["streams"] = {f: a.clone() for f, a in self.streams.items()}
+        if self.source_bits is not None:
+            st["source_bits"] = self.source_bits.clone()
         return st

@@ -129,6 +129,7 @@ const char *m3tsz_status_string(int st) {
     case M3TSZ_ERR_TOO_MANY_ITERATORS: return "too many replicas / readers for one series";
     case M3TSZ_ERR_TOO_MANY_ENCODERS: return "too many encoders per block";
     case M3TSZ_ERR_AGGREGATION_CLOSED: return "aggregation is closed";
+    case M3TSZ_ERR_DUPLICATE_SOURCE: return "duplicate forwarding source";
     case M3TSZ_ERR_CHECKSUM_MISMATCH: return "checksum does not match expected checksum";
     case M3TSZ_ERR_CAPACITY: return "output capacity exceeded";
     case M3TSZ_ERR_INVALID_ARG: return "invalid argument";
@@ -1810,6 +1811,143 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
                                         int32_t *d_group_status, void *stream) {
   return element_set_forward(ctx, opts, src, src_ann, target_ns, d_group_off, d_members, n_members, n_groups, groups,
                              group_ann, d_src_status, d_group_status, stream, true);
+}
+
+// ---- element-set rollups across shards ----
+// The forward kernel writes each source's due windows to scratch (element_forward_scratch, with no group set), the
+// count pass counts each group's records and values, two scans place them, the write pass writes the groups that fit
+// and marks the members of the others, and the commit kernel frees the other sources' due windows.
+int m3tsz_element_set_forward_write(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                    int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
+                                    uint64_t n_members, uint64_t n_groups, const uint64_t *d_group_key,
+                                    uint32_t source_id, m3tsz_forwarded_metric *d_metrics, uint64_t metric_capacity,
+                                    double *d_values, uint64_t value_capacity, uint64_t *d_counts,
+                                    int32_t *d_src_status, int32_t *d_group_status, void *stream) {
+  ElementForwardedParams fp;
+  memset(&fp, 0, sizeof(fp));
+  ElementRollupParams &rp = fp.rp;
+  TileTransforms sx;
+  if (!ctx || !element_params(opts, src, rp.src, sx)) return M3TSZ_ERR_INVALID_ARG;
+  if (sx.n_types != 1 || n_groups > (1ull << 40) || n_members > (1ull << 40) || metric_capacity > (1ull << 40) ||
+      value_capacity > (1ull << 40) || (n_groups && !d_group_off) || (n_members && !d_members) ||
+      ((uintptr_t)d_group_off & 7u) || ((uintptr_t)d_members & 3u) || ((uintptr_t)d_group_key & 7u) || !d_counts ||
+      ((uintptr_t)d_counts & 7u) || (metric_capacity && (!d_metrics || ((uintptr_t)d_metrics & 7u))) ||
+      (value_capacity && (!d_values || ((uintptr_t)d_values & 7u))))
+    return M3TSZ_ERR_INVALID_ARG;
+  if (!forward_statuses_ok(rp.src.n, n_groups, d_src_status, d_group_status)) return M3TSZ_ERR_INVALID_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  cudaStream_t st = (cudaStream_t)stream;
+  CK(cudaMemsetAsync(d_counts, 0, 4 * 8, st));
+  if (rp.src.n == 0 && n_groups == 0) return M3TSZ_OK;
+  ScratchFence fence(ctx, st);
+  ElementParams none;  // (no group set: the fold's fields stay unused)
+  memset(&none, 0, sizeof(none));
+  int rc = element_forward_scratch(ctx, fence, rp, none, target_ns, d_group_off, d_members, n_members, n_groups,
+                                   d_src_status, d_group_status, src->discard_nan);
+  if (rc != M3TSZ_OK) return rc;
+  const uint64_t gn = n_groups ? n_groups : 1;
+  void *d_nr, *d_nv, *d_ro, *d_vo, *d_tmp;
+  size_t tmp_bytes = 0;
+  CK(forward_write_scan(nullptr, tmp_bytes, nullptr, nullptr, gn, st));
+  if ((rc = ensure(ctx, fence, kSlotElemFwdRecN, gn * 8, &d_nr))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdValN, gn * 8, &d_nv))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdRecOff, gn * 8, &d_ro))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdValOff, gn * 8, &d_vo))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemFwdScanTmp, tmp_bytes ? tmp_bytes : 1, &d_tmp))) return rc;
+  fp.group_key = d_group_key;
+  fp.source_id = source_id;
+  fp.out_rec = d_metrics;
+  fp.out_val = d_values;
+  fp.rec_cap = metric_capacity;
+  fp.val_cap = value_capacity;
+  fp.n_rec = (uint64_t *)d_nr;
+  fp.n_val = (uint64_t *)d_nv;
+  fp.rec_off = (uint64_t *)d_ro;
+  fp.val_off = (uint64_t *)d_vo;
+  fp.counts = d_counts;
+  CK(cudaMemsetAsync(rp.mark, 0, (rp.src.n ? rp.src.n : 1) * 4, st));
+  CK(launch_element_forward(rp, st));
+  CK(launch_forward_write_count(fp, st));
+  if (n_groups) {
+    CK(forward_write_scan(d_tmp, tmp_bytes, fp.n_rec, fp.rec_off, n_groups, st));
+    CK(forward_write_scan(d_tmp, tmp_bytes, fp.n_val, fp.val_off, n_groups, st));
+  }
+  CK(launch_forward_write(fp, st));
+  CK(launch_element_commit(rp, st));
+  ctx->launches += 6;
+  return M3TSZ_OK;
+}
+
+// The prep kernel writes each record's element key and index, the radix sort orders them by key (stable, so each
+// element's records stay in array order), and one lane per element takes its records.
+int m3tsz_element_set_add_forwarded(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                    const m3tsz_element_sources *sources, const m3tsz_forwarded_metric *d_metrics,
+                                    uint64_t n_metrics, const double *d_values, uint64_t n_values, int8_t *d_result,
+                                    int32_t *d_status, void *stream) {
+  ElementForwardedParams fp;
+  memset(&fp, 0, sizeof(fp));
+  ElementParams gp;
+  TileTransforms gx;
+  if (!ctx || !element_params(opts, set, gp, gx)) return M3TSZ_ERR_INVALID_ARG;
+  if (!sources || sources->reserved != 0 || sources->capacity == 0 || (sources->capacity & 31u) ||
+      sources->capacity > M3TSZ_MAX_FORWARD_SOURCES || !sources->d_bits || ((uintptr_t)sources->d_bits & 3u) ||
+      n_metrics > (1ull << 40) || n_values > (1ull << 40) || (n_metrics && (!d_metrics || !d_result)) ||
+      ((uintptr_t)d_metrics & 7u) || (n_values && !d_values) || ((uintptr_t)d_values & 7u) ||
+      (gp.n && (!d_status || ((uintptr_t)d_status & 3u))))
+    return M3TSZ_ERR_INVALID_ARG;
+  if (gp.n == 0 && n_metrics == 0) return M3TSZ_OK;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return set_cuda_error(ctx, guard.err, "cudaSetDevice");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (gp.n) CK(cudaMemsetAsync(d_status, 0, gp.n * 4, st));
+  if (n_metrics == 0) return M3TSZ_OK;
+  ScratchFence fence(ctx, st);
+  int end_bit = 1;  // the key bits: elements 0 .. n - 1, and n for an invalid key
+  while (end_bit < 64 && (gp.n >> end_bit) != 0) end_bit++;
+  size_t tmp_bytes = 0;
+  CK(add_forwarded_sort(nullptr, tmp_bytes, nullptr, nullptr, nullptr, nullptr, n_metrics, end_bit, st));
+  void *d_k, *d_i, *d_sk, *d_si, *d_tmp;
+  int rc;
+  if ((rc = ensure(ctx, fence, kSlotElemAddFwdKey, n_metrics * 8, &d_k))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemAddFwdIdx, n_metrics * 8, &d_i))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemAddFwdSortedKey, n_metrics * 8, &d_sk))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemAddFwdSortedIdx, n_metrics * 8, &d_si))) return rc;
+  if ((rc = ensure(ctx, fence, kSlotElemAddFwdSortTmp, tmp_bytes ? tmp_bytes : 1, &d_tmp))) return rc;
+  ElementRollupParams &rp = fp.rp;
+  rp.src.n = gp.n;
+  rp.src.counter = gp.counter;
+  rp.src.resolution = gp.resolution;
+  rp.n_groups = gp.n;
+  rp.g_slots = gp.n_slots;
+  rp.g_start = gp.start;
+  rp.g_count = gp.count;
+  rp.g_sum = gp.sum;
+  rp.g_min = gp.min;
+  rp.g_max = gp.max;
+  rp.g_sum_sq = gp.sum_sq;
+  rp.g_last = gp.last;
+  rp.g_last_at = gp.last_at;
+  rp.g_watermark = gp.watermark;
+  fp.rec = d_metrics;
+  fp.val = d_values;
+  fp.n_recs = n_metrics;
+  fp.n_vals = n_values;
+  fp.sort_key = (uint64_t *)d_k;
+  fp.sort_idx = (uint64_t *)d_i;
+  fp.sorted_key = (const uint64_t *)d_sk;
+  fp.sorted_idx = (const uint64_t *)d_si;
+  fp.bits = sources->d_bits;
+  fp.bit_words = sources->capacity / 32u;
+  fp.trunc_off = gp.trunc_off;
+  fp.result = d_result;
+  fp.status = d_status;
+  CK(launch_add_forwarded_prep(fp, st));
+  CK(add_forwarded_sort(d_tmp, tmp_bytes, fp.sort_key, (uint64_t *)d_sk, fp.sort_idx, (uint64_t *)d_si, n_metrics,
+                        end_bit, st));
+  CK(launch_add_forwarded(fp, st));
+  ctx->launches += 3;
+  return M3TSZ_OK;
 }
 
 // element_set_forward with the Timer forward and fold kernels: the same groups, scratch, annotation scratch and

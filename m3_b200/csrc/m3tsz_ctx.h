@@ -135,7 +135,19 @@ enum Slot : int {
   // ... that keep annotations
   kSlotElemFwdAnnPresent = 80,
   kSlotElemFwdAnn = 81,
-  kNumSlots = 82
+  // element-set rollups across shards: the writer's per-group counts, their scans and the scan's scratch; the
+  // AddUnique's sort keys and indices before and after the sort, and the sort's scratch
+  kSlotElemFwdRecN = 82,
+  kSlotElemFwdValN = 83,
+  kSlotElemFwdRecOff = 84,
+  kSlotElemFwdValOff = 85,
+  kSlotElemFwdScanTmp = 86,
+  kSlotElemAddFwdKey = 87,
+  kSlotElemAddFwdIdx = 88,
+  kSlotElemAddFwdSortedKey = 89,
+  kSlotElemAddFwdSortedIdx = 90,
+  kSlotElemAddFwdSortTmp = 91,
+  kNumSlots = 92
 };
 
 // Buffer k (0-8) of pipeline lane `lane` (0 or 1): slots 16-24 and 26-34.

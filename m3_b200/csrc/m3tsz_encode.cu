@@ -16,6 +16,7 @@
 //   m3tsz/m3tsz.go:78-119, ostream.go:133-221, scheme.go:198-220.
 #include <cstring>
 #include <type_traits>
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cuda.h>  // CUtensorMap (types only: the encoder is resolved through cudaGetDriverEntryPoint)
 
@@ -3926,6 +3927,277 @@ cudaError_t launch_element_commit(const ElementRollupParams &p, cudaStream_t str
   if ((p.src.n + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
   element_commit_kernel<<<elem_blocks(p.src.n), ELEM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------
+// element-set rollups across shards (DESIGN.md §4.12): the forwarded writer and AddUnique of its records
+// ---------------------------------------------------------------------------
+// The smallest forwarded window start of group g's members above `prev` (have: a start was found before); each
+// member's forwarded starts ascend with q, so a member's first start above prev is its candidate
+__device__ __forceinline__ bool fw_next_start(const ElementRollupParams &p, uint64_t lo, uint64_t hi, bool have,
+                                              int64_t prev, int64_t &next) {
+  bool found = false;
+  for (uint64_t i = lo; i < hi; i++) {
+    const uint64_t m = p.members[i];
+    const uint32_t n = p.fwd_n[m];
+    const uint64_t pr = p.fwd_present[m];
+    for (uint32_t q = 0; q < n; q++) {
+      if (!((pr >> q) & 1u)) continue;
+      const int64_t ws = p.fwd_start[(uint64_t)q * p.src.n + m];
+      if (have && ws <= prev) continue;
+      if (!found || ws < next) next = ws;
+      found = true;
+      break;
+    }
+  }
+  return found;
+}
+
+// Group g's range and member checks (INVALID_ARG: no records), its record count (distinct forwarded starts) and value
+// count (forwarded values)
+__device__ __forceinline__ void fw_count_group(const ElementForwardedParams &p, uint64_t g) {
+  const ElementRollupParams &rp = p.rp;
+  const uint64_t lo = rp.group_off[g], hi = rp.group_off[g + 1];
+  bool bad = lo > hi || hi > rp.n_members;
+  uint64_t nv = 0;
+  for (uint64_t i = lo; i < hi && !bad; i++) {
+    const uint64_t m = rp.members[i];
+    if (m >= rp.src.n) {
+      bad = true;
+    } else {
+      const uint32_t n = rp.fwd_n[m];
+      nv += __popcll(rp.fwd_present[m] & (n >= 64 ? ~0ull : ((1ull << n) - 1)));
+    }
+  }
+  uint64_t nr = 0;
+  if (!bad) {
+    int64_t ws = 0, nx = 0;
+    while (fw_next_start(rp, lo, hi, nr != 0, ws, nx)) {
+      ws = nx;
+      nr++;
+    }
+  } else {
+    nv = 0;
+  }
+  p.n_rec[g] = nr;
+  p.n_val[g] = nv;
+  rp.group_status[g] = bad ? M3TSZ_ERR_INVALID_ARG : M3TSZ_OK;
+}
+__global__ void __launch_bounds__(ELEM_THREADS) forward_write_count_kernel(const ElementForwardedParams p) {
+  const uint64_t g = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (g < p.rp.n_groups) fw_count_group(p, g);
+}
+
+// A valid group that fits (its records and values end within the capacities) writes them at its scanned offsets; a
+// later one gets CAPACITY.  The last group that fits writes the written counts, the last group the needed ones (the
+// caller zeroes `counts`).  Returns the group's status (also written to group_status[g]).
+__device__ __forceinline__ int32_t fw_write_group(const ElementForwardedParams &p, uint64_t g) {
+  const ElementRollupParams &rp = p.rp;
+  const uint64_t G = rp.n_groups;
+  const uint64_t rec_end = p.rec_off[g] + p.n_rec[g], val_end = p.val_off[g] + p.n_val[g];
+  const bool fit = rec_end <= p.rec_cap && val_end <= p.val_cap;
+  // (the next group's offsets are this group's ends: it fits when its own ends do)
+  if (fit && (g + 1 == G || p.rec_off[g + 1] + p.n_rec[g + 1] > p.rec_cap ||
+              p.val_off[g + 1] + p.n_val[g + 1] > p.val_cap)) {
+    p.counts[0] = rec_end;
+    p.counts[1] = val_end;
+  }
+  if (g + 1 == G) {
+    p.counts[2] = rec_end;
+    p.counts[3] = val_end;
+  }
+  const uint64_t lo = rp.group_off[g], hi = rp.group_off[g + 1];
+  int32_t st = rp.group_status[g];
+  if (st == M3TSZ_OK && !fit) st = M3TSZ_ERR_CAPACITY;
+  if (st == M3TSZ_OK) {
+    uint64_t r = p.rec_off[g], v = p.val_off[g];
+    int64_t ws = 0, nx = 0;
+    bool have = false;
+    while (fw_next_start(rp, lo, hi, have, ws, nx)) {
+      ws = nx;
+      have = true;
+      const uint64_t v0 = v;
+      for (uint64_t i = lo; i < hi; i++) {
+        const uint64_t m = rp.members[i];
+        const uint32_t n = rp.fwd_n[m];
+        const uint64_t pr = rp.fwd_present[m];
+        for (uint32_t q = 0; q < n; q++) {
+          const int64_t s = rp.fwd_start[(uint64_t)q * rp.src.n + m];
+          if (s > ws) break;
+          if (s == ws && ((pr >> q) & 1u)) p.out_val[v++] = rp.fwd_val[(uint64_t)q * rp.src.n + m];
+        }
+      }
+      m3tsz_forwarded_metric &f = p.out_rec[r++];
+      f.key = p.group_key ? p.group_key[g] : g;
+      f.time_ns = (int64_t)((uint64_t)ws + (uint64_t)rp.src.resolution);
+      f.value_off = v0;
+      f.n_values = (uint32_t)(v - v0);
+      f.source_id = p.source_id;
+      f.version = 0;
+      f.reserved = 0;
+    }
+  }
+  rp.group_status[g] = st;
+  return st;
+}
+// A failed group marks its members for the commit.
+__global__ void __launch_bounds__(ELEM_THREADS) forward_write_kernel(const ElementForwardedParams p) {
+  const uint64_t g = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  const ElementRollupParams &rp = p.rp;
+  if (g >= rp.n_groups) return;
+  const int32_t st = fw_write_group(p, g);
+  const uint64_t lo = rp.group_off[g], hi = rp.group_off[g + 1];
+  if (st != M3TSZ_OK && lo <= hi) {
+    const uint64_t end = hi < rp.n_members ? hi : rp.n_members;
+    for (uint64_t i = lo; i < end; i++) {
+      const uint32_t m = rp.members[i];
+      if (m < rp.src.n) atomicMax(rp.mark + m, st);
+    }
+  }
+}
+
+// The radix sort's inputs: record i's element (n for an invalid key) and its index
+__global__ void __launch_bounds__(ELEM_THREADS) add_forwarded_prep_kernel(const ElementForwardedParams p) {
+  const uint64_t i = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (i >= p.n_recs) return;
+  const uint64_t k = p.rec[i].key, n = p.rp.n_groups;
+  p.sort_key[i] = k < n ? k : n;
+  p.sort_idx[i] = i;
+}
+
+// AddUnique of element e's records (sorted positions j .. while the key is e), in array order.  The window the last
+// record went to stays in registers (elem_fold_load / elem_fold_store), as in the fold; a new window's source bits are
+// zeroed when it is opened.
+template <bool CTR>
+__device__ __forceinline__ void add_forwarded_lane(const ElementForwardedParams &p, uint64_t j) {
+  const ElementRollupParams &rp = p.rp;
+  const uint64_t e = p.sorted_key[j], G = rp.n_groups;
+  if (e >= G) {
+    for (; j < p.n_recs && p.sorted_key[j] == e; j++) p.result[p.sorted_idx[j]] = (int8_t)M3TSZ_ERR_INVALID_ARG;
+    return;
+  }
+  const int64_t res = rp.src.resolution, wm = rp.g_watermark[e];
+  const uint32_t W = p.bit_words;
+  ElemFoldAcc<CTR> f;
+  int cur = -1;
+  int32_t status = M3TSZ_OK;
+  for (; j < p.n_recs && p.sorted_key[j] == e; j++) {
+    const uint64_t i = p.sorted_idx[j];
+    const m3tsz_forwarded_metric m = p.rec[i];
+    int r = M3TSZ_ERR_CAPACITY;  // (after a CAPACITY, the rest of the element's records)
+    if (status == M3TSZ_OK) {
+      int64_t t0 = 0;
+      if (m.n_values == 0 || m.value_off > p.n_vals || m.n_values > p.n_vals - m.value_off || m.version != 0 ||
+          m.reserved != 0 || !elem_window_start(m.time_ns, res, p.trunc_off, t0) ||
+          t0 < (int64_t)0x8000000000000000ull + res) {
+        r = M3TSZ_ERR_INVALID_ARG;
+      } else if (elem_ends_by(t0 - res, res, wm)) {
+        r = M3TSZ_ERR_AGGREGATION_CLOSED;
+      } else if (m.source_id >= W * 32u) {
+        status = r = M3TSZ_ERR_CAPACITY;
+      } else {
+        const int64_t ws = t0 - res;
+        r = M3TSZ_OK;
+        if (cur < 0 || ws != f.start) {  // the window's slot, or a free one
+          int hit = -1, fr = -1;
+          for (uint32_t s = 0; s < rp.g_slots; s++) {
+            if ((int)s == cur) continue;
+            const uint64_t o = (uint64_t)s * G + e;
+            if (rp.g_count[o] == 0) {
+              if (fr < 0) fr = (int)s;
+            } else if (rp.g_start[o] == ws) {
+              hit = (int)s;
+              break;
+            }
+          }
+          if (hit < 0 && fr < 0) {
+            status = r = M3TSZ_ERR_CAPACITY;
+          } else {
+            if (cur >= 0) elem_fold_store(rp, (uint64_t)cur * G + e, f);
+            cur = hit >= 0 ? hit : fr;
+            if (hit >= 0) {
+              elem_fold_load(rp, (uint64_t)hit * G + e, f);
+            } else {
+              f.start = ws;
+              if constexpr (CTR)
+                rollup_counter_init(f.a);
+              else
+                rollup_gauge_init(f.a);
+              for (uint32_t w = 0; w < W; w++) p.bits[((uint64_t)cur * W + w) * G + e] = 0u;
+            }
+          }
+        }
+        if (r == M3TSZ_OK) {
+          uint32_t *word = p.bits + ((uint64_t)cur * W + (m.source_id >> 5)) * G + e;
+          const uint32_t bit = 1u << (m.source_id & 31u);
+          if (*word & bit) {
+            r = M3TSZ_ERR_DUPLICATE_SOURCE;
+          } else {
+            *word |= bit;
+            for (uint32_t k = 0; k < m.n_values; k++) {
+              const double v = p.val[m.value_off + k];
+              if constexpr (CTR)
+                rollup_counter_add(f.a, v);
+              else
+                rollup_gauge_add(f.a, v);
+            }
+          }
+        }
+      }
+    }
+    p.result[i] = (int8_t)r;
+  }
+  if (cur >= 0) elem_fold_store(rp, (uint64_t)cur * G + e, f);
+  p.status[e] = status;
+}
+
+template <bool CTR>
+__global__ void __launch_bounds__(ELEM_THREADS) add_forwarded_kernel(const ElementForwardedParams p) {
+  const uint64_t j = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (j >= p.n_recs || (j && p.sorted_key[j - 1] == p.sorted_key[j])) return;  // one lane per element with records
+  add_forwarded_lane<CTR>(p, j);
+}
+
+cudaError_t launch_forward_write_count(const ElementForwardedParams &p, cudaStream_t stream) {
+  if (p.rp.n_groups == 0) return cudaSuccess;
+  if ((p.rp.n_groups + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  forward_write_count_kernel<<<elem_blocks(p.rp.n_groups), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_forward_write(const ElementForwardedParams &p, cudaStream_t stream) {
+  if (p.rp.n_groups == 0) return cudaSuccess;
+  if ((p.rp.n_groups + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  forward_write_kernel<<<elem_blocks(p.rp.n_groups), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_add_forwarded_prep(const ElementForwardedParams &p, cudaStream_t stream) {
+  if (p.n_recs == 0) return cudaSuccess;
+  if ((p.n_recs + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  add_forwarded_prep_kernel<<<elem_blocks(p.n_recs), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_add_forwarded(const ElementForwardedParams &p, cudaStream_t stream) {
+  if (p.n_recs == 0) return cudaSuccess;
+  if ((p.n_recs + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  if (p.rp.src.counter)
+    add_forwarded_kernel<true><<<elem_blocks(p.n_recs), ELEM_THREADS, 0, stream>>>(p);
+  else
+    add_forwarded_kernel<false><<<elem_blocks(p.n_recs), ELEM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t forward_write_scan(void *tmp, size_t &bytes, const uint64_t *in, uint64_t *out, uint64_t n,
+                               cudaStream_t stream) {
+  return cub::DeviceScan::ExclusiveSum(tmp, bytes, in, out, n, stream);
+}
+
+cudaError_t add_forwarded_sort(void *tmp, size_t &bytes, const uint64_t *key_in, uint64_t *key_out,
+                               const uint64_t *idx_in, uint64_t *idx_out, uint64_t n, int end_bit,
+                               cudaStream_t stream) {
+  return cub::DeviceRadixSort::SortPairs(tmp, bytes, key_in, key_out, idx_in, idx_out, n, 0, end_bit, stream);
 }
 
 // ---------------------------------------------------------------------------

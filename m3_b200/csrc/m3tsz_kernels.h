@@ -531,6 +531,43 @@ cudaError_t launch_element_forward(const ElementRollupParams &p, cudaStream_t st
 // (p.mark must be zero)
 cudaError_t launch_element_fold(const ElementRollupParams &p, cudaStream_t stream);
 cudaError_t launch_element_commit(const ElementRollupParams &p, cudaStream_t stream);
+// element-set rollups across shards (m3tsz_element_set_forward_write / _add_forwarded; m3tsz_encode.cu).
+// forward_write: p.fwd_* from launch_element_forward; the count pass writes each group's record and value counts (and
+// INVALID_ARG / OK to group_status), the caller scans them into rec_off / val_off, and the write pass writes the groups
+// that fit, the statuses, the commit marks and `counts`.  add_forwarded: the records' element keys (key, or n for an
+// invalid key) and indices for the caller's radix sort, then one lane per element over the sorted indices.
+struct ElementForwardedParams {
+  ElementRollupParams rp;  // forward_write: the forward's; add_forwarded: the group set as rp.g_* / rp.n_groups
+  const uint64_t *group_key;
+  uint32_t source_id;
+  m3tsz_forwarded_metric *out_rec;
+  double *out_val;
+  uint64_t rec_cap, val_cap;
+  uint64_t *n_rec, *n_val, *rec_off, *val_off;
+  uint64_t *counts;
+  // add_forwarded
+  const m3tsz_forwarded_metric *rec;
+  const double *val;
+  uint64_t n_recs, n_vals;
+  uint64_t *sort_key, *sort_idx;          // prep: key / index in record order
+  const uint64_t *sorted_key, *sorted_idx;  // the lanes: after the sort
+  uint32_t *bits;
+  uint32_t bit_words;  // capacity / 32
+  int64_t trunc_off;
+  int8_t *result;
+  int32_t *status;
+};
+cudaError_t launch_forward_write_count(const ElementForwardedParams &p, cudaStream_t stream);
+cudaError_t launch_forward_write(const ElementForwardedParams &p, cudaStream_t stream);
+cudaError_t launch_add_forwarded_prep(const ElementForwardedParams &p, cudaStream_t stream);
+cudaError_t launch_add_forwarded(const ElementForwardedParams &p, cudaStream_t stream);
+// cub scratch sizes and calls for the two passes (tmp NULL: *bytes gets the size)
+cudaError_t forward_write_scan(void *tmp, size_t &bytes, const uint64_t *in, uint64_t *out, uint64_t n,
+                               cudaStream_t stream);
+cudaError_t add_forwarded_sort(void *tmp, size_t &bytes, const uint64_t *key_in, uint64_t *key_out,
+                               const uint64_t *idx_in, uint64_t *idx_out, uint64_t n, int end_bit,
+                               cudaStream_t stream);
+
 // Timer sets through a rollup (m3tsz_element_set_forward_timer): p as above (its g_min / g_max / g_last unused), with
 // the source set's streams and one type in `src` and the group set's streams and quantile list in `groups`; the commit
 // is launch_element_commit's.  (p.mark must be zero for the fold.)  The annotated kernels when p.src.ann_len is set, with

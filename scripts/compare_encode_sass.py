@@ -11,7 +11,8 @@ build's <CTR> is compared with a new build's <CTR, false>.  The element rollup's
 element_fold_kernel and element_commit_kernel are compared too; the annotated element rollup added a second argument,
 ANN, to the first two, so an old build's <CTR> is compared with a new build's <CTR, false>.  The Timer element sets'
 element_timer_{add,consume,forward,fold}_kernel are compared too; the annotated Timer element sets made them templates
-over ANN, so an old build's untemplated kernel is compared with a new build's <false>.  Instantiations only one build
+over ANN, so an old build's untemplated kernel is compared with a new build's <false>.  The cross-shard rollup's
+forward_write_{count_,}kernel and add_forwarded_{prep_,}kernel are compared too.  Instantiations only one build
 has (the append mode, new decode modes, the annotated element kernels) are listed, not compared.
 
     python scripts/compare_encode_sass.py OLD.(o|so) NEW.(o|so)     # exit code 1 on any difference
@@ -47,6 +48,9 @@ def kernels(path):
                 out[cur] = []
             elif re.search(r"element_(forward|fold|commit)_kernel", name):  # (element sets through a rollup)
                 cur = re.sub(r"(element_(?:forward|fold)_kernelILb[01]E)Lb0E", r"\1", name)
+                out[cur] = []
+            elif re.search(r"(forward_write|add_forwarded)", name):  # (element-set rollups across shards)
+                cur = name
                 out[cur] = []
             elif "rollup_forward_kernel" in name or "rollup_fold_kernel" in name:
                 cur = re.sub(r"(rollup_(?:forward|fold)_kernel)ILb0EEEvNS_", r"\1ENS_", name)

@@ -809,6 +809,7 @@ def main():
     timer_goldens()
     timer_rollup_goldens()
     timer_annotation_goldens()
+    forwarded_goldens()
 
 
 def timer_goldens():
@@ -896,6 +897,54 @@ def timer_annotation_goldens():
     ]
     with open(out, "w") as f:
         json.dump({"cases": cases}, f, indent=1)
+    print("wrote", out)
+
+
+def forwarded_goldens():
+    """tests/golden/m3tsz_forwarded_goldens.json: the reference's AddUnique and forwarded-writer expectations.
+    "add_unique" cases are AddUnique calls in order, each step [at_s, values, source_id] with the result the reference
+    returns ("ok" or "duplicate") and what it checks after the step: "windows_s" the open window starts, and in
+    "window_s" the aggregation's "sum" / "count" / "max" / "sum_sq" (sums with "eps" as InEpsilon, the rest exact).
+    The reference checks SumSq only where it computes it (an expensive type in the list, the custom forms).  Steps with
+    a version above 0 (a resend) and the tombstoned element's errElemClosed are not transcribed.  "writer" cases are
+    writeFn calls in order as [id, time_ns, value] and the ForwardedMetrics onDone sends as [id, time_ns, values]."""
+    out = os.path.join(os.path.dirname(OUT), "m3tsz_forwarded_goldens.json")
+    src = "aggregator/aggregator/elem_test.go:120-125,"
+    add_unique = [
+        {"name": "TestCounterElemAddUnique", "src_line": src + "308-390", "metric": "counter", "resolution_s": 10,
+         "custom": False,
+         "steps": [[216, [345.0], 1234, "ok", [210], 210, {"sum": 345, "count": 1}],
+                   [217, [500.0], 5678, "ok", [210], 210, {"sum": 845, "count": 2}],
+                   [221, [278.0], 1234, "ok", [210, 220], 220, {"sum": 278, "count": 1}],
+                   [221, [278.0], 1234, "duplicate", [210, 220], 220, {"sum": 278, "count": 1}]]},
+        {"name": "TestCounterElemAddUniqueWithCustomAggregation", "src_line": src + "392-466", "metric": "counter",
+         "resolution_s": 10, "custom": True,
+         "steps": [[216, [12.0], 1234, "ok", [210], 210, {"sum": 12, "max": 12, "sum_sq": 144}],
+                   [217, [14.0], 5678, "ok", [210], 210, {"sum": 26, "max": 14}],
+                   [221, [20.0], 1234, "ok", [210, 220], 220, {"sum": 20, "max": 20, "sum_sq": 400}],
+                   [221, [30.0], 1234, "duplicate", [210, 220], 220, {"sum": 20, "count": 1, "sum_sq": 400}]]},
+        {"name": "TestGaugeElemAddUnique", "src_line": src + "1473-1546", "metric": "gauge", "resolution_s": 10,
+         "custom": False,
+         "steps": [[216, [12.3, 34.5], 1234, "ok", [210], 210, {"sum": 46.8, "count": 2}],
+                   [217, [50.0], 5678, "ok", [210], 210, {"sum": 96.8, "count": 3}],
+                   [221, [27.8], 1234, "ok", [210, 220], 220, {"sum": 27.8, "count": 1}],
+                   [221, [27.8], 1234, "duplicate", [210, 220], 220, {"sum": 27.8, "count": 1}]]},
+        {"name": "TestGaugeElemAddUniqueWithCustomAggregation", "src_line": src + "1572-1643", "metric": "gauge",
+         "resolution_s": 10, "custom": True,
+         "steps": [[216, [1.2], 1234, "ok", [210], 210, {"sum": 1.2, "max": 1.2, "sum_sq": 1.44}],
+                   [217, [1.4], 5678, "ok", [210], 210, {"sum": 2.6, "max": 1.4, "eps": 1e-10}],
+                   [221, [2.0], 1234, "ok", [210, 220], 220, {"sum": 2.0, "max": 2.0, "sum_sq": 4.0}],
+                   [221, [3.0], 1234, "duplicate", [210, 220], 220, {"sum": 2.0, "max": 2.0, "sum_sq": 4.0}]]},
+    ]
+    writer = [
+        {"name": "TestForwardedWriterPrepare", "src_line": "aggregator/aggregator/forwarded_writer_test.go:351-435",
+         "source_id": 0,
+         "writes": [["foo", 1234, 3.4], ["foo", 1234, 3.5], ["foo", 1240, 98.2], ["bar", 1238, 3.4],
+                    ["bar", 1239, 3.5]],
+         "want": [["foo", 1234, [3.4, 3.5]], ["foo", 1240, [98.2]], ["bar", 1238, [3.4]], ["bar", 1239, [3.5]]]},
+    ]
+    with open(out, "w") as f:
+        json.dump({"add_unique": add_unique, "writer": writer}, f, indent=1)
     print("wrote", out)
 
 
