@@ -27,7 +27,7 @@
  * m3tsz_encode_batch_packed(_ex), m3tsz_compact_streams,
  * m3tsz_encoder_set_write, m3tsz_element_set_reset of a set with output rows,
  * m3tsz_element_set_consume(_annotated), m3tsz_element_set_forward(_annotated),
- * m3tsz_element_set_forward_write, m3tsz_element_set_add_forwarded) are
+ * m3tsz_element_set_forward_write(_timer), m3tsz_element_set_add_forwarded(_timer)) are
  * ordered in the order they are issued: each one's stream waits on the device
  * for the context's previous such call, whatever stream that was on.  Two such
  * calls on one context therefore never overlap; a caller who wants them to
@@ -1182,7 +1182,8 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
  * window, the values of its local sources and sends one aggregated.ForwardedMetric with ForwardMetadata.SourceID; the
  * group shard takes it through GenericElem.AddUnique (generic_elem.go:241-288), which refuses a (source, version) its
  * window has already seen.  m3tsz_element_set_forward_write is the first half, m3tsz_element_set_add_forwarded the
- * second.  Gauge and Counter sets only, without annotations.
+ * second, for Gauge and Counter sets; m3tsz_element_set_forward_write_timer and m3tsz_element_set_add_forwarded_timer
+ * (after the Timer calls below) are the pair for Timer sets.  Without annotations.
  *
  * One forwarded metric, pointer-free so that a batch (records + one float64 values array) can be copied, concatenated
  * or sent as bytes (40 bytes, 8-byte aligned): */
@@ -1429,6 +1430,47 @@ int m3tsz_element_set_forward_timer_annotated(
     const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members, uint64_t n_groups,
     const m3tsz_element_set *groups, const m3tsz_element_timer_streams *group_streams,
     const m3tsz_element_annotations *group_ann, int32_t *d_src_status, int32_t *d_group_status, void *stream);
+
+/* Timer element-set rollups across shards (DESIGN.md §4.12): the cross-shard pair above for Timer sets, without
+ * annotations.  A latency timer rolled up with its host or pod tag dropped has members on every shard, and arrival
+ * order changes the group's quantiles, not only its Last.
+ *
+ * The source shard's writer: m3tsz_element_set_forward_write with the source's streams.  src is a Timer set of one
+ * type (any but Last); each source forwards its due windows as m3tsz_element_set_forward_timer does (rule 1: Flush,
+ * ValueOf of the type through the pre-rollup ops, the flushed headers written back).  Records, the prefix capacity
+ * rule, d_counts, held-back members and statuses are m3tsz_element_set_forward_write's.
+ * Host checks: those of m3tsz_element_set_forward_write, with src checked as m3tsz_element_set_add_timer checks a set
+ * and its streams; a set that is not a Timer set is refused.  m3tsz_element_set_forward_write keeps refusing Timer
+ * sets. */
+int m3tsz_element_set_forward_write_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                          const m3tsz_element_timer_streams *src_streams, int64_t target_ns,
+                                          const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                          uint64_t n_groups, const uint64_t *d_group_key, uint32_t source_id,
+                                          m3tsz_forwarded_metric *d_metrics, uint64_t metric_capacity,
+                                          double *d_values, uint64_t value_capacity, uint64_t *d_counts,
+                                          int32_t *d_src_status, int32_t *d_group_status, void *stream);
+
+/* AddUnique of forwarded metrics into a Timer group set (its streams in set_streams).  Each element takes its records
+ * in array order, which stands in for arrival order and for a Timer also fixes the quantiles.  Per record, rules 1-5
+ * of m3tsz_element_set_add_forwarded, then:
+ *   6. the window's list samples + pending values + the record's n_values exceed set_streams->sample_capacity:
+ *      M3TSZ_ERR_CAPACITY for the record and every later record of the element in this call; the source's bit stays
+ *      clear, and a slot opened for the record stays free;
+ *   7. else the source's bit is set and each value, in the record's order, is one Timer.Add into the window (count +
+ *      1, sum and sumSq as m3tsz_element_set_add_timer sums them, then AddBatch of that one value), as
+ *      m3tsz_element_set_forward_timer folds a value.
+ * d_result and d_status as in m3tsz_element_set_add_forwarded.  After a CAPACITY stop and
+ * m3tsz_element_set_forward_timer's grow (open windows and / or sample capacity), sending the refused records again,
+ * or the whole batch, gives the unstopped result.
+ * Host checks: those of m3tsz_element_set_add_forwarded, with the set checked as m3tsz_element_set_add_timer checks a
+ * set and its streams; a set that is not a Timer set is refused.  m3tsz_element_set_add_forwarded keeps refusing
+ * Timer sets. */
+int m3tsz_element_set_add_forwarded_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                          const m3tsz_element_timer_streams *set_streams,
+                                          const m3tsz_element_sources *sources,
+                                          const m3tsz_forwarded_metric *d_metrics, uint64_t n_metrics,
+                                          const double *d_values, uint64_t n_values, int8_t *d_result,
+                                          int32_t *d_status, void *stream);
 
 /* ------------------------------------------------------------------------
  * Per-series streaming handles: what a cgo shim binds METHOD FOR METHOD to the

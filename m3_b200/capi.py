@@ -176,6 +176,7 @@ EXPORTED_SYMBOLS = [
     "m3tsz_element_set_forward_timer", "m3tsz_element_set_add_timer_annotated",
     "m3tsz_element_set_consume_timer_annotated", "m3tsz_element_set_forward_timer_annotated",
     "m3tsz_element_set_forward_write", "m3tsz_element_set_add_forwarded",
+    "m3tsz_element_set_forward_write_timer", "m3tsz_element_set_add_forwarded_timer",
 ]
 
 ENCODER_STATE_BYTES = 128  # sizeof(m3tsz_encoder_state)
@@ -394,6 +395,12 @@ def lib():
     L.m3tsz_element_set_forward_timer_annotated.restype = C.c_int
     L.m3tsz_element_set_forward_timer_annotated.argtypes = [vp, po, pes, pts, pea, i64, vp, vp, u64, u64, pes, pts,
                                                             pea, vp, vp, vp]
+    L.m3tsz_element_set_forward_write_timer.restype = C.c_int
+    L.m3tsz_element_set_forward_write_timer.argtypes = [vp, po, pes, pts, i64, vp, vp, u64, u64, vp, C.c_uint32, vp,
+                                                        u64, vp, u64, vp, vp, vp, vp]
+    L.m3tsz_element_set_add_forwarded_timer.restype = C.c_int
+    L.m3tsz_element_set_add_forwarded_timer.argtypes = [vp, po, pes, pts, C.POINTER(ElementSources), vp, u64, vp,
+                                                        u64, vp, vp, vp]
     _lib = L
     return L
 

@@ -1309,9 +1309,23 @@ class ElementSet:
         end, its members' values in listed order.  Groups are written in order while they fit metric_capacity /
         value_capacity (default: room for every record); every later group gets ERR_CAPACITY and holds its members
         back, so calling again with exactly the failed groups and more room gives the rest.  Returns (ForwardedBatch,
-        source statuses int32 [N], group statuses int32 [G]: OK, ERR_CAPACITY or ERR_INVALID_ARG)."""
+        source statuses int32 [N], group statuses int32 [G]: OK, ERR_CAPACITY or ERR_INVALID_ARG).  Timer sets write
+        with forward_write_timer."""
         if self.timer:
-            raise ValueError("Timer sets take no forward_write")
+            raise ValueError("Timer sets take no forward_write; they write with forward_write_timer")
+        return self._forward_write(target_ns, group_off, members, source_id, keys, metric_capacity, value_capacity)
+
+    def forward_write_timer(self, target_ns, group_off: torch.Tensor, members: torch.Tensor, source_id: int,
+                            keys: Optional[torch.Tensor] = None, metric_capacity: Optional[int] = None,
+                            value_capacity: Optional[int] = None):
+        """forward_write for a Timer set (m3tsz_element_set_forward_write_timer, DESIGN.md §4.12), with the same
+        arguments and return values: this set (one type, any but Last; its transformations the pre-rollup ones)
+        flushes each due window's stream and forwards ValueOf(its type), as forward_timer does."""
+        if not self.timer:
+            raise ValueError("forward_write_timer takes a Timer set; other sets write with forward_write")
+        return self._forward_write(target_ns, group_off, members, source_id, keys, metric_capacity, value_capacity)
+
+    def _forward_write(self, target_ns, group_off, members, source_id, keys, metric_capacity, value_capacity):
         assert group_off.is_cuda and group_off.dtype == torch.int64 and group_off.is_contiguous()
         assert members.is_cuda and members.dtype == torch.int32 and members.is_contiguous()
         if keys is not None:
@@ -1330,12 +1344,17 @@ class ElementSet:
         counts = torch.zeros(4, dtype=torch.int64, device=dev)
         src_status = torch.empty(max(1, self.n_elements), dtype=torch.int32, device=dev)
         group_status = torch.empty(max(1, G), dtype=torch.int32, device=dev)
-        rc = capi.lib().m3tsz_element_set_forward_write(
-            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(self._desc()), int(target_ns), _ptr(group_off),
-            _ptr(members), members.numel(), G, _ptr(keys), int(source_id), metrics.data_ptr(), int(metric_capacity),
-            values.data_ptr(), int(value_capacity), counts.data_ptr(), _ptr(src_status), _ptr(group_status),
-            _cuda_stream_ptr(dev))
-        self.codec.ctx.check(rc, "m3tsz_element_set_forward_write")
+        head = (self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(self._desc()))
+        tail = (int(target_ns), _ptr(group_off), _ptr(members), members.numel(), G, _ptr(keys), int(source_id),
+                metrics.data_ptr(), int(metric_capacity), values.data_ptr(), int(value_capacity), counts.data_ptr(),
+                _ptr(src_status), _ptr(group_status), _cuda_stream_ptr(dev))
+        if self.timer:
+            name = "m3tsz_element_set_forward_write_timer"
+            rc = getattr(capi.lib(), name)(*head, C.byref(self._streams()), *tail)
+        else:
+            name = "m3tsz_element_set_forward_write"
+            rc = getattr(capi.lib(), name)(*head, *tail)
+        self.codec.ctx.check(rc, name)
         c = counts.tolist()
         batch = ForwardedBatch(metrics[: c[0]], values[: c[1]], c)
         return batch, src_status[: self.n_elements], group_status[:G]
@@ -1346,9 +1365,21 @@ class ElementSet:
         rebased), each element taking its records in that order.  Returns (result int8 [M] in record order: OK,
         ERR_INVALID_ARG, ERR_AGGREGATION_CLOSED, ERR_CAPACITY -- the element stopped: grow() and send the refused
         records again --, or ERR_DUPLICATE_SOURCE -- the window has seen that source --; status int32 [N]: OK or
-        ERR_CAPACITY)."""
+        ERR_CAPACITY).  Timer sets add with add_forwarded_timer."""
         if self.timer:
-            raise ValueError("Timer sets take no add_forwarded")
+            raise ValueError("Timer sets take no add_forwarded; they add with add_forwarded_timer")
+        return self._add_forwarded(batches)
+
+    def add_forwarded_timer(self, batches):
+        """add_forwarded for a Timer set (m3tsz_element_set_add_forwarded_timer, DESIGN.md §4.12), with the same
+        arguments and return values: each accepted record's values are Timer.Adds into its window, in order.  A
+        record that would take its window past sample_capacity samples also stops the element with ERR_CAPACITY:
+        grow(open_windows=..., sample_capacity=...) and send the refused records (or the whole batch) again."""
+        if not self.timer:
+            raise ValueError("add_forwarded_timer takes a Timer set; other sets add with add_forwarded")
+        return self._add_forwarded(batches)
+
+    def _add_forwarded(self, batches):
         if self.source_bits is None:
             raise ValueError("add_forwarded needs an element set with a source_capacity")
         b = batches if isinstance(batches, ForwardedBatch) else ForwardedBatch.concat(batches)
@@ -1360,11 +1391,16 @@ class ElementSet:
         src = capi.ElementSources()
         src.d_bits = self.source_bits.data_ptr()
         src.capacity = self.source_capacity
-        rc = capi.lib().m3tsz_element_set_add_forwarded(
-            self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(self._desc()), C.byref(src),
-            metrics.data_ptr() if M else None, M, values.data_ptr() if values.numel() else None, values.numel(),
-            result.data_ptr(), status.data_ptr(), _cuda_stream_ptr(dev))
-        self.codec.ctx.check(rc, "m3tsz_element_set_add_forwarded")
+        head = (self.codec.ctx.handle, C.byref(self.codec.opts), C.byref(self._desc()))
+        tail = (C.byref(src), metrics.data_ptr() if M else None, M, values.data_ptr() if values.numel() else None,
+                values.numel(), result.data_ptr(), status.data_ptr(), _cuda_stream_ptr(dev))
+        if self.timer:
+            name = "m3tsz_element_set_add_forwarded_timer"
+            rc = getattr(capi.lib(), name)(*head, C.byref(self._streams()), *tail)
+        else:
+            name = "m3tsz_element_set_add_forwarded"
+            rc = getattr(capi.lib(), name)(*head, *tail)
+        self.codec.ctx.check(rc, name)
         return result[:M], status[: self.n_elements]
 
     def state(self):

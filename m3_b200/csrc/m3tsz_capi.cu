@@ -1817,17 +1817,23 @@ int m3tsz_element_set_forward_annotated(m3tsz_ctx *ctx, const m3tsz_options *opt
 // The forward kernel writes each source's due windows to scratch (element_forward_scratch, with no group set), the
 // count pass counts each group's records and values, two scans place them, the write pass writes the groups that fit
 // and marks the members of the others, and the commit kernel frees the other sources' due windows.
-int m3tsz_element_set_forward_write(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
-                                    int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
-                                    uint64_t n_members, uint64_t n_groups, const uint64_t *d_group_key,
-                                    uint32_t source_id, m3tsz_forwarded_metric *d_metrics, uint64_t metric_capacity,
-                                    double *d_values, uint64_t value_capacity, uint64_t *d_counts,
-                                    int32_t *d_src_status, int32_t *d_group_status, void *stream) {
+// m3tsz_element_set_forward_write(_timer): `timer` selects the source check (timer_params on src and src_streams, or
+// element_params) and the source forward (element_timer_forward_kernel, or element_forward_kernel).
+static int element_set_forward_write(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                     const m3tsz_element_timer_streams *src_streams, int64_t target_ns,
+                                     const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                     uint64_t n_groups, const uint64_t *d_group_key, uint32_t source_id,
+                                     m3tsz_forwarded_metric *d_metrics, uint64_t metric_capacity, double *d_values,
+                                     uint64_t value_capacity, uint64_t *d_counts, int32_t *d_src_status,
+                                     int32_t *d_group_status, void *stream, bool timer) {
   ElementForwardedParams fp;
   memset(&fp, 0, sizeof(fp));
   ElementRollupParams &rp = fp.rp;
+  ElementTimerParams sp;
   TileTransforms sx;
-  if (!ctx || !element_params(opts, src, rp.src, sx)) return M3TSZ_ERR_INVALID_ARG;
+  if (!ctx || !(timer ? timer_params(opts, src, src_streams, sp, sx) : element_params(opts, src, rp.src, sx)))
+    return M3TSZ_ERR_INVALID_ARG;
+  if (timer) rp.src = sp.e;
   if (sx.n_types != 1 || n_groups > (1ull << 40) || n_members > (1ull << 40) || metric_capacity > (1ull << 40) ||
       value_capacity > (1ull << 40) || (n_groups && !d_group_off) || (n_members && !d_members) ||
       ((uintptr_t)d_group_off & 7u) || ((uintptr_t)d_members & 3u) || ((uintptr_t)d_group_key & 7u) || !d_counts ||
@@ -1867,7 +1873,12 @@ int m3tsz_element_set_forward_write(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   fp.val_off = (uint64_t *)d_vo;
   fp.counts = d_counts;
   CK(cudaMemsetAsync(rp.mark, 0, (rp.src.n ? rp.src.n : 1) * 4, st));
-  CK(launch_element_forward(rp, st));
+  if (timer) {
+    sp.e = rp.src;
+    CK(launch_element_timer_forward(rp, sp, st));
+  } else {
+    CK(launch_element_forward(rp, st));
+  }
   CK(launch_forward_write_count(fp, st));
   if (n_groups) {
     CK(forward_write_scan(d_tmp, tmp_bytes, fp.n_rec, fp.rec_off, n_groups, st));
@@ -1879,17 +1890,45 @@ int m3tsz_element_set_forward_write(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   return M3TSZ_OK;
 }
 
+int m3tsz_element_set_forward_write(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                    int64_t target_ns, const uint64_t *d_group_off, const uint32_t *d_members,
+                                    uint64_t n_members, uint64_t n_groups, const uint64_t *d_group_key,
+                                    uint32_t source_id, m3tsz_forwarded_metric *d_metrics, uint64_t metric_capacity,
+                                    double *d_values, uint64_t value_capacity, uint64_t *d_counts,
+                                    int32_t *d_src_status, int32_t *d_group_status, void *stream) {
+  return element_set_forward_write(ctx, opts, src, nullptr, target_ns, d_group_off, d_members, n_members, n_groups,
+                                   d_group_key, source_id, d_metrics, metric_capacity, d_values, value_capacity,
+                                   d_counts, d_src_status, d_group_status, stream, false);
+}
+
+int m3tsz_element_set_forward_write_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *src,
+                                          const m3tsz_element_timer_streams *src_streams, int64_t target_ns,
+                                          const uint64_t *d_group_off, const uint32_t *d_members, uint64_t n_members,
+                                          uint64_t n_groups, const uint64_t *d_group_key, uint32_t source_id,
+                                          m3tsz_forwarded_metric *d_metrics, uint64_t metric_capacity,
+                                          double *d_values, uint64_t value_capacity, uint64_t *d_counts,
+                                          int32_t *d_src_status, int32_t *d_group_status, void *stream) {
+  return element_set_forward_write(ctx, opts, src, src_streams, target_ns, d_group_off, d_members, n_members,
+                                   n_groups, d_group_key, source_id, d_metrics, metric_capacity, d_values,
+                                   value_capacity, d_counts, d_src_status, d_group_status, stream, true);
+}
+
 // The prep kernel writes each record's element key and index, the radix sort orders them by key (stable, so each
 // element's records stay in array order), and one lane per element takes its records.
-int m3tsz_element_set_add_forwarded(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
-                                    const m3tsz_element_sources *sources, const m3tsz_forwarded_metric *d_metrics,
-                                    uint64_t n_metrics, const double *d_values, uint64_t n_values, int8_t *d_result,
-                                    int32_t *d_status, void *stream) {
+// m3tsz_element_set_add_forwarded(_timer): `timer` selects the set check (timer_params on set and set_streams, or
+// element_params) and the lane (add_forwarded_timer_kernel, or add_forwarded_kernel).
+static int element_set_add_forwarded(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                     const m3tsz_element_timer_streams *set_streams,
+                                     const m3tsz_element_sources *sources, const m3tsz_forwarded_metric *d_metrics,
+                                     uint64_t n_metrics, const double *d_values, uint64_t n_values, int8_t *d_result,
+                                     int32_t *d_status, void *stream, bool timer) {
   ElementForwardedParams fp;
   memset(&fp, 0, sizeof(fp));
-  ElementParams gp;
+  ElementTimerParams gt;
+  ElementParams &gp = gt.e;
   TileTransforms gx;
-  if (!ctx || !element_params(opts, set, gp, gx)) return M3TSZ_ERR_INVALID_ARG;
+  if (!ctx || !(timer ? timer_params(opts, set, set_streams, gt, gx) : element_params(opts, set, gp, gx)))
+    return M3TSZ_ERR_INVALID_ARG;
   if (!sources || sources->reserved != 0 || sources->capacity == 0 || (sources->capacity & 31u) ||
       sources->capacity > M3TSZ_MAX_FORWARD_SOURCES || !sources->d_bits || ((uintptr_t)sources->d_bits & 3u) ||
       n_metrics > (1ull << 40) || n_values > (1ull << 40) || (n_metrics && (!d_metrics || !d_result)) ||
@@ -1945,9 +1984,27 @@ int m3tsz_element_set_add_forwarded(m3tsz_ctx *ctx, const m3tsz_options *opts, c
   CK(launch_add_forwarded_prep(fp, st));
   CK(add_forwarded_sort(d_tmp, tmp_bytes, fp.sort_key, (uint64_t *)d_sk, fp.sort_idx, (uint64_t *)d_si, n_metrics,
                         end_bit, st));
-  CK(launch_add_forwarded(fp, st));
+  CK(timer ? launch_add_forwarded_timer(fp, gt, st) : launch_add_forwarded(fp, st));
   ctx->launches += 3;
   return M3TSZ_OK;
+}
+
+int m3tsz_element_set_add_forwarded(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                    const m3tsz_element_sources *sources, const m3tsz_forwarded_metric *d_metrics,
+                                    uint64_t n_metrics, const double *d_values, uint64_t n_values, int8_t *d_result,
+                                    int32_t *d_status, void *stream) {
+  return element_set_add_forwarded(ctx, opts, set, nullptr, sources, d_metrics, n_metrics, d_values, n_values,
+                                   d_result, d_status, stream, false);
+}
+
+int m3tsz_element_set_add_forwarded_timer(m3tsz_ctx *ctx, const m3tsz_options *opts, const m3tsz_element_set *set,
+                                          const m3tsz_element_timer_streams *set_streams,
+                                          const m3tsz_element_sources *sources,
+                                          const m3tsz_forwarded_metric *d_metrics, uint64_t n_metrics,
+                                          const double *d_values, uint64_t n_values, int8_t *d_result,
+                                          int32_t *d_status, void *stream) {
+  return element_set_add_forwarded(ctx, opts, set, set_streams, sources, d_metrics, n_metrics, d_values, n_values,
+                                   d_result, d_status, stream, true);
 }
 
 // element_set_forward with the Timer forward and fold kernels: the same groups, scratch, annotation scratch and

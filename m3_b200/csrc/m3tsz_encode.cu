@@ -4099,17 +4099,8 @@ __device__ __forceinline__ void add_forwarded_lane(const ElementForwardedParams 
         const int64_t ws = t0 - res;
         r = M3TSZ_OK;
         if (cur < 0 || ws != f.start) {  // the window's slot, or a free one
-          int hit = -1, fr = -1;
-          for (uint32_t s = 0; s < rp.g_slots; s++) {
-            if ((int)s == cur) continue;
-            const uint64_t o = (uint64_t)s * G + e;
-            if (rp.g_count[o] == 0) {
-              if (fr < 0) fr = (int)s;
-            } else if (rp.g_start[o] == ws) {
-              hit = (int)s;
-              break;
-            }
-          }
+          int hit, fr;
+          rp.group_slot(e, cur, ws, hit, fr);
           if (hit < 0 && fr < 0) {
             status = r = M3TSZ_ERR_CAPACITY;
           } else {
@@ -4373,16 +4364,8 @@ __device__ __forceinline__ int32_t elem_timer_fold_group(const ElementRollupPara
         }
         if (cur < 0 || ws != w_start) {  // the window's slot, or a free one (the first pass counted them)
           if (cur >= 0) store();
-          int hit = -1, fr = -1;
-          for (uint32_t r = 0; r < p.g_slots; r++) {
-            const uint64_t o = (uint64_t)r * G + g;
-            if (p.g_count[o] == 0) {
-              if (fr < 0) fr = (int)r;
-            } else if (p.g_start[o] == ws) {
-              hit = (int)r;
-              break;
-            }
-          }
+          int hit, fr;
+          p.group_slot(g, -1, ws, hit, fr);
           cur = hit >= 0 ? hit : fr;
           const uint64_t o = (uint64_t)cur * G + g;
           w_start = ws;
@@ -4472,6 +4455,124 @@ cudaError_t launch_element_timer_fold(const ElementRollupParams &p, const Elemen
     element_timer_fold_kernel<true><<<elem_blocks(p.n_groups), ELEM_THREADS, 0, stream>>>(p, groups);
   else
     element_timer_fold_kernel<false><<<elem_blocks(p.n_groups), ELEM_THREADS, 0, stream>>>(p, groups);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------
+// Timer element-set rollups across shards (DESIGN.md §4.12): the writer is forward_write's kernels after
+// element_timer_forward_kernel; AddUnique into a Timer group set is the lane below
+// ---------------------------------------------------------------------------
+// add_forwarded_lane for Timer element e (gt: the group set's streams): the same record loop, checks, slot search and
+// source bits, with one check after the duplicate one: a record whose values would take its window past gt.cap
+// samples (list, pending and the record's values) stops the element with CAPACITY, its bit clear (a slot opened for it
+// stays free).  Each value is then one Timer.Add as elem_timer_fold_group makes it.  The window the last record went
+// to (its count, sums and stream header) stays in registers.  (The record checks and the Timer.Add are copies of
+// add_forwarded_lane's and elem_timer_fold_group's; tests/test_device_element_timer_forwarded_on_host.py pins them.)
+__device__ __forceinline__ void add_forwarded_timer_lane(const ElementForwardedParams &p, const ElementTimerParams &gt,
+                                                         uint64_t j) {
+  const ElementRollupParams &rp = p.rp;
+  const uint64_t e = p.sorted_key[j], G = rp.n_groups;
+  if (e >= G) {
+    for (; j < p.n_recs && p.sorted_key[j] == e; j++) p.result[p.sorted_idx[j]] = (int8_t)M3TSZ_ERR_INVALID_ARG;
+    return;
+  }
+  const int64_t res = rp.src.resolution, wm = rp.g_watermark[e];
+  const uint32_t W = p.bit_words;
+  int cur = -1;  // the group slot the registers hold, -1: none
+  int64_t w_start = 0, cnt = 0;
+  double sum = 0.0, sq = 0.0;
+  CmStream c = timer_stream(gt, 0u, e);  // (set again for the slot whenever `cur` changes)
+  auto store = [&]() {
+    if (cnt == 0) return;  // (a slot opened for a refused record)
+    const uint64_t o = (uint64_t)cur * G + e;
+    rp.g_start[o] = w_start;
+    rp.g_count[o] = cnt;
+    static_cast<double *>(rp.g_sum)[o] = sum;
+    static_cast<double *>(rp.g_sum_sq)[o] = sq;
+    gt.hdr[o] = c.h;
+  };
+  int32_t status = M3TSZ_OK;
+  for (; j < p.n_recs && p.sorted_key[j] == e; j++) {
+    const uint64_t i = p.sorted_idx[j];
+    const m3tsz_forwarded_metric m = p.rec[i];
+    int r = M3TSZ_ERR_CAPACITY;  // (after a CAPACITY, the rest of the element's records)
+    if (status == M3TSZ_OK) {
+      int64_t t0 = 0;
+      if (m.n_values == 0 || m.value_off > p.n_vals || m.n_values > p.n_vals - m.value_off || m.version != 0 ||
+          m.reserved != 0 || !elem_window_start(m.time_ns, res, p.trunc_off, t0) ||
+          t0 < (int64_t)0x8000000000000000ull + res) {
+        r = M3TSZ_ERR_INVALID_ARG;
+      } else if (elem_ends_by(t0 - res, res, wm)) {
+        r = M3TSZ_ERR_AGGREGATION_CLOSED;
+      } else if (m.source_id >= W * 32u) {
+        status = r = M3TSZ_ERR_CAPACITY;
+      } else {
+        const int64_t ws = t0 - res;
+        r = M3TSZ_OK;
+        if (cur < 0 || ws != w_start) {  // the window's slot, or a free one
+          int hit, fr;
+          rp.group_slot(e, cur, ws, hit, fr);
+          if (hit < 0 && fr < 0) {
+            status = r = M3TSZ_ERR_CAPACITY;
+          } else {
+            if (cur >= 0) store();
+            cur = hit >= 0 ? hit : fr;
+            const uint64_t o = (uint64_t)cur * G + e;
+            w_start = ws;
+            c = timer_stream(gt, (uint32_t)cur, e);
+            if (hit >= 0) {
+              cnt = rp.g_count[o];
+              sum = static_cast<const double *>(rp.g_sum)[o];
+              sq = static_cast<const double *>(rp.g_sum_sq)[o];
+              c.h = gt.hdr[o];
+            } else {
+              cnt = 0;
+              sum = sq = 0.0;
+              c.init();
+              for (uint32_t w = 0; w < W; w++) p.bits[((uint64_t)cur * W + w) * G + e] = 0u;
+            }
+          }
+        }
+        if (r == M3TSZ_OK) {
+          uint32_t *word = p.bits + ((uint64_t)cur * W + (m.source_id >> 5)) * G + e;
+          const uint32_t bit = 1u << (m.source_id & 31u);
+          if (*word & bit) {
+            r = M3TSZ_ERR_DUPLICATE_SOURCE;
+          } else if ((uint64_t)c.size() + m.n_values > gt.cap) {
+            status = r = M3TSZ_ERR_CAPACITY;
+          } else {
+            *word |= bit;
+            for (uint32_t k = 0; k < m.n_values; k++) {
+              const double v = p.val[m.value_off + k];
+              cnt++;
+              sum = amd64_op(__dadd_rn(sum, v), sum, v);
+              const double v2 = amd64_op(__dmul_rn(v, v), v, v);
+              sq = amd64_op(__dadd_rn(sq, v2), sq, v2);
+              c.add_batch(1u, [&](uint32_t) { return v; });
+            }
+          }
+        }
+      }
+    }
+    p.result[i] = (int8_t)r;
+  }
+  if (cur >= 0) store();
+  p.status[e] = status;
+}
+
+// (__maxnreg__ as the other Timer kernels: the stream's code is the same)
+__global__ void __maxnreg__(128) add_forwarded_timer_kernel(const ElementForwardedParams p,
+                                                            const ElementTimerParams gt) {
+  const uint64_t j = (uint64_t)blockIdx.x * ELEM_THREADS + threadIdx.x;
+  if (j >= p.n_recs || (j && p.sorted_key[j - 1] == p.sorted_key[j])) return;  // one lane per element with records
+  add_forwarded_timer_lane(p, gt, j);
+}
+
+cudaError_t launch_add_forwarded_timer(const ElementForwardedParams &p, const ElementTimerParams &groups,
+                                       cudaStream_t stream) {
+  if (p.n_recs == 0) return cudaSuccess;
+  if ((p.n_recs + ELEM_THREADS - 1) / ELEM_THREADS > 0x7fffffffull) return cudaErrorInvalidValue;
+  add_forwarded_timer_kernel<<<elem_blocks(p.n_recs), ELEM_THREADS, 0, stream>>>(p, groups);
   return cudaGetLastError();
 }
 

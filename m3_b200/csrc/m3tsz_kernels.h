@@ -525,6 +525,21 @@ struct ElementRollupParams {
     uint64_t *dst = reinterpret_cast<uint64_t *>(g_ann_slot + o * g_ann_cap);
     for (uint32_t w = lane; w < (len + 7u) / 8u; w += n_lanes) dst[w] = from[w];
   }
+  // AddUnique's and the Timer fold's slot search: group g's slot holding window ws (hit), else its first free slot
+  // (fr), -1 for none; slot `skip` (the one a lane holds in registers, -1: none) is passed over
+  __device__ __forceinline__ void group_slot(uint64_t g, int skip, int64_t ws, int &hit, int &fr) const {
+    hit = fr = -1;
+    for (uint32_t s = 0; s < g_slots; s++) {
+      if ((int)s == skip) continue;
+      const uint64_t o = (uint64_t)s * n_groups + g;
+      if (g_count[o] == 0) {
+        if (fr < 0) fr = (int)s;
+      } else if (g_start[o] == ws) {
+        hit = (int)s;
+        break;
+      }
+    }
+  }
 };
 // (the annotated kernels when p.src.ann_len is set)
 cudaError_t launch_element_forward(const ElementRollupParams &p, cudaStream_t stream);
@@ -576,6 +591,11 @@ cudaError_t launch_element_timer_forward(const ElementRollupParams &p, const Ele
                                          cudaStream_t stream);
 cudaError_t launch_element_timer_fold(const ElementRollupParams &p, const ElementTimerParams &groups,
                                       cudaStream_t stream);
+// Timer sets across shards (m3tsz_element_set_forward_write_timer / _add_forwarded_timer): the writer runs
+// launch_element_timer_forward in place of launch_element_forward; the add runs the prep kernel and the sort as
+// add_forwarded does, then one lane per element with `groups` the group set's streams and quantile list.
+cudaError_t launch_add_forwarded_timer(const ElementForwardedParams &p, const ElementTimerParams &groups,
+                                       cudaStream_t stream);
 
 // exclusive scan of aligned lengths + gather into a packed buffer
 cudaError_t launch_compact(const uint8_t *slots, uint64_t slot_stride, const uint64_t *len,

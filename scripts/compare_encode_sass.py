@@ -12,8 +12,8 @@ element_fold_kernel and element_commit_kernel are compared too; the annotated el
 ANN, to the first two, so an old build's <CTR> is compared with a new build's <CTR, false>.  The Timer element sets'
 element_timer_{add,consume,forward,fold}_kernel are compared too; the annotated Timer element sets made them templates
 over ANN, so an old build's untemplated kernel is compared with a new build's <false>.  The cross-shard rollup's
-forward_write_{count_,}kernel and add_forwarded_{prep_,}kernel are compared too.  Instantiations only one build
-has (the append mode, new decode modes, the annotated element kernels) are listed, not compared.
+forward_write_{count_,}kernel and add_forwarded_{prep_,timer_,}kernel are compared too.  Instantiations only one
+build has (the append mode, new decode modes, the annotated element kernels) are listed, not compared.
 
     python scripts/compare_encode_sass.py OLD.(o|so) NEW.(o|so)     # exit code 1 on any difference
 
@@ -49,7 +49,7 @@ def kernels(path):
             elif re.search(r"element_(forward|fold|commit)_kernel", name):  # (element sets through a rollup)
                 cur = re.sub(r"(element_(?:forward|fold)_kernelILb[01]E)Lb0E", r"\1", name)
                 out[cur] = []
-            elif re.search(r"(forward_write|add_forwarded)", name):  # (element-set rollups across shards)
+            elif re.search(r"(forward_write|add_forwarded)", name):  # (element-set rollups across shards, Timer too)
                 cur = name
                 out[cur] = []
             elif "rollup_forward_kernel" in name or "rollup_fold_kernel" in name:

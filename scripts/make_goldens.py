@@ -810,6 +810,7 @@ def main():
     timer_rollup_goldens()
     timer_annotation_goldens()
     forwarded_goldens()
+    timer_forwarded_goldens()
 
 
 def timer_goldens():
@@ -945,6 +946,30 @@ def forwarded_goldens():
     ]
     with open(out, "w") as f:
         json.dump({"add_unique": add_unique, "writer": writer}, f, indent=1)
+    print("wrote", out)
+
+
+def timer_forwarded_goldens():
+    """tests/golden/m3tsz_timer_forwarded_goldens.json: the reference's TimerElem.AddUnique expectations with their
+    source ids.  Each step is [at_s, values, source_id] with the result the reference returns ("ok" or "duplicate") and
+    what it checks after the step: "windows_s" the open window starts, and in "window_s" the Timer's "count", "sum",
+    "sum_sq" (sums as InEpsilon 1e-10, the rest exact), "q0.5" (Quantile(0.5)) and "seen" (source ids whose
+    sourcesSeen entry it asserts).  The tombstoned element's errElemClosed is not transcribed."""
+    out = os.path.join(os.path.dirname(OUT), "m3tsz_timer_forwarded_goldens.json")
+    default = [2, 3, 4, 5, 6, 7, 8, 9, 14, 19, 20]  # the default Timer types, ascending
+    cases = [
+        {"name": "TestTimerElemAddUnique", "src_line": "aggregator/aggregator/elem_test.go:120-125,927-999",
+         "resolution_s": 10, "types": default, "eps": 1e-3, "every": 1024,
+         "steps": [[216, [11.1], 1, "ok", [210], 210, {}],
+                   [216, [12.2], 2, "ok", [210], 210, {}],
+                   [216, [13.3], 3, "ok", [210], 210, {"count": 3, "sum": 36.6, "q0.5": 12.2}],
+                   [217, [14.4], 4, "ok", [210], 210, {"count": 4, "sum": 51.0}],
+                   [221, [20.0], 1, "ok", [210, 220], 220, {"count": 1, "sum": 20.0}],
+                   [221, [30.0], 1, "duplicate", [210, 220], 220,
+                    {"count": 1, "sum": 20.0, "sum_sq": 400.0, "seen": [1]}]]},
+    ]
+    with open(out, "w") as f:
+        json.dump({"add_unique": cases}, f, indent=1)
     print("wrote", out)
 
 
